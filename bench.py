@@ -36,7 +36,9 @@ sys.path.insert(0, str(ROOT))
 from headtrackr_b200 import synth  # noqa: E402
 
 N_UNIQUE = 64          # distinct synthetic frames generated on the CPU; the batch tiles them with x-rolls
-HBM_PEAK_FALLBACK = 6650.0
+HBM_PEAK_FALLBACK = 3350.0
+L2_BYTES = 50 * 2**20  # H100 SXM
+DUMP_LIMIT = 64 * 2**20
 WORKLOADS = {
     "detect_track30": dict(width=640, height=480, batch=1024, interval=5, track_calls=30,
                            metric="frames/sec @640x480 (detect+CAMShift)"),
@@ -72,14 +74,14 @@ def measured_peaks():
             return float(json.loads(p.read_text())["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return HBM_PEAK_FALLBACK, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return HBM_PEAK_FALLBACK, "fallback (H100 SXM data sheet, 3.35 TB/s)"
 
 
 def captured_traffic(W, H):
-    """dram__bytes_read + dram__bytes_write of k_cascade per frame from this round's committed ncu capture
-    (profiles/r02_cascade_dram.json, written by tools/ncu_dram.py from the .ncu-rep) - None when there is no capture
+    """dram__bytes_read + dram__bytes_write of k_cascade per frame from a local ncu capture (build/cascade_dram.json,
+    written by tools/ncu_dram.py from the .ncu-rep; git-ignored, never committed) - None when there is no capture
     for this frame size.  Never a constant in this file."""
-    p = ROOT / "profiles" / "r02_cascade_dram.json"
+    p = ROOT / "build" / "cascade_dram.json"
     try:
         d = json.loads(p.read_text())
         if (d["width"], d["height"]) == (W, H):
@@ -136,9 +138,33 @@ class ClockSampler:
                 "reasons": sorted(reasons)}
 
 
+def rect_arrays(rects):
+    """(..., K, 6) float64 view of ht_rect records -> x/y/width/height/confidence and the int32 neighbour count."""
+    r = np.ascontiguousarray(rects, dtype=np.float64)
+    return {"rects": r[..., :5], "neighbors": r.view(np.int32)[..., 10].astype(np.float64)}
+
+
+def dump_outputs(out_dir, arrays, axis=0):
+    """--dump-outputs: every array as <name>.npy in float64 (integers are exact in it).  `axis` is the frame (or stream)
+    axis of every array.  Above DUMP_LIMIT bytes in all, a fixed, seeded sample of that axis is written instead, with
+    its indices as sample_index.npy, so that the same arguments always dump the same entries."""
+    out = Path(out_dir)
+    out.mkdir(parents=True, exist_ok=True)
+    arrays = {k: np.ascontiguousarray(v, dtype=np.float64) for k, v in arrays.items()}
+    total = sum(a.nbytes for a in arrays.values())
+    if total > DUMP_LIMIT:
+        n = next(iter(arrays.values())).shape[axis]
+        keep = max(1, n * (DUMP_LIMIT - 8 * n) // total)
+        idx = np.sort(np.random.default_rng(0).choice(n, keep, replace=False))
+        arrays = {k: np.take(a, idx, axis=axis) for k, a in arrays.items()}
+        arrays["sample_index"] = idx.astype(np.float64)
+    for k, a in arrays.items():
+        np.save(out / f"{k}.npy", a)
+
+
 def bind_to_gpu_numa_node(local):
     """Pin this rank's host threads (and, by first touch, its pinned staging buffers) to the NUMA node of its GPU:
-    eight ranks pushing 1.26 GB per step each over PCIe from the wrong socket cost the 8-GPU e2e line 10 % in round 1."""
+    eight ranks pushing 1.26 GB per step each over PCIe from the wrong socket slow the multi-GPU e2e line down."""
     try:
         import torch
         p = torch.cuda.get_device_properties(local)
@@ -462,6 +488,20 @@ def run_ours(args, cfg):
     e1.record(stream)
     barrier()
     ms_local = e0.elapsed_time(e1)
+    if args.dump_outputs and rank == 0:
+        # what the last timed step handed its caller, before the secondary measurements below re-use the buffers
+        if streams:
+            ev = d_events.cpu().numpy()
+            dump_outputs(args.dump_outputs, {"event_detection": ev.view(np.int32)[..., 0],
+                                             "event_status": ev.view(np.int32)[..., 1],
+                                             "event_values": ev.view(np.float64)[..., 1:]}, axis=1)
+        else:
+            rects, counts, found, objs, wins = (t.cpu().numpy() for t in last_outputs())
+            arrays = dict(rect_arrays(rects), counts=counts)
+            if workload == "detect_track30":
+                arrays.update(found=found, track_xywh=objs[:, :4], track_angle=objs.view(np.float64)[:, 2],
+                              windows=wins)
+            dump_outputs(args.dump_outputs, arrays)
     prof = ctx.profile_read(reset=True)
     ctx.profile(False)
     track_stats = ctx.debug_track_stats(reset=True)
@@ -640,7 +680,7 @@ def run_ours(args, cfg):
                 "data": "synthetic",
                 "config": dict(config_dict(cfg, world, frames_per_step),
                                l2=f"inputs larger than L2 ({frames_per_step * W * H * 4 / 1e6:.0f} MB of frames per GPU per step)"
-                                  if frames_per_step * W * H * 4 > 126e6 else "L2 flushed by the step itself: every step streams "
+                                  if frames_per_step * W * H * 4 > L2_BYTES else "L2 flushed by the step itself: every step streams "
                                   f"{frames_per_step * W * H * 4 / 1e6:.0f} MB of frames and re-writes the pyramid arena",
                                unique_frames=N_UNIQUE if not streams else B * T,
                                track_memo="off (strict: every pass re-summed)",
@@ -658,8 +698,8 @@ def run_ours(args, cfg):
                              "kernel_ms_per_launch": casc_ms / casc_n if casc_n else None,
                              "whole_path": {"achieved": path_gbs, "frac": path_gbs / peak,
                                             "note": "value x one RGBA frame read, per GPU (SURVEY 8d's judged fraction)"},
-                             "note": "k_cascade is bound by shared-memory load wavefronts and issue slots, not by HBM; "
-                                     "see DESIGN.md §5.1 and profiles/"},
+                             "note": "k_cascade is designed to be bound by shared-memory loads and issue slots, not by HBM; "
+                                     "see DESIGN.md §5.1"},
                 "kernel_ms_per_step": kernel_ms,
                 "track_stats": track_stats,
                 "per_rank": per_rank,
@@ -733,7 +773,12 @@ def main():
     ap.add_argument("--pipeline", type=int, default=int(os.environ.get("HT_BENCH_PIPELINE", "0")),
                     help="detect+track: 0 (default) = every step joins its own tracking, 1 = pipelined steps "
                          "(ht_set_pipeline); on one GPU the other mode is measured too and reported beside the headline")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed as DIR/<name>.npy (float64; a fixed, seeded sample of "
+                         "the frames above 64 MB).  On more than one GPU: rank 0's own frames, not the gathered records")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     cfg = dict(WORKLOADS[args.workload], workload=args.workload, stream_frames=args.stream_frames)
     for k, v in (("width", args.width), ("height", args.height), ("interval", args.interval),
                  ("batch", args.streams if args.streams is not None else args.batch)):

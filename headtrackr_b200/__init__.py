@@ -1,4 +1,4 @@
-"""headtrackr_b200 — B200-native (sm_100a) replacement for headtrackr's detect+track pixel kernels.
+"""headtrackr_b200 — H100-native (sm_90a) replacement for headtrackr's detect+track pixel kernels.
 
 Host-side mirror of the reference's L1 interface (SURVEY.md §1):
     headtrackr_b200.ccv.grayscale / ccv.detect_objects      <- /root/reference/src/ccv.js

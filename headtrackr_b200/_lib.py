@@ -1,10 +1,11 @@
 """ctypes binding of libheadtrackr_b200.so (C ABI: include/headtrackr_b200.h).
 
-There is no CPU fallback: if the shared library is missing it is built with nvcc (sm_100a); if that
+There is no CPU fallback: if the shared library is missing it is built with nvcc (sm_90a); if that
 is impossible the import fails loudly.  Nothing here imports the oracle.
 """
 import ctypes as C
 import os
+import shutil
 import subprocess
 from pathlib import Path
 
@@ -68,10 +69,18 @@ def sources_newer_than_so():
     return any(s.stat().st_mtime > t for s in srcs)
 
 
+def nvcc():
+    """The CUDA compiler: $CUDA_HOME/bin/nvcc, else nvcc on PATH, else the toolkit's default install prefix."""
+    home = os.environ.get("CUDA_HOME") or os.environ.get("CUDA_PATH")
+    if home and (Path(home) / "bin" / "nvcc").exists():
+        return str(Path(home) / "bin" / "nvcc")
+    return shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
+
+
 def build(force=False):
-    """Compile the sm_100a shared library in-tree (nvcc cross-compiles without a GPU)."""
+    """Compile the sm_90a shared library in-tree (nvcc cross-compiles without a GPU)."""
     if force or sources_newer_than_so():
-        subprocess.check_call(["make", "-s", "-C", str(CSRC)] + (["-B"] if force else []))
+        subprocess.check_call(["make", "-s", "-C", str(CSRC), f"NVCC={nvcc()}"] + (["-B"] if force else []))
     if not SO_PATH.exists():
         raise ImportError(f"{SO_PATH} was not produced by the build")
     return SO_PATH

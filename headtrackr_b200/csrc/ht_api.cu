@@ -1,5 +1,5 @@
 // ht_api.cu — host side of libheadtrackr_b200.so: the C ABI declared in include/headtrackr_b200.h,
-// the pyramid/tile planner, and the kernel launches.  sm_100a only; there is no CPU fallback.
+// the pyramid/tile planner, and the kernel launches.  sm_90a only; there is no CPU fallback.
 #include "../../include/headtrackr_b200.h"
 
 #include <cuda.h>
@@ -458,6 +458,7 @@ int parse_cascade(const void *blob, size_t len, HostCascade &hc, std::string &er
 struct ht_ctx {
   ht_config cfg{};
   int K = 64, raw_cap = 1024;
+  int sms = 132;                            // SMs of the device: grid sizes of the small-batch kernels
   cudaStream_t stream = nullptr;
   bool own_stream = false;
   std::string err;
@@ -516,13 +517,12 @@ struct ht_ctx {
   cudaStream_t main_stream = nullptr;       // the context's stream while ctx->stream is temporarily the aux stream
   size_t bins_off = 0, hist_off = 0;        // element offsets of the active bin-plane / histogram buffer (parity)
   // Tracking of part p on a second stream while part p+1 is uploaded / detected (ht_detect_track).  Default (-1):
-  // only for HOST frames, where the batch arrives at PCIe speed and the GPU has idle time to fill - measured e2e
-  // 37.6k vs 33.0k frames/s with 4 parts (8 parts 36.8k, 16 parts 28.6k).  For device-resident frames it was
-  // measured slower (24.4-26.7 vs 22.3 ms per step) and stays off.  HT_OVERLAP=0 disables, HT_OVERLAP=<parts> forces.
+  // only for HOST frames, where the batch arrives at PCIe speed and the GPU has idle time to fill.  For
+  // device-resident frames there is no idle time to fill and it stays off.  HT_OVERLAP=0 disables, HT_OVERLAP=<parts> forces.
   int detect_pipe = 0;                      // HT_DETECT_PIPE=1: gray + pyramid of wave w+1 on a second stream under the cascade of wave w
   int wave_frames = 0;                      // frames per wave of run_detect (HT_WAVE); 0: from wave_mb
-  int wave_mb = 2048;                       // pyramid-arena budget of one wave in MB (HT_WAVE_MB).  64 (half of the L2) keeps
-                                            // the pyramid out of HBM but costs 28 % throughput in launch tails: lab notes
+  int wave_mb = 2048;                       // pyramid-arena budget of one wave in MB (HT_WAVE_MB).  Half of the L2 keeps
+                                            // the pyramid out of HBM but costs throughput in launch tails (DESIGN.md §5.5)
   int force_ties = 0;                       // ht_debug_set_exactness: force the exactness fallbacks (tests)
   cudaStream_t pipe_stream = nullptr;
   cudaEvent_t pipe_start = nullptr, pipe_events[4] = {};
@@ -556,8 +556,6 @@ struct ht_ctx {
   int track_heavy_div = 128;                // >0: the n/div costliest streams run on a cluster of
   int track_heavy_cluster = 8;              //     track_heavy_cluster CTAs on sched_stream (HT_TRACK_HEAVY=div[,cluster])
   int track_mid_div = 32, track_mid_cluster = 4;  // HT_TRACK_MID=div[,cluster]: the next n/32 costliest streams on clusters of 4
-                                                  // (call 4: 4.12 -> 3.40 ms per 1024 x 30 calls with n/16; call 17, with
-                                                  // prioritised tier streams: n/64 + n/16 3.17, n/128 + n/32 2.97, n/64 + n/48 3.00)
   double track_light_div = 0; int track_light_nt = 256;  // HT_TRACK_LIGHT=div[,threads]: the cheapest n/div streams (div may be fractional) on single CTAs
   cudaStream_t tier_stream[4] = {nullptr, nullptr, nullptr, nullptr};   // heavy, mid, light, rest (side 3: when tiers are on)
   cudaEvent_t tier_done[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -684,7 +682,7 @@ int launch_hist(ht_ctx *ctx, const uint8_t *d_rgba, int n, int w, int h, uint32_
                 const uint8_t *enable = nullptr) {
   const int n_px = w * h;
   int chunks = 1;
-  if (n < 592) chunks = std::min(64, std::max(1, 1184 / n));  // keep ~8 CTAs per SM busy for small batches
+  if (n < 4 * ctx->sms) chunks = std::min(64, std::max(1, 8 * ctx->sms / n));  // keep ~8 CTAs per SM busy for small batches
   if (chunks > 1) CK(cudaMemsetAsync(hist, 0, (size_t)n * 4096 * sizeof(uint32_t), ctx->stream));   // (also for disabled frames: harmless)
   ctx->prof_begin(HT_PROF_HIST);
   k_hist<<<dim3(chunks, n), 256, 0, ctx->stream>>>(d_rgba, (size_t)n_px * 4, n_px, hist, bins, chunks, enable);
@@ -776,7 +774,7 @@ int launch_track(ht_ctx *ctx, int n, int f0, const uint16_t *bins, int w, int h,
   // several track() calls on this frame: mark the plane entries whose weight is +0.0 first (k_bins_mask), k_track then
   // skips whole row segments of them.  (One call per frame - ht_stream_step - does not repay the extra pass.)
   if (ctx->track_mask_min > 0 && n_calls >= ctx->track_mask_min) {
-    const int chunks = std::max(1, std::min(64, 1184 / std::max(1, n)));
+    const int chunks = std::max(1, std::min(64, 8 * ctx->sms / std::max(1, n)));
     // selective (default): only streams whose previous launch visited more than track_mask_frames whole frames' worth
     // of pixels (history of the slot; first launch: nobody) - 1/10 of the bench mix, and nearly all of its pixel visits
     const int min_px256 = (int)std::min<long long>(((long long)ctx->track_mask_frames * w * h) >> 8, 0x7fffffff);
@@ -794,7 +792,7 @@ int launch_track(ht_ctx *ctx, int n, int f0, const uint16_t *bins, int w, int h,
   int32_t *bail_count = ctx->d_sched.as<int32_t>() + 2 * (size_t)ctx->cfg.max_frames + (ctx->sched_seq++ & 63);
   cudaError_t e = cudaSuccess;
   if (ctx->track_bail_area > 0) {
-    // two-phase (HT_TRACK_BAIL=<px>): measured 8.1-8.9 ms per 1024x30 calls vs 7.2 ms for the single-phase cluster of 4
+    // two-phase (HT_TRACK_BAIL=<px>): an A/B option; the single-phase launch below is the default
     e = cudaMemsetAsync(bail_count, 0, sizeof(int32_t), st);
     if (e != cudaSuccess) return ctx->fail(HT_ERR_CUDA, "memset: %s", cudaGetErrorString(e));
     e = launch_track_c<1>(st, n, bins, w, h, d_slots, mh, ch, state, n_calls, d_objs, d_win, flag, stats, ctx->track_bail_area,
@@ -805,7 +803,6 @@ int launch_track(ht_ctx *ctx, int n, int f0, const uint16_t *bins, int w, int h,
     ctx->launches += 2;
   } else {
     // few streams -> 8 CTAs per stream (latency of one stream); many streams -> 2 (more streams resident).
-    // measured on 1024 streams x 30 calls in index order: 1 CTA 9.7 ms, 2 CTAs 6.1 ms, 4 CTAs 6.2 ms, 8 CTAs 10.1 ms
     int c = ctx->track_cluster;
     if (c <= 0) c = (n >= 256) ? 2 : (n >= 32 ? 4 : 8);
     const int nt = ctx->track_nt;
@@ -835,9 +832,9 @@ int launch_track(ht_ctx *ctx, int n, int f0, const uint16_t *bins, int w, int h,
       take(ctx->track_heavy_div, ctx->track_heavy_cluster, 256, 0);
       take(ctx->track_mid_div, ctx->track_mid_cluster, 256, 1);
       const int n_light = (ctx->track_light_div > 0) ? std::min(left, (int)((double)n / ctx->track_light_div)) : 0;
-      // Round 2, call 8 timeline: with the default tier on the context's own stream (no event wait) its 1,888 CTAs
-      // reached the GPU first and filled every slot with ITS costliest streams; the heavy and middle tiers - the
-      // longest chains of the launch - started 1.4 ms late and the launch ended at 1.4 + 2.3 ms.  Now every tier sits
+      // With the default tier on the context's own stream (no event wait) its CTAs would reach the GPU first and fill
+      // every slot with ITS costliest streams, and the heavy and middle tiers - the longest chains of the launch -
+      // would start late and set the end of the launch.  So every tier sits
       // on a side stream behind the same event, submitted costliest tier first, and the side streams carry
       // descending priorities (heavy > mid > rest > light), so a free slot always goes to the longest pending chain.
       const bool rest_side = ctx->track_prio != 0 && (ctx->track_heavy_div > 0 || ctx->track_mid_div > 0);
@@ -977,8 +974,8 @@ struct HistOut {
 // Every per-frame buffer is indexed by absolute frame number so that chunks can be pipelined.
 //
 // The frames are processed in WAVES of ctx->wave_frames (whole frame quads): the pyramid arena holds one wave
-// (8 MB per 640x480 quad) and is re-used by the next one, so that it lives in the 126 MB L2 instead of making a
-// round trip through HBM for the whole batch (round 1: 1.86 GB read by k_cascade per 1024 frames).  With
+// (8 MB per 640x480 quad) and is re-used by the next one, so that it can live in the L2 instead of making a
+// round trip through HBM for the whole batch.  With
 // ctx->detect_pipe the gray + pyramid kernels of wave w+1 run on a second stream (and a second arena) under the
 // cascade of wave w.
 int run_detect(ht_ctx *ctx, Plan *P, const uint8_t *d_rgba_batch, int f0, int n, int min_neighbors, Rect *d_rects_batch,
@@ -1029,7 +1026,7 @@ int run_detect(ht_ctx *ctx, Plan *P, const uint8_t *d_rgba_batch, int f0, int n,
     // K1 grayscale (+ histogram + bin plane) -> plane 0
     {
       const bool hist = ho.hist != nullptr;
-      const int target = hist ? 592 : 1184;      // CTAs: 4 (32 KB of histograms each, register-limited) or 8 per SM
+      const int target = (hist ? 4 : 8) * ctx->sms;   // CTAs: 4 (32 KB of histograms each, register-limited) or 8 per SM
       int chunks = std::max(1, std::min(h, (target + quads - 1) / quads));
       if (hist) chunks = std::max(chunks, (w * h + 59999) / 60000);   // 16-bit histogram counters per CTA
       uint32_t *hp = hist ? ho.hist + (size_t)w0 * 4096 : nullptr;
@@ -1180,13 +1177,14 @@ int ht_create(ht_ctx **out, const ht_config *cfg, const void *cascade_blob, size
   if (cfg->device < 0 || cfg->device >= n_dev) { g_create_error = "ht_create: bad device ordinal"; return HT_ERR_ARG; }
   cudaDeviceProp prop{};
   if (cudaGetDeviceProperties(&prop, cfg->device) != cudaSuccess) { g_create_error = "ht_create: cudaGetDeviceProperties failed"; return HT_ERR_CUDA; }
-  if (prop.major != 10) {
-    g_create_error = "ht_create: device is sm_" + std::to_string(prop.major * 10 + prop.minor) + ", this build is sm_100a only";
+  if (prop.major != 9 || prop.minor != 0) {
+    g_create_error = "ht_create: device is sm_" + std::to_string(prop.major * 10 + prop.minor) + ", this build is sm_90a only";
     return HT_ERR_CUDA;
   }
   if (cudaSetDevice(cfg->device) != cudaSuccess) { g_create_error = "ht_create: cudaSetDevice failed"; return HT_ERR_CUDA; }
   std::unique_ptr<ht_ctx> c(new ht_ctx());
   c->cfg = *cfg;
+  c->sms = prop.multiProcessorCount;
   c->K = cfg->max_rects_per_frame > 0 ? cfg->max_rects_per_frame : 64;
   c->raw_cap = cfg->max_raw_per_frame > 0 ? cfg->max_raw_per_frame : 1024;
   std::string err;
@@ -1518,10 +1516,10 @@ int ht_detect_track(ht_ctx *ctx, const uint8_t *rgba, int n, int w, int h, int i
   if ((reinterpret_cast<uintptr_t>(rgba) & 3u) != 0) return ctx->fail(HT_ERR_ARG, "rgba must be 4-byte aligned");
   const size_t frame_bytes = (size_t)w * h * 4;
   // Detect and track have complementary bottlenecks (k_cascade: shared-memory load wavefronts; k_track: a latency
-  // chain of fp64 window passes with < 20 % LSU use), so the batch is cut into parts and the tracking of part p
+  // chain of fp64 window passes), so the batch is cut into parts and the tracking of part p
   // runs on a second stream while part p+1 is being detected.
-  // (Tracking host-frame parts on the main stream as their chunks arrive was also measured: e2e 27.3k vs 33.6k fps
-  // for one k_track over the whole batch — every k_track launch costs at least its slowest stream.)
+  // (Tracking host-frame parts on the main stream as their chunks arrive is slower than one k_track over the whole
+  // batch: every k_track launch costs at least its slowest stream.)
   const bool use_aux = n_calls > 0 && (ctx->overlap_track > 0 || (ctx->overlap_track < 0 && !is_device_ptr(rgba)));
   int parts = use_aux ? ((n >= 512) ? 4 : (n >= 128 ? 2 : 1)) : 1;
   if (use_aux && ctx->overlap_parts > 1) parts = std::min(ctx->overlap_parts, std::max(1, n / 32));
@@ -1809,7 +1807,7 @@ int ht_whitebalance(ht_ctx *ctx, const uint8_t *rgba, int n, int w, int h, doubl
   CK(ctx->d_wb_sums.reserve(mf * 3 * sizeof(unsigned long long)));
   CK(ctx->d_wb_out.reserve(mf * sizeof(double)));
   CK(cudaMemsetAsync(ctx->d_wb_sums.p, 0, (size_t)n * 3 * sizeof(unsigned long long), ctx->stream));
-  const int chunks = std::min(64, std::max(1, 1184 / n));
+  const int chunks = std::min(64, std::max(1, 8 * ctx->sms / n));
   k_wb_sums<<<dim3(chunks, n), 256, 0, ctx->stream>>>(d_rgba, (size_t)w * h * 4, w * h, ctx->d_wb_sums.as<unsigned long long>(), chunks);
   const bool out_dev = is_device_ptr(out);
   double *d_out = out_dev ? out : ctx->d_wb_out.as<double>();

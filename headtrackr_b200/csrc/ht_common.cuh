@@ -1,4 +1,4 @@
-// ht_common.cuh — structures shared by the host planner and the sm_100a kernels.
+// ht_common.cuh — structures shared by the host planner and the sm_90a kernels.
 //
 // Data layout in HBM (see DESIGN.md §3):
 //   frames   : caller-owned RGBA8, n contiguous frames of w*h*4 bytes (the "canvas" of the reference).
@@ -19,7 +19,7 @@ namespace ht {
 // Frame quads.  The pyramid arena is stored FRAME-QUAD-INTERLEAVED: one 32-bit word per pixel holds the gray
 // value of that pixel in four consecutive frames of the batch (byte f = frame & 3).  One LDS.32 / LDG.32 therefore
 // serves the same window of four frames, the resampler's tap arithmetic is shared by four frames, and a window's
-// base address never splits a bank word (round 1 lost 23 % of its shared-memory wavefronts to that).
+// base address never splits a bank word (a split word costs an extra shared-memory wavefront).
 // Arena of quad g starts at g * quad_stride words; plane offsets and pitches are in WORDS (pitch % 4 == 0).
 //
 // Cascade-tile geometry (k_cascade).  A tile is TW x TH quarter-resolution window positions x 4 phases x 4 frames.
@@ -51,7 +51,7 @@ constexpr int L2_COLS = TW + 5;               // 37 per copy
 constexpr int P2 = 76;
 // Two shared-memory arrangements of the three levels:
 //   HT_UNIBASE == 0 (default): three separate blocks (level 1 a dense box that the TMA engine can write), two per-window bases.
-//   HT_UNIBASE == 1: "super-rows" (measured 1.6 % SLOWER: 6.41 vs 6.31 ms, level 1 loses its TMA staging) - for every v one row [level-0 row 2v | level-0 row 2v+1 | level-1 row v |
+//   HT_UNIBASE == 1: "super-rows" (level 1 loses its TMA staging) - for every v one row [level-0 row 2v | level-0 row 2v+1 | level-1 row v |
 //     level-2 row v] of SR words.  Every point of every level is then  base + constant  for ONE base  v * SR + u:
 //     the late stages form an address with one add instead of select + add, and a window carries one base register.
 #ifndef HT_UNIBASE
@@ -185,8 +185,8 @@ struct ConstCascade {
 struct alignas(16) LateFeat {
   // slots 0-4: p points, 5-9: n points.  An entry is the BYTE offset of the point (4 x point_word) with bit 31 set
   // when it is relative to baseB, or 0xFFFFFFFF when the slot is unused: the kernel forms the address with one
-  // select and one add, `(int(o) < 0 ? sB - 2^31 : sA) + o` (round 2's first version unpacked 16-bit word offsets:
-  // 9 instructions per slot, 25 % of the kernel's instructions).
+  // select and one add, `(int(o) < 0 ? sB - 2^31 : sA) + o` (unpacking 16-bit word offsets instead costs
+  // 9 instructions per slot).
   uint32_t off[10];
   int32_t a_int;     // alpha[2k+1] * 1e8 (0 for the padding records of a stage's last chunk)
   uint32_t pad_;

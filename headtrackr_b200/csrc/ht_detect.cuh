@@ -1,4 +1,4 @@
-// ht_detect.cuh — sm_100a kernels for ccv.grayscale + ccv.detect_objects
+// ht_detect.cuh — sm_90a kernels for ccv.grayscale + ccv.detect_objects
 // (/root/reference/src/ccv.js:22-32, 109-333).  No tensor cores: byte compares + ordered fp64 adds.
 // The whole library is compiled with -fmad=false so that every a*b+c below is two IEEE roundings,
 // as in JavaScript.
@@ -28,7 +28,7 @@ __host__ __device__ __forceinline__ uint32_t rgb_bin(uint32_t px) {  // src/cams
 // No integer formula reproduces this: with q = 30r + 59g + 11b the exact value is q/100, and for the 167,836 of the
 // 2^24 triples with q % 100 == 50 the fp64 sum lands on either side of k + 0.5 (226 of the 253 tie values of q go
 // BOTH ways depending on (r,g,b): tests/test_gray_formula.py), so the three products and two sums are kept in fp64.
-// What round 1 paid for were the int<->fp64 CONVERSIONS (I2F.F64 / F2I.F64 run at a quarter of the fp64 rate): here
+// What costs time are the int<->fp64 CONVERSIONS (I2F.F64 / F2I.F64 run at a fraction of the fp64 rate): here
 // a byte becomes a double by planting it in the mantissa of 2^52 and subtracting 2^52 (exact), and the round-half-
 // even store is `v + 2^52` read back from the low mantissa bits (exact for 0 <= v < 2^31; proven equal to
 // rint() for every triple in the same test).  9 fp64 pipe operations per pixel, no conversions.
@@ -220,8 +220,8 @@ __global__ void __launch_bounds__(256) k_ingest(const uint8_t *__restrict__ src,
 // K2  pyramid level = canvas-shim drawImage (exact integer bilinear, see oracle/ht_oracle.h and
 // src/ccv.js:121,128,135,140,145).  One launch per pyramid "generation" (levels whose sources are
 // complete).  Block = 32 x 32 pixels of one destination plane of one frame quad; thread = one column x 4 rows.
-// Every load and store is a whole word (4 frames): the tap positions, weights and addresses - most of round 1's
-// 43 instructions per output pixel - are computed once for four frames.
+// Every load and store is a whole word (4 frames): the tap positions, weights and addresses - most of the
+// instructions of a per-frame resampler - are computed once for four frames.
 // byte f (= frame f of the quad) of a pyramid word, zero-extended
 __host__ __device__ __forceinline__ uint32_t quad_byte(uint32_t w, int f) {
 #ifdef __CUDA_ARCH__
@@ -522,7 +522,7 @@ __device__ __forceinline__ long long warp_sum_i64(long long v) {
   return (long long)(((unsigned long long)hi << 24) + lo) - (32ll << 46);
 }
 // position of the r-th (0-based) set bit of w, r < popc(w): five popcount halvings, ~25 instructions (__fns is a
-// software loop; round 2, call 8: 7 % of k_cascade's samples sat in it and its caller)
+// software loop)
 __device__ __forceinline__ int nth_bit32(uint32_t w, int r) {
   int pos = 0, t;
   t = __popc(w & 0xffffu); if (r >= t) { r -= t; pos += 16; w >>= 16; }
@@ -757,8 +757,7 @@ __global__ void __launch_bounds__(CASCADE_THREADS, HT_CASC_MINB) k_cascade(DevPl
 
   // ---- survivor masks: lane L walks the set bits of class L; warp w takes the entries of rank w, w + NW, ... ----
   // One group = stages [jb, je).  For the generated cascade the bounds are compile-time constants (integral_constant
-  // arguments): the stage loop unrolls and gen_stage's switch folds away (round 2, call 8: 3.4 % of the samples sat in
-  // that dispatch).  Returns true when the CTA is finished.
+  // arguments): the stage loop unrolls and gen_stage's switch folds away.  Returns true when the CTA is finished.
   auto run_group = [&](auto JB, auto JE, const bool emit_here) __attribute__((always_inline)) -> bool {
     const int jb = JB, je = JE;
     int n = 0;
@@ -767,8 +766,7 @@ __global__ void __launch_bounds__(CASCADE_THREADS, HT_CASC_MINB) k_cascade(DevPl
     if (warp_max_i32(n) == 0) return true;   // uniform over the CTA
     for (int i = tid; i < MASK_WORDS * 32; i += CASCADE_THREADS) m_clr[i] = 0u;   // the mask of the group after next
     // warp w takes the entries of rank [w n / NW, (w+1) n / NW) of every class: one nth_set_bit per lane and group,
-    // then a walk over consecutive set bits (round-2 call 3: rank-strided entries spent 16 % of the kernel's
-    // instructions in __fns)
+    // then a walk over consecutive set bits (rank-strided entries would need one __fns per entry)
     const int r_beg = (warp * n) / CASCADE_WARPS, r_end = ((warp + 1) * n) / CASCADE_WARPS;
     const int my_iters = r_end - r_beg;
     const int iters = warp_max_i32(my_iters);
@@ -831,7 +829,7 @@ __global__ void __launch_bounds__(CASCADE_THREADS, HT_CASC_MINB) k_cascade(DevPl
 #else
     if (run_group(IntC<6>{}, IntC<8>{}, !has_late)) return;
 #endif
-#else   // one rolled copy of the group code (62 registers, no spills) - measured slower: 6.55 vs 6.28 ms per 1024 frames
+#else   // one rolled copy of the group code (fewer registers, no spills; the stage dispatch stays in the loop)
     for (; g < c_casc.n_groups; ++g)
       if (run_group(c_casc.group_first[g], c_casc.group_first[g + 1], (g == c_casc.n_groups - 1) && !has_late)) return;
 #endif

@@ -1,5 +1,5 @@
-// ht_track.cuh — sm_100a kernels for camshift.Tracker (/root/reference/src/camshift.js) and
-// getWhitebalance (/root/reference/src/whitebalance.js).
+// ht_track.cuh — sm_90a kernels for camshift.Tracker (src/camshift.js) and
+// getWhitebalance (src/whitebalance.js) of the reference.
 //
 // The reference materialises a whole-frame back-projection (307,200 doubles in nested arrays,
 // src/camshift.js:332-353) on every track(); here the weight of a pixel is looked up on the fly
@@ -138,8 +138,8 @@ __global__ void k_pick_face(const Rect *__restrict__ det, const int32_t *__restr
 // ------------------------------------------------------------------------------------------------
 // Zero-weight marking of the bin plane.  getWeights (src/camshift.js:314-330) gives a pixel the weight
 // min(model[bin] / current[bin], 1): it is exactly +0.0 for every colour bin that does not occur in the model
-// histogram, i.e. in the face rectangle of initTracker - the vast majority of a frame's pixels (85-99 % on the bench
-// frames; a face has a few dozen to a few hundred of the 4096 bins).  Adding +0.0 to a moment sum never changes it,
+// histogram, i.e. in the face rectangle of initTracker - the vast majority of a frame's pixels (a face has a few
+// dozen to a few hundred of the 4096 bins).  Adding +0.0 to a moment sum never changes it,
 // so those pixels can be skipped.  This pass rewrites their plane entries to ZERO (0x8000 = 8 * 4096, the table's
 // extra +0.0 entry): k_track then skips every 128-pixel row segment whose entries are all ZERO with one warp vote.
 // One read + one write of the u16 plane per frame, worth it when several track() calls follow on the same frame.
@@ -230,7 +230,7 @@ __device__ __noinline__ Mom moments_serial(const uint16_t *__restrict__ px, int 
 }
 
 #ifndef HT_TRACK_MBAR
-#define HT_TRACK_MBAR 0   // 1: partial moments travel with st.async + mbarrier (no cluster barrier, one CTA barrier per pass); measured 3.20 vs 3.15 ms - no gain, left off
+#define HT_TRACK_MBAR 0   // 1: partial moments travel with st.async + mbarrier (no cluster barrier, one CTA barrier per pass); an A/B option, off by default
 #endif
 __device__ __forceinline__ double warp_sum_all(double v) {   // every lane gets the total (same tree in every warp)
 #pragma unroll
@@ -354,14 +354,14 @@ k_track(const uint16_t *__restrict__ bins, int W, int H, const int32_t *__restri
   __shared__ double red[NW][6];
   // Every CTA of the cluster keeps its OWN copy of the reference's loop state and runs the scalar mean-shift step
   // redundantly (same inputs, same operations -> bit-identical windows), so a pass needs ONE cluster barrier - the
-  // exchange of the partial moments - instead of two (round 1: partials to rank 0, barrier, rank 0 publishes the
+  // exchange of the partial moments - instead of two (partials to rank 0, barrier, rank 0 publishes the
   // next window, barrier).  cpart is double-buffered by pass parity: a CTA that is already exchanging pass p+1
   // cannot overwrite what a slower CTA still reads for pass p.
   __shared__ double cpart[2][TRACK_CLUSTER_MAX][6];  // partial moments of every CTA of the cluster (written remotely)
   // HT_TRACK_MBAR: every WARP of every CTA of the cluster sends its six partial sums straight into every CTA's wpart
   // (st.async through distributed shared memory, completing bytes on the receiver's mbarrier); warp 0 of each CTA waits
   // for 48 * C * NW bytes and adds them up in a fixed order.  Replaces red[] + __syncthreads + the cross-warp sum +
-  // cluster.sync (arrive.release / wait.acquire: 11 % of the kernel's samples plus 3.5 % for the CTA barrier).
+  // cluster.sync (arrive.release / wait.acquire).
   constexpr bool MBAR = HT_TRACK_MBAR && TRACK_CLUSTER > 1 && TRACK_CLUSTER * NW <= 128;   // (12 KB of slots at most)
   __shared__ double wpart[MBAR ? 2 : 1][MBAR ? TRACK_CLUSTER * NW : 1][6];
   __shared__ __align__(8) unsigned long long mbar[2];
@@ -458,7 +458,7 @@ k_track(const uint16_t *__restrict__ bins, int W, int H, const int32_t *__restri
   __syncthreads();
 
 #ifndef HT_TRACK_LOOP2
-#define HT_TRACK_LOOP2 0   // 1: column blocks outer, x factors per block, edge selects only where needed - measured 3.01 vs 2.97 ms: no gain, left off
+#define HT_TRACK_LOOP2 0   // 1: column blocks outer, x factors per block, edge selects only where needed - an A/B option, off by default
 #endif
 #ifndef HT_TRACK_PASSTRACE
 #define HT_TRACK_PASSTRACE 0   // 1 (profiling build): the leader thread accumulates the clock cycles of each phase of a pass
@@ -492,8 +492,8 @@ k_track(const uint16_t *__restrict__ bins, int W, int H, const int32_t *__restri
     const int yy0 = (mine - (wy % ROW_STRIDE) + ROW_STRIDE) % ROW_STRIDE;
 #if HT_TRACK_LOOP2
     if (vec4) {
-      // Round 2, call 16: under load a pass is bound by the instructions its warps issue (6 warps per scheduler), and a
-      // 16-pixel step cost ~330 of them - 50 for the four loads' address / predicate arithmetic, 16 selects for the window
+      // Under load a pass is bound by the instructions its warps issue, and a
+      // 16-pixel step costs ~330 of them - 50 for the four loads' address / predicate arithmetic, 16 selects for the window
       // edge, the x factors (4 I2F.F64 + 4 DMUL) recomputed in every step.  Here: column blocks are the OUTER loop (x
       // factors once per block, kept across its row groups), 32-bit row offsets, selects only in blocks that contain a
       // window edge (warp-uniform), the row coordinate advanced by additions.

@@ -1,5 +1,5 @@
 /*
- * headtrackr_b200.h — C ABI of libheadtrackr_b200.so: the B200-native (sm_100a) replacement for
+ * headtrackr_b200.h — C ABI of libheadtrackr_b200.so: the H100-native (sm_90a) replacement for
  * headtrackr's per-frame detect-then-track pixel kernels.
  *
  * This is the drop-in boundary (SURVEY.md §8b).  Every entry point replaces a call that
@@ -35,7 +35,7 @@
  *     ht_last_error(ctx) describes the last non-zero return.  Nothing throws across the ABI.
  *   - One context per host thread / GPU; calls on one context must be serialised by the caller
  *     (the reference is single-threaded, src/main.js:303).
- *   - There is NO CPU fallback: every entry point fails with HT_ERR_CUDA when no sm_100 device is usable.
+ *   - There is NO CPU fallback: every entry point fails with HT_ERR_CUDA when no sm_90 device is usable.
  */
 #ifndef HEADTRACKR_B200_H
 #define HEADTRACKR_B200_H

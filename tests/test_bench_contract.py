@@ -45,6 +45,25 @@ def test_gpu_arm_has_no_cpu_fallback():
     assert "no CUDA device" in (p.stderr + p.stdout)
 
 
+def test_dump_outputs_samples_a_large_output(tmp_path, monkeypatch):
+    """Above the size limit --dump-outputs writes a fixed, seeded sample of the frame axis instead of giving up."""
+    import numpy as np
+    sys.path.insert(0, str(ROOT))
+    import bench
+    monkeypatch.setattr(bench, "DUMP_LIMIT", 16000)
+    a, b = np.arange(4000).reshape(2, 1000, 2), np.arange(1000)[None, :]   # 32 KB + 8 KB in float64, frames on axis 1
+    for d in (tmp_path / "x", tmp_path / "y"):
+        bench.dump_outputs(d, {"a": a, "b": b}, axis=1)
+    files = sorted((tmp_path / "x").glob("*.npy"))
+    assert [f.stem for f in files] == ["a", "b", "sample_index"]
+    assert sum(np.load(f).nbytes for f in files) <= 16000
+    idx = np.load(tmp_path / "x" / "sample_index.npy").astype(int)
+    assert len(idx) > 0 and (np.diff(idx) > 0).all()
+    assert np.array_equal(np.load(tmp_path / "x" / "a.npy"), a[:, idx]) and np.array_equal(np.load(tmp_path / "x" / "b.npy"), b[:, idx])
+    for f in files:
+        assert np.array_equal(np.load(f), np.load(tmp_path / "y" / f.name))
+
+
 def test_usable_cores_is_bounded_by_the_affinity_mask():
     sys.path.insert(0, str(ROOT))
     import bench

@@ -209,6 +209,22 @@ def test_single_rank_line(pipeline):
     assert line["config"]["pipeline"].startswith("on" if pipeline else "off")
 
 
+@pytest.mark.parametrize("pipeline", [0, 1])
+def test_dump_outputs_of_the_last_timed_step(pipeline, tmp_path):
+    """--steps sets the timed steps (one fake launch each); --dump-outputs writes the last one's records as float64."""
+    argv = ["--width", "64", "--height", "48", "--batch", "8", "--steps", "2", "--warmup", "1", "--no-cpu-baseline",
+            "--pipeline", str(pipeline), "--dump-outputs", str(tmp_path)]
+    line = json.loads(launch(1, argv)[0].strip().splitlines()[-1])
+    assert line["steps"] == 2 and line["gpu_launches"] == 2
+    names = {p.stem for p in tmp_path.glob("*.npy")}
+    assert names == {"rects", "neighbors", "counts", "found", "track_xywh", "track_angle", "windows"}
+    xywh = np.load(tmp_path / "track_xywh.npy")
+    assert xywh.dtype == np.float64 and xywh.shape == (8, 4)
+    from headtrackr_b200 import synth
+    want = [checksum(synth.frame(i, 64, 48)) for i in range(8)]     # the bench's batch: frames 0..7, unrolled
+    assert xywh[:, 0].tolist() == want                              # (pipelined: the last step's tracking was joined)
+
+
 @pytest.mark.parametrize("pipeline,workload", [(0, "detect_track30"), (1, "detect_track30"), (0, "detect")])
 def test_two_ranks_same_collectives_and_right_records(pipeline, workload):
     """Skewed ranks: a rank-local loop exit or a mis-ordered gather would hang gloo (the queue read times out) or trip

@@ -16,7 +16,7 @@ import numpy as np
 import pytest
 
 import oracle
-from headtrackr_b200 import synth
+from headtrackr_b200 import _lib, synth
 
 ROOT = Path(__file__).resolve().parent.parent
 CSRC = ROOT / "headtrackr_b200" / "csrc"
@@ -25,7 +25,7 @@ CSRC = ROOT / "headtrackr_b200" / "csrc"
 @pytest.fixture(scope="module")
 def st(tmp_path_factory):
     so = tmp_path_factory.mktemp("selftest") / "libht_selftest.so"
-    subprocess.check_call(["/usr/local/cuda/bin/nvcc", "-DHT_HOST_SELFTEST", "-gencode", "arch=compute_100a,code=sm_100a",
+    subprocess.check_call([_lib.nvcc(), "-DHT_HOST_SELFTEST", "-gencode", "arch=compute_90a,code=sm_90a",
                            "-O2", "-std=c++17", "-fmad=false", "-Xcompiler", "-fPIC", "-shared", "-o", str(so),
                            str(CSRC / "ht_api.cu")], stderr=subprocess.DEVNULL)
     L = C.CDLL(str(so))

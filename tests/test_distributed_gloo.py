@@ -72,10 +72,11 @@ def loop_worker(rank, world, port, q):
     os.environ["MASTER_ADDR"] = "127.0.0.1"
     os.environ["MASTER_PORT"] = str(port)
     dist.init_process_group("gloo", rank=rank, world_size=world)
+    dist.barrier()                                   # the group's first collective (connection set-up) stays out of the window
     t_w = time.perf_counter() - 0.05 * rank          # rank 1's clock started 50 ms "earlier": it would leave the loop first
     iters = 0
     rec = torch.full((4,), float(rank))
-    while agreed(time.perf_counter() - t_w < 0.25):
+    while agreed(time.perf_counter() - t_w < 1.0):   # a window long enough for >= 10 iterations on a loaded host
         out = [torch.zeros(4) for _ in range(world)]
         dist.all_gather(out, rec)                    # the step's result gather
         time.sleep(0.005)

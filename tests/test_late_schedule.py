@@ -10,6 +10,8 @@ from pathlib import Path
 
 import pytest
 
+from headtrackr_b200 import _lib
+
 ROOT = Path(__file__).resolve().parent.parent
 CSRC = ROOT / "headtrackr_b200" / "csrc"
 
@@ -17,7 +19,7 @@ CSRC = ROOT / "headtrackr_b200" / "csrc"
 @pytest.fixture(scope="module")
 def selftest(tmp_path_factory):
     exe = tmp_path_factory.mktemp("selftest") / "ht_selftest"
-    subprocess.check_call(["/usr/local/cuda/bin/nvcc", "-DHT_HOST_SELFTEST", "-gencode", "arch=compute_100a,code=sm_100a",
+    subprocess.check_call([_lib.nvcc(), "-DHT_HOST_SELFTEST", "-gencode", "arch=compute_90a,code=sm_90a",
                            "-O1", "-std=c++17", "-fmad=false", "-o", str(exe), str(CSRC / "ht_api.cu")],
                           stderr=subprocess.DEVNULL)
     out = subprocess.check_output([str(exe), str(ROOT / "headtrackr_b200" / "data" / "cascade_face.bin")], text=True)

@@ -5,8 +5,9 @@ For one synthetic frame it evaluates the cascade for every window with numpy (sa
 reference; checked against the oracle's survivor count), then replays the kernel's work distribution tile by tile —
 dense first group, 32 bank-class survivor lists, lane-per-window stage groups, warp-per-window late stages — and
 counts the LDS wavefronts each variant would issue, including bank-conflict replays.  Used to rank layout /
-grouping ideas before spending GPU time on them (profiles/r01_lab_notes.md); the `current` variant is calibrated
-against the ncu capture (2.13 M shared-load wavefronts and 0.49 M conflict replays per 640x480 frame).
+grouping ideas before spending GPU time on them.  Its counts depend on the kernel's layout, not on the GPU; check
+the `current` variant against an ncu capture of k_cascade (shared-load wavefronts and conflict replays per frame)
+before relying on it.
 
     python tools/cascade_wavefront_model.py [frame_index] [W H]
 """

@@ -2,9 +2,8 @@
 """CPU model of k_track's launch schedule (strict mode: every mean-shift pass summed).
 
 Per-stream work comes from the CPU oracle (passes per call and window sizes of the bench mix); the time of a pass on a
-cluster of c CTAs is read off the measured single-stream chain times (tools/track_chain_probe.py, profiles/
-r01_lab_notes.md); the GPU is 444 CTA slots (3 CTAs of 256 threads per SM) filled strictly in launch order, as the
-block scheduler does.  Prints the makespan of a few launch orders / cluster assignments to rank ideas for the
+cluster of c CTAs is read off single-stream chain times (PX_T / US below, from tools/track_chain_probe.py); the GPU
+is 3 * SMS CTA slots (3 CTAs of 256 threads per SM) filled strictly in launch order, as the block scheduler does.  Prints the makespan of a few launch orders / cluster assignments to rank ideas for the
 streams whose chains end last.
 
     python tools/track_schedule_model.py [n_streams]
@@ -21,8 +20,11 @@ sys.path.insert(0, str(ROOT))
 import oracle  # noqa: E402  (analysis tool, not the product)
 from headtrackr_b200 import synth  # noqa: E402
 
-W, H, CALLS, SLOTS = 640, 480, 30, 444
-# microseconds per pass vs pixels per thread, one stream alone (frame 58 at 1/2/4/8 CTAs; a whole-frame window at 2)
+SMS = 132              # H100 SXM
+W, H, CALLS, SLOTS = 640, 480, 30, 3 * SMS
+# microseconds per pass vs pixels per thread, one stream alone (frame 58 at 1/2/4/8 CTAs; a whole-frame window at 2).
+# Taken on an earlier GPU and not re-measured on H100: re-run tools/track_chain_probe.py there before trusting
+# absolute makespans (the model ranks launch orders, which depend mostly on the shape of this curve).
 PX_T = [0, 24, 48, 96, 192, 600, 1200]
 US = [2.6, 3.4, 4.65, 6.6, 8.85, 16.0, 30.0]
 LOAD_FACTOR = 1.3      # passes are ~30 % slower when every SM holds 3 busy CTAs (timeline vs probe)
