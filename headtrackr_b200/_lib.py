@@ -54,6 +54,20 @@ class HeadEvent(C.Structure):
                 ("fx", C.c_double), ("fy", C.c_double), ("fwidth", C.c_double), ("fheight", C.c_double)]
 
 
+class TrackerParams(C.Structure):
+    _fields_ = [("retry_detection", C.c_int32), ("calc_angles", C.c_int32), ("pad_", C.c_int32 * 2), ("head", HeadParams)]
+
+
+class TrackerEvent(C.Structure):
+    _fields_ = [("detection", C.c_int32), ("status", C.c_int32), ("x", C.c_double), ("y", C.c_double),
+                ("width", C.c_double), ("height", C.c_double), ("angle", C.c_double), ("confidence", C.c_double),
+                ("wb", C.c_double), ("running", C.c_int32), ("pad_", C.c_int32), ("fov", C.c_double), ("head", HeadEvent)]
+
+
+# headtrackrStatus names of ht_tracker_event.status, bit 0 first (= the order src/main.js dispatches them in)
+TRACKER_STATUS = ("whitebalance", "detecting", "hints", "redetecting", "lost", "stopped", "found")
+
+
 class Config(C.Structure):
     _fields_ = [("device", C.c_int32), ("max_width", C.c_int32), ("max_height", C.c_int32),
                 ("max_frames", C.c_int32), ("max_raw_per_frame", C.c_int32), ("max_rects_per_frame", C.c_int32),
@@ -89,7 +103,8 @@ def build(force=False):
 _lib = None
 
 EXPORTS = ["ht_version", "ht_create", "ht_destroy", "ht_last_error", "ht_sync", "ht_max_rects", "ht_detect",
-           "ht_track_init", "ht_track_init_from_detect", "ht_track", "ht_detect_track", "ht_stream_reset", "ht_stream_step", "ht_stream_head_config", "ht_stream_step_head", "ht_ingest", "ht_backprojection", "ht_whitebalance",
+           "ht_track_init", "ht_track_init_from_detect", "ht_track", "ht_detect_track", "ht_stream_reset", "ht_stream_step", "ht_stream_head_config", "ht_stream_step_head",
+           "ht_tracker_config", "ht_tracker_reset", "ht_tracker_start", "ht_tracker_stop", "ht_tracker_step", "ht_ingest", "ht_backprojection", "ht_whitebalance",
            "ht_plan_info", "ht_debug_plane", "ht_debug_raw", "ht_debug_model_hist", "ht_debug_track_stats", "ht_set_track_memo", "ht_set_pipeline", "ht_join", "ht_debug_set_exactness", "ht_debug_track_trace", "ht_debug_track_phases", "ht_launch_count",
            "ht_profile", "ht_profile_read"]
 
@@ -125,6 +140,10 @@ def lib():
     L.ht_stream_step.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp]
     L.ht_stream_head_config.argtypes = [vp, vp]
     L.ht_stream_step_head.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp]
+    L.ht_tracker_config.argtypes = [vp, vp]
+    for f in (L.ht_tracker_reset, L.ht_tracker_start, L.ht_tracker_stop):
+        f.argtypes = [vp, C.c_int, C.c_int]
+    L.ht_tracker_step.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, C.c_double, vp]
     L.ht_ingest.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, vp, C.c_int, C.c_int]
     L.ht_backprojection.argtypes = [vp, C.c_int, vp, C.c_int, C.c_int, vp]
     L.ht_whitebalance.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, vp]

@@ -8,7 +8,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from ._lib import HeadEvent, HeadParams, HtError, Rect, StreamEvent, TrackObj, Window
+from ._lib import HeadEvent, HeadParams, HtError, Rect, StreamEvent, TrackerEvent, TrackerParams, TrackObj, Window
 from .synth import load_cascade_blob
 
 
@@ -218,6 +218,42 @@ class Context:
         return [dict(detection=("", "VJ", "CS")[e.detection], x=e.x, y=e.y, width=e.width, height=e.height, angle=e.angle,
                      confidence=e.confidence, found=bool(e.status & 1), lost=bool(e.status & 2)) for e in ev]
 
+    # ---- headtrackr.Tracker lifecycle for n streams, on the device ----
+    def tracker_config(self, retryDetection=True, calcAngles=False, smoothing=True, fov=None, cameraOffset=11.5,
+                       headPosition=True, edgecorrection=True, alpha=0.35, distance_to_screen=60.0, enable=True):
+        """Switch the per-stream headtrackr.Tracker lifecycle on with the reference's parameters (src/main.js:39-55),
+        or off (enable=False: every stream goes back to stream_reset's state)."""
+        if not enable:
+            self._check(self._L.ht_tracker_config(self._h, None))
+            return
+        head = HeadParams(int(bool(smoothing)), int(bool(headPosition)), int(bool(edgecorrection)), 0, alpha,
+                          float(fov) if fov is not None else 0.0, cameraOffset, distance_to_screen)
+        p = TrackerParams(int(bool(retryDetection)), int(bool(calcAngles)), (C.c_int32 * 2)(), head)
+        self._check(self._L.ht_tracker_config(self._h, C.addressof(p)))
+
+    def tracker_reset(self, first=0, n=None):
+        """Streams [first, first+n): a new headtrackr.Tracker, initialised, not running."""
+        self._check(self._L.ht_tracker_reset(self._h, first, self.max_frames - first if n is None else n))
+
+    def tracker_start(self, first=0, n=None):
+        """start() for streams [first, first+n): their next frame goes through the starter (no-op if running)."""
+        self._check(self._L.ht_tracker_start(self._h, first, self.max_frames - first if n is None else n))
+
+    def tracker_stop(self, first=0, n=None):
+        """stop() for streams [first, first+n); the "stopped" status is the caller's to emit."""
+        self._check(self._L.ht_tracker_stop(self._h, first, self.max_frames - first if n is None else n))
+
+    def tracker_step(self, frames, now_ms, out=None):
+        """One timer tick of streams [0, n) -> list of ht_tracker_event records as dicts (tracker_event_dict).
+        out: a torch CUDA uint8 tensor of n*144 bytes -> asynchronous, nothing returned (tracker_events_from_bytes)."""
+        ptr, n, H, W, keep = _frames_ptr(frames)
+        if out is not None:
+            self._check(self._L.ht_tracker_step(self._h, ptr, n, W, H, float(now_ms), out.data_ptr()))
+            return None
+        ev = (TrackerEvent * n)()
+        self._check(self._L.ht_tracker_step(self._h, ptr, n, W, H, float(now_ms), C.addressof(ev)))
+        return [tracker_event_dict(e) for e in ev]
+
     def ingest(self, frames, width, height, out=None):
         """drawImage(video, 0, 0, width, height) for a batch (src/main.js:170).  numpy in -> numpy (n, height, width, 4)
         out; with a torch CUDA `out` tensor the result stays on the device."""
@@ -301,3 +337,19 @@ class Context:
         out = np.zeros(4096, np.uint32)
         self._check(self._L.ht_debug_model_hist(self._h, slot, out.ctypes.data))
         return out
+
+
+def tracker_event_dict(e):
+    """ht_tracker_event -> dict with the reference's names; status = the list of headtrackrStatus messages dispatched"""
+    return dict(detection=("", "VJ", "CS", "WB")[e.detection], x=e.x, y=e.y, width=e.width, height=e.height,
+                angle=e.angle, confidence=e.confidence, wb=e.wb, running=bool(e.running), fov=e.fov,
+                status=[s for b, s in enumerate(_lib.TRACKER_STATUS) if e.status >> b & 1],
+                head=dict(valid=bool(e.head.valid), x=e.head.x, y=e.head.y, z=e.head.z,
+                          face=(e.head.fx, e.head.fy, e.head.fwidth, e.head.fheight)))
+
+
+def tracker_events_from_bytes(buf):
+    """records written to a device buffer by Context.tracker_step(out=...), copied back as bytes"""
+    n = len(buf) // C.sizeof(TrackerEvent)
+    arr = (TrackerEvent * n).from_buffer_copy(bytes(buf[: n * C.sizeof(TrackerEvent)]))
+    return [tracker_event_dict(e) for e in arr]

@@ -551,6 +551,9 @@ struct ht_ctx {
   DevBuf d_stream_mode, d_stream_mask, d_stream_cs, d_stream_init, d_stream_events;   // ht_stream_step
   DevBuf d_head_state, d_head_params, d_head_events;                                  // ht_stream_head_config
   bool head_on = false;
+  DevBuf d_tracker_state, d_tracker_params, d_tracker_events, d_tracker_wb;          // ht_tracker_config
+  bool tracker_on = false;
+  int tracker_calc_angles = 0;
   bool track_history = true;                // order by the cost of each stream's previous launch (HT_TRACK_HISTORY=0: by window area)
   DevBuf d_track_cost;                      // [max_frames][2] {passes, window pixels / 256} per slot
   int track_heavy_div = 128;                // >0: the n/div costliest streams run on a cluster of
@@ -1156,7 +1159,7 @@ int upload_chunks(ht_ctx *ctx, const uint8_t *rgba, int n, size_t frame_bytes, i
 // ================================================================================================
 extern "C" {
 
-uint32_t ht_version(void) { return (1u << 16) | 0u; }
+uint32_t ht_version(void) { return (1u << 16) | 1u; }
 
 const char *ht_last_error(const ht_ctx *ctx) { return ctx ? ctx->err.c_str() : g_create_error.c_str(); }
 
@@ -1272,7 +1275,7 @@ void ht_destroy(ht_ctx *ctx) {
   for (auto &kv : ctx->plans) kv.second->dev.release();
   DevBuf *bufs[] = {&ctx->d_casc, &ctx->arena, &ctx->d_frames, &ctx->raw_keys, &ctx->raw_conf, &ctx->raw_count, &ctx->sorted,
                     &ctx->labels, &ctx->seq2, &ctx->d_out_rects, &ctx->d_out_counts, &ctx->d_flags, &ctx->model_hist,
-                    &ctx->bins, &ctx->d_sched, &ctx->d_trace, &ctx->d_tmaps, &ctx->d_late_chunk0, &ctx->d_track_cost, &ctx->d_stream_mode, &ctx->d_stream_mask, &ctx->d_stream_cs, &ctx->d_stream_init, &ctx->d_stream_events, &ctx->d_head_state, &ctx->d_head_params, &ctx->d_head_events, &ctx->cur_hist, &ctx->track_state, &ctx->d_slots, &ctx->d_rects, &ctx->d_found, &ctx->d_objs,
+                    &ctx->bins, &ctx->d_sched, &ctx->d_trace, &ctx->d_tmaps, &ctx->d_late_chunk0, &ctx->d_track_cost, &ctx->d_stream_mode, &ctx->d_stream_mask, &ctx->d_stream_cs, &ctx->d_stream_init, &ctx->d_stream_events, &ctx->d_head_state, &ctx->d_head_params, &ctx->d_head_events, &ctx->d_tracker_state, &ctx->d_tracker_params, &ctx->d_tracker_events, &ctx->d_tracker_wb, &ctx->cur_hist, &ctx->track_state, &ctx->d_slots, &ctx->d_rects, &ctx->d_found, &ctx->d_objs,
                     &ctx->d_windows, &ctx->d_wb_sums, &ctx->d_wb_out, &ctx->d_scratch};
   for (DevBuf *b : bufs) b->release();
   for (auto &sp : ctx->prof_spans) { cudaEventDestroy(sp.a); cudaEventDestroy(sp.b); }
@@ -1676,6 +1679,7 @@ int ht_stream_step_head(ht_ctx *ctx, const uint8_t *rgba, int n, int w, int h, i
   if (!ctx) return HT_ERR_ARG;
   if (!out_events) return ctx->fail(HT_ERR_ARG, "out_events is NULL");
   if (out_head && !ctx->head_on) return ctx->fail(HT_ERR_STATE, "ht_stream_head_config has not been called");
+  if (ctx->tracker_on) return ctx->fail(HT_ERR_STATE, "the tracker lifecycle is configured (ht_tracker_config): its streams own the tracker slots");
   int rc = check_batch(ctx, n);
   if (rc != HT_OK) return rc;
   CK(cudaSetDevice(ctx->cfg.device));
@@ -1728,6 +1732,138 @@ int ht_stream_step_head(ht_ctx *ctx, const uint8_t *rgba, int n, int w, int h, i
   if (!is_device_ptr(out_events)) { CK(cudaMemcpyAsync(out_events, d_ev, sizeof(StreamEvent) * (size_t)n, cudaMemcpyDeviceToHost, st)); any_host = true; }
   if (out_head && !is_device_ptr(out_head)) { CK(cudaMemcpyAsync(out_head, d_he, sizeof(HeadEvent) * (size_t)n, cudaMemcpyDeviceToHost, st)); any_host = true; }
   if (any_host) return ht_sync(ctx);
+  return HT_OK;
+}
+
+static_assert(sizeof(ht_tracker_event) == sizeof(TrackerEvent) && sizeof(ht_tracker_event) == 144, "ht_tracker_event layout");
+static_assert(sizeof(ht_tracker_params) == 64, "ht_tracker_params layout");
+
+static TrackerParams make_tracker_params(const ht_tracker_params *p) {
+  TrackerParams tp{};
+  tp.retry_detection = p->retry_detection;
+  tp.calc_angles = p->calc_angles;
+  tp.head = make_head_params(&p->head);
+  return tp;
+}
+
+static int tracker_control(ht_ctx *ctx, int first, int n, int op) {
+  if (!ctx) return HT_ERR_ARG;
+  if (!ctx->tracker_on) return ctx->fail(HT_ERR_STATE, "ht_tracker_config has not been called");
+  if (first < 0 || n <= 0 || first + n > ctx->cfg.max_frames) return ctx->fail(HT_ERR_ARG, "stream range outside [0,%d)", ctx->cfg.max_frames);
+  { const int jr = join_aux(ctx); if (jr != HT_OK) return jr; }
+  CK(cudaSetDevice(ctx->cfg.device));
+  k_tracker_control<<<(unsigned)((n + 127) / 128), 128, 0, ctx->stream>>>(ctx->d_tracker_state.as<TrackerState>(), first, n, op);
+  ++ctx->launches;
+  CK(cudaGetLastError());
+  return HT_OK;
+}
+
+int ht_tracker_config(ht_ctx *ctx, const ht_tracker_params *params) {
+  if (!ctx) return HT_ERR_ARG;
+  { const int jr = join_aux(ctx); if (jr != HT_OK) return jr; }
+  CK(cudaSetDevice(ctx->cfg.device));
+  const size_t mf = (size_t)ctx->cfg.max_frames;
+  if (!params) {                 // off: every stream as after ht_stream_reset (the lifecycle has used the tracker slots)
+    if (ctx->tracker_on) {
+      ctx->tracker_on = false;
+      if (ctx->d_stream_mode.p) CK(cudaMemsetAsync(ctx->d_stream_mode.p, 0, mf * sizeof(int32_t), ctx->stream));
+      if (ctx->d_head_state.p) {
+        k_head_reset<<<(unsigned)((mf + 127) / 128), 128, 0, ctx->stream>>>(ctx->d_head_state.as<HeadState>(), 0, (int)mf);
+        ++ctx->launches;
+      }
+      CK(cudaGetLastError());
+    }
+    return HT_OK;
+  }
+  const ht_head_params &hp = params->head;
+  if (!(hp.alpha >= 0.0 && hp.alpha <= 1.0) || !(hp.distance_to_screen > 0.0)) return ctx->fail(HT_ERR_ARG, "bad head parameters");
+  if (!ctx->d_tracker_state.p) {
+    CK(ctx->d_tracker_state.reserve(mf * sizeof(TrackerState)));
+    CK(ctx->d_tracker_params.reserve(sizeof(TrackerParams)));
+    CK(ctx->d_tracker_events.reserve(mf * sizeof(TrackerEvent)));
+    CK(ctx->d_tracker_wb.reserve(mf));
+  }
+  const TrackerParams tp = make_tracker_params(params);
+  CK(cudaMemcpyAsync(ctx->d_tracker_params.p, &tp, sizeof(tp), cudaMemcpyHostToDevice, ctx->stream));
+  if (!ctx->tracker_on) {
+    k_tracker_control<<<(unsigned)((mf + 127) / 128), 128, 0, ctx->stream>>>(ctx->d_tracker_state.as<TrackerState>(), 0, (int)mf, 0);
+    ++ctx->launches;
+    CK(cudaGetLastError());
+  }
+  CK(cudaStreamSynchronize(ctx->stream));    // `tp` is a local
+  ctx->tracker_calc_angles = params->calc_angles ? 1 : 0;
+  ctx->tracker_on = true;
+  return HT_OK;
+}
+
+int ht_tracker_reset(ht_ctx *ctx, int first, int n) { return tracker_control(ctx, first, n, 0); }
+int ht_tracker_start(ht_ctx *ctx, int first, int n) { return tracker_control(ctx, first, n, 1); }
+int ht_tracker_stop(ht_ctx *ctx, int first, int n) { return tracker_control(ctx, first, n, 2); }
+
+// One timer tick of n headtrackr.Tracker streams, entirely on the device:
+//   k_tracker_plan   modes -> VJ frame-quad mask, CS enable, whitebalance enable
+//   k_wb_sums        whitebalance sums of the STARTING and WB streams only       src/whitebalance.js, src/main.js:316
+//   run_detect       the VJ streams (interval 5, min_neighbors 1)                 src/facetrackr.js:147-149
+//   k_hist, k_track  one track() of the CS streams                                src/camshift.js:213-312
+//   k_tracker_update starter, whitebalance gate, facetrackr and main.js transitions, status bits, head epilogue
+//   k_track_init     initTracker for the streams that found their face           src/facetrackr.js:97-108
+int ht_tracker_step(ht_ctx *ctx, const uint8_t *rgba, int n, int w, int h, double now_ms, ht_tracker_event *out) {
+  if (!ctx) return HT_ERR_ARG;
+  if (!ctx->tracker_on) return ctx->fail(HT_ERR_STATE, "ht_tracker_config has not been called");
+  if (!out) return ctx->fail(HT_ERR_ARG, "out is NULL");
+  int rc = check_batch(ctx, n);
+  if (rc != HT_OK) return rc;
+  CK(cudaSetDevice(ctx->cfg.device));
+  Plan *P = nullptr;
+  rc = get_plan(ctx, w, h, 5, &P);
+  if (rc != HT_OK) return rc;
+  rc = ensure_tracker_buffers(ctx);
+  if (rc != HT_OK) return rc;
+  rc = ensure_stream_buffers(ctx);           // the mask scratch of ht_stream_step (the two never run on one context at once)
+  if (rc != HT_OK) return rc;
+  const uint8_t *d_rgba = nullptr;
+  rc = device_frames(ctx, rgba, n, w, h, &d_rgba);
+  if (rc != HT_OK) return rc;
+  CK(ctx->bins.reserve((size_t)n * w * h * sizeof(uint16_t)));
+  CK(ctx->d_wb_sums.reserve((size_t)ctx->cfg.max_frames * 3 * sizeof(unsigned long long)));
+  cudaStream_t st = ctx->stream;
+  TrackerState *ts = ctx->d_tracker_state.as<TrackerState>();
+  uint8_t *vj_mask = ctx->d_stream_mask.as<uint8_t>(), *cs_en = ctx->d_stream_cs.as<uint8_t>(), *init_en = ctx->d_stream_init.as<uint8_t>();
+  uint8_t *wb_en = ctx->d_tracker_wb.as<uint8_t>();
+  k_tracker_plan<<<(n + 127) / 128, 128, 0, st>>>(ts, n, vj_mask, cs_en, init_en, wb_en);
+  CK(cudaMemsetAsync(ctx->d_wb_sums.p, 0, (size_t)n * 3 * sizeof(unsigned long long), st));
+  const int chunks = std::min(64, std::max(1, 8 * ctx->sms / n));
+  k_wb_sums<<<dim3(chunks, n), 256, 0, st>>>(d_rgba, (size_t)w * h * 4, w * h, ctx->d_wb_sums.as<unsigned long long>(), chunks, wb_en);
+  ctx->launches += 2;
+  rc = run_detect(ctx, P, d_rgba, 0, n, 1, ctx->d_out_rects.as<Rect>(), ctx->d_out_counts.as<int32_t>(),
+                  HistOut{nullptr, nullptr}, vj_mask);
+  if (rc != HT_OK) return rc;
+  rc = launch_hist(ctx, d_rgba, n, w, h, ctx->cur_hist.as<uint32_t>(), ctx->bins.as<uint16_t>(), cs_en);
+  if (rc != HT_OK) return rc;
+  ctx->prof_begin(HT_PROF_TRACK);
+  rc = launch_track(ctx, n, 0, ctx->bins.as<uint16_t>(), w, h, nullptr, ctx->model_hist.as<uint32_t>(),
+                    ctx->cur_hist.as<uint32_t>(), ctx->track_state.as<TrackState>(), 1, ctx->d_objs.as<int32_t>(), nullptr,
+                    ctx->d_flags.as<int32_t>() + 2, cs_en);
+  if (rc != HT_OK) return rc;
+  ctx->prof_end();
+  const bool out_dev = is_device_ptr(out);
+  TrackerEvent *d_ev = out_dev ? reinterpret_cast<TrackerEvent *>(out) : ctx->d_tracker_events.as<TrackerEvent>();
+  k_tracker_update<<<(n + 127) / 128, 128, 0, st>>>(ts, ctx->d_tracker_params.as<TrackerParams>(), n,
+                                                    ctx->d_wb_sums.as<unsigned long long>(), w * h, ctx->d_out_rects.as<Rect>(),
+                                                    ctx->d_out_counts.as<int32_t>(), ctx->K, ctx->d_objs.as<int32_t>(),
+                                                    ctx->d_rects.as<int32_t>(), init_en, now_ms, w, h, d_ev);
+  ctx->prof_begin(HT_PROF_TRACK_INIT);
+  k_track_init<<<n, 256, 0, st>>>(d_rgba, (size_t)w * h * 4, w, h, nullptr, ctx->d_rects.as<int32_t>(), ctx->tracker_calc_angles,
+                                  ctx->model_hist.as<uint32_t>(), ctx->track_state.as<TrackState>(), nullptr, init_en);
+  ctx->prof_end();
+  ctx->launches += 2;
+  CK(cudaGetLastError());
+  ctx->last_plan = P;
+  ctx->last_n = n;
+  if (!out_dev) {
+    CK(cudaMemcpyAsync(out, d_ev, sizeof(TrackerEvent) * (size_t)n, cudaMemcpyDeviceToHost, st));
+    return ht_sync(ctx);
+  }
   return HT_OK;
 }
 
@@ -2016,6 +2152,31 @@ extern "C" int ht_selftest_head(const ht_head_params *params, int n, const doubl
     memcpy(out + i, &he, sizeof(he));
   }
   return 0;
+}
+
+// the lifecycle state machine of k_tracker_update / k_tracker_control (tracker_step, tracker_start, ...) for one stream,
+// one call at a time, fed by the caller with the pixel results the stream's mode asks for.  op: 0 = new state,
+// 1 = start(), 2 = stop(), 3 = one frame (wb, det[0, count), obj as tracker_step takes them; out = its record;
+// seed[5] = {initTracker follows, x, y, w, h}).  `state` holds ht_selftest_tracker_size() bytes.  -> the mode after op.
+extern "C" int ht_selftest_tracker_size(void) { return (int)sizeof(TrackerState); }
+extern "C" int ht_selftest_tracker(void *state, int op, const ht_tracker_params *params, double wb, const ht_rect *det,
+                                   int count, const ht_trackobj *obj, double now_ms, int camw, int camh, ht_tracker_event *out,
+                                   int32_t *seed) {
+  TrackerState &s = *static_cast<TrackerState *>(state);
+  if (op == 0) tracker_new_state(s);
+  else if (op == 1) tracker_start(s);
+  else if (op == 2) tracker_stop(s);
+  else {
+    const TrackerParams tp = make_tracker_params(params);
+    int32_t zero_obj[6] = {0, 0, 0, 0, 0, 0};
+    TrackerEvent e;
+    bool sd;
+    tracker_step(s, tp, wb, reinterpret_cast<const Rect *>(det), count, obj ? reinterpret_cast<const int32_t *>(obj) : zero_obj,
+                 now_ms, (double)camw, (double)camh, e, seed + 1, sd);
+    seed[0] = sd ? 1 : 0;
+    memcpy(out, &e, sizeof(e));
+  }
+  return s.mode;
 }
 
 // k_ingest's per-pixel code over a whole frame batch

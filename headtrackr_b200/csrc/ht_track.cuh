@@ -913,14 +913,17 @@ __host__ __device__ inline void head_new_state(HeadState &s) {
   s.fov_saved_deg = 0.0; s.tan_fov_width = 0.0; s.head_diag_cam = 0.0;
 }
 
-// one frame of one stream: (x, y, w, h) = the CS TrackObj, lost = width or height 0
+// one frame of one stream: (x, y, w, h) = the CS TrackObj, lost = width or height 0.  retry: what a lost face does -
+// with retryDetection (src/main.js:231-238) faceFound and headposition start over; without it (src/main.js:246-247,
+// stop() :347-355) only faceFound does: smoother, head diagonals, firstRun, fov and headposition survive.
 __host__ __device__ inline void head_step(HeadState &s, const HeadParams &p, bool is_cs, double x, double y, double w, double h,
-                                          bool lost, double camw, double camh, HeadEvent &out) {
+                                          bool lost, double camw, double camh, HeadEvent &out, bool retry = true) {
   const double PI = 3.141592653589793;
   out.valid = 0; out.status = 0; out.x = out.y = out.z = 0.0; out.fx = out.fy = out.fwidth = out.fheight = 0.0;
   if (!is_cs) return;
-  if (lost) {                                  // src/main.js:230-244: new facetrackr, faceFound = false, headposition = undefined
-    s.face_found = 0; s.hp_init = 0;
+  if (lost) {
+    s.face_found = 0;
+    if (retry) s.hp_init = 0;
     return;
   }
   if (!s.face_found) { out.status |= 1; s.face_found = 1; }          // :246-249
@@ -1034,6 +1037,47 @@ __global__ void k_stream_plan(const int32_t *__restrict__ mode, int n, uint8_t *
   }
 }
 
+// One "VJ" or "CS" pass of facetrackr for one stream (shared by ht_stream_step and ht_tracker_step).
+//   vj: pick from the ccv result list det[0, count); else read the camshift TrackObj obj = {x, y, w, h, angle (fp64)}.
+// Fills the TrackObj record e (status bit 0: face found, bit 1: face lost) and returns the next mode (0 = "VJ",
+// 1 = "CS").  seed: the tracker must be seeded with rect on this same frame.
+__host__ __device__ inline int facetrackr_pass(bool vj, const Rect *det, int count, const int32_t *obj, StreamEvent &e,
+                                               int32_t rect[4], bool &seed) {
+  seed = false;
+  e.status = 0;
+  e.x = e.y = e.width = e.height = e.angle = 0.0;     // new TrackObj(), src/facetrackr.js:233-241
+  e.confidence = -10000.0;
+  if (vj) {                                            // doVJDetection, src/facetrackr.js:137-175
+    e.detection = 1;
+    if (count > 0) {
+      int best = 0;
+      for (int i = 1; i < count; ++i)
+        if (det[i].confidence > det[best].confidence) best = i;   // first maximum, :161-165
+      e.x = det[best].x; e.y = det[best].y; e.width = det[best].width; e.height = det[best].height;
+      e.confidence = det[best].confidence;
+    }
+    if (e.confidence > -10.0) {                        // :97: switch to camshift, initTracker on THIS frame
+      rect[0] = (int32_t)floor(e.x); rect[1] = (int32_t)floor(e.y);
+      rect[2] = (int32_t)floor(e.width); rect[3] = (int32_t)floor(e.height);
+      seed = true;
+      e.status |= 1;
+      return 1;
+    }
+    return 0;
+  }
+  e.detection = 2;                                     // doCSDetection, src/facetrackr.js:178-209
+  e.x = obj[0]; e.y = obj[1]; e.width = obj[2]; e.height = obj[3];
+  double angle;
+  memcpy(&angle, obj + 4, sizeof(angle));
+  e.angle = angle;
+  e.confidence = 1.0;
+  if (obj[2] == 0 || obj[3] == 0) {                    // src/main.js:230: lost -> a fresh facetrackr without whitebalancing
+    e.status |= 2;
+    return 0;
+  }
+  return 1;
+}
+
 __global__ void k_stream_update(int32_t *__restrict__ mode, int n, const Rect *__restrict__ det,
                                 const int32_t *__restrict__ counts, int K, const int32_t *__restrict__ objs,
                                 int32_t *__restrict__ rects, uint8_t *__restrict__ init_enable,
@@ -1045,37 +1089,13 @@ __global__ void k_stream_update(int32_t *__restrict__ mode, int n, const Rect *_
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= n) return;
   StreamEvent e;
-  e.status = 0;
-  e.x = e.y = e.width = e.height = e.angle = 0.0;     // new TrackObj(), src/facetrackr.js:233-241
-  e.confidence = -10000.0;
-  if (mode[k] == 0) {                                  // doVJDetection, src/facetrackr.js:137-175
-    e.detection = 1;
-    const int c = counts[k];
-    if (c > 0) {
-      const Rect *d = det + (size_t)k * K;
-      int best = 0;
-      for (int i = 1; i < c; ++i)
-        if (d[i].confidence > d[best].confidence) best = i;   // first maximum, :161-165
-      e.x = d[best].x; e.y = d[best].y; e.width = d[best].width; e.height = d[best].height;
-      e.confidence = d[best].confidence;
-    }
-    if (e.confidence > -10.0) {                        // :97: switch to camshift, initTracker on THIS frame
-      rects[4 * k + 0] = (int32_t)floor(e.x); rects[4 * k + 1] = (int32_t)floor(e.y);
-      rects[4 * k + 2] = (int32_t)floor(e.width); rects[4 * k + 3] = (int32_t)floor(e.height);
-      init_enable[k] = 1;
-      mode[k] = 1;
-      e.status |= 1;
-    }
-  } else {                                             // doCSDetection, src/facetrackr.js:178-209
-    e.detection = 2;
-    const int32_t *o = objs + 6 * (size_t)k;
-    e.x = o[0]; e.y = o[1]; e.width = o[2]; e.height = o[3];
-    e.angle = *reinterpret_cast<const double *>(o + 4);
-    e.confidence = 1.0;
-    if (o[2] == 0 || o[3] == 0) {                      // src/main.js:230: lost -> a fresh facetrackr without whitebalancing
-      mode[k] = 0;
-      e.status |= 2;
-    }
+  const bool vj = mode[k] == 0;
+  bool seed;
+  int32_t rect[4];
+  mode[k] = facetrackr_pass(vj, det + (size_t)k * K, vj ? counts[k] : 0, objs + 6 * (size_t)k, e, rect, seed);
+  if (seed) {
+    for (int i = 0; i < 4; ++i) rects[4 * k + i] = rect[i];
+    init_enable[k] = 1;
   }
   events[k] = e;
   if (head_state) {
@@ -1103,8 +1123,11 @@ __global__ void k_backproj(const uint8_t *__restrict__ rgba, int n_px, const uin
 // ------------------------------------------------------------------------------------------------
 // getWhitebalance — src/whitebalance.js:17-26.  The reference sums bytes in fp64; the sums are
 // exact integers, so integer accumulation in any order is bit-identical.
+// enable (ht_tracker_step): per frame, 0 = no whitebalance wanted (the frame is not read); NULL = every frame
 __global__ void __launch_bounds__(256) k_wb_sums(const uint8_t *__restrict__ rgba, size_t frame_bytes, int n_px,
-                                                 unsigned long long *__restrict__ sums, int chunks) {
+                                                 unsigned long long *__restrict__ sums, int chunks,
+                                                 const uint8_t *__restrict__ enable = nullptr) {
+  if (enable && !enable[blockIdx.y]) return;
   const uint32_t *px = reinterpret_cast<const uint32_t *>(rgba + (size_t)blockIdx.y * frame_bytes);
   const int per = (n_px + chunks - 1) / chunks;
   const int beg = blockIdx.x * per, end = min(n_px, beg + per);
@@ -1125,12 +1148,176 @@ __global__ void __launch_bounds__(256) k_wb_sums(const uint8_t *__restrict__ rgb
   }
 }
 
+__host__ __device__ inline double wb_value(const unsigned long long *s, int n_px) {
+  const double sz = (double)n_px;
+  const double avgr = (double)s[0] / sz, avgg = (double)s[1] / sz, avgb = (double)s[2] / sz;
+  return (avgr + avgg + avgb) / 3;  // src/whitebalance.js:23-26
+}
+
 __global__ void k_wb_final(const unsigned long long *__restrict__ sums, int n, int n_px, double *__restrict__ out) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= n) return;
-  const double sz = (double)n_px;
-  const double avgr = (double)sums[3 * k] / sz, avgg = (double)sums[3 * k + 1] / sz, avgb = (double)sums[3 * k + 2] / sz;
-  out[k] = (avgr + avgg + avgb) / 3;  // src/whitebalance.js:23-26
+  out[k] = wb_value(sums + 3 * (size_t)k, n_px);
+}
+
+// ------------------------------------------------------------------------------------------------
+// headtrackr.Tracker's lifecycle per stream on the device (src/main.js:168-355 with facetrackr.js:67-126): the starter's
+// content check, the whitebalance gate, VJ -> CS, the status events, lost-face handling with and without
+// retryDetection, start() / stop(), and the head-position epilogue - ht_tracker_step.
+enum { TM_IDLE = 0, TM_STARTING = 1, TM_WB = 2, TM_VJ = 3, TM_CS = 4 };
+// headtrackrStatus bits of one frame, in the order src/main.js dispatches them (:182,183,193,233,246,350,251)
+enum { ST_WHITEBALANCE = 1, ST_DETECTING = 2, ST_HINTS = 4, ST_REDETECTING = 8, ST_LOST = 16, ST_STOPPED = 32, ST_FOUND = 64 };
+constexpr int WB_WINDOW = 15;                  // pwbLength, src/facetrackr.js:59
+
+struct TrackerParams {          // ht_tracker_params with the head parameters as make_head_params completes them
+  int32_t retry_detection;      // src/main.js:40
+  int32_t calc_angles;          // src/main.js:54
+  HeadParams head;
+};
+struct TrackerState {
+  int32_t mode;                 // TM_*
+  int32_t n_wb;                 // previousWhitebalances.length
+  int32_t timer_set, pad_;      // detectionTimer !== undefined (src/main.js:188-193)
+  double timer_ms;
+  double wb[WB_WINDOW];         // previousWhitebalances, newest first
+  HeadState head;               // faceFound, firstRun, smoother, head diagonals, fov, headposition
+};
+struct TrackerEvent {           // == ht_tracker_event (include/headtrackr_b200.h)
+  int32_t detection;            // 0 = no pass, 1 = "VJ", 2 = "CS", 3 = "WB"
+  int32_t status;               // ST_* bits
+  double x, y, width, height, angle, confidence;
+  double wb;
+  int32_t running, pad_;
+  double fov;
+  HeadEvent head;
+};
+
+__host__ __device__ inline void tracker_new_state(TrackerState &s) {   // new headtrackr.Tracker + init(): not running
+  s.mode = TM_IDLE; s.n_wb = 0; s.timer_set = 0; s.pad_ = 0; s.timer_ms = 0.0;
+  for (int i = 0; i < WB_WINDOW; ++i) s.wb[i] = 0.0;
+  head_new_state(s.head);
+}
+// start() (src/main.js:328-345): the next frame goes through starter().  On a stream that is already running the
+// reference would run an extra, unscheduled pass; here it does nothing.
+__host__ __device__ inline void tracker_start(TrackerState &s) {
+  if (s.mode == TM_IDLE) s.mode = TM_STARTING;
+}
+// stop() (src/main.js:347-355): clears the track() timer and faceFound.  A pending starter() retry is another timer and
+// survives, as in the reference; the detection timer survives too.
+__host__ __device__ inline void tracker_stop(TrackerState &s) {
+  if (s.mode != TM_STARTING) s.mode = TM_IDLE;
+  s.head.face_found = 0;
+}
+
+// One frame of one stream.  Inputs, as the stream's mode asks for them: wb = getWhitebalance (TM_STARTING, TM_WB),
+// det[0, count) = detect_objects(frame, cascade, 5, 1) (TM_VJ), obj = camshift TrackObj after track() (TM_CS).
+// seed: initTracker(frame, rect) must follow on this frame.
+__host__ __device__ inline void tracker_step(TrackerState &s, const TrackerParams &p, double wb, const Rect *det, int count,
+                                             const int32_t *obj, double now_ms, double camw, double camh, TrackerEvent &out,
+                                             int32_t rect[4], bool &seed) {
+  seed = false;
+  out.detection = 0; out.status = 0; out.pad_ = 0;
+  out.x = out.y = out.width = out.height = out.angle = 0.0;
+  out.confidence = -10000.0;
+  out.wb = 0.0;
+  int mode = s.mode;
+  head_step(s.head, p.head, false, 0.0, 0.0, 0.0, 0.0, false, camw, camh, out.head);   // clears out.head
+  if (mode == TM_STARTING) {                   // starter(), src/main.js:307-326
+    out.wb = wb;
+    if (wb > 0) {                              // run = true; track(): a new facetrackr with whitebalancing (:173-176)
+      s.n_wb = 0;
+      mode = TM_WB;
+    }
+  }
+  if (mode == TM_WB) {                         // checkWhitebalance + the gate, src/facetrackr.js:79-95,220-227
+    out.detection = 3; out.wb = wb;
+    if (s.n_wb >= WB_WINDOW) s.n_wb = WB_WINDOW - 1;                    // pop()
+    for (int i = s.n_wb; i > 0; --i) s.wb[i] = s.wb[i - 1];            // unshift(wb)
+    s.wb[0] = wb;
+    ++s.n_wb;
+    if (s.n_wb == WB_WINDOW) {
+      double mx = s.wb[0], mn = s.wb[0];
+      for (int i = 1; i < WB_WINDOW; ++i) { mx = s.wb[i] > mx ? s.wb[i] : mx; mn = s.wb[i] < mn ? s.wb[i] : mn; }
+      if ((mx - mn) < 2) mode = TM_VJ;
+    }
+    out.status |= ST_WHITEBALANCE;                                     // src/main.js:182
+  } else if (mode == TM_VJ || mode == TM_CS) {
+    const bool vj = mode == TM_VJ;
+    StreamEvent e;
+    const int next = facetrackr_pass(vj, det, count, obj, e, rect, seed);
+    out.detection = e.detection;
+    out.x = e.x; out.y = e.y; out.width = e.width; out.height = e.height; out.angle = e.angle; out.confidence = e.confidence;
+    mode = next == 1 ? TM_CS : TM_VJ;
+    if (vj && s.head.first_run) out.status |= ST_DETECTING;            // :183
+    if (!(e.confidence == 0)) {                                        // :186
+      if (vj) {
+        if (!s.timer_set) { s.timer_set = 1; s.timer_ms = now_ms; }   // :187-194
+        if ((now_ms - s.timer_ms) > 5000) out.status |= ST_HINTS;
+      } else {
+        s.timer_set = 0;                                               // :209
+        const bool lost = (e.status & 2) != 0;
+        const bool retry = p.retry_detection != 0;
+        if (lost) {
+          if (retry) out.status |= ST_REDETECTING;                     // :231-244
+          else { out.status |= ST_LOST | ST_STOPPED; mode = TM_IDLE; } // :245-248, stop()
+        }
+        head_step(s.head, p.head, true, e.x, e.y, e.width, e.height, lost, camw, camh, out.head, retry);
+        if (out.head.status & 1) out.status |= ST_FOUND;               // :250-253
+      }
+    }
+  }
+  s.mode = mode;
+  out.running = (mode != TM_IDLE && mode != TM_STARTING) ? 1 : 0;
+  out.fov = s.head.fov_saved_deg;                                      // getFOV(), :363-365
+}
+
+// modes -> the masks of the frame's kernels (a TM_IDLE stream's frame is never read)
+__global__ void k_tracker_plan(const TrackerState *__restrict__ st, int n, uint8_t *__restrict__ vj_quad_mask,
+                               uint8_t *__restrict__ cs_enable, uint8_t *__restrict__ init_enable,
+                               uint8_t *__restrict__ wb_enable) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  const int m = st[k].mode;
+  cs_enable[k] = m == TM_CS ? 1 : 0;
+  wb_enable[k] = (m == TM_STARTING || m == TM_WB) ? 1 : 0;
+  init_enable[k] = 0;
+  if ((k & 3) == 0) {
+    unsigned mask = 0;
+    for (int f = 0; f < 4 && k + f < n; ++f) mask |= (st[k + f].mode == TM_VJ ? 1u : 0u) << f;
+    vj_quad_mask[k >> 2] = (uint8_t)mask;
+  }
+}
+
+__global__ void k_tracker_update(TrackerState *__restrict__ st, const TrackerParams *__restrict__ params, int n,
+                                 const unsigned long long *__restrict__ wb_sums, int n_px, const Rect *__restrict__ det,
+                                 const int32_t *__restrict__ counts, int K, const int32_t *__restrict__ objs,
+                                 int32_t *__restrict__ rects, uint8_t *__restrict__ init_enable, double now_ms, int camw,
+                                 int camh, TrackerEvent *__restrict__ events) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  TrackerState &s = st[k];                     // updated in place: the window and the head state stay in memory
+  const bool wants_wb = s.mode == TM_STARTING || s.mode == TM_WB;
+  const double wb = wants_wb ? wb_value(wb_sums + 3 * (size_t)k, n_px) : 0.0;
+  TrackerEvent e;
+  int32_t rect[4];
+  bool seed;
+  tracker_step(s, *params, wb, det + (size_t)k * K, s.mode == TM_VJ ? counts[k] : 0, objs + 6 * (size_t)k, now_ms,
+               (double)camw, (double)camh, e, rect, seed);
+  if (seed) {
+    for (int i = 0; i < 4; ++i) rects[4 * k + i] = rect[i];
+    init_enable[k] = 1;
+  }
+  events[k] = e;
+}
+
+// op: 0 = new state, 1 = start(), 2 = stop()
+__global__ void k_tracker_control(TrackerState *st, int first, int n, int op) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  TrackerState &s = st[first + k];
+  if (op == 0) tracker_new_state(s);
+  else if (op == 1) tracker_start(s);
+  else tracker_stop(s);
 }
 
 }  // namespace ht

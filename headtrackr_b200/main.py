@@ -189,7 +189,8 @@ class Tracker:
         return False
 
     def stop(self):                                                 # :347-355
-        self._timer = None
+        if self._timer == "track":                                  # clearTimeout(detector): a pending starter() retry survives
+            self._timer = None
         self._run = False
         self._headtrackerStatus("stopped")
         self._facetracker = None

@@ -9,6 +9,8 @@ for records with detection == "CS" (src/facetrackr.js:112-125).
 """
 import time
 
+from .context import tracker_events_from_bytes
+
 
 class StreamSet:
     def __init__(self, context, n_streams, interval=5, min_neighbors=1, calc_angles=False):
@@ -62,3 +64,105 @@ class StreamSet:
 
     def getTrackingObject(self, stream):
         return dict(self.current[stream]) if self.current[stream] is not None else None
+
+
+def lifecycle_events(rec, status):
+    """One ht_tracker_event record (Context.tracker_step dict) -> (the payload dicts headtrackr.Tracker dispatches on
+    that frame, in its order; ht.status after the frame).  facetrackingEvent first (src/facetrackr.js:112-125), then the
+    headtrackrStatus messages, with status "tracking" set silently on every CS frame before redetecting / lost / found
+    (src/main.js:227), then headtrackingEvent (src/headposition.js:183-188)."""
+    out = []
+    if rec["detection"] == "CS":
+        out.append(dict(type="facetrackingEvent", height=rec["height"], width=rec["width"], angle=rec["angle"], x=rec["x"],
+                        y=rec["y"], confidence=rec["confidence"], detection="CS"))
+        status = "tracking"             # whitebalance / detecting / hints, dispatched before :227, never come with CS
+    for msg in rec["status"]:
+        out.append(dict(type="headtrackrStatus", status=msg))
+        status = msg
+    if rec["head"]["valid"]:
+        h = rec["head"]
+        out.append(dict(type="headtrackingEvent", x=h["x"], y=h["y"], z=h["z"]))
+    return out, status
+
+
+class TrackerSet:
+    """headtrackr.Tracker (src/main.js) for n streams on the GPU (ht_tracker_step): stream k is one Tracker whose
+    `setTimeout` fires once per step() call.  start(k) / stop(k) are the Tracker's start() / stop() (stop() emits
+    "stopped" at once, src/main.js:350); step(frames) runs one timer tick of every stream - starter, whitebalance gate,
+    detection, tracking, status events and head position all on the device - and dispatches the reference's payload
+    dicts in the reference's order to the listeners as fn(stream, evt).  `status[k]` is ht.status, getFOV(k) its fov.
+    Differs from the reference in one place: start() on a running stream does nothing (the reference runs an extra,
+    unscheduled pass)."""
+
+    def __init__(self, context, n_streams, params=None, device_events=False):
+        if n_streams > context.max_frames:
+            raise ValueError("more streams than tracker slots in the context")
+        p = dict(params or {})
+        self.ctx, self.n = context, n_streams
+        self._device_events = device_events          # records written to a torch CUDA buffer, then copied back
+        self._listeners = []
+        self.status = [""] * n_streams
+        self._fov = [0] * n_streams
+        self.current = [None] * n_streams
+        context.tracker_config(retryDetection=p.get("retryDetection", True), calcAngles=p.get("calcAngles", False),
+                               smoothing=p.get("smoothing", True), fov=p.get("fov"),
+                               cameraOffset=p.get("cameraOffset", 11.5), headPosition=p.get("headPosition", True))
+        context.tracker_reset(0, n_streams)
+
+    def addEventListener(self, fn):
+        """fn(stream_index, evt): evt is a headtrackrStatus / facetrackingEvent / headtrackingEvent payload dict."""
+        self._listeners.append(fn)
+
+    def _emit(self, k, evt):
+        for fn in self._listeners:
+            fn(k, evt)
+
+    def _range(self, k):
+        return (0, self.n) if k is None else (k, 1)
+
+    def start(self, k=None):
+        """start() of stream k (all streams if None): the next step() runs its starter."""
+        self.ctx.tracker_start(*self._range(k))
+        return True
+
+    def stop(self, k=None):
+        """stop() of stream k (all streams if None): "stopped" is dispatched now."""
+        first, n = self._range(k)
+        self.ctx.tracker_stop(first, n)
+        for s in range(first, first + n):
+            self.status[s] = "stopped"
+            self._emit(s, dict(type="headtrackrStatus", status="stopped"))
+        return True
+
+    def reset(self, k=None):
+        """A new headtrackr.Tracker for stream k (all streams if None), initialised and not running."""
+        first, n = self._range(k)
+        self.ctx.tracker_reset(first, n)
+        for s in range(first, first + n):
+            self.status[s], self._fov[s], self.current[s] = "", 0, None
+
+    def step(self, frames, now_ms=None):
+        """frames: (n, H, W, 4) u8 (numpy or torch CUDA) - the current frame of every stream."""
+        now = time.time() * 1000.0 if now_ms is None else now_ms
+        t0 = time.time()
+        if self._device_events:
+            import torch
+            buf = torch.empty(self.n * 144, dtype=torch.uint8, device="cuda")
+            self.ctx.tracker_step(frames, now, out=buf)
+            self.ctx.sync()                            # the records are written on the library's stream
+            recs = tracker_events_from_bytes(buf.cpu().numpy().tobytes())
+        else:
+            recs = self.ctx.tracker_step(frames, now)
+        dt = int((time.time() - t0) * 1000)
+        for k, rec in enumerate(recs):
+            self.current[k] = rec
+            self._fov[k] = rec["fov"]
+            evts, self.status[k] = lifecycle_events(rec, self.status[k])
+            for e in evts:
+                if e["type"] == "facetrackingEvent":
+                    e["time"] = dt
+                self._emit(k, e)
+        return recs
+
+    def getFOV(self, k):
+        return self._fov[k]

@@ -183,6 +183,54 @@ int ht_stream_reset(ht_ctx *ctx, int first, int n);
 int ht_stream_step(ht_ctx *ctx, const uint8_t *rgba, int n, int w, int h, int interval, int min_neighbors,
                    int calc_angles, ht_stream_event *out_events);
 
+/* headtrackr.Tracker per stream on the device from its first frame (SURVEY.md 8f-5, ABI 1.1): what src/main.js does
+ * between start() and stop() - the starter's content check (src/main.js:307-326: a frame whose getWhitebalance is 0
+ * is retried on the next frame), facetrackr with whitebalancing (src/facetrackr.js:42-52,79-95: 15 whitebalance
+ * samples within 2 gray levels before detection starts), VJ -> CS, the headtrackrStatus events, the lost face with or
+ * without retryDetection, and the head-position epilogue of ht_stream_step_head.  Stream k uses tracker slot k.
+ * Per stream the mode is one of IDLE (not running: its frame is never read), STARTING, WB, VJ, CS; one
+ * ht_tracker_step call is one timer tick of every stream.  Detection runs with interval 5 and min_neighbors 1
+ * (src/facetrackr.js:147-149).
+ * While the lifecycle is configured ht_stream_step / ht_stream_step_head return HT_ERR_STATE (the two share the
+ * tracker slots).  One deliberate difference: start() on a running stream does nothing, where the reference would
+ * run an extra, unscheduled pass. */
+typedef struct {
+  int32_t retry_detection;   /* params.retryDetection (src/main.js:40, default 1) */
+  int32_t calc_angles;       /* params.calcAngles     (src/main.js:54, default 0) */
+  int32_t pad_[2];
+  ht_head_params head;       /* smoothing, headPosition, fov, cameraOffset: as for ht_stream_head_config */
+} ht_tracker_params;
+/* headtrackrStatus events of one frame: bit order == dispatch order (src/main.js:182,183,193,233,246,350,251) */
+#define HT_STATUS_WHITEBALANCE 1
+#define HT_STATUS_DETECTING 2
+#define HT_STATUS_HINTS 4
+#define HT_STATUS_REDETECTING 8
+#define HT_STATUS_LOST 16
+#define HT_STATUS_STOPPED 32     /* the stop() of a lost face without retryDetection; ht_tracker_stop emits none */
+#define HT_STATUS_FOUND 64
+/* One record per stream and frame.  Dispatch order of the reference: `facetrackingEvent` (detection == 2) first, then
+ * the status bits from low to high, then `headtrackingEvent` (head.valid).  status "tracking" is set without an
+ * event on every "CS" frame before its redetecting / lost / found (src/main.js:227). */
+typedef struct {
+  int32_t detection;         /* 0 = no pass ran (idle, or the starter saw no content), 1 = "VJ", 2 = "CS", 3 = "WB" */
+  int32_t status;            /* HT_STATUS_* */
+  double x, y, width, height, angle, confidence;   /* facetrackr TrackObj (VJ: top-left; CS: centre) */
+  double wb;                 /* getWhitebalance of the frame when the starter or a "WB" pass ran, else 0 */
+  int32_t running;           /* 1: a track() pass is scheduled for the next frame */
+  int32_t pad_;
+  double fov;                /* getFOV() after this frame (src/main.js:363-365) */
+  ht_head_event head;        /* smoothed face and headtrackingEvent {x, y, z} */
+} ht_tracker_event;
+/* params == NULL switches the lifecycle off and puts every stream back into ht_stream_reset's state.  Switching it on
+ * starts every stream as ht_tracker_reset; changing parameters while on keeps the stream states. */
+int ht_tracker_config(ht_ctx *ctx, const ht_tracker_params *params);
+int ht_tracker_reset(ht_ctx *ctx, int first, int n);   /* new headtrackr.Tracker + init(): not running */
+int ht_tracker_start(ht_ctx *ctx, int first, int n);   /* start(): the next frame of the stream goes through starter() */
+int ht_tracker_stop(ht_ctx *ctx, int first, int n);    /* stop() (src/main.js:347-355); the caller emits "stopped" */
+/* one frame per stream for streams [0, n): rgba = n frames, stream-major; now_ms = (new Date).getTime() of this tick
+ * (the "hints" timer, src/main.js:187-194); out[n] host or device (device: enqueue only) */
+int ht_tracker_step(ht_ctx *ctx, const uint8_t *rgba, int n, int w, int h, double now_ms, ht_tracker_event *out);
+
 /* Frame ingest (SURVEY.md 8f-4): canvasContext.drawImage(videoElement, 0, 0, canvas.width, canvas.height)
  * (src/main.js:170) for n frames - the video frame (sw x sh) scaled onto the working canvas (dw x dh), all four
  * channels, with the canvas resampler this build defines (DESIGN.md 2).  src and dst may be host or device
