@@ -8,7 +8,8 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from ._lib import HeadEvent, HeadParams, HtError, Rect, StreamEvent, TrackerEvent, TrackerParams, TrackObj, Window
+from ._lib import (HeadEvent, HeadParams, HtError, Rect, StreamEvent, TrackerEvent, TrackerParams, TrackObj, VideoFrame,
+                   Window)
 from .synth import load_cascade_blob
 
 
@@ -252,6 +253,48 @@ class Context:
             return None
         ev = (TrackerEvent * n)()
         self._check(self._L.ht_tracker_step(self._h, ptr, n, W, H, float(now_ms), C.addressof(ev)))
+        return [tracker_event_dict(e) for e in ev]
+
+    def tracker_feed(self, streams, frames, now_ms, width, height, out=None):
+        """One timer tick of each listed stream on its own video frame and clock (ht_tracker_feed): drawImage(video, 0,
+        0, width, height) onto the working canvas, then what tracker_step does for that stream.  Unlisted streams do
+        not tick.  streams: distinct stream ids; frames: one (h, w, 4) u8 video frame per stream, all numpy arrays or
+        all torch CUDA tensors (any size; a row-padded view - last two strides (4, 1) - passes its row stride as the
+        pitch); now_ms: one clock for all or one per record.  -> event dicts in record order; with a torch CUDA `out`
+        tensor of len(streams)*144 bytes: asynchronous, nothing returned."""
+        streams = list(streams)
+        n = len(frames)
+        if len(streams) != n or n == 0:
+            raise ValueError("one frame per listed stream")
+        clocks = [float(t) for t in now_ms] if hasattr(now_ms, "__len__") else [float(now_ms)] * n
+        if len(clocks) != n:
+            raise ValueError("one clock per listed stream")
+        on_device = _is_torch(frames[0])
+        recs = (VideoFrame * n)()
+        keep = []
+        for b, (k, f) in enumerate(zip(streams, frames)):
+            if _is_torch(f) != on_device:
+                raise ValueError("frames must be all numpy arrays or all torch CUDA tensors")
+            if on_device:
+                if f.dim() != 3 or f.element_size() != 1 or f.shape[2] != 4 or f.stride(2) != 1 or f.stride(1) != 4:
+                    raise ValueError("frame tensors must be uint8 (h, w, 4) with strides (pitch, 4, 1)")
+                ptr, pitch = f.data_ptr(), f.stride(0)
+            else:
+                a = np.asarray(f)
+                if a.dtype != np.uint8 or a.ndim != 3 or a.shape[2] != 4:
+                    raise ValueError("frames must be (h, w, 4) uint8")
+                if a.strides[2] != 1 or a.strides[1] != 4 or a.strides[0] < 4 * a.shape[1]:
+                    a = np.ascontiguousarray(a)
+                ptr, pitch = a.ctypes.data, a.strides[0]
+                f = a
+            keep.append(f)
+            recs[b] = VideoFrame(ptr, int(k), f.shape[1], f.shape[0], pitch, clocks[b])
+        if out is not None:
+            self._check(self._L.ht_tracker_feed(self._h, C.addressof(recs), n, int(on_device), width, height,
+                                                out.data_ptr()))
+            return None
+        ev = (TrackerEvent * n)()
+        self._check(self._L.ht_tracker_feed(self._h, C.addressof(recs), n, int(on_device), width, height, C.addressof(ev)))
         return [tracker_event_dict(e) for e in ev]
 
     def ingest(self, frames, width, height, out=None):

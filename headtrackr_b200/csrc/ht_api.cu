@@ -8,6 +8,7 @@
 #include <algorithm>
 #include <cmath>
 #include <cstdarg>
+#include <cstddef>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -554,6 +555,11 @@ struct ht_ctx {
   DevBuf d_tracker_state, d_tracker_params, d_tracker_events, d_tracker_wb;          // ht_tracker_config
   bool tracker_on = false;
   int tracker_calc_angles = 0;
+  // ht_tracker_feed: the record table {ids[n], clocks[n], FeedRec[n]} goes up in one copy from pinned memory; the
+  // videos are drawn into the canvas arena ([max_frames] canvases, indexed by record), zeroed when allocated
+  DevBuf d_feed_table, d_feed_draw, d_feed_canvas;
+  void *h_feed_table = nullptr;
+  cudaEvent_t feed_copied = nullptr;        // the last table upload has left h_feed_table
   bool track_history = true;                // order by the cost of each stream's previous launch (HT_TRACK_HISTORY=0: by window area)
   DevBuf d_track_cost;                      // [max_frames][2] {passes, window pixels / 256} per slot
   int track_heavy_div = 128;                // >0: the n/div costliest streams run on a cluster of
@@ -1159,7 +1165,7 @@ int upload_chunks(ht_ctx *ctx, const uint8_t *rgba, int n, size_t frame_bytes, i
 // ================================================================================================
 extern "C" {
 
-uint32_t ht_version(void) { return (1u << 16) | 1u; }
+uint32_t ht_version(void) { return (1u << 16) | 2u; }
 
 const char *ht_last_error(const ht_ctx *ctx) { return ctx ? ctx->err.c_str() : g_create_error.c_str(); }
 
@@ -1276,8 +1282,11 @@ void ht_destroy(ht_ctx *ctx) {
   DevBuf *bufs[] = {&ctx->d_casc, &ctx->arena, &ctx->d_frames, &ctx->raw_keys, &ctx->raw_conf, &ctx->raw_count, &ctx->sorted,
                     &ctx->labels, &ctx->seq2, &ctx->d_out_rects, &ctx->d_out_counts, &ctx->d_flags, &ctx->model_hist,
                     &ctx->bins, &ctx->d_sched, &ctx->d_trace, &ctx->d_tmaps, &ctx->d_late_chunk0, &ctx->d_track_cost, &ctx->d_stream_mode, &ctx->d_stream_mask, &ctx->d_stream_cs, &ctx->d_stream_init, &ctx->d_stream_events, &ctx->d_head_state, &ctx->d_head_params, &ctx->d_head_events, &ctx->d_tracker_state, &ctx->d_tracker_params, &ctx->d_tracker_events, &ctx->d_tracker_wb, &ctx->cur_hist, &ctx->track_state, &ctx->d_slots, &ctx->d_rects, &ctx->d_found, &ctx->d_objs,
-                    &ctx->d_windows, &ctx->d_wb_sums, &ctx->d_wb_out, &ctx->d_scratch};
+                    &ctx->d_windows, &ctx->d_wb_sums, &ctx->d_wb_out, &ctx->d_scratch, &ctx->d_feed_table, &ctx->d_feed_draw,
+                    &ctx->d_feed_canvas};
   for (DevBuf *b : bufs) b->release();
+  if (ctx->h_feed_table) cudaFreeHost(ctx->h_feed_table);
+  if (ctx->feed_copied) cudaEventDestroy(ctx->feed_copied);
   for (auto &sp : ctx->prof_spans) { cudaEventDestroy(sp.a); cudaEventDestroy(sp.b); }
   for (cudaEvent_t e : ctx->prof_free) cudaEventDestroy(e);
   for (cudaEvent_t e : ctx->chunk_events) cudaEventDestroy(e);
@@ -1800,29 +1809,28 @@ int ht_tracker_reset(ht_ctx *ctx, int first, int n) { return tracker_control(ctx
 int ht_tracker_start(ht_ctx *ctx, int first, int n) { return tracker_control(ctx, first, n, 1); }
 int ht_tracker_stop(ht_ctx *ctx, int first, int n) { return tracker_control(ctx, first, n, 2); }
 
-// One timer tick of n headtrackr.Tracker streams, entirely on the device:
-//   k_tracker_plan   modes -> VJ frame-quad mask, CS enable, whitebalance enable
+// The video draw of ht_tracker_feed: record table, per-record draw flags (written by k_tracker_plan), canvas constants.
+struct FeedDraw {
+  const FeedRec *recs;
+  uint8_t *draw;
+  IngestGeom g;
+};
+
+// One timer tick of n headtrackr.Tracker streams, entirely on the device (shared by ht_tracker_step and
+// ht_tracker_feed).  d_rgba: n canvases of w x h; batch entry k is stream d_ids[k] (NULL: stream k) and ticks at
+// d_now[k] (NULL: every entry at now_ms).
+//   k_tracker_plan   modes -> VJ frame-quad mask, CS enable, whitebalance enable (feed: draw flags)
+//   k_feed_draw      (feed) drawImage(video, 0, 0, w, h) of every stream that is not IDLE   src/main.js:170,312
 //   k_wb_sums        whitebalance sums of the STARTING and WB streams only       src/whitebalance.js, src/main.js:316
 //   run_detect       the VJ streams (interval 5, min_neighbors 1)                 src/facetrackr.js:147-149
 //   k_hist, k_track  one track() of the CS streams                                src/camshift.js:213-312
 //   k_tracker_update starter, whitebalance gate, facetrackr and main.js transitions, status bits, head epilogue
 //   k_track_init     initTracker for the streams that found their face           src/facetrackr.js:97-108
-int ht_tracker_step(ht_ctx *ctx, const uint8_t *rgba, int n, int w, int h, double now_ms, ht_tracker_event *out) {
-  if (!ctx) return HT_ERR_ARG;
-  if (!ctx->tracker_on) return ctx->fail(HT_ERR_STATE, "ht_tracker_config has not been called");
-  if (!out) return ctx->fail(HT_ERR_ARG, "out is NULL");
-  int rc = check_batch(ctx, n);
-  if (rc != HT_OK) return rc;
-  CK(cudaSetDevice(ctx->cfg.device));
-  Plan *P = nullptr;
-  rc = get_plan(ctx, w, h, 5, &P);
-  if (rc != HT_OK) return rc;
-  rc = ensure_tracker_buffers(ctx);
+static int tracker_tick(ht_ctx *ctx, Plan *P, const uint8_t *d_rgba, int n, int w, int h, const int32_t *d_ids,
+                        double now_ms, const double *d_now, const FeedDraw *feed, ht_tracker_event *out) {
+  int rc = ensure_tracker_buffers(ctx);
   if (rc != HT_OK) return rc;
   rc = ensure_stream_buffers(ctx);           // the mask scratch of ht_stream_step (the two never run on one context at once)
-  if (rc != HT_OK) return rc;
-  const uint8_t *d_rgba = nullptr;
-  rc = device_frames(ctx, rgba, n, w, h, &d_rgba);
   if (rc != HT_OK) return rc;
   CK(ctx->bins.reserve((size_t)n * w * h * sizeof(uint16_t)));
   CK(ctx->d_wb_sums.reserve((size_t)ctx->cfg.max_frames * 3 * sizeof(unsigned long long)));
@@ -1830,7 +1838,13 @@ int ht_tracker_step(ht_ctx *ctx, const uint8_t *rgba, int n, int w, int h, doubl
   TrackerState *ts = ctx->d_tracker_state.as<TrackerState>();
   uint8_t *vj_mask = ctx->d_stream_mask.as<uint8_t>(), *cs_en = ctx->d_stream_cs.as<uint8_t>(), *init_en = ctx->d_stream_init.as<uint8_t>();
   uint8_t *wb_en = ctx->d_tracker_wb.as<uint8_t>();
-  k_tracker_plan<<<(n + 127) / 128, 128, 0, st>>>(ts, n, vj_mask, cs_en, init_en, wb_en);
+  k_tracker_plan<<<(n + 127) / 128, 128, 0, st>>>(ts, d_ids, n, vj_mask, cs_en, init_en, wb_en, feed ? feed->draw : nullptr);
+  if (feed) {
+    const int tiles_x = (w + 63) / 64, tiles = tiles_x * ((h + 15) / 16);
+    k_feed_draw<<<dim3((unsigned)tiles, (unsigned)n), 256, 0, st>>>(feed->recs, feed->draw, const_cast<uint8_t *>(d_rgba),
+                                                                    feed->g, tiles_x);
+    ++ctx->launches;
+  }
   CK(cudaMemsetAsync(ctx->d_wb_sums.p, 0, (size_t)n * 3 * sizeof(unsigned long long), st));
   const int chunks = std::min(64, std::max(1, 8 * ctx->sms / n));
   k_wb_sums<<<dim3(chunks, n), 256, 0, st>>>(d_rgba, (size_t)w * h * 4, w * h, ctx->d_wb_sums.as<unsigned long long>(), chunks, wb_en);
@@ -1841,19 +1855,19 @@ int ht_tracker_step(ht_ctx *ctx, const uint8_t *rgba, int n, int w, int h, doubl
   rc = launch_hist(ctx, d_rgba, n, w, h, ctx->cur_hist.as<uint32_t>(), ctx->bins.as<uint16_t>(), cs_en);
   if (rc != HT_OK) return rc;
   ctx->prof_begin(HT_PROF_TRACK);
-  rc = launch_track(ctx, n, 0, ctx->bins.as<uint16_t>(), w, h, nullptr, ctx->model_hist.as<uint32_t>(),
+  rc = launch_track(ctx, n, 0, ctx->bins.as<uint16_t>(), w, h, d_ids, ctx->model_hist.as<uint32_t>(),
                     ctx->cur_hist.as<uint32_t>(), ctx->track_state.as<TrackState>(), 1, ctx->d_objs.as<int32_t>(), nullptr,
                     ctx->d_flags.as<int32_t>() + 2, cs_en);
   if (rc != HT_OK) return rc;
   ctx->prof_end();
   const bool out_dev = is_device_ptr(out);
   TrackerEvent *d_ev = out_dev ? reinterpret_cast<TrackerEvent *>(out) : ctx->d_tracker_events.as<TrackerEvent>();
-  k_tracker_update<<<(n + 127) / 128, 128, 0, st>>>(ts, ctx->d_tracker_params.as<TrackerParams>(), n,
+  k_tracker_update<<<(n + 127) / 128, 128, 0, st>>>(ts, d_ids, ctx->d_tracker_params.as<TrackerParams>(), n,
                                                     ctx->d_wb_sums.as<unsigned long long>(), w * h, ctx->d_out_rects.as<Rect>(),
                                                     ctx->d_out_counts.as<int32_t>(), ctx->K, ctx->d_objs.as<int32_t>(),
-                                                    ctx->d_rects.as<int32_t>(), init_en, now_ms, w, h, d_ev);
+                                                    ctx->d_rects.as<int32_t>(), init_en, now_ms, d_now, w, h, d_ev);
   ctx->prof_begin(HT_PROF_TRACK_INIT);
-  k_track_init<<<n, 256, 0, st>>>(d_rgba, (size_t)w * h * 4, w, h, nullptr, ctx->d_rects.as<int32_t>(), ctx->tracker_calc_angles,
+  k_track_init<<<n, 256, 0, st>>>(d_rgba, (size_t)w * h * 4, w, h, d_ids, ctx->d_rects.as<int32_t>(), ctx->tracker_calc_angles,
                                   ctx->model_hist.as<uint32_t>(), ctx->track_state.as<TrackState>(), nullptr, init_en);
   ctx->prof_end();
   ctx->launches += 2;
@@ -1865,6 +1879,108 @@ int ht_tracker_step(ht_ctx *ctx, const uint8_t *rgba, int n, int w, int h, doubl
     return ht_sync(ctx);
   }
   return HT_OK;
+}
+
+int ht_tracker_step(ht_ctx *ctx, const uint8_t *rgba, int n, int w, int h, double now_ms, ht_tracker_event *out) {
+  if (!ctx) return HT_ERR_ARG;
+  if (!ctx->tracker_on) return ctx->fail(HT_ERR_STATE, "ht_tracker_config has not been called");
+  if (!out) return ctx->fail(HT_ERR_ARG, "out is NULL");
+  int rc = check_batch(ctx, n);
+  if (rc != HT_OK) return rc;
+  CK(cudaSetDevice(ctx->cfg.device));
+  Plan *P = nullptr;
+  rc = get_plan(ctx, w, h, 5, &P);
+  if (rc != HT_OK) return rc;
+  const uint8_t *d_rgba = nullptr;
+  rc = device_frames(ctx, rgba, n, w, h, &d_rgba);
+  if (rc != HT_OK) return rc;
+  return tracker_tick(ctx, P, d_rgba, n, w, h, nullptr, now_ms, nullptr, nullptr, out);
+}
+
+static_assert(sizeof(ht_video_frame) == 32 && sizeof(FeedRec) == sizeof(ht_video_frame), "ht_video_frame layout");
+static_assert(offsetof(ht_video_frame, now_ms) == offsetof(FeedRec, now_ms) && offsetof(ht_video_frame, pitch) == offsetof(FeedRec, pitch),
+              "ht_video_frame layout");
+
+// One timer tick of each listed stream on its own video and clock.  Everything is checked before anything is enqueued;
+// then ONE host-to-device copy carries the record table {stream ids, clocks, FeedRec with device pointers and resolved
+// pitches} from pinned memory, and tracker_tick draws the videos of the streams that are not IDLE into the canvas arena
+// (batch entry b = record b) before the kernels of ht_tracker_step run on it through the stream ids.
+int ht_tracker_feed(ht_ctx *ctx, const ht_video_frame *frames, int n, int frames_on_device, int canvas_w, int canvas_h,
+                    ht_tracker_event *out) {
+  if (!ctx) return HT_ERR_ARG;
+  if (!ctx->tracker_on) return ctx->fail(HT_ERR_STATE, "ht_tracker_config has not been called");
+  if (!frames || !out) return ctx->fail(HT_ERR_ARG, "frames or out is NULL");
+  const int mf = ctx->cfg.max_frames;
+  if (n <= 0 || n > mf) return ctx->fail(HT_ERR_ARG, "n=%d outside [1,%d]", n, mf);
+  std::vector<uint8_t> seen((size_t)mf, 0);
+  for (int b = 0; b < n; ++b) {
+    const ht_video_frame &f = frames[b];
+    if (f.stream < 0 || f.stream >= mf) return ctx->fail(HT_ERR_ARG, "record %d: stream %d outside [0,%d)", b, f.stream, mf);
+    if (seen[(size_t)f.stream]++) return ctx->fail(HT_ERR_ARG, "record %d: stream %d is listed twice", b, f.stream);
+    if (!f.rgba) return ctx->fail(HT_ERR_ARG, "record %d: rgba is NULL", b);
+    if (reinterpret_cast<uintptr_t>(f.rgba) & 3u) return ctx->fail(HT_ERR_ARG, "record %d: rgba must be 4-byte aligned", b);
+    if (f.width <= 0 || f.height <= 0 || f.width > 16384 || f.height > 16384)
+      return ctx->fail(HT_ERR_SIZE, "record %d: video %dx%d outside 1..16384", b, f.width, f.height);
+    if ((f.pitch & 3) || (f.pitch != 0 && f.pitch < 4 * f.width))
+      return ctx->fail(HT_ERR_ARG, "record %d: pitch %d is not a multiple of 4 >= 4*width", b, f.pitch);
+  }
+  if (canvas_w <= 0 || canvas_h <= 0) return ctx->fail(HT_ERR_SIZE, "0-sized canvas (a browser draws nothing; the detector then throws)");
+  IngestGeom g{0, 0, canvas_w, canvas_h, 0, 0, 0};
+  if (!bilinear_division_constants(4ull * canvas_w * canvas_h, g.magic, g.shift))
+    return ctx->fail(HT_ERR_SIZE, "canvas too large for 32-bit bilinear numerators");
+  g.half = (uint32_t)(2ull * canvas_w * canvas_h);
+  if (is_device_ptr(frames[0].rgba) != (frames_on_device != 0))
+    return ctx->fail(HT_ERR_ARG, "the frames are %s memory, frames_on_device says otherwise", frames_on_device ? "host" : "device");
+  { const int jr = join_aux(ctx); if (jr != HT_OK) return jr; }
+  CK(cudaSetDevice(ctx->cfg.device));
+  Plan *P = nullptr;
+  int rc = get_plan(ctx, canvas_w, canvas_h, 5, &P);     // HT_ERR_SIZE: above the maximum, or too small for the pyramid
+  if (rc != HT_OK) return rc;
+  const size_t canvas_bytes = (size_t)canvas_w * canvas_h * 4;
+  if (ctx->d_feed_canvas.cap < (size_t)mf * canvas_bytes) {   // the masked detection reads whole frame quads: never garbage
+    CK(ctx->d_feed_canvas.reserve((size_t)mf * canvas_bytes));
+    CK(cudaMemsetAsync(ctx->d_feed_canvas.p, 0, ctx->d_feed_canvas.cap, ctx->stream));
+  }
+  // record table: ids [n] i32 | clocks [n] f64 | FeedRec [n], one copy
+  const size_t off_now = align_up<size_t>(4 * (size_t)mf, 16), off_rec = off_now + 8 * (size_t)mf;
+  const size_t table_cap = off_rec + sizeof(FeedRec) * (size_t)mf;
+  if (!ctx->h_feed_table) {
+    CK(cudaMallocHost(&ctx->h_feed_table, table_cap));
+    CK(cudaEventCreateWithFlags(&ctx->feed_copied, cudaEventDisableTiming));
+    CK(ctx->d_feed_table.reserve(table_cap));
+    CK(ctx->d_feed_draw.reserve((size_t)mf));
+  } else {
+    CK(cudaEventSynchronize(ctx->feed_copied));           // the previous call's upload may still read the table
+  }
+  uint8_t *tab = static_cast<uint8_t *>(ctx->h_feed_table);
+  int32_t *ids = reinterpret_cast<int32_t *>(tab);
+  double *now = reinterpret_cast<double *>(tab + off_now);
+  FeedRec *recs = reinterpret_cast<FeedRec *>(tab + off_rec);
+  size_t video_bytes = 0;
+  for (int b = 0; b < n; ++b) video_bytes += align_up<size_t>((size_t)frames[b].width * frames[b].height * 4, 256);
+  if (!frames_on_device) CK(ctx->d_frames.reserve(video_bytes));
+  size_t voff = 0;
+  for (int b = 0; b < n; ++b) {
+    const ht_video_frame &f = frames[b];
+    ids[b] = f.stream;
+    now[b] = f.now_ms;
+    FeedRec r{f.rgba, f.stream, f.width, f.height, f.pitch ? f.pitch : 4 * f.width, f.now_ms};
+    if (!frames_on_device) {                               // pack the host videos into the device staging buffer
+      uint8_t *dst = ctx->d_frames.as<uint8_t>() + voff;
+      CK(cudaMemcpy2DAsync(dst, 4 * (size_t)f.width, f.rgba, (size_t)r.pitch, 4 * (size_t)f.width, (size_t)f.height,
+                           cudaMemcpyHostToDevice, ctx->stream));
+      r.src = dst;
+      r.pitch = 4 * f.width;
+      voff += align_up<size_t>((size_t)f.width * f.height * 4, 256);
+    }
+    recs[b] = r;
+  }
+  uint8_t *dtab = ctx->d_feed_table.as<uint8_t>();
+  CK(cudaMemcpyAsync(dtab, tab, off_rec + sizeof(FeedRec) * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaEventRecord(ctx->feed_copied, ctx->stream));
+  const FeedDraw feed{reinterpret_cast<const FeedRec *>(dtab + off_rec), ctx->d_feed_draw.as<uint8_t>(), g};
+  return tracker_tick(ctx, P, ctx->d_feed_canvas.as<uint8_t>(), n, canvas_w, canvas_h, reinterpret_cast<const int32_t *>(dtab),
+                      0.0, reinterpret_cast<const double *>(dtab + off_now), &feed, out);
 }
 
 // canvasContext.drawImage(video, 0, 0, canvas.width, canvas.height) for n frames (src/main.js:170)
@@ -2187,6 +2303,22 @@ extern "C" int ht_selftest_ingest(const uint8_t *src, int n, int sw, int sh, uin
   for (int f = 0; f < n; ++f)
     for (int Y = 0; Y < dh; ++Y)
       for (int X = 0; X < dw; ++X) ingest_pixel(src, dst, g, X, Y, f);
+  return 0;
+}
+
+// k_feed_draw's per-record code over a heterogeneous record batch: canvas b = record b (dw x dh); draw[b] == 0 leaves
+// canvas b untouched.  Host pointers in the records.
+extern "C" int ht_selftest_feed_draw(const ht_video_frame *frames, int n, const uint8_t *draw, uint8_t *canvas, int dw, int dh) {
+  IngestGeom g{0, 0, dw, dh, 0, 0, 0};
+  if (!bilinear_division_constants(4ull * dw * dh, g.magic, g.shift)) return -1;
+  g.half = (uint32_t)(2ull * dw * dh);
+  for (int b = 0; b < n; ++b) {
+    if (!draw[b]) continue;
+    const ht_video_frame &f = frames[b];
+    const FeedRec r{f.rgba, f.stream, f.width, f.height, f.pitch ? f.pitch : 4 * f.width, f.now_ms};
+    for (int Y = 0; Y < dh; ++Y)
+      for (int X = 0; X < dw; ++X) feed_draw_pixel(r, canvas, g, X, Y, b);
+  }
   return 0;
 }
 

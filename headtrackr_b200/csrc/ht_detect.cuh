@@ -184,21 +184,20 @@ struct IngestGeom {
   int sw, sh, dw, dh;
   uint32_t magic, shift, half;   // floor(n / (4 dw dh)) == (uint64(n) * magic) >> shift for n <= 255.5 * 4 dw dh
 };
-// one destination pixel (also run on the host by tests/test_ingest_host.py)
-__host__ __device__ __forceinline__ void ingest_pixel(const uint8_t *__restrict__ src, uint8_t *__restrict__ dst, const IngestGeom &g,
-                                                      int X, int Y, int frame) {
-  const uint32_t *s = reinterpret_cast<const uint32_t *>(src) + (size_t)frame * g.sw * g.sh;
+// canvas pixel (X, Y) of the sw x sh source s (rows of `spitch` pixels) drawn onto the canvas of g (g.sw / g.sh unused)
+__host__ __device__ __forceinline__ uint32_t draw_pixel(const uint32_t *__restrict__ s, int sw, int sh, size_t spitch,
+                                                        const IngestGeom &g, int X, int Y) {
   // u = (X + 1/2) sw / dw - 1/2 = ((2X + 1) sw - dw) / (2 dw): floor and numerator of the fraction, exactly
-  const int un = (2 * X + 1) * g.sw - g.dw, vn = (2 * Y + 1) * g.sh - g.dh;
+  const int un = (2 * X + 1) * sw - g.dw, vn = (2 * Y + 1) * sh - g.dh;
   const int Dx = 2 * g.dw, Dy = 2 * g.dh;
   int x0 = un / Dx, y0 = vn / Dy;
   if (un < 0 && x0 * Dx != un) --x0;       // floor for negative numerators (the first column / row when upscaling)
   if (vn < 0 && y0 * Dy != vn) --y0;
   const uint32_t fx = (uint32_t)(un - x0 * Dx), fy = (uint32_t)(vn - y0 * Dy);
-  const int xa = x0 < 0 ? 0 : (x0 > g.sw - 1 ? g.sw - 1 : x0), xb = x0 + 1 < 0 ? 0 : (x0 + 1 > g.sw - 1 ? g.sw - 1 : x0 + 1);
-  const int ya = y0 < 0 ? 0 : (y0 > g.sh - 1 ? g.sh - 1 : y0), yb = y0 + 1 < 0 ? 0 : (y0 + 1 > g.sh - 1 ? g.sh - 1 : y0 + 1);
-  const uint32_t p00 = ld_ro(s + (size_t)ya * g.sw + xa), p01 = ld_ro(s + (size_t)ya * g.sw + xb);
-  const uint32_t p10 = ld_ro(s + (size_t)yb * g.sw + xa), p11 = ld_ro(s + (size_t)yb * g.sw + xb);
+  const int xa = x0 < 0 ? 0 : (x0 > sw - 1 ? sw - 1 : x0), xb = x0 + 1 < 0 ? 0 : (x0 + 1 > sw - 1 ? sw - 1 : x0 + 1);
+  const int ya = y0 < 0 ? 0 : (y0 > sh - 1 ? sh - 1 : y0), yb = y0 + 1 < 0 ? 0 : (y0 + 1 > sh - 1 ? sh - 1 : y0 + 1);
+  const uint32_t p00 = ld_ro(s + (size_t)ya * spitch + xa), p01 = ld_ro(s + (size_t)ya * spitch + xb);
+  const uint32_t p10 = ld_ro(s + (size_t)yb * spitch + xa), p11 = ld_ro(s + (size_t)yb * spitch + xb);
   const uint32_t w00 = ((uint32_t)Dx - fx) * ((uint32_t)Dy - fy), w01 = fx * ((uint32_t)Dy - fy);
   const uint32_t w10 = ((uint32_t)Dx - fx) * fy, w11 = fx * fy;
   uint32_t out = 0;
@@ -208,12 +207,60 @@ __host__ __device__ __forceinline__ void ingest_pixel(const uint8_t *__restrict_
                          w10 * ((p10 >> (8 * c)) & 0xffu) + w11 * ((p11 >> (8 * c)) & 0xffu) + g.half;
     out |= (uint32_t)(((uint64_t)num * g.magic) >> g.shift) << (8 * c);
   }
-  reinterpret_cast<uint32_t *>(dst)[((size_t)frame * g.dh + Y) * g.dw + X] = out;
+  return out;
+}
+// one destination pixel (also run on the host by tests/test_ingest_host.py)
+__host__ __device__ __forceinline__ void ingest_pixel(const uint8_t *__restrict__ src, uint8_t *__restrict__ dst, const IngestGeom &g,
+                                                      int X, int Y, int frame) {
+  const uint32_t *s = reinterpret_cast<const uint32_t *>(src) + (size_t)frame * g.sw * g.sh;
+  reinterpret_cast<uint32_t *>(dst)[((size_t)frame * g.dh + Y) * g.dw + X] = draw_pixel(s, g.sw, g.sh, (size_t)g.sw, g, X, Y);
 }
 __global__ void __launch_bounds__(256) k_ingest(const uint8_t *__restrict__ src, uint8_t *__restrict__ dst, IngestGeom g) {
   const int X = blockIdx.x * 64 + (threadIdx.x & 63), Y = blockIdx.y * 4 + (threadIdx.x >> 6);
   if (X >= g.dw || Y >= g.dh) return;
   ingest_pixel(src, dst, g, X, Y, (int)blockIdx.z);
+}
+
+// ht_tracker_feed: one record per listed stream, each with its own video geometry (== ht_video_frame, pitch resolved)
+struct FeedRec {
+  const uint8_t *src;
+  int32_t stream, width, height, pitch;   // pitch in bytes
+  double now_ms;
+};
+// canvas pixel (X, Y) of record b into canvas b of the arena; g holds the canvas size and its division constants, which
+// do not depend on the video (also run on the host by tests/test_ingest_host.py)
+__host__ __device__ __forceinline__ void feed_draw_pixel(const FeedRec &r, uint8_t *__restrict__ canvas, const IngestGeom &g,
+                                                         int X, int Y, int b) {
+  const uint32_t *s = reinterpret_cast<const uint32_t *>(r.src);
+  const size_t spitch = (size_t)(r.pitch >> 2);
+  const uint32_t out = (r.width == g.dw && r.height == g.dh) ? ld_ro(s + (size_t)Y * spitch + X)   // a 1:1 draw is a copy
+                                                            : draw_pixel(s, r.width, r.height, spitch, g, X, Y);
+  reinterpret_cast<uint32_t *>(canvas)[((size_t)b * g.dh + Y) * g.dw + X] = out;
+}
+// grid = (canvas tiles of 64 x 16 pixels, records).  draw[b] == 0 (an IDLE stream): the record's video is not read.
+// A CTA covers 16 rows (four 4-row passes) so that the two loads every CTA starts with - the record and its flag,
+// issued together - are paid once per 1024 pixels.  A 1:1 record whose rows are 16-byte aligned is copied with 16-byte
+// loads and stores (4 pixels per thread, one pass).
+__global__ void __launch_bounds__(256) k_feed_draw(const FeedRec *__restrict__ recs, const uint8_t *__restrict__ draw,
+                                                   uint8_t *__restrict__ canvas, IngestGeom g, int tiles_x) {
+  const int b = blockIdx.y;
+  const FeedRec r = recs[b];
+  if (!draw[b]) return;
+  const int X0 = (blockIdx.x % tiles_x) * 64, Y0 = (blockIdx.x / tiles_x) * 16;
+  if (r.width == g.dw && r.height == g.dh && (g.dw & 3) == 0 &&
+      ((reinterpret_cast<uintptr_t>(r.src) | (uintptr_t)r.pitch) & 15u) == 0) {
+    const int X = X0 + 4 * (threadIdx.x & 15), Y = Y0 + (threadIdx.x >> 4);
+    if (X >= g.dw || Y >= g.dh) return;
+    const uint4 v = ld_ro(reinterpret_cast<const uint4 *>(r.src + (size_t)Y * r.pitch) + (X >> 2));
+    reinterpret_cast<uint4 *>(canvas + ((size_t)b * g.dh + Y) * g.dw * 4)[X >> 2] = v;
+    return;
+  }
+  const int X = X0 + (threadIdx.x & 63);
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int Y = Y0 + 4 * i + (threadIdx.x >> 6);
+    if (X < g.dw && Y < g.dh) feed_draw_pixel(r, canvas, g, X, Y, b);
+  }
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -1271,31 +1271,38 @@ __host__ __device__ inline void tracker_step(TrackerState &s, const TrackerParam
   out.fov = s.head.fov_saved_deg;                                      // getFOV(), :363-365
 }
 
-// modes -> the masks of the frame's kernels (a TM_IDLE stream's frame is never read)
-__global__ void k_tracker_plan(const TrackerState *__restrict__ st, int n, uint8_t *__restrict__ vj_quad_mask,
-                               uint8_t *__restrict__ cs_enable, uint8_t *__restrict__ init_enable,
-                               uint8_t *__restrict__ wb_enable) {
+// modes -> the masks of the frame's kernels (a TM_IDLE stream's frame is never read).  Batch entry k is stream ids[k]
+// (ids == NULL: stream k); all masks are indexed by batch entry.  draw (ht_tracker_feed, else NULL): the entry's video
+// is drawn onto its canvas - every stream that is not TM_IDLE.
+__global__ void k_tracker_plan(const TrackerState *__restrict__ st, const int32_t *__restrict__ ids, int n,
+                               uint8_t *__restrict__ vj_quad_mask, uint8_t *__restrict__ cs_enable,
+                               uint8_t *__restrict__ init_enable, uint8_t *__restrict__ wb_enable,
+                               uint8_t *__restrict__ draw) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= n) return;
-  const int m = st[k].mode;
+  const int m = st[ids ? ids[k] : k].mode;
   cs_enable[k] = m == TM_CS ? 1 : 0;
   wb_enable[k] = (m == TM_STARTING || m == TM_WB) ? 1 : 0;
   init_enable[k] = 0;
+  if (draw) draw[k] = m != TM_IDLE ? 1 : 0;
   if ((k & 3) == 0) {
     unsigned mask = 0;
-    for (int f = 0; f < 4 && k + f < n; ++f) mask |= (st[k + f].mode == TM_VJ ? 1u : 0u) << f;
+    for (int f = 0; f < 4 && k + f < n; ++f) mask |= (st[ids ? ids[k + f] : k + f].mode == TM_VJ ? 1u : 0u) << f;
     vj_quad_mask[k >> 2] = (uint8_t)mask;
   }
 }
 
-__global__ void k_tracker_update(TrackerState *__restrict__ st, const TrackerParams *__restrict__ params, int n,
+// now (ht_tracker_feed, else NULL): the clock of each batch entry; otherwise every entry ticks at now_ms
+__global__ void k_tracker_update(TrackerState *__restrict__ st, const int32_t *__restrict__ ids,
+                                 const TrackerParams *__restrict__ params, int n,
                                  const unsigned long long *__restrict__ wb_sums, int n_px, const Rect *__restrict__ det,
                                  const int32_t *__restrict__ counts, int K, const int32_t *__restrict__ objs,
-                                 int32_t *__restrict__ rects, uint8_t *__restrict__ init_enable, double now_ms, int camw,
-                                 int camh, TrackerEvent *__restrict__ events) {
+                                 int32_t *__restrict__ rects, uint8_t *__restrict__ init_enable, double now_ms,
+                                 const double *__restrict__ now, int camw, int camh, TrackerEvent *__restrict__ events) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= n) return;
-  TrackerState &s = st[k];                     // updated in place: the window and the head state stay in memory
+  if (now) now_ms = now[k];
+  TrackerState &s = st[ids ? ids[k] : k];      // updated in place: the window and the head state stay in memory
   const bool wants_wb = s.mode == TM_STARTING || s.mode == TM_WB;
   const double wb = wants_wb ? wb_value(wb_sums + 3 * (size_t)k, n_px) : 0.0;
   TrackerEvent e;

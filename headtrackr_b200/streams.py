@@ -90,7 +90,9 @@ class TrackerSet:
     `setTimeout` fires once per step() call.  start(k) / stop(k) are the Tracker's start() / stop() (stop() emits
     "stopped" at once, src/main.js:350); step(frames) runs one timer tick of every stream - starter, whitebalance gate,
     detection, tracking, status events and head position all on the device - and dispatches the reference's payload
-    dicts in the reference's order to the listeners as fn(stream, evt).  `status[k]` is ht.status, getFOV(k) its fov.
+    dicts in the reference's order to the listeners as fn(stream, evt).  feed({stream: video}) ticks only the listed
+    streams, each on its own video frame (any size) and clock, as cameras whose timers fire independently do.
+    `status[k]` is ht.status, getFOV(k) its fov.
     Differs from the reference in one place: start() on a running stream does nothing (the reference runs an extra,
     unscheduled pass)."""
 
@@ -153,8 +155,38 @@ class TrackerSet:
             recs = tracker_events_from_bytes(buf.cpu().numpy().tobytes())
         else:
             recs = self.ctx.tracker_step(frames, now)
-        dt = int((time.time() - t0) * 1000)
-        for k, rec in enumerate(recs):
+        self._dispatch(range(len(recs)), recs, int((time.time() - t0) * 1000))
+        return recs
+
+    def feed(self, frames, now_ms=None, width=None, height=None):
+        """One timer tick of the listed streams only (ht_tracker_feed): frames = {stream: (h, w, 4) u8 video frame}
+        (numpy or torch CUDA, any video size), drawn onto a width x height canvas; now_ms = None (the wall clock), one
+        clock, or {stream: ms}.  Streams not listed do not tick.  -> {stream: record}."""
+        if width is None or height is None:
+            raise ValueError("the canvas size (width, height) is required")
+        ks = list(frames)
+        for k in ks:
+            if not 0 <= k < self.n:
+                raise ValueError(f"stream {k} outside [0, {self.n})")
+        wall = time.time() * 1000.0
+        if isinstance(now_ms, dict):
+            now = [now_ms[k] for k in ks]
+        else:
+            now = wall if now_ms is None else now_ms
+        t0 = time.time()
+        if self._device_events:
+            import torch
+            buf = torch.empty(len(ks) * 144, dtype=torch.uint8, device="cuda")
+            self.ctx.tracker_feed(ks, [frames[k] for k in ks], now, width, height, out=buf)
+            self.ctx.sync()                            # the records are written on the library's stream
+            recs = tracker_events_from_bytes(buf.cpu().numpy().tobytes())
+        else:
+            recs = self.ctx.tracker_feed(ks, [frames[k] for k in ks], now, width, height)
+        self._dispatch(ks, recs, int((time.time() - t0) * 1000))
+        return dict(zip(ks, recs))
+
+    def _dispatch(self, ks, recs, dt):
+        for k, rec in zip(ks, recs):
             self.current[k] = rec
             self._fov[k] = rec["fov"]
             evts, self.status[k] = lifecycle_events(rec, self.status[k])
@@ -162,7 +194,6 @@ class TrackerSet:
                 if e["type"] == "facetrackingEvent":
                     e["time"] = dt
                 self._emit(k, e)
-        return recs
 
     def getFOV(self, k):
         return self._fov[k]

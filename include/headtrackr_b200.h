@@ -189,7 +189,8 @@ int ht_stream_step(ht_ctx *ctx, const uint8_t *rgba, int n, int w, int h, int in
  * samples within 2 gray levels before detection starts), VJ -> CS, the headtrackrStatus events, the lost face with or
  * without retryDetection, and the head-position epilogue of ht_stream_step_head.  Stream k uses tracker slot k.
  * Per stream the mode is one of IDLE (not running: its frame is never read), STARTING, WB, VJ, CS; one
- * ht_tracker_step call is one timer tick of every stream.  Detection runs with interval 5 and min_neighbors 1
+ * ht_tracker_step call is one timer tick of streams [0, n) (ht_tracker_feed: of any subset, each with its own video
+ * and clock).  Detection runs with interval 5 and min_neighbors 1
  * (src/facetrackr.js:147-149).
  * While the lifecycle is configured ht_stream_step / ht_stream_step_head return HT_ERR_STATE (the two share the
  * tracker slots).  One deliberate difference: start() on a running stream does nothing, where the reference would
@@ -230,6 +231,33 @@ int ht_tracker_stop(ht_ctx *ctx, int first, int n);    /* stop() (src/main.js:34
 /* one frame per stream for streams [0, n): rgba = n frames, stream-major; now_ms = (new Date).getTime() of this tick
  * (the "hints" timer, src/main.js:187-194); out[n] host or device (device: enqueue only) */
 int ht_tracker_step(ht_ctx *ctx, const uint8_t *rgba, int n, int w, int h, double now_ms, ht_tracker_event *out);
+
+/* One stream's video frame for ht_tracker_feed (ABI 1.2). */
+typedef struct {
+  const uint8_t *rgba;    /* the stream's video frame: RGBA8, `height` rows of `pitch` bytes */
+  int32_t stream;         /* tracker stream id in [0, max_frames) */
+  int32_t width, height;  /* video size, 1..16384 */
+  int32_t pitch;          /* bytes per row; 0 -> 4*width; a multiple of 4 and >= 4*width */
+  double now_ms;          /* (new Date).getTime() when this stream's timer fired */
+} ht_video_frame;         /* 32 bytes */
+/* One timer tick of each listed stream, each on its own video and clock: drawImage(video, 0, 0, canvas_w, canvas_h)
+ * (src/main.js:170, 312; the canvas resampler of ht_ingest) followed by exactly what ht_tracker_step does for that
+ * stream - a track() pass (src/main.js:168-305) or the starter (src/main.js:307-326).  Cameras tick independently, so
+ * any subset of the streams may be listed, in any order; streams that are not listed do not tick and their state does
+ * not change.  A listed IDLE stream yields ht_tracker_step's IDLE record and its video is neither read nor drawn.
+ *   frames: n HOST records with distinct stream ids.  Their pixel pointers are all device memory (frames_on_device
+ *           = 1) or all host memory (0: the library uploads them); only the first record's pointer is checked.
+ *   canvas_w x canvas_h: the working canvas of every record of the call (it sets the pyramid plan), at most
+ *           max_width x max_height.  The library draws into its own canvas arena ([max_frames] canvases, allocated at
+ *           the first call).
+ *   out[n]: one ht_tracker_event per record, in record order; host or device (device: enqueue only).
+ * Errors (nothing is enqueued): HT_ERR_STATE without ht_tracker_config; HT_ERR_ARG for n outside [1, max_frames], a
+ * stream id out of range or listed twice, a NULL pixel pointer, a pointer or pitch that is not a multiple of 4, a
+ * pitch below 4*width, or a first pointer whose memory space contradicts frames_on_device; HT_ERR_SIZE for a video
+ * size outside 1..16384 or a canvas that is 0-sized, larger than max_width x max_height or too small for the pyramid.
+ * ht_tracker_step and ht_tracker_feed may be mixed on one context: both tick the same per-stream state. */
+int ht_tracker_feed(ht_ctx *ctx, const ht_video_frame *frames, int n, int frames_on_device, int canvas_w, int canvas_h,
+                    ht_tracker_event *out);
 
 /* Frame ingest (SURVEY.md 8f-4): canvasContext.drawImage(videoElement, 0, 0, canvas.width, canvas.height)
  * (src/main.js:170) for n frames - the video frame (sw x sh) scaled onto the working canvas (dw x dh), all four

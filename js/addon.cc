@@ -19,6 +19,11 @@
 //   streamStepHead(handle, rgba, n, w, h, interval, minNeighbors, calcAngles)
 //        -> {events: [...as streamStep...], heads: Array<{valid, found, x, y, z}>}    (ht_stream_step_head)
 //   ingest(handle, rgba /* n video frames */, n, sw, sh, dw, dh) -> Uint8ClampedArray (n canvases)   (ht_ingest)
+//   trackerConfig(handle, {retryDetection, calcAngles, smoothing, fov, cameraOffset, headPosition} | null)
+//   trackerReset / trackerStart / trackerStop(handle, first, n)
+//   trackerStep(handle, rgba /* n canvases */, n, w, h, nowMs) -> Array<{detection, status: [...], running, fov, ...}>
+//   trackerFeed(handle, [{stream, rgba, width, height, nowMs}], canvasWidth, canvasHeight) -> Array<record>
+//        (ht_tracker_feed: only the listed streams tick, each from its own video frame and clock)
 //   destroy(handle)
 #include <node_api.h>
 
@@ -348,8 +353,147 @@ static napi_value Backprojection(napi_env env, napi_callback_info info) {
   return ta;
 }
 
+// headtrackr.Tracker's {retryDetection, calcAngles, smoothing, fov, cameraOffset, headPosition} (src/main.js:35-56), or
+// null to switch the per-stream lifecycle off
+static napi_value TrackerConfig(napi_env env, napi_callback_info info) {
+  size_t argc = 2;
+  napi_value argv[2];
+  NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+  ht_ctx *ctx = Ctx(env, argv[0]);
+  napi_valuetype t = napi_undefined;
+  if (argc > 1) napi_typeof(env, argv[1], &t);
+  int rc;
+  if (t != napi_object) rc = ht_tracker_config(ctx, nullptr);
+  else {
+    ht_tracker_params p;
+    std::memset(&p, 0, sizeof(p));
+    p.retry_detection = GetBoolProp(env, argv[1], "retryDetection", true);
+    p.calc_angles = GetBoolProp(env, argv[1], "calcAngles", false);
+    p.head.smoothing = GetBoolProp(env, argv[1], "smoothing", true);
+    p.head.head_position = GetBoolProp(env, argv[1], "headPosition", true);
+    p.head.edgecorrection = 1;
+    p.head.alpha = 0.35;                                         // src/main.js:163
+    p.head.fov_deg = GetNumProp(env, argv[1], "fov", 0.0);       // <= 0: estimate (src/main.js:283-288)
+    p.head.camera_offset = GetNumProp(env, argv[1], "cameraOffset", 11.5);
+    p.head.distance_to_screen = 60.0;
+    rc = ht_tracker_config(ctx, &p);
+  }
+  if (rc < 0) return Throw(env, ctx, rc);
+  return nullptr;
+}
+
+// trackerReset / trackerStart / trackerStop(handle, first, n)
+static napi_value TrackerRange(napi_env env, napi_callback_info info, int (*fn)(ht_ctx *, int, int)) {
+  size_t argc = 3;
+  napi_value argv[3];
+  NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+  ht_ctx *ctx = Ctx(env, argv[0]);
+  int32_t first, n;
+  napi_get_value_int32(env, argv[1], &first); napi_get_value_int32(env, argv[2], &n);
+  int rc = fn(ctx, first, n);
+  if (rc < 0) return Throw(env, ctx, rc);
+  return nullptr;
+}
+static napi_value TrackerReset(napi_env env, napi_callback_info info) { return TrackerRange(env, info, ht_tracker_reset); }
+static napi_value TrackerStart(napi_env env, napi_callback_info info) { return TrackerRange(env, info, ht_tracker_start); }
+static napi_value TrackerStop(napi_env env, napi_callback_info info) { return TrackerRange(env, info, ht_tracker_stop); }
+
+static const char *kTrackerStatus[] = {"whitebalance", "detecting", "hints", "redetecting", "lost", "stopped", "found"};
+
+// one ht_tracker_event -> {detection: ""|"VJ"|"CS"|"WB", x, y, width, height, angle, confidence, wb, running, fov,
+// status: [headtrackrStatus messages in dispatch order], head: {valid, x, y, z}}
+static napi_value TrackerEventObject(napi_env env, const ht_tracker_event &e) {
+  static const char *kDet[] = {"", "VJ", "CS", "WB"};
+  napi_value o, s, b, st, head;
+  napi_create_object(env, &o);
+  const char *det = (e.detection >= 0 && e.detection <= 3) ? kDet[e.detection] : "";
+  napi_create_string_utf8(env, det, NAPI_AUTO_LENGTH, &s);
+  napi_set_named_property(env, o, "detection", s);
+  SetNum(env, o, "x", e.x); SetNum(env, o, "y", e.y); SetNum(env, o, "width", e.width); SetNum(env, o, "height", e.height);
+  SetNum(env, o, "angle", e.angle); SetNum(env, o, "confidence", e.confidence); SetNum(env, o, "wb", e.wb);
+  SetNum(env, o, "fov", e.fov);
+  napi_get_boolean(env, e.running != 0, &b); napi_set_named_property(env, o, "running", b);
+  napi_create_array(env, &st);
+  uint32_t m = 0;
+  for (int bit = 0; bit < 7; ++bit)
+    if ((e.status >> bit) & 1) {
+      napi_create_string_utf8(env, kTrackerStatus[bit], NAPI_AUTO_LENGTH, &s);
+      napi_set_element(env, st, m++, s);
+    }
+  napi_set_named_property(env, o, "status", st);
+  napi_create_object(env, &head);
+  napi_get_boolean(env, e.head.valid != 0, &b); napi_set_named_property(env, head, "valid", b);
+  SetNum(env, head, "x", e.head.x); SetNum(env, head, "y", e.head.y); SetNum(env, head, "z", e.head.z);
+  napi_set_named_property(env, o, "head", head);
+  return o;
+}
+
+// trackerStep(handle, rgba /* n canvases, one per stream */, n, w, h, nowMs) -> Array<record>   (ht_tracker_step)
+static napi_value TrackerStep(napi_env env, napi_callback_info info) {
+  size_t argc = 6;
+  napi_value argv[6];
+  NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+  ht_ctx *ctx = Ctx(env, argv[0]);
+  uint8_t *rgba; size_t len;
+  int32_t n, w, h;
+  double now_ms;
+  if (!GetBytes(env, argv[1], &rgba, &len)) return Throw(env, ctx, HT_ERR_ARG);
+  napi_get_value_int32(env, argv[2], &n); napi_get_value_int32(env, argv[3], &w); napi_get_value_int32(env, argv[4], &h);
+  napi_get_value_double(env, argv[5], &now_ms);
+  if (n <= 0 || len < (size_t)n * w * h * 4) return Throw(env, ctx, HT_ERR_ARG);
+  std::vector<ht_tracker_event> ev((size_t)n);
+  int rc = ht_tracker_step(ctx, rgba, n, w, h, now_ms, ev.data());
+  if (rc < 0) return Throw(env, ctx, rc);
+  napi_value out;
+  napi_create_array_with_length(env, (size_t)n, &out);
+  for (int k = 0; k < n; ++k) napi_set_element(env, out, (uint32_t)k, TrackerEventObject(env, ev[k]));
+  return out;
+}
+
+// trackerFeed(handle, [{stream, rgba, width, height, nowMs}], canvasWidth, canvasHeight) -> Array<record>, in record
+// order (ht_tracker_feed with host frames: one tick of each listed stream on its own video and clock)
+static napi_value TrackerFeed(napi_env env, napi_callback_info info) {
+  size_t argc = 4;
+  napi_value argv[4];
+  NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+  ht_ctx *ctx = Ctx(env, argv[0]);
+  uint32_t n = 0;
+  int32_t cw, ch;
+  NAPI_OK(napi_get_array_length(env, argv[1], &n));
+  napi_get_value_int32(env, argv[2], &cw); napi_get_value_int32(env, argv[3], &ch);
+  if (n == 0) return Throw(env, ctx, HT_ERR_ARG);
+  std::vector<ht_video_frame> frames(n);
+  for (uint32_t b = 0; b < n; ++b) {
+    napi_value r, v;
+    NAPI_OK(napi_get_element(env, argv[1], b, &r));
+    ht_video_frame &f = frames[b];
+    std::memset(&f, 0, sizeof(f));
+    f.stream = (int32_t)GetNumProp(env, r, "stream", -1);
+    f.width = (int32_t)GetNumProp(env, r, "width", 0);
+    f.height = (int32_t)GetNumProp(env, r, "height", 0);
+    f.now_ms = GetNumProp(env, r, "nowMs", 0.0);
+    uint8_t *rgba; size_t len;
+    NAPI_OK(napi_get_named_property(env, r, "rgba", &v));
+    if (!GetBytes(env, v, &rgba, &len) || len < (size_t)f.width * f.height * 4) return Throw(env, ctx, HT_ERR_ARG);
+    f.rgba = rgba;
+  }
+  std::vector<ht_tracker_event> ev(n);
+  int rc = ht_tracker_feed(ctx, frames.data(), (int)n, 0, cw, ch, ev.data());
+  if (rc < 0) return Throw(env, ctx, rc);
+  napi_value out;
+  napi_create_array_with_length(env, (size_t)n, &out);
+  for (uint32_t b = 0; b < n; ++b) napi_set_element(env, out, b, TrackerEventObject(env, ev[b]));
+  return out;
+}
+
 static napi_value Init(napi_env env, napi_value exports) {
   napi_property_descriptor d[] = {
+      {"trackerConfig", nullptr, TrackerConfig, nullptr, nullptr, nullptr, napi_default, nullptr},
+      {"trackerReset", nullptr, TrackerReset, nullptr, nullptr, nullptr, napi_default, nullptr},
+      {"trackerStart", nullptr, TrackerStart, nullptr, nullptr, nullptr, napi_default, nullptr},
+      {"trackerStop", nullptr, TrackerStop, nullptr, nullptr, nullptr, napi_default, nullptr},
+      {"trackerStep", nullptr, TrackerStep, nullptr, nullptr, nullptr, napi_default, nullptr},
+      {"trackerFeed", nullptr, TrackerFeed, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"create", nullptr, Create, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"detect", nullptr, Detect, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackInit", nullptr, TrackInit, nullptr, nullptr, nullptr, napi_default, nullptr},

@@ -5,6 +5,7 @@ streams: N 640x480 streams, device-resident frames and outputs, CUDA events arou
   tracker_wb      ht_tracker_step while every stream is in the whitebalance gate
   tracker_cs      ht_tracker_step in steady tracking (every stream in "CS")
   stream_head_cs  ht_stream_step_head in steady tracking
+  feed_*          ht_tracker_feed against ht_ingest + ht_tracker_step and ht_tracker_step (feed_arms)
 
 Prints one JSON line with the card's name and power limit read in the same run; --out also writes it to a file."""
 import argparse
@@ -41,10 +42,126 @@ def timed(torch, fn, steps):
     return float(np.median(ts)), float(min(ts))
 
 
+def feed_arms(torch, frames, stream, N, W, H, steps, rounds):
+    """ht_tracker_feed against the ways to get the same ticks without it, in steady tracking, every arm on its own
+    context and all arms alternating tick by tick (the arm order rotates), CUDA events around each call:
+
+      feed_cs          N streams, W x H device video drawn onto a W/2 x H/2 canvas by ht_tracker_feed
+      ingest_step_cs   the same ticks as ht_ingest of the batch into a W/2 x H/2 canvas batch + ht_tracker_step
+      feed_half_idle   feed_cs with every other stream stopped but still listed
+      feed_1to1_cs     ht_tracker_feed of the W x H video onto a W x H canvas (the copy into the canvas arena) ...
+      step_1to1_cs     ... against ht_tracker_step reading the same frames in place
+
+    The records of the timed ticks must agree: feed_cs == ingest_step_cs, feed_1to1_cs == step_1to1_cs, and the running
+    half of feed_half_idle == the same streams of feed_cs.  -> {arm_ms: median, arm_spread_ms: max - min of the
+    per-round medians, ...}"""
+    import ctypes as C
+    from headtrackr_b200 import Context, _lib
+    CW, CH = W // 2, H // 2
+    rec_bytes = C.sizeof(_lib.TrackerEvent)
+    now = [1.0e12]
+
+    def records(n, w, h):
+        arr = (_lib.VideoFrame * n)()
+        for k in range(n):
+            arr[k] = _lib.VideoFrame(frames[k].data_ptr(), k, w, h, 0, 0.0)
+        return arr
+
+    def feed_arm(cw, ch):
+        c = Context(max_width=cw, max_height=ch, max_frames=N, stream=stream)
+        arr, out = records(N, W, H), torch.empty(N * rec_bytes, dtype=torch.uint8, device="cuda")
+
+        def prep():
+            for k in range(N):
+                arr[k].now_ms = now[0]
+
+        def run():
+            c._check(c._L.ht_tracker_feed(c._h, C.addressof(arr), N, 1, cw, ch, out.data_ptr()))
+        return c, prep, run, out
+
+    def ingest_step_arm():
+        c = Context(max_width=CW, max_height=CH, max_frames=N, stream=stream)
+        canvas = torch.empty((N, CH, CW, 4), dtype=torch.uint8, device="cuda")
+        out = torch.empty(N * rec_bytes, dtype=torch.uint8, device="cuda")
+
+        def run():
+            c._check(c._L.ht_ingest(c._h, frames.data_ptr(), N, W, H, canvas.data_ptr(), CW, CH))
+            c._check(c._L.ht_tracker_step(c._h, canvas.data_ptr(), N, CW, CH, now[0], out.data_ptr()))
+        return c, None, run, out
+
+    def step_arm():
+        c = Context(max_width=W, max_height=H, max_frames=N, stream=stream)
+        out = torch.empty(N * rec_bytes, dtype=torch.uint8, device="cuda")
+
+        def run():
+            c._check(c._L.ht_tracker_step(c._h, frames.data_ptr(), N, W, H, now[0], out.data_ptr()))
+        return c, None, run, out
+
+    arms = {"feed_cs": feed_arm(CW, CH), "ingest_step_cs": ingest_step_arm(), "feed_half_idle": feed_arm(CW, CH),
+            "feed_1to1_cs": feed_arm(W, H), "step_1to1_cs": step_arm()}
+    names = list(arms)
+    for c, _, _, _ in arms.values():
+        c.tracker_config()
+        c.tracker_reset(0, N)
+        c.tracker_start(0, N)
+
+    def tick(name):
+        c, prep, run, out = arms[name]
+        if prep:
+            prep()
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        a.record()
+        run()
+        b.record()
+        b.synchronize()
+        return a.elapsed_time(b)
+
+    def recs(name):
+        return np.frombuffer(arms[name][3].cpu().numpy().tobytes(), np.uint8).reshape(N, rec_bytes)
+
+    for _ in range(17):                          # the whitebalance gate, detection, the first CS frames
+        now[0] += 20.0
+        for name in names:
+            tick(name)
+    hc = arms["feed_half_idle"][0]
+    for k in range(1, N, 2):                     # stop() every other stream; they stay listed
+        hc.tracker_stop(k, 1)
+    hc.sync()
+    times = {name: [[] for _ in range(rounds)] for name in names}
+    mismatches = 0
+    for r in range(rounds):
+        for s in range(steps):
+            now[0] += 20.0
+            rot = (r * steps + s) % len(names)
+            for name in names[rot:] + names[:rot]:
+                times[name][r].append(tick(name))
+            fa, fb = recs("feed_cs"), recs("ingest_step_cs")
+            mismatches += int((fa != fb).any(axis=1).sum())
+            mismatches += int((recs("feed_1to1_cs") != recs("step_1to1_cs")).any(axis=1).sum())
+            mismatches += int((recs("feed_half_idle")[0::2] != fa[0::2]).any(axis=1).sum())
+    if mismatches:
+        raise SystemExit(f"feed arms disagree on {mismatches} records of the timed ticks")
+    res = {}
+    for name in names:
+        med = [float(np.median(t)) for t in times[name]]
+        res[f"{name}_ms"] = float(np.median(sum(times[name], [])))
+        res[f"{name}_spread_ms"] = max(med) - min(med)
+    ev = [_lib.TrackerEvent.from_buffer_copy(bytes(row)) for row in recs("feed_cs")]
+    res["feed_cs_streams"] = sum(e.detection == 2 for e in ev)
+    ev = [_lib.TrackerEvent.from_buffer_copy(bytes(row)) for row in recs("feed_half_idle")]
+    res["feed_half_idle_running"] = sum(e.running for e in ev)
+    res["feed_canvas"] = f"{CW}x{CH}"
+    res["feed_records_agree"] = True
+    for c, _, _, _ in arms.values():
+        c.close()
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--streams", type=int, default=1024)
     ap.add_argument("--steps", type=int, default=10)
+    ap.add_argument("--rounds", type=int, default=5, help="rounds of the alternating feed arms (their spread)")
     ap.add_argument("--out")
     a = ap.parse_args()
     import torch
@@ -94,6 +211,7 @@ def main():
     res["stream_head_cs_ms"] = timed(torch, step_head, a.steps)[0]
     res["stream_head_cs_streams"] = sum(e["detection"] == "CS" for e in c.stream_step_head(frames)[0])
     c.close()
+    res.update(feed_arms(torch, frames, stream, N, W, H, a.steps, a.rounds))
     line = json.dumps(res)
     print(line)
     if a.out:
