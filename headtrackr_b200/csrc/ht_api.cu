@@ -6,6 +6,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <cassert>
 #include <cmath>
 #include <cstdarg>
 #include <cstddef>
@@ -16,6 +17,7 @@
 #include <memory>
 #include <string>
 #include <tuple>
+#include <utility>
 #include <vector>
 
 #include "ht_common.cuh"
@@ -36,10 +38,32 @@ template <class T>
 inline T align_up(T v, T a) { return (v + a - 1) / a * a; }
 
 // ------------------------------------------------------------------------------------------------
-// device buffer that only ever grows (no allocation on the steady-state per-frame path)
+// Move-only owner of one CUDA handle, released with its owner.  A null handle (never created, or a host-only
+// self-test build) releases nothing.
+template <class T, cudaError_t (*Release)(T)>
+struct Owned {
+  T h = nullptr;
+  Owned() = default;
+  Owned(const Owned &) = delete;
+  Owned &operator=(const Owned &) = delete;
+  Owned(Owned &&o) noexcept : h(o.h) { o.h = nullptr; }
+  Owned &operator=(Owned &&o) noexcept { std::swap(h, o.h); return *this; }
+  ~Owned() { if (h) Release(h); }
+  operator T() const { return h; }
+};
+using Stream = Owned<cudaStream_t, cudaStreamDestroy>;
+using Event = Owned<cudaEvent_t, cudaEventDestroy>;
+using PinnedHost = Owned<void *, cudaFreeHost>;
+
+// device buffer that only ever grows (no allocation on the steady-state per-frame path); move-only, freed with its owner
 struct DevBuf {
   void *p = nullptr;
   size_t cap = 0;
+  DevBuf() = default;
+  DevBuf(const DevBuf &) = delete;
+  DevBuf &operator=(const DevBuf &) = delete;
+  DevBuf(DevBuf &&o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+  ~DevBuf() { if (p) cudaFree(p); }
   cudaError_t reserve(size_t bytes) {
     if (bytes <= cap) return cudaSuccess;
     if (p) cudaFree(p);
@@ -48,7 +72,6 @@ struct DevBuf {
     if (e == cudaSuccess) cap = bytes;
     return e;
   }
-  void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
   template <class T> T *as() const { return reinterpret_cast<T *>(p); }
 };
 
@@ -460,8 +483,8 @@ struct ht_ctx {
   ht_config cfg{};
   int K = 64, raw_cap = 1024;
   int sms = 132;                            // SMs of the device: grid sizes of the small-batch kernels
-  cudaStream_t stream = nullptr;
-  bool own_stream = false;
+  Stream created_stream;                    // the context's stream when ht_create made it (cfg->cuda_stream is borrowed)
+  cudaStream_t stream = nullptr;            // the context's stream: set once by ht_create
   std::string err;
   uint64_t launches = 0;
 
@@ -478,31 +501,31 @@ struct ht_ctx {
 
   // optional per-kernel-class device timing (CUDA events on the launching stream) for bench.py's roofline
   bool prof_on = false;
-  struct ProfSpan { int cls; cudaEvent_t a, b; };
+  struct ProfSpan { int cls; Event a, b; };
   std::vector<ProfSpan> prof_spans;
-  std::vector<cudaEvent_t> prof_free;
+  std::vector<Event> prof_free;
   double prof_ms[HT_PROF_N] = {0};
   uint64_t prof_launches[HT_PROF_N] = {0};
 
-  cudaEvent_t prof_event() {
-    cudaEvent_t e = nullptr;
-    if (!prof_free.empty()) { e = prof_free.back(); prof_free.pop_back(); }
-    else cudaEventCreate(&e);
+  Event prof_event() {
+    Event e;
+    if (!prof_free.empty()) { e = std::move(prof_free.back()); prof_free.pop_back(); }
+    else cudaEventCreate(&e.h);
     return e;
   }
-  void prof_begin(int cls) {
+  // the span of the launches that follow on `st`, up to prof_end on the same stream
+  void prof_begin(int cls, cudaStream_t st) {
     if (!prof_on) return;
-    ProfSpan s{cls, prof_event(), prof_event()};
-    cudaEventRecord(s.a, stream);
-    prof_spans.push_back(s);
+    prof_spans.push_back(ProfSpan{cls, prof_event(), prof_event()});
+    cudaEventRecord(prof_spans.back().a, st);
   }
-  void prof_end() {
+  void prof_end(cudaStream_t st) {
     if (!prof_on) return;
-    cudaEventRecord(prof_spans.back().b, stream);
+    cudaEventRecord(prof_spans.back().b, st);
   }
 
-  cudaStream_t aux_stream = nullptr;        // tracking of part p overlaps the detection of part p+1 (ht_detect_track)
-  cudaEvent_t aux_done = nullptr, part_events[4] = {nullptr, nullptr, nullptr, nullptr};
+  Stream aux_stream;                        // tracking of part p overlaps the detection of part p+1 (ht_detect_track)
+  Event aux_done, part_events[4];
   unsigned part_seq = 0;
   // ht_set_pipeline: ht_detect_track on device-resident frames with device outputs leaves the tracking of call s on
   // the aux stream and returns; it runs under the detection of call s+1 (k_track is a latency chain that leaves
@@ -513,9 +536,8 @@ struct ht_ctx {
   int pipe_bg = 0;                          // HT_PIPE_BG=1: pipelined tracking runs BELOW the priority of the context's stream,
                                             // and k_cascade leaves room for one k_track CTA per SM while it is in flight
   bool aux_pending = false;                 // work on aux_stream that the context's stream has not waited for yet
-  cudaEvent_t pipe_detect_done = nullptr;
+  Event pipe_detect_done;
   int pipe_parity = 0;
-  cudaStream_t main_stream = nullptr;       // the context's stream while ctx->stream is temporarily the aux stream
   size_t bins_off = 0, hist_off = 0;        // element offsets of the active bin-plane / histogram buffer (parity)
   // Tracking of part p on a second stream while part p+1 is uploaded / detected (ht_detect_track).  Default (-1):
   // only for HOST frames, where the batch arrives at PCIe speed and the GPU has idle time to fill.  For
@@ -525,8 +547,8 @@ struct ht_ctx {
   int wave_mb = 2048;                       // pyramid-arena budget of one wave in MB (HT_WAVE_MB).  Half of the L2 keeps
                                             // the pyramid out of HBM but costs throughput in launch tails (DESIGN.md §5.5)
   int force_ties = 0;                       // ht_debug_set_exactness: force the exactness fallbacks (tests)
-  cudaStream_t pipe_stream = nullptr;
-  cudaEvent_t pipe_start = nullptr, pipe_events[4] = {};
+  Stream pipe_stream;
+  Event pipe_start, pipe_events[4];
   bool use_tma = true;                      // stage level-1 cascade tiles with cp.async.bulk.tensor (HT_TMA=0: 16-byte cp.async)
   DevBuf d_tmaps;                           // [arenas][scales] 128 B CUtensorMaps over the level-1 planes
   const void *tmap_arena = nullptr;
@@ -538,9 +560,9 @@ struct ht_ctx {
   DevBuf d_late_chunk0;
   int overlap_track = -1;
   int overlap_parts = 0;
-  cudaStream_t copy_stream = nullptr;       // H2D staging stream of ht_detect_track
-  cudaEvent_t compute_done = nullptr;
-  std::vector<cudaEvent_t> chunk_events;
+  Stream copy_stream;                       // H2D staging stream of ht_detect_track
+  Event compute_done;
+  std::vector<Event> chunk_events;
   int h2d_chunk = 64;                       // frames per pipelined upload chunk
   int track_cluster = 0;                    // >0: force single-phase k_track with that cluster size (A/B profiling)
   bool track_memo = true;                   // k_track re-uses the moments of windows it has already summed in this
@@ -558,21 +580,20 @@ struct ht_ctx {
   // ht_tracker_feed: the record table {ids[n], clocks[n], FeedRec[n]} goes up in one copy from pinned memory; the
   // videos are drawn into the canvas arena ([max_frames] canvases, indexed by record), zeroed when allocated
   DevBuf d_feed_table, d_feed_draw, d_feed_canvas;
-  void *h_feed_table = nullptr;
-  cudaEvent_t feed_copied = nullptr;        // the last table upload has left h_feed_table
+  PinnedHost h_feed_table;
+  Event feed_copied;                        // the last table upload has left h_feed_table
   bool track_history = true;                // order by the cost of each stream's previous launch (HT_TRACK_HISTORY=0: by window area)
   DevBuf d_track_cost;                      // [max_frames][2] {passes, window pixels / 256} per slot
   int track_heavy_div = 128;                // >0: the n/div costliest streams run on a cluster of
-  int track_heavy_cluster = 8;              //     track_heavy_cluster CTAs on sched_stream (HT_TRACK_HEAVY=div[,cluster])
+  int track_heavy_cluster = 8;              //     track_heavy_cluster CTAs on tier_stream[0] (HT_TRACK_HEAVY=div[,cluster])
   int track_mid_div = 32, track_mid_cluster = 4;  // HT_TRACK_MID=div[,cluster]: the next n/32 costliest streams on clusters of 4
   double track_light_div = 0; int track_light_nt = 256;  // HT_TRACK_LIGHT=div[,threads]: the cheapest n/div streams (div may be fractional) on single CTAs
-  cudaStream_t tier_stream[4] = {nullptr, nullptr, nullptr, nullptr};   // heavy, mid, light, rest (side 3: when tiers are on)
-  cudaEvent_t tier_done[4] = {nullptr, nullptr, nullptr, nullptr};
+  Stream tier_stream[4];                    // heavy, mid, light, rest (side 3: when tiers are on)
+  Event tier_done[4];
   int track_mask_frames = 4;                // >0: mask only streams whose last launch swept more than this many frames' worth of pixels
   int track_mask_min = 4;                   // HT_TRACK_MASK=<min n_calls> (0: off): zero-weight marking of the bin plane before k_track
   int track_prio = 1;                       // HT_TRACK_PRIO=0: tier streams without priorities, the default tier on the context's stream
-  cudaStream_t sched_stream = nullptr;
-  cudaEvent_t sched_ready = nullptr, sched_done = nullptr;
+  Event sched_ready;
   int track_bail_area = 0;                  // >0: two-phase k_track; phase A hands streams with a larger window (px) to phase B
   DevBuf d_sched;                           // k_track two-phase scheduling scratch
   unsigned sched_seq = 0;
@@ -628,17 +649,72 @@ int get_plan(ht_ctx *ctx, int w, int h, int interval, Plan **out) {
   return HT_OK;
 }
 
-// stage n frames on the device if the caller passed host memory
-int device_frames(ht_ctx *ctx, const uint8_t *rgba, int n, int w, int h, const uint8_t **out) {
-  if (!rgba) return ctx->fail(HT_ERR_ARG, "rgba is NULL");
-  if ((reinterpret_cast<uintptr_t>(rgba) & 3u) != 0) return ctx->fail(HT_ERR_ARG, "rgba must be 4-byte aligned");
-  if (is_device_ptr(rgba)) { *out = rgba; return HT_OK; }
-  const size_t bytes = (size_t)n * w * h * 4;
-  CK(ctx->d_frames.reserve(bytes));
-  CK(cudaMemcpyAsync(ctx->d_frames.p, rgba, bytes, cudaMemcpyHostToDevice, ctx->stream));
-  *out = ctx->d_frames.as<uint8_t>();
+// A caller's input of `bytes`: device memory is used in place, host memory goes up asynchronously on `st` into `scratch`.
+template <class T>
+int stage_input(ht_ctx *ctx, cudaStream_t st, const T *src, bool on_device, size_t bytes, DevBuf &scratch, const T **out) {
+  if (on_device) { *out = src; return HT_OK; }
+  CK(scratch.reserve(bytes));
+  CK(cudaMemcpyAsync(scratch.p, src, bytes, cudaMemcpyHostToDevice, st));
+  *out = scratch.as<T>();
   return HT_OK;
 }
+
+int check_frames(ht_ctx *ctx, const uint8_t *rgba) {
+  if (!rgba) return ctx->fail(HT_ERR_ARG, "rgba is NULL");
+  if ((reinterpret_cast<uintptr_t>(rgba) & 3u) != 0) return ctx->fail(HT_ERR_ARG, "rgba must be 4-byte aligned");
+  return HT_OK;
+}
+
+// n frames of w x h: checked, then staged in ctx->d_frames if they are host memory
+int stage_frames(ht_ctx *ctx, cudaStream_t st, const uint8_t *rgba, int n, int w, int h, const uint8_t **out) {
+  const int rc = check_frames(ctx, rgba);
+  if (rc != HT_OK) return rc;
+  return stage_input(ctx, st, rgba, is_device_ptr(rgba), (size_t)n * w * h * 4, ctx->d_frames, out);
+}
+
+// The caller's output buffers of one call.  add() classifies each pointer once: device memory is written in place,
+// host memory through a scratch buffer of the context.  dst() is the pointer the kernels write (NULL for an absent
+// optional output); the scratch buffer must be reserved by then.  finish() copies the host outputs back in registration
+// order on the context's stream, then waits with ht_sync (which also reports the flags the kernels raised) or with a
+// plain stream synchronise - each entry point keeps the one it has always used.  Nothing is copied or awaited when
+// every output is device memory.
+class Outputs {
+ public:
+  enum Sync { SYNC_FLAGS, SYNC_STREAM };
+  explicit Outputs(ht_ctx *c) : ctx(c) {}
+  int add(void *caller, DevBuf &scratch, size_t bytes) {
+    assert(n_ < MAX_OUTPUTS);
+    outs_[n_] = Out{caller, &scratch, bytes, caller && is_device_ptr(caller)};
+    return n_++;
+  }
+  template <class T> T *dst(int i) const {
+    const Out &o = outs_[i];
+    return static_cast<T *>(!o.caller ? nullptr : o.on_device ? o.caller : o.scratch->p);
+  }
+  template <class T> T *out(void *caller, DevBuf &scratch, size_t bytes) { return dst<T>(add(caller, scratch, bytes)); }
+  bool on_device() const {
+    for (int i = 0; i < n_; ++i)
+      if (outs_[i].caller && !outs_[i].on_device) return false;
+    return true;
+  }
+  int finish(Sync sync) {
+    if (on_device()) return HT_OK;
+    for (int i = 0; i < n_; ++i)
+      if (outs_[i].caller && !outs_[i].on_device)
+        CK(cudaMemcpyAsync(outs_[i].caller, outs_[i].scratch->p, outs_[i].bytes, cudaMemcpyDeviceToHost, ctx->stream));
+    if (sync == SYNC_FLAGS) return ht_sync(ctx);
+    CK(cudaStreamSynchronize(ctx->stream));
+    return HT_OK;
+  }
+
+ private:
+  // the most outputs one entry point has (ht_detect_track: rects, counts, found, objs, windows); raise it with a new one
+  static constexpr int MAX_OUTPUTS = 5;
+  struct Out { void *caller; DevBuf *scratch; size_t bytes; bool on_device; };
+  ht_ctx *ctx;
+  Out outs_[MAX_OUTPUTS];
+  int n_ = 0;
+};
 
 // argument check of every batched entry point; it also joins a pipelined call's tracking (ht_set_pipeline) unless the
 // caller is the pipelined path itself
@@ -648,54 +724,54 @@ int check_batch(ht_ctx *ctx, int n, bool join = true) {
   return HT_OK;
 }
 
-int upload_slots(ht_ctx *ctx, const int32_t *slots, int n, const int32_t **d_slots) {
+int upload_slots(ht_ctx *ctx, cudaStream_t st, const int32_t *slots, int n, const int32_t **d_slots) {
   *d_slots = nullptr;
   if (!slots) return HT_OK;
-  if (is_device_ptr(slots)) { *d_slots = slots; return HT_OK; }
-  // two entries with the same slot would make two clusters of k_track (or two CTAs of k_track_init) race on
-  // state[slot] / model_hist[slot].  (Device-resident slot arrays are the caller's responsibility: see the header.)
-  std::vector<uint8_t> seen((size_t)ctx->cfg.max_frames, 0);
-  for (int i = 0; i < n; ++i) {
-    if (slots[i] < 0 || slots[i] >= ctx->cfg.max_frames) return ctx->fail(HT_ERR_ARG, "slot %d out of range", slots[i]);
-    if (seen[(size_t)slots[i]]++) return ctx->fail(HT_ERR_ARG, "slot %d appears twice in one batch", slots[i]);
+  const bool on_device = is_device_ptr(slots);
+  if (!on_device) {
+    // two entries with the same slot would make two clusters of k_track (or two CTAs of k_track_init) race on
+    // state[slot] / model_hist[slot].  (Device-resident slot arrays are the caller's responsibility: see the header.)
+    std::vector<uint8_t> seen((size_t)ctx->cfg.max_frames, 0);
+    for (int i = 0; i < n; ++i) {
+      if (slots[i] < 0 || slots[i] >= ctx->cfg.max_frames) return ctx->fail(HT_ERR_ARG, "slot %d out of range", slots[i]);
+      if (seen[(size_t)slots[i]]++) return ctx->fail(HT_ERR_ARG, "slot %d appears twice in one batch", slots[i]);
+    }
+    CK(ctx->d_slots.reserve(sizeof(int32_t) * ctx->cfg.max_frames));
   }
-  CK(ctx->d_slots.reserve(sizeof(int32_t) * ctx->cfg.max_frames));
-  CK(cudaMemcpyAsync(ctx->d_slots.p, slots, sizeof(int32_t) * n, cudaMemcpyHostToDevice, ctx->stream));
-  *d_slots = ctx->d_slots.as<int32_t>();
-  return HT_OK;
+  return stage_input(ctx, st, slots, on_device, sizeof(int32_t) * n, ctx->d_slots, d_slots);
 }
 
-int ensure_tracker_buffers(ht_ctx *ctx) {
+int ensure_tracker_buffers(ht_ctx *ctx, cudaStream_t st) {
   const size_t mf = (size_t)ctx->cfg.max_frames;
   if (!ctx->model_hist.p) {
     CK(ctx->model_hist.reserve(mf * 4096 * sizeof(uint32_t)));
     CK(ctx->cur_hist.reserve(2 * mf * 4096 * sizeof(uint32_t)));   // two parities (ht_set_pipeline)
     CK(ctx->track_state.reserve(mf * sizeof(TrackState)));
-    CK(cudaMemsetAsync(ctx->track_state.p, 0, mf * sizeof(TrackState), ctx->stream));
+    CK(cudaMemsetAsync(ctx->track_state.p, 0, mf * sizeof(TrackState), st));
     CK(ctx->d_rects.reserve(mf * 4 * sizeof(int32_t)));
     CK(ctx->d_found.reserve(mf * sizeof(int32_t)));
     CK(ctx->d_objs.reserve(mf * 6 * sizeof(int32_t)));
     CK(ctx->d_windows.reserve(mf * 4 * sizeof(int32_t)));
     CK(ctx->d_sched.reserve((2 * mf + 64) * sizeof(int32_t)));
     CK(ctx->d_track_cost.reserve(2 * mf * sizeof(int32_t)));
-    CK(cudaMemsetAsync(ctx->d_track_cost.p, 0, 2 * mf * sizeof(int32_t), ctx->stream));
+    CK(cudaMemsetAsync(ctx->d_track_cost.p, 0, 2 * mf * sizeof(int32_t), st));
     if (ctx->track_trace) {   // [mf x 4] per-stream records, then [mf x 8] phase totals (HT_TRACK_PASSTRACE builds)
       CK(ctx->d_trace.reserve(12 * mf * sizeof(unsigned long long)));
-      CK(cudaMemsetAsync(ctx->d_trace.p, 0, 12 * mf * sizeof(unsigned long long), ctx->stream));
+      CK(cudaMemsetAsync(ctx->d_trace.p, 0, 12 * mf * sizeof(unsigned long long), st));
     }
   }
   return HT_OK;
 }
 
-int launch_hist(ht_ctx *ctx, const uint8_t *d_rgba, int n, int w, int h, uint32_t *hist, uint16_t *bins,
+int launch_hist(ht_ctx *ctx, cudaStream_t st, const uint8_t *d_rgba, int n, int w, int h, uint32_t *hist, uint16_t *bins,
                 const uint8_t *enable = nullptr) {
   const int n_px = w * h;
   int chunks = 1;
   if (n < 4 * ctx->sms) chunks = std::min(64, std::max(1, 8 * ctx->sms / n));  // keep ~8 CTAs per SM busy for small batches
-  if (chunks > 1) CK(cudaMemsetAsync(hist, 0, (size_t)n * 4096 * sizeof(uint32_t), ctx->stream));   // (also for disabled frames: harmless)
-  ctx->prof_begin(HT_PROF_HIST);
-  k_hist<<<dim3(chunks, n), 256, 0, ctx->stream>>>(d_rgba, (size_t)n_px * 4, n_px, hist, bins, chunks, enable);
-  ctx->prof_end();
+  if (chunks > 1) CK(cudaMemsetAsync(hist, 0, (size_t)n * 4096 * sizeof(uint32_t), st));   // (also for disabled frames: harmless)
+  ctx->prof_begin(HT_PROF_HIST, st);
+  k_hist<<<dim3(chunks, n), 256, 0, st>>>(d_rgba, (size_t)n_px * 4, n_px, hist, bins, chunks, enable);
+  ctx->prof_end(st);
   ++ctx->launches;
   CK(cudaGetLastError());
   return HT_OK;
@@ -705,8 +781,30 @@ int launch_hist(ht_ctx *ctx, const uint8_t *d_rgba, int n, int w, int h, uint32_
 // outgrows bail_area stop and are queued.  Phase B: one 8-CTA cluster per queued stream finishes their calls.
 // Mean-shift is a serial chain of window passes per stream, so the few streams with large windows would
 // otherwise set the duration of the whole launch.
-// per-launch options of k_track that do not depend on the batch
-struct TrackOpts {
+using TrackKernel = void (*)(const uint16_t *, int, int, const int32_t *, const uint32_t *, const uint32_t *, TrackState *,
+                             int, int32_t *, int32_t *, int32_t *, unsigned long long *, int, int32_t *, int32_t *, int32_t *,
+                             int, int, unsigned long long *, size_t, int, int, int32_t *, const uint8_t *);
+
+// The k_track instantiations the host picks from at run time: clusters of 1, 2, 4, 8 or 16 CTAs of 128, 256 or 512
+// threads.  Any other cluster size runs on clusters of 8, any other CTA size with 256 threads.
+template <int NT>
+TrackKernel track_kernel(int c) {
+  switch (c) {
+    case 1: return k_track<1, NT>;
+    case 2: return k_track<2, NT>;
+    case 4: return k_track<4, NT>;
+    case 16: return k_track<16, NT>;
+    default: return k_track<8, NT>;
+  }
+}
+TrackKernel track_kernel(int c, int nt) {
+  return nt == 512 ? track_kernel<512>(c) : nt == 128 ? track_kernel<128>(c) : track_kernel<256>(c);
+}
+
+// the arguments of k_track that every launch of one launch_track call shares (the kernel's parameters, in order)
+struct TrackArgs {
+  const uint16_t *bins; int w, h; const int32_t *slots; const uint32_t *mh, *ch; TrackState *state; int n_calls;
+  int32_t *objs, *win, *flag; unsigned long long *stats; int32_t *calls_done, *bail_list, *bail_count;
   unsigned long long *trace;   // HT_TRACK_TRACE=1: per-stream timeline buffer (else NULL)
   size_t trace_stride;         // u64 entries between a stream's record and its phase totals
   int memo;                    // ht_ctx::track_memo
@@ -715,71 +813,27 @@ struct TrackOpts {
   const uint8_t *enable;       // ht_stream_step: per stream, 0 = not tracking this frame (else NULL)
 };
 
-template <int C, int NT = 256>
-cudaError_t launch_track_c(cudaStream_t st, int n, const uint16_t *bins, int w, int h, const int32_t *d_slots,
-                           const uint32_t *mh, const uint32_t *ch, TrackState *state, int n_calls, int32_t *d_objs,
-                           int32_t *d_win, int32_t *flag, unsigned long long *stats, int bail_area, int32_t *calls_done,
-                           int32_t *bail_list, int32_t *bail_count, int use_list, int list_off, TrackOpts opt) {
-  // Same shared-memory carve-out as k_cascade (the maximum): an SM only changes its L1 / shared split when it is idle,
-  // so CTAs of kernels that ask for different splits do not mix on one SM - and k_track is meant to run beside the
-  // detection kernels of the next call (ht_set_pipeline).
-  static bool carveout_set = false;
-  if (!carveout_set) {
-    cudaError_t ce = cudaFuncSetAttribute(k_track<C, NT>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
-    if (ce != cudaSuccess) return ce;
-    carveout_set = true;
-  }
+// k_track over n streams on clusters of c CTAs of nt threads
+cudaError_t launch_k_track(const TrackArgs &a, int c, int nt, cudaStream_t st, int n, int bail_area, int use_list, int list_off) {
+  if (c != 1 && c != 2 && c != 4 && c != 16) c = 8;
+  if (nt != 128 && nt != 512) nt = 256;
   cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)n * C);
-  cfg.blockDim = dim3(NT);
+  cfg.gridDim = dim3((unsigned)n * c);
+  cfg.blockDim = dim3(nt);
   cfg.dynamicSmemBytes = 0;
   cfg.stream = st;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = C; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+  attr[0].val.clusterDim.x = c; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr; cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, k_track<C, NT>, bins, w, h, d_slots, mh, ch, state, n_calls, d_objs, d_win, flag, stats,
-                            bail_area, calls_done, bail_list, bail_count, use_list, list_off, opt.trace, opt.trace_stride, opt.memo, opt.force_serial, opt.cost, opt.enable);
+  return cudaLaunchKernelEx(&cfg, track_kernel(c, nt), a.bins, a.w, a.h, a.slots, a.mh, a.ch, a.state, a.n_calls, a.objs,
+                            a.win, a.flag, a.stats, bail_area, a.calls_done, a.bail_list, a.bail_count, use_list, list_off,
+                            a.trace, a.trace_stride, a.memo, a.force_serial, a.cost, a.enable);
 }
 
-// cluster size x CTA size chosen at run time
-template <int NT>
-cudaError_t launch_track_nt(int c, cudaStream_t st, int n, const uint16_t *bins, int w, int h, const int32_t *d_slots,
-                            const uint32_t *mh, const uint32_t *ch, TrackState *state, int n_calls, int32_t *d_objs,
-                            int32_t *d_win, int32_t *flag, unsigned long long *stats, int32_t *calls_done, int32_t *list,
-                            int32_t *count, int use_list, int list_off, TrackOpts opt) {
-  switch (c) {
-    case 1: return launch_track_c<1, NT>(st, n, bins, w, h, d_slots, mh, ch, state, n_calls, d_objs, d_win, flag, stats, 0, calls_done, list, count, use_list, list_off, opt);
-    case 2: return launch_track_c<2, NT>(st, n, bins, w, h, d_slots, mh, ch, state, n_calls, d_objs, d_win, flag, stats, 0, calls_done, list, count, use_list, list_off, opt);
-    case 4: return launch_track_c<4, NT>(st, n, bins, w, h, d_slots, mh, ch, state, n_calls, d_objs, d_win, flag, stats, 0, calls_done, list, count, use_list, list_off, opt);
-    case 16: {
-      static bool allowed = false;   // clusters of 16 are a non-portable size: opt in once per instantiation
-      if (!allowed) {
-        cudaError_t e = cudaFuncSetAttribute(k_track<16, NT>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
-        if (e != cudaSuccess) return e;
-        allowed = true;
-      }
-      return launch_track_c<16, NT>(st, n, bins, w, h, d_slots, mh, ch, state, n_calls, d_objs, d_win, flag, stats, 0, calls_done, list, count, use_list, list_off, opt);
-    }
-    default: return launch_track_c<8, NT>(st, n, bins, w, h, d_slots, mh, ch, state, n_calls, d_objs, d_win, flag, stats, 0, calls_done, list, count, use_list, list_off, opt);
-  }
-}
-cudaError_t launch_track_any(int c, int nt, cudaStream_t st, int n, const uint16_t *bins, int w, int h, const int32_t *d_slots,
-                             const uint32_t *mh, const uint32_t *ch, TrackState *state, int n_calls, int32_t *d_objs,
-                             int32_t *d_win, int32_t *flag, unsigned long long *stats, int32_t *calls_done, int32_t *list,
-                             int32_t *count, int use_list, int list_off, TrackOpts opt) {
-  if (nt == 512)
-    return launch_track_nt<512>(c, st, n, bins, w, h, d_slots, mh, ch, state, n_calls, d_objs, d_win, flag, stats, calls_done, list, count, use_list, list_off, opt);
-  if (nt == 128)
-    return launch_track_nt<128>(c, st, n, bins, w, h, d_slots, mh, ch, state, n_calls, d_objs, d_win, flag, stats, calls_done, list, count, use_list, list_off, opt);
-  return launch_track_nt<256>(c, st, n, bins, w, h, d_slots, mh, ch, state, n_calls, d_objs, d_win, flag, stats, calls_done, list, count, use_list, list_off, opt);
-}
-
-int launch_track(ht_ctx *ctx, int n, int f0, const uint16_t *bins, int w, int h, const int32_t *d_slots, const uint32_t *mh,
-                 const uint32_t *ch, TrackState *state, int n_calls, int32_t *d_objs, int32_t *d_win, int32_t *flag,
-                 const uint8_t *enable = nullptr) {
-  unsigned long long *stats = ctx->d_flags.as<unsigned long long>() + 8;
-  cudaStream_t st = ctx->stream;
+int launch_track(ht_ctx *ctx, cudaStream_t st, int n, int f0, const uint16_t *bins, int w, int h, const int32_t *d_slots,
+                 const uint32_t *mh, const uint32_t *ch, TrackState *state, int n_calls, int32_t *d_objs, int32_t *d_win,
+                 int32_t *flag, const uint8_t *enable = nullptr) {
   // several track() calls on this frame: mark the plane entries whose weight is +0.0 first (k_bins_mask), k_track then
   // skips whole row segments of them.  (One call per frame - ht_stream_step - does not repay the extra pass.)
   if (ctx->track_mask_min > 0 && n_calls >= ctx->track_mask_min) {
@@ -791,24 +845,23 @@ int launch_track(ht_ctx *ctx, int n, int f0, const uint16_t *bins, int w, int h,
                                                                      ctx->track_mask_frames > 0 ? ctx->d_track_cost.as<int32_t>() : nullptr, min_px256);
     ++ctx->launches;
   }
-  const TrackOpts opt{ctx->track_trace ? ctx->d_trace.as<unsigned long long>() + 4 * (size_t)f0 : nullptr,
-                      // (the kernel indexes both areas with the stream number relative to f0)
-                      4 * (size_t)ctx->cfg.max_frames - 4 * (size_t)f0 + 8 * (size_t)f0,
-                      ctx->track_memo ? 1 : 0, (ctx->force_ties & 4) ? 1 : 0, ctx->d_track_cost.as<int32_t>(), enable};
   // per-chunk scheduling scratch: [calls_done | area n][bail_list | order n][bail_count 1]
   int32_t *calls_done = ctx->d_sched.as<int32_t>() + (size_t)f0;
   int32_t *bail_list = ctx->d_sched.as<int32_t>() + (size_t)ctx->cfg.max_frames + f0;
   int32_t *bail_count = ctx->d_sched.as<int32_t>() + 2 * (size_t)ctx->cfg.max_frames + (ctx->sched_seq++ & 63);
+  const TrackArgs args{bins, w, h, d_slots, mh, ch, state, n_calls, d_objs, d_win, flag,
+                       ctx->d_flags.as<unsigned long long>() + 8, calls_done, bail_list, bail_count,
+                       ctx->track_trace ? ctx->d_trace.as<unsigned long long>() + 4 * (size_t)f0 : nullptr,
+                       // (the kernel indexes both areas with the stream number relative to f0)
+                       4 * (size_t)ctx->cfg.max_frames - 4 * (size_t)f0 + 8 * (size_t)f0,
+                       ctx->track_memo ? 1 : 0, (ctx->force_ties & 4) ? 1 : 0, ctx->d_track_cost.as<int32_t>(), enable};
   cudaError_t e = cudaSuccess;
   if (ctx->track_bail_area > 0) {
     // two-phase (HT_TRACK_BAIL=<px>): an A/B option; the single-phase launch below is the default
     e = cudaMemsetAsync(bail_count, 0, sizeof(int32_t), st);
     if (e != cudaSuccess) return ctx->fail(HT_ERR_CUDA, "memset: %s", cudaGetErrorString(e));
-    e = launch_track_c<1>(st, n, bins, w, h, d_slots, mh, ch, state, n_calls, d_objs, d_win, flag, stats, ctx->track_bail_area,
-                          calls_done, bail_list, bail_count, 0, 0, opt);
-    if (e == cudaSuccess)
-      e = launch_track_c<8>(st, n, bins, w, h, d_slots, mh, ch, state, n_calls, d_objs, d_win, flag, stats, 0, calls_done,
-                            bail_list, bail_count, 1, 0, opt);
+    e = launch_k_track(args, 1, 256, st, n, ctx->track_bail_area, 0, 0);
+    if (e == cudaSuccess) e = launch_k_track(args, 8, 256, st, n, 0, 1, 0);
     ctx->launches += 2;
   } else {
     // few streams -> 8 CTAs per stream (latency of one stream); many streams -> 2 (more streams resident).
@@ -817,8 +870,7 @@ int launch_track(ht_ctx *ctx, int n, int f0, const uint16_t *bins, int w, int h,
     const int nt = ctx->track_nt;
     const bool lpt = ctx->track_lpt && n >= 128;     // below that every stream is resident from the start
     if (!lpt) {
-      e = launch_track_any(c, nt, st, n, bins, w, h, d_slots, mh, ch, state, n_calls, d_objs, d_win, flag, stats, calls_done,
-                           bail_list, bail_count, 0, 0, opt);
+      e = launch_k_track(args, c, nt, st, n, 0, 0, 0);
       ++ctx->launches;
     } else {
       // longest chain first: order the streams by search-window area (k_track_area / k_track_rank); optionally the
@@ -855,25 +907,24 @@ int launch_track(ht_ctx *ctx, int n, int f0, const uint16_t *bins, int w, int h,
         int prio_top = prio_greatest;
         if (ctx->pipeline && ctx->pipe_bg) {   // background mode: every tier below the context's own stream
           int pm = 0;
-          CK(cudaStreamGetPriority(ctx->main_stream ? ctx->main_stream : ctx->stream, &pm));
+          CK(cudaStreamGetPriority(ctx->stream, &pm));
           prio_top = std::min(prio_least, pm + 1);
         }
         for (int t = 0; t < 4; ++t)
           if (!ctx->tier_stream[t]) {
             const int rank = (t == 0) ? 0 : (t == 1 ? 1 : (t == 3 ? 2 : 3));   // heavy, mid, rest, light
             const int prio = ctx->track_prio ? std::min(prio_least, prio_top + rank) : prio_least;
-            CK(cudaStreamCreateWithPriority(&ctx->tier_stream[t], cudaStreamNonBlocking, prio));
-            CK(cudaEventCreateWithFlags(&ctx->tier_done[t], cudaEventDisableTiming));
+            CK(cudaStreamCreateWithPriority(&ctx->tier_stream[t].h, cudaStreamNonBlocking, prio));
+            CK(cudaEventCreateWithFlags(&ctx->tier_done[t].h, cudaEventDisableTiming));
           }
-        if (!ctx->sched_ready) CK(cudaEventCreateWithFlags(&ctx->sched_ready, cudaEventDisableTiming));
+        if (!ctx->sched_ready) CK(cudaEventCreateWithFlags(&ctx->sched_ready.h, cudaEventDisableTiming));
         CK(cudaEventRecord(ctx->sched_ready, st));
       }
       int off = 0;
       for (int t = 0; t < n_tiers && e == cudaSuccess; ++t) {
         cudaStream_t ts = tiers[t].side >= 0 ? ctx->tier_stream[tiers[t].side] : st;
         if (tiers[t].side >= 0) CK(cudaStreamWaitEvent(ts, ctx->sched_ready, 0));
-        e = launch_track_any(tiers[t].cluster, tiers[t].threads, ts, tiers[t].count, bins, w, h, d_slots, mh, ch, state, n_calls,
-                             d_objs, d_win, flag, stats, calls_done, bail_list, bail_count, 2, off, opt);
+        e = launch_k_track(args, tiers[t].cluster, tiers[t].threads, ts, tiers[t].count, 0, 2, off);
         ++ctx->launches;
         if (tiers[t].side >= 0) CK(cudaEventRecord(ctx->tier_done[tiers[t].side], ts));
         off += tiers[t].count;
@@ -886,24 +937,20 @@ int launch_track(ht_ctx *ctx, int n, int f0, const uint16_t *bins, int w, int h,
   return HT_OK;
 }
 
-int track_init_common(ht_ctx *ctx, const int32_t *slots, int n, const uint8_t *d_rgba, int w, int h,
+int track_init_common(ht_ctx *ctx, cudaStream_t st, const int32_t *slots, int n, const uint8_t *d_rgba, int w, int h,
                       const int32_t *d_rects, int calc_angles, int32_t *out_found) {
   const int32_t *d_slots = nullptr;
-  int rc = upload_slots(ctx, slots, n, &d_slots);
+  int rc = upload_slots(ctx, st, slots, n, &d_slots);
   if (rc != HT_OK) return rc;
-  const bool found_dev = out_found && is_device_ptr(out_found);
-  int32_t *d_found = out_found ? (found_dev ? out_found : ctx->d_found.as<int32_t>()) : nullptr;
-  ctx->prof_begin(HT_PROF_TRACK_INIT);
-  k_track_init<<<n, 256, 0, ctx->stream>>>(d_rgba, (size_t)w * h * 4, w, h, d_slots, d_rects, calc_angles ? 1 : 0,
-                                           ctx->model_hist.as<uint32_t>(), ctx->track_state.as<TrackState>(), d_found, nullptr);
-  ctx->prof_end();
+  Outputs io(ctx);
+  int32_t *d_found = io.out<int32_t>(out_found, ctx->d_found, sizeof(int32_t) * n);
+  ctx->prof_begin(HT_PROF_TRACK_INIT, st);
+  k_track_init<<<n, 256, 0, st>>>(d_rgba, (size_t)w * h * 4, w, h, d_slots, d_rects, calc_angles ? 1 : 0,
+                                  ctx->model_hist.as<uint32_t>(), ctx->track_state.as<TrackState>(), d_found, nullptr);
+  ctx->prof_end(st);
   ++ctx->launches;
   CK(cudaGetLastError());
-  if (out_found && !found_dev) {
-    CK(cudaMemcpyAsync(out_found, d_found, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-  }
-  return HT_OK;
+  return io.finish(Outputs::SYNC_STREAM);
 }
 
 // Shared memory of one k_cascade CTA: the staged tile and three sets of per-class survivor bit masks.
@@ -921,13 +968,21 @@ int set_kernel_attributes(ht_ctx *ctx) {
   CK(cudaFuncSetAttribute(k_cascade<false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
   CK(cudaFuncSetAttribute(k_gray<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GRAY_HIST_SMEM));
   CK(cudaFuncSetAttribute(k_gray<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GRAY_HIST_SMEM));
+  // k_track: the same shared-memory carve-out as k_cascade (the maximum).  An SM only changes its L1 / shared split when
+  // it is idle, so CTAs of kernels that ask for different splits do not mix on one SM - and k_track is meant to run
+  // beside the detection kernels of the next call (ht_set_pipeline).  Clusters of 16 are a non-portable size.
+  for (const int c : {1, 2, 4, 8, 16})
+    for (const int nt : {128, 256, 512}) {
+      CK(cudaFuncSetAttribute(track_kernel(c, nt), cudaFuncAttributePreferredSharedMemoryCarveout, 100));
+      if (c == 16) CK(cudaFuncSetAttribute(track_kernel(c, nt), cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+    }
   return HT_OK;
 }
 
 // Tensor maps for the TMA staging of level-1 cascade tiles: one 3-D map (column, row, frame quad) per scale and
 // arena over the pyramid arena (32-bit elements: one word = the pixel in 4 frames).  Re-encoded whenever the arena
 // allocation, its partition into waves or the plan changes.
-int ensure_tensor_maps(ht_ctx *ctx, Plan *P, int n_arenas, size_t wave_words, int quads_per_arena) {
+int ensure_tensor_maps(ht_ctx *ctx, cudaStream_t st, Plan *P, int n_arenas, size_t wave_words, int quads_per_arena) {
   if (ctx->tmap_arena == ctx->arena.p && ctx->tmap_plan == P && ctx->tmap_wave_words == wave_words && ctx->tmap_arenas == n_arenas)
     return HT_OK;
   typedef CUresult (*encode_fn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
@@ -964,8 +1019,8 @@ int ensure_tensor_maps(ht_ctx *ctx, Plan *P, int n_arenas, size_t wave_words, in
       if (r != CUDA_SUCCESS) return ctx->fail(HT_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d) for scale %d", (int)r, (int)i);
     }
   CK(ctx->d_tmaps.reserve(maps.size() * sizeof(CUtensorMap)));
-  CK(cudaMemcpyAsync(ctx->d_tmaps.p, maps.data(), maps.size() * sizeof(CUtensorMap), cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));   // `maps` is a local; re-encoding only happens when buffers change
+  CK(cudaMemcpyAsync(ctx->d_tmaps.p, maps.data(), maps.size() * sizeof(CUtensorMap), cudaMemcpyHostToDevice, st));
+  CK(cudaStreamSynchronize(st));   // `maps` is a local; re-encoding only happens when buffers change
   ctx->tmap_arena = ctx->arena.p;
   ctx->tmap_plan = P;
   ctx->tmap_wave_words = wave_words;
@@ -987,10 +1042,9 @@ struct HistOut {
 // round trip through HBM for the whole batch.  With
 // ctx->detect_pipe the gray + pyramid kernels of wave w+1 run on a second stream (and a second arena) under the
 // cascade of wave w.
-int run_detect(ht_ctx *ctx, Plan *P, const uint8_t *d_rgba_batch, int f0, int n, int min_neighbors, Rect *d_rects_batch,
-               int32_t *d_counts_batch, HistOut ho = HistOut{nullptr, nullptr}, const uint8_t *quad_mask = nullptr,
-               cudaEvent_t before_group = nullptr) {
-  cudaStream_t st = ctx->stream;
+int run_detect(ht_ctx *ctx, cudaStream_t st, Plan *P, const uint8_t *d_rgba_batch, int f0, int n, int min_neighbors,
+               Rect *d_rects_batch, int32_t *d_counts_batch, HistOut ho = HistOut{nullptr, nullptr},
+               const uint8_t *quad_mask = nullptr, cudaEvent_t before_group = nullptr) {
   const int w = P->w, h = P->h;
   const size_t frame_bytes = (size_t)w * h * 4;
   // frames per wave: HT_WAVE, or as many as fit the arena budget (one frame of a quad costs arena_stride bytes)
@@ -1000,7 +1054,7 @@ int run_detect(ht_ctx *ctx, Plan *P, const uint8_t *d_rgba_batch, int f0, int n,
   const bool piped = ctx->detect_pipe > 0 && n > wave;
   CK(ctx->arena.reserve(wave_words * 4 * (piped ? 2 : 1)));
   if (ctx->use_tma) {
-    const int trc = ensure_tensor_maps(ctx, P, piped ? 2 : 1, wave_words, wave / 4);
+    const int trc = ensure_tensor_maps(ctx, st, P, piped ? 2 : 1, wave_words, wave / 4);
     if (trc != HT_OK) return trc;
   }
   CK(cudaMemsetAsync(ctx->raw_count.as<uint32_t>() + f0, 0, sizeof(uint32_t) * n, st));
@@ -1014,9 +1068,9 @@ int run_detect(ht_ctx *ctx, Plan *P, const uint8_t *d_rgba_batch, int f0, int n,
     g_loaded_cascade[ctx->cfg.device & 63] = ctx->hc.id;
   }
   if (piped && !ctx->pipe_stream) {
-    CK(cudaStreamCreateWithFlags(&ctx->pipe_stream, cudaStreamNonBlocking));
-    CK(cudaEventCreateWithFlags(&ctx->pipe_start, cudaEventDisableTiming));
-    for (int i = 0; i < 4; ++i) CK(cudaEventCreateWithFlags(&ctx->pipe_events[i], cudaEventDisableTiming));
+    CK(cudaStreamCreateWithFlags(&ctx->pipe_stream.h, cudaStreamNonBlocking));
+    CK(cudaEventCreateWithFlags(&ctx->pipe_start.h, cudaEventDisableTiming));
+    for (Event &e : ctx->pipe_events) CK(cudaEventCreateWithFlags(&e.h, cudaEventDisableTiming));
   }
   if (piped) {   // earlier work on the arena / frames is ordered before the first pyramid
     CK(cudaEventRecord(ctx->pipe_start, st));
@@ -1031,7 +1085,6 @@ int run_detect(ht_ctx *ctx, Plan *P, const uint8_t *d_rgba_batch, int f0, int n,
     const uint8_t *qm = quad_mask ? quad_mask + w0 / 4 : nullptr;   // (ht_stream_step) quads of this wave that have work
     cudaStream_t ps = piped ? ctx->pipe_stream : st;
     if (piped && wi >= 2) CK(cudaStreamWaitEvent(ps, ctx->pipe_events[2 + (wi & 1)], 0));   // cascade of wave wi-2 is done with this arena
-    ctx->stream = ps;
     // K1 grayscale (+ histogram + bin plane) -> plane 0
     {
       const bool hist = ho.hist != nullptr;
@@ -1040,7 +1093,7 @@ int run_detect(ht_ctx *ctx, Plan *P, const uint8_t *d_rgba_batch, int f0, int n,
       if (hist) chunks = std::max(chunks, (w * h + 59999) / 60000);   // 16-bit histogram counters per CTA
       uint32_t *hp = hist ? ho.hist + (size_t)w0 * 4096 : nullptr;
       uint16_t *bp = ho.bins ? ho.bins + (size_t)w0 * w * h : nullptr;
-      ctx->prof_begin(HT_PROF_GRAY);
+      ctx->prof_begin(HT_PROF_GRAY, ps);
       const dim3 grid((unsigned)chunks, (unsigned)quads);
       if (hist) {
         if (vec) k_gray<true, true><<<grid, 256, GRAY_HIST_SMEM, ps>>>(d_rgba, frame_bytes, nw, arena, P->arena_stride, w, h, P->planes[0].pitch, hp, bp, chunks, qm);
@@ -1049,27 +1102,26 @@ int run_detect(ht_ctx *ctx, Plan *P, const uint8_t *d_rgba_batch, int f0, int n,
         if (vec) k_gray<true, false><<<grid, 256, 0, ps>>>(d_rgba, frame_bytes, nw, arena, P->arena_stride, w, h, P->planes[0].pitch, nullptr, nullptr, chunks, qm);
         else k_gray<false, false><<<grid, 256, 0, ps>>>(d_rgba, frame_bytes, nw, arena, P->arena_stride, w, h, P->planes[0].pitch, nullptr, nullptr, chunks, qm);
       }
-      ctx->prof_end();
+      ctx->prof_end(ps);
       ++ctx->launches;
     }
     // K2 pyramid generations
     for (size_t g = 1; g + 1 < P->gen_tile_begin.size(); ++g) {
       const int t0 = P->gen_tile_begin[g], t1 = P->gen_tile_begin[g + 1];
       if (t1 > t0) {
-        ctx->prof_begin(HT_PROF_PYRAMID);
+        ctx->prof_begin(HT_PROF_PYRAMID, ps);
         k_resample<<<dim3(t1 - t0, quads), 256, 0, ps>>>(P->dplan, t0, arena, P->arena_stride, nw, qm);
-        ctx->prof_end();
+        ctx->prof_end(ps);
         ++ctx->launches;
       }
     }
-    ctx->stream = st;
     if (piped) {
       CK(cudaEventRecord(ctx->pipe_events[wi & 1], ps));
       CK(cudaStreamWaitEvent(st, ctx->pipe_events[wi & 1], 0));
     }
     // K3 cascade
     if (!P->casc_tiles.empty()) {
-      ctx->prof_begin(HT_PROF_CASCADE);
+      ctx->prof_begin(HT_PROF_CASCADE, st);
       auto kern = ctx->hc.fast ? k_cascade<true> : k_cascade<false>;
       // background mode: while the previous call's tracking is in flight, three cascade CTAs per SM instead of four
       const size_t casc_smem = (before_group && ctx->pipe_bg) ? std::max(CASC_SMEM, CASC_SMEM_BG) : CASC_SMEM;
@@ -1079,7 +1131,7 @@ int run_detect(ht_ctx *ctx, Plan *P, const uint8_t *d_rgba_batch, int f0, int n,
           arena, P->arena_stride, nw,
           ctx->raw_keys.as<uint32_t>() + (size_t)fa * ctx->raw_cap, ctx->raw_conf.as<double>() + (size_t)fa * ctx->raw_cap,
           ctx->raw_count.as<uint32_t>() + fa, ctx->raw_cap, ctx->force_ties, qm);
-      ctx->prof_end();
+      ctx->prof_end(st);
       ++ctx->launches;
     }
     if (piped) CK(cudaEventRecord(ctx->pipe_events[2 + (wi & 1)], st));
@@ -1089,7 +1141,7 @@ int run_detect(ht_ctx *ctx, Plan *P, const uint8_t *d_rgba_batch, int f0, int n,
   }
   // K4 sort + group
   if (before_group) CK(cudaStreamWaitEvent(st, before_group, 0));   // (pipelined calls) the previous call's tracking still reads the rectangle arrays
-  ctx->prof_begin(HT_PROF_GROUP);
+  ctx->prof_begin(HT_PROF_GROUP, st);
   k_group<<<(n + 3) / 4, 128, 0, st>>>(P->dplan, n, ctx->raw_keys.as<uint32_t>() + (size_t)f0 * ctx->raw_cap,
                                        ctx->raw_conf.as<double>() + (size_t)f0 * ctx->raw_cap,
                                        ctx->raw_count.as<uint32_t>() + f0, ctx->raw_cap,
@@ -1098,55 +1150,56 @@ int run_detect(ht_ctx *ctx, Plan *P, const uint8_t *d_rgba_batch, int f0, int n,
                                        ctx->seq2.as<Rect>() + (size_t)f0 * ctx->raw_cap, min_neighbors,
                                        d_rects_batch + (size_t)f0 * ctx->K, d_counts_batch + f0, ctx->K,
                                        ctx->d_flags.as<int32_t>());
-  ctx->prof_end();
+  ctx->prof_end(st);
   ++ctx->launches;
   CK(cudaGetLastError());
   return HT_OK;
 }
 
 // pick (optional) + initTracker + n_calls x track() for frames [f0, f0+n); slot of frame k is k (slots == NULL)
-int run_track_from_detect(ht_ctx *ctx, const uint8_t *d_rgba_batch, int w, int h, int f0, int n, const Rect *d_det,
-                          const int32_t *d_cnt, int calc_angles, int n_calls, int32_t *d_found, int32_t *d_objs,
-                          int32_t *d_win) {
-  cudaStream_t st = ctx->stream;
+int run_track_from_detect(ht_ctx *ctx, cudaStream_t st, const uint8_t *d_rgba_batch, int w, int h, int f0, int n,
+                          const Rect *d_det, const int32_t *d_cnt, int calc_angles, int n_calls, int32_t *d_found,
+                          int32_t *d_objs, int32_t *d_win) {
   const uint8_t *d_rgba = d_rgba_batch + (size_t)f0 * w * h * 4;
   int32_t *d_rects4 = ctx->d_rects.as<int32_t>() + 4 * (size_t)f0;
-  ctx->prof_begin(HT_PROF_TRACK_INIT);
+  ctx->prof_begin(HT_PROF_TRACK_INIT, st);
   k_pick_face<<<(n + 127) / 128, 128, 0, st>>>(d_det + (size_t)f0 * ctx->K, d_cnt + f0, ctx->K, n, d_rects4);
   k_track_init<<<n, 256, 0, st>>>(d_rgba, (size_t)w * h * 4, w, h, nullptr, d_rects4, calc_angles ? 1 : 0,
                                   ctx->model_hist.as<uint32_t>() + (size_t)f0 * 4096,
                                   ctx->track_state.as<TrackState>() + f0, d_found ? d_found + f0 : nullptr, nullptr);
-  ctx->prof_end();
+  ctx->prof_end(st);
   ctx->launches += 2;
   if (n_calls > 0) {
     // the current-frame histograms and the bin plane were produced by the gray pass of run_detect (one frame read)
     uint16_t *bins = ctx->bins.as<uint16_t>() + ctx->bins_off + (size_t)f0 * w * h;
-    ctx->prof_begin(HT_PROF_TRACK);
-    int rc = launch_track(ctx, n, f0, bins, w, h, nullptr, ctx->model_hist.as<uint32_t>() + (size_t)f0 * 4096,
+    ctx->prof_begin(HT_PROF_TRACK, st);
+    int rc = launch_track(ctx, st, n, f0, bins, w, h, nullptr, ctx->model_hist.as<uint32_t>() + (size_t)f0 * 4096,
                       ctx->cur_hist.as<uint32_t>() + ctx->hist_off + (size_t)f0 * 4096, ctx->track_state.as<TrackState>() + f0, n_calls,
                       d_objs + 6 * (size_t)f0, d_win ? d_win + 4 * (size_t)f0 : nullptr, ctx->d_flags.as<int32_t>() + 2);
     if (rc != HT_OK) return rc;
-    ctx->prof_end();
+    ctx->prof_end(st);
   }
   CK(cudaGetLastError());
   return HT_OK;
 }
 
-// Host frames -> ctx->d_frames in chunks on the copy stream; chunk c is complete when ctx->chunk_events[c] fires.
-int upload_chunks(ht_ctx *ctx, const uint8_t *rgba, int n, size_t frame_bytes, int *chunk_out, int *n_chunks_out) {
+// Host frames -> ctx->d_frames in chunks on the copy stream, after the work enqueued so far on `st`; chunk c is complete
+// when ctx->chunk_events[c] fires.
+int upload_chunks(ht_ctx *ctx, cudaStream_t st, const uint8_t *rgba, int n, size_t frame_bytes, int *chunk_out,
+                  int *n_chunks_out) {
   CK(ctx->d_frames.reserve(frame_bytes * (size_t)n));
   if (!ctx->copy_stream) {
-    CK(cudaStreamCreateWithFlags(&ctx->copy_stream, cudaStreamNonBlocking));
+    CK(cudaStreamCreateWithFlags(&ctx->copy_stream.h, cudaStreamNonBlocking));
   }
   const int chunk = std::max(1, std::min(n, ctx->h2d_chunk));
   const int n_chunks = (n + chunk - 1) / chunk;
   while ((int)ctx->chunk_events.size() < n_chunks) {
-    cudaEvent_t e;
-    CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    ctx->chunk_events.push_back(e);
+    Event e;
+    CK(cudaEventCreateWithFlags(&e.h, cudaEventDisableTiming));
+    ctx->chunk_events.push_back(std::move(e));
   }
   // the staging buffer may still be read by work enqueued earlier on the compute stream
-  CK(cudaEventRecord(ctx->compute_done, ctx->stream));
+  CK(cudaEventRecord(ctx->compute_done, st));
   CK(cudaStreamWaitEvent(ctx->copy_stream, ctx->compute_done, 0));
   uint8_t *d_frames = ctx->d_frames.as<uint8_t>();
   for (int c = 0; c < n_chunks; ++c) {
@@ -1157,6 +1210,25 @@ int upload_chunks(ht_ctx *ctx, const uint8_t *rgba, int n, size_t frame_bytes, i
   }
   *chunk_out = chunk;
   *n_chunks_out = n_chunks;
+  return HT_OK;
+}
+
+// The aux stream of ht_detect_track and its events, made by whichever of its two users comes first.  The pipelined
+// path (ht_set_pipeline) makes it at the top priority, or just below the context's stream in background mode
+// (HT_PIPE_BG=1); the overlap of parts makes it at the default priority.
+int ensure_aux_stream(ht_ctx *ctx, bool pipelined) {
+  if (ctx->aux_stream) return HT_OK;
+  if (pipelined) {
+    int prio_least = 0, prio_greatest = 0, aux_prio = 0;
+    CK(cudaDeviceGetStreamPriorityRange(&prio_least, &prio_greatest));
+    aux_prio = prio_greatest;
+    if (ctx->pipe_bg) { int pm = 0; CK(cudaStreamGetPriority(ctx->stream, &pm)); aux_prio = std::min(prio_least, pm + 1); }
+    CK(cudaStreamCreateWithPriority(&ctx->aux_stream.h, cudaStreamNonBlocking, aux_prio));
+  } else {
+    CK(cudaStreamCreateWithFlags(&ctx->aux_stream.h, cudaStreamNonBlocking));
+  }
+  CK(cudaEventCreateWithFlags(&ctx->aux_done.h, cudaEventDisableTiming));
+  for (Event &e : ctx->part_events) CK(cudaEventCreateWithFlags(&e.h, cudaEventDisableTiming));
   return HT_OK;
 }
 
@@ -1201,8 +1273,8 @@ int ht_create(ht_ctx **out, const ht_config *cfg, const void *cascade_blob, size
   if (rc != HT_OK) { g_create_error = "ht_create: " + err; return rc; }
   if (cfg->cuda_stream) c->stream = static_cast<cudaStream_t>(cfg->cuda_stream);
   else {
-    if (cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking) != cudaSuccess) { g_create_error = "ht_create: stream"; return HT_ERR_CUDA; }
-    c->own_stream = true;
+    if (cudaStreamCreateWithFlags(&c->created_stream.h, cudaStreamNonBlocking) != cudaSuccess) { g_create_error = "ht_create: stream"; return HT_ERR_CUDA; }
+    c->stream = c->created_stream;
   }
   if (const char *tc = getenv("HT_TRACK_CLUSTER")) c->track_cluster = atoi(tc);
   if (const char *ba = getenv("HT_TRACK_BAIL")) c->track_bail_area = atoi(ba);
@@ -1246,7 +1318,7 @@ int ht_create(ht_ctx **out, const ht_config *cfg, const void *cascade_blob, size
     c->track_mask_min = std::max(0, atoi(tk));
     if (const char *comma = strchr(tk, ',')) c->track_mask_frames = std::max(0, atoi(comma + 1));
   }
-  if (cudaEventCreateWithFlags(&c->compute_done, cudaEventDisableTiming) != cudaSuccess) { g_create_error = "ht_create: event"; return HT_ERR_CUDA; }
+  if (cudaEventCreateWithFlags(&c->compute_done.h, cudaEventDisableTiming) != cudaSuccess) { g_create_error = "ht_create: event"; return HT_ERR_CUDA; }
   // the cascade image is copied into __constant__ memory lazily by run_detect; the late-stage table lives in HBM
   if (c->d_casc.reserve(c->hc.late.size() * sizeof(LateFeat)) != cudaSuccess ||
       cudaMemcpy(c->d_casc.p, c->hc.late.data(), c->hc.late.size() * sizeof(LateFeat), cudaMemcpyHostToDevice) != cudaSuccess ||
@@ -1278,35 +1350,6 @@ void ht_destroy(ht_ctx *ctx) {
   cudaSetDevice(ctx->cfg.device);
   if (ctx->aux_stream) cudaStreamSynchronize(ctx->aux_stream);
   cudaStreamSynchronize(ctx->stream);
-  for (auto &kv : ctx->plans) kv.second->dev.release();
-  DevBuf *bufs[] = {&ctx->d_casc, &ctx->arena, &ctx->d_frames, &ctx->raw_keys, &ctx->raw_conf, &ctx->raw_count, &ctx->sorted,
-                    &ctx->labels, &ctx->seq2, &ctx->d_out_rects, &ctx->d_out_counts, &ctx->d_flags, &ctx->model_hist,
-                    &ctx->bins, &ctx->d_sched, &ctx->d_trace, &ctx->d_tmaps, &ctx->d_late_chunk0, &ctx->d_track_cost, &ctx->d_stream_mode, &ctx->d_stream_mask, &ctx->d_stream_cs, &ctx->d_stream_init, &ctx->d_stream_events, &ctx->d_head_state, &ctx->d_head_params, &ctx->d_head_events, &ctx->d_tracker_state, &ctx->d_tracker_params, &ctx->d_tracker_events, &ctx->d_tracker_wb, &ctx->cur_hist, &ctx->track_state, &ctx->d_slots, &ctx->d_rects, &ctx->d_found, &ctx->d_objs,
-                    &ctx->d_windows, &ctx->d_wb_sums, &ctx->d_wb_out, &ctx->d_scratch, &ctx->d_feed_table, &ctx->d_feed_draw,
-                    &ctx->d_feed_canvas};
-  for (DevBuf *b : bufs) b->release();
-  if (ctx->h_feed_table) cudaFreeHost(ctx->h_feed_table);
-  if (ctx->feed_copied) cudaEventDestroy(ctx->feed_copied);
-  for (auto &sp : ctx->prof_spans) { cudaEventDestroy(sp.a); cudaEventDestroy(sp.b); }
-  for (cudaEvent_t e : ctx->prof_free) cudaEventDestroy(e);
-  for (cudaEvent_t e : ctx->chunk_events) cudaEventDestroy(e);
-  if (ctx->compute_done) cudaEventDestroy(ctx->compute_done);
-  if (ctx->copy_stream) cudaStreamDestroy(ctx->copy_stream);
-  if (ctx->pipe_stream) cudaStreamDestroy(ctx->pipe_stream);
-  if (ctx->pipe_start) cudaEventDestroy(ctx->pipe_start);
-  for (cudaEvent_t e : ctx->pipe_events) if (e) cudaEventDestroy(e);
-  if (ctx->sched_stream) cudaStreamDestroy(ctx->sched_stream);
-  for (int t = 0; t < 4; ++t) {
-    if (ctx->tier_stream[t]) cudaStreamDestroy(ctx->tier_stream[t]);
-    if (ctx->tier_done[t]) cudaEventDestroy(ctx->tier_done[t]);
-  }
-  if (ctx->sched_ready) cudaEventDestroy(ctx->sched_ready);
-  if (ctx->sched_done) cudaEventDestroy(ctx->sched_done);
-  if (ctx->aux_stream) cudaStreamDestroy(ctx->aux_stream);
-  if (ctx->aux_done) cudaEventDestroy(ctx->aux_done);
-  if (ctx->pipe_detect_done) cudaEventDestroy(ctx->pipe_detect_done);
-  for (cudaEvent_t e : ctx->part_events) if (e) cudaEventDestroy(e);
-  if (ctx->own_stream) cudaStreamDestroy(ctx->stream);
   delete ctx;
 }
 
@@ -1335,33 +1378,30 @@ int ht_detect(ht_ctx *ctx, const uint8_t *rgba, int n, int w, int h, int interva
   Plan *P = nullptr;
   rc = get_plan(ctx, w, h, interval, &P);
   if (rc != HT_OK) return rc;
-  if (!rgba) return ctx->fail(HT_ERR_ARG, "rgba is NULL");
-  if ((reinterpret_cast<uintptr_t>(rgba) & 3u) != 0) return ctx->fail(HT_ERR_ARG, "rgba must be 4-byte aligned");
+  rc = check_frames(ctx, rgba);
+  if (rc != HT_OK) return rc;
   cudaStream_t st = ctx->stream;
-  const bool rects_dev = is_device_ptr(out_rects), counts_dev = is_device_ptr(out_counts);
-  Rect *d_rects = rects_dev ? reinterpret_cast<Rect *>(out_rects) : ctx->d_out_rects.as<Rect>();
-  int32_t *d_counts = counts_dev ? out_counts : ctx->d_out_counts.as<int32_t>();
+  Outputs io(ctx);
+  Rect *d_rects = io.out<Rect>(out_rects, ctx->d_out_rects, sizeof(Rect) * (size_t)n * ctx->K);
+  int32_t *d_counts = io.out<int32_t>(out_counts, ctx->d_out_counts, sizeof(int32_t) * n);
   if (is_device_ptr(rgba)) {
-    rc = run_detect(ctx, P, rgba, 0, n, min_neighbors, d_rects, d_counts);
+    rc = run_detect(ctx, st, P, rgba, 0, n, min_neighbors, d_rects, d_counts);
     if (rc != HT_OK) return rc;
   } else {
     // host frames: the H2D of chunk c+1 (copy stream) overlaps the kernels of chunk c
     int chunk = 0, n_chunks = 0;
-    rc = upload_chunks(ctx, rgba, n, (size_t)w * h * 4, &chunk, &n_chunks);
+    rc = upload_chunks(ctx, st, rgba, n, (size_t)w * h * 4, &chunk, &n_chunks);
     if (rc != HT_OK) return rc;
     for (int c = 0; c < n_chunks; ++c) {
       const int f0 = c * chunk, nf = std::min(chunk, n - f0);
       CK(cudaStreamWaitEvent(st, ctx->chunk_events[c], 0));
-      rc = run_detect(ctx, P, ctx->d_frames.as<uint8_t>(), f0, nf, min_neighbors, d_rects, d_counts);
+      rc = run_detect(ctx, st, P, ctx->d_frames.as<uint8_t>(), f0, nf, min_neighbors, d_rects, d_counts);
       if (rc != HT_OK) return rc;
     }
   }
   ctx->last_plan = P;
   ctx->last_n = n;
-  if (!rects_dev) CK(cudaMemcpyAsync(out_rects, d_rects, sizeof(Rect) * (size_t)n * ctx->K, cudaMemcpyDeviceToHost, st));
-  if (!counts_dev) CK(cudaMemcpyAsync(out_counts, d_counts, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, st));
-  if (!rects_dev || !counts_dev) return ht_sync(ctx);
-  return HT_OK;
+  return io.finish(Outputs::SYNC_FLAGS);
 }
 
 int ht_track_init(ht_ctx *ctx, const int32_t *slots, int n, const uint8_t *rgba, int w, int h, const int32_t *rects,
@@ -1372,20 +1412,21 @@ int ht_track_init(ht_ctx *ctx, const int32_t *slots, int n, const uint8_t *rgba,
   if (rc != HT_OK) return rc;
   if (w <= 0 || h <= 0) return ctx->fail(HT_ERR_ARG, "bad frame size");
   CK(cudaSetDevice(ctx->cfg.device));
-  rc = ensure_tracker_buffers(ctx);
+  cudaStream_t st = ctx->stream;
+  rc = ensure_tracker_buffers(ctx, st);
   if (rc != HT_OK) return rc;
   const uint8_t *d_rgba = nullptr;
-  rc = device_frames(ctx, rgba, n, w, h, &d_rgba);
+  rc = stage_frames(ctx, st, rgba, n, w, h, &d_rgba);
   if (rc != HT_OK) return rc;
-  const int32_t *d_rects = rects;
-  if (!is_device_ptr(rects)) {
+  const bool rects_dev = is_device_ptr(rects);
+  if (!rects_dev)
     for (int i = 0; i < n; ++i)
       if (rects[4 * i + 2] <= 0 || rects[4 * i + 3] <= 0)
         return ctx->fail(HT_ERR_ARG, "initTracker rectangle %d is empty (canvas getImageData would throw)", i);
-    CK(cudaMemcpyAsync(ctx->d_rects.p, rects, sizeof(int32_t) * 4 * n, cudaMemcpyHostToDevice, ctx->stream));
-    d_rects = ctx->d_rects.as<int32_t>();
-  }
-  return track_init_common(ctx, slots, n, d_rgba, w, h, d_rects, calc_angles, nullptr);
+  const int32_t *d_rects = nullptr;
+  rc = stage_input(ctx, st, rects, rects_dev, sizeof(int32_t) * 4 * n, ctx->d_rects, &d_rects);
+  if (rc != HT_OK) return rc;
+  return track_init_common(ctx, st, slots, n, d_rgba, w, h, d_rects, calc_angles, nullptr);
 }
 
 int ht_track_init_from_detect(ht_ctx *ctx, const int32_t *slots, int n, const uint8_t *rgba, int w, int h,
@@ -1396,27 +1437,24 @@ int ht_track_init_from_detect(ht_ctx *ctx, const int32_t *slots, int n, const ui
   if (rc != HT_OK) return rc;
   if (w <= 0 || h <= 0) return ctx->fail(HT_ERR_ARG, "bad frame size");
   CK(cudaSetDevice(ctx->cfg.device));
-  rc = ensure_tracker_buffers(ctx);
+  cudaStream_t st = ctx->stream;
+  rc = ensure_tracker_buffers(ctx, st);
   if (rc != HT_OK) return rc;
   const uint8_t *d_rgba = nullptr;
-  rc = device_frames(ctx, rgba, n, w, h, &d_rgba);
+  rc = stage_frames(ctx, st, rgba, n, w, h, &d_rgba);
   if (rc != HT_OK) return rc;
-  const Rect *d_det = reinterpret_cast<const Rect *>(det_rects);
-  const int32_t *d_cnt = det_counts;
-  if (!is_device_ptr(det_rects)) {
-    CK(cudaMemcpyAsync(ctx->d_out_rects.p, det_rects, sizeof(Rect) * (size_t)n * ctx->K, cudaMemcpyHostToDevice, ctx->stream));
-    d_det = ctx->d_out_rects.as<Rect>();
-  }
-  if (!is_device_ptr(det_counts)) {
-    CK(cudaMemcpyAsync(ctx->d_out_counts.p, det_counts, sizeof(int32_t) * n, cudaMemcpyHostToDevice, ctx->stream));
-    d_cnt = ctx->d_out_counts.as<int32_t>();
-  }
-  ctx->prof_begin(HT_PROF_TRACK_INIT);
-  k_pick_face<<<(n + 127) / 128, 128, 0, ctx->stream>>>(d_det, d_cnt, ctx->K, n, ctx->d_rects.as<int32_t>());
-  ctx->prof_end();
+  const ht_rect *d_det = nullptr;
+  const int32_t *d_cnt = nullptr;
+  rc = stage_input(ctx, st, det_rects, is_device_ptr(det_rects), sizeof(Rect) * (size_t)n * ctx->K, ctx->d_out_rects, &d_det);
+  if (rc != HT_OK) return rc;
+  rc = stage_input(ctx, st, det_counts, is_device_ptr(det_counts), sizeof(int32_t) * n, ctx->d_out_counts, &d_cnt);
+  if (rc != HT_OK) return rc;
+  ctx->prof_begin(HT_PROF_TRACK_INIT, st);
+  k_pick_face<<<(n + 127) / 128, 128, 0, st>>>(reinterpret_cast<const Rect *>(d_det), d_cnt, ctx->K, n, ctx->d_rects.as<int32_t>());
+  ctx->prof_end(st);
   ++ctx->launches;
   CK(cudaGetLastError());
-  return track_init_common(ctx, slots, n, d_rgba, w, h, ctx->d_rects.as<int32_t>(), calc_angles, out_found);
+  return track_init_common(ctx, st, slots, n, d_rgba, w, h, ctx->d_rects.as<int32_t>(), calc_angles, out_found);
 }
 
 int ht_track(ht_ctx *ctx, const int32_t *slots, int n, const uint8_t *rgba, int w, int h, int n_calls,
@@ -1428,31 +1466,29 @@ int ht_track(ht_ctx *ctx, const int32_t *slots, int n, const uint8_t *rgba, int 
   if (rc != HT_OK) return rc;
   if (w <= 0 || h <= 0) return ctx->fail(HT_ERR_ARG, "bad frame size");
   CK(cudaSetDevice(ctx->cfg.device));
-  rc = ensure_tracker_buffers(ctx);
+  cudaStream_t st = ctx->stream;
+  rc = ensure_tracker_buffers(ctx, st);
   if (rc != HT_OK) return rc;
   const uint8_t *d_rgba = nullptr;
-  rc = device_frames(ctx, rgba, n, w, h, &d_rgba);
+  rc = stage_frames(ctx, st, rgba, n, w, h, &d_rgba);
   if (rc != HT_OK) return rc;
   const int32_t *d_slots = nullptr;
-  rc = upload_slots(ctx, slots, n, &d_slots);
+  rc = upload_slots(ctx, st, slots, n, &d_slots);
   if (rc != HT_OK) return rc;
   CK(ctx->bins.reserve((size_t)n * w * h * sizeof(uint16_t)));
-  rc = launch_hist(ctx, d_rgba, n, w, h, ctx->cur_hist.as<uint32_t>(), ctx->bins.as<uint16_t>());   // camshift.js:268
+  rc = launch_hist(ctx, st, d_rgba, n, w, h, ctx->cur_hist.as<uint32_t>(), ctx->bins.as<uint16_t>());   // camshift.js:268
   if (rc != HT_OK) return rc;
-  const bool objs_dev = is_device_ptr(out_objs), win_dev = out_windows && is_device_ptr(out_windows);
-  int32_t *d_objs = objs_dev ? reinterpret_cast<int32_t *>(out_objs) : ctx->d_objs.as<int32_t>();
-  int32_t *d_win = out_windows ? (win_dev ? reinterpret_cast<int32_t *>(out_windows) : ctx->d_windows.as<int32_t>()) : nullptr;
-  ctx->prof_begin(HT_PROF_TRACK);
-  rc = launch_track(ctx, n, 0, ctx->bins.as<uint16_t>(), w, h, d_slots, ctx->model_hist.as<uint32_t>(),
+  Outputs io(ctx);
+  int32_t *d_objs = io.out<int32_t>(out_objs, ctx->d_objs, sizeof(ht_trackobj) * n);
+  int32_t *d_win = io.out<int32_t>(out_windows, ctx->d_windows, sizeof(ht_window) * n);
+  ctx->prof_begin(HT_PROF_TRACK, st);
+  rc = launch_track(ctx, st, n, 0, ctx->bins.as<uint16_t>(), w, h, d_slots, ctx->model_hist.as<uint32_t>(),
                     ctx->cur_hist.as<uint32_t>(), ctx->track_state.as<TrackState>(), n_calls, d_objs, d_win,
                     ctx->d_flags.as<int32_t>() + 1);
   if (rc != HT_OK) return rc;
-  ctx->prof_end();
+  ctx->prof_end(st);
   CK(cudaGetLastError());
-  if (!objs_dev) CK(cudaMemcpyAsync(out_objs, d_objs, sizeof(ht_trackobj) * n, cudaMemcpyDeviceToHost, ctx->stream));
-  if (out_windows && !win_dev) CK(cudaMemcpyAsync(out_windows, d_win, sizeof(ht_window) * n, cudaMemcpyDeviceToHost, ctx->stream));
-  if (!objs_dev || (out_windows && !win_dev)) return ht_sync(ctx);
-  return HT_OK;
+  return io.finish(Outputs::SYNC_FLAGS);
 }
 
 int ht_detect_track(ht_ctx *ctx, const uint8_t *rgba, int n, int w, int h, int interval, int min_neighbors,
@@ -1461,22 +1497,29 @@ int ht_detect_track(ht_ctx *ctx, const uint8_t *rgba, int n, int w, int h, int i
   if (!ctx) return HT_ERR_ARG;
   if (!out_rects || !out_counts || !out_objs) return ctx->fail(HT_ERR_ARG, "output pointers are NULL");
   if (n_calls < 0) return ctx->fail(HT_ERR_ARG, "n_calls must be >= 0");
-  const bool rects_dev = is_device_ptr(out_rects), counts_dev = is_device_ptr(out_counts);
-  const bool found_dev = out_found && is_device_ptr(out_found), objs_dev = is_device_ptr(out_objs);
-  const bool win_dev = out_windows && is_device_ptr(out_windows);
+  Outputs io(ctx);
+  const int o_rects = io.add(out_rects, ctx->d_out_rects, sizeof(Rect) * (size_t)n * ctx->K);
+  const int o_counts = io.add(out_counts, ctx->d_out_counts, sizeof(int32_t) * n);
+  const int o_found = io.add(out_found, ctx->d_found, sizeof(int32_t) * n);
+  const int o_objs = io.add(out_objs, ctx->d_objs, sizeof(ht_trackobj) * n);
+  const int o_win = io.add(out_windows, ctx->d_windows, sizeof(ht_window) * n);
+  const bool frames_dev = is_device_ptr(rgba);
   // pipelined call (ht_set_pipeline): everything stays on the device, so nothing forces this call to wait for its own
   // tracking - it is left on the aux stream and runs under the next call's detection
-  const bool deferred = ctx->pipeline > 0 && n_calls > 0 && rgba && is_device_ptr(rgba) && rects_dev && counts_dev && objs_dev &&
-                        (!out_found || found_dev) && (!out_windows || win_dev);
+  const bool deferred = ctx->pipeline > 0 && n_calls > 0 && frames_dev && io.on_device();
   int rc = check_batch(ctx, n, !deferred);
   if (rc != HT_OK) return rc;
   CK(cudaSetDevice(ctx->cfg.device));
   Plan *P = nullptr;
   rc = get_plan(ctx, w, h, interval, &P);
   if (rc != HT_OK) return rc;
-  rc = ensure_tracker_buffers(ctx);
-  if (rc != HT_OK) return rc;
   cudaStream_t st = ctx->stream;
+  rc = ensure_tracker_buffers(ctx, st);
+  if (rc != HT_OK) return rc;
+  // (the scratch buffers of host outputs are reserved from here on)
+  Rect *d_rects = io.dst<Rect>(o_rects);
+  int32_t *d_counts = io.dst<int32_t>(o_counts), *d_found = io.dst<int32_t>(o_found);
+  int32_t *d_objs = io.dst<int32_t>(o_objs), *d_win = io.dst<int32_t>(o_win);
   if (deferred) {
     const size_t plane_elems = (size_t)ctx->cfg.max_frames * w * h;     // one parity's bin planes
     if (ctx->bins.cap < 2 * plane_elems * sizeof(uint16_t)) {
@@ -1484,32 +1527,20 @@ int ht_detect_track(ht_ctx *ctx, const uint8_t *rgba, int n, int w, int h, int i
       CK(cudaStreamSynchronize(st));
       CK(ctx->bins.reserve(2 * plane_elems * sizeof(uint16_t)));
     }
-    if (!ctx->aux_stream) {
-      int prio_least = 0, prio_greatest = 0, aux_prio = 0;
-      CK(cudaDeviceGetStreamPriorityRange(&prio_least, &prio_greatest));
-      aux_prio = prio_greatest;
-      if (ctx->pipe_bg) { int pm = 0; CK(cudaStreamGetPriority(st, &pm)); aux_prio = std::min(prio_least, pm + 1); }
-      CK(cudaStreamCreateWithPriority(&ctx->aux_stream, cudaStreamNonBlocking, aux_prio));
-      CK(cudaEventCreateWithFlags(&ctx->aux_done, cudaEventDisableTiming));
-      for (int i = 0; i < 4; ++i) CK(cudaEventCreateWithFlags(&ctx->part_events[i], cudaEventDisableTiming));
-    }
-    if (!ctx->pipe_detect_done) CK(cudaEventCreateWithFlags(&ctx->pipe_detect_done, cudaEventDisableTiming));
+    rc = ensure_aux_stream(ctx, true);
+    if (rc != HT_OK) return rc;
+    if (!ctx->pipe_detect_done) CK(cudaEventCreateWithFlags(&ctx->pipe_detect_done.h, cudaEventDisableTiming));
     ctx->pipe_parity ^= 1;
     ctx->bins_off = (size_t)ctx->pipe_parity * plane_elems;
     ctx->hist_off = (size_t)ctx->pipe_parity * (size_t)ctx->cfg.max_frames * 4096;
-    Rect *dr = reinterpret_cast<Rect *>(out_rects);
-    rc = run_detect(ctx, P, rgba, 0, n, min_neighbors, dr, out_counts,
+    rc = run_detect(ctx, st, P, rgba, 0, n, min_neighbors, d_rects, d_counts,
                     HistOut{ctx->cur_hist.as<uint32_t>() + ctx->hist_off, ctx->bins.as<uint16_t>() + ctx->bins_off}, nullptr,
-                    ctx->aux_pending ? ctx->aux_done : nullptr);
+                    ctx->aux_pending ? ctx->aux_done.h : nullptr);
     if (rc != HT_OK) return rc;
     CK(cudaEventRecord(ctx->pipe_detect_done, st));
     CK(cudaStreamWaitEvent(ctx->aux_stream, ctx->pipe_detect_done, 0));
-    ctx->main_stream = st;
-    ctx->stream = ctx->aux_stream;
-    rc = run_track_from_detect(ctx, rgba, w, h, 0, n, dr, out_counts, calc_angles, n_calls, out_found,
-                               reinterpret_cast<int32_t *>(out_objs), reinterpret_cast<int32_t *>(out_windows));
-    ctx->stream = st;
-    ctx->main_stream = nullptr;
+    rc = run_track_from_detect(ctx, ctx->aux_stream, rgba, w, h, 0, n, d_rects, d_counts, calc_angles, n_calls, d_found,
+                               d_objs, d_win);
     if (rc != HT_OK) return rc;
     CK(cudaEventRecord(ctx->aux_done, ctx->aux_stream));
     ctx->aux_pending = true;
@@ -1518,21 +1549,16 @@ int ht_detect_track(ht_ctx *ctx, const uint8_t *rgba, int n, int w, int h, int i
     return HT_OK;
   }
   if (n_calls > 0) CK(ctx->bins.reserve((size_t)n * w * h * sizeof(uint16_t)));
-  Rect *d_rects = rects_dev ? reinterpret_cast<Rect *>(out_rects) : ctx->d_out_rects.as<Rect>();
-  int32_t *d_counts = counts_dev ? out_counts : ctx->d_out_counts.as<int32_t>();
-  int32_t *d_found = out_found ? (found_dev ? out_found : ctx->d_found.as<int32_t>()) : nullptr;
-  int32_t *d_objs = objs_dev ? reinterpret_cast<int32_t *>(out_objs) : ctx->d_objs.as<int32_t>();
-  int32_t *d_win = out_windows ? (win_dev ? reinterpret_cast<int32_t *>(out_windows) : ctx->d_windows.as<int32_t>()) : nullptr;
   if (n_calls == 0) CK(cudaMemsetAsync(d_objs, 0, sizeof(ht_trackobj) * n, st));
-  if (!rgba) return ctx->fail(HT_ERR_ARG, "rgba is NULL");
-  if ((reinterpret_cast<uintptr_t>(rgba) & 3u) != 0) return ctx->fail(HT_ERR_ARG, "rgba must be 4-byte aligned");
+  rc = check_frames(ctx, rgba);
+  if (rc != HT_OK) return rc;
   const size_t frame_bytes = (size_t)w * h * 4;
   // Detect and track have complementary bottlenecks (k_cascade: shared-memory load wavefronts; k_track: a latency
   // chain of fp64 window passes), so the batch is cut into parts and the tracking of part p
   // runs on a second stream while part p+1 is being detected.
   // (Tracking host-frame parts on the main stream as their chunks arrive is slower than one k_track over the whole
   // batch: every k_track launch costs at least its slowest stream.)
-  const bool use_aux = n_calls > 0 && (ctx->overlap_track > 0 || (ctx->overlap_track < 0 && !is_device_ptr(rgba)));
+  const bool use_aux = n_calls > 0 && (ctx->overlap_track > 0 || (ctx->overlap_track < 0 && !frames_dev));
   int parts = use_aux ? ((n >= 512) ? 4 : (n >= 128 ? 2 : 1)) : 1;
   if (use_aux && ctx->overlap_parts > 1) parts = std::min(ctx->overlap_parts, std::max(1, n / 32));
   auto part_begin = [&](int p) { return (int)(((long long)n * p) / parts); };
@@ -1541,27 +1567,22 @@ int ht_detect_track(ht_ctx *ctx, const uint8_t *rgba, int n, int w, int h, int i
                                  ctx->bins.as<uint16_t>() + ctx->bins_off + (size_t)f0 * w * h}
                        : HistOut{nullptr, nullptr};
   };
-  if (use_aux && parts > 1 && !ctx->aux_stream) {
-    CK(cudaStreamCreateWithFlags(&ctx->aux_stream, cudaStreamNonBlocking));
-    CK(cudaEventCreateWithFlags(&ctx->aux_done, cudaEventDisableTiming));
-    for (int i = 0; i < 4; ++i) CK(cudaEventCreateWithFlags(&ctx->part_events[i], cudaEventDisableTiming));
+  if (use_aux && parts > 1) {
+    rc = ensure_aux_stream(ctx, false);
+    if (rc != HT_OK) return rc;
   }
   // run tracking for frames [f0, f0+nf) — on the aux stream when overlapping
   auto track_part = [&](const uint8_t *d_frames_batch, int f0, int nf) -> int {
-    if (parts == 1 || !use_aux) return run_track_from_detect(ctx, d_frames_batch, w, h, f0, nf, d_rects, d_counts, calc_angles, n_calls, d_found, d_objs, d_win);
+    if (parts == 1 || !use_aux) return run_track_from_detect(ctx, st, d_frames_batch, w, h, f0, nf, d_rects, d_counts, calc_angles, n_calls, d_found, d_objs, d_win);
     const int pi = ctx->part_seq++ & 3;
     CK(cudaEventRecord(ctx->part_events[pi], st));
     CK(cudaStreamWaitEvent(ctx->aux_stream, ctx->part_events[pi], 0));
-    cudaStream_t saved = ctx->stream;
-    ctx->stream = ctx->aux_stream;
-    const int r = run_track_from_detect(ctx, d_frames_batch, w, h, f0, nf, d_rects, d_counts, calc_angles, n_calls, d_found, d_objs, d_win);
-    ctx->stream = saved;
-    return r;
+    return run_track_from_detect(ctx, ctx->aux_stream, d_frames_batch, w, h, f0, nf, d_rects, d_counts, calc_angles, n_calls, d_found, d_objs, d_win);
   };
-  if (is_device_ptr(rgba)) {
+  if (frames_dev) {
     for (int p = 0; p < parts; ++p) {
       const int f0 = part_begin(p), nf = part_begin(p + 1) - f0;
-      rc = run_detect(ctx, P, rgba, f0, nf, min_neighbors, d_rects, d_counts, hist_out(f0));
+      rc = run_detect(ctx, st, P, rgba, f0, nf, min_neighbors, d_rects, d_counts, hist_out(f0));
       if (rc != HT_OK) return rc;
       rc = track_part(rgba, f0, nf);
       if (rc != HT_OK) return rc;
@@ -1569,7 +1590,7 @@ int ht_detect_track(ht_ctx *ctx, const uint8_t *rgba, int n, int w, int h, int i
   } else {
     // host frames: upload in chunks on a copy stream so the H2D of chunk c+1 overlaps the kernels of chunk c
     int chunk = 0, n_chunks = 0;
-    rc = upload_chunks(ctx, rgba, n, frame_bytes, &chunk, &n_chunks);
+    rc = upload_chunks(ctx, st, rgba, n, frame_bytes, &chunk, &n_chunks);
     if (rc != HT_OK) return rc;
     uint8_t *d_frames = ctx->d_frames.as<uint8_t>();
     // detect per uploaded chunk; tracking per PART (a k_track launch costs at least its slowest stream, so it is
@@ -1578,7 +1599,7 @@ int ht_detect_track(ht_ctx *ctx, const uint8_t *rgba, int n, int w, int h, int i
     for (int c = 0; c < n_chunks; ++c) {
       const int f0 = c * chunk, nf = std::min(chunk, n - f0);
       CK(cudaStreamWaitEvent(st, ctx->chunk_events[c], 0));
-      rc = run_detect(ctx, P, d_frames, f0, nf, min_neighbors, d_rects, d_counts, hist_out(f0));
+      rc = run_detect(ctx, st, P, d_frames, f0, nf, min_neighbors, d_rects, d_counts, hist_out(f0));
       if (rc != HT_OK) return rc;
       const int done_to = f0 + nf;
       while (next_part < parts && part_begin(next_part + 1) <= done_to) {
@@ -1596,14 +1617,7 @@ int ht_detect_track(ht_ctx *ctx, const uint8_t *rgba, int n, int w, int h, int i
   }
   ctx->last_plan = P;
   ctx->last_n = n;
-  bool any_host = false;
-  if (!rects_dev) { CK(cudaMemcpyAsync(out_rects, d_rects, sizeof(Rect) * (size_t)n * ctx->K, cudaMemcpyDeviceToHost, st)); any_host = true; }
-  if (!counts_dev) { CK(cudaMemcpyAsync(out_counts, d_counts, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, st)); any_host = true; }
-  if (out_found && !found_dev) { CK(cudaMemcpyAsync(out_found, d_found, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, st)); any_host = true; }
-  if (!objs_dev) { CK(cudaMemcpyAsync(out_objs, d_objs, sizeof(ht_trackobj) * n, cudaMemcpyDeviceToHost, st)); any_host = true; }
-  if (out_windows && !win_dev) { CK(cudaMemcpyAsync(out_windows, d_win, sizeof(ht_window) * n, cudaMemcpyDeviceToHost, st)); any_host = true; }
-  if (any_host) return ht_sync(ctx);
-  return HT_OK;
+  return io.finish(Outputs::SYNC_FLAGS);
 }
 
 static_assert(sizeof(ht_stream_event) == sizeof(StreamEvent) && sizeof(ht_stream_event) == 56, "ht_stream_event layout");
@@ -1646,11 +1660,11 @@ int ht_stream_head_config(ht_ctx *ctx, const ht_head_params *params) {
 }
 
 
-static int ensure_stream_buffers(ht_ctx *ctx) {
+static int ensure_stream_buffers(ht_ctx *ctx, cudaStream_t st) {
   const size_t mf = (size_t)ctx->cfg.max_frames;
   if (!ctx->d_stream_mode.p) {
     CK(ctx->d_stream_mode.reserve(mf * sizeof(int32_t)));
-    CK(cudaMemsetAsync(ctx->d_stream_mode.p, 0, mf * sizeof(int32_t), ctx->stream));   // every stream starts in "VJ"
+    CK(cudaMemsetAsync(ctx->d_stream_mode.p, 0, mf * sizeof(int32_t), st));   // every stream starts in "VJ"
     CK(ctx->d_stream_mask.reserve((mf + 3) / 4 + 16));
     CK(ctx->d_stream_cs.reserve(mf));
     CK(ctx->d_stream_init.reserve(mf));
@@ -1664,7 +1678,7 @@ int ht_stream_reset(ht_ctx *ctx, int first, int n) {
   { const int jr = join_aux(ctx); if (jr != HT_OK) return jr; }
   if (first < 0 || n <= 0 || first + n > ctx->cfg.max_frames) return ctx->fail(HT_ERR_ARG, "stream range outside [0,%d)", ctx->cfg.max_frames);
   CK(cudaSetDevice(ctx->cfg.device));
-  int rc = ensure_stream_buffers(ctx);
+  int rc = ensure_stream_buffers(ctx, ctx->stream);
   if (rc != HT_OK) return rc;
   CK(cudaMemsetAsync(ctx->d_stream_mode.as<int32_t>() + first, 0, (size_t)n * sizeof(int32_t), ctx->stream));
   if (ctx->d_head_state.p)   // a new headtrackr.Tracker: smoother, head diagonals, fov estimate start over too
@@ -1695,53 +1709,51 @@ int ht_stream_step_head(ht_ctx *ctx, const uint8_t *rgba, int n, int w, int h, i
   Plan *P = nullptr;
   rc = get_plan(ctx, w, h, interval, &P);
   if (rc != HT_OK) return rc;
-  rc = ensure_tracker_buffers(ctx);
+  cudaStream_t st = ctx->stream;
+  rc = ensure_tracker_buffers(ctx, st);
   if (rc != HT_OK) return rc;
-  rc = ensure_stream_buffers(ctx);
+  rc = ensure_stream_buffers(ctx, st);
   if (rc != HT_OK) return rc;
   const uint8_t *d_rgba = nullptr;
-  rc = device_frames(ctx, rgba, n, w, h, &d_rgba);
+  rc = stage_frames(ctx, st, rgba, n, w, h, &d_rgba);
   if (rc != HT_OK) return rc;
   CK(ctx->bins.reserve((size_t)n * w * h * sizeof(uint16_t)));
-  cudaStream_t st = ctx->stream;
   int32_t *mode = ctx->d_stream_mode.as<int32_t>();
   uint8_t *vj_mask = ctx->d_stream_mask.as<uint8_t>(), *cs_en = ctx->d_stream_cs.as<uint8_t>(), *init_en = ctx->d_stream_init.as<uint8_t>();
   k_stream_plan<<<(n + 127) / 128, 128, 0, st>>>(mode, n, vj_mask, cs_en, init_en);
   ++ctx->launches;
   // detection for the streams in "VJ" (frame quads without such a stream exit at once)
-  rc = run_detect(ctx, P, d_rgba, 0, n, min_neighbors, ctx->d_out_rects.as<Rect>(), ctx->d_out_counts.as<int32_t>(),
+  rc = run_detect(ctx, st, P, d_rgba, 0, n, min_neighbors, ctx->d_out_rects.as<Rect>(), ctx->d_out_counts.as<int32_t>(),
                   HistOut{nullptr, nullptr}, vj_mask);
   if (rc != HT_OK) return rc;
   // one track() for the streams in "CS" (src/camshift.js:213-312; the whole-frame histogram is :268)
-  rc = launch_hist(ctx, d_rgba, n, w, h, ctx->cur_hist.as<uint32_t>(), ctx->bins.as<uint16_t>(), cs_en);
+  rc = launch_hist(ctx, st, d_rgba, n, w, h, ctx->cur_hist.as<uint32_t>(), ctx->bins.as<uint16_t>(), cs_en);
   if (rc != HT_OK) return rc;
-  ctx->prof_begin(HT_PROF_TRACK);
-  rc = launch_track(ctx, n, 0, ctx->bins.as<uint16_t>(), w, h, nullptr, ctx->model_hist.as<uint32_t>(),
+  ctx->prof_begin(HT_PROF_TRACK, st);
+  rc = launch_track(ctx, st, n, 0, ctx->bins.as<uint16_t>(), w, h, nullptr, ctx->model_hist.as<uint32_t>(),
                     ctx->cur_hist.as<uint32_t>(), ctx->track_state.as<TrackState>(), 1, ctx->d_objs.as<int32_t>(), nullptr,
                     ctx->d_flags.as<int32_t>() + 2, cs_en);
   if (rc != HT_OK) return rc;
-  ctx->prof_end();
-  // events + transitions, then initTracker for the streams that just found their face
-  StreamEvent *d_ev = is_device_ptr(out_events) ? reinterpret_cast<StreamEvent *>(out_events) : ctx->d_stream_events.as<StreamEvent>();
-  HeadEvent *d_he = nullptr;
-  if (ctx->head_on) d_he = (out_head && is_device_ptr(out_head)) ? reinterpret_cast<HeadEvent *>(out_head) : ctx->d_head_events.as<HeadEvent>();
+  ctx->prof_end(st);
+  // events + transitions, then initTracker for the streams that just found their face.  (out_head implies head_on;
+  // with the epilogue on and no out_head its records go to the scratch buffer.)
+  Outputs io(ctx);
+  StreamEvent *d_ev = io.out<StreamEvent>(out_events, ctx->d_stream_events, sizeof(StreamEvent) * (size_t)n);
+  HeadEvent *d_he = out_head ? io.out<HeadEvent>(out_head, ctx->d_head_events, sizeof(HeadEvent) * (size_t)n)
+                             : ctx->head_on ? ctx->d_head_events.as<HeadEvent>() : nullptr;
   k_stream_update<<<(n + 127) / 128, 128, 0, st>>>(mode, n, ctx->d_out_rects.as<Rect>(), ctx->d_out_counts.as<int32_t>(), ctx->K,
                                                    ctx->d_objs.as<int32_t>(), ctx->d_rects.as<int32_t>(), init_en, d_ev,
                                                    ctx->head_on ? ctx->d_head_state.as<HeadState>() : nullptr,
                                                    ctx->d_head_params.as<HeadParams>(), d_he, w, h);
-  ctx->prof_begin(HT_PROF_TRACK_INIT);
+  ctx->prof_begin(HT_PROF_TRACK_INIT, st);
   k_track_init<<<n, 256, 0, st>>>(d_rgba, (size_t)w * h * 4, w, h, nullptr, ctx->d_rects.as<int32_t>(), calc_angles ? 1 : 0,
                                   ctx->model_hist.as<uint32_t>(), ctx->track_state.as<TrackState>(), nullptr, init_en);
-  ctx->prof_end();
+  ctx->prof_end(st);
   ctx->launches += 2;
   CK(cudaGetLastError());
   ctx->last_plan = P;
   ctx->last_n = n;
-  bool any_host = false;
-  if (!is_device_ptr(out_events)) { CK(cudaMemcpyAsync(out_events, d_ev, sizeof(StreamEvent) * (size_t)n, cudaMemcpyDeviceToHost, st)); any_host = true; }
-  if (out_head && !is_device_ptr(out_head)) { CK(cudaMemcpyAsync(out_head, d_he, sizeof(HeadEvent) * (size_t)n, cudaMemcpyDeviceToHost, st)); any_host = true; }
-  if (any_host) return ht_sync(ctx);
-  return HT_OK;
+  return io.finish(Outputs::SYNC_FLAGS);
 }
 
 static_assert(sizeof(ht_tracker_event) == sizeof(TrackerEvent) && sizeof(ht_tracker_event) == 144, "ht_tracker_event layout");
@@ -1828,13 +1840,13 @@ struct FeedDraw {
 //   k_track_init     initTracker for the streams that found their face           src/facetrackr.js:97-108
 static int tracker_tick(ht_ctx *ctx, Plan *P, const uint8_t *d_rgba, int n, int w, int h, const int32_t *d_ids,
                         double now_ms, const double *d_now, const FeedDraw *feed, ht_tracker_event *out) {
-  int rc = ensure_tracker_buffers(ctx);
+  cudaStream_t st = ctx->stream;
+  int rc = ensure_tracker_buffers(ctx, st);
   if (rc != HT_OK) return rc;
-  rc = ensure_stream_buffers(ctx);           // the mask scratch of ht_stream_step (the two never run on one context at once)
+  rc = ensure_stream_buffers(ctx, st);       // the mask scratch of ht_stream_step (the two never run on one context at once)
   if (rc != HT_OK) return rc;
   CK(ctx->bins.reserve((size_t)n * w * h * sizeof(uint16_t)));
   CK(ctx->d_wb_sums.reserve((size_t)ctx->cfg.max_frames * 3 * sizeof(unsigned long long)));
-  cudaStream_t st = ctx->stream;
   TrackerState *ts = ctx->d_tracker_state.as<TrackerState>();
   uint8_t *vj_mask = ctx->d_stream_mask.as<uint8_t>(), *cs_en = ctx->d_stream_cs.as<uint8_t>(), *init_en = ctx->d_stream_init.as<uint8_t>();
   uint8_t *wb_en = ctx->d_tracker_wb.as<uint8_t>();
@@ -1849,36 +1861,32 @@ static int tracker_tick(ht_ctx *ctx, Plan *P, const uint8_t *d_rgba, int n, int 
   const int chunks = std::min(64, std::max(1, 8 * ctx->sms / n));
   k_wb_sums<<<dim3(chunks, n), 256, 0, st>>>(d_rgba, (size_t)w * h * 4, w * h, ctx->d_wb_sums.as<unsigned long long>(), chunks, wb_en);
   ctx->launches += 2;
-  rc = run_detect(ctx, P, d_rgba, 0, n, 1, ctx->d_out_rects.as<Rect>(), ctx->d_out_counts.as<int32_t>(),
+  rc = run_detect(ctx, st, P, d_rgba, 0, n, 1, ctx->d_out_rects.as<Rect>(), ctx->d_out_counts.as<int32_t>(),
                   HistOut{nullptr, nullptr}, vj_mask);
   if (rc != HT_OK) return rc;
-  rc = launch_hist(ctx, d_rgba, n, w, h, ctx->cur_hist.as<uint32_t>(), ctx->bins.as<uint16_t>(), cs_en);
+  rc = launch_hist(ctx, st, d_rgba, n, w, h, ctx->cur_hist.as<uint32_t>(), ctx->bins.as<uint16_t>(), cs_en);
   if (rc != HT_OK) return rc;
-  ctx->prof_begin(HT_PROF_TRACK);
-  rc = launch_track(ctx, n, 0, ctx->bins.as<uint16_t>(), w, h, d_ids, ctx->model_hist.as<uint32_t>(),
+  ctx->prof_begin(HT_PROF_TRACK, st);
+  rc = launch_track(ctx, st, n, 0, ctx->bins.as<uint16_t>(), w, h, d_ids, ctx->model_hist.as<uint32_t>(),
                     ctx->cur_hist.as<uint32_t>(), ctx->track_state.as<TrackState>(), 1, ctx->d_objs.as<int32_t>(), nullptr,
                     ctx->d_flags.as<int32_t>() + 2, cs_en);
   if (rc != HT_OK) return rc;
-  ctx->prof_end();
-  const bool out_dev = is_device_ptr(out);
-  TrackerEvent *d_ev = out_dev ? reinterpret_cast<TrackerEvent *>(out) : ctx->d_tracker_events.as<TrackerEvent>();
+  ctx->prof_end(st);
+  Outputs io(ctx);
+  TrackerEvent *d_ev = io.out<TrackerEvent>(out, ctx->d_tracker_events, sizeof(TrackerEvent) * (size_t)n);
   k_tracker_update<<<(n + 127) / 128, 128, 0, st>>>(ts, d_ids, ctx->d_tracker_params.as<TrackerParams>(), n,
                                                     ctx->d_wb_sums.as<unsigned long long>(), w * h, ctx->d_out_rects.as<Rect>(),
                                                     ctx->d_out_counts.as<int32_t>(), ctx->K, ctx->d_objs.as<int32_t>(),
                                                     ctx->d_rects.as<int32_t>(), init_en, now_ms, d_now, w, h, d_ev);
-  ctx->prof_begin(HT_PROF_TRACK_INIT);
+  ctx->prof_begin(HT_PROF_TRACK_INIT, st);
   k_track_init<<<n, 256, 0, st>>>(d_rgba, (size_t)w * h * 4, w, h, d_ids, ctx->d_rects.as<int32_t>(), ctx->tracker_calc_angles,
                                   ctx->model_hist.as<uint32_t>(), ctx->track_state.as<TrackState>(), nullptr, init_en);
-  ctx->prof_end();
+  ctx->prof_end(st);
   ctx->launches += 2;
   CK(cudaGetLastError());
   ctx->last_plan = P;
   ctx->last_n = n;
-  if (!out_dev) {
-    CK(cudaMemcpyAsync(out, d_ev, sizeof(TrackerEvent) * (size_t)n, cudaMemcpyDeviceToHost, st));
-    return ht_sync(ctx);
-  }
-  return HT_OK;
+  return io.finish(Outputs::SYNC_FLAGS);
 }
 
 int ht_tracker_step(ht_ctx *ctx, const uint8_t *rgba, int n, int w, int h, double now_ms, ht_tracker_event *out) {
@@ -1892,7 +1900,7 @@ int ht_tracker_step(ht_ctx *ctx, const uint8_t *rgba, int n, int w, int h, doubl
   rc = get_plan(ctx, w, h, 5, &P);
   if (rc != HT_OK) return rc;
   const uint8_t *d_rgba = nullptr;
-  rc = device_frames(ctx, rgba, n, w, h, &d_rgba);
+  rc = stage_frames(ctx, ctx->stream, rgba, n, w, h, &d_rgba);
   if (rc != HT_OK) return rc;
   return tracker_tick(ctx, P, d_rgba, n, w, h, nullptr, now_ms, nullptr, nullptr, out);
 }
@@ -1945,14 +1953,14 @@ int ht_tracker_feed(ht_ctx *ctx, const ht_video_frame *frames, int n, int frames
   const size_t off_now = align_up<size_t>(4 * (size_t)mf, 16), off_rec = off_now + 8 * (size_t)mf;
   const size_t table_cap = off_rec + sizeof(FeedRec) * (size_t)mf;
   if (!ctx->h_feed_table) {
-    CK(cudaMallocHost(&ctx->h_feed_table, table_cap));
-    CK(cudaEventCreateWithFlags(&ctx->feed_copied, cudaEventDisableTiming));
+    CK(cudaMallocHost(&ctx->h_feed_table.h, table_cap));
+    CK(cudaEventCreateWithFlags(&ctx->feed_copied.h, cudaEventDisableTiming));
     CK(ctx->d_feed_table.reserve(table_cap));
     CK(ctx->d_feed_draw.reserve((size_t)mf));
   } else {
     CK(cudaEventSynchronize(ctx->feed_copied));           // the previous call's upload may still read the table
   }
-  uint8_t *tab = static_cast<uint8_t *>(ctx->h_feed_table);
+  uint8_t *tab = static_cast<uint8_t *>(ctx->h_feed_table.h);
   int32_t *ids = reinterpret_cast<int32_t *>(tab);
   double *now = reinterpret_cast<double *>(tab + off_now);
   FeedRec *recs = reinterpret_cast<FeedRec *>(tab + off_rec);
@@ -1995,27 +2003,22 @@ int ht_ingest(ht_ctx *ctx, const uint8_t *src_rgba, int n, int sw, int sh, uint8
   g.half = (uint32_t)(2ull * dw * dh);
   CK(cudaSetDevice(ctx->cfg.device));
   const size_t sbytes = (size_t)n * sw * sh * 4, dbytes = (size_t)n * dw * dh * 4;
-  const uint8_t *d_src = src_rgba;
-  if (!is_device_ptr(src_rgba)) {
-    CK(ctx->d_frames.reserve(sbytes));
-    CK(cudaMemcpyAsync(ctx->d_frames.p, src_rgba, sbytes, cudaMemcpyHostToDevice, ctx->stream));
-    d_src = ctx->d_frames.as<uint8_t>();
-  }
-  const bool out_dev = is_device_ptr(dst_rgba);
-  uint8_t *d_dst = dst_rgba;
-  if (!out_dev) { CK(ctx->d_scratch.reserve(dbytes)); d_dst = ctx->d_scratch.as<uint8_t>(); }
+  cudaStream_t st = ctx->stream;
+  const uint8_t *d_src = nullptr;
+  int rc = stage_input(ctx, st, src_rgba, is_device_ptr(src_rgba), sbytes, ctx->d_frames, &d_src);
+  if (rc != HT_OK) return rc;
+  Outputs io(ctx);
+  const int o_dst = io.add(dst_rgba, ctx->d_scratch, dbytes);
+  if (!io.on_device()) CK(ctx->d_scratch.reserve(dbytes));   // a device destination is written in place: no scratch
+  uint8_t *d_dst = io.dst<uint8_t>(o_dst);
   if (sw == dw && sh == dh) {   // a 1:1 draw is a copy (oracle/ht_oracle.h)
-    CK(cudaMemcpyAsync(d_dst, d_src, dbytes, cudaMemcpyDeviceToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(d_dst, d_src, dbytes, cudaMemcpyDeviceToDevice, st));
   } else {
-    k_ingest<<<dim3((unsigned)(dw + 63) / 64, (unsigned)(dh + 3) / 4, (unsigned)n), 256, 0, ctx->stream>>>(d_src, d_dst, g);
+    k_ingest<<<dim3((unsigned)(dw + 63) / 64, (unsigned)(dh + 3) / 4, (unsigned)n), 256, 0, st>>>(d_src, d_dst, g);
     ++ctx->launches;
     CK(cudaGetLastError());
   }
-  if (!out_dev) {
-    CK(cudaMemcpyAsync(dst_rgba, d_dst, dbytes, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-  }
-  return HT_OK;
+  return io.finish(Outputs::SYNC_STREAM);
 }
 
 int ht_backprojection(ht_ctx *ctx, int slot, const uint8_t *rgba, int w, int h, uint8_t *out_rgba) {
@@ -2023,27 +2026,24 @@ int ht_backprojection(ht_ctx *ctx, int slot, const uint8_t *rgba, int w, int h, 
   { const int jr = join_aux(ctx); if (jr != HT_OK) return jr; }
   if (!out_rgba || slot < 0 || slot >= ctx->cfg.max_frames || w <= 0 || h <= 0) return ctx->fail(HT_ERR_ARG, "bad argument");
   CK(cudaSetDevice(ctx->cfg.device));
-  int rc = ensure_tracker_buffers(ctx);
+  cudaStream_t st = ctx->stream;
+  int rc = ensure_tracker_buffers(ctx, st);
   if (rc != HT_OK) return rc;
   const uint8_t *d_rgba = nullptr;
-  rc = device_frames(ctx, rgba, 1, w, h, &d_rgba);
+  rc = stage_frames(ctx, st, rgba, 1, w, h, &d_rgba);
   if (rc != HT_OK) return rc;
   const size_t bytes = (size_t)w * h * 4;
   CK(ctx->d_scratch.reserve(bytes + 4096 * sizeof(uint32_t)));
   uint32_t *hist = reinterpret_cast<uint32_t *>(ctx->d_scratch.as<uint8_t>() + bytes);
-  rc = launch_hist(ctx, d_rgba, 1, w, h, hist, nullptr);
+  rc = launch_hist(ctx, st, d_rgba, 1, w, h, hist, nullptr);
   if (rc != HT_OK) return rc;
-  const bool out_dev = is_device_ptr(out_rgba);
-  uint8_t *d_out = out_dev ? out_rgba : ctx->d_scratch.as<uint8_t>();
-  k_backproj<<<(w * h + 255) / 256, 256, 0, ctx->stream>>>(d_rgba, w * h, ctx->model_hist.as<uint32_t>() + (size_t)slot * 4096,
-                                                          hist, d_out);
+  Outputs io(ctx);
+  uint8_t *d_out = io.out<uint8_t>(out_rgba, ctx->d_scratch, bytes);
+  k_backproj<<<(w * h + 255) / 256, 256, 0, st>>>(d_rgba, w * h, ctx->model_hist.as<uint32_t>() + (size_t)slot * 4096, hist,
+                                                  d_out);
   ++ctx->launches;
   CK(cudaGetLastError());
-  if (!out_dev) {
-    CK(cudaMemcpyAsync(out_rgba, d_out, bytes, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-  }
-  return HT_OK;
+  return io.finish(Outputs::SYNC_STREAM);
 }
 
 int ht_whitebalance(ht_ctx *ctx, const uint8_t *rgba, int n, int w, int h, double *out) {
@@ -2052,25 +2052,22 @@ int ht_whitebalance(ht_ctx *ctx, const uint8_t *rgba, int n, int w, int h, doubl
   int rc = check_batch(ctx, n);
   if (rc != HT_OK) return rc;
   CK(cudaSetDevice(ctx->cfg.device));
+  cudaStream_t st = ctx->stream;
   const uint8_t *d_rgba = nullptr;
-  rc = device_frames(ctx, rgba, n, w, h, &d_rgba);
+  rc = stage_frames(ctx, st, rgba, n, w, h, &d_rgba);
   if (rc != HT_OK) return rc;
   const size_t mf = (size_t)ctx->cfg.max_frames;
   CK(ctx->d_wb_sums.reserve(mf * 3 * sizeof(unsigned long long)));
   CK(ctx->d_wb_out.reserve(mf * sizeof(double)));
-  CK(cudaMemsetAsync(ctx->d_wb_sums.p, 0, (size_t)n * 3 * sizeof(unsigned long long), ctx->stream));
+  CK(cudaMemsetAsync(ctx->d_wb_sums.p, 0, (size_t)n * 3 * sizeof(unsigned long long), st));
   const int chunks = std::min(64, std::max(1, 8 * ctx->sms / n));
-  k_wb_sums<<<dim3(chunks, n), 256, 0, ctx->stream>>>(d_rgba, (size_t)w * h * 4, w * h, ctx->d_wb_sums.as<unsigned long long>(), chunks);
-  const bool out_dev = is_device_ptr(out);
-  double *d_out = out_dev ? out : ctx->d_wb_out.as<double>();
-  k_wb_final<<<(n + 127) / 128, 128, 0, ctx->stream>>>(ctx->d_wb_sums.as<unsigned long long>(), n, w * h, d_out);
+  k_wb_sums<<<dim3(chunks, n), 256, 0, st>>>(d_rgba, (size_t)w * h * 4, w * h, ctx->d_wb_sums.as<unsigned long long>(), chunks);
+  Outputs io(ctx);
+  double *d_out = io.out<double>(out, ctx->d_wb_out, sizeof(double) * n);
+  k_wb_final<<<(n + 127) / 128, 128, 0, st>>>(ctx->d_wb_sums.as<unsigned long long>(), n, w * h, d_out);
   ctx->launches += 2;
   CK(cudaGetLastError());
-  if (!out_dev) {
-    CK(cudaMemcpyAsync(out, d_out, sizeof(double) * n, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-  }
-  return HT_OK;
+  return io.finish(Outputs::SYNC_STREAM);
 }
 
 int ht_profile(ht_ctx *ctx, int enable) {
@@ -2090,8 +2087,8 @@ int ht_profile_read(ht_ctx *ctx, double *ms, uint64_t *launches, int reset) {
       ctx->prof_ms[sp.cls] += t;
       ctx->prof_launches[sp.cls] += 1;
     } else cudaGetLastError();
-    ctx->prof_free.push_back(sp.a);
-    ctx->prof_free.push_back(sp.b);
+    ctx->prof_free.push_back(std::move(sp.a));
+    ctx->prof_free.push_back(std::move(sp.b));
   }
   ctx->prof_spans.clear();
   for (int i = 0; i < HT_PROF_N; ++i) {
@@ -2218,8 +2215,6 @@ int ht_debug_track_phases(ht_ctx *ctx, uint64_t *out, int n) {
 
 int ht_debug_model_hist(ht_ctx *ctx, int slot, uint32_t *out4096) {
   if (!ctx) return HT_ERR_ARG;
-  { const int jr = join_aux(ctx); if (jr != HT_OK) return jr; }
-  { const int jr = join_aux(ctx); if (jr != HT_OK) return jr; }
   { const int jr = join_aux(ctx); if (jr != HT_OK) return jr; }
   if (!out4096 || slot < 0 || slot >= ctx->cfg.max_frames || !ctx->model_hist.p) return ctx->fail(HT_ERR_ARG, "bad slot");
   CK(cudaSetDevice(ctx->cfg.device));
