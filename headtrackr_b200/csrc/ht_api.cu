@@ -2265,6 +2265,23 @@ extern "C" int ht_selftest_head(const ht_head_params *params, int n, const doubl
   return 0;
 }
 
+// k_track's truncation radius (trunc_tolerance) for moments m[6] = {m00, m10, m01, m11, m20, m02} of a window with at
+// most n_px non-zero pixels -> out[5] = {vx, vy, l1, l2, b}
+extern "C" int ht_selftest_track_tolerance(const double *m, double n_px, double sw, double sh, int calc_angles, double *out) {
+  const Mom mm = {m[0], m[1], m[2], m[3], m[4], m[5]};
+  const TruncTol t = trunc_tolerance(mm, n_px, sw, sh, calc_angles != 0);
+  out[0] = t.vx; out[1] = t.vy; out[2] = t.l1; out[3] = t.l2; out[4] = t.b;
+  return 0;
+}
+// the caps k_track screens with (trunc_cap) on a w x h frame, for a call with search window sw x sh and shape values
+// l1, l2 -> out[5] in the same layout
+extern "C" int ht_selftest_track_cap(int w, int h, double sw, double sh, double l1, double l2, double *out) {
+  const TruncCap c = trunc_cap(w, h);
+  out[0] = out[1] = shift_tolerance(c.eps, c.M, 0.5 * fmax(sw, sh));
+  out[2] = c.root + 4.0 * TRUNC_U * l1; out[3] = c.root + 4.0 * TRUNC_U * l2; out[4] = c.b;
+  return 0;
+}
+
 // the lifecycle state machine of k_tracker_update / k_tracker_control (tracker_step, tracker_start, ...) for one stream,
 // one call at a time, fed by the caller with the pixel results the stream's mode asks for.  op: 0 = new state,
 // 1 = start(), 2 = stop(), 3 = one frame (wb, det[0, count), obj as tracker_step takes them; out = its record;

@@ -203,9 +203,76 @@ __device__ __forceinline__ int32_t js_to_int32(double v) {  // ES ToInt32 for |v
   return (int32_t)v;  // cvt.rzi: truncation toward zero
 }
 
-// true when truncating v could flip under the (tiny) summation-order error of a parallel reduction
-__device__ __forceinline__ bool trunc_ambiguous(double v) {
-  return isfinite(v) && fabs(v - rint(v)) < 1e-7;
+// true when truncating v could flip under the summation-order error of a parallel reduction: v lies within tol of an
+// integer (trunc_tolerance gives tol)
+__host__ __device__ __forceinline__ bool trunc_ambiguous(double v, double tol) {
+  return isfinite(v) && fabs(v - rint(v)) < tol;
+}
+
+// How far apart k_track's parallel-order values and the reference's serial-order values of one window can lie, for
+// each decision a pass makes (DESIGN.md §4 item 2).  Every term of every moment is >= 0, so ANY order of summing the
+// window's n non-zero pixels - the serial one, or the kernel's per-thread chains, trees and FMAs (adding a zero term
+// is exact) - is within gamma(n) * m of the exact sum (a term meets at most n roundings on its way; +64 covers the
+// fixed trees and the products).  That relative error eps is carried through the reference's formulas with the
+// magnitudes of THIS window: the mass centre X (from the window's origin), the raw second moments X2 = m20 / m00, Y2,
+// and m10 * xc <= m20, |m11|, m01 * xc <= sqrt(m20 m02) (Cauchy-Schwarz).  a = (m20 - m10 xc) / m00 is a difference of
+// two numbers of size X2, so its error scales with X2, not with a.  Each bound E is for one evaluation against exact;
+// two evaluations differ by up to 2E.
+constexpr double TRUNC_U = 1.1102230246251565e-16;                 // 2^-53
+__host__ __device__ __forceinline__ double sum_eps(double n_px) {   // n_px: an upper bound of n
+  const double nu = (n_px + 64.0) * TRUNC_U;
+  return nu * (1.0 + 2.0 * nu) + TRUNC_U;                           // >= gamma(n + 64) (nu <= 1/2), plus one rounding
+}
+// the shift xc - half (half = sw / 2): xc = m10 * (1 / m00) has two moments and two roundings, then one rounding of
+// the subtraction.  Cheap: k_track evaluates it for every shift within the frame's cap (trunc_cap) of an integer.
+__host__ __device__ __forceinline__ double shift_tolerance(double eps, double xc, double half) {
+  return 2.0 * (4.0 * eps * fabs(xc) + 2.0 * TRUNC_U * (fabs(xc) + half));
+}
+//   vx, vy : xc - sw/2, yc - sh/2        l1, l2 : the square roots that are truncated (<< 2)
+//   b      : mu11 / m00, whose sign picks the angle's branch
+struct TruncTol { double vx, vy, l1, l2, b; };
+__host__ __device__ inline TruncTol trunc_tolerance(const Mom &m, double n_px, double sw, double sh, bool calc_angles) {
+  const double u = TRUNC_U;
+  const double eps = sum_eps(n_px);
+  const double inv = 1.0 / m.m00;
+  const double X = m.m10 * inv, Y = m.m01 * inv, X2 = m.m20 * inv, Y2 = m.m02 * inv;
+  TruncTol t;
+  t.vx = shift_tolerance(eps, X, 0.5 * sw);
+  t.vy = shift_tolerance(eps, Y, 0.5 * sh);
+  // a, c, b: the moments (eps each) and about six roundings, all on the scale of X2, Y2 and sqrt(X2 Y2)
+  const double ea = 8.0 * eps * X2, ec = 8.0 * eps * Y2, eb = 8.0 * eps * sqrt(X2 * Y2);
+  const double a = (m.m20 - m.m10 * X) * inv, c = (m.m02 - m.m01 * Y) * inv;
+  double lam1, lam2, e1, e2;                                  // the two radicands and their error bounds
+  if (calc_angles) {
+    // lambda = (a + c -+ e) / 2 with e = |(2b, a - c)| (1-Lipschitz): errors ea + ec + eb, plus the roundings of d
+    // and e (e <= a + c <= X2 + Y2)
+    const double b = (m.m11 - m.m01 * X) * inv;
+    const double e = sqrt(4 * b * b + (a - c) * (a - c));
+    lam1 = (a + c - e) * 0.5; lam2 = (a + c + e) * 0.5;
+    e1 = e2 = ea + ec + eb + 4.0 * u * (X2 + Y2);
+  } else {
+    lam1 = a; lam2 = c;
+    e1 = ea; e2 = ec;
+  }
+  // sqrt: two radicands 2E apart give square roots min(sqrt(2E), 2E / l) apart - the first form near l = 0; plus the
+  // rounding of each sqrt
+  const double l1 = sqrt(fmax(lam1, 0.0)), l2 = sqrt(fmax(lam2, 0.0));
+  t.l1 = fmin(sqrt(2.0 * e1), 2.0 * e1 / l1) + 4.0 * u * l1;
+  t.l2 = fmin(sqrt(2.0 * e2), 2.0 * e2 / l2) + 4.0 * u * l2;
+  t.b = 2.0 * eb;
+  return t;
+}
+// Upper bounds of those radii over every window of a W x H frame (n <= W H; xc, yc <= M = max(W, H); X2, Y2 <= M^2):
+// one comparison screens out the values far from an integer, only the rest need the window's own radius.
+//   shift: shift_tolerance(eps, M, max(sw, sh) / 2)    l1, l2: root + 4u l    b: b
+struct TruncCap { double eps, M, root, b; };
+__host__ __device__ inline TruncCap trunc_cap(int W, int H) {
+  TruncCap c;
+  c.eps = sum_eps((double)W * (double)H);
+  c.M = (double)(W > H ? W : H);
+  c.root = sqrt(2.0 * (24.0 * c.eps + 8.0 * TRUNC_U) * c.M * c.M);
+  c.b = 16.0 * c.eps * c.M * c.M;
+  return c;
 }
 
 // Moments in the reference's exact order (x outer, y inner, one accumulator each) —
@@ -389,7 +456,8 @@ k_track(const uint16_t *__restrict__ bins, int W, int H, const int32_t *__restri
   const bool stepper = (tid == 0);                 // thread 0 of EVERY CTA runs the mean-shift step
   // The reference's loop state lives in shared memory: only the leader thread touches it after this point, and
   // keeping it out of registers leaves them to the pipelined pass loop.
-  struct Lead { TrackState s; unsigned long long st_pass, st_serial, st_px; int call, it, prevx, prevy; bool bailed; };
+  struct Lead { TrackState s; unsigned long long st_pass, st_serial, st_px; int call, it, prevx, prevy; bool bailed;
+                double shift_cap; };
   __shared__ Lead lead_sh;
   if (tid == 0) {
     lead_sh.s = state[slot];
@@ -417,16 +485,26 @@ k_track(const uint16_t *__restrict__ bins, int W, int H, const int32_t *__restri
     return;
   }
   // getWeights — src/camshift.js:314-330 (every CTA keeps its own copy)
+  // The smallest non-zero weight (per warp here): a window has at most m00 / wmin non-zero pixels, which bounds its
+  // summation error (trunc_tolerance) far below its area when the weights are sparse.
+  __shared__ double wmin[NW];
+  __shared__ double nz_per_mass;                  // (1 + 1e-6) / wmin, set by the stepper; 1e-6 covers m00's own error
+  __shared__ TruncCap cap;                        // (stepper) the frame's caps of the radii
   {
     const uint32_t *mh = model_hist + (size_t)slot * 4096, *ch = cur_hist + (size_t)k * 4096;
+    double wm = INFINITY;
     for (int i = tid; i < 4096; i += NT) {
       const uint32_t c = ch[i], m = mh[i];
       double p = 0.0;
       // (a bin absent from the model gives 0 / c = +0.0: no division for it - that is nearly all of the 4096 bins)
       if (c != 0 && m != 0) p = fmin((double)m / (double)c, 1.0);
       wsm[i] = p;
+      if (p > 0.0) wm = fmin(wm, p);
     }
     if (tid == 0) wsm[4096] = 0.0;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) wm = fmin(wm, __shfl_xor_sync(0xffffffffu, wm, o));
+    if (lane == 0) wmin[warp] = wm;
   }
   const uint16_t *px = bins + (size_t)k * W * H;   // 12-bit colour bin of every pixel of this slot's frame (k_hist)
   const bool vec4 = (W & 3) == 0;
@@ -434,6 +512,7 @@ k_track(const uint16_t *__restrict__ bins, int W, int H, const int32_t *__restri
 
   // leader-only bookkeeping of the reference's loops (src/camshift.js:213-312)
   unsigned long long &st_pass = lead_sh.st_pass, &st_serial = lead_sh.st_serial, &st_px = lead_sh.st_px;
+  double &shift_cap = lead_sh.shift_cap;
   int &call = lead_sh.call, &it = lead_sh.it, &prevx = lead_sh.prevx, &prevy = lead_sh.prevy;
   bool &bailed = lead_sh.bailed;
   auto publish = [&](int done) {   // stepper: next window (or the finish flag) for this CTA
@@ -446,6 +525,7 @@ k_track(const uint16_t *__restrict__ bins, int W, int H, const int32_t *__restri
     if (call >= n_calls) return true;
     if (bail_area > 0 && (long long)s.sw * (long long)s.sh > (long long)bail_area) { bailed = true; return true; }
     it = 0; prevx = s.sx; prevy = s.sy;                            // :280-281
+    shift_cap = shift_tolerance(cap.eps, cap.M, 0.5 * fmax((double)s.sw, (double)s.sh));   // (trunc_cap)
     return false;
   };
   if (MBAR && tid == 0) {
@@ -454,8 +534,16 @@ k_track(const uint16_t *__restrict__ bins, int W, int H, const int32_t *__restri
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   if (TRACK_CLUSTER > 1) cluster.sync();  // every CTA is resident (and its mbarriers initialised) before the first remote access
-  if (stepper) publish(start_call() ? 1 : 0);
+  if (stepper) {
+    cap = trunc_cap(W, H);           // (start_call reads it)
+    publish(start_call() ? 1 : 0);
+  }
   __syncthreads();
+  if (stepper) {                     // (only the stepper reads nz_per_mass)
+    double wm = wmin[0];
+    for (int i = 1; i < NW; ++i) wm = fmin(wm, wmin[i]);
+    nz_per_mass = (1.0 + 1e-6) / wm;
+  }
 
 #ifndef HT_TRACK_LOOP2
 #define HT_TRACK_LOOP2 0   // 1: column blocks outer, x factors per block, edge selects only where needed - an A/B option, off by default
@@ -720,10 +808,19 @@ k_track(const uint16_t *__restrict__ bins, int W, int H, const int32_t *__restri
       int cw0 = win[0], cw1 = win[1], cw2 = win[2], cw3 = win[3];   // the window m belongs to
       ++st_pass;
       st_px += (unsigned long long)(max(ww, 0)) * (unsigned long long)(max(wh, 0));
+      // non-zero pixels of window cw, the one the parallel-order moments m belong to: at most its area, and at most
+      // m00 / wmin - the n of the decisions' radii (trunc_tolerance)
+      auto window_n = [&]() { return fmin((double)(cw2 - cw0) * (double)(cw3 - cw1), m.m00 * nz_per_mass); };
       for (;;) {
         double inv = 1.0 / m.m00;                                    // :109-111
         double vxf = m.m10 * inv - s.sw / 2.0, vyf = m.m01 * inv - s.sh / 2.0;
-        if (!exact && (force_serial || trunc_ambiguous(vxf) || trunc_ambiguous(vyf))) {
+        bool amb_shift = force_serial;
+        if (!exact && !amb_shift && (trunc_ambiguous(vxf, shift_cap) || trunc_ambiguous(vyf, shift_cap))) {
+          const double eps = sum_eps(window_n());
+          amb_shift = trunc_ambiguous(vxf, shift_tolerance(eps, m.m10 * inv, s.sw / 2.0)) ||
+                      trunc_ambiguous(vyf, shift_tolerance(eps, m.m01 * inv, s.sh / 2.0));
+        }
+        if (!exact && amb_shift) {
           m = moments_serial(px, W, cw0, cw1, cw2, cw3, wsm);
           exact = true;
           ++st_serial;
@@ -746,27 +843,29 @@ k_track(const uint16_t *__restrict__ bins, int W, int H, const int32_t *__restri
             const double xc = m.m10 * invM00, yc = m.m01 * invM00;
             const double mu20 = m.m20 - m.m10 * xc, mu02 = m.m02 - m.m01 * yc, mu11 = m.m11 - m.m01 * xc;
             const double a = mu20 * invM00, c = mu02 * invM00;
-            double l1, l2, ang = 3.141592653589793 / 2;
-            bool amb = false;
+            double l1, l2, b = 0.0, e = 0.0, ang = 3.141592653589793 / 2;
             if (s.calc_angles) {
-              const double b = mu11 * invM00;
+              b = mu11 * invM00;
               const double d = a + c;
-              const double e = sqrt((4 * b * b) + ((a - c) * (a - c)));
+              e = sqrt((4 * b * b) + ((a - c) * (a - c)));
               l1 = sqrt((d - e) * 0.5); l2 = sqrt((d + e) * 0.5);
-              // `if (ang < 0) ang += PI` (src/camshift.js:244) follows the SIGN of b = mu11 / m00: for a symmetric blob
-              // b is rounding residue and the parallel summation order may flip it (angle off by PI, far outside
-              // the 1e-4 tolerance) - take the strict order whenever b is not clearly away from 0
-              amb = fabs(b) <= 1e-9 * (fabs(a) + fabs(c) + 1.0);
-              if (exact || !(amb || trunc_ambiguous(l1) || trunc_ambiguous(l2))) {
-                ang = atan2(2 * b, a - c + e);
-                if (ang < 0) ang = ang + 3.141592653589793;
-              }
             } else {
               l1 = sqrt(a); l2 = sqrt(c);
             }
-            if (!exact && (amb || trunc_ambiguous(l1) || trunc_ambiguous(l2))) {
-              m = moments_serial(px, W, cw0, cw1, cw2, cw3, wsm); exact = true; ++st_serial;
-              continue;
+            // `if (ang < 0) ang += PI` (src/camshift.js:244) follows the SIGN of b = mu11 / m00: for a symmetric blob
+            // b is rounding residue and the parallel summation order may flip it (angle off by PI, far outside the
+            // 1e-4 tolerance) - so b within its radius of 0 takes the strict order too
+            if (!exact && ((s.calc_angles && fabs(b) <= cap.b) || trunc_ambiguous(l1, cap.root + 4.0 * TRUNC_U * l1) ||
+                           trunc_ambiguous(l2, cap.root + 4.0 * TRUNC_U * l2))) {
+              const TruncTol tol = trunc_tolerance(m, window_n(), s.sw, s.sh, s.calc_angles);
+              if ((s.calc_angles && fabs(b) <= tol.b) || trunc_ambiguous(l1, tol.l1) || trunc_ambiguous(l2, tol.l2)) {
+                m = moments_serial(px, W, cw0, cw1, cw2, cw3, wsm); exact = true; ++st_serial;
+                continue;
+              }
+            }
+            if (s.calc_angles) {
+              ang = atan2(2 * b, a - c + e);
+              if (ang < 0) ang = ang + 3.141592653589793;
             }
             s.tw = (int32_t)((uint32_t)js_to_int32(l1) << 2);
             s.th = (int32_t)((uint32_t)js_to_int32(l2) << 2);
