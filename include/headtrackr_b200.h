@@ -78,7 +78,12 @@ typedef struct {
 
 typedef struct {
   int32_t device;             /* CUDA device ordinal */
-  int32_t max_width;          /* largest frame the context must handle */
+  int32_t max_width;          /* largest frame the context must handle.  Detection has its own limit, whatever the
+                               * maximum: every pyramid resample job divides by 4*dw*dh with a 32-bit multiplier,
+                               * which needs dw*dh <= 2,968,721 for the largest job (W/s x H/s, s = 2^(1/(interval+1))).
+                               * Largest accepted 16:9 frame before the first rejected one: 2579x1450 at interval 5,
+                               * 2732x1536 at 3, 2895x1628 at 2, 3249x1827 at 1; 3840x2160 is rejected at every
+                               * interval (see ht_detect).  The reference has no such limit. */
   int32_t max_height;
   int32_t max_frames;         /* largest batch per call == number of tracker slots */
   int32_t max_raw_per_frame;  /* capacity of the pre-grouping list per frame (0 -> 1024) */
@@ -99,7 +104,16 @@ int ht_max_rects(const ht_ctx *ctx);            /* K */
 /* ccv.detect_objects(ccv.grayscale(frame), cascade, interval, min_neighbors) for n frames.
  *   out_rects : [n][K] ht_rect, reference order (src/ccv.js:293-330; raw order (scale,q,y,x) if min_neighbors<=0)
  *   out_counts: [n]    number of rects written for each frame
- * The input frames are not modified (the reference works on a copy, src/facetrackr.js:140-145). */
+ * The input frames are not modified (the reference works on a copy, src/facetrackr.js:140-145).
+ * HT_ERR_SIZE, before any kernel is launched, for a frame above max_width x max_height, for one whose pyramid has a
+ * 0-sized level (the smallest frames: 81x81 at interval 5, 77x77 at 3, 64x64 at 1 and 2; a browser throws there), and
+ * for one above the planner's size limit ("frame too large for 32-bit bilinear numerators").  That limit: k_resample
+ * computes floor(n / (4*dw*dh)) as (n * M) >> k with n and M 32-bit; the numerator n <= 1022*dw*dh fits up to
+ * dw*dh = 4,202,512, but the multiplier M (between n_max and 2*n_max) only up to dw*dh = 2,968,721, and again in
+ * 4,194,305..4,198,406.  So the largest accepted 16:9 frames are 2579x1450 at interval 5 (2580x1451 is rejected),
+ * 2732x1536 at 3, 2895x1628 at 2 and 3249x1827 at 1 (beyond those, a few isolated sizes are accepted again, such as
+ * 3864x2173 at 1); 3840x2160 is rejected at every interval.  The reference has no such limit: it detects at
+ * 2580x1451 and 3840x2160 too.  The same limit applies to every entry point that detects. */
 int ht_detect(ht_ctx *ctx, const uint8_t *rgba, int n, int w, int h, int interval, int min_neighbors,
               ht_rect *out_rects, int32_t *out_counts);
 
