@@ -53,6 +53,7 @@ class Context:
         if rc != 0:
             raise HtError(rc, (self._L.ht_last_error(None) or b"").decode())
         self.K = self._L.ht_max_rects(self._h)
+        self.raw_cap = max_raw_per_frame if max_raw_per_frame > 0 else 1024   # ht_config.max_raw_per_frame's default
         self.max_frames = max_frames
         self.last_warning = None
 
@@ -336,10 +337,13 @@ class Context:
         return buf[: w.value * h.value].reshape(h.value, w.value).copy()
 
     def debug_raw(self, frame, cap=65536):
+        """-> (the raw list k_group sorted, at most min(cap, raw_cap) entries; the number of windows the cascade found,
+        which exceeds raw_cap when the list overflowed)"""
         out = (Rect * cap)()
         cnt = C.c_int32()
         self._check(self._L.ht_debug_raw(self._h, frame, C.addressof(out), cap, C.addressof(cnt)))
-        return [(r.x, r.y, r.width, r.height, r.confidence, r.neighbors) for r in out[: min(cnt.value, cap)]], cnt.value
+        kept = min(cnt.value, cap, self.raw_cap)
+        return [(r.x, r.y, r.width, r.height, r.confidence, r.neighbors) for r in out[:kept]], cnt.value
 
     def debug_track_stats(self, reset=True):
         out = (C.c_uint64 * 5)()

@@ -496,6 +496,7 @@ struct ht_ctx {
   int last_n = 0;
 
   DevBuf arena, d_frames, raw_keys, raw_conf, raw_count, sorted, labels, seq2, d_out_rects, d_out_counts, d_flags;
+  DevBuf d_best;  // [frames] k_group's first-maximum record of each frame's whole list: the VJ->CS hand-offs read it
   DevBuf bins;  // [frames][h][w] u16 colour-bin planes written by k_hist, read by k_track
   DevBuf model_hist, cur_hist, track_state, d_slots, d_rects, d_found, d_objs, d_windows, d_wb_sums, d_wb_out, d_scratch;
 
@@ -531,7 +532,7 @@ struct ht_ctx {
   // the aux stream and returns; it runs under the detection of call s+1 (k_track is a latency chain that leaves
   // most issue slots idle, the detection kernels are throughput-bound).  What the two touch in common is double
   // buffered by call parity (bin planes, current-frame histograms) or ordered by an event (the caller's rectangle
-  // arrays: k_group of call s+1 waits for the tracking of call s).  Every other entry point joins first.
+  // arrays and d_best: k_group of call s+1 waits for the tracking of call s).  Every other entry point joins first.
   int pipeline = 0;
   int pipe_bg = 0;                          // HT_PIPE_BG=1: pipelined tracking runs BELOW the priority of the context's stream,
                                             // and k_cascade leaves room for one k_track CTA per SM while it is in flight
@@ -1149,7 +1150,7 @@ int run_detect(ht_ctx *ctx, cudaStream_t st, Plan *P, const uint8_t *d_rgba_batc
                                        ctx->labels.as<int>() + (size_t)f0 * ctx->raw_cap,
                                        ctx->seq2.as<Rect>() + (size_t)f0 * ctx->raw_cap, min_neighbors,
                                        d_rects_batch + (size_t)f0 * ctx->K, d_counts_batch + f0, ctx->K,
-                                       ctx->d_flags.as<int32_t>());
+                                       ctx->d_best.as<Rect>() + f0, ctx->d_flags.as<int32_t>());
   ctx->prof_end(st);
   ++ctx->launches;
   CK(cudaGetLastError());
@@ -1158,12 +1159,13 @@ int run_detect(ht_ctx *ctx, cudaStream_t st, Plan *P, const uint8_t *d_rgba_batc
 
 // pick (optional) + initTracker + n_calls x track() for frames [f0, f0+n); slot of frame k is k (slots == NULL)
 int run_track_from_detect(ht_ctx *ctx, cudaStream_t st, const uint8_t *d_rgba_batch, int w, int h, int f0, int n,
-                          const Rect *d_det, const int32_t *d_cnt, int calc_angles, int n_calls, int32_t *d_found,
+                          const int32_t *d_cnt, int calc_angles, int n_calls, int32_t *d_found,
                           int32_t *d_objs, int32_t *d_win) {
   const uint8_t *d_rgba = d_rgba_batch + (size_t)f0 * w * h * 4;
   int32_t *d_rects4 = ctx->d_rects.as<int32_t>() + 4 * (size_t)f0;
   ctx->prof_begin(HT_PROF_TRACK_INIT, st);
-  k_pick_face<<<(n + 127) / 128, 128, 0, st>>>(d_det + (size_t)f0 * ctx->K, d_cnt + f0, ctx->K, n, d_rects4);
+  // the first maximum of each frame's whole list, not only of the K entries copied out
+  k_pick_face<<<(n + 127) / 128, 128, 0, st>>>(ctx->d_best.as<Rect>() + f0, 1, d_cnt + f0, 1, n, d_rects4);
   k_track_init<<<n, 256, 0, st>>>(d_rgba, (size_t)w * h * 4, w, h, nullptr, d_rects4, calc_angles ? 1 : 0,
                                   ctx->model_hist.as<uint32_t>() + (size_t)f0 * 4096,
                                   ctx->track_state.as<TrackState>() + f0, d_found ? d_found + f0 : nullptr, nullptr);
@@ -1337,6 +1339,7 @@ int ht_create(ht_ctx **out, const ht_config *cfg, const void *cascade_blob, size
             c->seq2.reserve(mf * c->raw_cap * sizeof(Rect)) == cudaSuccess &&
             c->d_out_rects.reserve(mf * c->K * sizeof(Rect)) == cudaSuccess &&
             c->d_out_counts.reserve(mf * sizeof(int32_t)) == cudaSuccess &&
+            c->d_best.reserve(mf * sizeof(Rect)) == cudaSuccess &&
             c->d_flags.reserve(256) == cudaSuccess;
   if (!ok) { g_create_error = "ht_create: cudaMalloc failed"; return HT_ERR_CUDA; }
   cudaMemset(c->d_flags.p, 0, 256);
@@ -1450,7 +1453,8 @@ int ht_track_init_from_detect(ht_ctx *ctx, const int32_t *slots, int n, const ui
   rc = stage_input(ctx, st, det_counts, is_device_ptr(det_counts), sizeof(int32_t) * n, ctx->d_out_counts, &d_cnt);
   if (rc != HT_OK) return rc;
   ctx->prof_begin(HT_PROF_TRACK_INIT, st);
-  k_pick_face<<<(n + 127) / 128, 128, 0, st>>>(reinterpret_cast<const Rect *>(d_det), d_cnt, ctx->K, n, ctx->d_rects.as<int32_t>());
+  k_pick_face<<<(n + 127) / 128, 128, 0, st>>>(reinterpret_cast<const Rect *>(d_det), ctx->K, d_cnt, ctx->K, n,
+                                               ctx->d_rects.as<int32_t>());
   ctx->prof_end(st);
   ++ctx->launches;
   CK(cudaGetLastError());
@@ -1539,7 +1543,7 @@ int ht_detect_track(ht_ctx *ctx, const uint8_t *rgba, int n, int w, int h, int i
     if (rc != HT_OK) return rc;
     CK(cudaEventRecord(ctx->pipe_detect_done, st));
     CK(cudaStreamWaitEvent(ctx->aux_stream, ctx->pipe_detect_done, 0));
-    rc = run_track_from_detect(ctx, ctx->aux_stream, rgba, w, h, 0, n, d_rects, d_counts, calc_angles, n_calls, d_found,
+    rc = run_track_from_detect(ctx, ctx->aux_stream, rgba, w, h, 0, n, d_counts, calc_angles, n_calls, d_found,
                                d_objs, d_win);
     if (rc != HT_OK) return rc;
     CK(cudaEventRecord(ctx->aux_done, ctx->aux_stream));
@@ -1573,11 +1577,11 @@ int ht_detect_track(ht_ctx *ctx, const uint8_t *rgba, int n, int w, int h, int i
   }
   // run tracking for frames [f0, f0+nf) — on the aux stream when overlapping
   auto track_part = [&](const uint8_t *d_frames_batch, int f0, int nf) -> int {
-    if (parts == 1 || !use_aux) return run_track_from_detect(ctx, st, d_frames_batch, w, h, f0, nf, d_rects, d_counts, calc_angles, n_calls, d_found, d_objs, d_win);
+    if (parts == 1 || !use_aux) return run_track_from_detect(ctx, st, d_frames_batch, w, h, f0, nf, d_counts, calc_angles, n_calls, d_found, d_objs, d_win);
     const int pi = ctx->part_seq++ & 3;
     CK(cudaEventRecord(ctx->part_events[pi], st));
     CK(cudaStreamWaitEvent(ctx->aux_stream, ctx->part_events[pi], 0));
-    return run_track_from_detect(ctx, ctx->aux_stream, d_frames_batch, w, h, f0, nf, d_rects, d_counts, calc_angles, n_calls, d_found, d_objs, d_win);
+    return run_track_from_detect(ctx, ctx->aux_stream, d_frames_batch, w, h, f0, nf, d_counts, calc_angles, n_calls, d_found, d_objs, d_win);
   };
   if (frames_dev) {
     for (int p = 0; p < parts; ++p) {
@@ -1741,7 +1745,7 @@ int ht_stream_step_head(ht_ctx *ctx, const uint8_t *rgba, int n, int w, int h, i
   StreamEvent *d_ev = io.out<StreamEvent>(out_events, ctx->d_stream_events, sizeof(StreamEvent) * (size_t)n);
   HeadEvent *d_he = out_head ? io.out<HeadEvent>(out_head, ctx->d_head_events, sizeof(HeadEvent) * (size_t)n)
                              : ctx->head_on ? ctx->d_head_events.as<HeadEvent>() : nullptr;
-  k_stream_update<<<(n + 127) / 128, 128, 0, st>>>(mode, n, ctx->d_out_rects.as<Rect>(), ctx->d_out_counts.as<int32_t>(), ctx->K,
+  k_stream_update<<<(n + 127) / 128, 128, 0, st>>>(mode, n, ctx->d_best.as<Rect>(), ctx->d_out_counts.as<int32_t>(),
                                                    ctx->d_objs.as<int32_t>(), ctx->d_rects.as<int32_t>(), init_en, d_ev,
                                                    ctx->head_on ? ctx->d_head_state.as<HeadState>() : nullptr,
                                                    ctx->d_head_params.as<HeadParams>(), d_he, w, h);
@@ -1875,8 +1879,8 @@ static int tracker_tick(ht_ctx *ctx, Plan *P, const uint8_t *d_rgba, int n, int 
   Outputs io(ctx);
   TrackerEvent *d_ev = io.out<TrackerEvent>(out, ctx->d_tracker_events, sizeof(TrackerEvent) * (size_t)n);
   k_tracker_update<<<(n + 127) / 128, 128, 0, st>>>(ts, d_ids, ctx->d_tracker_params.as<TrackerParams>(), n,
-                                                    ctx->d_wb_sums.as<unsigned long long>(), w * h, ctx->d_out_rects.as<Rect>(),
-                                                    ctx->d_out_counts.as<int32_t>(), ctx->K, ctx->d_objs.as<int32_t>(),
+                                                    ctx->d_wb_sums.as<unsigned long long>(), w * h, ctx->d_best.as<Rect>(),
+                                                    ctx->d_out_counts.as<int32_t>(), ctx->d_objs.as<int32_t>(),
                                                     ctx->d_rects.as<int32_t>(), init_en, now_ms, d_now, w, h, d_ev);
   ctx->prof_begin(HT_PROF_TRACK_INIT, st);
   k_track_init<<<n, 256, 0, st>>>(d_rgba, (size_t)w * h * 4, w, h, d_ids, ctx->d_rects.as<int32_t>(), ctx->tracker_calc_angles,

@@ -960,13 +960,29 @@ __device__ __forceinline__ bool group_pred(const Rect &r1, const Rect &r2) {  //
          floor(r2.width * 1.5 + 0.5) >= r1.width;
 }
 
+// The first maximum of confidence over a list whose entries are dealt out to the lanes: each lane brings the first
+// maximum (c, i) of its own entries, i = -1 for none.  Returns the list index of the overall first maximum (-1: empty
+// list) on every lane - the (larger c, then smaller i) order is total, so the butterfly agrees on all lanes.
+__device__ __forceinline__ int warp_first_max(double c, int i) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const double c2 = __shfl_xor_sync(0xffffffffu, c, o);
+    const int i2 = __shfl_xor_sync(0xffffffffu, i, o);
+    if (i2 >= 0 && (i < 0 || c2 > c || (c2 == c && i2 < i))) { c = c2; i = i2; }
+  }
+  return i;
+}
+
+// out_rects / out_counts: the first K entries of each frame's list and min(length, K).  best[frame]: the first
+// maximum-confidence entry of the WHOLE list (written when the list is not empty) - facetrackr's VJ->CS hand-off
+// (src/facetrackr.js:157-165) reads it, so that K bounds only the copy-out and not which face gets tracked.
 __global__ void __launch_bounds__(128) k_group(DevPlan plan, int n_frames, const uint32_t *__restrict__ raw_keys,
                                                const double *__restrict__ raw_conf,
                                                const uint32_t *__restrict__ raw_count, int raw_cap,
                                                Rect *__restrict__ sorted, int *__restrict__ labels,
                                                Rect *__restrict__ seq2, int min_neighbors,
                                                Rect *__restrict__ out_rects, int32_t *__restrict__ out_counts, int K,
-                                               int32_t *__restrict__ overflow_flag) {
+                                               Rect *__restrict__ best, int32_t *__restrict__ overflow_flag) {
   const int lane = threadIdx.x & 31;
   const int frame = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (frame >= n_frames) return;
@@ -1008,8 +1024,15 @@ __global__ void __launch_bounds__(128) k_group(DevPlan plan, int n_frames, const
   __syncwarp();
 
   if (!(min_neighbors > 0)) {  // src/ccv.js:249-250: raw list
-    for (int i = lane; i < n && i < K; i += 32) O[i] = S[i];
+    double bc = 0.0;
+    int bi = -1;
+    for (int i = lane; i < n; i += 32) {
+      if (i < K) O[i] = S[i];
+      if (bi < 0 || S[i].confidence > bc) { bc = S[i].confidence; bi = i; }
+    }
+    bi = warp_first_max(bc, bi);
     if (lane == 0) {
+      if (bi >= 0) best[frame] = S[bi];
       out_counts[frame] = min(n, K);
       if (n > K) atomicOr(overflow_flag, 1);
     }
@@ -1081,6 +1104,8 @@ __global__ void __launch_bounds__(128) k_group(DevPlan plan, int n_frames, const
 
   // 4. drop rectangles contained in a better one, src/ccv.js:307-330
   int n_out = 0;
+  double bc = 0.0;   // this lane's first maximum over the kept rectangles it evaluates (index into S2, -1: none)
+  int bi = -1;
   for (int base = 0; base < n2; base += 32) {
     const int i = base + lane;
     bool flag = i < n2;
@@ -1102,10 +1127,13 @@ __global__ void __launch_bounds__(128) k_group(DevPlan plan, int n_frames, const
     if (flag) {
       const int pos = n_out + __popc(m & ((1u << lane) - 1u));
       if (pos < K) O[pos] = r1;
+      if (bi < 0 || r1.confidence > bc) { bc = r1.confidence; bi = i; }
     }
     n_out += __popc(m);
   }
+  bi = warp_first_max(bc, bi);   // the kept rectangles keep their S2 order, so the first in S2 is the first in the list
   if (lane == 0) {
+    if (bi >= 0) best[frame] = S2[bi];
     out_counts[frame] = min(n_out, K);
     if (n_out > K) atomicOr(overflow_flag, 1);
   }

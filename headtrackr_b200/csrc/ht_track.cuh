@@ -116,14 +116,16 @@ __global__ void __launch_bounds__(256) k_track_init(const uint8_t *__restrict__ 
 
 // facetrackr's VJ->CS hand-off on the device — src/facetrackr.js:157-165 (first max-confidence
 // candidate), :97 (confidence > -10), :101-106 (Math.floor of x,y,width,height).
-__global__ void k_pick_face(const Rect *__restrict__ det, const int32_t *__restrict__ counts, int K, int n,
+// Frame k's candidates are det[k * stride, k * stride + min(counts[k], cap)): a caller's lists (stride = cap = K), or
+// k_group's first-maximum records (stride = cap = 1), which stand for the whole grouped list when counts[k] > 0.
+__global__ void k_pick_face(const Rect *__restrict__ det, int stride, const int32_t *__restrict__ counts, int cap, int n,
                             int32_t *__restrict__ rects) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= n) return;
-  const int c = counts[k];
+  const int c = min(counts[k], cap);
   int32_t r[4] = {0, 0, 0, 0};
   if (c > 0) {
-    const Rect *d = det + (size_t)k * K;
+    const Rect *d = det + (size_t)k * stride;
     int best = 0;
     for (int i = 1; i < c; ++i)
       if (d[i].confidence > d[best].confidence) best = i;
@@ -1177,8 +1179,10 @@ __host__ __device__ inline int facetrackr_pass(bool vj, const Rect *det, int cou
   return 1;
 }
 
-__global__ void k_stream_update(int32_t *__restrict__ mode, int n, const Rect *__restrict__ det,
-                                const int32_t *__restrict__ counts, int K, const int32_t *__restrict__ objs,
+// best[k], counts[k]: k_group's first-maximum record of stream k's grouped list and the list's copied-out length
+// (> 0 exactly when the list is not empty)
+__global__ void k_stream_update(int32_t *__restrict__ mode, int n, const Rect *__restrict__ best,
+                                const int32_t *__restrict__ counts, const int32_t *__restrict__ objs,
                                 int32_t *__restrict__ rects, uint8_t *__restrict__ init_enable,
                                 StreamEvent *__restrict__ events,
                                 // optional head-position epilogue (ht_stream_head_config): per-stream state, parameters,
@@ -1191,7 +1195,7 @@ __global__ void k_stream_update(int32_t *__restrict__ mode, int n, const Rect *_
   const bool vj = mode[k] == 0;
   bool seed;
   int32_t rect[4];
-  mode[k] = facetrackr_pass(vj, det + (size_t)k * K, vj ? counts[k] : 0, objs + 6 * (size_t)k, e, rect, seed);
+  mode[k] = facetrackr_pass(vj, best + k, (vj && counts[k] > 0) ? 1 : 0, objs + 6 * (size_t)k, e, rect, seed);
   if (seed) {
     for (int i = 0; i < 4; ++i) rects[4 * k + i] = rect[i];
     init_enable[k] = 1;
@@ -1391,11 +1395,12 @@ __global__ void k_tracker_plan(const TrackerState *__restrict__ st, const int32_
   }
 }
 
-// now (ht_tracker_feed, else NULL): the clock of each batch entry; otherwise every entry ticks at now_ms
+// now (ht_tracker_feed, else NULL): the clock of each batch entry; otherwise every entry ticks at now_ms.
+// best, counts: as in k_stream_update, per batch entry
 __global__ void k_tracker_update(TrackerState *__restrict__ st, const int32_t *__restrict__ ids,
                                  const TrackerParams *__restrict__ params, int n,
-                                 const unsigned long long *__restrict__ wb_sums, int n_px, const Rect *__restrict__ det,
-                                 const int32_t *__restrict__ counts, int K, const int32_t *__restrict__ objs,
+                                 const unsigned long long *__restrict__ wb_sums, int n_px, const Rect *__restrict__ best,
+                                 const int32_t *__restrict__ counts, const int32_t *__restrict__ objs,
                                  int32_t *__restrict__ rects, uint8_t *__restrict__ init_enable, double now_ms,
                                  const double *__restrict__ now, int camw, int camh, TrackerEvent *__restrict__ events) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1407,7 +1412,7 @@ __global__ void k_tracker_update(TrackerState *__restrict__ st, const int32_t *_
   TrackerEvent e;
   int32_t rect[4];
   bool seed;
-  tracker_step(s, *params, wb, det + (size_t)k * K, s.mode == TM_VJ ? counts[k] : 0, objs + 6 * (size_t)k, now_ms,
+  tracker_step(s, *params, wb, best + k, (s.mode == TM_VJ && counts[k] > 0) ? 1 : 0, objs + 6 * (size_t)k, now_ms,
                (double)camw, (double)camh, e, rect, seed);
   if (seed) {
     for (int i = 0; i < 4; ++i) rects[4 * k + i] = rect[i];

@@ -147,5 +147,55 @@ def frame(index, W=640, H=480, n_faces=None, seed_base=SEED_BASE, kind="faces", 
     return (out, faces) if return_faces else out
 
 
+def _paste_face(out, x, y, side, blob=None):
+    """The face template resized to side x side with frame()'s tint, clipped to the frame at its right and bottom."""
+    H, W = out.shape[:2]
+    t = shim_resize(face_template(blob), side, side).astype(np.int32)[: H - y, : W - x]
+    h, w = t.shape
+    out[y:y + h, x:x + w, 0] = t.astype(np.uint8)
+    out[y:y + h, x:x + w, 1] = ((t * 200) >> 8).astype(np.uint8)
+    out[y:y + h, x:x + w, 2] = ((t * 150) >> 8).astype(np.uint8)
+
+
+def crowd_frame(seed, W=320, H=240, side=24, pitch=None, jitter=0, variant="grid", blob=None):
+    """A frame crowded with faces, for the grouping step: many raw windows and many groups.
+
+    The background is frame(seed, W, H, n_faces=0).  Faces of `side` px are pasted on a grid of `pitch` px from (0,0),
+    each cell shifted by rng.integers(0, jitter + 1) in x and in y (rng = default_rng(seed)) and clamped to the frame.
+    variant:
+      grid     the grid alone
+      sizes    rows alternate between side and side * 3 // 2 (two face sizes in one frame)
+      nested   the grid, then one face of 4 * side at the frame's centre with a face of side px inside it
+               (the containment filter of the grouping step)
+      edges    the grid shifted so that the last column and row are cut by the right and bottom edges
+      chains   rows of overlapping faces spaced by 2 * floor(side / 4 + 0.5) + {0, 1} px: the windows of neighbouring
+               faces lie near the grouping predicate's distance floor(w / 4 + 0.5) of each other
+    Integer-only, like frame()."""
+    pitch = side if pitch is None else pitch
+    rng = np.random.default_rng(seed)
+    out = frame(seed, W, H, n_faces=0, blob=blob)
+    if variant == "chains":
+        d = (side + 2) // 4                                # floor(side / 4 + 0.5)
+        for y in range(0, H - side + 1, pitch):
+            x = 0
+            while x + side <= W:
+                _paste_face(out, x, y, side, blob)
+                x += 2 * d + int(rng.integers(0, 2))
+        return out
+    off = (side // 2) if variant == "edges" else 0
+    for row, y0 in enumerate(range(off, H - (0 if variant == "edges" else side) + 1, pitch)):
+        s = side * 3 // 2 if (variant == "sizes" and row % 2) else side
+        for x0 in range(off, W - (0 if variant == "edges" else s) + 1, pitch):
+            x = min(x0 + int(rng.integers(0, jitter + 1)), W - (1 if variant == "edges" else s))
+            y = min(y0 + int(rng.integers(0, jitter + 1)), H - (1 if variant == "edges" else s))
+            _paste_face(out, x, y, s, blob)
+    if variant == "nested":
+        big = 4 * side
+        x, y = max(0, (W - big) // 2), max(0, (H - big) // 2)
+        _paste_face(out, x, y, big, blob)
+        _paste_face(out, x + big // 4, y + big // 4, side, blob)
+    return out
+
+
 def batch(n, W=640, H=480, start=0, **kw):
     return np.stack([frame(start + i, W, H, **kw) for i in range(n)])

@@ -86,8 +86,15 @@ typedef struct {
                                * interval (see ht_detect).  The reference has no such limit. */
   int32_t max_height;
   int32_t max_frames;         /* largest batch per call == number of tracker slots */
-  int32_t max_raw_per_frame;  /* capacity of the pre-grouping list per frame (0 -> 1024) */
-  int32_t max_rects_per_frame;/* K: capacity of the result list per frame (0 -> 64) */
+  int32_t max_raw_per_frame;  /* capacity of the pre-grouping list per frame (0 -> 1024).  A crowded 640x480 frame
+                               * already has more raw windows than 1024 (about 1,900 for a grid of 28 px faces).  On
+                               * overflow the call returns HT_WARN_OVERFLOW and groups a subset of the windows: which
+                               * subset depends on the cascade's arrival order, so the grouped list and the face the
+                               * VJ->CS hand-offs pick match the reference only when the raw list did not overflow. */
+  int32_t max_rects_per_frame;/* K: capacity of the result list per frame (0 -> 64).  K bounds only the list copied out
+                               * (the reference's first K entries, HT_WARN_OVERFLOW when longer): the VJ->CS hand-offs
+                               * of ht_detect_track, ht_stream_step(_head), ht_tracker_step and ht_tracker_feed pick the
+                               * first maximum of the WHOLE grouped list, as src/facetrackr.js:157-165 does. */
   void *cuda_stream;          /* cudaStream_t to run on; NULL -> the context creates its own */
 } ht_config;
 
@@ -127,7 +134,9 @@ int ht_track_init(ht_ctx *ctx, const int32_t *slots, int n, const uint8_t *rgba,
 
 /* The VJ->CS hand-off of facetrackr (src/facetrackr.js:157-165 first-max-confidence pick, :97-108
  * confidence > -10 gate and Math.floor of x,y,w,h) done on the device from ht_detect's outputs:
- *   det_rects [n][K], det_counts [n] (host or device).  out_found [n] (optional): 1 if the slot was seeded. */
+ *   det_rects [n][K], det_counts [n] (host or device).  out_found [n] (optional): 1 if the slot was seeded.
+ * The pick is over the list passed in: det_rects[k][0, min(det_counts[k], K)).  When ht_detect truncated a list to K
+ * entries, the pick can differ from the reference's; ht_detect_track picks from the whole list. */
 int ht_track_init_from_detect(ht_ctx *ctx, const int32_t *slots, int n, const uint8_t *rgba, int w, int h,
                               const ht_rect *det_rects, const int32_t *det_counts, int calc_angles,
                               int32_t *out_found);
@@ -141,6 +150,7 @@ int ht_track(ht_ctx *ctx, const int32_t *slots, int n, const uint8_t *rgba, int 
 /* One facetrackr VJ frame followed by its CS frames, for a batch (src/facetrackr.js:67-126):
  *   ht_detect -> first-max-confidence pick, confidence > -10 gate, floor -> initTracker on slot k for frame k
  *   -> n_calls x track().  Frames with no usable face leave out_found[k] = 0 and a zero TrackObj.
+ * The pick is over the whole grouped list, also when out_rects holds only its first K entries (HT_WARN_OVERFLOW).
  * With HOST frames the upload is pipelined in chunks against the kernels of the previous chunk.
  * out_found and out_windows are optional. */
 int ht_detect_track(ht_ctx *ctx, const uint8_t *rgba, int n, int w, int h, int interval, int min_neighbors,
@@ -194,6 +204,9 @@ int ht_stream_step_head(ht_ctx *ctx, const uint8_t *rgba, int n, int w, int h, i
 
 /* put streams [first, first+n) back into "VJ" (new facetrackr.Tracker) */
 int ht_stream_reset(ht_ctx *ctx, int first, int n);
+/* The "VJ" pick is over the whole grouped list of the stream's frame: K (max_rects_per_frame) does not change which
+ * face is tracked.  A frame whose raw list overflows max_raw_per_frame returns HT_WARN_OVERFLOW, and its pick may differ
+ * from the reference's. */
 int ht_stream_step(ht_ctx *ctx, const uint8_t *rgba, int n, int w, int h, int interval, int min_neighbors,
                    int calc_angles, ht_stream_event *out_events);
 
@@ -269,7 +282,8 @@ typedef struct {
  * stream id out of range or listed twice, a NULL pixel pointer, a pointer or pitch that is not a multiple of 4, a
  * pitch below 4*width, or a first pointer whose memory space contradicts frames_on_device; HT_ERR_SIZE for a video
  * size outside 1..16384 or a canvas that is 0-sized, larger than max_width x max_height or too small for the pyramid.
- * ht_tracker_step and ht_tracker_feed may be mixed on one context: both tick the same per-stream state. */
+ * ht_tracker_step and ht_tracker_feed may be mixed on one context: both tick the same per-stream state.  In both, the
+ * "VJ" pick is over the whole grouped list (as for ht_stream_step), unless the raw list overflowed (HT_WARN_OVERFLOW). */
 int ht_tracker_feed(ht_ctx *ctx, const ht_video_frame *frames, int n, int frames_on_device, int canvas_w, int canvas_h,
                     ht_tracker_event *out);
 

@@ -602,17 +602,24 @@ void hto_backprojection_img(const hto_tracker *t, const uint8_t *rgba, int W, in
  * initTracker -> n_calls x track().  Returns the number of detections; *found = 1 if a tracker was seeded. */
 int hto_detect_track(const uint8_t *rgba, int W, int H, const void *blob, size_t blob_len, int interval,
                      int min_neighbors, int calc_angles, int n_calls, hto_tracker *t_out, int *found) {
-  hto_rect res[256];
+  hto_rect res_small[256], *res = res_small;
   int n = hto_detect(rgba, W, H, blob, blob_len, interval, min_neighbors, res, 256, NULL, 0, NULL);
   if (found) *found = 0;
   if (n <= 0) return n;
-  int m = n < 256 ? n : 256, best = 0;
-  for (int i = 1; i < m; ++i)
+  if (n > 256) {   /* the pick is over the whole list: detect again into a list that holds it */
+    res = (hto_rect *)malloc(sizeof(hto_rect) * (size_t)n);
+    if (!res) return -1;
+    hto_detect(rgba, W, H, blob, blob_len, interval, min_neighbors, res, n, NULL, 0, NULL);
+  }
+  int best = 0;
+  for (int i = 1; i < n; ++i)
     if (res[i].confidence > res[best].confidence) best = i;
-  if (!(res[best].confidence > -10)) return n;
+  const hto_rect cand = res[best];
+  if (res != res_small) free(res);
+  if (!(cand.confidence > -10)) return n;
   hto_tracker t;
-  if (hto_tracker_init(&t, rgba, W, H, (int)floor(res[best].x), (int)floor(res[best].y), (int)floor(res[best].width),
-                       (int)floor(res[best].height), calc_angles) != 0)
+  if (hto_tracker_init(&t, rgba, W, H, (int)floor(cand.x), (int)floor(cand.y), (int)floor(cand.width),
+                       (int)floor(cand.height), calc_angles) != 0)
     return n;
   for (int c = 0; c < n_calls; ++c) hto_tracker_track(&t, rgba, W, H, NULL);
   if (t_out) *t_out = t;
