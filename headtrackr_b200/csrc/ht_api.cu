@@ -2362,13 +2362,30 @@ extern "C" int ht_selftest_pyramid(int w, int h, int interval, const uint8_t *rg
   return 0;
 }
 
+// parse_cascade's verdict on a blob -> rc; out[0..5 + n_groups] = {fast, late_int, n_groups, first late stage,
+// n_stages, group_first[0], ..., group_first[n_groups]}
+extern "C" int ht_selftest_parse_cascade(const void *blob, size_t blob_len, int32_t *out, int cap) {
+  static HostCascade hc;
+  std::string err;
+  const int rc = parse_cascade(blob, blob_len, hc, err);
+  if (rc != HT_OK) return rc;
+  const ConstCascade &cc = hc.cc;
+  if (cap < 6 + cc.n_groups) return -100;
+  out[0] = hc.fast ? 1 : 0; out[1] = cc.late_int; out[2] = cc.n_groups; out[3] = cc.group_first[cc.n_groups];
+  out[4] = hc.n_stages;
+  for (int g = 0; g <= cc.n_groups; ++g) out[5 + g] = cc.group_first[g];
+  return HT_OK;
+}
+
+// k_cascade's tile evaluation over one frame quad of `arena`, for any cascade blob: the generated path (quad-form
+// dense group, generated stages, integer late stages) or the table-driven one (ordered fp64 dense group and group
+// loop, then integer late stages with the tie fallback, or no late stages on the fp path).
 extern "C" int ht_selftest_cascade(const void *blob, size_t blob_len, int w, int h, int interval, const uint32_t *arena,
                                    int n_frames, int force_ties, int quad_stages, double *out /* [4][cap][4] x,y,width,conf */,
                                    int32_t *counts, int cap) {
   static HostCascade hc;   // (ConstCascade is 63 KB: keep it off the stack)
   std::string err;
   if (parse_cascade(blob, blob_len, hc, err) != HT_OK) { fprintf(stderr, "%s\n", err.c_str()); return -1; }
-  if (!hc.fast) return -3;
   Plan P;
   if (build_plan(P, w, h, interval, hc.width, hc.height, err, false) != HT_OK) { fprintf(stderr, "%s\n", err.c_str()); return -2; }
   g_host_casc = &hc.cc;
@@ -2417,12 +2434,21 @@ extern "C" int ht_selftest_cascade(const void *blob, size_t blob_len, int w, int
       tA = tile_b + 4 * (v * VA + u) + f;
       tB = tile_b + 4 * (v * VB + u) + f;
     };
-    // dense group (quad form)
+    // dense group (quad form; ordered fp64 sums for any other cascade than the generated one)
     std::vector<int> list[32];
     for (int v = 0; v < 2 * TH; ++v)
       for (int u = 0; u < 2 * TW; ++u) {
         const int lx = u >> 1, ly = v >> 1;
         const uint32_t *tA = tile.data() + v * VA + u, *tB = tile.data() + v * VB + u;
+        if (!hc.fast) {   // table-driven: ordered fp64 sums over [group_first[0], group_first[1]), one frame at a time
+          for (int f = 0; f < 4; ++f) {
+            bool alive = (x0 + lx < sc.qw) && (y0 + ly < sc.qh) && ((fmask >> f) & 1u);
+            const uint8_t *bA = reinterpret_cast<const uint8_t *>(tA) + f, *bB = reinterpret_cast<const uint8_t *>(tB) + f;
+            for (int j = cc.group_first[0]; j < cc.group_first[1] && alive; ++j) alive = stage_pass_ordered(bA, bB, j);
+            if (alive) list[bank_class(u, v)].push_back((v << 6) | u | (f << 11));
+          }
+          continue;
+        }
         uint32_t a_lo = 0, a_hi = 0;
         if (x0 + lx < sc.qw && y0 + ly < sc.qh) {
           a_lo = ((fmask & 1u) ? 0x8000u : 0u) | ((fmask & 4u) ? 0x80000000u : 0u);
@@ -2454,7 +2480,11 @@ extern "C" int ht_selftest_cascade(const void *blob, size_t blob_len, int w, int
         const uint8_t *tA, *tB;
         bases(e, tA, tB);
         bool alive = true;
-        for (int j = quad_stages; j < late_first && alive; ++j) {
+        // table-driven: the kernel's group loop (g = 1 .. n_groups - 1); with n_groups == 1 its own emit block lists
+        // the dense group's survivors
+        for (int g = 1; !hc.fast && g < cc.n_groups && alive; ++g)
+          for (int j = cc.group_first[g]; j < cc.group_first[g + 1] && alive; ++j) alive = stage_pass_ordered(tA, tB, j);
+        for (int j = quad_stages; hc.fast && j < late_first && alive; ++j) {
           int r = gen_stage(j, tA, tB);
           if (force_ties & 1) r = -1;
           if (r < 0) r = stage_pass_ordered(tA, tB, j) ? 1 : 0;
