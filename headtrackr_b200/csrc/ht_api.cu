@@ -314,7 +314,7 @@ int parse_cascade(const void *blob, size_t len, HostCascade &hc, std::string &er
   auto point_off = [&](int z, int x, int y, bool &ok) -> uint16_t {
     const int lim = (24 >> z) - 1;
     if (z < 0 || z > 2 || x < 0 || y < 0 || x > lim || y > lim) { ok = false; return 0; }
-    return (uint16_t)(point_word(z, x, y) | ((z > 0 && !HT_UNIBASE) ? 0x8000 : 0));   // bit 15: relative to baseB (two-base layout)
+    return (uint16_t)(point_word(z, x, y) | (z > 0 ? 0x8000 : 0));   // bit 15: relative to baseB
   };
   for (int k = 0; k < hc.n_features; ++k) {
     const uint8_t *r = pf + (size_t)k * 32;
@@ -364,13 +364,7 @@ int parse_cascade(const void *blob, size_t len, HostCascade &hc, std::string &er
   // numbers are not 8-digit decimals, lane-per-window groups to the end.
   {
     int g = 0;
-#if HT_GROUP_SPLIT >= 2
-    const int cuts_fast[] = {0, 2, 3, 4, 5, 6, 7};   // {0,1} {2} {3} {4} {5} {6} {7}
-#elif HT_GROUP_SPLIT == 1
-    const int cuts_fast[] = {0, 2, 3, 4, 5, 6};      // {0,1} {2} {3} {4} {5} {6,7}
-#else
     const int cuts_fast[] = {0, 2, 3, 4, 6};         // {0,1} {2} {3} {4,5} {6,7}: the generated stages
-#endif
     const int cuts_int[] = {0, 2, 4, 6};
     const int cuts_fp[] = {0, 2, 4, 6, 9};
     static_assert(HT_GEN_STAGES == 8, "cuts_fast assumes 8 generated stages");
@@ -534,8 +528,6 @@ struct ht_ctx {
   // buffered by call parity (bin planes, current-frame histograms) or ordered by an event (the caller's rectangle
   // arrays and d_best: k_group of call s+1 waits for the tracking of call s).  Every other entry point joins first.
   int pipeline = 0;
-  int pipe_bg = 0;                          // HT_PIPE_BG=1: pipelined tracking runs BELOW the priority of the context's stream,
-                                            // and k_cascade leaves room for one k_track CTA per SM while it is in flight
   bool aux_pending = false;                 // work on aux_stream that the context's stream has not waited for yet
   Event pipe_detect_done;
   int pipe_parity = 0;
@@ -565,13 +557,12 @@ struct ht_ctx {
   Event compute_done;
   std::vector<Event> chunk_events;
   int h2d_chunk = 64;                       // frames per pipelined upload chunk
-  int track_cluster = 0;                    // >0: force single-phase k_track with that cluster size (A/B profiling)
+  int track_cluster = 0;                    // >0: k_track clusters of that size instead of 2/4/8 by stream count (the heavy and mid tiers keep theirs)
   bool track_memo = true;                   // k_track re-uses the moments of windows it has already summed in this
                                             // launch (ht_set_track_memo / HT_TRACK_MEMO=0 for the strict A/B)
   bool track_trace = false;                 // HT_TRACK_TRACE=1: k_track writes a per-stream timeline (ht_debug_track_trace)
   DevBuf d_trace;
   int track_nt = 256;                       // threads per k_track CTA (HT_TRACK_NT=128|256)
-  bool track_lpt = true;                    // longest-chain-first launch order (HT_TRACK_LPT=0 disables)
   DevBuf d_stream_mode, d_stream_mask, d_stream_cs, d_stream_init, d_stream_events;   // ht_stream_step
   DevBuf d_head_state, d_head_params, d_head_events;                                  // ht_stream_head_config
   bool head_on = false;
@@ -583,21 +574,16 @@ struct ht_ctx {
   DevBuf d_feed_table, d_feed_draw, d_feed_canvas;
   PinnedHost h_feed_table;
   Event feed_copied;                        // the last table upload has left h_feed_table
-  bool track_history = true;                // order by the cost of each stream's previous launch (HT_TRACK_HISTORY=0: by window area)
   DevBuf d_track_cost;                      // [max_frames][2] {passes, window pixels / 256} per slot
   int track_heavy_div = 128;                // >0: the n/div costliest streams run on a cluster of
   int track_heavy_cluster = 8;              //     track_heavy_cluster CTAs on tier_stream[0] (HT_TRACK_HEAVY=div[,cluster])
   int track_mid_div = 32, track_mid_cluster = 4;  // HT_TRACK_MID=div[,cluster]: the next n/32 costliest streams on clusters of 4
-  double track_light_div = 0; int track_light_nt = 256;  // HT_TRACK_LIGHT=div[,threads]: the cheapest n/div streams (div may be fractional) on single CTAs
-  Stream tier_stream[4];                    // heavy, mid, light, rest (side 3: when tiers are on)
-  Event tier_done[4];
+  Stream tier_stream[3];                    // heavy, mid, rest (side 2: when tiers are on)
+  Event tier_done[3];
   int track_mask_frames = 4;                // >0: mask only streams whose last launch swept more than this many frames' worth of pixels
   int track_mask_min = 4;                   // HT_TRACK_MASK=<min n_calls> (0: off): zero-weight marking of the bin plane before k_track
-  int track_prio = 1;                       // HT_TRACK_PRIO=0: tier streams without priorities, the default tier on the context's stream
   Event sched_ready;
-  int track_bail_area = 0;                  // >0: two-phase k_track; phase A hands streams with a larger window (px) to phase B
-  DevBuf d_sched;                           // k_track two-phase scheduling scratch
-  unsigned sched_seq = 0;
+  DevBuf d_sched;                           // k_track launch-order scratch (k_track_area / k_track_rank)
 
   int fail(int code, const char *fmt, ...) {
     char buf[512];
@@ -753,7 +739,7 @@ int ensure_tracker_buffers(ht_ctx *ctx, cudaStream_t st) {
     CK(ctx->d_found.reserve(mf * sizeof(int32_t)));
     CK(ctx->d_objs.reserve(mf * 6 * sizeof(int32_t)));
     CK(ctx->d_windows.reserve(mf * 4 * sizeof(int32_t)));
-    CK(ctx->d_sched.reserve((2 * mf + 64) * sizeof(int32_t)));
+    CK(ctx->d_sched.reserve(2 * mf * sizeof(int32_t)));
     CK(ctx->d_track_cost.reserve(2 * mf * sizeof(int32_t)));
     CK(cudaMemsetAsync(ctx->d_track_cost.p, 0, 2 * mf * sizeof(int32_t), st));
     if (ctx->track_trace) {   // [mf x 4] per-stream records, then [mf x 8] phase totals (HT_TRACK_PASSTRACE builds)
@@ -778,13 +764,9 @@ int launch_hist(ht_ctx *ctx, cudaStream_t st, const uint8_t *d_rgba, int n, int 
   return HT_OK;
 }
 
-// k_track runs in two phases.  Phase A: one CTA per stream (no cluster overhead) — streams whose search window
-// outgrows bail_area stop and are queued.  Phase B: one 8-CTA cluster per queued stream finishes their calls.
-// Mean-shift is a serial chain of window passes per stream, so the few streams with large windows would
-// otherwise set the duration of the whole launch.
 using TrackKernel = void (*)(const uint16_t *, int, int, const int32_t *, const uint32_t *, const uint32_t *, TrackState *,
-                             int, int32_t *, int32_t *, int32_t *, unsigned long long *, int, int32_t *, int32_t *, int32_t *,
-                             int, int, unsigned long long *, size_t, int, int, int32_t *, const uint8_t *);
+                             int, int32_t *, int32_t *, int32_t *, unsigned long long *, const int32_t *, int,
+                             unsigned long long *, size_t, int, int, int32_t *, const uint8_t *);
 
 // The k_track instantiations the host picks from at run time: clusters of 1, 2, 4, 8 or 16 CTAs of 128, 256 or 512
 // threads.  Any other cluster size runs on clusters of 8, any other CTA size with 256 threads.
@@ -805,7 +787,7 @@ TrackKernel track_kernel(int c, int nt) {
 // the arguments of k_track that every launch of one launch_track call shares (the kernel's parameters, in order)
 struct TrackArgs {
   const uint16_t *bins; int w, h; const int32_t *slots; const uint32_t *mh, *ch; TrackState *state; int n_calls;
-  int32_t *objs, *win, *flag; unsigned long long *stats; int32_t *calls_done, *bail_list, *bail_count;
+  int32_t *objs, *win, *flag; unsigned long long *stats;
   unsigned long long *trace;   // HT_TRACK_TRACE=1: per-stream timeline buffer (else NULL)
   size_t trace_stride;         // u64 entries between a stream's record and its phase totals
   int memo;                    // ht_ctx::track_memo
@@ -814,8 +796,8 @@ struct TrackArgs {
   const uint8_t *enable;       // ht_stream_step: per stream, 0 = not tracking this frame (else NULL)
 };
 
-// k_track over n streams on clusters of c CTAs of nt threads
-cudaError_t launch_k_track(const TrackArgs &a, int c, int nt, cudaStream_t st, int n, int bail_area, int use_list, int list_off) {
+// k_track over n streams on clusters of c CTAs of nt threads: cluster k runs stream order[list_off + k] (order NULL: k)
+cudaError_t launch_k_track(const TrackArgs &a, int c, int nt, cudaStream_t st, int n, const int32_t *order, int list_off) {
   if (c != 1 && c != 2 && c != 4 && c != 16) c = 8;
   if (nt != 128 && nt != 512) nt = 256;
   cudaLaunchConfig_t cfg{};
@@ -828,7 +810,7 @@ cudaError_t launch_k_track(const TrackArgs &a, int c, int nt, cudaStream_t st, i
   attr[0].val.clusterDim.x = c; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr; cfg.numAttrs = 1;
   return cudaLaunchKernelEx(&cfg, track_kernel(c, nt), a.bins, a.w, a.h, a.slots, a.mh, a.ch, a.state, a.n_calls, a.objs,
-                            a.win, a.flag, a.stats, bail_area, a.calls_done, a.bail_list, a.bail_count, use_list, list_off,
+                            a.win, a.flag, a.stats, order, list_off,
                             a.trace, a.trace_stride, a.memo, a.force_serial, a.cost, a.enable);
 }
 
@@ -846,93 +828,68 @@ int launch_track(ht_ctx *ctx, cudaStream_t st, int n, int f0, const uint16_t *bi
                                                                      ctx->track_mask_frames > 0 ? ctx->d_track_cost.as<int32_t>() : nullptr, min_px256);
     ++ctx->launches;
   }
-  // per-chunk scheduling scratch: [calls_done | area n][bail_list | order n][bail_count 1]
-  int32_t *calls_done = ctx->d_sched.as<int32_t>() + (size_t)f0;
-  int32_t *bail_list = ctx->d_sched.as<int32_t>() + (size_t)ctx->cfg.max_frames + f0;
-  int32_t *bail_count = ctx->d_sched.as<int32_t>() + 2 * (size_t)ctx->cfg.max_frames + (ctx->sched_seq++ & 63);
   const TrackArgs args{bins, w, h, d_slots, mh, ch, state, n_calls, d_objs, d_win, flag,
-                       ctx->d_flags.as<unsigned long long>() + 8, calls_done, bail_list, bail_count,
+                       ctx->d_flags.as<unsigned long long>() + 8,
                        ctx->track_trace ? ctx->d_trace.as<unsigned long long>() + 4 * (size_t)f0 : nullptr,
                        // (the kernel indexes both areas with the stream number relative to f0)
                        4 * (size_t)ctx->cfg.max_frames - 4 * (size_t)f0 + 8 * (size_t)f0,
                        ctx->track_memo ? 1 : 0, (ctx->force_ties & 4) ? 1 : 0, ctx->d_track_cost.as<int32_t>(), enable};
   cudaError_t e = cudaSuccess;
-  if (ctx->track_bail_area > 0) {
-    // two-phase (HT_TRACK_BAIL=<px>): an A/B option; the single-phase launch below is the default
-    e = cudaMemsetAsync(bail_count, 0, sizeof(int32_t), st);
-    if (e != cudaSuccess) return ctx->fail(HT_ERR_CUDA, "memset: %s", cudaGetErrorString(e));
-    e = launch_k_track(args, 1, 256, st, n, ctx->track_bail_area, 0, 0);
-    if (e == cudaSuccess) e = launch_k_track(args, 8, 256, st, n, 0, 1, 0);
-    ctx->launches += 2;
+  // few streams -> 8 CTAs per stream (latency of one stream); many streams -> 2 (more streams resident).
+  int c = ctx->track_cluster;
+  if (c <= 0) c = (n >= 256) ? 2 : (n >= 32 ? 4 : 8);
+  if (n < 128) {                         // every stream is resident from the start
+    e = launch_k_track(args, c, ctx->track_nt, st, n, nullptr, 0);
+    ++ctx->launches;
   } else {
-    // few streams -> 8 CTAs per stream (latency of one stream); many streams -> 2 (more streams resident).
-    int c = ctx->track_cluster;
-    if (c <= 0) c = (n >= 256) ? 2 : (n >= 32 ? 4 : 8);
-    const int nt = ctx->track_nt;
-    const bool lpt = ctx->track_lpt && n >= 128;     // below that every stream is resident from the start
-    if (!lpt) {
-      e = launch_k_track(args, c, nt, st, n, 0, 0, 0);
-      ++ctx->launches;
-    } else {
-      // longest chain first: order the streams by search-window area (k_track_area / k_track_rank); optionally the
-      // n / track_heavy_div largest get a cluster of 8 on a second stream, concurrently with the others
-      k_track_area<<<(n + 255) / 256, 256, 0, st>>>(state, d_slots, n, ctx->track_history ? ctx->d_track_cost.as<int32_t>() : nullptr, calls_done);
-      k_track_rank<<<(n + 255) / 256, 256, 0, st>>>(calls_done, n, bail_list);
-      ctx->launches += 2;
-      // Tiers by cost rank, each on its own stream so that they run concurrently, costliest first:
-      //   the costliest n / heavy_div streams on clusters of 8 (long chains over large windows: shorten every pass),
-      //   the next n / mid_div on clusters of 4, the cheapest n / light_div on single CTAs (small windows, few passes:
-      //   no cluster barrier at all, and half the CTA slots), the rest on clusters of `c` (2).
-      struct Tier { int count, cluster, threads, side; };   // side >= 0: ctx->tier_stream[side]; -1: the context's stream
-      Tier tiers[4];
-      int n_tiers = 0, left = n;
-      auto take = [&](int div, int cl, int threads, int side) {
-        const int k = (div > 0) ? std::min(left, n / div) : 0;
-        if (k > 0) { tiers[n_tiers++] = Tier{k, cl, threads, side}; left -= k; }
-        return k;
-      };
-      take(ctx->track_heavy_div, ctx->track_heavy_cluster, 256, 0);
-      take(ctx->track_mid_div, ctx->track_mid_cluster, 256, 1);
-      const int n_light = (ctx->track_light_div > 0) ? std::min(left, (int)((double)n / ctx->track_light_div)) : 0;
-      // With the default tier on the context's own stream (no event wait) its CTAs would reach the GPU first and fill
-      // every slot with ITS costliest streams, and the heavy and middle tiers - the longest chains of the launch -
-      // would start late and set the end of the launch.  So every tier sits
-      // on a side stream behind the same event, submitted costliest tier first, and the side streams carry
-      // descending priorities (heavy > mid > rest > light), so a free slot always goes to the longest pending chain.
-      const bool rest_side = ctx->track_prio != 0 && (ctx->track_heavy_div > 0 || ctx->track_mid_div > 0);
-      if (left - n_light > 0) tiers[n_tiers++] = Tier{left - n_light, c, nt, rest_side ? 3 : -1};
-      if (n_light > 0) tiers[n_tiers++] = Tier{n_light, 1, ctx->track_light_nt, 2};
-      if (n_tiers > 1) {
-        int prio_least = 0, prio_greatest = 0;
-        CK(cudaDeviceGetStreamPriorityRange(&prio_least, &prio_greatest));   // numerically lower = more urgent
-        int prio_top = prio_greatest;
-        if (ctx->pipeline && ctx->pipe_bg) {   // background mode: every tier below the context's own stream
-          int pm = 0;
-          CK(cudaStreamGetPriority(ctx->stream, &pm));
-          prio_top = std::min(prio_least, pm + 1);
+    // longest chain first: order the streams by their cost in the previous launch (k_track_area / k_track_rank);
+    // per-chunk scratch: [area n][order n]
+    int32_t *area = ctx->d_sched.as<int32_t>() + (size_t)f0;
+    int32_t *order = ctx->d_sched.as<int32_t>() + (size_t)ctx->cfg.max_frames + f0;
+    k_track_area<<<(n + 255) / 256, 256, 0, st>>>(state, d_slots, n, ctx->d_track_cost.as<int32_t>(), area);
+    k_track_rank<<<(n + 255) / 256, 256, 0, st>>>(area, n, order);
+    ctx->launches += 2;
+    // Tiers by cost rank, each on its own stream so that they run concurrently, costliest first:
+    //   the costliest n / heavy_div streams on clusters of 8 (long chains over large windows: shorten every pass),
+    //   the next n / mid_div on clusters of 4, the rest on clusters of `c` (2).
+    struct Tier { int count, cluster, threads, side; };   // side >= 0: ctx->tier_stream[side]; -1: the context's stream
+    Tier tiers[3];
+    int n_tiers = 0, left = n;
+    auto take = [&](int div, int cl, int side) {
+      const int k = (div > 0) ? std::min(left, n / div) : 0;
+      if (k > 0) { tiers[n_tiers++] = Tier{k, cl, 256, side}; left -= k; }
+    };
+    take(ctx->track_heavy_div, ctx->track_heavy_cluster, 0);
+    take(ctx->track_mid_div, ctx->track_mid_cluster, 1);
+    // With the rest tier on the context's own stream (no event wait) its CTAs would reach the GPU first and fill
+    // every slot with ITS costliest streams, and the heavy and middle tiers - the longest chains of the launch -
+    // would start late and set the end of the launch.  So every tier sits on a side stream behind the same event,
+    // submitted costliest tier first, and the side streams carry descending priorities (heavy > mid > rest), so a
+    // free slot always goes to the longest pending chain.
+    const bool rest_side = ctx->track_heavy_div > 0 || ctx->track_mid_div > 0;
+    if (left > 0) tiers[n_tiers++] = Tier{left, c, ctx->track_nt, rest_side ? 2 : -1};
+    if (n_tiers > 1) {
+      int prio_least = 0, prio_greatest = 0;
+      CK(cudaDeviceGetStreamPriorityRange(&prio_least, &prio_greatest));   // numerically lower = more urgent
+      for (int t = 0; t < 3; ++t)
+        if (!ctx->tier_stream[t]) {
+          CK(cudaStreamCreateWithPriority(&ctx->tier_stream[t].h, cudaStreamNonBlocking, std::min(prio_least, prio_greatest + t)));
+          CK(cudaEventCreateWithFlags(&ctx->tier_done[t].h, cudaEventDisableTiming));
         }
-        for (int t = 0; t < 4; ++t)
-          if (!ctx->tier_stream[t]) {
-            const int rank = (t == 0) ? 0 : (t == 1 ? 1 : (t == 3 ? 2 : 3));   // heavy, mid, rest, light
-            const int prio = ctx->track_prio ? std::min(prio_least, prio_top + rank) : prio_least;
-            CK(cudaStreamCreateWithPriority(&ctx->tier_stream[t].h, cudaStreamNonBlocking, prio));
-            CK(cudaEventCreateWithFlags(&ctx->tier_done[t].h, cudaEventDisableTiming));
-          }
-        if (!ctx->sched_ready) CK(cudaEventCreateWithFlags(&ctx->sched_ready.h, cudaEventDisableTiming));
-        CK(cudaEventRecord(ctx->sched_ready, st));
-      }
-      int off = 0;
-      for (int t = 0; t < n_tiers && e == cudaSuccess; ++t) {
-        cudaStream_t ts = tiers[t].side >= 0 ? ctx->tier_stream[tiers[t].side] : st;
-        if (tiers[t].side >= 0) CK(cudaStreamWaitEvent(ts, ctx->sched_ready, 0));
-        e = launch_k_track(args, tiers[t].cluster, tiers[t].threads, ts, tiers[t].count, 0, 2, off);
-        ++ctx->launches;
-        if (tiers[t].side >= 0) CK(cudaEventRecord(ctx->tier_done[tiers[t].side], ts));
-        off += tiers[t].count;
-      }
-      for (int t = 0; t < n_tiers; ++t)
-        if (tiers[t].side >= 0) CK(cudaStreamWaitEvent(st, ctx->tier_done[tiers[t].side], 0));
+      if (!ctx->sched_ready) CK(cudaEventCreateWithFlags(&ctx->sched_ready.h, cudaEventDisableTiming));
+      CK(cudaEventRecord(ctx->sched_ready, st));
     }
+    int off = 0;
+    for (int t = 0; t < n_tiers && e == cudaSuccess; ++t) {
+      cudaStream_t ts = tiers[t].side >= 0 ? ctx->tier_stream[tiers[t].side] : st;
+      if (tiers[t].side >= 0) CK(cudaStreamWaitEvent(ts, ctx->sched_ready, 0));
+      e = launch_k_track(args, tiers[t].cluster, tiers[t].threads, ts, tiers[t].count, order, off);
+      ++ctx->launches;
+      if (tiers[t].side >= 0) CK(cudaEventRecord(ctx->tier_done[tiers[t].side], ts));
+      off += tiers[t].count;
+    }
+    for (int t = 0; t < n_tiers; ++t)
+      if (tiers[t].side >= 0) CK(cudaStreamWaitEvent(st, ctx->tier_done[tiers[t].side], 0));
   }
   if (e != cudaSuccess) return ctx->fail(HT_ERR_CUDA, "k_track launch: %s", cudaGetErrorString(e));
   return HT_OK;
@@ -957,14 +914,10 @@ int track_init_common(ht_ctx *ctx, cudaStream_t st, const int32_t *slots, int n,
 // Shared memory of one k_cascade CTA: the staged tile and three sets of per-class survivor bit masks.
 constexpr size_t CASC_SMEM = (size_t)TILE_WORDS * 4 + 3 * (size_t)MASK_WORDS * 32 * sizeof(uint32_t);
 constexpr size_t GRAY_HIST_SMEM = 2 * 4096 * sizeof(uint32_t);   // two frames per word, 16-bit counters
-// (ht_set_pipeline, background mode) dynamic shared memory that lets exactly THREE k_cascade CTAs share an SM and leaves
-// room for one k_track CTA (35.5 KB static): 4 x (57,600 + 1 KB reserved) > 228 KB, 3 x 58,624 + 36,480 <= 233,472
-constexpr size_t CASC_SMEM_BG = 57600;
-static_assert(CASC_SMEM <= CASC_SMEM_BG || HT_TILE_TH > 8, "background padding assumes the 32x8 tile");
 
 int set_kernel_attributes(ht_ctx *ctx) {
-  CK(cudaFuncSetAttribute(k_cascade<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max(CASC_SMEM, CASC_SMEM_BG)));
-  CK(cudaFuncSetAttribute(k_cascade<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max(CASC_SMEM, CASC_SMEM_BG)));
+  CK(cudaFuncSetAttribute(k_cascade<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CASC_SMEM));
+  CK(cudaFuncSetAttribute(k_cascade<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CASC_SMEM));
   CK(cudaFuncSetAttribute(k_cascade<true>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
   CK(cudaFuncSetAttribute(k_cascade<false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
   CK(cudaFuncSetAttribute(k_gray<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GRAY_HIST_SMEM));
@@ -1124,9 +1077,7 @@ int run_detect(ht_ctx *ctx, cudaStream_t st, Plan *P, const uint8_t *d_rgba_batc
     if (!P->casc_tiles.empty()) {
       ctx->prof_begin(HT_PROF_CASCADE, st);
       auto kern = ctx->hc.fast ? k_cascade<true> : k_cascade<false>;
-      // background mode: while the previous call's tracking is in flight, three cascade CTAs per SM instead of four
-      const size_t casc_smem = (before_group && ctx->pipe_bg) ? std::max(CASC_SMEM, CASC_SMEM_BG) : CASC_SMEM;
-      kern<<<dim3((unsigned)P->casc_tiles.size(), quads), CASCADE_THREADS, casc_smem, st>>>(
+      kern<<<dim3((unsigned)P->casc_tiles.size(), quads), CASCADE_THREADS, CASC_SMEM, st>>>(
           P->dplan, ctx->d_casc.as<LateFeat>(), ctx->d_casc.as<LateFeat>() + ctx->hc.n_sched, ctx->d_late_chunk0.as<int32_t>(),
           (ctx->use_tma && ctx->d_tmaps.p) ? ctx->d_tmaps.as<uint8_t>() + (piped ? (size_t)(wi & 1) : 0) * P->scales.size() * 128 : nullptr, 0,
           arena, P->arena_stride, nw,
@@ -1216,16 +1167,13 @@ int upload_chunks(ht_ctx *ctx, cudaStream_t st, const uint8_t *rgba, int n, size
 }
 
 // The aux stream of ht_detect_track and its events, made by whichever of its two users comes first.  The pipelined
-// path (ht_set_pipeline) makes it at the top priority, or just below the context's stream in background mode
-// (HT_PIPE_BG=1); the overlap of parts makes it at the default priority.
+// path (ht_set_pipeline) makes it at the top priority; the overlap of parts makes it at the default priority.
 int ensure_aux_stream(ht_ctx *ctx, bool pipelined) {
   if (ctx->aux_stream) return HT_OK;
   if (pipelined) {
-    int prio_least = 0, prio_greatest = 0, aux_prio = 0;
+    int prio_least = 0, prio_greatest = 0;
     CK(cudaDeviceGetStreamPriorityRange(&prio_least, &prio_greatest));
-    aux_prio = prio_greatest;
-    if (ctx->pipe_bg) { int pm = 0; CK(cudaStreamGetPriority(ctx->stream, &pm)); aux_prio = std::min(prio_least, pm + 1); }
-    CK(cudaStreamCreateWithPriority(&ctx->aux_stream.h, cudaStreamNonBlocking, aux_prio));
+    CK(cudaStreamCreateWithPriority(&ctx->aux_stream.h, cudaStreamNonBlocking, prio_greatest));
   } else {
     CK(cudaStreamCreateWithFlags(&ctx->aux_stream.h, cudaStreamNonBlocking));
   }
@@ -1279,25 +1227,15 @@ int ht_create(ht_ctx **out, const ht_config *cfg, const void *cascade_blob, size
     c->stream = c->created_stream;
   }
   if (const char *tc = getenv("HT_TRACK_CLUSTER")) c->track_cluster = atoi(tc);
-  if (const char *ba = getenv("HT_TRACK_BAIL")) c->track_bail_area = atoi(ba);
   if (const char *dp = getenv("HT_DETECT_PIPE")) c->detect_pipe = std::max(0, atoi(dp));
   if (const char *tm2 = getenv("HT_TRACK_MEMO")) c->track_memo = atoi(tm2) != 0;
   if (const char *tt = getenv("HT_TRACK_TRACE")) c->track_trace = atoi(tt) != 0;
   if (const char *tn = getenv("HT_TRACK_NT")) c->track_nt = (atoi(tn) == 128) ? 128 : (atoi(tn) == 512 ? 512 : 256);
-  if (const char *tl = getenv("HT_TRACK_LPT")) c->track_lpt = atoi(tl) != 0;
-  if (const char *thi = getenv("HT_TRACK_HISTORY")) c->track_history = atoi(thi) != 0;
   if (const char *th = getenv("HT_TRACK_HEAVY")) {
     c->track_heavy_div = std::max(0, atoi(th));
     if (const char *comma = strchr(th, ',')) {
       const int hc = atoi(comma + 1);
       if (hc == 1 || hc == 2 || hc == 4 || hc == 8 || hc == 16) c->track_heavy_cluster = hc;
-    }
-  }
-  if (const char *tli = getenv("HT_TRACK_LIGHT")) {
-    c->track_light_div = std::max(0.0, atof(tli));
-    if (const char *comma = strchr(tli, ',')) {
-      const int ln = atoi(comma + 1);
-      if (ln == 128 || ln == 256 || ln == 512) c->track_light_nt = ln;
     }
   }
   if (const char *tmid = getenv("HT_TRACK_MID")) {
@@ -1310,12 +1248,9 @@ int ht_create(ht_ctx **out, const ht_config *cfg, const void *cascade_blob, size
   if (const char *wv = getenv("HT_WAVE")) c->wave_frames = std::max(4, atoi(wv));
   if (const char *wm = getenv("HT_WAVE_MB")) c->wave_mb = std::max(1, atoi(wm));
   if (const char *tm = getenv("HT_TMA")) c->use_tma = atoi(tm) != 0;
-  if (HT_UNIBASE) c->use_tma = false;       // super-row tiles: a dense TMA box cannot be written into them
   if (const char *ov = getenv("HT_OVERLAP")) { c->overlap_track = atoi(ov) != 0 ? 1 : 0; c->overlap_parts = atoi(ov); }
   if (const char *hc2 = getenv("HT_H2D_CHUNK")) c->h2d_chunk = std::max(1, atoi(hc2));
   if (const char *pl = getenv("HT_PIPELINE")) c->pipeline = atoi(pl) != 0 ? 1 : 0;
-  if (const char *bg = getenv("HT_PIPE_BG")) c->pipe_bg = atoi(bg) != 0 ? 1 : 0;
-  if (const char *tp = getenv("HT_TRACK_PRIO")) c->track_prio = atoi(tp) != 0 ? 1 : 0;
   if (const char *tk = getenv("HT_TRACK_MASK")) {   // HT_TRACK_MASK=<min n_calls>[,<min frames swept>]  (0: off / 0: every stream)
     c->track_mask_min = std::max(0, atoi(tk));
     if (const char *comma = strchr(tk, ',')) c->track_mask_frames = std::max(0, atoi(comma + 1));
