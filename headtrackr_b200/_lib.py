@@ -70,6 +70,11 @@ class VideoFrame(C.Structure):
                 ("pitch", C.c_int32), ("now_ms", C.c_double)]
 
 
+class CanvasFrame(C.Structure):
+    """ht_canvas_frame: one stream's video frame and its own working canvas for ht_tracker_feed_canvases"""
+    _fields_ = [("video", VideoFrame), ("canvas_w", C.c_int32), ("canvas_h", C.c_int32), ("pad_", C.c_int32 * 2)]
+
+
 # headtrackrStatus names of ht_tracker_event.status, bit 0 first (= the order src/main.js dispatches them in)
 TRACKER_STATUS = ("whitebalance", "detecting", "hints", "redetecting", "lost", "stopped", "found")
 
@@ -110,7 +115,7 @@ _lib = None
 
 EXPORTS = ["ht_version", "ht_create", "ht_destroy", "ht_last_error", "ht_sync", "ht_max_rects", "ht_detect",
            "ht_track_init", "ht_track_init_from_detect", "ht_track", "ht_detect_track", "ht_stream_reset", "ht_stream_step", "ht_stream_head_config", "ht_stream_step_head",
-           "ht_tracker_config", "ht_tracker_reset", "ht_tracker_start", "ht_tracker_stop", "ht_tracker_step", "ht_tracker_feed", "ht_ingest", "ht_backprojection", "ht_whitebalance",
+           "ht_tracker_config", "ht_tracker_reset", "ht_tracker_start", "ht_tracker_stop", "ht_tracker_step", "ht_tracker_feed", "ht_tracker_set_params", "ht_tracker_feed_canvases", "ht_ingest", "ht_backprojection", "ht_whitebalance",
            "ht_plan_info", "ht_debug_plane", "ht_debug_raw", "ht_debug_model_hist", "ht_debug_track_stats", "ht_set_track_memo", "ht_set_pipeline", "ht_join", "ht_debug_set_exactness", "ht_debug_track_trace", "ht_debug_track_phases", "ht_launch_count",
            "ht_profile", "ht_profile_read"]
 
@@ -151,6 +156,8 @@ def lib():
         f.argtypes = [vp, C.c_int, C.c_int]
     L.ht_tracker_step.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, C.c_double, vp]
     L.ht_tracker_feed.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp]
+    L.ht_tracker_set_params.argtypes = [vp, C.c_int, C.c_int, vp]
+    L.ht_tracker_feed_canvases.argtypes = [vp, vp, C.c_int, C.c_int, vp]
     L.ht_ingest.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, vp, C.c_int, C.c_int]
     L.ht_backprojection.argtypes = [vp, C.c_int, vp, C.c_int, C.c_int, vp]
     L.ht_whitebalance.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, vp]

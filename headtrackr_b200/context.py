@@ -8,7 +8,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from ._lib import (HeadEvent, HeadParams, HtError, Rect, StreamEvent, TrackerEvent, TrackerParams, TrackObj, VideoFrame,
+from ._lib import (CanvasFrame, HeadEvent, HeadParams, HtError, Rect, StreamEvent, TrackerEvent, TrackerParams, TrackObj, VideoFrame,
                    Window)
 from .synth import load_cascade_blob
 
@@ -228,10 +228,17 @@ class Context:
         if not enable:
             self._check(self._L.ht_tracker_config(self._h, None))
             return
-        head = HeadParams(int(bool(smoothing)), int(bool(headPosition)), int(bool(edgecorrection)), 0, alpha,
-                          float(fov) if fov is not None else 0.0, cameraOffset, distance_to_screen)
-        p = TrackerParams(int(bool(retryDetection)), int(bool(calcAngles)), (C.c_int32 * 2)(), head)
+        p = tracker_params(retryDetection, calcAngles, smoothing, fov, cameraOffset, headPosition, edgecorrection, alpha,
+                           distance_to_screen)
         self._check(self._L.ht_tracker_config(self._h, C.addressof(p)))
+
+    def tracker_set_params(self, first, params):
+        """Parameters of streams first, first+1, ...: one dict of tracker_config's keywords (enable excluded) per stream,
+        each its own `new headtrackr.Tracker(params)`.  Stream states are kept; calcAngles takes effect at the stream's
+        next hand-off to camshift, the other fields at its next tick.  tracker_config() sets every stream again."""
+        params = list(params)
+        arr = (TrackerParams * max(1, len(params)))(*[tracker_params(**d) for d in params])
+        self._check(self._L.ht_tracker_set_params(self._h, int(first), len(params), C.addressof(arr)))
 
     def tracker_reset(self, first=0, n=None):
         """Streams [first, first+n): a new headtrackr.Tracker, initialised, not running."""
@@ -261,8 +268,9 @@ class Context:
         0, width, height) onto the working canvas, then what tracker_step does for that stream.  Unlisted streams do
         not tick.  streams: distinct stream ids; frames: one (h, w, 4) u8 video frame per stream, all numpy arrays or
         all torch CUDA tensors (any size; a row-padded view - last two strides (4, 1) - passes its row stride as the
-        pitch); now_ms: one clock for all or one per record.  -> event dicts in record order; with a torch CUDA `out`
-        tensor of len(streams)*144 bytes: asynchronous, nothing returned."""
+        pitch); now_ms: one clock for all or one per record; width, height: one canvas for all (ht_tracker_feed) or one
+        size per record (ht_tracker_feed_canvases: each stream on its own canvas).  -> event dicts in record order;
+        with a torch CUDA `out` tensor of len(streams)*144 bytes: asynchronous, nothing returned."""
         streams = list(streams)
         n = len(frames)
         if len(streams) != n or n == 0:
@@ -270,6 +278,12 @@ class Context:
         clocks = [float(t) for t in now_ms] if hasattr(now_ms, "__len__") else [float(now_ms)] * n
         if len(clocks) != n:
             raise ValueError("one clock per listed stream")
+        per_record = hasattr(width, "__len__") or hasattr(height, "__len__")
+        if per_record:
+            widths = [int(v) for v in width] if hasattr(width, "__len__") else [int(width)] * n
+            heights = [int(v) for v in height] if hasattr(height, "__len__") else [int(height)] * n
+            if len(widths) != n or len(heights) != n:
+                raise ValueError("one canvas width and height per listed stream")
         on_device = _is_torch(frames[0])
         recs = (VideoFrame * n)()
         keep = []
@@ -290,12 +304,15 @@ class Context:
                 f = a
             keep.append(f)
             recs[b] = VideoFrame(ptr, int(k), f.shape[1], f.shape[0], pitch, clocks[b])
+        ev = None if out is not None else (TrackerEvent * n)()
+        dst = out.data_ptr() if out is not None else C.addressof(ev)
+        if per_record:
+            crecs = (CanvasFrame * n)(*[CanvasFrame(recs[b], widths[b], heights[b]) for b in range(n)])
+            self._check(self._L.ht_tracker_feed_canvases(self._h, C.addressof(crecs), n, int(on_device), dst))
+        else:
+            self._check(self._L.ht_tracker_feed(self._h, C.addressof(recs), n, int(on_device), width, height, dst))
         if out is not None:
-            self._check(self._L.ht_tracker_feed(self._h, C.addressof(recs), n, int(on_device), width, height,
-                                                out.data_ptr()))
             return None
-        ev = (TrackerEvent * n)()
-        self._check(self._L.ht_tracker_feed(self._h, C.addressof(recs), n, int(on_device), width, height, C.addressof(ev)))
         return [tracker_event_dict(e) for e in ev]
 
     def ingest(self, frames, width, height, out=None):
@@ -384,6 +401,14 @@ class Context:
         out = np.zeros(4096, np.uint32)
         self._check(self._L.ht_debug_model_hist(self._h, slot, out.ctypes.data))
         return out
+
+
+def tracker_params(retryDetection=True, calcAngles=False, smoothing=True, fov=None, cameraOffset=11.5, headPosition=True,
+                   edgecorrection=True, alpha=0.35, distance_to_screen=60.0):
+    """ht_tracker_params from the reference's parameter names (src/main.js:39-55)"""
+    head = HeadParams(int(bool(smoothing)), int(bool(headPosition)), int(bool(edgecorrection)), 0, alpha,
+                      float(fov) if fov is not None else 0.0, cameraOffset, distance_to_screen)
+    return TrackerParams(int(bool(retryDetection)), int(bool(calcAngles)), (C.c_int32 * 2)(), head)
 
 
 def tracker_event_dict(e):

@@ -566,11 +566,12 @@ struct ht_ctx {
   DevBuf d_stream_mode, d_stream_mask, d_stream_cs, d_stream_init, d_stream_events;   // ht_stream_step
   DevBuf d_head_state, d_head_params, d_head_events;                                  // ht_stream_head_config
   bool head_on = false;
-  DevBuf d_tracker_state, d_tracker_params, d_tracker_events, d_tracker_wb;          // ht_tracker_config
+  // ht_tracker_config: per stream its state, its TrackerParams (ht_tracker_set_params), its event, its whitebalance flag
+  DevBuf d_tracker_state, d_tracker_params, d_tracker_events, d_tracker_wb;
   bool tracker_on = false;
-  int tracker_calc_angles = 0;
-  // ht_tracker_feed: the record table {ids[n], clocks[n], FeedRec[n]} goes up in one copy from pinned memory; the
-  // videos are drawn into the canvas arena ([max_frames] canvases, indexed by record), zeroed when allocated
+  // ht_tracker_feed(_canvases): the record table {ids[n], clocks[n], FeedRec[n], EntryCanvas[n], tile starts[n+1]}
+  // goes up in one copy from pinned memory; the videos are drawn into the canvas arena (batch entry k's canvas at
+  // EntryCanvas::base), zeroed when it grows
   DevBuf d_feed_table, d_feed_draw, d_feed_canvas;
   PinnedHost h_feed_table;
   Event feed_copied;                        // the last table upload has left h_feed_table
@@ -998,9 +999,13 @@ struct HistOut {
 // cascade of wave w.
 int run_detect(ht_ctx *ctx, cudaStream_t st, Plan *P, const uint8_t *d_rgba_batch, int f0, int n, int min_neighbors,
                Rect *d_rects_batch, int32_t *d_counts_batch, HistOut ho = HistOut{nullptr, nullptr},
-               const uint8_t *quad_mask = nullptr, cudaEvent_t before_group = nullptr) {
+               const uint8_t *quad_mask = nullptr, cudaEvent_t before_group = nullptr,
+               const uint8_t *frames_f0 = nullptr) {
   const int w = P->w, h = P->h;
   const size_t frame_bytes = (size_t)w * h * 4;
+  // frame f0 + k is at frames_f0 + k frames (ht_tracker_feed: a canvas-size group's block of the arena); by default
+  // every per-frame input is indexed by absolute frame number
+  if (!frames_f0) frames_f0 = d_rgba_batch + (size_t)f0 * frame_bytes;
   // frames per wave: HT_WAVE, or as many as fit the arena budget (one frame of a quad costs arena_stride bytes)
   const int wave = ctx->wave_frames > 0 ? std::max(4, ctx->wave_frames & ~3)
                                         : std::max(4, (int)std::min<size_t>(((size_t)ctx->wave_mb << 20) / P->arena_stride, 1u << 20) & ~3);
@@ -1030,12 +1035,12 @@ int run_detect(ht_ctx *ctx, cudaStream_t st, Plan *P, const uint8_t *d_rgba_batc
     CK(cudaEventRecord(ctx->pipe_start, st));
     CK(cudaStreamWaitEvent(ctx->pipe_stream, ctx->pipe_start, 0));
   }
-  const bool vec = (w % 4 == 0) && ((reinterpret_cast<uintptr_t>(d_rgba_batch) & 15u) == 0);
+  const bool vec = (w % 4 == 0) && ((reinterpret_cast<uintptr_t>(frames_f0) & 15u) == 0);
   int wi = 0;
   for (int w0 = 0; w0 < n; w0 += wave, ++wi) {
     const int nw = std::min(wave, n - w0), fa = f0 + w0, quads = (nw + 3) / 4;
     uint32_t *arena = ctx->arena.as<uint32_t>() + (piped ? (size_t)(wi & 1) * wave_words : 0);
-    const uint8_t *d_rgba = d_rgba_batch + (size_t)fa * frame_bytes;
+    const uint8_t *d_rgba = frames_f0 + (size_t)w0 * frame_bytes;
     const uint8_t *qm = quad_mask ? quad_mask + w0 / 4 : nullptr;   // (ht_stream_step) quads of this wave that have work
     cudaStream_t ps = piped ? ctx->pipe_stream : st;
     if (piped && wi >= 2) CK(cudaStreamWaitEvent(ps, ctx->pipe_events[2 + (wi & 1)], 0));   // cascade of wave wi-2 is done with this arena
@@ -1187,7 +1192,7 @@ int ensure_aux_stream(ht_ctx *ctx, bool pipelined) {
 // ================================================================================================
 extern "C" {
 
-uint32_t ht_version(void) { return (1u << 16) | 2u; }
+uint32_t ht_version(void) { return (1u << 16) | 3u; }
 
 const char *ht_last_error(const ht_ctx *ctx) { return ctx ? ctx->err.c_str() : g_create_error.c_str(); }
 
@@ -1604,7 +1609,7 @@ static int ensure_stream_buffers(ht_ctx *ctx, cudaStream_t st) {
   if (!ctx->d_stream_mode.p) {
     CK(ctx->d_stream_mode.reserve(mf * sizeof(int32_t)));
     CK(cudaMemsetAsync(ctx->d_stream_mode.p, 0, mf * sizeof(int32_t), st));   // every stream starts in "VJ"
-    CK(ctx->d_stream_mask.reserve((mf + 3) / 4 + 16));
+    CK(ctx->d_stream_mask.reserve(mf + 16));   // quads: (mf + 3) / 4, or up to mf over the canvas groups of a feed
     CK(ctx->d_stream_cs.reserve(mf));
     CK(ctx->d_stream_init.reserve(mf));
     CK(ctx->d_stream_events.reserve(mf * sizeof(StreamEvent)));
@@ -1718,6 +1723,10 @@ static int tracker_control(ht_ctx *ctx, int first, int n, int op) {
   return HT_OK;
 }
 
+static bool tracker_params_ok(const ht_tracker_params &p) {
+  return p.head.alpha >= 0.0 && p.head.alpha <= 1.0 && p.head.distance_to_screen > 0.0;
+}
+
 int ht_tracker_config(ht_ctx *ctx, const ht_tracker_params *params) {
   if (!ctx) return HT_ERR_ARG;
   { const int jr = join_aux(ctx); if (jr != HT_OK) return jr; }
@@ -1735,24 +1744,42 @@ int ht_tracker_config(ht_ctx *ctx, const ht_tracker_params *params) {
     }
     return HT_OK;
   }
-  const ht_head_params &hp = params->head;
-  if (!(hp.alpha >= 0.0 && hp.alpha <= 1.0) || !(hp.distance_to_screen > 0.0)) return ctx->fail(HT_ERR_ARG, "bad head parameters");
+  if (!tracker_params_ok(*params)) return ctx->fail(HT_ERR_ARG, "bad head parameters");
   if (!ctx->d_tracker_state.p) {
     CK(ctx->d_tracker_state.reserve(mf * sizeof(TrackerState)));
-    CK(ctx->d_tracker_params.reserve(sizeof(TrackerParams)));
+    CK(ctx->d_tracker_params.reserve(mf * sizeof(TrackerParams)));
     CK(ctx->d_tracker_events.reserve(mf * sizeof(TrackerEvent)));
     CK(ctx->d_tracker_wb.reserve(mf));
   }
-  const TrackerParams tp = make_tracker_params(params);
-  CK(cudaMemcpyAsync(ctx->d_tracker_params.p, &tp, sizeof(tp), cudaMemcpyHostToDevice, ctx->stream));
+  const std::vector<TrackerParams> tp(mf, make_tracker_params(params));   // every stream: per-stream values are discarded
+  CK(cudaMemcpyAsync(ctx->d_tracker_params.p, tp.data(), mf * sizeof(TrackerParams), cudaMemcpyHostToDevice, ctx->stream));
   if (!ctx->tracker_on) {
     k_tracker_control<<<(unsigned)((mf + 127) / 128), 128, 0, ctx->stream>>>(ctx->d_tracker_state.as<TrackerState>(), 0, (int)mf, 0);
     ++ctx->launches;
     CK(cudaGetLastError());
   }
   CK(cudaStreamSynchronize(ctx->stream));    // `tp` is a local
-  ctx->tracker_calc_angles = params->calc_angles ? 1 : 0;
   ctx->tracker_on = true;
+  return HT_OK;
+}
+
+// The parameters of streams [first, first + n), each its own headtrackr.Tracker's.  Stream states are kept; calcAngles
+// reaches a stream at its next initTracker (k_track_init reads it per entry), the rest at its next tick.
+int ht_tracker_set_params(ht_ctx *ctx, int first, int n, const ht_tracker_params *params) {
+  if (!ctx) return HT_ERR_ARG;
+  if (!ctx->tracker_on) return ctx->fail(HT_ERR_STATE, "ht_tracker_config has not been called");
+  const int mf = ctx->cfg.max_frames;
+  if (first < 0 || n <= 0 || first > mf - n) return ctx->fail(HT_ERR_ARG, "stream range outside [0,%d)", mf);
+  if (!params) return ctx->fail(HT_ERR_ARG, "params is NULL");
+  for (int i = 0; i < n; ++i)
+    if (!tracker_params_ok(params[i])) return ctx->fail(HT_ERR_ARG, "record %d: bad head parameters", i);
+  { const int jr = join_aux(ctx); if (jr != HT_OK) return jr; }
+  CK(cudaSetDevice(ctx->cfg.device));
+  std::vector<TrackerParams> tp((size_t)n);
+  for (int i = 0; i < n; ++i) tp[(size_t)i] = make_tracker_params(params + i);
+  CK(cudaMemcpyAsync(ctx->d_tracker_params.as<TrackerParams>() + first, tp.data(), (size_t)n * sizeof(TrackerParams),
+                     cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));    // `tp` is a local
   return HT_OK;
 }
 
@@ -1760,71 +1787,103 @@ int ht_tracker_reset(ht_ctx *ctx, int first, int n) { return tracker_control(ctx
 int ht_tracker_start(ht_ctx *ctx, int first, int n) { return tracker_control(ctx, first, n, 1); }
 int ht_tracker_stop(ht_ctx *ctx, int first, int n) { return tracker_control(ctx, first, n, 2); }
 
-// The video draw of ht_tracker_feed: record table, per-record draw flags (written by k_tracker_plan), canvas constants.
+// The video draw of ht_tracker_feed: record table, per-record draw flags (written by k_tracker_plan), canvas constants
+// (one canvas size), or the flattened tile list of mixed sizes (tile_start [n + 1], `tiles` in all).
 struct FeedDraw {
   const FeedRec *recs;
   uint8_t *draw;
   IngestGeom g;
+  const int32_t *tile_start;
+  int tiles;
+};
+
+// One canvas size of a tracker tick: batch entries [k0, k0 + n) on canvases of w x h (plan P) at frames (n consecutive
+// canvases); their bin planes start px0 pixels into ctx->bins, their VJ frame quads at quad q0 of the mask.
+struct TickGroup {
+  Plan *P;
+  int k0, n, w, h, q0;
+  const uint8_t *frames;
+  size_t px0;
 };
 
 // One timer tick of n headtrackr.Tracker streams, entirely on the device (shared by ht_tracker_step and
-// ht_tracker_feed).  d_rgba: n canvases of w x h; batch entry k is stream d_ids[k] (NULL: stream k) and ticks at
-// d_now[k] (NULL: every entry at now_ms).
+// ht_tracker_feed).  Batch entry k is stream d_ids[k] (NULL: stream k) and ticks at d_now[k] (NULL: every entry at
+// now_ms).  The entries form n_groups canvas-size groups; geo (NULL with one group) gives each entry's canvas in
+// d_rgba.  The kernels that are planned per geometry run once per group, as on an ordinary uniform batch; the
+// per-stream kernels once per call.
 //   k_tracker_plan   modes -> VJ frame-quad mask, CS enable, whitebalance enable (feed: draw flags)
 //   k_feed_draw      (feed) drawImage(video, 0, 0, w, h) of every stream that is not IDLE   src/main.js:170,312
 //   k_wb_sums        whitebalance sums of the STARTING and WB streams only       src/whitebalance.js, src/main.js:316
-//   run_detect       the VJ streams (interval 5, min_neighbors 1)                 src/facetrackr.js:147-149
-//   k_hist, k_track  one track() of the CS streams                                src/camshift.js:213-312
+//   run_detect       per group: the VJ streams (interval 5, min_neighbors 1)     src/facetrackr.js:147-149
+//   k_hist, k_track  per group: one track() of the CS streams                    src/camshift.js:213-312
 //   k_tracker_update starter, whitebalance gate, facetrackr and main.js transitions, status bits, head epilogue
 //   k_track_init     initTracker for the streams that found their face           src/facetrackr.js:97-108
-static int tracker_tick(ht_ctx *ctx, Plan *P, const uint8_t *d_rgba, int n, int w, int h, const int32_t *d_ids,
-                        double now_ms, const double *d_now, const FeedDraw *feed, ht_tracker_event *out) {
+static int tracker_tick(ht_ctx *ctx, const TickGroup *grp, int n_groups, const uint8_t *d_rgba, int n, const int32_t *d_ids,
+                        double now_ms, const double *d_now, const FeedDraw *feed, const EntryCanvas *geo,
+                        ht_tracker_event *out) {
   cudaStream_t st = ctx->stream;
   int rc = ensure_tracker_buffers(ctx, st);
   if (rc != HT_OK) return rc;
   rc = ensure_stream_buffers(ctx, st);       // the mask scratch of ht_stream_step (the two never run on one context at once)
   if (rc != HT_OK) return rc;
-  CK(ctx->bins.reserve((size_t)n * w * h * sizeof(uint16_t)));
+  const TickGroup &g0 = grp[0], &gl = grp[n_groups - 1];
+  CK(ctx->bins.reserve((gl.px0 + (size_t)gl.n * gl.w * gl.h) * sizeof(uint16_t)));
   CK(ctx->d_wb_sums.reserve((size_t)ctx->cfg.max_frames * 3 * sizeof(unsigned long long)));
   TrackerState *ts = ctx->d_tracker_state.as<TrackerState>();
   uint8_t *vj_mask = ctx->d_stream_mask.as<uint8_t>(), *cs_en = ctx->d_stream_cs.as<uint8_t>(), *init_en = ctx->d_stream_init.as<uint8_t>();
   uint8_t *wb_en = ctx->d_tracker_wb.as<uint8_t>();
-  k_tracker_plan<<<(n + 127) / 128, 128, 0, st>>>(ts, d_ids, n, vj_mask, cs_en, init_en, wb_en, feed ? feed->draw : nullptr);
+  k_tracker_plan<<<(n + 127) / 128, 128, 0, st>>>(ts, d_ids, n, vj_mask, cs_en, init_en, wb_en, feed ? feed->draw : nullptr, geo);
   if (feed) {
-    const int tiles_x = (w + 63) / 64, tiles = tiles_x * ((h + 15) / 16);
-    k_feed_draw<<<dim3((unsigned)tiles, (unsigned)n), 256, 0, st>>>(feed->recs, feed->draw, const_cast<uint8_t *>(d_rgba),
-                                                                    feed->g, tiles_x);
+    uint8_t *canvas = const_cast<uint8_t *>(d_rgba);
+    if (!feed->tile_start) {
+      const int tiles_x = (g0.w + 63) / 64, tiles = tiles_x * ((g0.h + 15) / 16);
+      k_feed_draw<<<dim3((unsigned)tiles, (unsigned)n), 256, 0, st>>>(feed->recs, feed->draw, canvas, feed->g, tiles_x,
+                                                                      nullptr, nullptr, n);
+    } else {
+      k_feed_draw<<<(unsigned)feed->tiles, 256, 0, st>>>(feed->recs, feed->draw, canvas, feed->g, 0, geo, feed->tile_start, n);
+    }
     ++ctx->launches;
   }
   CK(cudaMemsetAsync(ctx->d_wb_sums.p, 0, (size_t)n * 3 * sizeof(unsigned long long), st));
   const int chunks = std::min(64, std::max(1, 8 * ctx->sms / n));
-  k_wb_sums<<<dim3(chunks, n), 256, 0, st>>>(d_rgba, (size_t)w * h * 4, w * h, ctx->d_wb_sums.as<unsigned long long>(), chunks, wb_en);
+  const size_t frame_bytes = (size_t)g0.w * g0.h * 4;   // (one group; geo has each entry's canvas otherwise)
+  k_wb_sums<<<dim3(chunks, n), 256, 0, st>>>(d_rgba, frame_bytes, g0.w * g0.h, ctx->d_wb_sums.as<unsigned long long>(), chunks,
+                                             wb_en, geo);
   ctx->launches += 2;
-  rc = run_detect(ctx, st, P, d_rgba, 0, n, 1, ctx->d_out_rects.as<Rect>(), ctx->d_out_counts.as<int32_t>(),
-                  HistOut{nullptr, nullptr}, vj_mask);
-  if (rc != HT_OK) return rc;
-  rc = launch_hist(ctx, st, d_rgba, n, w, h, ctx->cur_hist.as<uint32_t>(), ctx->bins.as<uint16_t>(), cs_en);
-  if (rc != HT_OK) return rc;
-  ctx->prof_begin(HT_PROF_TRACK, st);
-  rc = launch_track(ctx, st, n, 0, ctx->bins.as<uint16_t>(), w, h, d_ids, ctx->model_hist.as<uint32_t>(),
-                    ctx->cur_hist.as<uint32_t>(), ctx->track_state.as<TrackState>(), 1, ctx->d_objs.as<int32_t>(), nullptr,
-                    ctx->d_flags.as<int32_t>() + 2, cs_en);
-  if (rc != HT_OK) return rc;
-  ctx->prof_end(st);
+  for (int i = 0; i < n_groups; ++i) {
+    const TickGroup &G = grp[i];
+    rc = run_detect(ctx, st, G.P, d_rgba, G.k0, G.n, 1, ctx->d_out_rects.as<Rect>(), ctx->d_out_counts.as<int32_t>(),
+                    HistOut{nullptr, nullptr}, vj_mask + G.q0, nullptr, G.frames);
+    if (rc != HT_OK) return rc;
+  }
+  for (int i = 0; i < n_groups; ++i) {
+    const TickGroup &G = grp[i];
+    uint32_t *ch = ctx->cur_hist.as<uint32_t>() + (size_t)G.k0 * 4096;
+    uint16_t *bins = ctx->bins.as<uint16_t>() + G.px0;
+    rc = launch_hist(ctx, st, G.frames, G.n, G.w, G.h, ch, bins, cs_en + G.k0);
+    if (rc != HT_OK) return rc;
+    ctx->prof_begin(HT_PROF_TRACK, st);
+    rc = launch_track(ctx, st, G.n, G.k0, bins, G.w, G.h, d_ids ? d_ids + G.k0 : nullptr, ctx->model_hist.as<uint32_t>(), ch,
+                      ctx->track_state.as<TrackState>(), 1, ctx->d_objs.as<int32_t>() + 6 * (size_t)G.k0, nullptr,
+                      ctx->d_flags.as<int32_t>() + 2, cs_en + G.k0);
+    if (rc != HT_OK) return rc;
+    ctx->prof_end(st);
+  }
   Outputs io(ctx);
   TrackerEvent *d_ev = io.out<TrackerEvent>(out, ctx->d_tracker_events, sizeof(TrackerEvent) * (size_t)n);
   k_tracker_update<<<(n + 127) / 128, 128, 0, st>>>(ts, d_ids, ctx->d_tracker_params.as<TrackerParams>(), n,
-                                                    ctx->d_wb_sums.as<unsigned long long>(), w * h, ctx->d_best.as<Rect>(),
+                                                    ctx->d_wb_sums.as<unsigned long long>(), g0.w * g0.h, ctx->d_best.as<Rect>(),
                                                     ctx->d_out_counts.as<int32_t>(), ctx->d_objs.as<int32_t>(),
-                                                    ctx->d_rects.as<int32_t>(), init_en, now_ms, d_now, w, h, d_ev);
+                                                    ctx->d_rects.as<int32_t>(), init_en, now_ms, d_now, g0.w, g0.h, geo, d_ev);
   ctx->prof_begin(HT_PROF_TRACK_INIT, st);
-  k_track_init<<<n, 256, 0, st>>>(d_rgba, (size_t)w * h * 4, w, h, d_ids, ctx->d_rects.as<int32_t>(), ctx->tracker_calc_angles,
-                                  ctx->model_hist.as<uint32_t>(), ctx->track_state.as<TrackState>(), nullptr, init_en);
+  // calc_angles -1: each entry's own, from its stream's parameters (k_tracker_update)
+  k_track_init<<<n, 256, 0, st>>>(d_rgba, frame_bytes, g0.w, g0.h, d_ids, ctx->d_rects.as<int32_t>(), -1,
+                                  ctx->model_hist.as<uint32_t>(), ctx->track_state.as<TrackState>(), nullptr, init_en, geo);
   ctx->prof_end(st);
   ctx->launches += 2;
   CK(cudaGetLastError());
-  ctx->last_plan = P;
-  ctx->last_n = n;
+  ctx->last_plan = gl.P;
+  ctx->last_n = gl.n;
   return io.finish(Outputs::SYNC_FLAGS);
 }
 
@@ -1841,19 +1900,34 @@ int ht_tracker_step(ht_ctx *ctx, const uint8_t *rgba, int n, int w, int h, doubl
   const uint8_t *d_rgba = nullptr;
   rc = stage_frames(ctx, ctx->stream, rgba, n, w, h, &d_rgba);
   if (rc != HT_OK) return rc;
-  return tracker_tick(ctx, P, d_rgba, n, w, h, nullptr, now_ms, nullptr, nullptr, out);
+  const TickGroup G{P, 0, n, w, h, 0, d_rgba, 0};
+  return tracker_tick(ctx, &G, 1, d_rgba, n, nullptr, now_ms, nullptr, nullptr, nullptr, out);
 }
 
 static_assert(sizeof(ht_video_frame) == 32 && sizeof(FeedRec) == sizeof(ht_video_frame), "ht_video_frame layout");
 static_assert(offsetof(ht_video_frame, now_ms) == offsetof(FeedRec, now_ms) && offsetof(ht_video_frame, pitch) == offsetof(FeedRec, pitch),
               "ht_video_frame layout");
+static_assert(sizeof(ht_canvas_frame) == 48 && offsetof(ht_canvas_frame, canvas_w) == 32, "ht_canvas_frame layout");
 
-// One timer tick of each listed stream on its own video and clock.  Everything is checked before anything is enqueued;
-// then ONE host-to-device copy carries the record table {stream ids, clocks, FeedRec with device pointers and resolved
-// pitches} from pinned memory, and tracker_tick draws the videos of the streams that are not IDLE into the canvas arena
-// (batch entry b = record b) before the kernels of ht_tracker_step run on it through the stream ids.
-int ht_tracker_feed(ht_ctx *ctx, const ht_video_frame *frames, int n, int frames_on_device, int canvas_w, int canvas_h,
-                    ht_tracker_event *out) {
+// drawImage's canvas constants for w x h (false: too large for the 32-bit numerators)
+static bool canvas_geom(int w, int h, IngestGeom &g) {
+  g = IngestGeom{0, 0, w, h, 0, 0, 0};
+  if (!bilinear_division_constants(4ull * w * h, g.magic, g.shift)) return false;
+  g.half = (uint32_t)(2ull * w * h);
+  return true;
+}
+
+// ht_tracker_feed(_canvases).  Everything is checked before anything is enqueued (one_canvas: every record is on the
+// same canvas and the canvas errors are ht_tracker_feed's, without a record index).  The records are grouped by canvas
+// size - groups in order of first appearance, records in order within a group - and batch entry k is the k-th record
+// of that order.  Each group's canvases are a contiguous block of the canvas arena (256-byte aligned), so every kernel
+// planned per geometry sees an ordinary uniform batch.  Then ONE host-to-device copy carries the record table {stream
+// ids, clocks, FeedRec with device pointers and resolved pitches, and with several sizes EntryCanvas and the tile
+// starts} from pinned memory, and tracker_tick draws the videos of the streams that are not IDLE into the arena before
+// the kernels of ht_tracker_step run on it through the stream ids.  With one canvas size the launches are those of one
+// uniform batch.
+static int tracker_feed(ht_ctx *ctx, const ht_canvas_frame *frames, int n, int frames_on_device, bool one_canvas,
+                        ht_tracker_event *out) {
   if (!ctx) return HT_ERR_ARG;
   if (!ctx->tracker_on) return ctx->fail(HT_ERR_STATE, "ht_tracker_config has not been called");
   if (!frames || !out) return ctx->fail(HT_ERR_ARG, "frames or out is NULL");
@@ -1861,7 +1935,7 @@ int ht_tracker_feed(ht_ctx *ctx, const ht_video_frame *frames, int n, int frames
   if (n <= 0 || n > mf) return ctx->fail(HT_ERR_ARG, "n=%d outside [1,%d]", n, mf);
   std::vector<uint8_t> seen((size_t)mf, 0);
   for (int b = 0; b < n; ++b) {
-    const ht_video_frame &f = frames[b];
+    const ht_video_frame &f = frames[b].video;
     if (f.stream < 0 || f.stream >= mf) return ctx->fail(HT_ERR_ARG, "record %d: stream %d outside [0,%d)", b, f.stream, mf);
     if (seen[(size_t)f.stream]++) return ctx->fail(HT_ERR_ARG, "record %d: stream %d is listed twice", b, f.stream);
     if (!f.rgba) return ctx->fail(HT_ERR_ARG, "record %d: rgba is NULL", b);
@@ -1871,26 +1945,77 @@ int ht_tracker_feed(ht_ctx *ctx, const ht_video_frame *frames, int n, int frames
     if ((f.pitch & 3) || (f.pitch != 0 && f.pitch < 4 * f.width))
       return ctx->fail(HT_ERR_ARG, "record %d: pitch %d is not a multiple of 4 >= 4*width", b, f.pitch);
   }
-  if (canvas_w <= 0 || canvas_h <= 0) return ctx->fail(HT_ERR_SIZE, "0-sized canvas (a browser draws nothing; the detector then throws)");
-  IngestGeom g{0, 0, canvas_w, canvas_h, 0, 0, 0};
-  if (!bilinear_division_constants(4ull * canvas_w * canvas_h, g.magic, g.shift))
-    return ctx->fail(HT_ERR_SIZE, "canvas too large for 32-bit bilinear numerators");
-  g.half = (uint32_t)(2ull * canvas_w * canvas_h);
-  if (is_device_ptr(frames[0].rgba) != (frames_on_device != 0))
+  struct Group { int w, h, first, n; IngestGeom g; Plan *P; TickGroup tick; size_t base; };
+  std::vector<Group> groups;
+  std::vector<int> group_of((size_t)n);
+  std::map<std::pair<int, int>, int> index;
+  int last = -1;                          // the previous record's group: runs of one size skip the lookup
+  for (int b = 0; b < n; ++b) {
+    const int cw = frames[b].canvas_w, chh = frames[b].canvas_h;
+    if (last >= 0 && groups[(size_t)last].w == cw && groups[(size_t)last].h == chh) {
+      group_of[(size_t)b] = last;
+      ++groups[(size_t)last].n;
+      continue;
+    }
+    auto it = index.find(std::make_pair(cw, chh));
+    if (it == index.end()) {
+      char where[32] = "";
+      if (!one_canvas) snprintf(where, sizeof(where), "record %d: ", b);
+      if (cw <= 0 || chh <= 0) return ctx->fail(HT_ERR_SIZE, "%s0-sized canvas (a browser draws nothing; the detector then throws)", where);
+      Group G{cw, chh, b, 0, {}, nullptr, {}, 0};
+      if (!canvas_geom(cw, chh, G.g)) return ctx->fail(HT_ERR_SIZE, "%scanvas too large for 32-bit bilinear numerators", where);
+      it = index.emplace(std::make_pair(cw, chh), (int)groups.size()).first;
+      groups.push_back(G);
+    }
+    last = it->second;
+    group_of[(size_t)b] = last;
+    ++groups[(size_t)last].n;
+  }
+  if (is_device_ptr(frames[0].video.rgba) != (frames_on_device != 0))
     return ctx->fail(HT_ERR_ARG, "the frames are %s memory, frames_on_device says otherwise", frames_on_device ? "host" : "device");
   { const int jr = join_aux(ctx); if (jr != HT_OK) return jr; }
   CK(cudaSetDevice(ctx->cfg.device));
-  Plan *P = nullptr;
-  int rc = get_plan(ctx, canvas_w, canvas_h, 5, &P);     // HT_ERR_SIZE: above the maximum, or too small for the pyramid
-  if (rc != HT_OK) return rc;
-  const size_t canvas_bytes = (size_t)canvas_w * canvas_h * 4;
-  if (ctx->d_feed_canvas.cap < (size_t)mf * canvas_bytes) {   // the masked detection reads whole frame quads: never garbage
-    CK(ctx->d_feed_canvas.reserve((size_t)mf * canvas_bytes));
+  for (Group &G : groups) {
+    const int rc = get_plan(ctx, G.w, G.h, 5, &G.P);   // HT_ERR_SIZE: above the maximum, or too small for the pyramid
+    if (rc != HT_OK) {
+      if (one_canvas) return rc;
+      const std::string e = ctx->err;
+      return ctx->fail(rc, "record %d: %s", G.first, e.c_str());
+    }
+  }
+  // arena layout.  A frame quad may cover up to 3 slots past a group's last entry: they lie inside the arena (the next
+  // group's canvases, or the tail kept below), initialised memory.  The arena holds at least max_frames canvases of
+  // the call's largest size, so that its capacity settles at once for a steady mix of sizes.
+  const int n_groups = (int)groups.size();
+  size_t base = 0, need = 0, px = 0, largest = 0;
+  int k = 0, q = 0;
+  for (Group &G : groups) {
+    const size_t cb = (size_t)G.w * G.h * 4;
+    G.base = base;
+    G.tick = TickGroup{G.P, k, G.n, G.w, G.h, q, nullptr, px};
+    need = std::max(need, base + (size_t)((G.n + 3) & ~3) * cb);
+    largest = std::max(largest, cb);
+    base = align_up<size_t>(base + (size_t)G.n * cb, 256);
+    px = align_up<size_t>(px + (size_t)G.n * G.w * G.h, 64);   // bin planes are read and written in 16-byte vectors
+    k += G.n;
+    q += (G.n + 3) / 4;
+  }
+  need = std::max(need, (size_t)mf * largest);
+  if (ctx->d_feed_canvas.cap < need) {   // the masked detection reads whole frame quads: never garbage
+    CK(ctx->d_feed_canvas.reserve(need));
     CK(cudaMemsetAsync(ctx->d_feed_canvas.p, 0, ctx->d_feed_canvas.cap, ctx->stream));
   }
-  // record table: ids [n] i32 | clocks [n] f64 | FeedRec [n], one copy
-  const size_t off_now = align_up<size_t>(4 * (size_t)mf, 16), off_rec = off_now + 8 * (size_t)mf;
-  const size_t table_cap = off_rec + sizeof(FeedRec) * (size_t)mf;
+  uint8_t *arena = ctx->d_feed_canvas.as<uint8_t>();
+  // record table: ids [n] i32 | clocks [n] f64 | FeedRec [n] | (several sizes) EntryCanvas [n] | tile starts [n + 1] i32
+  auto table_offsets = [](size_t m, size_t off[4]) {
+    off[0] = align_up<size_t>(4 * m, 16);                 // clocks
+    off[1] = off[0] + 8 * m;                              // FeedRec
+    off[2] = off[1] + sizeof(FeedRec) * m;                // EntryCanvas
+    off[3] = off[2] + sizeof(EntryCanvas) * m;            // tile starts
+    return off[3] + 4 * (m + 1);
+  };
+  size_t off[4];
+  const size_t table_cap = table_offsets((size_t)mf, off);
   if (!ctx->h_feed_table) {
     CK(cudaMallocHost(&ctx->h_feed_table.h, table_cap));
     CK(cudaEventCreateWithFlags(&ctx->feed_copied.h, cudaEventDisableTiming));
@@ -1899,18 +2024,34 @@ int ht_tracker_feed(ht_ctx *ctx, const ht_video_frame *frames, int n, int frames
   } else {
     CK(cudaEventSynchronize(ctx->feed_copied));           // the previous call's upload may still read the table
   }
+  const bool mixed = n_groups > 1;
+  const size_t table_full = table_offsets((size_t)n, off);
+  const size_t table_bytes = mixed ? table_full : off[2];
   uint8_t *tab = static_cast<uint8_t *>(ctx->h_feed_table.h);
   int32_t *ids = reinterpret_cast<int32_t *>(tab);
-  double *now = reinterpret_cast<double *>(tab + off_now);
-  FeedRec *recs = reinterpret_cast<FeedRec *>(tab + off_rec);
+  double *now = reinterpret_cast<double *>(tab + off[0]);
+  FeedRec *recs = reinterpret_cast<FeedRec *>(tab + off[1]);
+  EntryCanvas *geo = reinterpret_cast<EntryCanvas *>(tab + off[2]);
+  int32_t *tile_start = reinterpret_cast<int32_t *>(tab + off[3]);
   size_t video_bytes = 0;
-  for (int b = 0; b < n; ++b) video_bytes += align_up<size_t>((size_t)frames[b].width * frames[b].height * 4, 256);
+  for (int b = 0; b < n; ++b) video_bytes += align_up<size_t>((size_t)frames[b].video.width * frames[b].video.height * 4, 256);
   if (!frames_on_device) CK(ctx->d_frames.reserve(video_bytes));
   size_t voff = 0;
-  for (int b = 0; b < n; ++b) {
-    const ht_video_frame &f = frames[b];
-    ids[b] = f.stream;
-    now[b] = f.now_ms;
+  std::vector<int> fill((size_t)n_groups, 0);
+  int t0 = 0;
+  std::vector<int> entry_of((size_t)n);
+  for (int b = 0; b < n; ++b) {           // entry of record b: its group's first entry + its rank in the group
+    const int gi = group_of[(size_t)b];
+    entry_of[(size_t)b] = groups[(size_t)gi].tick.k0 + fill[(size_t)gi]++;
+  }
+  std::vector<int> record_of((size_t)n);
+  for (int b = 0; b < n; ++b) record_of[(size_t)entry_of[(size_t)b]] = b;
+  for (int e = 0; e < n; ++e) {
+    const int b = record_of[(size_t)e];
+    const Group &G = groups[(size_t)group_of[(size_t)b]];
+    const ht_video_frame &f = frames[b].video;
+    ids[e] = f.stream;
+    now[e] = f.now_ms;
     FeedRec r{f.rgba, f.stream, f.width, f.height, f.pitch ? f.pitch : 4 * f.width, f.now_ms};
     if (!frames_on_device) {                               // pack the host videos into the device staging buffer
       uint8_t *dst = ctx->d_frames.as<uint8_t>() + voff;
@@ -1920,14 +2061,44 @@ int ht_tracker_feed(ht_ctx *ctx, const ht_video_frame *frames, int n, int frames
       r.pitch = 4 * f.width;
       voff += align_up<size_t>((size_t)f.width * f.height * 4, 256);
     }
-    recs[b] = r;
+    recs[e] = r;
+    if (mixed) {
+      const int j = e - G.tick.k0;
+      geo[e] = EntryCanvas{G.base + (size_t)j * G.w * G.h * 4, G.w, G.h, G.g.magic, G.g.shift, G.g.half,
+                           G.tick.k0, G.tick.k0 + G.n, G.tick.q0, b, 0};
+      tile_start[e] = t0;
+      t0 += ((G.w + 63) / 64) * ((G.h + 15) / 16);
+    }
   }
+  tile_start[n] = t0;
   uint8_t *dtab = ctx->d_feed_table.as<uint8_t>();
-  CK(cudaMemcpyAsync(dtab, tab, off_rec + sizeof(FeedRec) * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(dtab, tab, table_bytes, cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaEventRecord(ctx->feed_copied, ctx->stream));
-  const FeedDraw feed{reinterpret_cast<const FeedRec *>(dtab + off_rec), ctx->d_feed_draw.as<uint8_t>(), g};
-  return tracker_tick(ctx, P, ctx->d_feed_canvas.as<uint8_t>(), n, canvas_w, canvas_h, reinterpret_cast<const int32_t *>(dtab),
-                      0.0, reinterpret_cast<const double *>(dtab + off_now), &feed, out);
+  std::vector<TickGroup> ticks((size_t)n_groups);
+  for (int i = 0; i < n_groups; ++i) {
+    ticks[(size_t)i] = groups[(size_t)i].tick;
+    ticks[(size_t)i].frames = arena + groups[(size_t)i].base;
+  }
+  const FeedDraw feed{reinterpret_cast<const FeedRec *>(dtab + off[1]), ctx->d_feed_draw.as<uint8_t>(), groups[0].g,
+                      mixed ? reinterpret_cast<const int32_t *>(dtab + off[3]) : nullptr, t0};
+  return tracker_tick(ctx, ticks.data(), n_groups, arena, n, reinterpret_cast<const int32_t *>(dtab), 0.0,
+                      reinterpret_cast<const double *>(dtab + off[0]), &feed,
+                      mixed ? reinterpret_cast<const EntryCanvas *>(dtab + off[2]) : nullptr, out);
+}
+
+int ht_tracker_feed(ht_ctx *ctx, const ht_video_frame *frames, int n, int frames_on_device, int canvas_w, int canvas_h,
+                    ht_tracker_event *out) {
+  if (!ctx) return HT_ERR_ARG;
+  if (!ctx->tracker_on) return ctx->fail(HT_ERR_STATE, "ht_tracker_config has not been called");
+  if (!frames || !out) return ctx->fail(HT_ERR_ARG, "frames or out is NULL");
+  if (n <= 0 || n > ctx->cfg.max_frames) return ctx->fail(HT_ERR_ARG, "n=%d outside [1,%d]", n, ctx->cfg.max_frames);
+  std::vector<ht_canvas_frame> recs((size_t)n);
+  for (int b = 0; b < n; ++b) recs[(size_t)b] = ht_canvas_frame{frames[b], canvas_w, canvas_h, {0, 0}};
+  return tracker_feed(ctx, recs.data(), n, frames_on_device, true, out);
+}
+
+int ht_tracker_feed_canvases(ht_ctx *ctx, const ht_canvas_frame *frames, int n, int frames_on_device, ht_tracker_event *out) {
+  return tracker_feed(ctx, frames, n, frames_on_device, false, out);
 }
 
 // canvasContext.drawImage(video, 0, 0, canvas.width, canvas.height) for n frames (src/main.js:170)
@@ -2271,6 +2442,38 @@ extern "C" int ht_selftest_feed_draw(const ht_video_frame *frames, int n, const 
       for (int X = 0; X < dw; ++X) feed_draw_pixel(r, canvas, g, X, Y, b);
   }
   return 0;
+}
+
+// k_feed_draw's mixed-size path, tile by tile: every record on its own canvas (frames[b].canvas_w x canvas_h), the
+// records' tiles flattened, each tile's record found by the kernel's search and drawn with its per-pixel code.  The
+// canvases are packed back to back in record order into `canvas`; draw[b] == 0 leaves canvas b untouched.  -> the
+// number of tiles, or -1 for a canvas the draw rejects.
+extern "C" int ht_selftest_feed_canvases(const ht_canvas_frame *frames, int n, const uint8_t *draw, uint8_t *canvas) {
+  std::vector<EntryCanvas> geo((size_t)n);
+  std::vector<int32_t> tile_start((size_t)n + 1);
+  size_t base = 0;
+  int t = 0;
+  for (int b = 0; b < n; ++b) {
+    IngestGeom g;
+    const int w = frames[b].canvas_w, h = frames[b].canvas_h;
+    if (w <= 0 || h <= 0 || !canvas_geom(w, h, g)) return -1;
+    geo[(size_t)b] = EntryCanvas{base, w, h, g.magic, g.shift, g.half, b, b + 1, b, b, 0};
+    tile_start[(size_t)b] = t;
+    t += ((w + 63) / 64) * ((h + 15) / 16);
+    base += (size_t)w * h * 4;
+  }
+  tile_start[(size_t)n] = t;
+  for (int tile = 0; tile < t; ++tile) {
+    const int b = feed_tile_record(tile_start.data(), n, tile);
+    if (!draw[b]) continue;
+    const EntryCanvas &e = geo[(size_t)b];
+    const int tx = (e.w + 63) / 64, j = tile - tile_start[(size_t)b];
+    const ht_video_frame &f = frames[b].video;
+    const FeedRec r{f.rgba, f.stream, f.width, f.height, f.pitch ? f.pitch : 4 * f.width, f.now_ms};
+    for (int Y = (j / tx) * 16; Y < std::min(e.h, (j / tx) * 16 + 16); ++Y)
+      for (int X = (j % tx) * 64; X < std::min(e.w, (j % tx) * 64 + 64); ++X) feed_canvas_pixel(r, canvas, e, X, Y);
+  }
+  return t;
 }
 
 // gray + pyramid of one frame quad with the kernels' own per-thread code (gray_item, resample_thread), thread by thread

@@ -237,29 +237,77 @@ __host__ __device__ __forceinline__ void feed_draw_pixel(const FeedRec &r, uint8
                                                             : draw_pixel(s, r.width, r.height, spitch, g, X, Y);
   reinterpret_cast<uint32_t *>(canvas)[((size_t)b * g.dh + Y) * g.dw + X] = out;
 }
-// grid = (canvas tiles of 64 x 16 pixels, records).  draw[b] == 0 (an IDLE stream): the record's video is not read.
+// ht_tracker_feed_canvases: batch entry k's canvas.  The host groups the records by canvas size: each group is a
+// contiguous range [g0, g_end) of batch entries with one pyramid plan, and its canvases are a contiguous block of the
+// arena.  All of it goes up with the record table.
+struct EntryCanvas {
+  uint64_t base;                // byte offset of the entry's canvas in the arena
+  int32_t w, h;                 // canvas size
+  uint32_t magic, shift, half;  // the draw's division constants for w x h (IngestGeom)
+  int32_t g0, g_end;            // the entry's group
+  int32_t q0;                   // the group's first frame quad in the detection mask
+  int32_t record;               // the caller's record index: where the entry's event goes
+  int32_t pad_;
+};
+static_assert(sizeof(EntryCanvas) == 48, "EntryCanvas layout");
+__host__ __device__ __forceinline__ IngestGeom entry_geom(const EntryCanvas &e) {
+  return IngestGeom{0, 0, e.w, e.h, e.magic, e.shift, e.half};
+}
+// the record of flattened tile t: tile_start[b] <= t < tile_start[b + 1] (tile_start[0] = 0; every record has a tile)
+__host__ __device__ __forceinline__ int feed_tile_record(const int32_t *__restrict__ tile_start, int n, int t) {
+  int lo = 0, hi = n - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (tile_start[mid] <= t) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
+// canvas pixel (X, Y) of record r onto its own canvas e of the arena (also run on the host by ht_selftest_feed_canvases)
+__host__ __device__ __forceinline__ void feed_canvas_pixel(const FeedRec &r, uint8_t *__restrict__ arena, const EntryCanvas &e,
+                                                           int X, int Y) {
+  feed_draw_pixel(r, arena + e.base, entry_geom(e), X, Y, 0);
+}
+// Tiles of 64 x 16 canvas pixels.  One canvas size (tile_start == NULL): grid = (tiles of the canvas g, records),
+// canvas b of the arena is record b's.  Mixed sizes: grid = every record's tiles, flattened (tile_start [n + 1]): a CTA
+// finds its record by binary search and takes the canvas geometry from geo[b], so no CTA idles on a small canvas.
+// draw[b] == 0 (an IDLE stream): the record's video is not read.
 // A CTA covers 16 rows (four 4-row passes) so that the two loads every CTA starts with - the record and its flag,
 // issued together - are paid once per 1024 pixels.  A 1:1 record whose rows are 16-byte aligned is copied with 16-byte
 // loads and stores (4 pixels per thread, one pass).
 __global__ void __launch_bounds__(256) k_feed_draw(const FeedRec *__restrict__ recs, const uint8_t *__restrict__ draw,
-                                                   uint8_t *__restrict__ canvas, IngestGeom g, int tiles_x) {
-  const int b = blockIdx.y;
+                                                   uint8_t *__restrict__ canvas, IngestGeom g, int tiles_x,
+                                                   const EntryCanvas *__restrict__ geo, const int32_t *__restrict__ tile_start,
+                                                   int n) {
+  int b, tile;
+  uint8_t *cv;
+  if (tile_start) {
+    b = feed_tile_record(tile_start, n, (int)blockIdx.x);
+    const EntryCanvas e = geo[b];
+    tile = (int)blockIdx.x - tile_start[b];
+    g = entry_geom(e);
+    tiles_x = (e.w + 63) / 64;
+    cv = canvas + e.base;
+  } else {
+    b = blockIdx.y;
+    tile = blockIdx.x;
+    cv = canvas + (size_t)b * g.dh * g.dw * 4;
+  }
   const FeedRec r = recs[b];
   if (!draw[b]) return;
-  const int X0 = (blockIdx.x % tiles_x) * 64, Y0 = (blockIdx.x / tiles_x) * 16;
+  const int X0 = (tile % tiles_x) * 64, Y0 = (tile / tiles_x) * 16;
   if (r.width == g.dw && r.height == g.dh && (g.dw & 3) == 0 &&
-      ((reinterpret_cast<uintptr_t>(r.src) | (uintptr_t)r.pitch) & 15u) == 0) {
+      ((reinterpret_cast<uintptr_t>(r.src) | (uintptr_t)r.pitch | reinterpret_cast<uintptr_t>(cv)) & 15u) == 0) {
     const int X = X0 + 4 * (threadIdx.x & 15), Y = Y0 + (threadIdx.x >> 4);
     if (X >= g.dw || Y >= g.dh) return;
     const uint4 v = ld_ro(reinterpret_cast<const uint4 *>(r.src + (size_t)Y * r.pitch) + (X >> 2));
-    reinterpret_cast<uint4 *>(canvas + ((size_t)b * g.dh + Y) * g.dw * 4)[X >> 2] = v;
+    reinterpret_cast<uint4 *>(cv + (size_t)Y * g.dw * 4)[X >> 2] = v;
     return;
   }
   const int X = X0 + (threadIdx.x & 63);
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     const int Y = Y0 + 4 * i + (threadIdx.x >> 6);
-    if (X < g.dw && Y < g.dh) feed_draw_pixel(r, canvas, g, X, Y, b);
+    if (X < g.dw && Y < g.dh) feed_draw_pixel(r, cv, g, X, Y, 0);
   }
 }
 

@@ -70,14 +70,26 @@ __global__ void __launch_bounds__(256) k_hist(const uint8_t *__restrict__ rgba, 
 // initTracker — src/camshift.js:198-211.  One CTA per slot: model histogram of the rectangle
 // (pixels outside the canvas read as 0,0,0,0 -> bin 0, like getImageData), _searchWindow := rect,
 // _trackObj := new TrackObj().  rects == NULL -> take the rectangle from det_pick (device pick).
+// calc_angles < 0 (ht_tracker_step / feed): per entry, enable[k] & 2 (k_tracker_update sets it from the stream's
+// parameters).  geo (ht_tracker_feed, else NULL): per-entry canvas size and place in the arena, instead of W, H and
+// frame k at k * frame_bytes.
 __global__ void __launch_bounds__(256) k_track_init(const uint8_t *__restrict__ rgba, size_t frame_bytes, int W, int H,
                                                     const int32_t *__restrict__ slots,
                                                     const int32_t *__restrict__ rects, int calc_angles,
                                                     uint32_t *__restrict__ model_hist, TrackState *__restrict__ state,
-                                                    int32_t *__restrict__ found, const uint8_t *__restrict__ enable) {
+                                                    int32_t *__restrict__ found, const uint8_t *__restrict__ enable,
+                                                    const EntryCanvas *__restrict__ geo = nullptr) {
   __shared__ uint32_t sh[4096];
   const int k = blockIdx.x;
   if (enable && !enable[k]) return;            // ht_stream_step: only the streams that just found a face
+  if (calc_angles < 0) calc_angles = (enable[k] >> 1) & 1;
+  const uint8_t *frame = rgba + (size_t)k * frame_bytes;
+  if (geo) {
+    const EntryCanvas &e = geo[k];
+    frame = rgba + e.base;
+    W = e.w;
+    H = e.h;
+  }
   const int slot = slots ? slots[k] : k;
   const int rx = rects[4 * k + 0], ry = rects[4 * k + 1], rw = rects[4 * k + 2], rh = rects[4 * k + 3];
   if (rw <= 0 || rh <= 0) {  // no candidate (device pick): the slot becomes uninitialised
@@ -89,7 +101,7 @@ __global__ void __launch_bounds__(256) k_track_init(const uint8_t *__restrict__ 
   }
   for (int i = threadIdx.x; i < 4096; i += 256) sh[i] = 0;
   __syncthreads();
-  const uint32_t *px = reinterpret_cast<const uint32_t *>(rgba + (size_t)k * frame_bytes);
+  const uint32_t *px = reinterpret_cast<const uint32_t *>(frame);
   for (int yy = threadIdx.x >> 5; yy < rh; yy += 8) {
     const int cy = ry + yy;
     for (int xx = threadIdx.x & 31; xx < rw; xx += 32) {
@@ -1057,11 +1069,18 @@ __global__ void k_backproj(const uint8_t *__restrict__ rgba, int n_px, const uin
 // getWhitebalance — src/whitebalance.js:17-26.  The reference sums bytes in fp64; the sums are
 // exact integers, so integer accumulation in any order is bit-identical.
 // enable (ht_tracker_step): per frame, 0 = no whitebalance wanted (the frame is not read); NULL = every frame
+// geo (ht_tracker_feed, else NULL): per-entry canvas size and place in the arena
 __global__ void __launch_bounds__(256) k_wb_sums(const uint8_t *__restrict__ rgba, size_t frame_bytes, int n_px,
                                                  unsigned long long *__restrict__ sums, int chunks,
-                                                 const uint8_t *__restrict__ enable = nullptr) {
+                                                 const uint8_t *__restrict__ enable = nullptr,
+                                                 const EntryCanvas *__restrict__ geo = nullptr) {
   if (enable && !enable[blockIdx.y]) return;
   const uint32_t *px = reinterpret_cast<const uint32_t *>(rgba + (size_t)blockIdx.y * frame_bytes);
+  if (geo) {
+    const EntryCanvas &e = geo[blockIdx.y];
+    px = reinterpret_cast<const uint32_t *>(rgba + e.base);
+    n_px = e.w * e.h;
+  }
   const int per = (n_px + chunks - 1) / chunks;
   const int beg = blockIdx.x * per, end = min(n_px, beg + per);
   unsigned long long r = 0, g = 0, b = 0;
@@ -1206,11 +1225,12 @@ __host__ __device__ inline void tracker_step(TrackerState &s, const TrackerParam
 
 // modes -> the masks of the frame's kernels (a TM_IDLE stream's frame is never read).  Batch entry k is stream ids[k]
 // (ids == NULL: stream k); all masks are indexed by batch entry.  draw (ht_tracker_feed, else NULL): the entry's video
-// is drawn onto its canvas - every stream that is not TM_IDLE.
+// is drawn onto its canvas - every stream that is not TM_IDLE.  The VJ frame quads are those of each canvas-size group
+// (geo, ht_tracker_feed; NULL: one group [0, n) whose quads start at 0): no quad mixes canvas sizes.
 __global__ void k_tracker_plan(const TrackerState *__restrict__ st, const int32_t *__restrict__ ids, int n,
                                uint8_t *__restrict__ vj_quad_mask, uint8_t *__restrict__ cs_enable,
                                uint8_t *__restrict__ init_enable, uint8_t *__restrict__ wb_enable,
-                               uint8_t *__restrict__ draw) {
+                               uint8_t *__restrict__ draw, const EntryCanvas *__restrict__ geo) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= n) return;
   const int m = st[ids ? ids[k] : k].mode;
@@ -1218,37 +1238,49 @@ __global__ void k_tracker_plan(const TrackerState *__restrict__ st, const int32_
   wb_enable[k] = (m == TM_STARTING || m == TM_WB) ? 1 : 0;
   init_enable[k] = 0;
   if (draw) draw[k] = m != TM_IDLE ? 1 : 0;
-  if ((k & 3) == 0) {
+  const int g0 = geo ? geo[k].g0 : 0, g_end = geo ? geo[k].g_end : n, q0 = geo ? geo[k].q0 : 0;
+  if (((k - g0) & 3) == 0) {
     unsigned mask = 0;
-    for (int f = 0; f < 4 && k + f < n; ++f) mask |= (st[ids ? ids[k + f] : k + f].mode == TM_VJ ? 1u : 0u) << f;
-    vj_quad_mask[k >> 2] = (uint8_t)mask;
+    for (int f = 0; f < 4 && k + f < g_end; ++f) mask |= (st[ids ? ids[k + f] : k + f].mode == TM_VJ ? 1u : 0u) << f;
+    vj_quad_mask[q0 + ((k - g0) >> 2)] = (uint8_t)mask;
   }
 }
 
+// Batch entry k is stream ids[k] (NULL: stream k) with the parameters params[stream].
 // now (ht_tracker_feed, else NULL): the clock of each batch entry; otherwise every entry ticks at now_ms.
-// best, counts: as in k_stream_update, per batch entry
+// geo (ht_tracker_feed, else NULL): per entry the canvas size (whitebalance pixel count, headposition's camera size)
+// and the record whose event it is; otherwise every entry is on camw x camh and its event is events[k].
+// best, counts: as in k_stream_update, per batch entry.  init_enable[k] := 1 | 2 * calcAngles when initTracker follows.
 __global__ void k_tracker_update(TrackerState *__restrict__ st, const int32_t *__restrict__ ids,
                                  const TrackerParams *__restrict__ params, int n,
                                  const unsigned long long *__restrict__ wb_sums, int n_px, const Rect *__restrict__ best,
                                  const int32_t *__restrict__ counts, const int32_t *__restrict__ objs,
                                  int32_t *__restrict__ rects, uint8_t *__restrict__ init_enable, double now_ms,
-                                 const double *__restrict__ now, int camw, int camh, TrackerEvent *__restrict__ events) {
+                                 const double *__restrict__ now, int camw, int camh, const EntryCanvas *__restrict__ geo,
+                                 TrackerEvent *__restrict__ events) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= n) return;
   if (now) now_ms = now[k];
-  TrackerState &s = st[ids ? ids[k] : k];      // updated in place: the window and the head state stay in memory
+  int out = k;
+  if (geo) {
+    const EntryCanvas &g = geo[k];
+    camw = g.w; camh = g.h; n_px = g.w * g.h; out = g.record;
+  }
+  const int id = ids ? ids[k] : k;
+  TrackerState &s = st[id];                    // updated in place: the window and the head state stay in memory
+  const TrackerParams &p = params[id];
   const bool wants_wb = s.mode == TM_STARTING || s.mode == TM_WB;
   const double wb = wants_wb ? wb_value(wb_sums + 3 * (size_t)k, n_px) : 0.0;
   TrackerEvent e;
   int32_t rect[4];
   bool seed;
-  tracker_step(s, *params, wb, best + k, (s.mode == TM_VJ && counts[k] > 0) ? 1 : 0, objs + 6 * (size_t)k, now_ms,
+  tracker_step(s, p, wb, best + k, (s.mode == TM_VJ && counts[k] > 0) ? 1 : 0, objs + 6 * (size_t)k, now_ms,
                (double)camw, (double)camh, e, rect, seed);
   if (seed) {
     for (int i = 0; i < 4; ++i) rects[4 * k + i] = rect[i];
-    init_enable[k] = 1;
+    init_enable[k] = (uint8_t)(1 | (p.calc_angles ? 2 : 0));
   }
-  events[k] = e;
+  events[out] = e;
 }
 
 // op: 0 = new state, 1 = start(), 2 = stop()

@@ -85,6 +85,14 @@ def lifecycle_events(rec, status):
     return out, status
 
 
+def _tracker_kwargs(params):
+    """Context.tracker_config keywords of one Tracker's parameter dict (src/main.js:39-55 names and defaults)"""
+    p = dict(params or {})
+    return dict(retryDetection=p.get("retryDetection", True), calcAngles=p.get("calcAngles", False),
+                smoothing=p.get("smoothing", True), fov=p.get("fov"), cameraOffset=p.get("cameraOffset", 11.5),
+                headPosition=p.get("headPosition", True))
+
+
 class TrackerSet:
     """headtrackr.Tracker (src/main.js) for n streams on the GPU (ht_tracker_step): stream k is one Tracker whose
     `setTimeout` fires once per step() call.  start(k) / stop(k) are the Tracker's start() / stop() (stop() emits
@@ -92,24 +100,35 @@ class TrackerSet:
     detection, tracking, status events and head position all on the device - and dispatches the reference's payload
     dicts in the reference's order to the listeners as fn(stream, evt).  feed({stream: video}) ticks only the listed
     streams, each on its own video frame (any size) and clock, as cameras whose timers fire independently do.
-    `status[k]` is ht.status, getFOV(k) its fov.
+    `status[k]` is ht.status, getFOV(k) its fov.  params: one dict of the reference's parameters for every stream, or
+    a list of n dicts, one per stream (each stream its own `new headtrackr.Tracker(params)`); set_params(k, params)
+    changes one stream's.
     Differs from the reference in one place: start() on a running stream does nothing (the reference runs an extra,
     unscheduled pass)."""
 
     def __init__(self, context, n_streams, params=None, device_events=False):
         if n_streams > context.max_frames:
             raise ValueError("more streams than tracker slots in the context")
-        p = dict(params or {})
+        per_stream = isinstance(params, (list, tuple))
+        if per_stream and len(params) != n_streams:
+            raise ValueError("one params dict per stream")
         self.ctx, self.n = context, n_streams
         self._device_events = device_events          # records written to a torch CUDA buffer, then copied back
         self._listeners = []
         self.status = [""] * n_streams
         self._fov = [0] * n_streams
         self.current = [None] * n_streams
-        context.tracker_config(retryDetection=p.get("retryDetection", True), calcAngles=p.get("calcAngles", False),
-                               smoothing=p.get("smoothing", True), fov=p.get("fov"),
-                               cameraOffset=p.get("cameraOffset", 11.5), headPosition=p.get("headPosition", True))
+        context.tracker_config(**_tracker_kwargs(None if per_stream else params))
+        if per_stream:
+            context.tracker_set_params(0, [_tracker_kwargs(p) for p in params])
         context.tracker_reset(0, n_streams)
+
+    def set_params(self, k, params):
+        """The parameters of stream k (a dict as for the constructor).  Its state is kept: calcAngles takes effect at
+        its next hand-off to camshift, the other parameters on its next tick."""
+        if not 0 <= k < self.n:
+            raise ValueError(f"stream {k} outside [0, {self.n})")
+        self.ctx.tracker_set_params(k, [_tracker_kwargs(params)])
 
     def addEventListener(self, fn):
         """fn(stream_index, evt): evt is a headtrackrStatus / facetrackingEvent / headtrackingEvent payload dict."""
@@ -161,10 +180,15 @@ class TrackerSet:
     def feed(self, frames, now_ms=None, width=None, height=None):
         """One timer tick of the listed streams only (ht_tracker_feed): frames = {stream: (h, w, 4) u8 video frame}
         (numpy or torch CUDA, any video size), drawn onto a width x height canvas; now_ms = None (the wall clock), one
-        clock, or {stream: ms}.  Streams not listed do not tick.  -> {stream: record}."""
+        clock, or {stream: ms}; width and height: one canvas size for all, or {stream: pixels} (each stream on its own
+        canvas, ht_tracker_feed_canvases).  Streams not listed do not tick.  -> {stream: record}."""
         if width is None or height is None:
             raise ValueError("the canvas size (width, height) is required")
         ks = list(frames)
+        if isinstance(width, dict):
+            width = [width[k] for k in ks]
+        if isinstance(height, dict):
+            height = [height[k] for k in ks]
         for k in ks:
             if not 0 <= k < self.n:
                 raise ValueError(f"stream {k} outside [0, {self.n})")

@@ -250,8 +250,16 @@ typedef struct {
   ht_head_event head;        /* smoothed face and headtrackingEvent {x, y, z} */
 } ht_tracker_event;
 /* params == NULL switches the lifecycle off and puts every stream back into ht_stream_reset's state.  Switching it on
- * starts every stream as ht_tracker_reset; changing parameters while on keeps the stream states. */
+ * starts every stream as ht_tracker_reset; changing parameters while on keeps the stream states.  Either way every
+ * stream gets `params`: per-stream values of ht_tracker_set_params are discarded. */
 int ht_tracker_config(ht_ctx *ctx, const ht_tracker_params *params);
+/* Per-stream parameters (ABI 1.3): stream first+i gets params[i] (host), for i in [0, n) - the parameters of its own
+ * `new headtrackr.Tracker(params)`.  Stream states are kept, as when ht_tracker_config changes parameters while on.
+ * calc_angles takes effect at the stream's next hand-off to camshift (initTracker: facetrackr creates its camshift
+ * tracker with it, src/main.js:173,241); every other field on the stream's next tick.
+ * Errors (nothing changes): HT_ERR_STATE before ht_tracker_config; HT_ERR_ARG for a range outside [0, max_frames),
+ * n <= 0, params NULL, or any record ht_tracker_config would reject (alpha outside [0,1], distance_to_screen <= 0). */
+int ht_tracker_set_params(ht_ctx *ctx, int first, int n, const ht_tracker_params *params);
 int ht_tracker_reset(ht_ctx *ctx, int first, int n);   /* new headtrackr.Tracker + init(): not running */
 int ht_tracker_start(ht_ctx *ctx, int first, int n);   /* start(): the next frame of the stream goes through starter() */
 int ht_tracker_stop(ht_ctx *ctx, int first, int n);    /* stop() (src/main.js:347-355); the caller emits "stopped" */
@@ -275,8 +283,9 @@ typedef struct {
  *   frames: n HOST records with distinct stream ids.  Their pixel pointers are all device memory (frames_on_device
  *           = 1) or all host memory (0: the library uploads them); only the first record's pointer is checked.
  *   canvas_w x canvas_h: the working canvas of every record of the call (it sets the pyramid plan), at most
- *           max_width x max_height.  The library draws into its own canvas arena ([max_frames] canvases, allocated at
- *           the first call).
+ *           max_width x max_height.  The library draws into its own canvas arena (at least [max_frames] canvases of
+ *           the call's largest size, grown and zeroed when a call needs more).  This is ht_tracker_feed_canvases with
+ *           every record on canvas_w x canvas_h.
  *   out[n]: one ht_tracker_event per record, in record order; host or device (device: enqueue only).
  * Errors (nothing is enqueued): HT_ERR_STATE without ht_tracker_config; HT_ERR_ARG for n outside [1, max_frames], a
  * stream id out of range or listed twice, a NULL pixel pointer, a pointer or pitch that is not a multiple of 4, a
@@ -286,6 +295,22 @@ typedef struct {
  * "VJ" pick is over the whole grouped list (as for ht_stream_step), unless the raw list overflowed (HT_WARN_OVERFLOW). */
 int ht_tracker_feed(ht_ctx *ctx, const ht_video_frame *frames, int n, int frames_on_device, int canvas_w, int canvas_h,
                     ht_tracker_event *out);
+
+/* One stream's video frame and working canvas for ht_tracker_feed_canvases (ABI 1.3): in the reference each
+ * headtrackr.Tracker draws onto its own canvas, whose size also feeds headposition (src/main.js:170, 284-291). */
+typedef struct {
+  ht_video_frame video;
+  int32_t canvas_w, canvas_h;   /* this record's working canvas */
+  int32_t pad_[2];
+} ht_canvas_frame;              /* 48 bytes */
+/* ht_tracker_feed with a canvas per record; the same contract otherwise (any subset of streams in any order, host or
+ * device videos, out[n] in record order, everything checked before anything is enqueued).  Records on different
+ * canvas sizes tick in the same call: the library groups them by size and runs the detector and camshift once per
+ * size, every per-stream kernel once per call.  A record gives the same canvas and the same event whatever else is in
+ * the call.  Errors as for ht_tracker_feed; a record's canvas that is 0-sized, larger than max_width x max_height, too
+ * small for the pyramid or too large for the resampler is HT_ERR_SIZE with the record's index in ht_last_error. */
+int ht_tracker_feed_canvases(ht_ctx *ctx, const ht_canvas_frame *frames, int n, int frames_on_device,
+                             ht_tracker_event *out);
 
 /* Frame ingest (SURVEY.md 8f-4): canvasContext.drawImage(videoElement, 0, 0, canvas.width, canvas.height)
  * (src/main.js:170) for n frames - the video frame (sw x sh) scaled onto the working canvas (dw x dh), all four

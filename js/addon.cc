@@ -22,8 +22,10 @@
 //   trackerConfig(handle, {retryDetection, calcAngles, smoothing, fov, cameraOffset, headPosition} | null)
 //   trackerReset / trackerStart / trackerStop(handle, first, n)
 //   trackerStep(handle, rgba /* n canvases */, n, w, h, nowMs) -> Array<{detection, status: [...], running, fov, ...}>
-//   trackerFeed(handle, [{stream, rgba, width, height, nowMs}], canvasWidth, canvasHeight) -> Array<record>
-//        (ht_tracker_feed: only the listed streams tick, each from its own video frame and clock)
+//   trackerSetParams(handle, first, [params, ...])   (ht_tracker_set_params: each stream its own Tracker parameters)
+//   trackerFeed(handle, [{stream, rgba, width, height, nowMs, canvasWidth?, canvasHeight?}], canvasWidth, canvasHeight)
+//        -> Array<record> (ht_tracker_feed_canvases: only the listed streams tick, each from its own video frame, clock
+//        and canvas)
 //   destroy(handle)
 #include <node_api.h>
 
@@ -353,8 +355,23 @@ static napi_value Backprojection(napi_env env, napi_callback_info info) {
   return ta;
 }
 
-// headtrackr.Tracker's {retryDetection, calcAngles, smoothing, fov, cameraOffset, headPosition} (src/main.js:35-56), or
-// null to switch the per-stream lifecycle off
+// headtrackr.Tracker's {retryDetection, calcAngles, smoothing, fov, cameraOffset, headPosition} (src/main.js:35-56)
+static ht_tracker_params TrackerParamsOf(napi_env env, napi_value o) {
+  ht_tracker_params p;
+  std::memset(&p, 0, sizeof(p));
+  p.retry_detection = GetBoolProp(env, o, "retryDetection", true);
+  p.calc_angles = GetBoolProp(env, o, "calcAngles", false);
+  p.head.smoothing = GetBoolProp(env, o, "smoothing", true);
+  p.head.head_position = GetBoolProp(env, o, "headPosition", true);
+  p.head.edgecorrection = 1;
+  p.head.alpha = 0.35;                                         // src/main.js:163
+  p.head.fov_deg = GetNumProp(env, o, "fov", 0.0);             // <= 0: estimate (src/main.js:283-288)
+  p.head.camera_offset = GetNumProp(env, o, "cameraOffset", 11.5);
+  p.head.distance_to_screen = 60.0;
+  return p;
+}
+
+// the same parameters, or null to switch the per-stream lifecycle off
 static napi_value TrackerConfig(napi_env env, napi_callback_info info) {
   size_t argc = 2;
   napi_value argv[2];
@@ -365,19 +382,30 @@ static napi_value TrackerConfig(napi_env env, napi_callback_info info) {
   int rc;
   if (t != napi_object) rc = ht_tracker_config(ctx, nullptr);
   else {
-    ht_tracker_params p;
-    std::memset(&p, 0, sizeof(p));
-    p.retry_detection = GetBoolProp(env, argv[1], "retryDetection", true);
-    p.calc_angles = GetBoolProp(env, argv[1], "calcAngles", false);
-    p.head.smoothing = GetBoolProp(env, argv[1], "smoothing", true);
-    p.head.head_position = GetBoolProp(env, argv[1], "headPosition", true);
-    p.head.edgecorrection = 1;
-    p.head.alpha = 0.35;                                         // src/main.js:163
-    p.head.fov_deg = GetNumProp(env, argv[1], "fov", 0.0);       // <= 0: estimate (src/main.js:283-288)
-    p.head.camera_offset = GetNumProp(env, argv[1], "cameraOffset", 11.5);
-    p.head.distance_to_screen = 60.0;
+    const ht_tracker_params p = TrackerParamsOf(env, argv[1]);
     rc = ht_tracker_config(ctx, &p);
   }
+  if (rc < 0) return Throw(env, ctx, rc);
+  return nullptr;
+}
+
+// trackerSetParams(handle, first, [{retryDetection, calcAngles, ...}, ...]): stream first+i gets params[i]
+static napi_value TrackerSetParams(napi_env env, napi_callback_info info) {
+  size_t argc = 3;
+  napi_value argv[3];
+  NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+  ht_ctx *ctx = Ctx(env, argv[0]);
+  int32_t first = 0;
+  uint32_t n = 0;
+  napi_get_value_int32(env, argv[1], &first);
+  NAPI_OK(napi_get_array_length(env, argv[2], &n));
+  std::vector<ht_tracker_params> ps(n);
+  for (uint32_t i = 0; i < n; ++i) {
+    napi_value r;
+    NAPI_OK(napi_get_element(env, argv[2], i, &r));
+    ps[i] = TrackerParamsOf(env, r);
+  }
+  int rc = ht_tracker_set_params(ctx, first, (int)n, ps.data());
   if (rc < 0) return Throw(env, ctx, rc);
   return nullptr;
 }
@@ -450,8 +478,9 @@ static napi_value TrackerStep(napi_env env, napi_callback_info info) {
   return out;
 }
 
-// trackerFeed(handle, [{stream, rgba, width, height, nowMs}], canvasWidth, canvasHeight) -> Array<record>, in record
-// order (ht_tracker_feed with host frames: one tick of each listed stream on its own video and clock)
+// trackerFeed(handle, [{stream, rgba, width, height, nowMs, canvasWidth?, canvasHeight?}], canvasWidth, canvasHeight)
+// -> Array<record>, in record order (ht_tracker_feed_canvases with host frames: one tick of each listed stream on its
+// own video, clock and canvas; a record without its own canvas size uses the call's)
 static napi_value TrackerFeed(napi_env env, napi_callback_info info) {
   size_t argc = 4;
   napi_value argv[4];
@@ -462,12 +491,14 @@ static napi_value TrackerFeed(napi_env env, napi_callback_info info) {
   NAPI_OK(napi_get_array_length(env, argv[1], &n));
   napi_get_value_int32(env, argv[2], &cw); napi_get_value_int32(env, argv[3], &ch);
   if (n == 0) return Throw(env, ctx, HT_ERR_ARG);
-  std::vector<ht_video_frame> frames(n);
+  std::vector<ht_canvas_frame> frames(n);
   for (uint32_t b = 0; b < n; ++b) {
     napi_value r, v;
     NAPI_OK(napi_get_element(env, argv[1], b, &r));
-    ht_video_frame &f = frames[b];
-    std::memset(&f, 0, sizeof(f));
+    std::memset(&frames[b], 0, sizeof(frames[b]));
+    frames[b].canvas_w = (int32_t)GetNumProp(env, r, "canvasWidth", cw);
+    frames[b].canvas_h = (int32_t)GetNumProp(env, r, "canvasHeight", ch);
+    ht_video_frame &f = frames[b].video;
     f.stream = (int32_t)GetNumProp(env, r, "stream", -1);
     f.width = (int32_t)GetNumProp(env, r, "width", 0);
     f.height = (int32_t)GetNumProp(env, r, "height", 0);
@@ -478,7 +509,7 @@ static napi_value TrackerFeed(napi_env env, napi_callback_info info) {
     f.rgba = rgba;
   }
   std::vector<ht_tracker_event> ev(n);
-  int rc = ht_tracker_feed(ctx, frames.data(), (int)n, 0, cw, ch, ev.data());
+  int rc = ht_tracker_feed_canvases(ctx, frames.data(), (int)n, 0, ev.data());
   if (rc < 0) return Throw(env, ctx, rc);
   napi_value out;
   napi_create_array_with_length(env, (size_t)n, &out);
@@ -493,6 +524,7 @@ static napi_value Init(napi_env env, napi_value exports) {
       {"trackerStart", nullptr, TrackerStart, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerStop", nullptr, TrackerStop, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerStep", nullptr, TrackerStep, nullptr, nullptr, nullptr, napi_default, nullptr},
+      {"trackerSetParams", nullptr, TrackerSetParams, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerFeed", nullptr, TrackerFeed, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"create", nullptr, Create, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"detect", nullptr, Detect, nullptr, nullptr, nullptr, napi_default, nullptr},

@@ -6,6 +6,8 @@ streams: N 640x480 streams, device-resident frames and outputs, CUDA events arou
   tracker_cs      ht_tracker_step in steady tracking (every stream in "CS")
   stream_head_cs  ht_stream_step_head in steady tracking
   feed_*          ht_tracker_feed against ht_ingest + ht_tracker_step and ht_tracker_step (feed_arms)
+  canvases_*      ht_tracker_feed_canvases on four canvas sizes against four one-size ht_tracker_feed calls, and
+                  one-size ht_tracker_feed against another build of the library (--before-lib) (canvas_arms)
 
 Prints one JSON line with the card's name and power limit read in the same run; --out also writes it to a file."""
 import argparse
@@ -157,11 +159,162 @@ def feed_arms(torch, frames, stream, N, W, H, steps, rounds):
     return res
 
 
+CANVASES = ((320, 240), (256, 192), (200, 150), (160, 120))
+
+
+def canvas_arms(torch, frames, stream, N, W, H, steps, rounds, before_lib=None):
+    """Streams with their own canvas sizes, in steady tracking; every arm on its own context, all arms alternating tick
+    by tick (the arm order rotates), CUDA events around each tick:
+
+      canvases_mixed_cs   N streams of W x H device video, stream k on canvas CANVASES[k % 4], in ONE
+                          ht_tracker_feed_canvases call (four canvas-size groups: detection and camshift once per size)
+      canvases_split_cs   the same ticks as four ht_tracker_feed calls, one per canvas size
+      one_size_cs         ht_tracker_feed of all N streams onto CANVASES[0] (this build)
+      one_size_before_cs  the same with the library at `before_lib` (another build, e.g. the parent commit's)
+
+    The records must agree: mixed == split, one_size == one_size_before.  -> {arm_ms, arm_spread_ms, ...}"""
+    import ctypes as C
+    from headtrackr_b200 import Context, _lib
+    rec_bytes = C.sizeof(_lib.TrackerEvent)
+    MW, MH = max(c[0] for c in CANVASES), max(c[1] for c in CANVASES)
+    now = [1.0e12]
+    groups = [list(range(g, N, len(CANVASES))) for g in range(len(CANVASES))]
+
+    def context():
+        return Context(max_width=MW, max_height=MH, max_frames=N, stream=stream)
+
+    def before_context():
+        # the other build may predate entry points that _lib.lib() binds: bind only what these arms call
+        L = C.CDLL(str(Path(before_lib).resolve()))
+        vp = C.c_void_p
+        L.ht_create.argtypes = [C.POINTER(vp), C.POINTER(_lib.Config), C.c_char_p, C.c_size_t]
+        L.ht_destroy.argtypes, L.ht_destroy.restype = [vp], None
+        L.ht_last_error.argtypes, L.ht_last_error.restype = [vp], C.c_char_p
+        for f in (L.ht_sync, L.ht_max_rects):
+            f.argtypes = [vp]
+        L.ht_tracker_config.argtypes = [vp, vp]
+        for f in (L.ht_tracker_reset, L.ht_tracker_start, L.ht_tracker_stop):
+            f.argtypes = [vp, C.c_int, C.c_int]
+        L.ht_tracker_feed.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp]
+        saved = _lib.lib
+        _lib.lib = lambda: L
+        try:
+            return context()
+        finally:
+            _lib.lib = saved
+
+    def mixed_arm():
+        c = context()
+        arr = (_lib.CanvasFrame * N)()
+        for k in range(N):
+            cw, ch = CANVASES[k % len(CANVASES)]
+            arr[k] = _lib.CanvasFrame(_lib.VideoFrame(frames[k].data_ptr(), k, W, H, 0, 0.0), cw, ch)
+        out = torch.empty(N * rec_bytes, dtype=torch.uint8, device="cuda")
+
+        def run():
+            for k in range(N):
+                arr[k].video.now_ms = now[0]
+            c._check(c._L.ht_tracker_feed_canvases(c._h, C.addressof(arr), N, 1, out.data_ptr()))
+        return c, run, out
+
+    def split_arm():
+        c = context()
+        arrs = []
+        for ks in groups:
+            arr = (_lib.VideoFrame * len(ks))()
+            for i, k in enumerate(ks):
+                arr[i] = _lib.VideoFrame(frames[k].data_ptr(), k, W, H, 0, 0.0)
+            arrs.append(arr)
+        out = torch.empty(N * rec_bytes, dtype=torch.uint8, device="cuda")
+        order = torch.tensor(sum(groups, []), device="cuda")
+        inv = torch.empty_like(order)
+        inv[order] = torch.arange(N, device="cuda")
+        view = out.view(N, rec_bytes)
+
+        def run():
+            off = 0
+            for (cw, ch), arr in zip(CANVASES, arrs):
+                for i in range(len(arr)):
+                    arr[i].now_ms = now[0]
+                c._check(c._L.ht_tracker_feed(c._h, C.addressof(arr), len(arr), 1, cw, ch, view[off].data_ptr()))
+                off += len(arr)
+        return c, run, out, inv
+
+    def one_size_arm(c):
+        arr = (_lib.VideoFrame * N)()
+        for k in range(N):
+            arr[k] = _lib.VideoFrame(frames[k].data_ptr(), k, W, H, 0, 0.0)
+        out = torch.empty(N * rec_bytes, dtype=torch.uint8, device="cuda")
+        cw, ch = CANVASES[0]
+
+        def run():
+            for k in range(N):
+                arr[k].now_ms = now[0]
+            c._check(c._L.ht_tracker_feed(c._h, C.addressof(arr), N, 1, cw, ch, out.data_ptr()))
+        return c, run, out
+
+    mixed, split = mixed_arm(), split_arm()
+    arms = {"canvases_mixed_cs": mixed[:3], "canvases_split_cs": split[:3], "one_size_cs": one_size_arm(context())}
+    if before_lib:
+        arms["one_size_before_cs"] = one_size_arm(before_context())
+    names = list(arms)
+    for c, _, _ in arms.values():
+        c.tracker_config()
+        c.tracker_reset(0, N)
+        c.tracker_start(0, N)
+
+    def tick(name):
+        _, run, _ = arms[name]
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        a.record()
+        run()
+        b.record()
+        b.synchronize()
+        return a.elapsed_time(b)
+
+    def recs(name):
+        return arms[name][2].view(N, rec_bytes)
+
+    for _ in range(17):                          # the whitebalance gate, detection, the first CS frames
+        now[0] += 20.0
+        for name in names:
+            tick(name)
+    times = {name: [[] for _ in range(rounds)] for name in names}
+    mismatches = 0
+    for r in range(rounds):
+        for s in range(steps):
+            now[0] += 20.0
+            rot = (r * steps + s) % len(names)
+            for name in names[rot:] + names[:rot]:
+                times[name][r].append(tick(name))
+            mismatches += int((recs("canvases_mixed_cs") != recs("canvases_split_cs")[split[3]]).any(dim=1).sum())
+            if before_lib:
+                mismatches += int((recs("one_size_cs") != recs("one_size_before_cs")).any(dim=1).sum())
+    if mismatches:
+        raise SystemExit(f"canvas arms disagree on {mismatches} records of the timed ticks")
+    res = {}
+    for name in names:
+        med = [float(np.median(t)) for t in times[name]]
+        res[f"{name}_ms"] = float(np.median(sum(times[name], [])))
+        res[f"{name}_spread_ms"] = max(med) - min(med)
+    ev = [_lib.TrackerEvent.from_buffer_copy(bytes(row)) for row in recs("canvases_mixed_cs").cpu().numpy()]
+    res["canvases_mixed_cs_streams"] = sum(e.detection == 2 for e in ev)
+    ev = [_lib.TrackerEvent.from_buffer_copy(bytes(row)) for row in recs("one_size_cs").cpu().numpy()]
+    res["one_size_cs_streams"] = sum(e.detection == 2 for e in ev)
+    res["canvases"] = ["%dx%d" % c for c in CANVASES]
+    res["canvas_records_agree"] = True
+    for c, _, _ in arms.values():
+        c.close()
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--streams", type=int, default=1024)
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--rounds", type=int, default=5, help="rounds of the alternating feed arms (their spread)")
+    ap.add_argument("--before-lib", help="another build of libheadtrackr_b200.so for the one-size feed arm")
+    ap.add_argument("--only-canvases", action="store_true", help="only the canvas arms (canvas_arms)")
     ap.add_argument("--out")
     a = ap.parse_args()
     import torch
@@ -175,6 +328,9 @@ def main():
     ts = torch.cuda.Stream()                # the library runs on this stream and the events below are recorded on it
     torch.cuda.set_stream(ts)
     stream = ts.cuda_stream
+    if a.only_canvases:
+        res.update(canvas_arms(torch, frames, stream, N, W, H, a.steps, a.rounds, a.before_lib))
+        return report(res, a.out)
     c = Context(max_width=W, max_height=H, max_frames=N, stream=stream)
     ev = torch.empty(N * 144, dtype=torch.uint8, device="cuda")
     c.tracker_config()
@@ -212,11 +368,16 @@ def main():
     res["stream_head_cs_streams"] = sum(e["detection"] == "CS" for e in c.stream_step_head(frames)[0])
     c.close()
     res.update(feed_arms(torch, frames, stream, N, W, H, a.steps, a.rounds))
+    res.update(canvas_arms(torch, frames, stream, N, W, H, a.steps, a.rounds, a.before_lib))
+    report(res, a.out)
+
+
+def report(res, out):
     line = json.dumps(res)
     print(line)
-    if a.out:
-        Path(a.out).parent.mkdir(parents=True, exist_ok=True)
-        Path(a.out).write_text(line + "\n")
+    if out:
+        Path(out).parent.mkdir(parents=True, exist_ok=True)
+        Path(out).write_text(line + "\n")
 
 
 if __name__ == "__main__":
