@@ -8,7 +8,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from ._lib import (CanvasFrame, HeadEvent, HeadParams, HtError, Rect, StreamEvent, TrackerEvent, TrackerParams, TrackObj, VideoFrame,
+from ._lib import (CanvasFrame, DebugCanvas, HeadEvent, HeadParams, HtError, Rect, StreamEvent, TrackerEvent, TrackerParams, TrackObj, VideoFrame,
                    Window)
 from .synth import load_cascade_blob
 
@@ -56,6 +56,7 @@ class Context:
         self.raw_cap = max_raw_per_frame if max_raw_per_frame > 0 else 1024   # ht_config.max_raw_per_frame's default
         self.max_frames = max_frames
         self.last_warning = None
+        self._debug = {}                  # stream -> its debug canvas tensor, kept alive while the library writes it
 
     def close(self):
         if getattr(self, "_h", None) and self._h.value:
@@ -227,10 +228,12 @@ class Context:
         or off (enable=False: every stream goes back to stream_reset's state)."""
         if not enable:
             self._check(self._L.ht_tracker_config(self._h, None))
+            self._debug = {}
             return
         p = tracker_params(retryDetection, calcAngles, smoothing, fov, cameraOffset, headPosition, edgecorrection, alpha,
                            distance_to_screen)
         self._check(self._L.ht_tracker_config(self._h, C.addressof(p)))
+        self._debug = {}                  # ht_tracker_config discards every debug canvas
 
     def tracker_set_params(self, first, params):
         """Parameters of streams first, first+1, ...: one dict of tracker_config's keywords (enable excluded) per stream,
@@ -239,6 +242,28 @@ class Context:
         params = list(params)
         arr = (TrackerParams * max(1, len(params)))(*[tracker_params(**d) for d in params])
         self._check(self._L.ht_tracker_set_params(self._h, int(first), len(params), C.addressof(arr)))
+
+    def tracker_set_debug(self, first, canvases):
+        """Debug canvases (params.debug) of streams first, first+1, ...: per stream None (none) or a torch CUDA uint8
+        (Dh, Dw, 4) tensor; a row-padded view - last two strides (4, 1) - passes its row stride as the pitch.  On every
+        tick whose facetrackr pass is "CS" the library puts the stream's back-projection image at its top-left corner,
+        clipped to it (src/facetrackr.js:193-196).  The context keeps the tensors alive while they are set."""
+        canvases = list(canvases)
+        arr = (DebugCanvas * max(1, len(canvases)))()
+        for i, t in enumerate(canvases):
+            if t is None:
+                continue
+            if not _is_torch(t) or not t.is_cuda:
+                raise ValueError("a debug canvas is a torch CUDA tensor")
+            if t.dim() != 3 or t.element_size() != 1 or t.shape[2] != 4 or t.stride(2) != 1 or t.stride(1) != 4:
+                raise ValueError("debug canvases must be uint8 (Dh, Dw, 4) with strides (pitch, 4, 1)")
+            arr[i] = DebugCanvas(t.data_ptr(), t.shape[1], t.shape[0], t.stride(0), 0)
+        self._check(self._L.ht_tracker_set_debug(self._h, int(first), len(canvases), C.addressof(arr)))
+        for i, t in enumerate(canvases):
+            if t is None:
+                self._debug.pop(int(first) + i, None)
+            else:
+                self._debug[int(first) + i] = t
 
     def tracker_reset(self, first=0, n=None):
         """Streams [first, first+n): a new headtrackr.Tracker, initialised, not running."""

@@ -569,6 +569,11 @@ struct ht_ctx {
   // ht_tracker_config: per stream its state, its TrackerParams (ht_tracker_set_params), its event, its whitebalance flag
   DevBuf d_tracker_state, d_tracker_params, d_tracker_events, d_tracker_wb;
   bool tracker_on = false;
+  // ht_tracker_set_debug: per stream its DebugCanvas (device array and host copy), the number of streams that have
+  // one (0: a tick launches nothing for debug), and the value tables of a tick's entries [max_frames][DBG_TAB]
+  DevBuf d_debug, d_debug_tab;
+  std::vector<DebugCanvas> h_debug;
+  int debug_count = 0;
   // ht_tracker_feed(_canvases): the record table {ids[n], clocks[n], FeedRec[n], EntryCanvas[n], tile starts[n+1]}
   // goes up in one copy from pinned memory; the videos are drawn into the canvas arena (batch entry k's canvas at
   // EntryCanvas::base), zeroed when it grows
@@ -1732,6 +1737,12 @@ int ht_tracker_config(ht_ctx *ctx, const ht_tracker_params *params) {
   { const int jr = join_aux(ctx); if (jr != HT_OK) return jr; }
   CK(cudaSetDevice(ctx->cfg.device));
   const size_t mf = (size_t)ctx->cfg.max_frames;
+  if (params && !tracker_params_ok(*params)) return ctx->fail(HT_ERR_ARG, "bad head parameters");
+  if (ctx->debug_count > 0) {    // either form discards the debug canvases (the device array is all NULL otherwise)
+    CK(cudaMemsetAsync(ctx->d_debug.p, 0, mf * sizeof(DebugCanvas), ctx->stream));
+    ctx->h_debug.assign(mf, DebugCanvas{});
+    ctx->debug_count = 0;
+  }
   if (!params) {                 // off: every stream as after ht_stream_reset (the lifecycle has used the tracker slots)
     if (ctx->tracker_on) {
       ctx->tracker_on = false;
@@ -1744,7 +1755,6 @@ int ht_tracker_config(ht_ctx *ctx, const ht_tracker_params *params) {
     }
     return HT_OK;
   }
-  if (!tracker_params_ok(*params)) return ctx->fail(HT_ERR_ARG, "bad head parameters");
   if (!ctx->d_tracker_state.p) {
     CK(ctx->d_tracker_state.reserve(mf * sizeof(TrackerState)));
     CK(ctx->d_tracker_params.reserve(mf * sizeof(TrackerParams)));
@@ -1780,6 +1790,60 @@ int ht_tracker_set_params(ht_ctx *ctx, int first, int n, const ht_tracker_params
   CK(cudaMemcpyAsync(ctx->d_tracker_params.as<TrackerParams>() + first, tp.data(), (size_t)n * sizeof(TrackerParams),
                      cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));    // `tp` is a local
+  return HT_OK;
+}
+
+static_assert(sizeof(ht_debug_canvas) == 24 && sizeof(DebugCanvas) == sizeof(ht_debug_canvas) &&
+                  offsetof(ht_debug_canvas, pitch) == offsetof(DebugCanvas, pitch),
+              "ht_debug_canvas layout");
+
+// The debug canvases of streams [first, first + n).  Everything is checked on the host before anything changes,
+// overlap over every stream that has a canvas after the call.
+int ht_tracker_set_debug(ht_ctx *ctx, int first, int n, const ht_debug_canvas *canvases) {
+  if (!ctx) return HT_ERR_ARG;
+  if (!ctx->tracker_on) return ctx->fail(HT_ERR_STATE, "ht_tracker_config has not been called");
+  const int mf = ctx->cfg.max_frames;
+  if (first < 0 || n <= 0 || first > mf - n) return ctx->fail(HT_ERR_ARG, "stream range outside [0,%d)", mf);
+  if (!canvases) return ctx->fail(HT_ERR_ARG, "canvases is NULL");
+  std::vector<DebugCanvas> next = ctx->h_debug;
+  next.resize((size_t)mf, DebugCanvas{});
+  for (int i = 0; i < n; ++i) {
+    const ht_debug_canvas &c = canvases[i];
+    DebugCanvas d{};
+    if (c.rgba) {
+      if (reinterpret_cast<uintptr_t>(c.rgba) & 3u) return ctx->fail(HT_ERR_ARG, "record %d: rgba must be 4-byte aligned", i);
+      if (!is_device_ptr(c.rgba)) return ctx->fail(HT_ERR_ARG, "record %d: rgba is not device memory", i);
+      if (c.width < 1 || c.height < 1 || c.width > 16384 || c.height > 16384)
+        return ctx->fail(HT_ERR_SIZE, "record %d: debug canvas %dx%d outside 1..16384", i, c.width, c.height);
+      if ((c.pitch & 3) || (c.pitch != 0 && c.pitch < 4 * c.width))
+        return ctx->fail(HT_ERR_ARG, "record %d: pitch %d is not a multiple of 4 >= 4*width", i, c.pitch);
+      d = DebugCanvas{c.rgba, c.width, c.height, c.pitch ? c.pitch : 4 * c.width, 0};
+    }
+    next[(size_t)(first + i)] = d;
+  }
+  // two canvases of one tick's streams must not share a byte: [start, end) of every canvas, sorted by start
+  std::vector<std::pair<uintptr_t, uintptr_t>> spans;
+  for (const DebugCanvas &d : next)
+    if (d.rgba) {
+      const uintptr_t s = reinterpret_cast<uintptr_t>(d.rgba);
+      spans.emplace_back(s, s + (size_t)(d.h - 1) * d.pitch + 4 * (size_t)d.w);
+    }
+  std::sort(spans.begin(), spans.end());
+  for (size_t i = 1; i < spans.size(); ++i)
+    if (spans[i].first < spans[i - 1].second)
+      return ctx->fail(HT_ERR_ARG, "a debug canvas overlaps another stream's debug canvas");
+  { const int jr = join_aux(ctx); if (jr != HT_OK) return jr; }
+  CK(cudaSetDevice(ctx->cfg.device));
+  if (!ctx->d_debug.p) {
+    CK(ctx->d_debug.reserve((size_t)mf * sizeof(DebugCanvas)));
+    CK(ctx->d_debug_tab.reserve((size_t)mf * DBG_TAB));
+    CK(cudaMemsetAsync(ctx->d_debug.p, 0, (size_t)mf * sizeof(DebugCanvas), ctx->stream));
+  }
+  CK(cudaMemcpyAsync(ctx->d_debug.as<DebugCanvas>() + first, next.data() + first, (size_t)n * sizeof(DebugCanvas),
+                     cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));    // `next` is a local
+  ctx->debug_count = (int)spans.size();
+  ctx->h_debug.swap(next);
   return HT_OK;
 }
 
@@ -1862,6 +1926,17 @@ static int tracker_tick(ht_ctx *ctx, const TickGroup *grp, int n_groups, const u
     uint16_t *bins = ctx->bins.as<uint16_t>() + G.px0;
     rc = launch_hist(ctx, st, G.frames, G.n, G.w, G.h, ch, bins, cs_en + G.k0);
     if (rc != HT_OK) return rc;
+    if (ctx->debug_count > 0) {   // the debug canvases of this group's CS entries, from this frame's histogram
+      const int32_t *ids = d_ids ? d_ids + G.k0 : nullptr;
+      const DebugCanvas *dbg = ctx->d_debug.as<DebugCanvas>();
+      uint8_t *tab = ctx->d_debug_tab.as<uint8_t>() + (size_t)G.k0 * DBG_TAB;
+      k_debug_table<<<(unsigned)G.n, 256, 0, st>>>(ids, cs_en + G.k0, dbg, ctx->model_hist.as<uint32_t>(), ch, tab);
+      const int tiles_x = (G.w + DBG_TX - 1) / DBG_TX, tiles = tiles_x * ((G.h + DBG_TY - 1) / DBG_TY);
+      k_debug_backproj<<<dim3((unsigned)tiles, (unsigned)G.n), 256, 0, st>>>(bins, G.w, G.h, tiles_x, ids, cs_en + G.k0,
+                                                                              dbg, tab);
+      ctx->launches += 2;
+      CK(cudaGetLastError());
+    }
     ctx->prof_begin(HT_PROF_TRACK, st);
     rc = launch_track(ctx, st, G.n, G.k0, bins, G.w, G.h, d_ids ? d_ids + G.k0 : nullptr, ctx->model_hist.as<uint32_t>(), ch,
                       ctx->track_state.as<TrackState>(), 1, ctx->d_objs.as<int32_t>() + 6 * (size_t)G.k0, nullptr,
@@ -2415,6 +2490,36 @@ extern "C" int ht_selftest_tracker(void *state, int op, const ht_tracker_params 
     memcpy(out, &e, sizeof(e));
   }
   return s.mode;
+}
+
+// k_debug_table's per-bin code: table[DBG_TAB] of one stream's model and current histograms -> DBG_TAB
+extern "C" int ht_selftest_debug_table(const uint32_t *mh, const uint32_t *ch, uint8_t *table) {
+  for (int b = 0; b < DBG_TAB; ++b) debug_table_entry(mh, ch, table, b);
+  return DBG_TAB;
+}
+
+// k_debug_backproj's tile walk and per-thread writer on the host: the bin plane (w x h, 8 * bin or BIN_ZERO per pixel)
+// through `table` onto a debug canvas (dw x dh, pitch bytes per row), clipped as the kernel clips it.  -> the number of
+// 16-byte stores (vec paths taken).
+extern "C" int ht_selftest_debug_write(const uint16_t *bins, int w, int h, const uint8_t *table, uint8_t *rgba, int dw,
+                                       int dh, int pitch) {
+  const int cw = std::min(w, dw), chh = std::min(h, dh);
+  const bool vec = ((reinterpret_cast<uintptr_t>(rgba) | (uintptr_t)pitch) & 15u) == 0;
+  const int tiles_x = (w + DBG_TX - 1) / DBG_TX, tiles = tiles_x * ((h + DBG_TY - 1) / DBG_TY);
+  int stores = 0;
+  for (int t = 0; t < tiles; ++t) {
+    const int x0 = (t % tiles_x) * DBG_TX, y0 = (t / tiles_x) * DBG_TY;
+    if (x0 >= cw || y0 >= chh) continue;
+    for (int tid = 0; tid < 256; ++tid) {
+      const int x = x0 + 4 * (tid & 31);
+      if (x >= cw) continue;
+      for (int y = y0 + (tid >> 5); y < std::min(y0 + DBG_TY, chh); y += 8) {
+        debug_px4(bins + (size_t)y * w, table, rgba + (size_t)y * pitch, x, cw, vec);
+        stores += (vec && cw - x >= 4) ? 1 : 0;
+      }
+    }
+  }
+  return stores;
 }
 
 // k_ingest's per-pixel code over a whole frame batch

@@ -1052,17 +1052,94 @@ __global__ void k_stream_update(int32_t *__restrict__ mode, int n, const Rect *_
   }
 }
 
+// getBackProjectionImg's grey level of a pixel whose colour bin has m model and c current counts: Math.floor(255 *
+// weight), the weight of getWeights (src/camshift.js:177-196, 314-330) in fp64.  An integer floor(255 * m / c) would
+// differ where fl(m / c) rounds across k / 255.
+__host__ __device__ __forceinline__ uint32_t backproj_value(uint32_t m, uint32_t c) {
+  double p = 0.0;
+  if (c != 0) p = fmin((double)m / (double)c, 1.0);
+  return (uint32_t)floor(255 * p);
+}
+
 // getBackProjectionImg — src/camshift.js:177-196 (debug path)
 __global__ void k_backproj(const uint8_t *__restrict__ rgba, int n_px, const uint32_t *__restrict__ mh,
                            const uint32_t *__restrict__ ch, uint8_t *__restrict__ out) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n_px) return;
   const uint32_t bin = rgb_bin(reinterpret_cast<const uint32_t *>(rgba)[i]);
-  const uint32_t c = ch[bin];
-  double p = 0.0;
-  if (c != 0) p = fmin((double)mh[bin] / (double)c, 1.0);
-  const uint32_t v = (uint32_t)floor(255 * p);
+  const uint32_t v = backproj_value(mh[bin], ch[bin]);
   reinterpret_cast<uint32_t *>(out)[i] = v | (v << 8) | (v << 16) | 0xff000000u;
+}
+
+// ------------------------------------------------------------------------------------------------
+// The debug canvas of a headtrackr.Tracker stream (ht_tracker_set_debug): on every CS pass facetrackr puts
+// getBackProjectionImg() at (0, 0) of params.debug (src/facetrackr.js:193-196), clipped to that canvas.
+// Layout of ht_debug_canvas, with the pitch resolved; rgba NULL: the stream has none.
+struct DebugCanvas {
+  uint8_t *rgba;
+  int32_t w, h, pitch, pad_;
+};
+constexpr int DBG_TAB = 4112;                     // bytes per value table: 4096 bins + BIN_ZERO's 0, padded to 16 B
+constexpr int DBG_TX = 128, DBG_TY = 32;          // pixels per tile of k_debug_backproj
+
+// Value table of one stream's tick: table[b] = backproj_value(model[b], current[b]) for the 4096 colour bins, and
+// table[4096] = 0 for the BIN_ZERO entries k_bins_mask writes (bins that are absent from the model: value 0, exact).
+__host__ __device__ __forceinline__ void debug_table_entry(const uint32_t *mh, const uint32_t *ch, uint8_t *table, int b) {
+  table[b] = b < 4096 ? (uint8_t)backproj_value(mh[b], ch[b]) : 0;
+}
+
+// pixels [x, min(x + 4, cw)) of one row: bin-plane entries (8 * bin) -> RGBA (v, v, v, 255).  vec: dst + 4 * x is
+// 16-byte aligned (then four whole pixels go in one store).
+__host__ __device__ __forceinline__ void debug_px4(const uint16_t *src, const uint8_t *table, uint8_t *dst, int x, int cw,
+                                                   bool vec) {
+  const int m = cw - x < 4 ? cw - x : 4;
+  uint32_t o[4] = {0, 0, 0, 0};
+  for (int i = 0; i < m; ++i) o[i] = (uint32_t)table[src[x + i] >> 3] * 0x010101u | 0xff000000u;
+  if (vec && m == 4) {
+    *reinterpret_cast<uint4 *>(dst + 4 * (size_t)x) = make_uint4(o[0], o[1], o[2], o[3]);
+  } else {
+    for (int i = 0; i < m; ++i) reinterpret_cast<uint32_t *>(dst)[x + i] = o[i];
+  }
+}
+
+// One CTA per batch entry: the value table of each entry that ran track() (cs_en) on a stream with a debug canvas.
+// ids: the entries' stream ids (NULL: entry j is stream j); ch: the entries' current histograms.
+__global__ void __launch_bounds__(256) k_debug_table(const int32_t *__restrict__ ids, const uint8_t *__restrict__ cs_en,
+                                                     const DebugCanvas *__restrict__ dbg, const uint32_t *__restrict__ model_hist,
+                                                     const uint32_t *__restrict__ ch, uint8_t *__restrict__ tables) {
+  const int j = blockIdx.x;
+  if (!cs_en[j]) return;
+  const int id = ids ? ids[j] : j;
+  if (!dbg[id].rgba) return;
+  const uint32_t *mh = model_hist + (size_t)id * 4096, *c = ch + (size_t)j * 4096;
+  for (int b = threadIdx.x; b < DBG_TAB; b += 256) debug_table_entry(mh, c, tables + (size_t)j * DBG_TAB, b);
+}
+
+// putImageData(getBackProjectionImg(), 0, 0) on the debug canvases of one canvas-size group, from its bin plane (2 B
+// per pixel instead of the canvas's 4).  grid = (tiles of DBG_TX x DBG_TY over w x h, entries); pixels outside
+// min(w, Dw) x min(h, Dh) are not written.
+__global__ void __launch_bounds__(256) k_debug_backproj(const uint16_t *__restrict__ bins, int w, int h, int tiles_x,
+                                                        const int32_t *__restrict__ ids, const uint8_t *__restrict__ cs_en,
+                                                        const DebugCanvas *__restrict__ dbg, const uint8_t *__restrict__ tables) {
+  const int j = blockIdx.y;
+  if (!cs_en[j]) return;
+  const DebugCanvas d = dbg[ids ? ids[j] : j];
+  if (!d.rgba) return;
+  const int cw = min(w, d.w), chh = min(h, d.h);
+  const int x0 = (blockIdx.x % tiles_x) * DBG_TX, y0 = (blockIdx.x / tiles_x) * DBG_TY;
+  if (x0 >= cw || y0 >= chh) return;
+  __shared__ uint4 tab4[DBG_TAB / 16];
+  const uint4 *src = reinterpret_cast<const uint4 *>(tables + (size_t)j * DBG_TAB);
+  for (int i = threadIdx.x; i < DBG_TAB / 16; i += 256) tab4[i] = src[i];
+  __syncthreads();
+  const uint8_t *table = reinterpret_cast<const uint8_t *>(tab4);
+  const bool vec = ((reinterpret_cast<uintptr_t>(d.rgba) | (uintptr_t)d.pitch) & 15u) == 0;
+  const int x = x0 + 4 * (threadIdx.x & 31);
+  if (x >= cw) return;
+  const uint16_t *plane = bins + (size_t)j * w * h;
+  const int y1 = min(y0 + DBG_TY, chh);
+  for (int y = y0 + (threadIdx.x >> 5); y < y1; y += 8)
+    debug_px4(plane + (size_t)y * w, table, d.rgba + (size_t)y * d.pitch, x, cw, vec);
 }
 
 // ------------------------------------------------------------------------------------------------

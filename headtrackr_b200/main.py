@@ -10,7 +10,8 @@ orchestration ABOVE it so that a user of `headtrackr.Tracker` finds the same met
     for every new frame and calls `step()` where the browser would fire the `setTimeout(track, interval)` timer;
   * DOM events (`headtrackrStatus`, `facetrackingEvent`, `headtrackingEvent`, dispatched on `document` in the
     reference) become callbacks registered with `addEventListener(type, fn)`; payload keys are the reference's;
-  * the debug overlay, the UI messages (src/ui.js) and the video fade are dropped.
+  * the debug overlay (on the device it is `params.debug` of streams.TrackerSet, ht_tracker_set_debug), the UI
+    messages (src/ui.js) and the video fade are dropped.
 
 Pinned against the reference's own main.js executed by oracle/jsmini.py (tests/golden/reference_js_main.json,
 tools/make_goldens_main.py, tests/test_host_main.py).

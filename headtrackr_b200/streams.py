@@ -7,6 +7,7 @@ for n streams per call: stream k owns tracker slot k of the context; the mode sw
 drains one event record per stream and frame.  `facetrackingEvent`s are dispatched exactly as the reference does:
 for records with detection == "CS" (src/facetrackr.js:112-125).
 """
+import math
 import time
 
 from .context import tracker_events_from_bytes
@@ -85,6 +86,33 @@ def lifecycle_events(rec, status):
     return out, status
 
 
+def _to_int32(v):
+    """JavaScript's `v >> 0` (ToInt32)"""
+    if not math.isfinite(v):
+        return 0
+    n = math.trunc(v) & 0xffffffff
+    return n - (1 << 32) if n >= 1 << 31 else n
+
+
+def debug_calls(rec):
+    """The 2D-context calls src/main.js:199-219 makes on the debug canvas after one tick's record, in order, as tuples
+    ("strokeRect", strokeStyle, x, y, w, h), ("translate", x, y), ("rotate", angle): the detected face on a "VJ" record
+    whose confidence is not 0 (a VJ tick without a face strokes 0, 0, 0, 0), the tracked face, rotated about its
+    centre, on a "CS" one.  The library puts the back-projection image under them (ht_tracker_set_debug); the strokes
+    are left to the caller's 2D library."""
+    if rec is None or rec["confidence"] == 0:
+        return []
+    x, y, w, h = rec["x"], rec["y"], rec["width"], rec["height"]
+    if rec["detection"] == "VJ":
+        return [("strokeRect", "#0000CC", x, y, w, h)]
+    if rec["detection"] == "CS":
+        a = rec["angle"]
+        return [("translate", x, y), ("rotate", a - math.pi / 2),
+                ("strokeRect", "#00CC00", _to_int32(-(w / 2)), _to_int32(-(h / 2)), w, h),
+                ("rotate", math.pi / 2 - a), ("translate", -x, -y)]
+    return []
+
+
 def _tracker_kwargs(params):
     """Context.tracker_config keywords of one Tracker's parameter dict (src/main.js:39-55 names and defaults)"""
     p = dict(params or {})
@@ -102,7 +130,9 @@ class TrackerSet:
     streams, each on its own video frame (any size) and clock, as cameras whose timers fire independently do.
     `status[k]` is ht.status, getFOV(k) its fov.  params: one dict of the reference's parameters for every stream, or
     a list of n dicts, one per stream (each stream its own `new headtrackr.Tracker(params)`); set_params(k, params)
-    changes one stream's.
+    changes one stream's.  A stream's "debug" key is its debug canvas, a torch CUDA uint8 (Dh, Dw, 4) tensor: the
+    library puts the back-projection image of every "CS" tick on it, and debug_calls(k) gives the strokes main.js
+    draws on top.  No two streams may share a debug canvas.
     Differs from the reference in one place: start() on a running stream does nothing (the reference runs an extra,
     unscheduled pass)."""
 
@@ -122,6 +152,9 @@ class TrackerSet:
         if per_stream:
             context.tracker_set_params(0, [_tracker_kwargs(p) for p in params])
         context.tracker_reset(0, n_streams)
+        debug = [(p or {}).get("debug") for p in (params if per_stream else [params] * n_streams)]
+        if any(d is not None for d in debug):      # after tracker_config, which clears every debug canvas
+            context.tracker_set_debug(0, debug)
 
     def set_params(self, k, params):
         """The parameters of stream k (a dict as for the constructor).  Its state is kept: calcAngles takes effect at
@@ -129,6 +162,7 @@ class TrackerSet:
         if not 0 <= k < self.n:
             raise ValueError(f"stream {k} outside [0, {self.n})")
         self.ctx.tracker_set_params(k, [_tracker_kwargs(params)])
+        self.ctx.tracker_set_debug(k, [(params or {}).get("debug")])   # no "debug" key: none, as in the reference
 
     def addEventListener(self, fn):
         """fn(stream_index, evt): evt is a headtrackrStatus / facetrackingEvent / headtrackingEvent payload dict."""
@@ -218,6 +252,10 @@ class TrackerSet:
                 if e["type"] == "facetrackingEvent":
                     e["time"] = dt
                 self._emit(k, e)
+
+    def debug_calls(self, k):
+        """debug_calls of stream k's last record"""
+        return debug_calls(self.current[k])
 
     def getFOV(self, k):
         return self._fov[k]

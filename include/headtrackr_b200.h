@@ -251,7 +251,8 @@ typedef struct {
 } ht_tracker_event;
 /* params == NULL switches the lifecycle off and puts every stream back into ht_stream_reset's state.  Switching it on
  * starts every stream as ht_tracker_reset; changing parameters while on keeps the stream states.  Either way every
- * stream gets `params`: per-stream values of ht_tracker_set_params are discarded. */
+ * stream gets `params`: per-stream values of ht_tracker_set_params are discarded, and so are the debug canvases of
+ * ht_tracker_set_debug. */
 int ht_tracker_config(ht_ctx *ctx, const ht_tracker_params *params);
 /* Per-stream parameters (ABI 1.3): stream first+i gets params[i] (host), for i in [0, n) - the parameters of its own
  * `new headtrackr.Tracker(params)`.  Stream states are kept, as when ht_tracker_config changes parameters while on.
@@ -311,6 +312,33 @@ typedef struct {
  * small for the pyramid or too large for the resampler is HT_ERR_SIZE with the record's index in ht_last_error. */
 int ht_tracker_feed_canvases(ht_ctx *ctx, const ht_canvas_frame *frames, int n, int frames_on_device,
                              ht_tracker_event *out);
+
+/* A stream's debug canvas: `params.debug` of its headtrackr.Tracker (src/main.js:42-50). */
+typedef struct {
+  uint8_t *rgba;          /* DEVICE memory, `height` rows of `pitch` bytes; NULL: the stream has no debug canvas */
+  int32_t width, height;  /* 1..16384 */
+  int32_t pitch;          /* 0 -> 4*width; a multiple of 4, >= 4*width */
+  int32_t pad_;
+} ht_debug_canvas;        /* 24 bytes */
+/* Stream first+i gets canvases[i] (host array), for i in [0, n); stream states are kept.  On every tick of a stream
+ * whose facetrackr pass is "CS" - track() ran, including the pass that loses the face - the library does what
+ * facetrackr does with params.debug (src/facetrackr.js:193-196): putImageData(getBackProjectionImg(), 0, 0).  Each
+ * pixel of the working canvas becomes (v, v, v, 255), v = floor(255 * min(model[bin] / current[bin], 1)) in fp64 (0
+ * where current[bin] is 0), with this frame's histogram; the image is clipped to the debug canvas, and pixels outside
+ * min(w, width) x min(h, height) keep what they held.  IDLE, STARTING, WB and VJ ticks (also the VJ tick that finds a
+ * face) write nothing.  The canvas is never cleared, and survives stop, start, reset and a lost face, as main.js hands
+ * one params.debug to every facetrackr it creates.  The strokes main.js draws on top (src/main.js:199-219) are not
+ * rasterized: they are pure functions of the tick's ht_tracker_event (streams.debug_calls in the Python package).
+ * The writes are enqueued on the context's stream before a tick's outputs: with host `out` they have landed when the
+ * tick returns, with device `out` after ht_sync or in stream order.  ht_tracker_config clears every stream's debug
+ * canvas; ht_tracker_set_params does not.
+ * Two streams may not share bytes of their debug canvases: the streams of one tick run concurrently and would race,
+ * where the reference's timers write one after another.
+ * Errors (nothing changes): HT_ERR_STATE before ht_tracker_config; HT_ERR_ARG for a range outside [0, max_frames),
+ * n <= 0, canvases NULL, a host pointer, a pointer or pitch that is not a multiple of 4, a pitch below 4*width, or a
+ * canvas whose byte range overlaps another stream's (over all streams that have a canvas after the call);
+ * HT_ERR_SIZE for a size outside 1..16384. */
+int ht_tracker_set_debug(ht_ctx *ctx, int first, int n, const ht_debug_canvas *canvases);
 
 /* Frame ingest (SURVEY.md 8f-4): canvasContext.drawImage(videoElement, 0, 0, canvas.width, canvas.height)
  * (src/main.js:170) for n frames - the video frame (sw x sh) scaled onto the working canvas (dw x dh), all four

@@ -23,6 +23,7 @@
 //   trackerReset / trackerStart / trackerStop(handle, first, n)
 //   trackerStep(handle, rgba /* n canvases */, n, w, h, nowMs) -> Array<{detection, status: [...], running, fov, ...}>
 //   trackerSetParams(handle, first, [params, ...])   (ht_tracker_set_params: each stream its own Tracker parameters)
+//   trackerSetDebug(handle, first, [canvas|null, ...])  (ht_tracker_set_debug: each stream's debug canvas, device memory)
 //   trackerFeed(handle, [{stream, rgba, width, height, nowMs, canvasWidth?, canvasHeight?}], canvasWidth, canvasHeight)
 //        -> Array<record> (ht_tracker_feed_canvases: only the listed streams tick, each from its own video frame, clock
 //        and canvas)
@@ -410,6 +411,37 @@ static napi_value TrackerSetParams(napi_env env, napi_callback_info info) {
   return nullptr;
 }
 
+// trackerSetDebug(handle, first, [{rgba: BigInt device address, width, height, pitch}, null, ...]): stream first+i
+// gets canvases[i] (params.debug); null or undefined: none
+static napi_value TrackerSetDebug(napi_env env, napi_callback_info info) {
+  size_t argc = 3;
+  napi_value argv[3];
+  NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+  ht_ctx *ctx = Ctx(env, argv[0]);
+  int32_t first = 0;
+  uint32_t n = 0;
+  napi_get_value_int32(env, argv[1], &first);
+  NAPI_OK(napi_get_array_length(env, argv[2], &n));
+  std::vector<ht_debug_canvas> cs(n, ht_debug_canvas{nullptr, 0, 0, 0, 0});
+  for (uint32_t i = 0; i < n; ++i) {
+    napi_value r, v;
+    napi_valuetype t = napi_undefined;
+    NAPI_OK(napi_get_element(env, argv[2], i, &r));
+    napi_typeof(env, r, &t);
+    if (t != napi_object) continue;
+    uint64_t addr = 0;
+    bool lossless = false;
+    if (napi_get_named_property(env, r, "rgba", &v) == napi_ok) napi_get_value_bigint_uint64(env, v, &addr, &lossless);
+    cs[i].rgba = reinterpret_cast<uint8_t *>(static_cast<uintptr_t>(addr));
+    if (napi_get_named_property(env, r, "width", &v) == napi_ok) napi_get_value_int32(env, v, &cs[i].width);
+    if (napi_get_named_property(env, r, "height", &v) == napi_ok) napi_get_value_int32(env, v, &cs[i].height);
+    if (napi_get_named_property(env, r, "pitch", &v) == napi_ok) napi_get_value_int32(env, v, &cs[i].pitch);
+  }
+  int rc = ht_tracker_set_debug(ctx, first, (int)n, cs.data());
+  if (rc < 0) return Throw(env, ctx, rc);
+  return nullptr;
+}
+
 // trackerReset / trackerStart / trackerStop(handle, first, n)
 static napi_value TrackerRange(napi_env env, napi_callback_info info, int (*fn)(ht_ctx *, int, int)) {
   size_t argc = 3;
@@ -525,6 +557,7 @@ static napi_value Init(napi_env env, napi_value exports) {
       {"trackerStop", nullptr, TrackerStop, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerStep", nullptr, TrackerStep, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerSetParams", nullptr, TrackerSetParams, nullptr, nullptr, nullptr, napi_default, nullptr},
+      {"trackerSetDebug", nullptr, TrackerSetDebug, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerFeed", nullptr, TrackerFeed, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"create", nullptr, Create, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"detect", nullptr, Detect, nullptr, nullptr, nullptr, napi_default, nullptr},

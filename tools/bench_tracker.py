@@ -8,6 +8,8 @@ streams: N 640x480 streams, device-resident frames and outputs, CUDA events arou
   feed_*          ht_tracker_feed against ht_ingest + ht_tracker_step and ht_tracker_step (feed_arms)
   canvases_*      ht_tracker_feed_canvases on four canvas sizes against four one-size ht_tracker_feed calls, and
                   one-size ht_tracker_feed against another build of the library (--before-lib) (canvas_arms)
+  debug_*         (--debug-streams) ht_tracker_feed with debug canvases on none, 1/64 and all of the streams, the
+                  achieved bandwidth of k_debug_backproj, and the no-debug arm against --before-lib (debug_arms)
 
 Prints one JSON line with the card's name and power limit read in the same run; --out also writes it to a file."""
 import argparse
@@ -162,6 +164,30 @@ def feed_arms(torch, frames, stream, N, W, H, steps, rounds):
 CANVASES = ((320, 240), (256, 192), (200, 150), (160, 120))
 
 
+def other_build_context(before_lib, **kw):
+    """a Context on another build of the library (e.g. the parent commit's).  It may predate entry points that
+    _lib.lib() binds: bind only what the feed arms call."""
+    import ctypes as C
+    from headtrackr_b200 import Context, _lib
+    L = C.CDLL(str(Path(before_lib).resolve()))
+    vp = C.c_void_p
+    L.ht_create.argtypes = [C.POINTER(vp), C.POINTER(_lib.Config), C.c_char_p, C.c_size_t]
+    L.ht_destroy.argtypes, L.ht_destroy.restype = [vp], None
+    L.ht_last_error.argtypes, L.ht_last_error.restype = [vp], C.c_char_p
+    for f in (L.ht_sync, L.ht_max_rects):
+        f.argtypes = [vp]
+    L.ht_tracker_config.argtypes = [vp, vp]
+    for f in (L.ht_tracker_reset, L.ht_tracker_start, L.ht_tracker_stop):
+        f.argtypes = [vp, C.c_int, C.c_int]
+    L.ht_tracker_feed.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp]
+    saved = _lib.lib
+    _lib.lib = lambda: L
+    try:
+        return Context(**kw)
+    finally:
+        _lib.lib = saved
+
+
 def canvas_arms(torch, frames, stream, N, W, H, steps, rounds, before_lib=None):
     """Streams with their own canvas sizes, in steady tracking; every arm on its own context, all arms alternating tick
     by tick (the arm order rotates), CUDA events around each tick:
@@ -184,24 +210,7 @@ def canvas_arms(torch, frames, stream, N, W, H, steps, rounds, before_lib=None):
         return Context(max_width=MW, max_height=MH, max_frames=N, stream=stream)
 
     def before_context():
-        # the other build may predate entry points that _lib.lib() binds: bind only what these arms call
-        L = C.CDLL(str(Path(before_lib).resolve()))
-        vp = C.c_void_p
-        L.ht_create.argtypes = [C.POINTER(vp), C.POINTER(_lib.Config), C.c_char_p, C.c_size_t]
-        L.ht_destroy.argtypes, L.ht_destroy.restype = [vp], None
-        L.ht_last_error.argtypes, L.ht_last_error.restype = [vp], C.c_char_p
-        for f in (L.ht_sync, L.ht_max_rects):
-            f.argtypes = [vp]
-        L.ht_tracker_config.argtypes = [vp, vp]
-        for f in (L.ht_tracker_reset, L.ht_tracker_start, L.ht_tracker_stop):
-            f.argtypes = [vp, C.c_int, C.c_int]
-        L.ht_tracker_feed.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp]
-        saved = _lib.lib
-        _lib.lib = lambda: L
-        try:
-            return context()
-        finally:
-            _lib.lib = saved
+        return other_build_context(before_lib, max_width=MW, max_height=MH, max_frames=N, stream=stream)
 
     def mixed_arm():
         c = context()
@@ -308,6 +317,114 @@ def canvas_arms(torch, frames, stream, N, W, H, steps, rounds, before_lib=None):
     return res
 
 
+HBM_BYTES_PER_S = 3.35e12       # H100 SXM HBM3, NVIDIA data sheet
+
+
+def debug_arms(torch, frames, stream, N, W, H, steps, rounds, before_lib=None):
+    """Debug canvases (ht_tracker_set_debug) in steady tracking: N streams of W x H device video fed onto W x H canvases
+    by ht_tracker_feed, every arm on its own context, all arms alternating tick by tick (the arm order rotates), CUDA
+    events around each tick:
+
+      debug0_cs         no stream has a debug canvas (the tick launches what it launched before debug canvases)
+      debug64_cs        every 64th stream has a W x H debug canvas
+      debugall_cs       every stream has one
+      debug0_before_cs  debug0_cs with the library at `before_lib` (e.g. the parent commit's build)
+
+    Then, in a run of its own under torch.profiler, the kernel time of k_debug_table and k_debug_backproj over `steps`
+    ticks of debugall_cs, and k_debug_backproj's achieved bytes/s: per CS entry with a canvas it reads the 2-byte bin
+    plane (2*w*h) and writes the clipped image (4*min(w,Dw)*min(h,Dh)); k_debug_table reads the model and current
+    histograms (2 * 16 KB) and writes a 4112-byte table.  The records of every arm must agree."""
+    import ctypes as C
+    from headtrackr_b200 import Context, _lib
+    rec_bytes = C.sizeof(_lib.TrackerEvent)
+    now = [1.0e12]
+    recs_arr = (_lib.VideoFrame * N)()
+    for k in range(N):
+        recs_arr[k] = _lib.VideoFrame(frames[k].data_ptr(), k, W, H, 0, 0.0)
+    kw = dict(max_width=W, max_height=H, max_frames=N, stream=stream)
+    canvases = {}
+
+    def arm(every, before=False):
+        c = other_build_context(before_lib, **kw) if before else Context(**kw)
+        c.tracker_config()
+        c.tracker_reset(0, N)
+        c.tracker_start(0, N)
+        if every:
+            dbg = [torch.zeros((H, W, 4), dtype=torch.uint8, device="cuda") if k % every == 0 else None for k in range(N)]
+            c.tracker_set_debug(0, dbg)
+            canvases[every] = sum(d is not None for d in dbg)
+        return c, torch.empty(N * rec_bytes, dtype=torch.uint8, device="cuda")
+
+    arms = {"debug0_cs": arm(0), "debug64_cs": arm(64), "debugall_cs": arm(1)}
+    if before_lib:
+        arms["debug0_before_cs"] = arm(0, before=True)
+    names = list(arms)
+
+    def tick(name):
+        c, out = arms[name]
+        for k in range(N):
+            recs_arr[k].now_ms = now[0]
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        a.record()
+        c._check(c._L.ht_tracker_feed(c._h, C.addressof(recs_arr), N, 1, W, H, out.data_ptr()))
+        b.record()
+        b.synchronize()
+        return a.elapsed_time(b)
+
+    for _ in range(17):                          # the whitebalance gate, detection, the first CS frames
+        now[0] += 20.0
+        for name in names:
+            tick(name)
+    times = {name: [[] for _ in range(rounds)] for name in names}
+    for r in range(rounds):
+        for s in range(steps):
+            now[0] += 20.0
+            rot = (r * steps + s) % len(names)
+            for name in names[rot:] + names[:rot]:
+                times[name][r].append(tick(name))
+            first = arms[names[0]][1].cpu()
+            if any(not torch.equal(first, arms[name][1].cpu()) for name in names[1:]):
+                raise SystemExit("debug arms disagree on the records of a timed tick")
+    res = {}
+    for name in names:
+        med = [float(np.median(t)) for t in times[name]]
+        res[f"{name}_ms"] = float(np.median(sum(times[name], [])))
+        res[f"{name}_spread_ms"] = max(med) - min(med)
+    ev = [_lib.TrackerEvent.from_buffer_copy(bytes(row))
+          for row in arms["debugall_cs"][1].cpu().numpy().reshape(N, rec_bytes)]
+    cs = sum(e.detection == 2 for e in ev)
+    res["debug_cs_streams"] = cs
+    res["debug64_canvases"], res["debugall_canvases"] = canvases[64], canvases[1]
+    res["debug_records_agree"] = True
+
+    from torch.profiler import ProfilerActivity, profile
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(steps):
+            now[0] += 20.0
+            tick("debugall_cs")
+        torch.cuda.synchronize()
+    kernel_us = {}
+    for e in prof.key_averages():
+        for kname in ("k_debug_backproj", "k_debug_table"):
+            if kname in e.key:
+                t = getattr(e, "device_time_total", None)
+                kernel_us[kname] = kernel_us.get(kname, 0.0) + (t if t is not None else e.cuda_time_total)
+    for kname, us in kernel_us.items():
+        res[f"{kname}_ms"] = us / 1000.0 / steps
+    bp_bytes = cs * (2 * W * H + 4 * W * H)
+    tab_bytes = cs * (2 * 4 * 4096 + 4112)
+    res["k_debug_backproj_bytes"] = bp_bytes
+    if "k_debug_backproj" in kernel_us:
+        rate = bp_bytes / (kernel_us["k_debug_backproj"] / steps * 1e-6)
+        res["k_debug_backproj_TBps"] = rate / 1e12
+        res["k_debug_backproj_of_3.35TBps"] = rate / HBM_BYTES_PER_S
+    if "k_debug_table" in kernel_us:
+        res["k_debug_table_GBps"] = tab_bytes / (kernel_us["k_debug_table"] / steps * 1e-6) / 1e9
+    for c, _ in arms.values():
+        c.close()
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--streams", type=int, default=1024)
@@ -315,6 +432,7 @@ def main():
     ap.add_argument("--rounds", type=int, default=5, help="rounds of the alternating feed arms (their spread)")
     ap.add_argument("--before-lib", help="another build of libheadtrackr_b200.so for the one-size feed arm")
     ap.add_argument("--only-canvases", action="store_true", help="only the canvas arms (canvas_arms)")
+    ap.add_argument("--debug-streams", action="store_true", help="only the debug-canvas arms (debug_arms)")
     ap.add_argument("--out")
     a = ap.parse_args()
     import torch
@@ -328,6 +446,9 @@ def main():
     ts = torch.cuda.Stream()                # the library runs on this stream and the events below are recorded on it
     torch.cuda.set_stream(ts)
     stream = ts.cuda_stream
+    if a.debug_streams:
+        res.update(debug_arms(torch, frames, stream, N, W, H, a.steps, a.rounds, a.before_lib))
+        return report(res, a.out)
     if a.only_canvases:
         res.update(canvas_arms(torch, frames, stream, N, W, H, a.steps, a.rounds, a.before_lib))
         return report(res, a.out)
