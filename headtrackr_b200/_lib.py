@@ -82,6 +82,9 @@ class DebugCanvas(C.Structure):
                 ("pad_", C.c_int32)]
 
 
+# ht_tracker_export / ht_tracker_import: bytes of one tracker record (HT_TRACKER_RECORD_BYTES)
+TRACKER_RECORD_BYTES = 16864
+
 # headtrackrStatus names of ht_tracker_event.status, bit 0 first (= the order src/main.js dispatches them in)
 TRACKER_STATUS = ("whitebalance", "detecting", "hints", "redetecting", "lost", "stopped", "found")
 
@@ -122,7 +125,7 @@ _lib = None
 
 EXPORTS = ["ht_version", "ht_create", "ht_destroy", "ht_last_error", "ht_sync", "ht_max_rects", "ht_detect",
            "ht_track_init", "ht_track_init_from_detect", "ht_track", "ht_detect_track", "ht_stream_reset", "ht_stream_step", "ht_stream_head_config", "ht_stream_step_head",
-           "ht_tracker_config", "ht_tracker_reset", "ht_tracker_start", "ht_tracker_stop", "ht_tracker_step", "ht_tracker_feed", "ht_tracker_set_params", "ht_tracker_feed_canvases", "ht_tracker_set_debug", "ht_ingest", "ht_backprojection", "ht_whitebalance",
+           "ht_tracker_config", "ht_tracker_reset", "ht_tracker_start", "ht_tracker_stop", "ht_tracker_step", "ht_tracker_feed", "ht_tracker_set_params", "ht_tracker_feed_canvases", "ht_tracker_set_debug", "ht_tracker_export", "ht_tracker_import", "ht_ingest", "ht_backprojection", "ht_whitebalance",
            "ht_plan_info", "ht_debug_plane", "ht_debug_raw", "ht_debug_model_hist", "ht_debug_track_stats", "ht_set_track_memo", "ht_set_pipeline", "ht_join", "ht_debug_set_exactness", "ht_debug_track_trace", "ht_debug_track_phases", "ht_launch_count",
            "ht_profile", "ht_profile_read"]
 
@@ -166,6 +169,8 @@ def lib():
     L.ht_tracker_set_params.argtypes = [vp, C.c_int, C.c_int, vp]
     L.ht_tracker_feed_canvases.argtypes = [vp, vp, C.c_int, C.c_int, vp]
     L.ht_tracker_set_debug.argtypes = [vp, C.c_int, C.c_int, vp]
+    L.ht_tracker_export.argtypes = [vp, vp, C.c_int, vp]
+    L.ht_tracker_import.argtypes = [vp, vp, C.c_int, vp]
     L.ht_ingest.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, vp, C.c_int, C.c_int]
     L.ht_backprojection.argtypes = [vp, C.c_int, vp, C.c_int, C.c_int, vp]
     L.ht_whitebalance.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, vp]

@@ -55,6 +55,7 @@ class Context:
         self.K = self._L.ht_max_rects(self._h)
         self.raw_cap = max_raw_per_frame if max_raw_per_frame > 0 else 1024   # ht_config.max_raw_per_frame's default
         self.max_frames = max_frames
+        self.max_width, self.max_height, self.device = max_width, max_height, device
         self.last_warning = None
         self._debug = {}                  # stream -> its debug canvas tensor, kept alive while the library writes it
 
@@ -264,6 +265,39 @@ class Context:
                 self._debug.pop(int(first) + i, None)
             else:
                 self._debug[int(first) + i] = t
+
+    def tracker_export(self, streams, out=None):
+        """The tracker records of the listed streams (ht_tracker_export): a (len(streams), TRACKER_RECORD_BYTES) uint8
+        numpy array, or with a contiguous torch CUDA uint8 `out` of that many bytes on this context's device the
+        records written there, asynchronously on the library's stream (sync() before reading them elsewhere)."""
+        ids = (C.c_int32 * max(1, len(streams)))(*[int(k) for k in streams])
+        n = len(streams)
+        if out is not None:
+            if not _is_torch(out) or not out.is_cuda or not out.is_contiguous() or out.element_size() != 1 or \
+                    out.numel() != n * _lib.TRACKER_RECORD_BYTES:
+                raise ValueError("out must be a contiguous torch CUDA uint8 tensor of len(streams) records")
+            self._check(self._L.ht_tracker_export(self._h, C.addressof(ids), n, out.data_ptr()))
+            return out
+        recs = np.zeros((n, _lib.TRACKER_RECORD_BYTES), np.uint8)
+        self._check(self._L.ht_tracker_export(self._h, C.addressof(ids), n, recs.ctypes.data))
+        return recs
+
+    def tracker_import(self, streams, records):
+        """Stream streams[i] := records[i] (ht_tracker_import): its state, parameters and camshift tracker become the
+        exported stream's; its debug canvas stays.  records: (n, TRACKER_RECORD_BYTES) uint8, a numpy array or a
+        contiguous torch CUDA tensor on this context's device.  Every record is checked first; on an error (HtError)
+        no stream changes."""
+        n = len(streams)
+        ids = (C.c_int32 * max(1, n))(*[int(k) for k in streams])
+        if _is_torch(records):
+            if not records.is_contiguous() or records.element_size() != 1 or records.numel() != n * _lib.TRACKER_RECORD_BYTES:
+                raise ValueError("records must be a contiguous uint8 tensor of len(streams) records")
+            self._check(self._L.ht_tracker_import(self._h, C.addressof(ids), n, records.data_ptr()))
+            return
+        a = np.ascontiguousarray(records, dtype=np.uint8)
+        if a.size != n * _lib.TRACKER_RECORD_BYTES:
+            raise ValueError("records must hold len(streams) records")
+        self._check(self._L.ht_tracker_import(self._h, C.addressof(ids), n, a.ctypes.data))
 
     def tracker_reset(self, first=0, n=None):
         """Streams [first, first+n): a new headtrackr.Tracker, initialised, not running."""

@@ -581,6 +581,7 @@ struct ht_ctx {
   PinnedHost h_feed_table;
   Event feed_copied;                        // the last table upload has left h_feed_table
   DevBuf d_track_cost;                      // [max_frames][2] {passes, window pixels / 256} per slot
+  DevBuf d_records, d_record_status;        // ht_tracker_export / import: host records staged on the device, check results
   int track_heavy_div = 128;                // >0: the n/div costliest streams run on a cluster of
   int track_heavy_cluster = 8;              //     track_heavy_cluster CTAs on tier_stream[0] (HT_TRACK_HEAVY=div[,cluster])
   int track_mid_div = 32, track_mid_cluster = 4;  // HT_TRACK_MID=div[,cluster]: the next n/32 costliest streams on clusters of 4
@@ -1729,7 +1730,7 @@ static int tracker_control(ht_ctx *ctx, int first, int n, int op) {
 }
 
 static bool tracker_params_ok(const ht_tracker_params &p) {
-  return p.head.alpha >= 0.0 && p.head.alpha <= 1.0 && p.head.distance_to_screen > 0.0;
+  return tracker_head_ok(p.head.alpha, p.head.distance_to_screen);
 }
 
 int ht_tracker_config(ht_ctx *ctx, const ht_tracker_params *params) {
@@ -1847,6 +1848,108 @@ int ht_tracker_set_debug(ht_ctx *ctx, int first, int n, const ht_debug_canvas *c
   return HT_OK;
 }
 
+static_assert(REC_BYTES == HT_TRACKER_RECORD_BYTES && REC_MAGIC == HT_TRACKER_RECORD_MAGIC &&
+                  REC_VERSION == HT_TRACKER_RECORD_VERSION,
+              "tracker record (include/headtrackr_b200.h)");
+static_assert(REC_STATE == 32 && REC_PARAMS == 320 && REC_TRACK == 416 && REC_COST == 464 && REC_HIST == 480 &&
+                  offsetof(TrackerState, mode) == 0,
+              "tracker record sections (include/headtrackr_b200.h)");
+
+// The checks shared by ht_tracker_export and ht_tracker_import, then the joins and the id upload: streams is a host
+// array of n distinct ids, records host memory or device memory of the context's device (on_device).
+static int tracker_records_args(ht_ctx *ctx, const int32_t *streams, int n, const void *records, bool *on_device) {
+  if (!ctx->tracker_on) return ctx->fail(HT_ERR_STATE, "ht_tracker_config has not been called");
+  const int mf = ctx->cfg.max_frames;
+  if (n <= 0 || n > mf) return ctx->fail(HT_ERR_ARG, "n=%d outside [1,%d]", n, mf);
+  if (!streams) return ctx->fail(HT_ERR_ARG, "streams is NULL");
+  if (!records) return ctx->fail(HT_ERR_ARG, "records is NULL");
+  if (is_device_ptr(streams)) return ctx->fail(HT_ERR_ARG, "streams must be host memory");
+  std::vector<uint8_t> seen((size_t)mf, 0);
+  for (int i = 0; i < n; ++i) {
+    if (streams[i] < 0 || streams[i] >= mf) return ctx->fail(HT_ERR_ARG, "stream %d outside [0,%d)", streams[i], mf);
+    if (seen[(size_t)streams[i]]++) return ctx->fail(HT_ERR_ARG, "stream %d is listed twice", streams[i]);
+  }
+  cudaPointerAttributes a{};
+  if (cudaPointerGetAttributes(&a, records) != cudaSuccess) { cudaGetLastError(); a.type = cudaMemoryTypeUnregistered; }
+  *on_device = a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
+  if (*on_device && a.device != ctx->cfg.device)
+    return ctx->fail(HT_ERR_ARG, "records are memory of device %d, the context is on device %d", a.device, ctx->cfg.device);
+  if (*on_device && (reinterpret_cast<uintptr_t>(records) & 15u))
+    return ctx->fail(HT_ERR_ARG, "device records must be 16-byte aligned");
+  { const int jr = join_aux(ctx); if (jr != HT_OK) return jr; }
+  CK(cudaSetDevice(ctx->cfg.device));
+  const int rc = ensure_tracker_buffers(ctx, ctx->stream);
+  if (rc != HT_OK) return rc;
+  CK(ctx->d_slots.reserve(sizeof(int32_t) * (size_t)mf));
+  CK(cudaMemcpyAsync(ctx->d_slots.p, streams, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
+  if (!*on_device) CK(ctx->d_records.reserve((size_t)n * REC_BYTES));
+  return HT_OK;
+}
+
+int ht_tracker_export(ht_ctx *ctx, const int32_t *streams, int n, void *records) {
+  if (!ctx) return HT_ERR_ARG;
+  bool on_device = false;
+  int rc = tracker_records_args(ctx, streams, n, records, &on_device);
+  if (rc != HT_OK) return rc;
+  uint8_t *dst = on_device ? static_cast<uint8_t *>(records) : ctx->d_records.as<uint8_t>();
+  k_tracker_export<<<(unsigned)n, 256, 0, ctx->stream>>>(ctx->d_slots.as<int32_t>(), ctx->d_tracker_state.as<TrackerState>(),
+                                                         ctx->d_tracker_params.as<TrackerParams>(),
+                                                         ctx->track_state.as<TrackState>(), ctx->model_hist.as<uint32_t>(),
+                                                         ctx->d_track_cost.as<int32_t>(), dst);
+  ++ctx->launches;
+  CK(cudaGetLastError());
+  if (on_device) return HT_OK;
+  CK(cudaMemcpyAsync(records, dst, (size_t)n * REC_BYTES, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  return HT_OK;
+}
+
+static const char *record_problem(int status) {
+  switch (status) {
+    case REC_BAD_MAGIC: return "not a tracker record (bad magic)";
+    case REC_BAD_VERSION: return "tracker record of another format version";
+    case REC_BAD_SIZE: return "bad record size";
+    case REC_BAD_CHECKSUM: return "bad checksum";
+    case REC_BAD_MODE: return "mode outside [0,4]";
+    case REC_BAD_WB: return "whitebalance sample count outside [0,15]";
+    case REC_BAD_DIAG: return "head diagonal count outside [0,6]";
+    case REC_BAD_PARAMS: return "bad head parameters";
+    case REC_BAD_TRACK: return "a CS stream without an initialised camshift window";
+    default: return "unknown check";
+  }
+}
+
+// Every record is checked on the device and the results read back before anything is written: on an error no stream
+// changes.  Then one scatter; the call returns after it, so the caller may reuse `records` at once.
+int ht_tracker_import(ht_ctx *ctx, const int32_t *streams, int n, const void *records) {
+  if (!ctx) return HT_ERR_ARG;
+  bool on_device = false;
+  int rc = tracker_records_args(ctx, streams, n, records, &on_device);
+  if (rc != HT_OK) return rc;
+  cudaStream_t st = ctx->stream;
+  const uint8_t *src = static_cast<const uint8_t *>(records);
+  if (!on_device) {
+    CK(cudaMemcpyAsync(ctx->d_records.p, records, (size_t)n * REC_BYTES, cudaMemcpyHostToDevice, st));
+    src = ctx->d_records.as<uint8_t>();
+  }
+  CK(ctx->d_record_status.reserve(sizeof(int32_t) * (size_t)ctx->cfg.max_frames));
+  k_tracker_import_check<<<(unsigned)n, 256, 0, st>>>(src, ctx->d_record_status.as<int32_t>());
+  ++ctx->launches;
+  CK(cudaGetLastError());
+  std::vector<int32_t> status((size_t)n);
+  CK(cudaMemcpyAsync(status.data(), ctx->d_record_status.p, sizeof(int32_t) * (size_t)n, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  for (int i = 0; i < n; ++i)
+    if (status[(size_t)i] != REC_OK) return ctx->fail(HT_ERR_ARG, "record %d: %s", i, record_problem(status[(size_t)i]));
+  k_tracker_import<<<(unsigned)n, 256, 0, st>>>(ctx->d_slots.as<int32_t>(), src, ctx->d_tracker_state.as<TrackerState>(),
+                                                ctx->d_tracker_params.as<TrackerParams>(), ctx->track_state.as<TrackState>(),
+                                                ctx->model_hist.as<uint32_t>(), ctx->d_track_cost.as<int32_t>());
+  ++ctx->launches;
+  CK(cudaGetLastError());
+  CK(cudaStreamSynchronize(st));
+  return HT_OK;
+}
+
 int ht_tracker_reset(ht_ctx *ctx, int first, int n) { return tracker_control(ctx, first, n, 0); }
 int ht_tracker_start(ht_ctx *ctx, int first, int n) { return tracker_control(ctx, first, n, 1); }
 int ht_tracker_stop(ht_ctx *ctx, int first, int n) { return tracker_control(ctx, first, n, 2); }
@@ -1953,7 +2056,8 @@ static int tracker_tick(ht_ctx *ctx, const TickGroup *grp, int n_groups, const u
   ctx->prof_begin(HT_PROF_TRACK_INIT, st);
   // calc_angles -1: each entry's own, from its stream's parameters (k_tracker_update)
   k_track_init<<<n, 256, 0, st>>>(d_rgba, frame_bytes, g0.w, g0.h, d_ids, ctx->d_rects.as<int32_t>(), -1,
-                                  ctx->model_hist.as<uint32_t>(), ctx->track_state.as<TrackState>(), nullptr, init_en, geo);
+                                  ctx->model_hist.as<uint32_t>(), ctx->track_state.as<TrackState>(), nullptr, init_en, geo,
+                                  ctx->d_track_cost.as<int32_t>());
   ctx->prof_end(st);
   ctx->launches += 2;
   CK(cudaGetLastError());
@@ -2490,6 +2594,43 @@ extern "C" int ht_selftest_tracker(void *state, int op, const ht_tracker_params 
     memcpy(out, &e, sizeof(e));
   }
   return s.mode;
+}
+
+// Tracker records on the host, through the functions the kernels use.  `params` here is TrackerParams as the device
+// holds it (ht_selftest_tracker_params converts an ht_tracker_params; ht_selftest_tracker_params_size() bytes).
+extern "C" int ht_selftest_tracker_params_size(void) { return (int)sizeof(TrackerParams); }
+extern "C" int ht_selftest_tracker_params(const ht_tracker_params *params, void *out) {
+  const TrackerParams tp = make_tracker_params(params);
+  memcpy(out, &tp, sizeof(tp));
+  return 0;
+}
+// k_tracker_export for one stream: state (TrackerState), params, track (TrackState), hist[4096], cost[2] -> rec
+extern "C" int ht_selftest_tracker_pack(const void *state, const void *params, const void *track, const uint32_t *hist,
+                                        const int32_t *cost, uint8_t *rec) {
+  TrackerState s;
+  TrackerParams p;
+  TrackState t;
+  memcpy(&s, state, sizeof(s));
+  memcpy(&p, params, sizeof(p));
+  memcpy(&t, track, sizeof(t));
+  tracker_record_pack(rec, s, p, t, hist, cost);
+  return REC_BYTES;
+}
+// k_tracker_import_check for one record -> REC_OK (0) or the first failed check
+extern "C" int ht_selftest_tracker_check(const uint8_t *rec) { return tracker_record_check(rec, tracker_record_sum(rec)); }
+// k_tracker_import for one checked record -> the sections, as ht_selftest_tracker_pack takes them
+extern "C" int ht_selftest_tracker_unpack(const uint8_t *rec, void *state, void *params, void *track, uint32_t *hist,
+                                          int32_t *cost) {
+  TrackerState s;
+  TrackerParams p;
+  TrackState t;
+  const bool cs = rec_word(rec, REC_STATE / 4) == (uint32_t)TM_CS;
+  for (int i = 0; i < REC_HEAD_WORDS; ++i) tracker_record_unpack_word(i, rec_word(rec, i), cs, s, p, t, cost);
+  for (int i = 0; i < 4096; ++i) hist[i] = cs ? rec_word(rec + REC_HIST, i) : 0u;
+  memcpy(state, &s, sizeof(s));
+  memcpy(params, &p, sizeof(p));
+  memcpy(track, &t, sizeof(t));
+  return 0;
 }
 
 // k_debug_table's per-bin code: table[DBG_TAB] of one stream's model and current histograms -> DBG_TAB

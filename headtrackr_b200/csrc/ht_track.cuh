@@ -8,6 +8,7 @@
 #pragma once
 #include <cooperative_groups.h>
 
+#include <cstring>
 #include <limits>
 
 #include "ht_common.cuh"
@@ -72,13 +73,15 @@ __global__ void __launch_bounds__(256) k_hist(const uint8_t *__restrict__ rgba, 
 // _trackObj := new TrackObj().  rects == NULL -> take the rectangle from det_pick (device pick).
 // calc_angles < 0 (ht_tracker_step / feed): per entry, enable[k] & 2 (k_tracker_update sets it from the stream's
 // parameters).  geo (ht_tracker_feed, else NULL): per-entry canvas size and place in the arena, instead of W, H and
-// frame k at k * frame_bytes.
+// frame k at k * frame_bytes.  cost (ht_tracker_step / feed, else NULL): a seeded slot's k_track scheduling history
+// starts over, so that the whole camshift section of a tracker stream follows from its last hand-off (tracker records).
 __global__ void __launch_bounds__(256) k_track_init(const uint8_t *__restrict__ rgba, size_t frame_bytes, int W, int H,
                                                     const int32_t *__restrict__ slots,
                                                     const int32_t *__restrict__ rects, int calc_angles,
                                                     uint32_t *__restrict__ model_hist, TrackState *__restrict__ state,
                                                     int32_t *__restrict__ found, const uint8_t *__restrict__ enable,
-                                                    const EntryCanvas *__restrict__ geo = nullptr) {
+                                                    const EntryCanvas *__restrict__ geo = nullptr,
+                                                    int32_t *__restrict__ cost = nullptr) {
   __shared__ uint32_t sh[4096];
   const int k = blockIdx.x;
   if (enable && !enable[k]) return;            // ht_stream_step: only the streams that just found a face
@@ -123,6 +126,7 @@ __global__ void __launch_bounds__(256) k_track_init(const uint8_t *__restrict__ 
     s.initialised = 1;
     state[slot] = s;
     if (found) found[k] = 1;
+    if (cost) cost[2 * slot] = cost[2 * slot + 1] = 0;
   }
 }
 
@@ -1368,6 +1372,194 @@ __global__ void k_tracker_control(TrackerState *st, int first, int n, int op) {
   if (op == 0) tracker_new_state(s);
   else if (op == 1) tracker_start(s);
   else tracker_stop(s);
+}
+
+// the parameter check of ht_tracker_config / ht_tracker_set_params, also applied to imported records
+__host__ __device__ inline bool tracker_head_ok(double alpha, double distance_to_screen) {
+  return alpha >= 0.0 && alpha <= 1.0 && distance_to_screen > 0.0;
+}
+
+// ------------------------------------------------------------------------------------------------
+// Tracker records (ht_tracker_export / ht_tracker_import): one stream's whole headtrackr.Tracker as a fixed-size,
+// position-independent, little-endian byte string, so that a stream can move to another slot, context or GPU and
+// outlive its process.  Byte offsets (include/headtrackr_b200.h; every section 16-byte aligned, the gaps zero):
+//   0           header: u32 magic "HTR1", u32 format version, u32 record bytes, u32 0, u64 checksum, u32 0, u32 0
+//   REC_STATE   TrackerState, as tracker_step keeps it
+//   REC_PARAMS  TrackerParams as the device holds them (the head-model constants travel: import does not recompute them)
+//   REC_TRACK   camshift section: the slot's TrackState, then (REC_COST) its two d_track_cost words, then
+//   REC_HIST    its 4096-bin model histogram
+// checksum = sum of w_i * (2i + 1) mod 2^64 over the 32-bit words from byte 24 on (i = 0, 1, ...): a flipped bit changes
+// it (2^b times an odd number is never 0 mod 2^64), and so does swapping two unequal words (2 |j - i| |w_i - w_j| <
+// 2^64).  Canonical form: the camshift section of a stream that is not in CS is dead state (the next hand-off re-seeds
+// it) and is written as zeros, so export(import(r)) == r and two exports of one state are byte-identical.
+constexpr uint32_t REC_MAGIC = 0x31525448u;        // "HTR1"
+constexpr uint32_t REC_VERSION = 1;
+__host__ __device__ constexpr int rec_align16(size_t b) { return (int)((b + 15) / 16 * 16); }
+constexpr int REC_STATE = 32;
+constexpr int REC_PARAMS = rec_align16(REC_STATE + sizeof(TrackerState));
+constexpr int REC_TRACK = rec_align16(REC_PARAMS + sizeof(TrackerParams));
+constexpr int REC_COST = REC_TRACK + (int)sizeof(TrackState);
+constexpr int REC_HIST = rec_align16(REC_COST + 2 * sizeof(int32_t));
+constexpr int REC_BYTES = REC_HIST + 4096 * (int)sizeof(uint32_t);
+constexpr int REC_HEAD_WORDS = REC_HIST / 4;       // the words before the histogram
+constexpr int REC_SUM0 = 6;                        // the first word under the checksum
+static_assert(sizeof(TrackerState) % 4 == 0 && sizeof(TrackerParams) % 4 == 0 && sizeof(TrackState) % 4 == 0 &&
+                  REC_BYTES % 16 == 0, "tracker record sections are whole words, the record whole 16-byte vectors");
+// import status of a record, in the order the checks run
+enum { REC_OK = 0, REC_BAD_MAGIC, REC_BAD_VERSION, REC_BAD_SIZE, REC_BAD_CHECKSUM, REC_BAD_MODE, REC_BAD_WB, REC_BAD_DIAG,
+       REC_BAD_PARAMS, REC_BAD_TRACK };
+
+__host__ __device__ inline uint32_t rec_word(const void *p, int j) {
+  uint32_t w;
+  memcpy(&w, static_cast<const char *>(p) + 4 * j, 4);
+  return w;
+}
+__host__ __device__ inline void rec_put(void *p, int j, uint32_t w) { memcpy(static_cast<char *>(p) + 4 * j, &w, 4); }
+__host__ __device__ __forceinline__ unsigned long long rec_term(int i, uint32_t w) {   // word i's share of the checksum
+  return (unsigned long long)w * (2ull * (unsigned)(i - REC_SUM0) + 1ull);
+}
+
+// word i < REC_HEAD_WORDS of a stream's record, the checksum words (4, 5) as 0.  cs: the stream is in CS, so its
+// camshift section is live.
+__host__ __device__ inline uint32_t tracker_record_head_word(int i, const TrackerState &s, const TrackerParams &p,
+                                                             const TrackState &t, const int32_t *cost, bool cs) {
+  const int b = 4 * i;
+  if (i == 0) return REC_MAGIC;
+  if (i == 1) return REC_VERSION;
+  if (i == 2) return (uint32_t)REC_BYTES;
+  if (b >= REC_STATE && b < REC_STATE + (int)sizeof(TrackerState)) return rec_word(&s, (b - REC_STATE) / 4);
+  if (b >= REC_PARAMS && b < REC_PARAMS + (int)sizeof(TrackerParams)) return rec_word(&p, (b - REC_PARAMS) / 4);
+  if (!cs) return 0;
+  if (b >= REC_TRACK && b < REC_COST) return rec_word(&t, (b - REC_TRACK) / 4);
+  if (b >= REC_COST && b < REC_COST + 8) return (uint32_t)cost[(b - REC_COST) / 4];
+  return 0;
+}
+
+// word i < REC_HEAD_WORDS of a checked record, w, into the stream's sections; cs: the record's mode is CS (otherwise
+// its camshift section is stored as zeros, whatever the record holds)
+__host__ __device__ inline void tracker_record_unpack_word(int i, uint32_t w, bool cs, TrackerState &s, TrackerParams &p,
+                                                           TrackState &t, int32_t *cost) {
+  const int b = 4 * i;
+  if (b >= REC_STATE && b < REC_STATE + (int)sizeof(TrackerState)) rec_put(&s, (b - REC_STATE) / 4, w);
+  else if (b >= REC_PARAMS && b < REC_PARAMS + (int)sizeof(TrackerParams)) rec_put(&p, (b - REC_PARAMS) / 4, w);
+  else if (b >= REC_TRACK && b < REC_COST) rec_put(&t, (b - REC_TRACK) / 4, cs ? w : 0u);
+  else if (b >= REC_COST && b < REC_COST + 8) cost[(b - REC_COST) / 4] = cs ? (int32_t)w : 0;
+}
+
+// The whole record of a stream, sequentially (k_tracker_export does the same per word with one CTA).  hist: the
+// slot's model histogram; track, hist and cost are read only when the stream is in CS.
+__host__ __device__ inline void tracker_record_pack(uint8_t *rec, const TrackerState &s, const TrackerParams &p,
+                                                    const TrackState &t, const uint32_t *hist, const int32_t *cost) {
+  const bool cs = s.mode == TM_CS;
+  unsigned long long sum = 0;
+  for (int i = 0; i < REC_BYTES / 4; ++i) {
+    const uint32_t w = i < REC_HEAD_WORDS ? tracker_record_head_word(i, s, p, t, cost, cs) : cs ? hist[i - REC_HEAD_WORDS] : 0u;
+    rec_put(rec, i, w);
+    if (i >= REC_SUM0) sum += rec_term(i, w);
+  }
+  memcpy(rec + 16, &sum, 8);
+}
+
+// the checksum of a record's words, sequentially (k_tracker_import_check sums them with one CTA)
+__host__ __device__ inline unsigned long long tracker_record_sum(const uint8_t *rec) {
+  unsigned long long sum = 0;
+  for (int i = REC_SUM0; i < REC_BYTES / 4; ++i) sum += rec_term(i, rec_word(rec, i));
+  return sum;
+}
+
+// The checks of import, given the checksum of the record's words: the header, the checksum, then every field that
+// indexes an array or selects a branch.  -> REC_OK or the first failed check.
+__host__ __device__ inline int tracker_record_check(const uint8_t *rec, unsigned long long sum) {
+  if (rec_word(rec, 0) != REC_MAGIC) return REC_BAD_MAGIC;
+  if (rec_word(rec, 1) != REC_VERSION) return REC_BAD_VERSION;
+  if (rec_word(rec, 2) != (uint32_t)REC_BYTES || rec_word(rec, 3) != 0u) return REC_BAD_SIZE;
+  unsigned long long stored;
+  memcpy(&stored, rec + 16, 8);
+  if (stored != sum) return REC_BAD_CHECKSUM;
+  TrackerState s;
+  TrackerParams p;
+  TrackState t;
+  memcpy(&s, rec + REC_STATE, sizeof(s));
+  memcpy(&p, rec + REC_PARAMS, sizeof(p));
+  memcpy(&t, rec + REC_TRACK, sizeof(t));
+  if (s.mode < TM_IDLE || s.mode > TM_CS) return REC_BAD_MODE;
+  if (s.n_wb < 0 || s.n_wb > WB_WINDOW) return REC_BAD_WB;
+  if (s.head.n_diag < 0 || s.head.n_diag > 6) return REC_BAD_DIAG;              // head_step: s.diag[s.n_diag++]
+  if (!tracker_head_ok(p.head.alpha, p.head.distance_to_screen)) return REC_BAD_PARAMS;
+  if (s.mode == TM_CS && !(t.initialised == 1 && t.sw > 0 && t.sh > 0)) return REC_BAD_TRACK;   // k_track's window
+  return REC_OK;
+}
+
+// sum of v over the CTA (256 threads), valid in thread 0
+__device__ __forceinline__ unsigned long long cta_sum_u64(unsigned long long v, unsigned long long *part) {
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
+  if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = v;
+  __syncthreads();
+  unsigned long long s = 0;
+  if (threadIdx.x == 0)
+    for (int w = 0; w < 8; ++w) s += part[w];
+  return s;
+}
+
+// Record k of `records` (16-byte aligned, REC_BYTES apart) := stream ids[k].  One CTA per record: the head word by word,
+// the histogram in 16-byte vectors (zeros when the stream is not in CS), then the checksum.
+__global__ void __launch_bounds__(256) k_tracker_export(const int32_t *__restrict__ ids, const TrackerState *__restrict__ st,
+                                                        const TrackerParams *__restrict__ params,
+                                                        const TrackState *__restrict__ track,
+                                                        const uint32_t *__restrict__ model_hist,
+                                                        const int32_t *__restrict__ cost, uint8_t *__restrict__ records) {
+  __shared__ unsigned long long part[8];
+  const int id = ids[blockIdx.x];
+  uint8_t *rec = records + (size_t)blockIdx.x * REC_BYTES;
+  const bool cs = st[id].mode == TM_CS;
+  unsigned long long sum = 0;
+  for (int i = threadIdx.x; i < REC_HEAD_WORDS; i += 256) {
+    if (i == 4 || i == 5) continue;                // the checksum, written last
+    const uint32_t w = tracker_record_head_word(i, st[id], params[id], track[id], cost + 2 * (size_t)id, cs);
+    reinterpret_cast<uint32_t *>(rec)[i] = w;
+    if (i >= REC_SUM0) sum += rec_term(i, w);
+  }
+  const uint4 *src = reinterpret_cast<const uint4 *>(model_hist + (size_t)id * 4096);
+  uint4 *dst = reinterpret_cast<uint4 *>(rec + REC_HIST);
+  for (int j = threadIdx.x; j < 1024; j += 256) {
+    const uint4 v = cs ? src[j] : make_uint4(0u, 0u, 0u, 0u);
+    dst[j] = v;
+    const int i = REC_HEAD_WORDS + 4 * j;
+    sum += rec_term(i, v.x) + rec_term(i + 1, v.y) + rec_term(i + 2, v.z) + rec_term(i + 3, v.w);
+  }
+  sum = cta_sum_u64(sum, part);
+  if (threadIdx.x == 0) *reinterpret_cast<unsigned long long *>(rec + 16) = sum;
+}
+
+// status[k] := tracker_record_check of record k.  One CTA per record, the checksum in 16-byte vectors.
+__global__ void __launch_bounds__(256) k_tracker_import_check(const uint8_t *__restrict__ records, int32_t *__restrict__ status) {
+  __shared__ unsigned long long part[8];
+  const uint8_t *rec = records + (size_t)blockIdx.x * REC_BYTES;
+  const uint4 *v = reinterpret_cast<const uint4 *>(rec);
+  unsigned long long sum = 0;
+  for (int j = threadIdx.x; j < REC_BYTES / 16; j += 256) {
+    const uint4 q = v[j];
+    const int i = 4 * j;
+    if (j == 1) sum += rec_term(6, q.z) + rec_term(7, q.w);          // words 4 and 5 are the checksum itself
+    else if (j > 1) sum += rec_term(i, q.x) + rec_term(i + 1, q.y) + rec_term(i + 2, q.z) + rec_term(i + 3, q.w);
+  }
+  sum = cta_sum_u64(sum, part);
+  if (threadIdx.x == 0) status[blockIdx.x] = tracker_record_check(rec, sum);
+}
+
+// stream ids[k] := record k (checked by k_tracker_import_check).  One CTA per record.
+__global__ void __launch_bounds__(256) k_tracker_import(const int32_t *__restrict__ ids, const uint8_t *__restrict__ records,
+                                                        TrackerState *__restrict__ st, TrackerParams *__restrict__ params,
+                                                        TrackState *__restrict__ track, uint32_t *__restrict__ model_hist,
+                                                        int32_t *__restrict__ cost) {
+  const int id = ids[blockIdx.x];
+  const uint8_t *rec = records + (size_t)blockIdx.x * REC_BYTES;
+  const bool cs = rec_word(rec, REC_STATE / 4) == (uint32_t)TM_CS;   // TrackerState::mode
+  for (int i = threadIdx.x; i < REC_HEAD_WORDS; i += 256)
+    tracker_record_unpack_word(i, rec_word(rec, i), cs, st[id], params[id], track[id], cost + 2 * (size_t)id);
+  const uint4 *src = reinterpret_cast<const uint4 *>(rec + REC_HIST);
+  uint4 *dst = reinterpret_cast<uint4 *>(model_hist + (size_t)id * 4096);
+  for (int j = threadIdx.x; j < 1024; j += 256) dst[j] = cs ? src[j] : make_uint4(0u, 0u, 0u, 0u);
 }
 
 }  // namespace ht

@@ -10,6 +10,7 @@ for records with detection == "CS" (src/facetrackr.js:112-125).
 import math
 import time
 
+from . import _lib
 from .context import tracker_events_from_bytes
 
 
@@ -252,6 +253,38 @@ class TrackerSet:
                 if e["type"] == "facetrackingEvent":
                     e["time"] = dt
                 self._emit(k, e)
+
+    def snapshot(self, ks, device=False):
+        """The Trackers of streams ks as they stand: {"records": their tracker records (Context.tracker_export; a torch
+        CUDA tensor on this context's device if `device`, else numpy), and the fields a Tracker has on the host:
+        "status" (ht.status, derived from the events), "current" (the last record, for debug_calls), "fov" (getFOV)}."""
+        ks = [int(k) for k in ks]
+        if device:
+            import torch
+            out = torch.empty((len(ks), _lib.TRACKER_RECORD_BYTES), dtype=torch.uint8, device=f"cuda:{self.ctx.device}")
+            recs = self.ctx.tracker_export(ks, out=out)
+            self.ctx.sync()                            # the records are written on the library's stream
+        else:
+            recs = self.ctx.tracker_export(ks)
+        return dict(records=recs, status=[self.status[k] for k in ks], current=[self.current[k] for k in ks],
+                    fov=[self._fov[k] for k in ks])
+
+    def restore(self, ks, snap):
+        """Streams ks of this set become the Trackers of a snapshot, taken from any set, context or GPU: the records go
+        to this context's device through the host, or by a torch copy when they are on another device.  Each stream
+        keeps its debug canvas."""
+        ks = [int(k) for k in ks]
+        for k in ks:
+            if not 0 <= k < self.n:
+                raise ValueError(f"stream {k} outside [0, {self.n})")
+        recs = snap["records"]
+        if hasattr(recs, "is_cuda") and recs.is_cuda:
+            import torch
+            recs = recs.to(f"cuda:{self.ctx.device}")
+            torch.cuda.synchronize(recs.device)        # torch's copy runs on its stream, the import on the library's
+        self.ctx.tracker_import(ks, recs)
+        for k, s, cur, fov in zip(ks, snap["status"], snap["current"], snap["fov"]):
+            self.status[k], self.current[k], self._fov[k] = s, cur, fov
 
     def debug_calls(self, k):
         """debug_calls of stream k's last record"""

@@ -340,6 +340,43 @@ typedef struct {
  * HT_ERR_SIZE for a size outside 1..16384. */
 int ht_tracker_set_debug(ht_ctx *ctx, int first, int n, const ht_debug_canvas *canvases);
 
+/* Tracker records: a stream's whole headtrackr.Tracker as one fixed-size, position-independent, little-endian byte
+ * string without pointers, so that a stream can move to another id, context or GPU, be cloned, or outlive its process.
+ * Layout (byte offsets; the gaps between sections are zero):
+ *       0  u32 magic HT_TRACKER_RECORD_MAGIC ("HTR1"), u32 format version HT_TRACKER_RECORD_VERSION,
+ *          u32 record size HT_TRACKER_RECORD_BYTES, u32 0
+ *      16  u64 checksum = sum of w_i * (2i + 1) mod 2^64 over the u32 words w_0, w_1, ... from byte 24 to the end
+ *      32  the lifecycle state (280 bytes): mode, whitebalance window, "hints" timer, faceFound, Smoother, head
+ *          diagonals, fov estimate, headposition state
+ *     320  the stream's parameters as the device holds them (88 bytes, with the head-model constants)
+ *     416  camshift section: the tracker (48 bytes: search window, TrackObj, angle, calcAngles, initialised),
+ *     464  its two scheduling-history words (a pass count and window pixels / 256 of its last track()),
+ *     480  its 4096-bin model histogram (u32)
+ * Canonical form: when the stream's mode is not CS the camshift section is dead state (the next hand-off re-seeds it)
+ * and is exported as zeros; so exporting an imported record gives the same bytes, and two exports of one state are
+ * identical whatever the slot held before. */
+#define HT_TRACKER_RECORD_BYTES 16864
+#define HT_TRACKER_RECORD_MAGIC 0x31525448u
+#define HT_TRACKER_RECORD_VERSION 1u
+/* records[i] (HT_TRACKER_RECORD_BYTES each, contiguous) := stream streams[i], for i in [0, n).  One launch.
+ *   streams: HOST array of n distinct ids in [0, max_frames), 1 <= n <= max_frames.
+ *   records: host memory (returns after the records have landed) or 16-byte aligned device memory of the context's
+ *            device (enqueue only: use ht_sync, or stream order on the context's stream).
+ * Errors (nothing is enqueued): HT_ERR_STATE before ht_tracker_config; HT_ERR_ARG for n out of range, NULL pointers,
+ * a device `streams`, an id out of range or listed twice, or device records of another device or misaligned. */
+int ht_tracker_export(ht_ctx *ctx, const int32_t *streams, int n, void *records);
+/* Stream streams[i] := records[i], for i in [0, n): its lifecycle state, parameters and camshift tracker become exactly
+ * the exported stream's, and what it held before is discarded.  Its debug canvas (ht_tracker_set_debug) stays as it
+ * was: that is a device resource of this stream id, not part of the Tracker's state.  streams and records as for
+ * ht_tracker_export; the source and the destination may be one context (clone: import into an idle id; swap: export
+ * [a, b], import [b, a]).  Every record is checked on the device first - magic, format version (records of another
+ * version are rejected, not converted), size, checksum, and every field that indexes an array or selects a branch:
+ * mode in [0, 4], whitebalance samples in [0, 15], head diagonals in [0, 6], the parameters ht_tracker_set_params
+ * accepts, and for a CS stream an initialised camshift tracker with a positive window - and the call synchronises.
+ * Any failure is HT_ERR_ARG naming the first bad record in ht_last_error, and no stream changes.  On success the call
+ * returns after the records have been consumed (also device records).  Two launches, whatever n. */
+int ht_tracker_import(ht_ctx *ctx, const int32_t *streams, int n, const void *records);
+
 /* Frame ingest (SURVEY.md 8f-4): canvasContext.drawImage(videoElement, 0, 0, canvas.width, canvas.height)
  * (src/main.js:170) for n frames - the video frame (sw x sh) scaled onto the working canvas (dw x dh), all four
  * channels, with the canvas resampler this build defines (DESIGN.md 2).  src and dst may be host or device

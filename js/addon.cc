@@ -24,6 +24,8 @@
 //   trackerStep(handle, rgba /* n canvases */, n, w, h, nowMs) -> Array<{detection, status: [...], running, fov, ...}>
 //   trackerSetParams(handle, first, [params, ...])   (ht_tracker_set_params: each stream its own Tracker parameters)
 //   trackerSetDebug(handle, first, [canvas|null, ...])  (ht_tracker_set_debug: each stream's debug canvas, device memory)
+//   trackerExport(handle, [stream, ...]) -> Buffer of records; trackerImport(handle, [stream, ...], records)
+//        (ht_tracker_export / ht_tracker_import: a stream's whole Tracker as HT_TRACKER_RECORD_BYTES per stream)
 //   trackerFeed(handle, [{stream, rgba, width, height, nowMs, canvasWidth?, canvasHeight?}], canvasWidth, canvasHeight)
 //        -> Array<record> (ht_tracker_feed_canvases: only the listed streams tick, each from its own video frame, clock
 //        and canvas)
@@ -442,6 +444,51 @@ static napi_value TrackerSetDebug(napi_env env, napi_callback_info info) {
   return nullptr;
 }
 
+// stream ids of an Array of numbers
+static bool GetStreams(napi_env env, napi_value arr, std::vector<int32_t> *ids) {
+  uint32_t n = 0;
+  if (napi_get_array_length(env, arr, &n) != napi_ok) return false;
+  ids->assign(n, -1);
+  for (uint32_t i = 0; i < n; ++i) {
+    napi_value v;
+    if (napi_get_element(env, arr, i, &v) != napi_ok || napi_get_value_int32(env, v, &(*ids)[i]) != napi_ok) return false;
+  }
+  return true;
+}
+
+// trackerExport(handle, [stream, ...]) -> Buffer of streams.length tracker records (ht_tracker_export)
+static napi_value TrackerExport(napi_env env, napi_callback_info info) {
+  size_t argc = 2;
+  napi_value argv[2];
+  NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+  ht_ctx *ctx = Ctx(env, argv[0]);
+  std::vector<int32_t> ids;
+  if (!GetStreams(env, argv[1], &ids)) return Throw(env, ctx, HT_ERR_ARG);
+  void *data = nullptr;
+  napi_value buf;
+  NAPI_OK(napi_create_buffer(env, ids.size() * HT_TRACKER_RECORD_BYTES, &data, &buf));
+  int rc = ht_tracker_export(ctx, ids.data(), (int)ids.size(), data);
+  if (rc < 0) return Throw(env, ctx, rc);
+  return buf;
+}
+
+// trackerImport(handle, [stream, ...], records: Buffer | TypedArray of streams.length records) (ht_tracker_import)
+static napi_value TrackerImport(napi_env env, napi_callback_info info) {
+  size_t argc = 3;
+  napi_value argv[3];
+  NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+  ht_ctx *ctx = Ctx(env, argv[0]);
+  std::vector<int32_t> ids;
+  uint8_t *recs;
+  size_t len;
+  if (!GetStreams(env, argv[1], &ids) || !GetBytes(env, argv[2], &recs, &len) ||
+      len != ids.size() * HT_TRACKER_RECORD_BYTES)
+    return Throw(env, ctx, HT_ERR_ARG);
+  int rc = ht_tracker_import(ctx, ids.data(), (int)ids.size(), recs);
+  if (rc < 0) return Throw(env, ctx, rc);
+  return nullptr;
+}
+
 // trackerReset / trackerStart / trackerStop(handle, first, n)
 static napi_value TrackerRange(napi_env env, napi_callback_info info, int (*fn)(ht_ctx *, int, int)) {
   size_t argc = 3;
@@ -558,6 +605,8 @@ static napi_value Init(napi_env env, napi_value exports) {
       {"trackerStep", nullptr, TrackerStep, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerSetParams", nullptr, TrackerSetParams, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerSetDebug", nullptr, TrackerSetDebug, nullptr, nullptr, nullptr, napi_default, nullptr},
+      {"trackerExport", nullptr, TrackerExport, nullptr, nullptr, nullptr, napi_default, nullptr},
+      {"trackerImport", nullptr, TrackerImport, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerFeed", nullptr, TrackerFeed, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"create", nullptr, Create, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"detect", nullptr, Detect, nullptr, nullptr, nullptr, napi_default, nullptr},

@@ -8,6 +8,8 @@ streams: N 640x480 streams, device-resident frames and outputs, CUDA events arou
   feed_*          ht_tracker_feed against ht_ingest + ht_tracker_step and ht_tracker_step (feed_arms)
   canvases_*      ht_tracker_feed_canvases on four canvas sizes against four one-size ht_tracker_feed calls, and
                   one-size ht_tracker_feed against another build of the library (--before-lib) (canvas_arms)
+  migrate_*       (--migrate) ht_tracker_export + ht_tracker_import of every stream, device to device and through
+                  pinned host memory, and a steady tick before and after an import (migrate_arms)
   debug_*         (--debug-streams) ht_tracker_feed with debug canvases on none, 1/64 and all of the streams, the
                   achieved bandwidth of k_debug_backproj, and the no-debug arm against --before-lib (debug_arms)
 
@@ -425,6 +427,97 @@ def debug_arms(torch, frames, stream, N, W, H, steps, rounds, before_lib=None):
     return res
 
 
+def migrate_arms(torch, frames, stream, N, W, H, steps, rounds):
+    """Tracker records (ht_tracker_export / ht_tracker_import) of N streams in steady tracking, W x H video on W/2 x H/2
+    canvases, CUDA events on the library's stream around each call, repeated `rounds` x `steps` times:
+
+      migrate_d2d       export of every stream into device memory + import of those records into a second context
+      migrate_host      the same through pinned host memory (export returns after the records have landed; import
+                        stages them on the device, checks them, synchronises and scatters)
+      tick_before / tick_after   one steady-state ht_tracker_feed tick of the source context and of the destination
+                        after the import, alternating arm by arm: a migrated stream keeps its track() scheduling history
+                        (the d_track_cost words travel), so its tier placement should cost nothing
+
+    Achieved bytes/s: N * HT_TRACKER_RECORD_BYTES per direction (written by export, read by import's check and again
+    by its scatter; the model-histogram reads and writes on the device side are the same size again).  The records of
+    the two contexts' ticks must agree."""
+    import ctypes as C
+    from headtrackr_b200 import Context, _lib
+    R = _lib.TRACKER_RECORD_BYTES
+    CW, CH = W // 2, H // 2
+    rec_bytes = C.sizeof(_lib.TrackerEvent)
+    now = [1.0e12]
+    arr = (_lib.VideoFrame * N)()
+    for k in range(N):
+        arr[k] = _lib.VideoFrame(frames[k].data_ptr(), k, W, H, 0, 0.0)
+    src = Context(max_width=CW, max_height=CH, max_frames=N, stream=stream)
+    dst = Context(max_width=CW, max_height=CH, max_frames=N, stream=stream)
+    for c in (src, dst):
+        c.tracker_config(calcAngles=True)
+    src.tracker_start(0, N)
+    outs = {c: torch.empty(N * rec_bytes, dtype=torch.uint8, device="cuda") for c in (src, dst)}
+
+    def tick(c):
+        for k in range(N):
+            arr[k].now_ms = now[0]
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        a.record()
+        c._check(c._L.ht_tracker_feed(c._h, C.addressof(arr), N, 1, CW, CH, outs[c].data_ptr()))
+        b.record()
+        b.synchronize()
+        return a.elapsed_time(b)
+
+    for _ in range(20):                          # the whitebalance gate, detection, the first CS frames
+        now[0] += 20.0
+        tick(src)
+    ids = (C.c_int32 * N)(*range(N))
+    dev = torch.empty((N, R), dtype=torch.uint8, device="cuda")
+    host = torch.empty((N, R), dtype=torch.uint8, pin_memory=True)
+
+    def timed_call(fn):
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        a.record()
+        fn()
+        b.record()
+        b.synchronize()
+        return a.elapsed_time(b)
+
+    def exp(ptr):
+        return lambda: src._check(src._L.ht_tracker_export(src._h, C.addressof(ids), N, ptr))
+
+    def imp(ptr):
+        return lambda: dst._check(dst._L.ht_tracker_import(dst._h, C.addressof(ids), N, ptr))
+
+    t = {k: [] for k in ("export_d2d", "import_d2d", "export_host", "import_host", "tick_before", "tick_after")}
+    for _ in range(3):                           # warm-up of both paths
+        exp(dev.data_ptr())(), imp(dev.data_ptr())(), exp(host.data_ptr())(), imp(host.data_ptr())()
+    for _ in range(rounds * steps):
+        t["export_d2d"].append(timed_call(exp(dev.data_ptr())))
+        t["import_d2d"].append(timed_call(imp(dev.data_ptr())))
+        t["export_host"].append(timed_call(exp(host.data_ptr())))
+        t["import_host"].append(timed_call(imp(host.data_ptr())))
+    mismatches = 0
+    for _ in range(rounds * steps):              # both contexts hold the same streams: tick them alternately
+        now[0] += 20.0
+        t["tick_before"].append(tick(src))
+        t["tick_after"].append(tick(dst))
+        mismatches += int(not torch.equal(outs[src], outs[dst]))
+    if mismatches:
+        raise SystemExit(f"migrated streams disagree with the source on {mismatches} ticks")
+    res = {f"{k}_ms": float(np.median(v)) for k, v in t.items()}
+    res.update({f"{k}_min_ms": float(min(v)) for k, v in t.items()})
+    nbytes = N * R
+    res["record_bytes"], res["migrate_bytes"] = R, nbytes
+    for k in ("export_d2d", "import_d2d", "export_host", "import_host"):
+        res[f"{k}_GBps"] = nbytes / (res[f"{k}_ms"] * 1e-3) / 1e9
+    ev = [_lib.TrackerEvent.from_buffer_copy(bytes(row)) for row in outs[dst].cpu().numpy().reshape(N, rec_bytes)]
+    res["migrate_cs_streams"] = sum(e.detection == 2 for e in ev)
+    res["migrate_records_agree"] = True
+    src.close()
+    dst.close()
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--streams", type=int, default=1024)
@@ -433,6 +526,7 @@ def main():
     ap.add_argument("--before-lib", help="another build of libheadtrackr_b200.so for the one-size feed arm")
     ap.add_argument("--only-canvases", action="store_true", help="only the canvas arms (canvas_arms)")
     ap.add_argument("--debug-streams", action="store_true", help="only the debug-canvas arms (debug_arms)")
+    ap.add_argument("--migrate", action="store_true", help="only the tracker-record arms (migrate_arms)")
     ap.add_argument("--out")
     a = ap.parse_args()
     import torch
@@ -446,6 +540,9 @@ def main():
     ts = torch.cuda.Stream()                # the library runs on this stream and the events below are recorded on it
     torch.cuda.set_stream(ts)
     stream = ts.cuda_stream
+    if a.migrate:
+        res.update(migrate_arms(torch, frames, stream, N, W, H, a.steps, a.rounds))
+        return report(res, a.out)
     if a.debug_streams:
         res.update(debug_arms(torch, frames, stream, N, W, H, a.steps, a.rounds, a.before_lib))
         return report(res, a.out)
