@@ -82,6 +82,23 @@ class DebugCanvas(C.Structure):
                 ("pad_", C.c_int32)]
 
 
+class Camera(C.Structure):
+    """ht_camera: a stream's head-coupled camera (HT_CAMERA_BYTES, in device memory; camera_from_bytes decodes it)"""
+    _fields_ = [("position", C.c_double * 3), ("fov", C.c_double), ("view", C.c_double * 6), ("events", C.c_uint32),
+                ("has_view_offset", C.c_int32), ("projection", C.c_float * 16), ("view_matrix", C.c_float * 16),
+                ("pad_", C.c_uint32 * 2)]
+
+
+class CameraControl(C.Structure):
+    """ht_camera_control: one stream's realisticAbsoluteCameraControl for ht_tracker_set_camera (camera NULL = none)"""
+    _fields_ = [("camera", C.c_void_p), ("scaling", C.c_double), ("fixed_position", C.c_double * 3),
+                ("look_at", C.c_double * 3), ("screen_height", C.c_double), ("damping", C.c_double),
+                ("fov", C.c_double), ("aspect", C.c_double), ("near", C.c_double), ("far", C.c_double)]
+
+
+CAMERA_BYTES = 224
+assert C.sizeof(Camera) == CAMERA_BYTES and C.sizeof(CameraControl) == 112
+
 # ht_tracker_export / ht_tracker_import: bytes of one tracker record (HT_TRACKER_RECORD_BYTES)
 TRACKER_RECORD_BYTES = 16864
 
@@ -125,7 +142,7 @@ _lib = None
 
 EXPORTS = ["ht_version", "ht_create", "ht_destroy", "ht_last_error", "ht_sync", "ht_max_rects", "ht_detect",
            "ht_track_init", "ht_track_init_from_detect", "ht_track", "ht_detect_track", "ht_stream_reset", "ht_stream_step", "ht_stream_head_config", "ht_stream_step_head",
-           "ht_tracker_config", "ht_tracker_reset", "ht_tracker_start", "ht_tracker_stop", "ht_tracker_step", "ht_tracker_feed", "ht_tracker_set_params", "ht_tracker_feed_canvases", "ht_tracker_set_debug", "ht_tracker_export", "ht_tracker_import", "ht_ingest", "ht_backprojection", "ht_whitebalance",
+           "ht_tracker_config", "ht_tracker_reset", "ht_tracker_start", "ht_tracker_stop", "ht_tracker_step", "ht_tracker_feed", "ht_tracker_set_params", "ht_tracker_feed_canvases", "ht_tracker_set_debug", "ht_tracker_set_camera", "ht_tracker_export", "ht_tracker_import", "ht_ingest", "ht_backprojection", "ht_whitebalance",
            "ht_plan_info", "ht_debug_plane", "ht_debug_raw", "ht_debug_model_hist", "ht_debug_track_stats", "ht_set_track_memo", "ht_set_pipeline", "ht_join", "ht_debug_set_exactness", "ht_debug_track_trace", "ht_debug_track_phases", "ht_launch_count",
            "ht_profile", "ht_profile_read"]
 
@@ -169,6 +186,7 @@ def lib():
     L.ht_tracker_set_params.argtypes = [vp, C.c_int, C.c_int, vp]
     L.ht_tracker_feed_canvases.argtypes = [vp, vp, C.c_int, C.c_int, vp]
     L.ht_tracker_set_debug.argtypes = [vp, C.c_int, C.c_int, vp]
+    L.ht_tracker_set_camera.argtypes = [vp, C.c_int, C.c_int, vp]
     L.ht_tracker_export.argtypes = [vp, vp, C.c_int, vp]
     L.ht_tracker_import.argtypes = [vp, vp, C.c_int, vp]
     L.ht_ingest.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, vp, C.c_int, C.c_int]

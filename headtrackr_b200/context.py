@@ -8,7 +8,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from ._lib import (CanvasFrame, DebugCanvas, HeadEvent, HeadParams, HtError, Rect, StreamEvent, TrackerEvent, TrackerParams, TrackObj, VideoFrame,
+from ._lib import (Camera, CameraControl, CanvasFrame, DebugCanvas, HeadEvent, HeadParams, HtError, Rect, StreamEvent, TrackerEvent, TrackerParams, TrackObj, VideoFrame,
                    Window)
 from .synth import load_cascade_blob
 
@@ -32,6 +32,22 @@ def _frames_ptr(frames):
     if a.ndim != 4 or a.shape[-1] != 4:
         raise ValueError("frames must be (n,H,W,4) uint8")
     return a.ctypes.data, a.shape[0], a.shape[1], a.shape[2], a
+
+
+def camera_from_bytes(b):
+    """An ht_camera (CAMERA_BYTES bytes: numpy, bytes, or a torch tensor, copied to the host) -> dict: position [3],
+    fov, view [6] (fullWidth, fullHeight, x, y, width, height), events, has_view_offset, and projection and
+    view_matrix as float32 (4, 4) numpy arrays (row-major views of the column-major matrices, so m[row, col])."""
+    if _is_torch(b):
+        b = b.detach().cpu().numpy()
+    raw = np.frombuffer(bytes(np.ascontiguousarray(b, dtype=np.uint8).reshape(-1)), np.uint8)
+    if raw.size != _lib.CAMERA_BYTES:
+        raise ValueError(f"an ht_camera is {_lib.CAMERA_BYTES} bytes")
+    c = Camera.from_buffer_copy(raw.tobytes())
+    return dict(position=list(c.position), fov=c.fov, view=list(c.view), events=c.events,
+                has_view_offset=c.has_view_offset,
+                projection=np.frombuffer(raw[88:152].tobytes(), np.float32).reshape(4, 4).T.copy(),
+                view_matrix=np.frombuffer(raw[152:216].tobytes(), np.float32).reshape(4, 4).T.copy())
 
 
 def rect_to_dict(r, raw=False):
@@ -58,6 +74,7 @@ class Context:
         self.max_width, self.max_height, self.device = max_width, max_height, device
         self.last_warning = None
         self._debug = {}                  # stream -> its debug canvas tensor, kept alive while the library writes it
+        self._camera = {}                 # stream -> its camera tensor, likewise
 
     def close(self):
         if getattr(self, "_h", None) and self._h.value:
@@ -230,11 +247,13 @@ class Context:
         if not enable:
             self._check(self._L.ht_tracker_config(self._h, None))
             self._debug = {}
+            self._camera = {}
             return
         p = tracker_params(retryDetection, calcAngles, smoothing, fov, cameraOffset, headPosition, edgecorrection, alpha,
                            distance_to_screen)
         self._check(self._L.ht_tracker_config(self._h, C.addressof(p)))
         self._debug = {}                  # ht_tracker_config discards every debug canvas
+        self._camera = {}                 # and every camera controller
 
     def tracker_set_params(self, first, params):
         """Parameters of streams first, first+1, ...: one dict of tracker_config's keywords (enable excluded) per stream,
@@ -265,6 +284,35 @@ class Context:
                 self._debug.pop(int(first) + i, None)
             else:
                 self._debug[int(first) + i] = t
+
+    def tracker_set_camera(self, first, controls):
+        """Head-coupled camera controllers of streams first, first+1, ...: per stream None (none) or a dict of
+        realisticAbsoluteCameraControl's arguments (src/controllers.js:28-38) - scaling, fixedPosition, lookAt (three
+        numbers each), screenHeight (default 20), damping (default 1) - the camera's own fov, aspect, near and far, and
+        `out`: a torch CUDA uint8 tensor of CAMERA_BYTES bytes, 16-byte aligned, on this context's device (it may be a
+        slice of a larger renderer buffer).  Setting a controller writes the constructed camera; then every tick with a
+        headtrackingEvent moves it on the device (camera_from_bytes decodes it).  The context keeps the tensors
+        alive while they are set."""
+        controls = list(controls)
+        arr = (CameraControl * max(1, len(controls)))()
+        for i, d in enumerate(controls):
+            if d is None:
+                continue
+            t = d["out"]
+            if not _is_torch(t) or not t.is_cuda:
+                raise ValueError("a camera is a torch CUDA tensor")
+            if t.element_size() != 1 or t.numel() != _lib.CAMERA_BYTES or not t.is_contiguous():
+                raise ValueError(f"a camera is a contiguous uint8 tensor of {_lib.CAMERA_BYTES} bytes")
+            arr[i] = CameraControl(t.data_ptr(), float(d["scaling"]), tuple(float(v) for v in d["fixedPosition"]),
+                                   tuple(float(v) for v in d["lookAt"]), float(d.get("screenHeight", 20.0)),
+                                   float(d.get("damping", 1.0)), float(d["fov"]), float(d["aspect"]),
+                                   float(d["near"]), float(d["far"]))
+        self._check(self._L.ht_tracker_set_camera(self._h, int(first), len(controls), C.addressof(arr)))
+        for i, d in enumerate(controls):
+            if d is None:
+                self._camera.pop(int(first) + i, None)
+            else:
+                self._camera[int(first) + i] = d["out"]
 
     def tracker_export(self, streams, out=None):
         """The tracker records of the listed streams (ht_tracker_export): a (len(streams), TRACKER_RECORD_BYTES) uint8

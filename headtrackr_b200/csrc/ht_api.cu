@@ -574,6 +574,11 @@ struct ht_ctx {
   DevBuf d_debug, d_debug_tab;
   std::vector<DebugCanvas> h_debug;
   int debug_count = 0;
+  // ht_tracker_set_camera: per stream its CameraCtl (device array and host copy) and the number of streams that have
+  // one (0: a tick launches nothing for cameras)
+  DevBuf d_camera;
+  std::vector<CameraCtl> h_camera;
+  int camera_count = 0;
   // ht_tracker_feed(_canvases): the record table {ids[n], clocks[n], FeedRec[n], EntryCanvas[n], tile starts[n+1]}
   // goes up in one copy from pinned memory; the videos are drawn into the canvas arena (batch entry k's canvas at
   // EntryCanvas::base), zeroed when it grows
@@ -1744,6 +1749,11 @@ int ht_tracker_config(ht_ctx *ctx, const ht_tracker_params *params) {
     ctx->h_debug.assign(mf, DebugCanvas{});
     ctx->debug_count = 0;
   }
+  if (ctx->camera_count > 0) {   // and every camera controller
+    CK(cudaMemsetAsync(ctx->d_camera.p, 0, mf * sizeof(CameraCtl), ctx->stream));
+    ctx->h_camera.assign(mf, CameraCtl{});
+    ctx->camera_count = 0;
+  }
   if (!params) {                 // off: every stream as after ht_stream_reset (the lifecycle has used the tracker slots)
     if (ctx->tracker_on) {
       ctx->tracker_on = false;
@@ -1845,6 +1855,88 @@ int ht_tracker_set_debug(ht_ctx *ctx, int first, int n, const ht_debug_canvas *c
   CK(cudaStreamSynchronize(ctx->stream));    // `next` is a local
   ctx->debug_count = (int)spans.size();
   ctx->h_debug.swap(next);
+  return HT_OK;
+}
+
+static_assert(sizeof(ht_camera) == HT_CAMERA_BYTES && HT_CAMERA_BYTES == 224 && offsetof(ht_camera, fov) == 24 &&
+                  offsetof(ht_camera, view) == 32 && offsetof(ht_camera, events) == 80 &&
+                  offsetof(ht_camera, has_view_offset) == 84 && offsetof(ht_camera, projection) == 88 &&
+                  offsetof(ht_camera, view_matrix) == 152 && sizeof(ht_camera_control) == 112,
+              "ht_camera layout (include/headtrackr_b200.h)");
+
+// One stream's controller from its ht_camera_control (the camera pointer is the caller's to check).  -> NULL, or
+// what is wrong with it.
+static const char *camera_ctl_make(const ht_camera_control &c, CameraCtl *out) {
+  const double v[13] = {c.scaling, c.fixed_position[0], c.fixed_position[1], c.fixed_position[2], c.look_at[0],
+                        c.look_at[1], c.look_at[2], c.screen_height, c.damping, c.fov, c.aspect, c.near, c.far};
+  for (double x : v)
+    if (!std::isfinite(x)) return "a field is not finite";
+  if (!(c.aspect > 0.0)) return "aspect <= 0";
+  if (!(c.near > 0.0)) return "near <= 0";
+  if (!(c.far > c.near)) return "far <= near";
+  if (!(c.fov > 0.0 && c.fov < 180.0)) return "fov outside (0, 180)";
+  CameraCtl k{};
+  if (!camera_lookat(c.fixed_position, c.look_at, k.rot))
+    return "degenerate lookAt (fixedPosition == lookAt, or a view direction parallel to +y)";
+  k.camera = c.camera;
+  k.scaling = c.scaling; k.damping = c.damping;
+  k.wh = c.screen_height * c.scaling;
+  k.ww = k.wh * c.aspect;
+  for (int i = 0; i < 3; ++i) k.fixed[i] = c.fixed_position[i];
+  k.fov = c.fov; k.aspect = c.aspect; k.near_ = c.near; k.far_ = c.far;
+  *out = k;
+  return nullptr;
+}
+
+// The camera controllers of streams [first, first + n).  Everything is checked on the host before anything changes,
+// overlap over every stream that has a controller after the call; then one launch constructs the new cameras.
+int ht_tracker_set_camera(ht_ctx *ctx, int first, int n, const ht_camera_control *controls) {
+  if (!ctx) return HT_ERR_ARG;
+  if (!ctx->tracker_on) return ctx->fail(HT_ERR_STATE, "ht_tracker_config has not been called");
+  const int mf = ctx->cfg.max_frames;
+  if (first < 0 || n <= 0 || first > mf - n) return ctx->fail(HT_ERR_ARG, "stream range outside [0,%d)", mf);
+  if (!controls) return ctx->fail(HT_ERR_ARG, "controls is NULL");
+  std::vector<CameraCtl> next = ctx->h_camera;
+  next.resize((size_t)mf, CameraCtl{});
+  for (int i = 0; i < n; ++i) {
+    const ht_camera_control &c = controls[i];
+    CameraCtl k{};
+    if (c.camera) {
+      if (reinterpret_cast<uintptr_t>(c.camera) & 15u) return ctx->fail(HT_ERR_ARG, "record %d: camera must be 16-byte aligned", i);
+      cudaPointerAttributes a{};
+      if (cudaPointerGetAttributes(&a, c.camera) != cudaSuccess) { cudaGetLastError(); a.type = cudaMemoryTypeUnregistered; }
+      if (a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged)
+        return ctx->fail(HT_ERR_ARG, "record %d: camera is not device memory", i);
+      if (a.device != ctx->cfg.device)
+        return ctx->fail(HT_ERR_ARG, "record %d: camera is memory of device %d, the context is on device %d", i, a.device,
+                         ctx->cfg.device);
+      const char *why = camera_ctl_make(c, &k);
+      if (why) return ctx->fail(HT_ERR_ARG, "record %d: %s", i, why);
+    }
+    next[(size_t)(first + i)] = k;
+  }
+  // two cameras of one tick's streams must not share a byte
+  std::vector<uintptr_t> starts;
+  for (const CameraCtl &k : next)
+    if (k.camera) starts.push_back(reinterpret_cast<uintptr_t>(k.camera));
+  std::sort(starts.begin(), starts.end());
+  for (size_t i = 1; i < starts.size(); ++i)
+    if (starts[i] < starts[i - 1] + sizeof(ht_camera))
+      return ctx->fail(HT_ERR_ARG, "a camera overlaps another stream's camera");
+  { const int jr = join_aux(ctx); if (jr != HT_OK) return jr; }
+  CK(cudaSetDevice(ctx->cfg.device));
+  if (!ctx->d_camera.p) {
+    CK(ctx->d_camera.reserve((size_t)mf * sizeof(CameraCtl)));
+    CK(cudaMemsetAsync(ctx->d_camera.p, 0, (size_t)mf * sizeof(CameraCtl), ctx->stream));
+  }
+  CK(cudaMemcpyAsync(ctx->d_camera.as<CameraCtl>() + first, next.data() + first, (size_t)n * sizeof(CameraCtl),
+                     cudaMemcpyHostToDevice, ctx->stream));
+  k_camera_construct<<<1, 256, 0, ctx->stream>>>(ctx->d_camera.as<CameraCtl>(), first, n);
+  ++ctx->launches;
+  CK(cudaGetLastError());
+  CK(cudaStreamSynchronize(ctx->stream));    // `next` is a local
+  ctx->camera_count = (int)starts.size();
+  ctx->h_camera.swap(next);
   return HT_OK;
 }
 
@@ -2053,6 +2145,10 @@ static int tracker_tick(ht_ctx *ctx, const TickGroup *grp, int n_groups, const u
                                                     ctx->d_wb_sums.as<unsigned long long>(), g0.w * g0.h, ctx->d_best.as<Rect>(),
                                                     ctx->d_out_counts.as<int32_t>(), ctx->d_objs.as<int32_t>(),
                                                     ctx->d_rects.as<int32_t>(), init_en, now_ms, d_now, g0.w, g0.h, geo, d_ev);
+  if (ctx->camera_count > 0) {  // the cameras of the entries whose record has a headtrackingEvent
+    k_camera_update<<<(n + 127) / 128, 128, 0, st>>>(d_ids, geo, n, d_ev, ctx->d_camera.as<CameraCtl>());
+    ++ctx->launches;
+  }
   ctx->prof_begin(HT_PROF_TRACK_INIT, st);
   // calc_angles -1: each entry's own, from its stream's parameters (k_tracker_update)
   k_track_init<<<n, 256, 0, st>>>(d_rgba, frame_bytes, g0.w, g0.h, d_ids, ctx->d_rects.as<int32_t>(), -1,
@@ -2631,6 +2727,21 @@ extern "C" int ht_selftest_tracker_unpack(const uint8_t *rec, void *state, void 
   memcpy(params, &p, sizeof(p));
   memcpy(track, &t, sizeof(t));
   return 0;
+}
+
+// The camera controller of ht_tracker_set_camera on the host: op 0 checks `control` and constructs *camera as
+// k_camera_construct does (-> 0, or -1 where ht_tracker_set_camera rejects it); op 1 applies the headtrackingEvent
+// (x, y, z) as k_camera_update does (-> the camera's event count).  control->camera is not read.
+extern "C" int ht_selftest_camera(const ht_camera_control *control, int op, double x, double y, double z,
+                                  ht_camera *camera) {
+  CameraCtl k{};
+  if (camera_ctl_make(*control, &k)) return -1;
+  if (op == 0) {
+    camera_construct(*camera, k);
+    return 0;
+  }
+  camera_step(*camera, k, x, y, z);
+  return (int)camera->events;
 }
 
 // k_debug_table's per-bin code: table[DBG_TAB] of one stream's model and current histograms -> DBG_TAB

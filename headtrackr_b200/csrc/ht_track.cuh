@@ -1374,6 +1374,132 @@ __global__ void k_tracker_control(TrackerState *st, int first, int n, int op) {
   else tracker_stop(s);
 }
 
+// ------------------------------------------------------------------------------------------------
+// The head-coupled camera of a headtrackr.Tracker stream (ht_tracker_set_camera): realisticAbsoluteCameraControl
+// (src/controllers.js:28-68) on an ht_camera in device memory, and three.js r48's updateProjectionMatrix as DESIGN.md
+// 5.4 f10 restates it.  All in fp64 (the library builds with -fmad=false: every product rounds), the matrices rounded
+// once to float32.
+struct CameraCtl {              // one stream's controller; camera NULL: none
+  ht_camera *camera;
+  double scaling, damping;
+  double wh, ww;                // screenHeight * scaling, wh * camera.aspect (src/controllers.js:45-46)
+  double fixed[3];              // fixedPosition
+  double fov, aspect, near_, far_;   // the camera's own
+  double rot[9];                // R of lookAt(fixedPosition -> lookAt, up +y): columns x, y, z
+};
+
+// Matrix4.lookAt(eye, target, up = (0, 1, 0)) of r48 without its epsilon nudge: z = normalize(eye - target),
+// x = normalize(up x z) = normalize((z2, 0, -z0)), y = z x x.  -> false for a degenerate lookAt (eye == target, a
+// view direction parallel to up) or a non-finite axis.
+__host__ __device__ inline bool camera_lookat(const double eye[3], const double target[3], double rot[9]) {
+  double z[3] = {eye[0] - target[0], eye[1] - target[1], eye[2] - target[2]};
+  const double zn = sqrt(z[0] * z[0] + z[1] * z[1] + z[2] * z[2]);
+  if (!(zn > 0.0) || !(zn < HUGE_VAL)) return false;
+  for (int i = 0; i < 3; ++i) z[i] = z[i] / zn;
+  double x[3] = {z[2], 0.0, -z[0]};
+  const double xn = sqrt(x[0] * x[0] + x[1] * x[1] + x[2] * x[2]);
+  if (!(xn > 0.0)) return false;
+  for (int i = 0; i < 3; ++i) x[i] = x[i] / xn;
+  const double y[3] = {z[1] * x[2] - z[2] * x[1], z[2] * x[0] - z[0] * x[2], z[0] * x[1] - z[1] * x[0]};
+  for (int i = 0; i < 3; ++i) {
+    rot[i] = x[i]; rot[3 + i] = y[i]; rot[6 + i] = z[i];
+  }
+  for (int i = 0; i < 9; ++i)
+    if (!(fabs(rot[i]) <= 1.0)) return false;
+  return true;
+}
+
+// makeFrustum of r48 -> column-major float32
+__host__ __device__ inline void camera_frustum(double l, double r, double b, double t, double n, double f, float m[16]) {
+  for (int i = 0; i < 16; ++i) m[i] = 0.0f;
+  m[0] = (float)(2 * n / (r - l));
+  m[5] = (float)(2 * n / (t - b));
+  m[8] = (float)((r + l) / (r - l));
+  m[9] = (float)((t + b) / (t - b));
+  m[10] = (float)(-(f + n) / (f - n));
+  m[11] = -1.0f;
+  m[14] = (float)(-2 * f * n / (f - n));
+}
+
+// updateProjectionMatrix (with or without the view offset) and the view matrix inverse(T(position) R) = R^T T(-position)
+__host__ __device__ inline void camera_matrices(ht_camera &c, const CameraCtl &k) {
+  const double PI = 3.141592653589793;
+  if (c.has_view_offset) {
+    const double fw = c.view[0], fh = c.view[1];
+    const double aspect = fw / fh;
+    const double top = tan(c.fov * PI / 360) * k.near_;
+    const double left = -(aspect * top);
+    const double width = 2 * (aspect * top), height = 2 * top;
+    camera_frustum(left + c.view[2] * width / fw, left + (c.view[2] + c.view[4]) * width / fw,
+                   top - (c.view[3] + c.view[5]) * height / fh, top - c.view[3] * height / fh, k.near_, k.far_,
+                   c.projection);
+  } else {                                     // makePerspective(fov, aspect, near, far)
+    const double ymax = k.near_ * tan(c.fov * PI / 360);
+    camera_frustum(-ymax * k.aspect, ymax * k.aspect, -ymax, ymax, k.near_, k.far_, c.projection);
+  }
+  const double *p = c.position;
+  for (int r = 0; r < 3; ++r) {
+    const double *a = k.rot + 3 * r;           // row r of R^T: axis r
+    for (int col = 0; col < 3; ++col) c.view_matrix[4 * col + r] = (float)a[col];
+    c.view_matrix[12 + r] = (float)(-(a[0] * p[0] + a[1] * p[1] + a[2] * p[2]));
+    c.view_matrix[4 * r + 3] = 0.0f;
+  }
+  c.view_matrix[15] = 1.0f;
+}
+
+// the constructed camera (src/controllers.js:40-46): position = fixedPosition, the camera's own fov, no view offset
+__host__ __device__ inline void camera_construct(ht_camera &c, const CameraCtl &k) {
+  for (int i = 0; i < 3; ++i) c.position[i] = k.fixed[i];
+  c.fov = k.fov;
+  for (int i = 0; i < 6; ++i) c.view[i] = 0.0;
+  c.events = 0; c.has_view_offset = 0; c.pad_[0] = c.pad_[1] = 0;
+  camera_matrices(c, k);
+}
+
+// the headtrackingEvent listener (src/controllers.js:48-67) for the event (x, y, z), operation for operation
+__host__ __device__ inline void camera_step(ht_camera &c, const CameraCtl &k, double x, double y, double z) {
+  const double PI = 3.141592653589793;
+  const double scaling = k.scaling, damping = k.damping;
+  const double xOffset = x > 0 ? 0.0 : -x * 2 * damping * scaling;
+  const double yOffset = y < 0 ? 0.0 : y * 2 * damping * scaling;
+  c.view[0] = k.ww + fabs(x * 2 * damping * scaling);
+  c.view[1] = k.wh + fabs(y * damping * 2 * scaling);
+  c.view[2] = xOffset; c.view[3] = yOffset; c.view[4] = k.ww; c.view[5] = k.wh;
+  c.has_view_offset = 1;
+  c.position[0] = k.fixed[0] + (x * scaling * damping);
+  c.position[1] = k.fixed[1] + (y * scaling * damping);
+  c.position[2] = k.fixed[2] + (z * scaling);
+  c.fov = atan((k.wh / 2 + fabs(y * scaling * damping)) / (fabs(z * scaling))) * 360 / PI;
+  ++c.events;
+  camera_matrices(c, k);
+}
+
+// After k_tracker_update: batch entry k (stream ids[k], NULL: k; its record events[geo[k].record], geo NULL: k) moves
+// its stream's camera when its record has a headtrackingEvent.
+__global__ void k_camera_update(const int32_t *__restrict__ ids, const EntryCanvas *__restrict__ geo, int n,
+                                const TrackerEvent *__restrict__ events, const CameraCtl *__restrict__ ctl) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  const CameraCtl &c = ctl[ids ? ids[k] : k];
+  if (!c.camera) return;
+  const HeadEvent &h = events[geo ? geo[k].record : k].head;
+  if (!h.valid) return;
+  ht_camera cam = *c.camera;
+  camera_step(cam, c, h.x, h.y, h.z);
+  *c.camera = cam;
+}
+
+// ht_tracker_set_camera: one CTA constructs the cameras of streams [first, first + n) that have a controller
+__global__ void k_camera_construct(const CameraCtl *__restrict__ ctl, int first, int n) {
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    const CameraCtl &c = ctl[first + i];
+    if (!c.camera) continue;
+    ht_camera cam;
+    camera_construct(cam, c);
+    *c.camera = cam;
+  }
+}
+
 // the parameter check of ht_tracker_config / ht_tracker_set_params, also applied to imported records
 __host__ __device__ inline bool tracker_head_ok(double alpha, double distance_to_screen) {
   return alpha >= 0.0 && alpha <= 1.0 && distance_to_screen > 0.0;

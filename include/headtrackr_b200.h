@@ -340,6 +340,57 @@ typedef struct {
  * HT_ERR_SIZE for a size outside 1..16384. */
 int ht_tracker_set_debug(ht_ctx *ctx, int first, int n, const ht_debug_canvas *canvases);
 
+/* A stream's head-coupled camera: the three.js r48 PerspectiveCamera that realisticAbsoluteCameraControl moves
+ * (src/controllers.js:28-68), in caller-owned DEVICE memory that a renderer can bind directly.  Byte offsets:
+ *     0  double position[3]      camera.position
+ *    24  double fov              camera.fov (degrees)
+ *    32  double view[6]          setViewOffset(fullWidth, fullHeight, x, y, width, height); zeros before the first event
+ *    80  uint32 events           headtrackingEvents applied since the controller was constructed
+ *    84  int32  has_view_offset  0 until the first event, then 1
+ *    88  float  projection[16]   projection matrix, column-major (DESIGN.md 5.4 f10)
+ *   152  float  view_matrix[16]  inverse of the camera's world matrix T(position) R, column-major
+ *   216  uint32 pad_[2]          0 */
+typedef struct {
+  double position[3];
+  double fov;
+  double view[6];
+  uint32_t events;
+  int32_t has_view_offset;
+  float projection[16];
+  float view_matrix[16];
+  uint32_t pad_[2];
+} ht_camera;
+#define HT_CAMERA_BYTES 224
+/* One stream's realisticAbsoluteCameraControl(camera, scaling, fixedPosition, lookAt, {screenHeight, damping}) and
+ * the camera's own fov, aspect, near and far.  Explicit values: the reference's defaults (screenHeight 20, damping 1)
+ * belong to the wrappers. */
+typedef struct {
+  ht_camera *camera;          /* 16-byte aligned DEVICE memory of the context's device; NULL removes the controller */
+  double scaling;
+  double fixed_position[3];
+  double look_at[3];
+  double screen_height, damping;
+  double fov, aspect, near, far;
+} ht_camera_control;          /* 112 bytes */
+/* Stream first+i gets controls[i] (host array), for i in [0, n); stream states are kept.  Setting a controller
+ * constructs it (src/controllers.js:40-46): the camera is enqueued to become position = fixed_position, fov = fov, no
+ * view offset, events = 0, with the matrices of that state; R of the view matrix is fixed here by lookAt(fixed_position
+ * -> look_at, up = +y), as the controller never calls lookAt again.  Setting one again re-constructs it.
+ * Then on every tick whose record has head.valid - the reference dispatched a headtrackingEvent - the listener body
+ * (src/controllers.js:48-67) runs on the device in fp64, in JavaScript's evaluation order, followed by
+ * updateProjectionMatrix.  Ticks without one leave the camera as it is; the controller survives stop, start, reset and
+ * a lost face, and ht_tracker_import (it is a device resource of the stream id, not part of the Tracker's state).  Each
+ * stream hears only its own events.  The writes are enqueued on the context's stream after the tick's records are
+ * computed: with host `out` they have landed when the tick returns, with device `out` after ht_sync or in stream order.
+ * ht_tracker_config removes every controller; ht_tracker_set_params does not.  A tick launches one more kernel while
+ * some stream has a controller, and nothing more otherwise.
+ * Errors (nothing changes): HT_ERR_STATE before ht_tracker_config; HT_ERR_ARG for a range outside [0, max_frames),
+ * n <= 0, controls NULL, a camera that is host memory, memory of another device or not 16-byte aligned, two streams
+ * whose cameras share bytes (over all streams that have one after the call: the streams of a tick run concurrently),
+ * a non-finite field, aspect <= 0, near <= 0, far <= near, fov outside (0, 180), or a degenerate lookAt (fixed_position
+ * == look_at, or a view direction parallel to +y). */
+int ht_tracker_set_camera(ht_ctx *ctx, int first, int n, const ht_camera_control *controls);
+
 /* Tracker records: a stream's whole headtrackr.Tracker as one fixed-size, position-independent, little-endian byte
  * string without pointers, so that a stream can move to another id, context or GPU, be cloned, or outlive its process.
  * Layout (byte offsets; the gaps between sections are zero):
@@ -366,8 +417,9 @@ int ht_tracker_set_debug(ht_ctx *ctx, int first, int n, const ht_debug_canvas *c
  * a device `streams`, an id out of range or listed twice, or device records of another device or misaligned. */
 int ht_tracker_export(ht_ctx *ctx, const int32_t *streams, int n, void *records);
 /* Stream streams[i] := records[i], for i in [0, n): its lifecycle state, parameters and camshift tracker become exactly
- * the exported stream's, and what it held before is discarded.  Its debug canvas (ht_tracker_set_debug) stays as it
- * was: that is a device resource of this stream id, not part of the Tracker's state.  streams and records as for
+ * the exported stream's, and what it held before is discarded.  Its debug canvas (ht_tracker_set_debug) and camera
+ * controller (ht_tracker_set_camera) stay as they were: those are device resources of this stream id, not part of the
+ * Tracker's state.  streams and records as for
  * ht_tracker_export; the source and the destination may be one context (clone: import into an idle id; swap: export
  * [a, b], import [b, a]).  Every record is checked on the device first - magic, format version (records of another
  * version are rejected, not converted), size, checksum, and every field that indexes an array or selects a branch:

@@ -24,6 +24,8 @@
 //   trackerStep(handle, rgba /* n canvases */, n, w, h, nowMs) -> Array<{detection, status: [...], running, fov, ...}>
 //   trackerSetParams(handle, first, [params, ...])   (ht_tracker_set_params: each stream its own Tracker parameters)
 //   trackerSetDebug(handle, first, [canvas|null, ...])  (ht_tracker_set_debug: each stream's debug canvas, device memory)
+//   trackerSetCamera(handle, first, [control|null, ...])  (ht_tracker_set_camera: each stream's head-coupled camera,
+//        realisticAbsoluteCameraControl on an ht_camera in device memory)
 //   trackerExport(handle, [stream, ...]) -> Buffer of records; trackerImport(handle, [stream, ...], records)
 //        (ht_tracker_export / ht_tracker_import: a stream's whole Tracker as HT_TRACKER_RECORD_BYTES per stream)
 //   trackerFeed(handle, [{stream, rgba, width, height, nowMs, canvasWidth?, canvasHeight?}], canvasWidth, canvasHeight)
@@ -444,6 +446,63 @@ static napi_value TrackerSetDebug(napi_env env, napi_callback_info info) {
   return nullptr;
 }
 
+static double GetNumber(napi_env env, napi_value obj, const char *name, double dflt) {
+  napi_value v;
+  napi_valuetype t = napi_undefined;
+  double d = dflt;
+  if (napi_get_named_property(env, obj, name, &v) == napi_ok && napi_typeof(env, v, &t) == napi_ok && t == napi_number)
+    napi_get_value_double(env, v, &d);
+  return d;
+}
+
+static void GetVec3(napi_env env, napi_value obj, const char *name, double out[3]) {
+  napi_value v, e;
+  for (int i = 0; i < 3; ++i) out[i] = 0.0;
+  if (napi_get_named_property(env, obj, name, &v) != napi_ok) return;
+  for (uint32_t i = 0; i < 3; ++i)
+    if (napi_get_element(env, v, i, &e) == napi_ok) napi_get_value_double(env, e, &out[i]);
+}
+
+// trackerSetCamera(handle, first, [{camera: BigInt device address, scaling, fixedPosition: [x, y, z], lookAt: [x, y, z],
+// screenHeight?, damping?, fov, aspect, near, far}, null, ...]): stream first+i gets controls[i]; null or undefined:
+// none.  screenHeight and damping default to the reference's 20 and 1 (src/controllers.js:31-38).
+static napi_value TrackerSetCamera(napi_env env, napi_callback_info info) {
+  size_t argc = 3;
+  napi_value argv[3];
+  NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+  ht_ctx *ctx = Ctx(env, argv[0]);
+  int32_t first = 0;
+  uint32_t n = 0;
+  napi_get_value_int32(env, argv[1], &first);
+  NAPI_OK(napi_get_array_length(env, argv[2], &n));
+  std::vector<ht_camera_control> cs(n);
+  memset(cs.data(), 0, n * sizeof(ht_camera_control));
+  for (uint32_t i = 0; i < n; ++i) {
+    napi_value r, v;
+    napi_valuetype t = napi_undefined;
+    NAPI_OK(napi_get_element(env, argv[2], i, &r));
+    napi_typeof(env, r, &t);
+    if (t != napi_object) continue;
+    uint64_t addr = 0;
+    bool lossless = false;
+    if (napi_get_named_property(env, r, "camera", &v) == napi_ok) napi_get_value_bigint_uint64(env, v, &addr, &lossless);
+    ht_camera_control &c = cs[i];
+    c.camera = reinterpret_cast<ht_camera *>(static_cast<uintptr_t>(addr));
+    c.scaling = GetNumber(env, r, "scaling", 0.0);
+    GetVec3(env, r, "fixedPosition", c.fixed_position);
+    GetVec3(env, r, "lookAt", c.look_at);
+    c.screen_height = GetNumber(env, r, "screenHeight", 20.0);
+    c.damping = GetNumber(env, r, "damping", 1.0);
+    c.fov = GetNumber(env, r, "fov", 0.0);
+    c.aspect = GetNumber(env, r, "aspect", 0.0);
+    c.near = GetNumber(env, r, "near", 0.0);
+    c.far = GetNumber(env, r, "far", 0.0);
+  }
+  int rc = ht_tracker_set_camera(ctx, first, (int)n, cs.data());
+  if (rc < 0) return Throw(env, ctx, rc);
+  return nullptr;
+}
+
 // stream ids of an Array of numbers
 static bool GetStreams(napi_env env, napi_value arr, std::vector<int32_t> *ids) {
   uint32_t n = 0;
@@ -605,6 +664,7 @@ static napi_value Init(napi_env env, napi_value exports) {
       {"trackerStep", nullptr, TrackerStep, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerSetParams", nullptr, TrackerSetParams, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerSetDebug", nullptr, TrackerSetDebug, nullptr, nullptr, nullptr, napi_default, nullptr},
+      {"trackerSetCamera", nullptr, TrackerSetCamera, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerExport", nullptr, TrackerExport, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerImport", nullptr, TrackerImport, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerFeed", nullptr, TrackerFeed, nullptr, nullptr, nullptr, napi_default, nullptr},

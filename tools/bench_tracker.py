@@ -12,6 +12,9 @@ streams: N 640x480 streams, device-resident frames and outputs, CUDA events arou
                   pinned host memory, and a steady tick before and after an import (migrate_arms)
   debug_*         (--debug-streams) ht_tracker_feed with debug canvases on none, 1/64 and all of the streams, the
                   achieved bandwidth of k_debug_backproj, and the no-debug arm against --before-lib (debug_arms)
+  camera_*        (--camera-streams) ht_tracker_feed with head-coupled camera controllers on none, 1/64 and all of
+                  the streams, k_camera_update's kernel time, and the no-controller arm against --before-lib
+                  (camera_arms)
 
 Prints one JSON line with the card's name and power limit read in the same run; --out also writes it to a file."""
 import argparse
@@ -427,6 +430,103 @@ def debug_arms(torch, frames, stream, N, W, H, steps, rounds, before_lib=None):
     return res
 
 
+def camera_arms(torch, frames, stream, N, W, H, steps, rounds, before_lib=None):
+    """Camera controllers (ht_tracker_set_camera) in steady tracking with head positions: N streams of W x H device
+    video fed onto W x H canvases by ht_tracker_feed, every arm on its own context, all arms alternating tick by tick
+    (the arm order rotates), CUDA events around each tick:
+
+      camera0_cs         no stream has a controller (the tick launches what it launched before controllers)
+      camera64_cs        every 64th stream has one
+      cameraall_cs       every stream has one
+      camera0_before_cs  camera0_cs with the library at `before_lib` (e.g. the parent commit's build)
+
+    Then, in a run of its own under torch.profiler, the kernel time of k_camera_update over `steps` ticks of
+    cameraall_cs.  The records of every arm must agree."""
+    import ctypes as C
+    from headtrackr_b200 import Context, _lib
+    rec_bytes = C.sizeof(_lib.TrackerEvent)
+    now = [1.0e12]
+    recs_arr = (_lib.VideoFrame * N)()
+    for k in range(N):
+        recs_arr[k] = _lib.VideoFrame(frames[k].data_ptr(), k, W, H, 0, 0.0)
+    kw = dict(max_width=W, max_height=H, max_frames=N, stream=stream)
+    cams, counts = {}, {}
+    control = dict(scaling=1.0, fixedPosition=[0.0, 0.0, 0.0], lookAt=[0.0, 0.0, -1.0], fov=75.0, aspect=4 / 3,
+                   near=1.0, far=10000.0)
+
+    def arm(every, before=False):
+        c = other_build_context(before_lib, **kw) if before else Context(**kw)
+        c.tracker_config()
+        c.tracker_reset(0, N)
+        c.tracker_start(0, N)
+        if every:
+            buf = torch.zeros(N * _lib.CAMERA_BYTES, dtype=torch.uint8, device="cuda")
+            c.tracker_set_camera(0, [dict(control, out=buf[_lib.CAMERA_BYTES * k: _lib.CAMERA_BYTES * (k + 1)])
+                                     if k % every == 0 else None for k in range(N)])
+            cams[every] = buf
+            counts[every] = len(range(0, N, every))
+        return c, torch.empty(N * rec_bytes, dtype=torch.uint8, device="cuda")
+
+    arms = {"camera0_cs": arm(0), "camera64_cs": arm(64), "cameraall_cs": arm(1)}
+    if before_lib:
+        arms["camera0_before_cs"] = arm(0, before=True)
+    names = list(arms)
+
+    def tick(name):
+        c, out = arms[name]
+        for k in range(N):
+            recs_arr[k].now_ms = now[0]
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        a.record()
+        c._check(c._L.ht_tracker_feed(c._h, C.addressof(recs_arr), N, 1, W, H, out.data_ptr()))
+        b.record()
+        b.synchronize()
+        return a.elapsed_time(b)
+
+    for _ in range(30):                          # the whitebalance gate, detection, CS until the head diagonal is stable
+        now[0] += 20.0
+        for name in names:
+            tick(name)
+    times = {name: [[] for _ in range(rounds)] for name in names}
+    for r in range(rounds):
+        for s in range(steps):
+            now[0] += 20.0
+            rot = (r * steps + s) % len(names)
+            for name in names[rot:] + names[:rot]:
+                times[name][r].append(tick(name))
+            first = arms[names[0]][1].cpu()
+            if any(not torch.equal(first, arms[name][1].cpu()) for name in names[1:]):
+                raise SystemExit("camera arms disagree on the records of a timed tick")
+    res = {}
+    for name in names:
+        med = [float(np.median(t)) for t in times[name]]
+        res[f"{name}_ms"] = float(np.median(sum(times[name], [])))
+        res[f"{name}_spread_ms"] = max(med) - min(med)
+    ev = [_lib.TrackerEvent.from_buffer_copy(bytes(row))
+          for row in arms["cameraall_cs"][1].cpu().numpy().reshape(N, rec_bytes)]
+    res["camera_head_events_per_tick"] = sum(e.head.valid for e in ev)
+    res["camera64_controllers"], res["cameraall_controllers"] = counts[64], counts[1]
+    res["camera_records_agree"] = True
+    res["cameraall_events_min"] = min(int(v) for v in cams[1].view(N, _lib.CAMERA_BYTES)[:, 80:84].cpu().numpy()
+                                      .view(np.uint32).ravel())
+
+    from torch.profiler import ProfilerActivity, profile
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(steps):
+            now[0] += 20.0
+            tick("cameraall_cs")
+        torch.cuda.synchronize()
+    us = 0.0
+    for e in prof.key_averages():
+        if "k_camera_update" in e.key:
+            t = getattr(e, "device_time_total", None)
+            us += t if t is not None else e.cuda_time_total
+    res["k_camera_update_ms"] = us / 1000.0 / steps
+    for c, _ in arms.values():
+        c.close()
+    return res
+
+
 def migrate_arms(torch, frames, stream, N, W, H, steps, rounds):
     """Tracker records (ht_tracker_export / ht_tracker_import) of N streams in steady tracking, W x H video on W/2 x H/2
     canvases, CUDA events on the library's stream around each call, repeated `rounds` x `steps` times:
@@ -527,6 +627,7 @@ def main():
     ap.add_argument("--only-canvases", action="store_true", help="only the canvas arms (canvas_arms)")
     ap.add_argument("--debug-streams", action="store_true", help="only the debug-canvas arms (debug_arms)")
     ap.add_argument("--migrate", action="store_true", help="only the tracker-record arms (migrate_arms)")
+    ap.add_argument("--camera-streams", action="store_true", help="only the camera-controller arms (camera_arms)")
     ap.add_argument("--out")
     a = ap.parse_args()
     import torch
@@ -542,6 +643,9 @@ def main():
     stream = ts.cuda_stream
     if a.migrate:
         res.update(migrate_arms(torch, frames, stream, N, W, H, a.steps, a.rounds))
+        return report(res, a.out)
+    if a.camera_streams:
+        res.update(camera_arms(torch, frames, stream, N, W, H, a.steps, a.rounds, a.before_lib))
         return report(res, a.out)
     if a.debug_streams:
         res.update(debug_arms(torch, frames, stream, N, W, H, a.steps, a.rounds, a.before_lib))
