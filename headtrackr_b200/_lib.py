@@ -75,6 +75,26 @@ class CanvasFrame(C.Structure):
     _fields_ = [("video", VideoFrame), ("canvas_w", C.c_int32), ("canvas_h", C.c_int32), ("pad_", C.c_int32 * 2)]
 
 
+# ht_yuv_image.format / .color
+YUV_FORMATS = {"nv12": 0, "i420": 1}
+YUV_COLORS = {"bt601": 0, "bt709": 1, "bt601-full": 2, "bt709-full": 3}
+
+
+class YuvImage(C.Structure):
+    """ht_yuv_image: a YUV 4:2:0 video frame (NV12: Y, UV, NULL; I420: Y, U, V; pitch 0 = the tight pitch)"""
+    _fields_ = [("planes", C.c_void_p * 3), ("pitch", C.c_int32 * 3), ("width", C.c_int32), ("height", C.c_int32),
+                ("format", C.c_int32), ("color", C.c_int32), ("pad_", C.c_int32)]
+
+
+class YuvFrame(C.Structure):
+    """ht_yuv_frame: one stream's YUV video frame, working canvas and clock for ht_tracker_feed_yuv"""
+    _fields_ = [("video", YuvImage), ("stream", C.c_int32), ("canvas_w", C.c_int32), ("canvas_h", C.c_int32),
+                ("pad_", C.c_int32), ("now_ms", C.c_double)]
+
+
+assert C.sizeof(YuvImage) == 56 and C.sizeof(YuvFrame) == 80 and YuvFrame.now_ms.offset == 72
+
+
 class DebugCanvas(C.Structure):
     """ht_debug_canvas: a stream's debug canvas for ht_tracker_set_debug (device memory; rgba NULL = none; pitch 0 =
     4 * width)"""
@@ -142,7 +162,7 @@ _lib = None
 
 EXPORTS = ["ht_version", "ht_create", "ht_destroy", "ht_last_error", "ht_sync", "ht_max_rects", "ht_detect",
            "ht_track_init", "ht_track_init_from_detect", "ht_track", "ht_detect_track", "ht_stream_reset", "ht_stream_step", "ht_stream_head_config", "ht_stream_step_head",
-           "ht_tracker_config", "ht_tracker_reset", "ht_tracker_start", "ht_tracker_stop", "ht_tracker_step", "ht_tracker_feed", "ht_tracker_set_params", "ht_tracker_feed_canvases", "ht_tracker_set_debug", "ht_tracker_set_camera", "ht_tracker_export", "ht_tracker_import", "ht_ingest", "ht_backprojection", "ht_whitebalance",
+           "ht_tracker_config", "ht_tracker_reset", "ht_tracker_start", "ht_tracker_stop", "ht_tracker_step", "ht_tracker_feed", "ht_tracker_set_params", "ht_tracker_feed_canvases", "ht_tracker_set_debug", "ht_tracker_set_camera", "ht_tracker_export", "ht_tracker_import", "ht_tracker_feed_yuv", "ht_ingest", "ht_ingest_yuv", "ht_backprojection", "ht_whitebalance",
            "ht_plan_info", "ht_debug_plane", "ht_debug_raw", "ht_debug_model_hist", "ht_debug_track_stats", "ht_set_track_memo", "ht_set_pipeline", "ht_join", "ht_debug_set_exactness", "ht_debug_track_trace", "ht_debug_track_phases", "ht_launch_count",
            "ht_profile", "ht_profile_read"]
 
@@ -190,6 +210,8 @@ def lib():
     L.ht_tracker_export.argtypes = [vp, vp, C.c_int, vp]
     L.ht_tracker_import.argtypes = [vp, vp, C.c_int, vp]
     L.ht_ingest.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, vp, C.c_int, C.c_int]
+    L.ht_tracker_feed_yuv.argtypes = [vp, vp, C.c_int, C.c_int, vp]
+    L.ht_ingest_yuv.argtypes = [vp, vp, C.c_int, C.c_int, vp, C.c_int, C.c_int]
     L.ht_backprojection.argtypes = [vp, C.c_int, vp, C.c_int, C.c_int, vp]
     L.ht_whitebalance.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, vp]
     L.ht_plan_info.argtypes = [vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, C.c_int]

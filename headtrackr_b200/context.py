@@ -9,7 +9,7 @@ import numpy as np
 
 from . import _lib
 from ._lib import (Camera, CameraControl, CanvasFrame, DebugCanvas, HeadEvent, HeadParams, HtError, Rect, StreamEvent, TrackerEvent, TrackerParams, TrackObj, VideoFrame,
-                   Window)
+                   Window, YuvFrame, YuvImage)
 from .synth import load_cascade_blob
 
 
@@ -32,6 +32,57 @@ def _frames_ptr(frames):
     if a.ndim != 4 or a.shape[-1] != 4:
         raise ValueError("frames must be (n,H,W,4) uint8")
     return a.ctypes.data, a.shape[0], a.shape[1], a.shape[2], a
+
+
+def _yuv_image(planes, fmt, color, keep):
+    """a YUV 4:2:0 frame - a tuple of 2-D uint8 planes, (Y, UV) for NV12 or (Y, U, V) for I420, all numpy arrays or torch
+    tensors (CPU or CUDA) with unit column stride; row strides become pitches - -> (ht_yuv_image, on_device).  The
+    planes are appended to `keep`."""
+    if fmt not in _lib.YUV_FORMATS:
+        raise ValueError(f"format must be one of {sorted(_lib.YUV_FORMATS)}")
+    if color not in _lib.YUV_COLORS:
+        raise ValueError(f"color must be one of {sorted(_lib.YUV_COLORS)}")
+    nv12 = fmt == "nv12"
+    if len(planes) != (2 if nv12 else 3):
+        raise ValueError("an NV12 frame is (Y, UV), an I420 frame (Y, U, V)")
+    ptrs, pitches, shapes, where = [], [], [], set()
+    for p in planes:
+        if _is_torch(p):
+            if p.dim() != 2 or p.element_size() != 1 or p.stride(1) != 1:
+                raise ValueError("plane tensors must be 2-D uint8 with unit column stride")
+            ptrs.append(p.data_ptr())
+            pitches.append(p.stride(0))
+            where.add(bool(p.is_cuda))
+        else:
+            a = np.asarray(p)
+            if a.dtype != np.uint8 or a.ndim != 2:
+                raise ValueError("planes must be 2-D uint8")
+            if a.strides[1] != 1 or a.strides[0] < a.shape[1]:
+                a = np.ascontiguousarray(a)
+            p = a
+            ptrs.append(a.ctypes.data)
+            pitches.append(a.strides[0])
+            where.add(False)
+        keep.append(p)
+        shapes.append(tuple(p.shape))
+    if len(where) != 1:
+        raise ValueError("the planes of a frame must all be host or all be device memory")
+    h, w = shapes[0]
+    ch, cw = (h + 1) // 2, (w + 1) // 2
+    for i, shape in enumerate(shapes[1:], 1):
+        need = (ch, 2 * cw) if nv12 else (ch, cw)
+        if shape[0] < need[0] or shape[1] < need[1]:
+            raise ValueError(f"plane {i} is {shape}, a {w}x{h} {fmt} frame needs {need}")
+    img = YuvImage((C.c_void_p * 3)(*(ptrs + [None] * (3 - len(ptrs)))), (C.c_int32 * 3)(*(pitches + [0] * (3 - len(pitches)))),
+                   w, h, _lib.YUV_FORMATS[fmt], _lib.YUV_COLORS[color])
+    return img, where.pop()
+
+
+def _per_record(v, n, what):
+    vs = list(v) if isinstance(v, (list, tuple)) else [v] * n
+    if len(vs) != n:
+        raise ValueError(f"one {what} per frame")
+    return vs
 
 
 def camera_from_bytes(b):
@@ -421,6 +472,65 @@ class Context:
         if out is not None:
             return None
         return [tracker_event_dict(e) for e in ev]
+
+    def tracker_feed_yuv(self, streams, frames, now_ms, width, height, format="nv12", color="bt601", out=None):
+        """tracker_feed on YUV 4:2:0 video (ht_tracker_feed_yuv): each frame is a tuple of 2-D uint8 planes, (Y, UV) for
+        NV12 or (Y, U, V) for I420, numpy arrays or torch tensors (CPU, or CUDA for every frame), whose row strides
+        are the pitches.  A decoder's packed NV12 buffer `buf` of h + ceil(h/2) rows splits without a copy:
+            frame = (buf[:h, :w], buf[h:, :2 * ((w + 1) // 2)])
+        The conversion is the library's (DESIGN.md 2): format "nv12" / "i420" and color "bt601" / "bt709" /
+        "bt601-full" / "bt709-full", one for all or one per record.  now_ms, width and height as for tracker_feed
+        (every record has its own canvas here).  -> event dicts in record order; with a torch CUDA `out` tensor of
+        len(streams)*144 bytes: asynchronous, nothing returned."""
+        streams = list(streams)
+        n = len(frames)
+        if len(streams) != n or n == 0:
+            raise ValueError("one frame per listed stream")
+        clocks = [float(t) for t in now_ms] if hasattr(now_ms, "__len__") else [float(now_ms)] * n
+        widths = [int(v) for v in _per_record(width, n, "canvas width")]
+        heights = [int(v) for v in _per_record(height, n, "canvas height")]
+        fmts, colors = _per_record(format, n, "format"), _per_record(color, n, "color")
+        if len(clocks) != n:
+            raise ValueError("one clock per listed stream")
+        recs = (YuvFrame * n)()
+        keep, where = [], set()
+        for b, (k, f) in enumerate(zip(streams, frames)):
+            img, on_device = _yuv_image(f, fmts[b], colors[b], keep)
+            where.add(on_device)
+            recs[b] = YuvFrame(img, int(k), widths[b], heights[b], 0, clocks[b])
+        if len(where) != 1:
+            raise ValueError("frames must be all host or all device memory")
+        ev = None if out is not None else (TrackerEvent * n)()
+        dst = out.data_ptr() if out is not None else C.addressof(ev)
+        self._check(self._L.ht_tracker_feed_yuv(self._h, C.addressof(recs), n, int(where.pop()), dst))
+        if out is not None:
+            return None
+        return [tracker_event_dict(e) for e in ev]
+
+    def ingest_yuv(self, frames, width, height, format="nv12", color="bt601", out=None):
+        """drawImage(video, 0, 0, width, height) of YUV 4:2:0 frames (ht_ingest_yuv): frames, format and color as for
+        tracker_feed_yuv (the frames may differ in size).  -> numpy (n, height, width, 4); with a torch `out` tensor
+        of that shape (CUDA or CPU) the result is written there."""
+        n = len(frames)
+        if n == 0:
+            raise ValueError("no frames")
+        fmts, colors = _per_record(format, n, "format"), _per_record(color, n, "color")
+        imgs = (YuvImage * n)()
+        keep, where = [], set()
+        for b, f in enumerate(frames):
+            imgs[b], on_device = _yuv_image(f, fmts[b], colors[b], keep)
+            where.add(on_device)
+        if len(where) != 1:
+            raise ValueError("frames must be all host or all device memory")
+        on_device = where.pop()
+        if out is not None:
+            if not out.is_contiguous() or tuple(out.shape) != (n, height, width, 4) or out.element_size() != 1:
+                raise ValueError(f"out must be a contiguous uint8 tensor of shape {(n, height, width, 4)}")
+            self._check(self._L.ht_ingest_yuv(self._h, C.addressof(imgs), n, int(on_device), out.data_ptr(), width, height))
+            return out
+        dst = np.zeros((n, height, width, 4), np.uint8)
+        self._check(self._L.ht_ingest_yuv(self._h, C.addressof(imgs), n, int(on_device), dst.ctypes.data, width, height))
+        return dst
 
     def ingest(self, frames, width, height, out=None):
         """drawImage(video, 0, 0, width, height) for a batch (src/main.js:170).  numpy in -> numpy (n, height, width, 4)

@@ -583,6 +583,7 @@ struct ht_ctx {
   // goes up in one copy from pinned memory; the videos are drawn into the canvas arena (batch entry k's canvas at
   // EntryCanvas::base), zeroed when it grows
   DevBuf d_feed_table, d_feed_draw, d_feed_canvas;
+  DevBuf d_ingest_recs;                     // ht_ingest_yuv: the call's YuvFeedRec table
   PinnedHost h_feed_table;
   Event feed_copied;                        // the last table upload has left h_feed_table
   DevBuf d_track_cost;                      // [max_frames][2] {passes, window pixels / 256} per slot
@@ -2054,6 +2055,7 @@ struct FeedDraw {
   IngestGeom g;
   const int32_t *tile_start;
   int tiles;
+  const YuvFeedRec *yuv;   // ht_tracker_feed_yuv: the records are these (recs unused), drawn by k_feed_draw_yuv
 };
 
 // One canvas size of a tracker tick: batch entries [k0, k0 + n) on canvases of w x h (plan P) at frames (n consecutive
@@ -2072,6 +2074,7 @@ struct TickGroup {
 // per-stream kernels once per call.
 //   k_tracker_plan   modes -> VJ frame-quad mask, CS enable, whitebalance enable (feed: draw flags)
 //   k_feed_draw      (feed) drawImage(video, 0, 0, w, h) of every stream that is not IDLE   src/main.js:170,312
+//                    (k_feed_draw_yuv for the YUV records of ht_tracker_feed_yuv)
 //   k_wb_sums        whitebalance sums of the STARTING and WB streams only       src/whitebalance.js, src/main.js:316
 //   run_detect       per group: the VJ streams (interval 5, min_neighbors 1)     src/facetrackr.js:147-149
 //   k_hist, k_track  per group: one track() of the CS streams                    src/camshift.js:213-312
@@ -2094,7 +2097,13 @@ static int tracker_tick(ht_ctx *ctx, const TickGroup *grp, int n_groups, const u
   k_tracker_plan<<<(n + 127) / 128, 128, 0, st>>>(ts, d_ids, n, vj_mask, cs_en, init_en, wb_en, feed ? feed->draw : nullptr, geo);
   if (feed) {
     uint8_t *canvas = const_cast<uint8_t *>(d_rgba);
-    if (!feed->tile_start) {
+    if (feed->yuv && !feed->tile_start) {
+      const int tiles_x = (g0.w + 63) / 64, tiles = tiles_x * ((g0.h + 15) / 16);
+      k_feed_draw_yuv<<<dim3((unsigned)tiles, (unsigned)n), 256, 0, st>>>(feed->yuv, feed->draw, canvas, feed->g, tiles_x,
+                                                                          nullptr, nullptr, n);
+    } else if (feed->yuv) {
+      k_feed_draw_yuv<<<(unsigned)feed->tiles, 256, 0, st>>>(feed->yuv, feed->draw, canvas, feed->g, 0, geo, feed->tile_start, n);
+    } else if (!feed->tile_start) {
       const int tiles_x = (g0.w + 63) / 64, tiles = tiles_x * ((g0.h + 15) / 16);
       k_feed_draw<<<dim3((unsigned)tiles, (unsigned)n), 256, 0, st>>>(feed->recs, feed->draw, canvas, feed->g, tiles_x,
                                                                       nullptr, nullptr, n);
@@ -2192,6 +2201,66 @@ static bool canvas_geom(int w, int h, IngestGeom &g) {
   return true;
 }
 
+// An ht_yuv_image checked and resolved into r: pitches resolved, NV12's V at U + 1.  -> HT_OK, or the error code with
+// the reason in why[256].
+static int yuv_record(const ht_yuv_image &v, YuvFeedRec &r, char *why) {
+  if (v.format != HT_YUV_NV12 && v.format != HT_YUV_I420)
+    return snprintf(why, 256, "format %d is neither HT_YUV_NV12 nor HT_YUV_I420", v.format), HT_ERR_ARG;
+  if (v.color < 0 || v.color > (HT_YUV_BT709 | HT_YUV_FULL_RANGE))
+    return snprintf(why, 256, "color %d is not HT_YUV_BT601 or HT_YUV_BT709 [| HT_YUV_FULL_RANGE]", v.color), HT_ERR_ARG;
+  if (v.width <= 0 || v.height <= 0 || v.width > 16384 || v.height > 16384)
+    return snprintf(why, 256, "video %dx%d outside 1..16384", v.width, v.height), HT_ERR_SIZE;
+  const bool nv12 = v.format == HT_YUV_NV12;
+  const int planes = nv12 ? 2 : 3, cw = (v.width + 1) / 2;
+  const int tight[3] = {v.width, nv12 ? 2 * cw : cw, cw};
+  int pitch[3] = {0, 0, 0};
+  for (int p = 0; p < planes; ++p) {
+    if (!v.planes[p]) return snprintf(why, 256, "planes[%d] is NULL", p), HT_ERR_ARG;
+    pitch[p] = v.pitch[p] ? v.pitch[p] : tight[p];
+    if (pitch[p] < tight[p]) return snprintf(why, 256, "pitch[%d] = %d is below %d", p, v.pitch[p], tight[p]), HT_ERR_ARG;
+  }
+  if (nv12 && v.planes[2]) return snprintf(why, 256, "planes[2] must be NULL for NV12"), HT_ERR_ARG;
+  r = YuvFeedRec{v.planes[0], v.planes[1], nv12 ? v.planes[1] + 1 : v.planes[2], pitch[0], pitch[1], nv12 ? pitch[1] : pitch[2],
+                 v.width, v.height, nv12 ? 2 : 1, v.color, 0};
+  return HT_OK;
+}
+static int check_yuv_record(ht_ctx *ctx, const ht_yuv_image &v, int b, YuvFeedRec &r) {
+  char why[256];
+  const int rc = yuv_record(v, r, why);
+  return rc == HT_OK ? HT_OK : ctx->fail(rc, "record %d: %s", b, why);
+}
+
+// bytes of r's planes packed at tight pitches, each plane 256-byte aligned
+static size_t yuv_staged_bytes(const YuvFeedRec &r) {
+  const size_t cw = (size_t)(r.width + 1) / 2, ch = (size_t)(r.height + 1) / 2;
+  const size_t luma = align_up<size_t>((size_t)r.width * r.height, 256);
+  return r.cstep == 2 ? luma + align_up<size_t>(2 * cw * ch, 256) : luma + 2 * align_up<size_t>(cw * ch, 256);
+}
+
+// r's host planes go up plane by plane to dst (yuv_staged_bytes of device memory), on the context's stream; r then
+// describes the packed copy
+static int stage_yuv(ht_ctx *ctx, YuvFeedRec &r, uint8_t *dst) {
+  const size_t w = (size_t)r.width, h = (size_t)r.height, cw = (w + 1) / 2, ch = (h + 1) / 2;
+  const size_t luma = align_up<size_t>(w * h, 256);
+  CK(cudaMemcpy2DAsync(dst, w, r.y, (size_t)r.ypitch, w, h, cudaMemcpyHostToDevice, ctx->stream));
+  r.y = dst;
+  r.ypitch = (int32_t)w;
+  if (r.cstep == 2) {
+    CK(cudaMemcpy2DAsync(dst + luma, 2 * cw, r.u, (size_t)r.upitch, 2 * cw, ch, cudaMemcpyHostToDevice, ctx->stream));
+    r.u = dst + luma;
+    r.v = r.u + 1;
+    r.upitch = r.vpitch = (int32_t)(2 * cw);
+  } else {
+    const size_t cb = align_up<size_t>(cw * ch, 256);
+    CK(cudaMemcpy2DAsync(dst + luma, cw, r.u, (size_t)r.upitch, cw, ch, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpy2DAsync(dst + luma + cb, cw, r.v, (size_t)r.vpitch, cw, ch, cudaMemcpyHostToDevice, ctx->stream));
+    r.u = dst + luma;
+    r.v = dst + luma + cb;
+    r.upitch = r.vpitch = (int32_t)cw;
+  }
+  return HT_OK;
+}
+
 // ht_tracker_feed(_canvases).  Everything is checked before anything is enqueued (one_canvas: every record is on the
 // same canvas and the canvas errors are ht_tracker_feed's, without a record index).  The records are grouped by canvas
 // size - groups in order of first appearance, records in order within a group - and batch entry k is the k-th record
@@ -2201,18 +2270,32 @@ static bool canvas_geom(int w, int h, IngestGeom &g) {
 // starts} from pinned memory, and tracker_tick draws the videos of the streams that are not IDLE into the arena before
 // the kernels of ht_tracker_step run on it through the stream ids.  With one canvas size the launches are those of one
 // uniform batch.
-static int tracker_feed(ht_ctx *ctx, const ht_canvas_frame *frames, int n, int frames_on_device, bool one_canvas,
-                        ht_tracker_event *out) {
+//
+// YUV records (ht_tracker_feed_yuv: frames NULL, yuv the records) take the same path; each is resolved into a
+// YuvFeedRec, host planes are packed plane by plane, and tracker_tick draws them with k_feed_draw_yuv.
+static int tracker_feed(ht_ctx *ctx, const ht_canvas_frame *frames, const ht_yuv_frame *yuv, int n, int frames_on_device,
+                        bool one_canvas, ht_tracker_event *out) {
   if (!ctx) return HT_ERR_ARG;
   if (!ctx->tracker_on) return ctx->fail(HT_ERR_STATE, "ht_tracker_config has not been called");
-  if (!frames || !out) return ctx->fail(HT_ERR_ARG, "frames or out is NULL");
+  if ((!frames && !yuv) || !out) return ctx->fail(HT_ERR_ARG, "frames or out is NULL");
   const int mf = ctx->cfg.max_frames;
   if (n <= 0 || n > mf) return ctx->fail(HT_ERR_ARG, "n=%d outside [1,%d]", n, mf);
+  auto stream_of = [&](int b) { return yuv ? yuv[b].stream : frames[b].video.stream; };
+  auto canvas_of = [&](int b) {
+    return yuv ? std::make_pair(yuv[b].canvas_w, yuv[b].canvas_h) : std::make_pair(frames[b].canvas_w, frames[b].canvas_h);
+  };
   std::vector<uint8_t> seen((size_t)mf, 0);
+  std::vector<YuvFeedRec> yrec(yuv ? (size_t)n : 0);
   for (int b = 0; b < n; ++b) {
+    const int s = stream_of(b);
+    if (s < 0 || s >= mf) return ctx->fail(HT_ERR_ARG, "record %d: stream %d outside [0,%d)", b, s, mf);
+    if (seen[(size_t)s]++) return ctx->fail(HT_ERR_ARG, "record %d: stream %d is listed twice", b, s);
+    if (yuv) {
+      const int rc = check_yuv_record(ctx, yuv[b].video, b, yrec[(size_t)b]);
+      if (rc != HT_OK) return rc;
+      continue;
+    }
     const ht_video_frame &f = frames[b].video;
-    if (f.stream < 0 || f.stream >= mf) return ctx->fail(HT_ERR_ARG, "record %d: stream %d outside [0,%d)", b, f.stream, mf);
-    if (seen[(size_t)f.stream]++) return ctx->fail(HT_ERR_ARG, "record %d: stream %d is listed twice", b, f.stream);
     if (!f.rgba) return ctx->fail(HT_ERR_ARG, "record %d: rgba is NULL", b);
     if (reinterpret_cast<uintptr_t>(f.rgba) & 3u) return ctx->fail(HT_ERR_ARG, "record %d: rgba must be 4-byte aligned", b);
     if (f.width <= 0 || f.height <= 0 || f.width > 16384 || f.height > 16384)
@@ -2226,7 +2309,7 @@ static int tracker_feed(ht_ctx *ctx, const ht_canvas_frame *frames, int n, int f
   std::map<std::pair<int, int>, int> index;
   int last = -1;                          // the previous record's group: runs of one size skip the lookup
   for (int b = 0; b < n; ++b) {
-    const int cw = frames[b].canvas_w, chh = frames[b].canvas_h;
+    const int cw = canvas_of(b).first, chh = canvas_of(b).second;
     if (last >= 0 && groups[(size_t)last].w == cw && groups[(size_t)last].h == chh) {
       group_of[(size_t)b] = last;
       ++groups[(size_t)last].n;
@@ -2246,7 +2329,7 @@ static int tracker_feed(ht_ctx *ctx, const ht_canvas_frame *frames, int n, int f
     group_of[(size_t)b] = last;
     ++groups[(size_t)last].n;
   }
-  if (is_device_ptr(frames[0].video.rgba) != (frames_on_device != 0))
+  if (is_device_ptr(yuv ? yuv[0].video.planes[0] : frames[0].video.rgba) != (frames_on_device != 0))
     return ctx->fail(HT_ERR_ARG, "the frames are %s memory, frames_on_device says otherwise", frames_on_device ? "host" : "device");
   { const int jr = join_aux(ctx); if (jr != HT_OK) return jr; }
   CK(cudaSetDevice(ctx->cfg.device));
@@ -2281,16 +2364,18 @@ static int tracker_feed(ht_ctx *ctx, const ht_canvas_frame *frames, int n, int f
     CK(cudaMemsetAsync(ctx->d_feed_canvas.p, 0, ctx->d_feed_canvas.cap, ctx->stream));
   }
   uint8_t *arena = ctx->d_feed_canvas.as<uint8_t>();
-  // record table: ids [n] i32 | clocks [n] f64 | FeedRec [n] | (several sizes) EntryCanvas [n] | tile starts [n + 1] i32
-  auto table_offsets = [](size_t m, size_t off[4]) {
+  // record table: ids [n] i32 | clocks [n] f64 | FeedRec or YuvFeedRec [n] | (several sizes) EntryCanvas [n] | tile
+  // starts [n + 1] i32
+  auto table_offsets = [](size_t m, size_t rec_bytes, size_t off[4]) {
     off[0] = align_up<size_t>(4 * m, 16);                 // clocks
-    off[1] = off[0] + 8 * m;                              // FeedRec
-    off[2] = off[1] + sizeof(FeedRec) * m;                // EntryCanvas
+    off[1] = off[0] + 8 * m;                              // FeedRec / YuvFeedRec
+    off[2] = off[1] + rec_bytes * m;                      // EntryCanvas
     off[3] = off[2] + sizeof(EntryCanvas) * m;            // tile starts
     return off[3] + 4 * (m + 1);
   };
+  static_assert(sizeof(YuvFeedRec) % 8 == 0 && sizeof(YuvFeedRec) >= sizeof(FeedRec), "YuvFeedRec layout");
   size_t off[4];
-  const size_t table_cap = table_offsets((size_t)mf, off);
+  const size_t table_cap = table_offsets((size_t)mf, sizeof(YuvFeedRec), off);
   if (!ctx->h_feed_table) {
     CK(cudaMallocHost(&ctx->h_feed_table.h, table_cap));
     CK(cudaEventCreateWithFlags(&ctx->feed_copied.h, cudaEventDisableTiming));
@@ -2300,16 +2385,19 @@ static int tracker_feed(ht_ctx *ctx, const ht_canvas_frame *frames, int n, int f
     CK(cudaEventSynchronize(ctx->feed_copied));           // the previous call's upload may still read the table
   }
   const bool mixed = n_groups > 1;
-  const size_t table_full = table_offsets((size_t)n, off);
+  const size_t table_full = table_offsets((size_t)n, yuv ? sizeof(YuvFeedRec) : sizeof(FeedRec), off);
   const size_t table_bytes = mixed ? table_full : off[2];
   uint8_t *tab = static_cast<uint8_t *>(ctx->h_feed_table.h);
   int32_t *ids = reinterpret_cast<int32_t *>(tab);
   double *now = reinterpret_cast<double *>(tab + off[0]);
   FeedRec *recs = reinterpret_cast<FeedRec *>(tab + off[1]);
+  YuvFeedRec *yrecs = reinterpret_cast<YuvFeedRec *>(tab + off[1]);
   EntryCanvas *geo = reinterpret_cast<EntryCanvas *>(tab + off[2]);
   int32_t *tile_start = reinterpret_cast<int32_t *>(tab + off[3]);
   size_t video_bytes = 0;
-  for (int b = 0; b < n; ++b) video_bytes += align_up<size_t>((size_t)frames[b].video.width * frames[b].video.height * 4, 256);
+  for (int b = 0; b < n; ++b)
+    video_bytes += yuv ? yuv_staged_bytes(yrec[(size_t)b])
+                       : align_up<size_t>((size_t)frames[b].video.width * frames[b].video.height * 4, 256);
   if (!frames_on_device) CK(ctx->d_frames.reserve(video_bytes));
   size_t voff = 0;
   std::vector<int> fill((size_t)n_groups, 0);
@@ -2324,19 +2412,31 @@ static int tracker_feed(ht_ctx *ctx, const ht_canvas_frame *frames, int n, int f
   for (int e = 0; e < n; ++e) {
     const int b = record_of[(size_t)e];
     const Group &G = groups[(size_t)group_of[(size_t)b]];
-    const ht_video_frame &f = frames[b].video;
-    ids[e] = f.stream;
-    now[e] = f.now_ms;
-    FeedRec r{f.rgba, f.stream, f.width, f.height, f.pitch ? f.pitch : 4 * f.width, f.now_ms};
-    if (!frames_on_device) {                               // pack the host videos into the device staging buffer
-      uint8_t *dst = ctx->d_frames.as<uint8_t>() + voff;
-      CK(cudaMemcpy2DAsync(dst, 4 * (size_t)f.width, f.rgba, (size_t)r.pitch, 4 * (size_t)f.width, (size_t)f.height,
-                           cudaMemcpyHostToDevice, ctx->stream));
-      r.src = dst;
-      r.pitch = 4 * f.width;
-      voff += align_up<size_t>((size_t)f.width * f.height * 4, 256);
+    if (yuv) {
+      ids[e] = yuv[b].stream;
+      now[e] = yuv[b].now_ms;
+      YuvFeedRec r = yrec[(size_t)b];
+      if (!frames_on_device) {
+        const int rc = stage_yuv(ctx, r, ctx->d_frames.as<uint8_t>() + voff);
+        if (rc != HT_OK) return rc;
+        voff += yuv_staged_bytes(r);
+      }
+      yrecs[e] = r;
+    } else {
+      const ht_video_frame &f = frames[b].video;
+      ids[e] = f.stream;
+      now[e] = f.now_ms;
+      FeedRec r{f.rgba, f.stream, f.width, f.height, f.pitch ? f.pitch : 4 * f.width, f.now_ms};
+      if (!frames_on_device) {                             // pack the host videos into the device staging buffer
+        uint8_t *dst = ctx->d_frames.as<uint8_t>() + voff;
+        CK(cudaMemcpy2DAsync(dst, 4 * (size_t)f.width, f.rgba, (size_t)r.pitch, 4 * (size_t)f.width, (size_t)f.height,
+                             cudaMemcpyHostToDevice, ctx->stream));
+        r.src = dst;
+        r.pitch = 4 * f.width;
+        voff += align_up<size_t>((size_t)f.width * f.height * 4, 256);
+      }
+      recs[e] = r;
     }
-    recs[e] = r;
     if (mixed) {
       const int j = e - G.tick.k0;
       geo[e] = EntryCanvas{G.base + (size_t)j * G.w * G.h * 4, G.w, G.h, G.g.magic, G.g.shift, G.g.half,
@@ -2354,8 +2454,9 @@ static int tracker_feed(ht_ctx *ctx, const ht_canvas_frame *frames, int n, int f
     ticks[(size_t)i] = groups[(size_t)i].tick;
     ticks[(size_t)i].frames = arena + groups[(size_t)i].base;
   }
-  const FeedDraw feed{reinterpret_cast<const FeedRec *>(dtab + off[1]), ctx->d_feed_draw.as<uint8_t>(), groups[0].g,
-                      mixed ? reinterpret_cast<const int32_t *>(dtab + off[3]) : nullptr, t0};
+  const FeedDraw feed{yuv ? nullptr : reinterpret_cast<const FeedRec *>(dtab + off[1]), ctx->d_feed_draw.as<uint8_t>(),
+                      groups[0].g, mixed ? reinterpret_cast<const int32_t *>(dtab + off[3]) : nullptr, t0,
+                      yuv ? reinterpret_cast<const YuvFeedRec *>(dtab + off[1]) : nullptr};
   return tracker_tick(ctx, ticks.data(), n_groups, arena, n, reinterpret_cast<const int32_t *>(dtab), 0.0,
                       reinterpret_cast<const double *>(dtab + off[0]), &feed,
                       mixed ? reinterpret_cast<const EntryCanvas *>(dtab + off[2]) : nullptr, out);
@@ -2369,11 +2470,15 @@ int ht_tracker_feed(ht_ctx *ctx, const ht_video_frame *frames, int n, int frames
   if (n <= 0 || n > ctx->cfg.max_frames) return ctx->fail(HT_ERR_ARG, "n=%d outside [1,%d]", n, ctx->cfg.max_frames);
   std::vector<ht_canvas_frame> recs((size_t)n);
   for (int b = 0; b < n; ++b) recs[(size_t)b] = ht_canvas_frame{frames[b], canvas_w, canvas_h, {0, 0}};
-  return tracker_feed(ctx, recs.data(), n, frames_on_device, true, out);
+  return tracker_feed(ctx, recs.data(), nullptr, n, frames_on_device, true, out);
 }
 
 int ht_tracker_feed_canvases(ht_ctx *ctx, const ht_canvas_frame *frames, int n, int frames_on_device, ht_tracker_event *out) {
-  return tracker_feed(ctx, frames, n, frames_on_device, false, out);
+  return tracker_feed(ctx, frames, nullptr, n, frames_on_device, false, out);
+}
+
+int ht_tracker_feed_yuv(ht_ctx *ctx, const ht_yuv_frame *frames, int n, int frames_on_device, ht_tracker_event *out) {
+  return tracker_feed(ctx, nullptr, frames, n, frames_on_device, false, out);
 }
 
 // canvasContext.drawImage(video, 0, 0, canvas.width, canvas.height) for n frames (src/main.js:170)
@@ -2403,6 +2508,51 @@ int ht_ingest(ht_ctx *ctx, const uint8_t *src_rgba, int n, int sw, int sh, uint8
     ++ctx->launches;
     CK(cudaGetLastError());
   }
+  return io.finish(Outputs::SYNC_STREAM);
+}
+
+// ht_ingest for YUV video: k_feed_draw_yuv over n records, every one drawn, canvas i at dst + i * dw * dh * 4
+int ht_ingest_yuv(ht_ctx *ctx, const ht_yuv_image *src, int n, int frames_on_device, uint8_t *dst_rgba, int dw, int dh) {
+  if (!ctx) return HT_ERR_ARG;
+  if (!src || !dst_rgba) return ctx->fail(HT_ERR_ARG, "src or dst_rgba is NULL");
+  if (n <= 0 || n > 65535) return ctx->fail(HT_ERR_ARG, "n=%d outside [1,65535]", n);   // (grid y)
+  if (reinterpret_cast<uintptr_t>(dst_rgba) & 3u) return ctx->fail(HT_ERR_ARG, "dst_rgba must be 4-byte aligned");
+  if (dw <= 0 || dh <= 0 || dw > 16384 || dh > 16384) return ctx->fail(HT_ERR_SIZE, "canvas %dx%d outside 1..16384", dw, dh);
+  IngestGeom g;
+  if (!canvas_geom(dw, dh, g)) return ctx->fail(HT_ERR_SIZE, "canvas too large for 32-bit bilinear numerators");
+  std::vector<YuvFeedRec> recs((size_t)n);
+  size_t video_bytes = 0;
+  for (int b = 0; b < n; ++b) {
+    const int rc = check_yuv_record(ctx, src[b], b, recs[(size_t)b]);
+    if (rc != HT_OK) return rc;
+    video_bytes += yuv_staged_bytes(recs[(size_t)b]);
+  }
+  if (is_device_ptr(src[0].planes[0]) != (frames_on_device != 0))
+    return ctx->fail(HT_ERR_ARG, "the frames are %s memory, frames_on_device says otherwise", frames_on_device ? "host" : "device");
+  { const int jr = join_aux(ctx); if (jr != HT_OK) return jr; }
+  CK(cudaSetDevice(ctx->cfg.device));
+  cudaStream_t st = ctx->stream;
+  if (!frames_on_device) {
+    CK(ctx->d_frames.reserve(video_bytes));
+    size_t voff = 0;
+    for (YuvFeedRec &r : recs) {
+      const int rc = stage_yuv(ctx, r, ctx->d_frames.as<uint8_t>() + voff);
+      if (rc != HT_OK) return rc;
+      voff += yuv_staged_bytes(r);
+    }
+  }
+  CK(ctx->d_ingest_recs.reserve(sizeof(YuvFeedRec) * (size_t)n));
+  // pageable source: the copy is staged before it returns, so `recs` may go out of scope
+  CK(cudaMemcpyAsync(ctx->d_ingest_recs.p, recs.data(), sizeof(YuvFeedRec) * (size_t)n, cudaMemcpyHostToDevice, st));
+  const size_t dbytes = (size_t)n * dw * dh * 4;
+  Outputs io(ctx);
+  const int o_dst = io.add(dst_rgba, ctx->d_scratch, dbytes);
+  if (!io.on_device()) CK(ctx->d_scratch.reserve(dbytes));
+  const int tiles_x = (dw + 63) / 64, tiles = tiles_x * ((dh + 15) / 16);
+  k_feed_draw_yuv<<<dim3((unsigned)tiles, (unsigned)n), 256, 0, st>>>(ctx->d_ingest_recs.as<YuvFeedRec>(), nullptr,
+                                                                      io.dst<uint8_t>(o_dst), g, tiles_x, nullptr, nullptr, n);
+  ++ctx->launches;
+  CK(cudaGetLastError());
   return io.finish(Outputs::SYNC_STREAM);
 }
 
@@ -2772,6 +2922,27 @@ extern "C" int ht_selftest_debug_write(const uint16_t *bins, int w, int h, const
     }
   }
   return stores;
+}
+
+// k_feed_draw_yuv's per-record code: one YUV image (host planes) onto a dw x dh canvas, 1:1 draws whose width is a
+// multiple of 4 through yuv_quad as the kernel takes them (the canvas is taken to be 16-byte aligned), every other draw
+// pixel by pixel.  -> 0, or the ht_ingest_yuv error code for a bad record.
+extern "C" int ht_selftest_feed_yuv(const ht_yuv_image *img, uint8_t *canvas, int dw, int dh) {
+  YuvFeedRec r;
+  char why[256];
+  const int rc = yuv_record(*img, r, why);
+  if (rc != HT_OK) return rc;
+  IngestGeom g;
+  if (!canvas_geom(dw, dh, g)) return HT_ERR_SIZE;
+  const bool quads = r.width == dw && r.height == dh && (dw & 3) == 0;
+  for (int Y = 0; Y < dh; ++Y) {
+    if (quads) {
+      for (int X = 0; X < dw; X += 4) reinterpret_cast<uint4 *>(canvas + (size_t)Y * dw * 4)[X >> 2] = yuv_quad(r, X, Y);
+    } else {
+      for (int X = 0; X < dw; ++X) feed_yuv_pixel(r, canvas, g, X, Y);
+    }
+  }
+  return 0;
 }
 
 // k_ingest's per-pixel code over a whole frame batch

@@ -184,9 +184,10 @@ struct IngestGeom {
   int sw, sh, dw, dh;
   uint32_t magic, shift, half;   // floor(n / (4 dw dh)) == (uint64(n) * magic) >> shift for n <= 255.5 * 4 dw dh
 };
-// canvas pixel (X, Y) of the sw x sh source s (rows of `spitch` pixels) drawn onto the canvas of g (g.sw / g.sh unused)
-__host__ __device__ __forceinline__ uint32_t draw_pixel(const uint32_t *__restrict__ s, int sw, int sh, size_t spitch,
-                                                        const IngestGeom &g, int X, int Y) {
+// canvas pixel (X, Y) of a sw x sh source drawn onto the canvas of g (g.sw / g.sh unused); texel(x, y) is the source's
+// RGBA8 pixel (x, y) as a little-endian word
+template <class Texel>
+__host__ __device__ __forceinline__ uint32_t bilinear_pixel(const Texel &texel, int sw, int sh, const IngestGeom &g, int X, int Y) {
   // u = (X + 1/2) sw / dw - 1/2 = ((2X + 1) sw - dw) / (2 dw): floor and numerator of the fraction, exactly
   const int un = (2 * X + 1) * sw - g.dw, vn = (2 * Y + 1) * sh - g.dh;
   const int Dx = 2 * g.dw, Dy = 2 * g.dh;
@@ -196,8 +197,8 @@ __host__ __device__ __forceinline__ uint32_t draw_pixel(const uint32_t *__restri
   const uint32_t fx = (uint32_t)(un - x0 * Dx), fy = (uint32_t)(vn - y0 * Dy);
   const int xa = x0 < 0 ? 0 : (x0 > sw - 1 ? sw - 1 : x0), xb = x0 + 1 < 0 ? 0 : (x0 + 1 > sw - 1 ? sw - 1 : x0 + 1);
   const int ya = y0 < 0 ? 0 : (y0 > sh - 1 ? sh - 1 : y0), yb = y0 + 1 < 0 ? 0 : (y0 + 1 > sh - 1 ? sh - 1 : y0 + 1);
-  const uint32_t p00 = ld_ro(s + (size_t)ya * spitch + xa), p01 = ld_ro(s + (size_t)ya * spitch + xb);
-  const uint32_t p10 = ld_ro(s + (size_t)yb * spitch + xa), p11 = ld_ro(s + (size_t)yb * spitch + xb);
+  const uint32_t p00 = texel(xa, ya), p01 = texel(xb, ya);
+  const uint32_t p10 = texel(xa, yb), p11 = texel(xb, yb);
   const uint32_t w00 = ((uint32_t)Dx - fx) * ((uint32_t)Dy - fy), w01 = fx * ((uint32_t)Dy - fy);
   const uint32_t w10 = ((uint32_t)Dx - fx) * fy, w11 = fx * fy;
   uint32_t out = 0;
@@ -208,6 +209,68 @@ __host__ __device__ __forceinline__ uint32_t draw_pixel(const uint32_t *__restri
     out |= (uint32_t)(((uint64_t)num * g.magic) >> g.shift) << (8 * c);
   }
   return out;
+}
+// canvas pixel (X, Y) of the sw x sh RGBA8 source s (rows of `spitch` pixels) drawn onto the canvas of g
+__host__ __device__ __forceinline__ uint32_t draw_pixel(const uint32_t *__restrict__ s, int sw, int sh, size_t spitch,
+                                                        const IngestGeom &g, int X, int Y) {
+  return bilinear_pixel([=](int x, int y) { return ld_ro(s + (size_t)y * spitch + x); }, sw, sh, g, X, Y);
+}
+
+// YUV 4:2:0 video (DESIGN.md 2, "YUV video"): luma pixel (x, y) takes chroma sample (x >> 1, y >> 1), and the triple
+// becomes RGBA8 in integers only - C = Y - y0, D = U - 128, E = V - 128, R = clamp((cy C + rv E + 128) >> 8),
+// G = clamp((cy C - gu D - gv E + 128) >> 8), B = clamp((cy C + bu D + 128) >> 8), A = 255 - with each coefficient
+// round(256 x the real one).  Every row is within 1 level of the real-valued conversion rounded half up, over all
+// 2^24 triples (tests/test_yuv_host.py).  color: HT_YUV_BT601 / HT_YUV_BT709, optionally | HT_YUV_FULL_RANGE.
+//                          y0   cy   rv   gu   gv   bu
+//   BT.601 limited range   16  298  409  100  208  516
+//   BT.709 limited range   16  298  459   55  136  541
+//   BT.601 full range       0  256  359   88  183  454
+//   BT.709 full range       0  256  403   48  120  475
+// |cy C| + |rv E| etc. stay below 2^18: int32 throughout.
+__host__ __device__ __forceinline__ uint32_t yuv_to_rgba(int color, uint32_t Y, uint32_t U, uint32_t V) {
+  const bool bt709 = (color & HT_YUV_BT709) != 0, full = (color & HT_YUV_FULL_RANGE) != 0;
+  const int y0 = full ? 0 : 16, cy = full ? 256 : 298;
+  const int rv = full ? (bt709 ? 403 : 359) : (bt709 ? 459 : 409);
+  const int gu = full ? (bt709 ? 48 : 88) : (bt709 ? 55 : 100);
+  const int gv = full ? (bt709 ? 120 : 183) : (bt709 ? 136 : 208);
+  const int bu = full ? (bt709 ? 475 : 454) : (bt709 ? 541 : 516);
+  const int c = cy * ((int)Y - y0), d = (int)U - 128, e = (int)V - 128;
+  const int r = (c + rv * e + 128) >> 8, gr = (c - gu * d - gv * e + 128) >> 8, b = (c + bu * d + 128) >> 8;
+  auto clamp255 = [](int v) { return (uint32_t)(v < 0 ? 0 : (v > 255 ? 255 : v)); };
+  return clamp255(r) | clamp255(gr) << 8 | clamp255(b) << 16 | 0xff000000u;
+}
+// ht_tracker_feed_yuv / ht_ingest_yuv: one YUV 4:2:0 video frame, pitches resolved.  Chroma sample (cx, cy) is
+// u[cy * upitch + cx * cstep] and v[cy * vpitch + cx * cstep]: NV12 is v = u + 1 with cstep 2 (one interleaved plane),
+// I420 two planes with cstep 1, so both layouts are one code path.
+struct YuvFeedRec {
+  const uint8_t *y, *u, *v;
+  int32_t ypitch, upitch, vpitch;   // bytes
+  int32_t width, height;
+  int32_t cstep;                    // bytes between horizontally adjacent chroma samples
+  int32_t color;                    // ht_yuv_image.color
+  int32_t pad_;
+};
+// RGBA8 pixel (x, y) of the converted video; an NV12 (U, V) pair at an even address is one 2-byte load
+__host__ __device__ __forceinline__ uint32_t yuv_texel(const YuvFeedRec &r, int x, int y) {
+  const size_t c = (size_t)(x >> 1) * r.cstep;
+  const uint8_t *up = r.u + (size_t)(y >> 1) * r.upitch + c;
+  uint32_t U, V;
+  if (r.cstep == 2 && (reinterpret_cast<uintptr_t>(up) & 1u) == 0) {
+    const uint32_t uv = ld_ro(reinterpret_cast<const uint16_t *>(up));
+    U = uv & 0xffu, V = uv >> 8;
+  } else {
+    U = ld_ro(up), V = ld_ro(r.v + (size_t)(y >> 1) * r.vpitch + c);
+  }
+  return yuv_to_rgba(r.color, ld_ro(r.y + (size_t)y * r.ypitch + x), U, V);
+}
+// canvas pixel (X, Y) of YUV record r onto a canvas of g: drawing the converted video, four converted taps per pixel
+// (a 1:1 draw is the conversion alone); also run on the host by ht_selftest_feed_yuv
+__host__ __device__ __forceinline__ void feed_yuv_pixel(const YuvFeedRec &r, uint8_t *__restrict__ canvas, const IngestGeom &g,
+                                                        int X, int Y) {
+  const uint32_t out = (r.width == g.dw && r.height == g.dh)
+                           ? yuv_texel(r, X, Y)
+                           : bilinear_pixel([&](int x, int y) { return yuv_texel(r, x, y); }, r.width, r.height, g, X, Y);
+  reinterpret_cast<uint32_t *>(canvas)[(size_t)Y * g.dw + X] = out;
 }
 // one destination pixel (also run on the host by tests/test_ingest_host.py)
 __host__ __device__ __forceinline__ void ingest_pixel(const uint8_t *__restrict__ src, uint8_t *__restrict__ dst, const IngestGeom &g,
@@ -270,16 +333,9 @@ __host__ __device__ __forceinline__ void feed_canvas_pixel(const FeedRec &r, uin
 // Tiles of 64 x 16 canvas pixels.  One canvas size (tile_start == NULL): grid = (tiles of the canvas g, records),
 // canvas b of the arena is record b's.  Mixed sizes: grid = every record's tiles, flattened (tile_start [n + 1]): a CTA
 // finds its record by binary search and takes the canvas geometry from geo[b], so no CTA idles on a small canvas.
-// draw[b] == 0 (an IDLE stream): the record's video is not read.
-// A CTA covers 16 rows (four 4-row passes) so that the two loads every CTA starts with - the record and its flag,
-// issued together - are paid once per 1024 pixels.  A 1:1 record whose rows are 16-byte aligned is copied with 16-byte
-// loads and stores (4 pixels per thread, one pass).
-__global__ void __launch_bounds__(256) k_feed_draw(const FeedRec *__restrict__ recs, const uint8_t *__restrict__ draw,
-                                                   uint8_t *__restrict__ canvas, IngestGeom g, int tiles_x,
-                                                   const EntryCanvas *__restrict__ geo, const int32_t *__restrict__ tile_start,
-                                                   int n) {
-  int b, tile;
-  uint8_t *cv;
+// -> this CTA's record b, its tile, and (g, tiles_x, cv) of the record's canvas
+__device__ __forceinline__ void feed_cta(uint8_t *canvas, IngestGeom &g, int &tiles_x, const EntryCanvas *__restrict__ geo,
+                                         const int32_t *__restrict__ tile_start, int n, int &b, int &tile, uint8_t *&cv) {
   if (tile_start) {
     b = feed_tile_record(tile_start, n, (int)blockIdx.x);
     const EntryCanvas e = geo[b];
@@ -292,6 +348,18 @@ __global__ void __launch_bounds__(256) k_feed_draw(const FeedRec *__restrict__ r
     tile = blockIdx.x;
     cv = canvas + (size_t)b * g.dh * g.dw * 4;
   }
+}
+// draw[b] == 0 (an IDLE stream): the record's video is not read.
+// A CTA covers 16 rows (four 4-row passes) so that the two loads every CTA starts with - the record and its flag,
+// issued together - are paid once per 1024 pixels.  A 1:1 record whose rows are 16-byte aligned is copied with 16-byte
+// loads and stores (4 pixels per thread, one pass).
+__global__ void __launch_bounds__(256) k_feed_draw(const FeedRec *__restrict__ recs, const uint8_t *__restrict__ draw,
+                                                   uint8_t *__restrict__ canvas, IngestGeom g, int tiles_x,
+                                                   const EntryCanvas *__restrict__ geo, const int32_t *__restrict__ tile_start,
+                                                   int n) {
+  int b, tile;
+  uint8_t *cv;
+  feed_cta(canvas, g, tiles_x, geo, tile_start, n, b, tile, cv);
   const FeedRec r = recs[b];
   if (!draw[b]) return;
   const int X0 = (tile % tiles_x) * 64, Y0 = (tile / tiles_x) * 16;
@@ -308,6 +376,56 @@ __global__ void __launch_bounds__(256) k_feed_draw(const FeedRec *__restrict__ r
   for (int i = 0; i < 4; ++i) {
     const int Y = Y0 + 4 * i + (threadIdx.x >> 6);
     if (X < g.dw && Y < g.dh) feed_draw_pixel(r, cv, g, X, Y, 0);
+  }
+}
+// pixels X..X+3 of row Y of YUV record r, converted (X a multiple of 4, X + 3 < width): one 4-byte luma load and one
+// 4-byte NV12 chroma load (U0 V0 U1 V1) where aligned, byte loads otherwise.  Also run on the host by
+// ht_selftest_feed_yuv.
+__host__ __device__ __forceinline__ uint4 yuv_quad(const YuvFeedRec &r, int X, int Y) {
+  const uint8_t *yp = r.y + (size_t)Y * r.ypitch + X;
+  const uint8_t *up = r.u + (size_t)(Y >> 1) * r.upitch + (size_t)(X >> 1) * r.cstep;
+  const uint8_t *vp = r.v + (size_t)(Y >> 1) * r.vpitch + (size_t)(X >> 1) * r.cstep;
+  uint32_t ys;
+  if ((reinterpret_cast<uintptr_t>(yp) & 3u) == 0) {
+    ys = ld_ro(reinterpret_cast<const uint32_t *>(yp));
+  } else {
+    ys = (uint32_t)ld_ro(yp) | (uint32_t)ld_ro(yp + 1) << 8 | (uint32_t)ld_ro(yp + 2) << 16 | (uint32_t)ld_ro(yp + 3) << 24;
+  }
+  uint32_t u0, v0, u1, v1;
+  if (r.cstep == 2 && (reinterpret_cast<uintptr_t>(up) & 3u) == 0) {
+    const uint32_t c = ld_ro(reinterpret_cast<const uint32_t *>(up));
+    u0 = c & 0xffu, v0 = (c >> 8) & 0xffu, u1 = (c >> 16) & 0xffu, v1 = c >> 24;
+  } else {
+    u0 = ld_ro(up), u1 = ld_ro(up + r.cstep), v0 = ld_ro(vp), v1 = ld_ro(vp + r.cstep);
+  }
+  return make_uint4(yuv_to_rgba(r.color, ys & 0xffu, u0, v0), yuv_to_rgba(r.color, (ys >> 8) & 0xffu, u0, v0),
+                    yuv_to_rgba(r.color, (ys >> 16) & 0xffu, u1, v1), yuv_to_rgba(r.color, ys >> 24, u1, v1));
+}
+// k_feed_draw for YUV records (ht_tracker_feed_yuv; ht_ingest_yuv with draw == NULL: every record), the same tiles and
+// grid.  The planes are read directly: no RGBA frame is written.  A 1:1 record on a canvas whose width is a multiple of
+// 4 converts 4 pixels per thread (yuv_quad) and stores them in 16 bytes; the two luma rows of a chroma row are
+// neighbouring threads' and read it from L1.
+__global__ void __launch_bounds__(256) k_feed_draw_yuv(const YuvFeedRec *__restrict__ recs, const uint8_t *__restrict__ draw,
+                                                       uint8_t *__restrict__ canvas, IngestGeom g, int tiles_x,
+                                                       const EntryCanvas *__restrict__ geo,
+                                                       const int32_t *__restrict__ tile_start, int n) {
+  int b, tile;
+  uint8_t *cv;
+  feed_cta(canvas, g, tiles_x, geo, tile_start, n, b, tile, cv);
+  const YuvFeedRec r = recs[b];
+  if (draw && !draw[b]) return;
+  const int X0 = (tile % tiles_x) * 64, Y0 = (tile / tiles_x) * 16;
+  if (r.width == g.dw && r.height == g.dh && (g.dw & 3) == 0 && (reinterpret_cast<uintptr_t>(cv) & 15u) == 0) {
+    const int X = X0 + 4 * (threadIdx.x & 15), Y = Y0 + (threadIdx.x >> 4);
+    if (X >= g.dw || Y >= g.dh) return;
+    reinterpret_cast<uint4 *>(cv + (size_t)Y * g.dw * 4)[X >> 2] = yuv_quad(r, X, Y);
+    return;
+  }
+  const int X = X0 + (threadIdx.x & 63);
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int Y = Y0 + 4 * i + (threadIdx.x >> 6);
+    if (X < g.dw && Y < g.dh) feed_yuv_pixel(r, cv, g, X, Y);
   }
 }
 

@@ -223,6 +223,21 @@ class TrackerSet:
         (numpy or torch CUDA, any video size), drawn onto a width x height canvas; now_ms = None (the wall clock), one
         clock, or {stream: ms}; width and height: one canvas size for all, or {stream: pixels} (each stream on its own
         canvas, ht_tracker_feed_canvases).  Streams not listed do not tick.  -> {stream: record}."""
+        return self._feed(frames, now_ms, width, height, self.ctx.tracker_feed)
+
+    def feed_yuv(self, frames, now_ms=None, width=None, height=None, format="nv12", color="bt601"):
+        """feed on YUV 4:2:0 video (ht_tracker_feed_yuv): frames = {stream: (Y, UV) NV12 or (Y, U, V) I420 planes}
+        (Context.tracker_feed_yuv), format and color one for all or {stream: value}; the rest as for feed, and events
+        are dispatched as feed dispatches them."""
+        ks = list(frames)
+        fmts = [format[k] for k in ks] if isinstance(format, dict) else format
+        colors = [color[k] for k in ks] if isinstance(color, dict) else color
+
+        def call(ks, vids, now, width, height, out=None):
+            return self.ctx.tracker_feed_yuv(ks, vids, now, width, height, format=fmts, color=colors, out=out)
+        return self._feed(frames, now_ms, width, height, call)
+
+    def _feed(self, frames, now_ms, width, height, tick):
         if width is None or height is None:
             raise ValueError("the canvas size (width, height) is required")
         ks = list(frames)
@@ -242,11 +257,11 @@ class TrackerSet:
         if self._device_events:
             import torch
             buf = torch.empty(len(ks) * 144, dtype=torch.uint8, device="cuda")
-            self.ctx.tracker_feed(ks, [frames[k] for k in ks], now, width, height, out=buf)
+            tick(ks, [frames[k] for k in ks], now, width, height, out=buf)
             self.ctx.sync()                            # the records are written on the library's stream
             recs = tracker_events_from_bytes(buf.cpu().numpy().tobytes())
         else:
-            recs = self.ctx.tracker_feed(ks, [frames[k] for k in ks], now, width, height)
+            recs = tick(ks, [frames[k] for k in ks], now, width, height)
         self._dispatch(ks, recs, int((time.time() - t0) * 1000))
         return dict(zip(ks, recs))
 

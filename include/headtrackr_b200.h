@@ -313,6 +313,60 @@ typedef struct {
 int ht_tracker_feed_canvases(ht_ctx *ctx, const ht_canvas_frame *frames, int n, int frames_on_device,
                              ht_tracker_event *out);
 
+/* YUV 4:2:0 video, as decoders write it: NV12 (hardware decoders), I420 (software decoders, JPEG decoders' 4:2:0
+ * output).  The frame is drawn as the RGBA8 frame this library's conversion makes of it (DESIGN.md 2, "YUV video"):
+ * luma pixel (x, y) takes chroma sample (x >> 1, y >> 1), then an integer BT.601 or BT.709 matrix, limited or full
+ * range, A = 255.  Byte offsets:
+ *     0  const uint8_t *planes[3]   NV12: Y, interleaved UV (U first), NULL.  I420: Y, U, V
+ *    24  int32 pitch[3]             bytes per row; 0 -> the tight pitch: width for Y, 2*ceil(width/2) for the NV12 UV
+ *                                   plane, ceil(width/2) for I420 U and V; otherwise >= that, any alignment (unused
+ *                                   for a NULL plane)
+ *    36  int32 width, height        luma size, 1..16384; the chroma planes are ceil(width/2) x ceil(height/2) samples
+ *    44  int32 format               HT_YUV_NV12 or HT_YUV_I420
+ *    48  int32 color                HT_YUV_BT601 or HT_YUV_BT709, optionally | HT_YUV_FULL_RANGE
+ *    52  int32 pad_ */
+#define HT_YUV_NV12 0
+#define HT_YUV_I420 1
+#define HT_YUV_BT601 0
+#define HT_YUV_BT709 1
+#define HT_YUV_FULL_RANGE 2
+typedef struct {
+  const uint8_t *planes[3];
+  int32_t pitch[3];
+  int32_t width, height;
+  int32_t format;
+  int32_t color;
+  int32_t pad_;
+} ht_yuv_image;           /* 56 bytes */
+/* One stream's YUV video frame, working canvas and clock for ht_tracker_feed_yuv: the YUV counterpart of
+ * ht_canvas_frame.  Byte offsets: 0 video, 56 stream, 60 canvas_w, 64 canvas_h, 68 pad_, 72 now_ms. */
+typedef struct {
+  ht_yuv_image video;
+  int32_t stream;               /* tracker stream id in [0, max_frames) */
+  int32_t canvas_w, canvas_h;   /* this record's working canvas */
+  int32_t pad_;
+  double now_ms;                /* (new Date).getTime() when this stream's timer fired */
+} ht_yuv_frame;                 /* 80 bytes */
+/* ht_tracker_feed_canvases on YUV video: drawImage(video, 0, 0, canvas_w, canvas_h) of the decoded frame, converted
+ * and scaled in one pass straight from the planes (no RGBA copy of the video is made), then the same tick.  A record
+ * gives exactly the canvas and the event of ht_tracker_feed_canvases on the RGBA8 frame the conversion makes of its
+ * video.  The contract is ht_tracker_feed_canvases's: any subset of streams in any order, each record with its own
+ * canvas and clock, out[n] in record order on the host or the device, an IDLE stream's planes never read.  The
+ * streams' state is the one every tick uses: a stream may tick from YUV, RGBA and ht_tracker_step in turn.  Host
+ * planes are packed into the library's staging buffer; only the first record's Y pointer is tested against
+ * frames_on_device.  Same launches as ht_tracker_feed_canvases on the same canvases.
+ * Errors (nothing is enqueued): those of ht_tracker_feed_canvases, and HT_ERR_ARG, with the record's index in
+ * ht_last_error, for a format or color outside the values above, a NULL Y or chroma plane, a non-NULL planes[2] for
+ * NV12, or a pitch below the tight pitch; HT_ERR_SIZE for a video size outside 1..16384. */
+int ht_tracker_feed_yuv(ht_ctx *ctx, const ht_yuv_frame *frames, int n, int frames_on_device, ht_tracker_event *out);
+/* ht_ingest for YUV video: src[i] (host records; planes all host or all device memory, as frames_on_device says, only
+ * src[0]'s Y pointer is tested) drawn onto the i-th tightly packed dw x dh RGBA8 canvas of dst_rgba (host or device
+ * memory; a 4-byte aligned pointer), for i in [0, n).  The frames may differ in size, format and color.  One launch.
+ * Errors (nothing is enqueued): HT_ERR_ARG for NULL pointers, n <= 0, a misaligned dst, a contradicting memory space
+ * or a bad record (as for ht_tracker_feed_yuv); HT_ERR_SIZE for sizes outside 1..16384 or a canvas too large for the
+ * resampler. */
+int ht_ingest_yuv(ht_ctx *ctx, const ht_yuv_image *src, int n, int frames_on_device, uint8_t *dst_rgba, int dw, int dh);
+
 /* A stream's debug canvas: `params.debug` of its headtrackr.Tracker (src/main.js:42-50). */
 typedef struct {
   uint8_t *rgba;          /* DEVICE memory, `height` rows of `pitch` bytes; NULL: the stream has no debug canvas */

@@ -31,6 +31,9 @@
 //   trackerFeed(handle, [{stream, rgba, width, height, nowMs, canvasWidth?, canvasHeight?}], canvasWidth, canvasHeight)
 //        -> Array<record> (ht_tracker_feed_canvases: only the listed streams tick, each from its own video frame, clock
 //        and canvas)
+//   trackerFeedYuv(handle, [{stream, nowMs, canvasWidth, canvasHeight, format, color, width, height, y, uv | u, v}])
+//        -> Array<record> (ht_tracker_feed_yuv: NV12 / I420 host planes, tight pitches)
+//   ingestYuv(handle, [{format, color, width, height, y, uv | u, v}], dw, dh) -> Uint8ClampedArray   (ht_ingest_yuv)
 //   destroy(handle)
 #include <node_api.h>
 
@@ -655,6 +658,94 @@ static napi_value TrackerFeed(napi_env env, napi_callback_info info) {
   return out;
 }
 
+// a YUV frame object {format: "nv12"|"i420", color: "bt601"|"bt709"|"bt601-full"|"bt709-full", width, height, y, uv | u, v}
+// (host Buffers / typed arrays, tight pitches) -> an ht_yuv_image; false for a bad object
+static bool YuvImageOf(napi_env env, napi_value r, ht_yuv_image *img) {
+  std::memset(img, 0, sizeof(*img));
+  char s[16] = "";
+  size_t sl = 0;
+  napi_value v;
+  bool has = false;
+  img->width = (int32_t)GetNumProp(env, r, "width", 0);
+  img->height = (int32_t)GetNumProp(env, r, "height", 0);
+  if (img->width <= 0 || img->height <= 0) return false;
+  if (napi_has_named_property(env, r, "format", &has) == napi_ok && has && napi_get_named_property(env, r, "format", &v) == napi_ok)
+    napi_get_value_string_utf8(env, v, s, sizeof(s), &sl);
+  img->format = (sl == 0 || std::strcmp(s, "nv12") == 0) ? HT_YUV_NV12 : std::strcmp(s, "i420") == 0 ? HT_YUV_I420 : -1;
+  sl = 0;
+  if (napi_has_named_property(env, r, "color", &has) == napi_ok && has && napi_get_named_property(env, r, "color", &v) == napi_ok)
+    napi_get_value_string_utf8(env, v, s, sizeof(s), &sl);
+  const char *names[4] = {"bt601", "bt709", "bt601-full", "bt709-full"};
+  img->color = sl == 0 ? HT_YUV_BT601 : -1;
+  for (int i = 0; i < 4 && sl; ++i)
+    if (std::strcmp(s, names[i]) == 0) img->color = i;   // HT_YUV_BT709 = 1, HT_YUV_FULL_RANGE = 2
+  const size_t cw = (size_t)(img->width + 1) / 2, ch = (size_t)(img->height + 1) / 2;
+  const bool nv12 = img->format == HT_YUV_NV12;
+  const char *keys[3] = {"y", nv12 ? "uv" : "u", "v"};
+  const size_t need[3] = {(size_t)img->width * img->height, (nv12 ? 2 : 1) * cw * ch, cw * ch};
+  for (int p = 0; p < (nv12 ? 2 : 3); ++p) {
+    uint8_t *data; size_t len;
+    if (napi_get_named_property(env, r, keys[p], &v) != napi_ok || !GetBytes(env, v, &data, &len) || len < need[p]) return false;
+    img->planes[p] = data;
+  }
+  return true;
+}
+
+// trackerFeedYuv(handle, [{stream, nowMs, canvasWidth, canvasHeight, ...a YUV frame object}]) -> Array<record>
+// (ht_tracker_feed_yuv with host planes)
+static napi_value TrackerFeedYuv(napi_env env, napi_callback_info info) {
+  size_t argc = 2;
+  napi_value argv[2];
+  NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+  ht_ctx *ctx = Ctx(env, argv[0]);
+  uint32_t n = 0;
+  NAPI_OK(napi_get_array_length(env, argv[1], &n));
+  if (n == 0) return Throw(env, ctx, HT_ERR_ARG);
+  std::vector<ht_yuv_frame> frames(n);
+  for (uint32_t b = 0; b < n; ++b) {
+    napi_value r;
+    NAPI_OK(napi_get_element(env, argv[1], b, &r));
+    std::memset(&frames[b], 0, sizeof(frames[b]));
+    if (!YuvImageOf(env, r, &frames[b].video)) return Throw(env, ctx, HT_ERR_ARG);
+    frames[b].stream = (int32_t)GetNumProp(env, r, "stream", -1);
+    frames[b].canvas_w = (int32_t)GetNumProp(env, r, "canvasWidth", 0);
+    frames[b].canvas_h = (int32_t)GetNumProp(env, r, "canvasHeight", 0);
+    frames[b].now_ms = GetNumProp(env, r, "nowMs", 0.0);
+  }
+  std::vector<ht_tracker_event> ev(n);
+  int rc = ht_tracker_feed_yuv(ctx, frames.data(), (int)n, 0, ev.data());
+  if (rc < 0) return Throw(env, ctx, rc);
+  napi_value out;
+  napi_create_array_with_length(env, (size_t)n, &out);
+  for (uint32_t b = 0; b < n; ++b) napi_set_element(env, out, b, TrackerEventObject(env, ev[b]));
+  return out;
+}
+
+// ingestYuv(handle, [YUV frame object, ...], dw, dh) -> Uint8ClampedArray (n canvases)   (ht_ingest_yuv)
+static napi_value IngestYuv(napi_env env, napi_callback_info info) {
+  size_t argc = 4;
+  napi_value argv[4];
+  NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+  ht_ctx *ctx = Ctx(env, argv[0]);
+  uint32_t n = 0;
+  int32_t dw, dh;
+  NAPI_OK(napi_get_array_length(env, argv[1], &n));
+  napi_get_value_int32(env, argv[2], &dw); napi_get_value_int32(env, argv[3], &dh);
+  if (n == 0 || dw <= 0 || dh <= 0) return Throw(env, ctx, HT_ERR_ARG);
+  std::vector<ht_yuv_image> imgs(n);
+  for (uint32_t b = 0; b < n; ++b) {
+    napi_value r;
+    NAPI_OK(napi_get_element(env, argv[1], b, &r));
+    if (!YuvImageOf(env, r, &imgs[b])) return Throw(env, ctx, HT_ERR_ARG);
+  }
+  void *data; napi_value ab, ta;
+  NAPI_OK(napi_create_arraybuffer(env, (size_t)n * dw * dh * 4, &data, &ab));
+  int rc = ht_ingest_yuv(ctx, imgs.data(), (int)n, 0, static_cast<uint8_t *>(data), dw, dh);
+  if (rc < 0) return Throw(env, ctx, rc);
+  NAPI_OK(napi_create_typedarray(env, napi_uint8_clamped_array, (size_t)n * dw * dh * 4, ab, 0, &ta));
+  return ta;
+}
+
 static napi_value Init(napi_env env, napi_value exports) {
   napi_property_descriptor d[] = {
       {"trackerConfig", nullptr, TrackerConfig, nullptr, nullptr, nullptr, napi_default, nullptr},
@@ -668,6 +759,8 @@ static napi_value Init(napi_env env, napi_value exports) {
       {"trackerExport", nullptr, TrackerExport, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerImport", nullptr, TrackerImport, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerFeed", nullptr, TrackerFeed, nullptr, nullptr, nullptr, napi_default, nullptr},
+      {"trackerFeedYuv", nullptr, TrackerFeedYuv, nullptr, nullptr, nullptr, napi_default, nullptr},
+      {"ingestYuv", nullptr, IngestYuv, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"create", nullptr, Create, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"detect", nullptr, Detect, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackInit", nullptr, TrackInit, nullptr, nullptr, nullptr, napi_default, nullptr},

@@ -15,6 +15,10 @@ streams: N 640x480 streams, device-resident frames and outputs, CUDA events arou
   camera_*        (--camera-streams) ht_tracker_feed with head-coupled camera controllers on none, 1/64 and all of
                   the streams, k_camera_update's kernel time, and the no-controller arm against --before-lib
                   (camera_arms)
+  yuv_* twopass_* rgba_*
+                  (--yuv) ht_tracker_feed_yuv from NV12 video against ht_ingest_yuv + ht_tracker_feed and against
+                  ht_tracker_feed from RGBA video of the same size (also --before-lib), and the draw kernels' time
+                  (yuv_arms)
 
 Prints one JSON line with the card's name and power limit read in the same run; --out also writes it to a file."""
 import argparse
@@ -527,6 +531,148 @@ def camera_arms(torch, frames, stream, N, W, H, steps, rounds, before_lib=None):
     return res
 
 
+YUV_LAYOUTS = [((1280, 720), (320, 240)), ((1280, 720), (640, 480)), ((640, 480), (640, 480))]
+
+
+def yuv_arms(torch, stream, N, steps, rounds, before_lib=None):
+    """YUV video (ht_tracker_feed_yuv) in steady tracking, for each (video, canvas) of YUV_LAYOUTS: N streams, each
+    with its own NV12 device video (BT.601 limited range), every arm on its own context, all arms of a layout
+    alternating tick by tick (the arm order rotates), CUDA events around each tick:
+
+      yuv_<layout>_cs          ht_tracker_feed_yuv from the NV12 planes onto the canvas
+      twopass_<layout>_cs      ht_ingest_yuv of the batch into a device RGBA buffer of the video's size, then
+                               ht_tracker_feed from it (what a caller writes without ht_tracker_feed_yuv)
+      rgba_<layout>_cs         ht_tracker_feed from RGBA video of the same size (the converted frames)
+      rgba_before_<layout>_cs  the same with the library at `before_lib` (e.g. the parent commit's build)
+
+    Then, in runs of their own under torch.profiler, the kernel time of the draw per tick: k_feed_draw_yuv in the yuv
+    arm, k_feed_draw in the rgba arm, with the bytes each must move (plane or RGBA bytes of the video read once, RGBA
+    canvas written) over that time.  The records of every arm must agree on every timed tick."""
+    import ctypes as C
+    from headtrackr_b200 import Context, _lib, synth
+    from headtrackr_b200.context import _yuv_image
+    rec_bytes = C.sizeof(_lib.TrackerEvent)
+    res = {}
+    for (W, H), (CW, CH) in YUV_LAYOUTS:
+        lay = f"{W}x{H}_{CW}x{CH}"
+        now = [1.0e12]
+        kw = dict(max_width=CW, max_height=CH, max_frames=N, stream=stream)
+        # each stream its own video: one of 8 synth frames, shifted right by its own offset, so that every tick reads
+        # N distinct frames from HBM as N cameras would
+        base = torch.stack([torch.from_numpy(synth.frame(i, W, H, n_faces=1)) for i in range(8)]).cuda()
+        ys = torch.empty((N, H, W), dtype=torch.uint8, device="cuda")
+        uvs = torch.empty((N, H // 2, W), dtype=torch.uint8, device="cuda")
+        for k0 in range(0, N, 64):
+            k1 = min(N, k0 + 64)
+            f = torch.stack([torch.roll(base[k % 8], shifts=2 * (k // 8) % 64, dims=1) for k in range(k0, k1)]).float()
+            r, g, b = f[..., 0], f[..., 1], f[..., 2]
+            y = 16 + (65.481 * r + 128.553 * g + 24.966 * b) / 255
+            u = 128 + (-37.797 * r - 74.203 * g + 112.0 * b) / 255
+            v = 128 + (112.0 * r - 93.786 * g - 18.214 * b) / 255
+            uv = torch.stack([u[:, 0::2, 0::2], v[:, 0::2, 0::2]], dim=-1).reshape(k1 - k0, H // 2, W)
+            ys[k0:k1] = torch.floor(y + 0.5).clamp(0, 255).to(torch.uint8)
+            uvs[k0:k1] = torch.floor(uv + 0.5).clamp(0, 255).to(torch.uint8)
+        del base, f, r, g, b, y, u, v, uv
+        planes = [(ys[k], uvs[k]) for k in range(N)]
+        keep = []
+        imgs = [_yuv_image(p, "nv12", "bt601", keep)[0] for p in planes]
+        conv = Context(max_width=CW, max_height=CH, max_frames=1, stream=stream)
+        rgba = torch.empty((N, H, W, 4), dtype=torch.uint8, device="cuda")      # the converted video, for the RGBA arms
+        conv.ingest_yuv(planes, W, H, out=rgba)
+        conv.sync()
+        conv.close()
+        yrecs = (_lib.YuvFrame * N)()
+        vrecs = (_lib.VideoFrame * N)()
+        for k in range(N):
+            yrecs[k] = _lib.YuvFrame(imgs[k], k, CW, CH, 0, 0.0)
+            vrecs[k] = _lib.VideoFrame(rgba[k].data_ptr(), k, W, H, 0, 0.0)
+        ingest_src = (_lib.YuvImage * N)(*imgs)
+        staged = torch.empty((N, H, W, 4), dtype=torch.uint8, device="cuda")
+        srecs = (_lib.VideoFrame * N)()
+        for k in range(N):
+            srecs[k] = _lib.VideoFrame(staged[k].data_ptr(), k, W, H, 0, 0.0)
+
+        def arm(kind):
+            c = other_build_context(before_lib, **kw) if kind == "rgba_before" else Context(**kw)
+            c.tracker_config()
+            c.tracker_reset(0, N)
+            c.tracker_start(0, N)
+            out = torch.empty(N * rec_bytes, dtype=torch.uint8, device="cuda")
+
+            def run():
+                t = now[0]
+                if kind == "yuv":
+                    for k in range(N):
+                        yrecs[k].now_ms = t
+                    c._check(c._L.ht_tracker_feed_yuv(c._h, C.addressof(yrecs), N, 1, out.data_ptr()))
+                    return
+                recs = vrecs
+                if kind == "twopass":
+                    c._check(c._L.ht_ingest_yuv(c._h, C.addressof(ingest_src), N, 1, staged.data_ptr(), W, H))
+                    recs = srecs
+                for k in range(N):
+                    recs[k].now_ms = t
+                c._check(c._L.ht_tracker_feed(c._h, C.addressof(recs), N, 1, CW, CH, out.data_ptr()))
+            return c, run, out
+
+        kinds = ["yuv", "twopass", "rgba"] + (["rgba_before"] if before_lib else [])
+        arms = {k: arm(k) for k in kinds}
+
+        def tick(name):
+            _, run, _ = arms[name]
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            a.record()
+            run()
+            b.record()
+            b.synchronize()
+            return a.elapsed_time(b)
+
+        for _ in range(17):                      # the whitebalance gate, detection, the first CS frames
+            now[0] += 20.0
+            for name in kinds:
+                tick(name)
+        times = {name: [[] for _ in range(rounds)] for name in kinds}
+        for r in range(rounds):
+            for s in range(steps):
+                now[0] += 20.0
+                rot = (r * steps + s) % len(kinds)
+                for name in kinds[rot:] + kinds[:rot]:
+                    times[name][r].append(tick(name))
+                first = arms["yuv"][2]
+                if any(not torch.equal(first, arms[name][2]) for name in kinds[1:]):
+                    raise SystemExit(f"yuv arms disagree on the records of a timed tick ({lay})")
+        for name in kinds:
+            med = [float(np.median(t)) for t in times[name]]
+            res[f"{name}_{lay}_cs_ms"] = float(np.median(sum(times[name], [])))
+            res[f"{name}_{lay}_cs_spread_ms"] = max(med) - min(med)
+        ev = [_lib.TrackerEvent.from_buffer_copy(bytes(row)) for row in arms["yuv"][2].cpu().numpy().reshape(N, rec_bytes)]
+        res[f"yuv_{lay}_cs_streams"] = sum(e.detection == 2 for e in ev)
+
+        from torch.profiler import ProfilerActivity, profile
+        canvas_bytes = N * CW * CH * 4
+        for name, kernel, video_bytes in (("yuv", "k_feed_draw_yuv", N * W * H * 3 // 2), ("rgba", "k_feed_draw", N * W * H * 4)):
+            with profile(activities=[ProfilerActivity.CUDA]) as prof:
+                for _ in range(steps):
+                    now[0] += 20.0
+                    arms[name][1]()
+                torch.cuda.synchronize()
+            us = 0.0
+            for e in prof.key_averages():
+                base = e.key.split("(")[0].split("<")[0]
+                if base.endswith(kernel) and (kernel == "k_feed_draw_yuv" or not base.endswith("k_feed_draw_yuv")):
+                    t = getattr(e, "device_time_total", None)
+                    us += t if t is not None else e.cuda_time_total
+            ms = us / 1000.0 / steps
+            res[f"{kernel}_{lay}_ms"] = ms
+            res[f"{kernel}_{lay}_gb_per_s"] = (video_bytes + canvas_bytes) / (ms * 1e-3) / 1e9 if ms > 0 else None
+        for c, _, _ in arms.values():
+            c.close()
+        del staged, rgba, planes, keep, ys, uvs
+        torch.cuda.empty_cache()
+    res["yuv_records_agree"] = True
+    return res
+
+
 def migrate_arms(torch, frames, stream, N, W, H, steps, rounds):
     """Tracker records (ht_tracker_export / ht_tracker_import) of N streams in steady tracking, W x H video on W/2 x H/2
     canvases, CUDA events on the library's stream around each call, repeated `rounds` x `steps` times:
@@ -628,6 +774,7 @@ def main():
     ap.add_argument("--debug-streams", action="store_true", help="only the debug-canvas arms (debug_arms)")
     ap.add_argument("--migrate", action="store_true", help="only the tracker-record arms (migrate_arms)")
     ap.add_argument("--camera-streams", action="store_true", help="only the camera-controller arms (camera_arms)")
+    ap.add_argument("--yuv", action="store_true", help="only the YUV video arms (yuv_arms)")
     ap.add_argument("--out")
     a = ap.parse_args()
     import torch
@@ -641,6 +788,9 @@ def main():
     ts = torch.cuda.Stream()                # the library runs on this stream and the events below are recorded on it
     torch.cuda.set_stream(ts)
     stream = ts.cuda_stream
+    if a.yuv:
+        res.update(yuv_arms(torch, stream, N, a.steps, a.rounds, a.before_lib))
+        return report(res, a.out)
     if a.migrate:
         res.update(migrate_arms(torch, frames, stream, N, W, H, a.steps, a.rounds))
         return report(res, a.out)
