@@ -76,12 +76,14 @@ class CanvasFrame(C.Structure):
 
 
 # ht_yuv_image.format / .color
-YUV_FORMATS = {"nv12": 0, "i420": 1}
-YUV_COLORS = {"bt601": 0, "bt709": 1, "bt601-full": 2, "bt709-full": 3}
+YUV_FORMATS = {"nv12": 0, "i420": 1, "nv21": 16, "i422": 17, "i444": 18, "yuyv": 19, "uyvy": 20, "p010": 21,
+               "bgra": 32, "bgr24": 33, "rgb24": 34}
+YUV_COLORS = {"bt601": 0, "bt709": 1, "bt601-full": 2, "bt709-full": 3, "bt2020": 8, "bt2020-full": 10}
 
 
 class YuvImage(C.Structure):
-    """ht_yuv_image: a YUV 4:2:0 video frame (NV12: Y, UV, NULL; I420: Y, U, V; pitch 0 = the tight pitch)"""
+    """ht_yuv_image: a video frame of one of YUV_FORMATS (the planes of each: include/headtrackr_b200.h; pitch 0 = the
+    tight pitch)"""
     _fields_ = [("planes", C.c_void_p * 3), ("pitch", C.c_int32 * 3), ("width", C.c_int32), ("height", C.c_int32),
                 ("format", C.c_int32), ("color", C.c_int32), ("pad_", C.c_int32)]
 

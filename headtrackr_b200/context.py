@@ -34,43 +34,71 @@ def _frames_ptr(frames):
     return a.ctypes.data, a.shape[0], a.shape[1], a.shape[2], a
 
 
+# planes of the planar formats, channels of the packed ones (an (h, w, channels) array)
+_PLANAR = {"nv12": 2, "i420": 3, "nv21": 2, "i422": 3, "i444": 3, "p010": 2}
+_PACKED = {"yuyv": 2, "uyvy": 2, "bgra": 4, "bgr24": 3, "rgb24": 3}
+
+
+def _plane(p, ndim, wide):
+    """one plane: a numpy array or torch tensor of `ndim` dimensions, uint8 (wide: 16-bit samples), unit column stride
+    (a packed array: contiguous pixels) -> (address, pitch in bytes, shape, on_device, the object to keep alive)"""
+    item = 2 if wide else 1
+    what = "uint16" if wide else "uint8"
+    if _is_torch(p):
+        inner = p.dim() == ndim and p.stride(ndim - 1) == 1 and (ndim == 2 or p.stride(1) == p.shape[2])
+        if not inner or p.element_size() != item or p.is_floating_point():
+            raise ValueError(f"plane tensors must be {ndim}-D {what} with unit column stride"
+                             + ("" if ndim == 2 else " and contiguous pixels"))
+        return p.data_ptr(), p.stride(0) * item, tuple(p.shape), bool(p.is_cuda), p
+    a = np.asarray(p)
+    if a.dtype != (np.uint16 if wide else np.uint8) or a.ndim != ndim:
+        raise ValueError(f"planes must be {ndim}-D {what}")
+    row = item * int(np.prod(a.shape[1:]))
+    if a.strides[-1] != item or (ndim == 3 and a.strides[1] != item * a.shape[2]) or a.strides[0] < row:
+        a = np.ascontiguousarray(a)
+    return a.ctypes.data, a.strides[0], tuple(a.shape), False, a
+
+
 def _yuv_image(planes, fmt, color, keep):
-    """a YUV 4:2:0 frame - a tuple of 2-D uint8 planes, (Y, UV) for NV12 or (Y, U, V) for I420, all numpy arrays or torch
-    tensors (CPU or CUDA) with unit column stride; row strides become pitches - -> (ht_yuv_image, on_device).  The
-    planes are appended to `keep`."""
+    """a video frame of one of _lib.YUV_FORMATS -> (ht_yuv_image, on_device); the planes are appended to `keep`.
+      planar formats: a tuple of 2-D planes, (Y, UV) for NV12, (Y, VU) for NV21, (Y, U, V) for I420, I422 and I444,
+        (Y, UV) of 16-bit samples for P010 (numpy uint16, torch uint16 or int16);
+      packed formats: ONE array, (h, w, 2) uint8 for YUYV and UYVY, (h, w, 4) for BGRA, (h, w, 3) for BGR24 and RGB24
+        (an OpenCV frame as it is); an odd-width packed 4:2:2 frame needs a row stride of at least 4 * ceil(w / 2).
+    numpy arrays or torch tensors (CPU or CUDA) with unit column stride; row strides become pitches."""
     if fmt not in _lib.YUV_FORMATS:
         raise ValueError(f"format must be one of {sorted(_lib.YUV_FORMATS)}")
     if color not in _lib.YUV_COLORS:
         raise ValueError(f"color must be one of {sorted(_lib.YUV_COLORS)}")
-    nv12 = fmt == "nv12"
-    if len(planes) != (2 if nv12 else 3):
-        raise ValueError("an NV12 frame is (Y, UV), an I420 frame (Y, U, V)")
+    if fmt in _PACKED:
+        if isinstance(planes, (tuple, list)):
+            raise ValueError(f"a {fmt} frame is one (h, w, {_PACKED[fmt]}) array")
+        ptr, pitch, shape, dev, obj = _plane(planes, 3, False)
+        if shape[2] != _PACKED[fmt]:
+            raise ValueError(f"a {fmt} frame is one (h, w, {_PACKED[fmt]}) array, not {shape}")
+        keep.append(obj)
+        img = YuvImage((C.c_void_p * 3)(ptr, None, None), (C.c_int32 * 3)(pitch, 0, 0), shape[1], shape[0],
+                       _lib.YUV_FORMATS[fmt], _lib.YUV_COLORS[color])
+        return img, dev
+    if len(planes) != _PLANAR[fmt]:
+        if fmt in ("nv12", "i420"):
+            raise ValueError("an NV12 frame is (Y, UV), an I420 frame (Y, U, V)")
+        raise ValueError(f"a {fmt} frame is {_PLANAR[fmt]} planes")
     ptrs, pitches, shapes, where = [], [], [], set()
     for p in planes:
-        if _is_torch(p):
-            if p.dim() != 2 or p.element_size() != 1 or p.stride(1) != 1:
-                raise ValueError("plane tensors must be 2-D uint8 with unit column stride")
-            ptrs.append(p.data_ptr())
-            pitches.append(p.stride(0))
-            where.add(bool(p.is_cuda))
-        else:
-            a = np.asarray(p)
-            if a.dtype != np.uint8 or a.ndim != 2:
-                raise ValueError("planes must be 2-D uint8")
-            if a.strides[1] != 1 or a.strides[0] < a.shape[1]:
-                a = np.ascontiguousarray(a)
-            p = a
-            ptrs.append(a.ctypes.data)
-            pitches.append(a.strides[0])
-            where.add(False)
-        keep.append(p)
-        shapes.append(tuple(p.shape))
+        ptr, pitch, shape, dev, obj = _plane(p, 2, fmt == "p010")
+        ptrs.append(ptr)
+        pitches.append(pitch)
+        shapes.append(shape)
+        where.add(dev)
+        keep.append(obj)
     if len(where) != 1:
         raise ValueError("the planes of a frame must all be host or all be device memory")
     h, w = shapes[0]
     ch, cw = (h + 1) // 2, (w + 1) // 2
+    need = {"nv12": (ch, 2 * cw), "nv21": (ch, 2 * cw), "p010": (ch, 2 * cw), "i420": (ch, cw), "i422": (h, cw),
+            "i444": (h, w)}[fmt]
     for i, shape in enumerate(shapes[1:], 1):
-        need = (ch, 2 * cw) if nv12 else (ch, cw)
         if shape[0] < need[0] or shape[1] < need[1]:
             raise ValueError(f"plane {i} is {shape}, a {w}x{h} {fmt} frame needs {need}")
     img = YuvImage((C.c_void_p * 3)(*(ptrs + [None] * (3 - len(ptrs)))), (C.c_int32 * 3)(*(pitches + [0] * (3 - len(pitches)))),
@@ -474,12 +502,15 @@ class Context:
         return [tracker_event_dict(e) for e in ev]
 
     def tracker_feed_yuv(self, streams, frames, now_ms, width, height, format="nv12", color="bt601", out=None):
-        """tracker_feed on YUV 4:2:0 video (ht_tracker_feed_yuv): each frame is a tuple of 2-D uint8 planes, (Y, UV) for
-        NV12 or (Y, U, V) for I420, numpy arrays or torch tensors (CPU, or CUDA for every frame), whose row strides
-        are the pitches.  A decoder's packed NV12 buffer `buf` of h + ceil(h/2) rows splits without a copy:
+        """tracker_feed on video in any of _lib.YUV_FORMATS (ht_tracker_feed_yuv): each frame is a tuple of 2-D planes
+        for a planar format ((Y, UV) for NV12, (Y, U, V) for I420, uint16 planes for P010) or one (h, w, channels)
+        array for a packed one (YUYV, UYVY, BGRA, BGR24, RGB24; _yuv_image), numpy arrays or torch tensors (CPU, or
+        CUDA for every frame), whose row strides are the pitches.  A decoder's packed NV12 buffer `buf` of
+        h + ceil(h/2) rows splits without a copy:
             frame = (buf[:h, :w], buf[h:, :2 * ((w + 1) // 2)])
-        The conversion is the library's (DESIGN.md 2): format "nv12" / "i420" and color "bt601" / "bt709" /
-        "bt601-full" / "bt709-full", one for all or one per record.  now_ms, width and height as for tracker_feed
+        The conversion is the library's (DESIGN.md 2): format (a key of _lib.YUV_FORMATS) and color ("bt601",
+        "bt709", "bt2020", each optionally "-full"; "bt601" for the packed RGB formats), one for all or one per
+        record.  now_ms, width and height as for tracker_feed
         (every record has its own canvas here).  -> event dicts in record order; with a torch CUDA `out` tensor of
         len(streams)*144 bytes: asynchronous, nothing returned."""
         streams = list(streams)
@@ -508,8 +539,8 @@ class Context:
         return [tracker_event_dict(e) for e in ev]
 
     def ingest_yuv(self, frames, width, height, format="nv12", color="bt601", out=None):
-        """drawImage(video, 0, 0, width, height) of YUV 4:2:0 frames (ht_ingest_yuv): frames, format and color as for
-        tracker_feed_yuv (the frames may differ in size).  -> numpy (n, height, width, 4); with a torch `out` tensor
+        """drawImage(video, 0, 0, width, height) of video frames (ht_ingest_yuv): frames, format and color as for
+        tracker_feed_yuv (the frames may differ in size and format).  -> numpy (n, height, width, 4); with a torch `out` tensor
         of that shape (CUDA or CPU) the result is written there."""
         n = len(frames)
         if n == 0:

@@ -2201,27 +2201,74 @@ static bool canvas_geom(int w, int h, IngestGeom &g) {
   return true;
 }
 
-// An ht_yuv_image checked and resolved into r: pitches resolved, NV12's V at U + 1.  -> HT_OK, or the error code with
-// the reason in why[256].
+// The planes of a w x h frame of `format` (the table at ht_yuv_image): -> how many it has (0: not a format), and the
+// tight pitch (bytes) and rows of each
+static int yuv_planes(int format, int w, int h, int tight[3], int rows[3]) {
+  const int cw = (w + 1) / 2, ch = (h + 1) / 2;
+  auto set = [&](int n, int t0, int r0, int t1 = 0, int r1 = 0, int t2 = 0, int r2 = 0) {
+    tight[0] = t0, tight[1] = t1, tight[2] = t2, rows[0] = r0, rows[1] = r1, rows[2] = r2;
+    return n;
+  };
+  switch (format) {
+    case HT_YUV_NV12: case HT_YUV_NV21: return set(2, w, h, 2 * cw, ch);
+    case HT_YUV_I420: return set(3, w, h, cw, ch, cw, ch);
+    case HT_YUV_I422: return set(3, w, h, cw, h, cw, h);
+    case HT_YUV_I444: return set(3, w, h, w, h, w, h);
+    case HT_YUV_YUYV: case HT_YUV_UYVY: return set(1, 4 * cw, h);
+    case HT_YUV_P010: return set(2, 2 * w, h, 4 * cw, ch);
+    case HT_YUV_BGRA: return set(1, 4 * w, h);
+    case HT_YUV_BGR24: case HT_YUV_RGB24: return set(1, 3 * w, h);
+    default: return 0;
+  }
+}
+
+// An ht_yuv_image checked and resolved into r: pitches resolved, each channel's first sample, steps and shifts (NV12's
+// V at U + 1).  -> HT_OK, or the error code with the reason in why[256].
 static int yuv_record(const ht_yuv_image &v, YuvFeedRec &r, char *why) {
-  if (v.format != HT_YUV_NV12 && v.format != HT_YUV_I420)
-    return snprintf(why, 256, "format %d is neither HT_YUV_NV12 nor HT_YUV_I420", v.format), HT_ERR_ARG;
-  if (v.color < 0 || v.color > (HT_YUV_BT709 | HT_YUV_FULL_RANGE))
-    return snprintf(why, 256, "color %d is not HT_YUV_BT601 or HT_YUV_BT709 [| HT_YUV_FULL_RANGE]", v.color), HT_ERR_ARG;
+  int tight[3], rows[3];
+  const int planes = yuv_planes(v.format, v.width > 0 ? v.width : 1, v.height > 0 ? v.height : 1, tight, rows);
+  if (!planes) return snprintf(why, 256, "format %d is not an HT_YUV_ format", v.format), HT_ERR_ARG;
+  const bool rgb = v.format >= HT_YUV_BGRA;
+  const int c = v.color;
+  const bool yuv_color = c >= 0 && (c & ~(HT_YUV_BT709 | HT_YUV_FULL_RANGE | HT_YUV_BT2020)) == 0 &&
+                         (c & (HT_YUV_BT709 | HT_YUV_BT2020)) != (HT_YUV_BT709 | HT_YUV_BT2020);
+  if (rgb ? c != 0 : !yuv_color)
+    return snprintf(why, 256, rgb ? "color %d: the packed RGB formats take color 0"
+                                  : "color %d is not HT_YUV_BT601, HT_YUV_BT709 or HT_YUV_BT2020 [| HT_YUV_FULL_RANGE]", c),
+           HT_ERR_ARG;
   if (v.width <= 0 || v.height <= 0 || v.width > 16384 || v.height > 16384)
     return snprintf(why, 256, "video %dx%d outside 1..16384", v.width, v.height), HT_ERR_SIZE;
-  const bool nv12 = v.format == HT_YUV_NV12;
-  const int planes = nv12 ? 2 : 3, cw = (v.width + 1) / 2;
-  const int tight[3] = {v.width, nv12 ? 2 * cw : cw, cw};
+  const bool p010 = v.format == HT_YUV_P010;
   int pitch[3] = {0, 0, 0};
   for (int p = 0; p < planes; ++p) {
     if (!v.planes[p]) return snprintf(why, 256, "planes[%d] is NULL", p), HT_ERR_ARG;
     pitch[p] = v.pitch[p] ? v.pitch[p] : tight[p];
     if (pitch[p] < tight[p]) return snprintf(why, 256, "pitch[%d] = %d is below %d", p, v.pitch[p], tight[p]), HT_ERR_ARG;
+    if (p010 && ((reinterpret_cast<uintptr_t>(v.planes[p]) | (uintptr_t)pitch[p]) & 1u))
+      return snprintf(why, 256, "planes[%d] or pitch[%d] is odd: P010 samples are 2 bytes", p, p), HT_ERR_ARG;
   }
-  if (nv12 && v.planes[2]) return snprintf(why, 256, "planes[2] must be NULL for NV12"), HT_ERR_ARG;
-  r = YuvFeedRec{v.planes[0], v.planes[1], nv12 ? v.planes[1] + 1 : v.planes[2], pitch[0], pitch[1], nv12 ? pitch[1] : pitch[2],
-                 v.width, v.height, nv12 ? 2 : 1, v.color, 0};
+  for (int p = planes; p < 3; ++p)
+    if (v.planes[p]) return snprintf(why, 256, "planes[%d] must be NULL for format %d", p, v.format), HT_ERR_ARG;
+  const uint8_t *P0 = v.planes[0], *P1 = v.planes[1];
+  // channel pointers, pitches, cstep, ystep, sx, sy, sample bytes, rgb, alpha
+  auto set = [&](const uint8_t *y, const uint8_t *u, const uint8_t *w, int yp, int up, int vp, int cstep, int ystep,
+                 int sx, int sy) {
+    r = YuvFeedRec{y, u, w, yp, up, vp, v.width, v.height, cstep, v.color, (uint8_t)v.format, (uint8_t)ystep,
+                   (uint8_t)sx, (uint8_t)sy, (uint8_t)(p010 ? 2 : 1), (uint8_t)rgb, (uint8_t)(v.format == HT_YUV_BGRA), 0};
+  };
+  switch (v.format) {
+    case HT_YUV_NV12: set(P0, P1, P1 + 1, pitch[0], pitch[1], pitch[1], 2, 1, 1, 1); break;
+    case HT_YUV_NV21: set(P0, P1 + 1, P1, pitch[0], pitch[1], pitch[1], 2, 1, 1, 1); break;
+    case HT_YUV_I420: set(P0, P1, v.planes[2], pitch[0], pitch[1], pitch[2], 1, 1, 1, 1); break;
+    case HT_YUV_I422: set(P0, P1, v.planes[2], pitch[0], pitch[1], pitch[2], 1, 1, 1, 0); break;
+    case HT_YUV_I444: set(P0, P1, v.planes[2], pitch[0], pitch[1], pitch[2], 1, 1, 0, 0); break;
+    case HT_YUV_YUYV: set(P0, P0 + 1, P0 + 3, pitch[0], pitch[0], pitch[0], 4, 2, 1, 0); break;
+    case HT_YUV_UYVY: set(P0 + 1, P0, P0 + 2, pitch[0], pitch[0], pitch[0], 4, 2, 1, 0); break;
+    case HT_YUV_P010: set(P0, P1, P1 + 2, pitch[0], pitch[1], pitch[1], 4, 2, 1, 1); break;
+    case HT_YUV_BGRA: set(P0 + 2, P0 + 1, P0, pitch[0], pitch[0], pitch[0], 4, 4, 0, 0); break;
+    case HT_YUV_BGR24: set(P0 + 2, P0 + 1, P0, pitch[0], pitch[0], pitch[0], 3, 3, 0, 0); break;
+    default: set(P0, P0 + 1, P0 + 2, pitch[0], pitch[0], pitch[0], 3, 3, 0, 0); break;       // RGB24
+  }
   return HT_OK;
 }
 static int check_yuv_record(ht_ctx *ctx, const ht_yuv_image &v, int b, YuvFeedRec &r) {
@@ -2232,33 +2279,29 @@ static int check_yuv_record(ht_ctx *ctx, const ht_yuv_image &v, int b, YuvFeedRe
 
 // bytes of r's planes packed at tight pitches, each plane 256-byte aligned
 static size_t yuv_staged_bytes(const YuvFeedRec &r) {
-  const size_t cw = (size_t)(r.width + 1) / 2, ch = (size_t)(r.height + 1) / 2;
-  const size_t luma = align_up<size_t>((size_t)r.width * r.height, 256);
-  return r.cstep == 2 ? luma + align_up<size_t>(2 * cw * ch, 256) : luma + 2 * align_up<size_t>(cw * ch, 256);
+  int tight[3], rows[3];
+  const int planes = yuv_planes(r.format, r.width, r.height, tight, rows);
+  size_t bytes = 0;
+  for (int p = 0; p < planes; ++p) bytes += align_up<size_t>((size_t)tight[p] * rows[p], 256);
+  return bytes;
 }
 
-// r's host planes go up plane by plane to dst (yuv_staged_bytes of device memory), on the context's stream; r then
-// describes the packed copy
-static int stage_yuv(ht_ctx *ctx, YuvFeedRec &r, uint8_t *dst) {
-  const size_t w = (size_t)r.width, h = (size_t)r.height, cw = (w + 1) / 2, ch = (h + 1) / 2;
-  const size_t luma = align_up<size_t>(w * h, 256);
-  CK(cudaMemcpy2DAsync(dst, w, r.y, (size_t)r.ypitch, w, h, cudaMemcpyHostToDevice, ctx->stream));
-  r.y = dst;
-  r.ypitch = (int32_t)w;
-  if (r.cstep == 2) {
-    CK(cudaMemcpy2DAsync(dst + luma, 2 * cw, r.u, (size_t)r.upitch, 2 * cw, ch, cudaMemcpyHostToDevice, ctx->stream));
-    r.u = dst + luma;
-    r.v = r.u + 1;
-    r.upitch = r.vpitch = (int32_t)(2 * cw);
-  } else {
-    const size_t cb = align_up<size_t>(cw * ch, 256);
-    CK(cudaMemcpy2DAsync(dst + luma, cw, r.u, (size_t)r.upitch, cw, ch, cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaMemcpy2DAsync(dst + luma + cb, cw, r.v, (size_t)r.vpitch, cw, ch, cudaMemcpyHostToDevice, ctx->stream));
-    r.u = dst + luma;
-    r.v = dst + luma + cb;
-    r.upitch = r.vpitch = (int32_t)cw;
+// the host planes of v (checked by yuv_record into r) go up plane by plane to dst (yuv_staged_bytes of device memory),
+// on the context's stream; r then describes the packed copy
+static int stage_yuv(ht_ctx *ctx, const ht_yuv_image &v, YuvFeedRec &r, uint8_t *dst) {
+  int tight[3], rows[3];
+  const int planes = yuv_planes(v.format, v.width, v.height, tight, rows);
+  ht_yuv_image staged = v;
+  for (int p = 0; p < planes; ++p) {
+    const size_t pitch = v.pitch[p] ? (size_t)v.pitch[p] : (size_t)tight[p];
+    CK(cudaMemcpy2DAsync(dst, (size_t)tight[p], v.planes[p], pitch, (size_t)tight[p], (size_t)rows[p], cudaMemcpyHostToDevice,
+                         ctx->stream));
+    staged.planes[p] = dst;
+    staged.pitch[p] = tight[p];
+    dst += align_up<size_t>((size_t)tight[p] * rows[p], 256);
   }
-  return HT_OK;
+  char why[256];
+  return yuv_record(staged, r, why);
 }
 
 // ht_tracker_feed(_canvases).  Everything is checked before anything is enqueued (one_canvas: every record is on the
@@ -2417,7 +2460,7 @@ static int tracker_feed(ht_ctx *ctx, const ht_canvas_frame *frames, const ht_yuv
       now[e] = yuv[b].now_ms;
       YuvFeedRec r = yrec[(size_t)b];
       if (!frames_on_device) {
-        const int rc = stage_yuv(ctx, r, ctx->d_frames.as<uint8_t>() + voff);
+        const int rc = stage_yuv(ctx, yuv[b].video, r, ctx->d_frames.as<uint8_t>() + voff);
         if (rc != HT_OK) return rc;
         voff += yuv_staged_bytes(r);
       }
@@ -2535,8 +2578,9 @@ int ht_ingest_yuv(ht_ctx *ctx, const ht_yuv_image *src, int n, int frames_on_dev
   if (!frames_on_device) {
     CK(ctx->d_frames.reserve(video_bytes));
     size_t voff = 0;
-    for (YuvFeedRec &r : recs) {
-      const int rc = stage_yuv(ctx, r, ctx->d_frames.as<uint8_t>() + voff);
+    for (int b = 0; b < n; ++b) {
+      YuvFeedRec &r = recs[(size_t)b];
+      const int rc = stage_yuv(ctx, src[b], r, ctx->d_frames.as<uint8_t>() + voff);
       if (rc != HT_OK) return rc;
       voff += yuv_staged_bytes(r);
     }
@@ -2924,9 +2968,9 @@ extern "C" int ht_selftest_debug_write(const uint16_t *bins, int w, int h, const
   return stores;
 }
 
-// k_feed_draw_yuv's per-record code: one YUV image (host planes) onto a dw x dh canvas, 1:1 draws whose width is a
-// multiple of 4 through yuv_quad as the kernel takes them (the canvas is taken to be 16-byte aligned), every other draw
-// pixel by pixel.  -> 0, or the ht_ingest_yuv error code for a bad record.
+// k_feed_draw_yuv's per-record code: one image of any format (host planes) onto a dw x dh canvas, 1:1 draws whose width
+// is a multiple of 4 through yuv_quad / fmt_quad as the kernel takes them (the canvas is taken to be 16-byte aligned),
+// every other draw pixel by pixel.  -> 0, or the ht_ingest_yuv error code for a bad record.
 extern "C" int ht_selftest_feed_yuv(const ht_yuv_image *img, uint8_t *canvas, int dw, int dh) {
   YuvFeedRec r;
   char why[256];
@@ -2935,11 +2979,13 @@ extern "C" int ht_selftest_feed_yuv(const ht_yuv_image *img, uint8_t *canvas, in
   IngestGeom g;
   if (!canvas_geom(dw, dh, g)) return HT_ERR_SIZE;
   const bool quads = r.width == dw && r.height == dh && (dw & 3) == 0;
+  const bool nv12_i420 = nv12_i420_path(r);
   for (int Y = 0; Y < dh; ++Y) {
     if (quads) {
-      for (int X = 0; X < dw; X += 4) reinterpret_cast<uint4 *>(canvas + (size_t)Y * dw * 4)[X >> 2] = yuv_quad(r, X, Y);
+      for (int X = 0; X < dw; X += 4)
+        reinterpret_cast<uint4 *>(canvas + (size_t)Y * dw * 4)[X >> 2] = nv12_i420 ? yuv_quad(r, X, Y) : fmt_quad(r, X, Y);
     } else {
-      for (int X = 0; X < dw; ++X) feed_yuv_pixel(r, canvas, g, X, Y);
+      for (int X = 0; X < dw; ++X) nv12_i420 ? feed_yuv_pixel(r, canvas, g, X, Y) : feed_fmt_pixel(r, canvas, g, X, Y);
     }
   }
   return 0;

@@ -220,36 +220,55 @@ __host__ __device__ __forceinline__ uint32_t draw_pixel(const uint32_t *__restri
 // becomes RGBA8 in integers only - C = Y - y0, D = U - 128, E = V - 128, R = clamp((cy C + rv E + 128) >> 8),
 // G = clamp((cy C - gu D - gv E + 128) >> 8), B = clamp((cy C + bu D + 128) >> 8), A = 255 - with each coefficient
 // round(256 x the real one).  Every row is within 1 level of the real-valued conversion rounded half up, over all
-// 2^24 triples (tests/test_yuv_host.py).  color: HT_YUV_BT601 / HT_YUV_BT709, optionally | HT_YUV_FULL_RANGE.
+// 2^24 triples (tests/test_yuv_host.py, tests/test_formats_host.py).  color: HT_YUV_BT601 / HT_YUV_BT709 /
+// HT_YUV_BT2020 (non-constant luminance), optionally | HT_YUV_FULL_RANGE.
 //                          y0   cy   rv   gu   gv   bu
 //   BT.601 limited range   16  298  409  100  208  516
 //   BT.709 limited range   16  298  459   55  136  541
+//   BT.2020 limited range  16  298  430   48  167  548
 //   BT.601 full range       0  256  359   88  183  454
 //   BT.709 full range       0  256  403   48  120  475
-// |cy C| + |rv E| etc. stay below 2^18: int32 throughout.
+//   BT.2020 full range      0  256  377   42  146  482
+// |cy C| + |rv E| etc. stay below 2^18: int32 throughout.  BT2020 = false: the BT.601 / BT.709 rows only (the NV12 /
+// I420 code of k_feed_draw_yuv, whose records with a BT.2020 colour take the other formats' path).
+template <bool BT2020 = true>
 __host__ __device__ __forceinline__ uint32_t yuv_to_rgba(int color, uint32_t Y, uint32_t U, uint32_t V) {
-  const bool bt709 = (color & HT_YUV_BT709) != 0, full = (color & HT_YUV_FULL_RANGE) != 0;
+  const bool bt709 = (color & HT_YUV_BT709) != 0, bt2020 = BT2020 && (color & HT_YUV_BT2020) != 0;
+  const bool full = (color & HT_YUV_FULL_RANGE) != 0;
   const int y0 = full ? 0 : 16, cy = full ? 256 : 298;
-  const int rv = full ? (bt709 ? 403 : 359) : (bt709 ? 459 : 409);
-  const int gu = full ? (bt709 ? 48 : 88) : (bt709 ? 55 : 100);
-  const int gv = full ? (bt709 ? 120 : 183) : (bt709 ? 136 : 208);
-  const int bu = full ? (bt709 ? 475 : 454) : (bt709 ? 541 : 516);
+  const int rv = full ? (bt2020 ? 377 : bt709 ? 403 : 359) : (bt2020 ? 430 : bt709 ? 459 : 409);
+  const int gu = full ? (bt2020 ? 42 : bt709 ? 48 : 88) : (bt2020 ? 48 : bt709 ? 55 : 100);
+  const int gv = full ? (bt2020 ? 146 : bt709 ? 120 : 183) : (bt2020 ? 167 : bt709 ? 136 : 208);
+  const int bu = full ? (bt2020 ? 482 : bt709 ? 475 : 454) : (bt2020 ? 548 : bt709 ? 541 : 516);
   const int c = cy * ((int)Y - y0), d = (int)U - 128, e = (int)V - 128;
   const int r = (c + rv * e + 128) >> 8, gr = (c - gu * d - gv * e + 128) >> 8, b = (c + bu * d + 128) >> 8;
   auto clamp255 = [](int v) { return (uint32_t)(v < 0 ? 0 : (v > 255 ? 255 : v)); };
   return clamp255(r) | clamp255(gr) << 8 | clamp255(b) << 16 | 0xff000000u;
 }
-// ht_tracker_feed_yuv / ht_ingest_yuv: one YUV 4:2:0 video frame, pitches resolved.  Chroma sample (cx, cy) is
-// u[cy * upitch + cx * cstep] and v[cy * vpitch + cx * cstep]: NV12 is v = u + 1 with cstep 2 (one interleaved plane),
-// I420 two planes with cstep 1, so both layouts are one code path.
+// ht_tracker_feed_yuv / ht_ingest_yuv: one video frame of any ht_yuv_image format, pitches resolved.  Channel 0 (Y, or
+// R of a packed RGB format) of pixel (x, y) is the sample at y[y * ypitch + x * ystep]; channels 1 and 2 (U and V, or
+// G and B) are at u[(y >> sy) * upitch + (x >> sx) * cstep] and v[(y >> sy) * vpitch + (x >> sx) * cstep].  NV12 is
+// v = u + 1 with cstep 2 (one interleaved plane), I420 two planes with cstep 1, so both are one code path (yuv_texel);
+// every other format is fmt_texel's.  A sample is one byte, or (P010, sample_bytes 2) a 16-bit little-endian word.
 struct YuvFeedRec {
   const uint8_t *y, *u, *v;
   int32_t ypitch, upitch, vpitch;   // bytes
   int32_t width, height;
   int32_t cstep;                    // bytes between horizontally adjacent chroma samples
   int32_t color;                    // ht_yuv_image.color
-  int32_t pad_;
+  uint8_t format;                   // ht_yuv_image.format
+  uint8_t ystep;                    // bytes between horizontally adjacent luma samples
+  uint8_t sx, sy;                   // chroma shifts
+  uint8_t sample_bytes;             // 1, or 2 for P010
+  uint8_t rgb;                      // the channels are R, G, B (no matrix)
+  uint8_t alpha;                    // BGRA: A is the byte 3 after channel 2's (B's) sample; otherwise A = 255
+  uint8_t pad_;
 };
+// whether record r is drawn by the NV12 / I420 code (yuv_texel, yuv_quad): NV12 and I420 in BT.601 or BT.709; every
+// other record, BT.2020 NV12 / I420 included, by fmt_texel and fmt_quad
+__host__ __device__ __forceinline__ bool nv12_i420_path(const YuvFeedRec &r) {
+  return (r.format == HT_YUV_NV12 || r.format == HT_YUV_I420) && (r.color & HT_YUV_BT2020) == 0;
+}
 // RGBA8 pixel (x, y) of the converted video; an NV12 (U, V) pair at an even address is one 2-byte load
 __host__ __device__ __forceinline__ uint32_t yuv_texel(const YuvFeedRec &r, int x, int y) {
   const size_t c = (size_t)(x >> 1) * r.cstep;
@@ -261,7 +280,7 @@ __host__ __device__ __forceinline__ uint32_t yuv_texel(const YuvFeedRec &r, int 
   } else {
     U = ld_ro(up), V = ld_ro(r.v + (size_t)(y >> 1) * r.vpitch + c);
   }
-  return yuv_to_rgba(r.color, ld_ro(r.y + (size_t)y * r.ypitch + x), U, V);
+  return yuv_to_rgba<false>(r.color, ld_ro(r.y + (size_t)y * r.ypitch + x), U, V);
 }
 // canvas pixel (X, Y) of YUV record r onto a canvas of g: drawing the converted video, four converted taps per pixel
 // (a 1:1 draw is the conversion alone); also run on the host by ht_selftest_feed_yuv
@@ -270,6 +289,35 @@ __host__ __device__ __forceinline__ void feed_yuv_pixel(const YuvFeedRec &r, uin
   const uint32_t out = (r.width == g.dw && r.height == g.dh)
                            ? yuv_texel(r, X, Y)
                            : bilinear_pixel([&](int x, int y) { return yuv_texel(r, x, y); }, r.width, r.height, g, X, Y);
+  reinterpret_cast<uint32_t *>(canvas)[(size_t)Y * g.dw + X] = out;
+}
+// a P010 sample reduced to 8 bits on its whole 16-bit word: 10-bit 64 -> 16, 940 -> 235, 512 -> 128 (v << 6)
+__host__ __device__ __forceinline__ uint32_t p010_reduce(uint32_t s) {
+  const uint32_t v = (s + 128u) >> 8;
+  return v < 255u ? v : 255u;
+}
+// one 8-bit sample at p: a byte, or (wide) a 2-byte-aligned 16-bit little-endian word reduced by p010_reduce
+__host__ __device__ __forceinline__ uint32_t fmt_sample(const uint8_t *p, bool wide) {
+  return wide ? p010_reduce(ld_ro(reinterpret_cast<const uint16_t *>(p))) : (uint32_t)ld_ro(p);
+}
+// RGBA8 pixel (x, y) of any record (nv12_i420_path: the others): the samples of its three channels, then yuv_to_rgba, or (packed
+// RGB) the channels as they are
+__host__ __device__ __forceinline__ uint32_t fmt_texel(const YuvFeedRec &r, int x, int y) {
+  const bool wide = r.sample_bytes == 2;
+  const size_t cx = (size_t)(x >> r.sx) * r.cstep, cy = (size_t)(y >> r.sy);
+  const uint32_t c0 = fmt_sample(r.y + (size_t)y * r.ypitch + (size_t)x * r.ystep, wide);
+  const uint32_t c1 = fmt_sample(r.u + cy * r.upitch + cx, wide);
+  const uint32_t c2 = fmt_sample(r.v + cy * r.vpitch + cx, wide);
+  if (!r.rgb) return yuv_to_rgba(r.color, c0, c1, c2);
+  const uint32_t a = r.alpha ? (uint32_t)ld_ro(r.v + cy * r.vpitch + cx + 3) : 255u;
+  return c0 | c1 << 8 | c2 << 16 | a << 24;
+}
+// feed_yuv_pixel for the formats of fmt_texel
+__host__ __device__ __forceinline__ void feed_fmt_pixel(const YuvFeedRec &r, uint8_t *__restrict__ canvas, const IngestGeom &g,
+                                                        int X, int Y) {
+  const uint32_t out = (r.width == g.dw && r.height == g.dh)
+                           ? fmt_texel(r, X, Y)
+                           : bilinear_pixel([&](int x, int y) { return fmt_texel(r, x, y); }, r.width, r.height, g, X, Y);
   reinterpret_cast<uint32_t *>(canvas)[(size_t)Y * g.dw + X] = out;
 }
 // one destination pixel (also run on the host by tests/test_ingest_host.py)
@@ -398,13 +446,131 @@ __host__ __device__ __forceinline__ uint4 yuv_quad(const YuvFeedRec &r, int X, i
   } else {
     u0 = ld_ro(up), u1 = ld_ro(up + r.cstep), v0 = ld_ro(vp), v1 = ld_ro(vp + r.cstep);
   }
-  return make_uint4(yuv_to_rgba(r.color, ys & 0xffu, u0, v0), yuv_to_rgba(r.color, (ys >> 8) & 0xffu, u0, v0),
-                    yuv_to_rgba(r.color, (ys >> 16) & 0xffu, u1, v1), yuv_to_rgba(r.color, ys >> 24, u1, v1));
+  return make_uint4(yuv_to_rgba<false>(r.color, ys & 0xffu, u0, v0), yuv_to_rgba<false>(r.color, (ys >> 8) & 0xffu, u0, v0),
+                    yuv_to_rgba<false>(r.color, (ys >> 16) & 0xffu, u1, v1), yuv_to_rgba<false>(r.color, ys >> 24, u1, v1));
+}
+// byte k of little-endian word w; whether p is a multiple of a (a power of 2); the little-endian word at p, one load
+// where p is 4-byte aligned
+__host__ __device__ __forceinline__ uint32_t byte_of(uint32_t w, int k) { return (w >> (8 * k)) & 0xffu; }
+__host__ __device__ __forceinline__ bool aligned_to(const uint8_t *p, unsigned a) {
+  return (reinterpret_cast<uintptr_t>(p) & (a - 1u)) == 0;
+}
+__host__ __device__ __forceinline__ uint32_t ld_word(const uint8_t *p) {
+  if (aligned_to(p, 4)) return ld_ro(reinterpret_cast<const uint32_t *>(p));
+  return (uint32_t)ld_ro(p) | (uint32_t)ld_ro(p + 1) << 8 | (uint32_t)ld_ro(p + 2) << 16 | (uint32_t)ld_ro(p + 3) << 24;
+}
+// yuv_quad for the formats of fmt_texel.  Wide loads where the layout and alignment allow: an 8-byte YUYV / UYVY group,
+// 12 bytes of BGR24 / RGB24 as three words, 16 bytes of BGRA, 4 bytes of 8-bit luma or I444 chroma, 8 bytes of P010
+// luma, 4 bytes of NV21 chroma (V0 U0 V1 U1) and 8 of P010 chroma (U0 V0 U1 V1); narrower loads otherwise.  Also run on
+// the host by ht_selftest_feed_yuv.
+__host__ __device__ __forceinline__ uint4 fmt_quad(const YuvFeedRec &r, int X, int Y) {
+  const uint8_t *row = r.y + (size_t)Y * r.ypitch + (size_t)X * r.ystep;            // channel 0 of pixel X
+  if (r.format == HT_YUV_YUYV || r.format == HT_YUV_UYVY) {
+    const uint8_t *p = r.format == HT_YUV_YUYV ? row : row - 1;                       // the first byte of the group
+    uint2 w;
+    if (aligned_to(p, 8)) {
+      w = ld_ro(reinterpret_cast<const uint2 *>(p));
+    } else {
+      w.x = ld_word(p), w.y = ld_word(p + 4);
+    }
+    if (r.format == HT_YUV_UYVY) {                                                    // U Y V Y -> Y U Y V
+      w.x = ((w.x >> 8) & 0x00ff00ffu) | ((w.x & 0x00ff00ffu) << 8);
+      w.y = ((w.y >> 8) & 0x00ff00ffu) | ((w.y & 0x00ff00ffu) << 8);
+    }
+    const uint32_t u0 = byte_of(w.x, 1), v0 = byte_of(w.x, 3), u1 = byte_of(w.y, 1), v1 = byte_of(w.y, 3);
+    return make_uint4(yuv_to_rgba(r.color, byte_of(w.x, 0), u0, v0), yuv_to_rgba(r.color, byte_of(w.x, 2), u0, v0),
+                      yuv_to_rgba(r.color, byte_of(w.y, 0), u1, v1), yuv_to_rgba(r.color, byte_of(w.y, 2), u1, v1));
+  }
+  if (r.rgb) {
+    // the first byte of pixel X: R's for RGB24, B's for BGR24 and BGRA
+    const uint8_t *p = r.format == HT_YUV_RGB24 ? row : r.v + (size_t)Y * r.vpitch + (size_t)X * r.cstep;
+    if (r.alpha) {                                                                    // B G R A -> R G B A
+      uint4 w;
+      if (aligned_to(p, 16)) {
+        w = ld_ro(reinterpret_cast<const uint4 *>(p));
+      } else {
+        w.x = ld_word(p), w.y = ld_word(p + 4), w.z = ld_word(p + 8), w.w = ld_word(p + 12);
+      }
+      w.x = (w.x & 0xff00ff00u) | ((w.x >> 16) & 0xffu) | ((w.x & 0xffu) << 16);
+      w.y = (w.y & 0xff00ff00u) | ((w.y >> 16) & 0xffu) | ((w.y & 0xffu) << 16);
+      w.z = (w.z & 0xff00ff00u) | ((w.z >> 16) & 0xffu) | ((w.z & 0xffu) << 16);
+      w.w = (w.w & 0xff00ff00u) | ((w.w >> 16) & 0xffu) | ((w.w & 0xffu) << 16);
+      return w;
+    }
+    const uint32_t w0 = ld_word(p), w1 = ld_word(p + 4), w2 = ld_word(p + 8);
+    // bytes: w0 = a0 b0 c0 a1, w1 = b1 c1 a2 b2, w2 = c2 a3 b3 c3 with (a, b, c) = (R, G, B) or (B, G, R)
+    uint4 o = make_uint4(w0 & 0xffffffu, (w0 >> 24) | (w1 & 0xffffu) << 8, (w1 >> 16) | (w2 & 0xffu) << 16, w2 >> 8);
+    if (r.format != HT_YUV_RGB24) {                                                   // B G R -> R G B
+      o.x = (o.x & 0xff00u) | (o.x >> 16) | ((o.x & 0xffu) << 16);
+      o.y = (o.y & 0xff00u) | (o.y >> 16) | ((o.y & 0xffu) << 16);
+      o.z = (o.z & 0xff00u) | (o.z >> 16) | ((o.z & 0xffu) << 16);
+      o.w = (o.w & 0xff00u) | (o.w >> 16) | ((o.w & 0xffu) << 16);
+    }
+    o.x |= 0xff000000u, o.y |= 0xff000000u, o.z |= 0xff000000u, o.w |= 0xff000000u;
+    return o;
+  }
+  const bool wide = r.sample_bytes == 2;                                              // NV21, I422, I444, P010
+  uint32_t l[4];
+  if (!wide) {
+    const uint32_t w = ld_word(row);
+    l[0] = byte_of(w, 0), l[1] = byte_of(w, 1), l[2] = byte_of(w, 2), l[3] = byte_of(w, 3);
+  } else if (aligned_to(row, 8)) {
+    const uint2 w = ld_ro(reinterpret_cast<const uint2 *>(row));
+    l[0] = p010_reduce(w.x & 0xffffu), l[1] = p010_reduce(w.x >> 16);
+    l[2] = p010_reduce(w.y & 0xffffu), l[3] = p010_reduce(w.y >> 16);
+  } else {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) l[i] = fmt_sample(row + 2 * i, true);
+  }
+  const uint8_t *up = r.u + (size_t)(Y >> r.sy) * r.upitch + (size_t)(X >> r.sx) * r.cstep;
+  const uint8_t *vp = r.v + (size_t)(Y >> r.sy) * r.vpitch + (size_t)(X >> r.sx) * r.cstep;
+  uint32_t u[4], v[4];
+  if (r.sx) {                                                                         // two chroma samples
+    uint32_t u0, v0, u1, v1;
+    if (r.format == HT_YUV_NV21 && aligned_to(vp, 4)) {
+      const uint32_t w = ld_ro(reinterpret_cast<const uint32_t *>(vp));
+      v0 = byte_of(w, 0), u0 = byte_of(w, 1), v1 = byte_of(w, 2), u1 = byte_of(w, 3);
+    } else if (wide && aligned_to(up, 8)) {
+      const uint2 w = ld_ro(reinterpret_cast<const uint2 *>(up));
+      u0 = p010_reduce(w.x & 0xffffu), v0 = p010_reduce(w.x >> 16);
+      u1 = p010_reduce(w.y & 0xffffu), v1 = p010_reduce(w.y >> 16);
+    } else {
+      u0 = fmt_sample(up, wide), u1 = fmt_sample(up + r.cstep, wide);
+      v0 = fmt_sample(vp, wide), v1 = fmt_sample(vp + r.cstep, wide);
+    }
+    u[0] = u[1] = u0, u[2] = u[3] = u1, v[0] = v[1] = v0, v[2] = v[3] = v1;
+  } else {                                                                            // I444
+    const uint32_t wu = ld_word(up), wv = ld_word(vp);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) u[i] = byte_of(wu, i), v[i] = byte_of(wv, i);
+  }
+  return make_uint4(yuv_to_rgba(r.color, l[0], u[0], v[0]), yuv_to_rgba(r.color, l[1], u[1], v[1]),
+                    yuv_to_rgba(r.color, l[2], u[2], v[2]), yuv_to_rgba(r.color, l[3], u[3], v[3]));
+}
+// k_feed_draw_yuv's CTA for a record off nv12_i420_path, rows Y0..Y0+15 from column X0 of canvas cv (g): the same
+// thread layout as the NV12 / I420 code.  Out of line, so that its registers are its own: the NV12 / I420 code of the
+// kernel is compiled as it was without the other formats.
+__device__ __noinline__ void feed_draw_fmt(const YuvFeedRec *__restrict__ rp, uint8_t *__restrict__ cv, const IngestGeom g,
+                                           int X0, int Y0) {
+  const YuvFeedRec r = *rp;
+  if (r.width == g.dw && r.height == g.dh && (g.dw & 3) == 0 && (reinterpret_cast<uintptr_t>(cv) & 15u) == 0) {
+    const int X = X0 + 4 * (threadIdx.x & 15), Y = Y0 + (threadIdx.x >> 4);
+    if (X >= g.dw || Y >= g.dh) return;
+    reinterpret_cast<uint4 *>(cv + (size_t)Y * g.dw * 4)[X >> 2] = fmt_quad(r, X, Y);
+    return;
+  }
+  const int X = X0 + (threadIdx.x & 63);
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int Y = Y0 + 4 * i + (threadIdx.x >> 6);
+    if (X < g.dw && Y < g.dh) feed_fmt_pixel(r, cv, g, X, Y);
+  }
 }
 // k_feed_draw for YUV records (ht_tracker_feed_yuv; ht_ingest_yuv with draw == NULL: every record), the same tiles and
 // grid.  The planes are read directly: no RGBA frame is written.  A 1:1 record on a canvas whose width is a multiple of
-// 4 converts 4 pixels per thread (yuv_quad) and stores them in 16 bytes; the two luma rows of a chroma row are
-// neighbouring threads' and read it from L1.
+// 4 converts 4 pixels per thread (yuv_quad, fmt_quad) and stores them in 16 bytes; the two luma rows of a chroma row
+// are neighbouring threads' and read it from L1.  A CTA draws one record, so the choice between the NV12 / I420 code
+// (here) and every other record (feed_draw_fmt) is uniform across it.
 __global__ void __launch_bounds__(256) k_feed_draw_yuv(const YuvFeedRec *__restrict__ recs, const uint8_t *__restrict__ draw,
                                                        uint8_t *__restrict__ canvas, IngestGeom g, int tiles_x,
                                                        const EntryCanvas *__restrict__ geo,
@@ -415,6 +581,10 @@ __global__ void __launch_bounds__(256) k_feed_draw_yuv(const YuvFeedRec *__restr
   const YuvFeedRec r = recs[b];
   if (draw && !draw[b]) return;
   const int X0 = (tile % tiles_x) * 64, Y0 = (tile / tiles_x) * 16;
+  if (!nv12_i420_path(r)) {
+    feed_draw_fmt(recs + b, cv, g, X0, Y0);
+    return;
+  }
   if (r.width == g.dw && r.height == g.dh && (g.dw & 3) == 0 && (reinterpret_cast<uintptr_t>(cv) & 15u) == 0) {
     const int X = X0 + 4 * (threadIdx.x & 15), Y = Y0 + (threadIdx.x >> 4);
     if (X >= g.dw || Y >= g.dh) return;

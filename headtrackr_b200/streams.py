@@ -226,7 +226,7 @@ class TrackerSet:
         return self._feed(frames, now_ms, width, height, self.ctx.tracker_feed)
 
     def feed_yuv(self, frames, now_ms=None, width=None, height=None, format="nv12", color="bt601"):
-        """feed on YUV 4:2:0 video (ht_tracker_feed_yuv): frames = {stream: (Y, UV) NV12 or (Y, U, V) I420 planes}
+        """feed on video in any of _lib.YUV_FORMATS (ht_tracker_feed_yuv): frames = {stream: planes or packed array}
         (Context.tracker_feed_yuv), format and color one for all or {stream: value}; the rest as for feed, and events
         are dispatched as feed dispatches them."""
         ks = list(frames)

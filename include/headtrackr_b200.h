@@ -313,23 +313,48 @@ typedef struct {
 int ht_tracker_feed_canvases(ht_ctx *ctx, const ht_canvas_frame *frames, int n, int frames_on_device,
                              ht_tracker_event *out);
 
-/* YUV 4:2:0 video, as decoders write it: NV12 (hardware decoders), I420 (software decoders, JPEG decoders' 4:2:0
- * output).  The frame is drawn as the RGBA8 frame this library's conversion makes of it (DESIGN.md 2, "YUV video"):
- * luma pixel (x, y) takes chroma sample (x >> 1, y >> 1), then an integer BT.601 or BT.709 matrix, limited or full
- * range, A = 255.  Byte offsets:
- *     0  const uint8_t *planes[3]   NV12: Y, interleaved UV (U first), NULL.  I420: Y, U, V
- *    24  int32 pitch[3]             bytes per row; 0 -> the tight pitch: width for Y, 2*ceil(width/2) for the NV12 UV
- *                                   plane, ceil(width/2) for I420 U and V; otherwise >= that, any alignment (unused
- *                                   for a NULL plane)
- *    36  int32 width, height        luma size, 1..16384; the chroma planes are ceil(width/2) x ceil(height/2) samples
- *    44  int32 format               HT_YUV_NV12 or HT_YUV_I420
- *    48  int32 color                HT_YUV_BT601 or HT_YUV_BT709, optionally | HT_YUV_FULL_RANGE
- *    52  int32 pad_ */
+/* Video as decoders, cameras and capture APIs write it.  The frame is drawn as the RGBA8 frame this library's
+ * conversion makes of it (DESIGN.md 2, "YUV video"): luma pixel (x, y) takes chroma sample (x >> sx, y >> sy) of its
+ * format, then an integer BT.601, BT.709 or BT.2020 matrix, limited or full range, A = 255; the packed RGB formats are
+ * taken as they are.  Byte offsets:
+ *     0  const uint8_t *planes[3]   per format, below; a plane the format does not use must be NULL
+ *    24  int32 pitch[3]             bytes per row; 0 -> the tight pitch below; otherwise >= that, any alignment (P010:
+ *                                   even pointers and pitches) (unused for a NULL plane)
+ *    36  int32 width, height        luma size w x h, 1..16384; cw = ceil(w/2), ch = ceil(h/2)
+ *    44  int32 format               one of the HT_YUV_ formats below
+ *    48  int32 color                HT_YUV_BT601, HT_YUV_BT709 or HT_YUV_BT2020, optionally | HT_YUV_FULL_RANGE (not
+ *                                   BT709 | BT2020); 0 for the packed RGB formats
+ *    52  int32 pad_
+ *  format        planes                         tight pitches   luma (x, y)      chroma / colour samples of pixel (x, y)
+ *  NV12  (0)     Y, UV (U first), NULL          w, 2cw          Y[y][x]          U = UV[y>>1][2(x>>1)], V = ... + 1
+ *  I420  (1)     Y, U, V                        w, cw, cw       Y[y][x]          U[y>>1][x>>1], V[y>>1][x>>1]
+ *  NV21  (16)    Y, VU (V first), NULL          w, 2cw          Y[y][x]          V = VU[y>>1][2(x>>1)], U = ... + 1
+ *  I422  (17)    Y, U, V (h chroma rows)        w, cw, cw       Y[y][x]          U[y][x>>1], V[y][x>>1]
+ *  I444  (18)    Y, U, V                        w, w, w         Y[y][x]          U[y][x], V[y][x]
+ *  YUYV  (19)    P, NULL, NULL                  4cw             P[y][2x]         U = P[y][4(x>>1)+1], V = ...+3
+ *  UYVY  (20)    P, NULL, NULL                  4cw             P[y][2x+1]       U = P[y][4(x>>1)],   V = ...+2
+ *  P010  (21)    Y, UV (U first), NULL:         2w, 4cw         r(Y[y][x])       U = r(UV[y>>1][2(x>>1)]),
+ *                16-bit little-endian samples                                    V = r(UV[y>>1][2(x>>1)+1])
+ *  BGRA  (32)    P, NULL, NULL                  4w              -                R, G, B, A = bytes 4x+2, 4x+1, 4x, 4x+3
+ *  BGR24 (33)    P, NULL, NULL                  3w              -                R, G, B = bytes 3x+2, 3x+1, 3x; A = 255
+ *  RGB24 (34)    P, NULL, NULL                  3w              -                R, G, B = bytes 3x, 3x+1, 3x+2; A = 255
+ * P010 samples are reduced to 8 bits, r(s) = min(255, (s + 128) >> 8) of the whole 16-bit word (P016 is valid P010),
+ * and then converted as 8-bit samples: a P010 frame draws exactly like the NV12 frame of its reduced samples. */
 #define HT_YUV_NV12 0
 #define HT_YUV_I420 1
+#define HT_YUV_NV21 16
+#define HT_YUV_I422 17
+#define HT_YUV_I444 18
+#define HT_YUV_YUYV 19
+#define HT_YUV_UYVY 20
+#define HT_YUV_P010 21
+#define HT_YUV_BGRA 32
+#define HT_YUV_BGR24 33
+#define HT_YUV_RGB24 34
 #define HT_YUV_BT601 0
 #define HT_YUV_BT709 1
 #define HT_YUV_FULL_RANGE 2
+#define HT_YUV_BT2020 8
 typedef struct {
   const uint8_t *planes[3];
   int32_t pitch[3];
@@ -354,10 +379,12 @@ typedef struct {
  * canvas and clock, out[n] in record order on the host or the device, an IDLE stream's planes never read.  The
  * streams' state is the one every tick uses: a stream may tick from YUV, RGBA and ht_tracker_step in turn.  Host
  * planes are packed into the library's staging buffer; only the first record's Y pointer is tested against
- * frames_on_device.  Same launches as ht_tracker_feed_canvases on the same canvases.
+ * frames_on_device.  Records may mix every format, colour and canvas size.  Same launches as ht_tracker_feed_canvases
+ * on the same canvases.
  * Errors (nothing is enqueued): those of ht_tracker_feed_canvases, and HT_ERR_ARG, with the record's index in
- * ht_last_error, for a format or color outside the values above, a NULL Y or chroma plane, a non-NULL planes[2] for
- * NV12, or a pitch below the tight pitch; HT_ERR_SIZE for a video size outside 1..16384. */
+ * ht_last_error, for a format outside the values above or a color not valid for it, a NULL plane the format uses, a
+ * non-NULL plane it does not use, a pitch below the tight pitch, or an odd P010 plane pointer or pitch; HT_ERR_SIZE for
+ * a video size outside 1..16384. */
 int ht_tracker_feed_yuv(ht_ctx *ctx, const ht_yuv_frame *frames, int n, int frames_on_device, ht_tracker_event *out);
 /* ht_ingest for YUV video: src[i] (host records; planes all host or all device memory, as frames_on_device says, only
  * src[0]'s Y pointer is tested) drawn onto the i-th tightly packed dw x dh RGBA8 canvas of dst_rgba (host or device

@@ -658,7 +658,9 @@ static napi_value TrackerFeed(napi_env env, napi_callback_info info) {
   return out;
 }
 
-// a YUV frame object {format: "nv12"|"i420", color: "bt601"|"bt709"|"bt601-full"|"bt709-full", width, height, y, uv | u, v}
+// a video frame object {format, color, width, height, planes}: format "nv12" (the default), "i420", "nv21", "i422",
+// "i444", "yuyv", "uyvy", "p010", "bgra", "bgr24" or "rgb24"; color "bt601" (the default), "bt709", "bt2020", each
+// optionally "-full"; planes under "y", "uv" (NV12, P010) / "vu" (NV21) / "u", "v", or "packed" for the packed formats
 // (host Buffers / typed arrays, tight pitches) -> an ht_yuv_image; false for a bad object
 static bool YuvImageOf(napi_env env, napi_value r, ht_yuv_image *img) {
   std::memset(img, 0, sizeof(*img));
@@ -671,19 +673,39 @@ static bool YuvImageOf(napi_env env, napi_value r, ht_yuv_image *img) {
   if (img->width <= 0 || img->height <= 0) return false;
   if (napi_has_named_property(env, r, "format", &has) == napi_ok && has && napi_get_named_property(env, r, "format", &v) == napi_ok)
     napi_get_value_string_utf8(env, v, s, sizeof(s), &sl);
-  img->format = (sl == 0 || std::strcmp(s, "nv12") == 0) ? HT_YUV_NV12 : std::strcmp(s, "i420") == 0 ? HT_YUV_I420 : -1;
+  static const struct { const char *name; int format; } formats[] = {
+      {"nv12", HT_YUV_NV12}, {"i420", HT_YUV_I420}, {"nv21", HT_YUV_NV21}, {"i422", HT_YUV_I422}, {"i444", HT_YUV_I444},
+      {"yuyv", HT_YUV_YUYV}, {"uyvy", HT_YUV_UYVY}, {"p010", HT_YUV_P010}, {"bgra", HT_YUV_BGRA},
+      {"bgr24", HT_YUV_BGR24}, {"rgb24", HT_YUV_RGB24}};
+  img->format = sl == 0 ? HT_YUV_NV12 : -1;
+  for (const auto &f : formats)
+    if (sl && std::strcmp(s, f.name) == 0) img->format = f.format;
+  if (img->format < 0) return false;
   sl = 0;
   if (napi_has_named_property(env, r, "color", &has) == napi_ok && has && napi_get_named_property(env, r, "color", &v) == napi_ok)
     napi_get_value_string_utf8(env, v, s, sizeof(s), &sl);
-  const char *names[4] = {"bt601", "bt709", "bt601-full", "bt709-full"};
+  static const struct { const char *name; int color; } colors[] = {
+      {"bt601", 0}, {"bt709", HT_YUV_BT709}, {"bt601-full", HT_YUV_FULL_RANGE},
+      {"bt709-full", HT_YUV_BT709 | HT_YUV_FULL_RANGE}, {"bt2020", HT_YUV_BT2020},
+      {"bt2020-full", HT_YUV_BT2020 | HT_YUV_FULL_RANGE}};
   img->color = sl == 0 ? HT_YUV_BT601 : -1;
-  for (int i = 0; i < 4 && sl; ++i)
-    if (std::strcmp(s, names[i]) == 0) img->color = i;   // HT_YUV_BT709 = 1, HT_YUV_FULL_RANGE = 2
-  const size_t cw = (size_t)(img->width + 1) / 2, ch = (size_t)(img->height + 1) / 2;
-  const bool nv12 = img->format == HT_YUV_NV12;
-  const char *keys[3] = {"y", nv12 ? "uv" : "u", "v"};
-  const size_t need[3] = {(size_t)img->width * img->height, (nv12 ? 2 : 1) * cw * ch, cw * ch};
-  for (int p = 0; p < (nv12 ? 2 : 3); ++p) {
+  for (const auto &c : colors)
+    if (sl && std::strcmp(s, c.name) == 0) img->color = c.color;
+  const size_t w = (size_t)img->width, h = (size_t)img->height, cw = (w + 1) / 2, ch = (h + 1) / 2;
+  const char *keys[3] = {"y", "uv", nullptr};
+  size_t need[3] = {w * h, 2 * cw * ch, 0};
+  switch (img->format) {
+    case HT_YUV_NV21: keys[1] = "vu"; break;
+    case HT_YUV_I420: keys[1] = "u", keys[2] = "v", need[1] = need[2] = cw * ch; break;
+    case HT_YUV_I422: keys[1] = "u", keys[2] = "v", need[1] = need[2] = cw * h; break;
+    case HT_YUV_I444: keys[1] = "u", keys[2] = "v", need[1] = need[2] = w * h; break;
+    case HT_YUV_P010: need[0] = 2 * w * h, need[1] = 4 * cw * ch; break;
+    case HT_YUV_YUYV: case HT_YUV_UYVY: keys[0] = "packed", keys[1] = nullptr, need[0] = 4 * cw * h; break;
+    case HT_YUV_BGRA: keys[0] = "packed", keys[1] = nullptr, need[0] = 4 * w * h; break;
+    case HT_YUV_BGR24: case HT_YUV_RGB24: keys[0] = "packed", keys[1] = nullptr, need[0] = 3 * w * h; break;
+    default: break;
+  }
+  for (int p = 0; p < 3 && keys[p]; ++p) {
     uint8_t *data; size_t len;
     if (napi_get_named_property(env, r, keys[p], &v) != napi_ok || !GetBytes(env, v, &data, &len) || len < need[p]) return false;
     img->planes[p] = data;

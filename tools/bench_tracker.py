@@ -19,6 +19,9 @@ streams: N 640x480 streams, device-resident frames and outputs, CUDA events arou
                   (--yuv) ht_tracker_feed_yuv from NV12 video against ht_ingest_yuv + ht_tracker_feed and against
                   ht_tracker_feed from RGBA video of the same size (also --before-lib), and the draw kernels' time
                   (yuv_arms)
+  <fmt>_*         (--formats) ht_tracker_feed_yuv from every video format against ht_ingest_yuv + ht_tracker_feed and
+                  ht_tracker_feed from the converted RGBA video, NV12 / I420 / RGBA also against --before-lib, and
+                  k_feed_draw_yuv's time per format (formats_arms)
 
 Prints one JSON line with the card's name and power limit read in the same run; --out also writes it to a file."""
 import argparse
@@ -189,6 +192,8 @@ def other_build_context(before_lib, **kw):
     for f in (L.ht_tracker_reset, L.ht_tracker_start, L.ht_tracker_stop):
         f.argtypes = [vp, C.c_int, C.c_int]
     L.ht_tracker_feed.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp]
+    if hasattr(L, "ht_tracker_feed_yuv"):
+        L.ht_tracker_feed_yuv.argtypes = [vp, vp, C.c_int, C.c_int, vp]
     saved = _lib.lib
     _lib.lib = lambda: L
     try:
@@ -673,6 +678,172 @@ def yuv_arms(torch, stream, N, steps, rounds, before_lib=None):
     return res
 
 
+FORMATS = ["nv21", "i422", "i444", "yuyv", "uyvy", "p010", "bgra", "bgr24", "rgb24", "nv12", "i420"]
+
+
+def format_video(torch, rgba, fmt):
+    """(N, H, W, 4) uint8 device RGBA -> the same video in `fmt` as Context takes it, one frame per stream (a test-local
+    BT.601 limited-range RGB -> YUV, chroma from the block's first pixel; P010 with the 8-bit value in the top byte)"""
+    N, H, W = rgba.shape[:3]
+    if fmt in ("bgra", "bgr24", "rgb24"):
+        order = {"bgra": [2, 1, 0, 3], "bgr24": [2, 1, 0], "rgb24": [0, 1, 2]}[fmt]
+        v = rgba[..., order].contiguous()
+        return [v[k] for k in range(N)]
+    f = rgba.float()
+    r, g, b = f[..., 0], f[..., 1], f[..., 2]
+    q = lambda a: torch.floor(a + 0.5).clamp(0, 255).to(torch.uint8)     # noqa: E731
+    y = q(16 + (65.481 * r + 128.553 * g + 24.966 * b) / 255)
+    u = q(128 + (-37.797 * r - 74.203 * g + 112.0 * b) / 255)
+    v = q(128 + (112.0 * r - 93.786 * g - 18.214 * b) / 255)
+    del f, r, g, b
+    if fmt == "i444":
+        return [(y[k], u[k].contiguous(), v[k].contiguous()) for k in range(N)]
+    if fmt in ("i422", "yuyv", "uyvy"):
+        u2, v2 = u[:, :, 0::2].contiguous(), v[:, :, 0::2].contiguous()
+        if fmt == "i422":
+            return [(y[k], u2[k], v2[k]) for k in range(N)]
+        a, c = (y[:, :, 0::2], u2) if fmt == "yuyv" else (u2, y[:, :, 0::2])
+        bb, d = (y[:, :, 1::2], v2) if fmt == "yuyv" else (v2, y[:, :, 1::2])
+        p = torch.stack([a, c, bb, d], dim=-1).reshape(N, H, W, 2)
+        return [p[k] for k in range(N)]
+    u4, v4 = u[:, 0::2, 0::2], v[:, 0::2, 0::2]
+    if fmt == "i420":
+        return [(y[k], u4[k].contiguous(), v4[k].contiguous()) for k in range(N)]
+    pair = torch.stack([v4, u4] if fmt == "nv21" else [u4, v4], dim=-1).reshape(N, H // 2, W)
+    if fmt == "p010":
+        w16 = lambda a: (a.to(torch.int32) << 8).to(torch.int16)           # noqa: E731
+        y16, p16 = w16(y), w16(pair)
+        return [(y16[k], p16[k]) for k in range(N)]
+    return [(y[k], pair[k]) for k in range(N)]
+
+
+def formats_arms(torch, stream, N, steps, rounds, before_lib=None):
+    """Every video format (ht_tracker_feed_yuv) in steady tracking, for each (video, canvas) of YUV_LAYOUTS: N streams,
+    each with its own device video, every arm on its own context, the arms of a (layout, format) alternating tick by
+    tick (the order rotates), CUDA events around each tick:
+
+      <fmt>_<layout>_cs          ht_tracker_feed_yuv from the video in <fmt>
+      <fmt>_twopass_<layout>_cs  ht_ingest_yuv of the batch into a device RGBA buffer, then ht_tracker_feed
+      <fmt>_rgba_<layout>_cs     ht_tracker_feed from the RGBA frames the conversion makes
+      <fmt>_before_<layout>_cs   (nv12, i420) ht_tracker_feed_yuv with the library at `before_lib`
+      <fmt>_rgba_before_<layout>_cs  (nv12) the RGBA arm with the library at `before_lib`
+
+    Then, in runs of their own under torch.profiler, k_feed_draw_yuv's time per tick for each format and its achieved
+    bytes/s (video bytes read once + canvas written).  The records of every arm must agree on every timed tick."""
+    import ctypes as C
+    from headtrackr_b200 import Context, _lib, synth
+    from headtrackr_b200.context import _yuv_image
+    rec_bytes = C.sizeof(_lib.TrackerEvent)
+    res = {}
+    for (W, H), (CW, CH) in YUV_LAYOUTS:
+        lay = f"{W}x{H}_{CW}x{CH}"
+        kw = dict(max_width=CW, max_height=CH, max_frames=N, stream=stream)
+        base = torch.stack([torch.from_numpy(synth.frame(i, W, H, n_faces=1)) for i in range(8)]).cuda()
+        rgba = torch.empty((N, H, W, 4), dtype=torch.uint8, device="cuda")
+        for k in range(N):
+            rgba[k] = torch.roll(base[k % 8], shifts=2 * (k // 8) % 64, dims=1)
+        del base
+        conv = torch.empty_like(rgba)
+        staged = torch.empty_like(rgba)
+        for fmt in FORMATS:
+            now = [1.0e12]
+            vid = format_video(torch, rgba, fmt)
+            keep = []
+            imgs = [_yuv_image(v, fmt, "bt601", keep)[0] for v in vid]
+            cc = Context(max_width=CW, max_height=CH, max_frames=1, stream=stream)
+            cc.ingest_yuv(vid, W, H, fmt, out=conv)
+            cc.sync()
+            cc.close()
+            yrecs = (_lib.YuvFrame * N)(*[_lib.YuvFrame(imgs[k], k, CW, CH, 0, 0.0) for k in range(N)])
+            vrecs = (_lib.VideoFrame * N)(*[_lib.VideoFrame(conv[k].data_ptr(), k, W, H, 0, 0.0) for k in range(N)])
+            srecs = (_lib.VideoFrame * N)(*[_lib.VideoFrame(staged[k].data_ptr(), k, W, H, 0, 0.0) for k in range(N)])
+            ingest_src = (_lib.YuvImage * N)(*imgs)
+
+            def arm(kind):
+                before = kind.endswith("before")
+                c = other_build_context(before_lib, **kw) if before else Context(**kw)
+                c.tracker_config()
+                c.tracker_reset(0, N)
+                c.tracker_start(0, N)
+                out = torch.empty(N * rec_bytes, dtype=torch.uint8, device="cuda")
+
+                def run():
+                    t = now[0]
+                    if kind in ("fmt", "before"):
+                        for k in range(N):
+                            yrecs[k].now_ms = t
+                        c._check(c._L.ht_tracker_feed_yuv(c._h, C.addressof(yrecs), N, 1, out.data_ptr()))
+                        return
+                    recs = vrecs
+                    if kind == "twopass":
+                        c._check(c._L.ht_ingest_yuv(c._h, C.addressof(ingest_src), N, 1, staged.data_ptr(), W, H))
+                        recs = srecs
+                    for k in range(N):
+                        recs[k].now_ms = t
+                    c._check(c._L.ht_tracker_feed(c._h, C.addressof(recs), N, 1, CW, CH, out.data_ptr()))
+                return c, run, out
+
+            kinds = ["fmt", "twopass", "rgba"]
+            if before_lib and fmt in ("nv12", "i420"):
+                kinds.append("before")
+            if before_lib and fmt == "nv12":
+                kinds.append("rgba_before")
+            arms = {k: arm(k) for k in kinds}
+
+            def tick(name):
+                a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                a.record()
+                arms[name][1]()
+                b.record()
+                b.synchronize()
+                return a.elapsed_time(b)
+
+            for _ in range(17):
+                now[0] += 20.0
+                for name in kinds:
+                    tick(name)
+            times = {name: [[] for _ in range(rounds)] for name in kinds}
+            for r in range(rounds):
+                for s in range(steps):
+                    now[0] += 20.0
+                    rot = (r * steps + s) % len(kinds)
+                    for name in kinds[rot:] + kinds[:rot]:
+                        times[name][r].append(tick(name))
+                    if any(not torch.equal(arms["fmt"][2], arms[name][2]) for name in kinds[1:]):
+                        raise SystemExit(f"format arms disagree on the records of a timed tick ({fmt}, {lay})")
+            for name in kinds:
+                med = [float(np.median(t)) for t in times[name]]
+                key = fmt if name == "fmt" else f"{fmt}_{name}"
+                res[f"{key}_{lay}_cs_ms"] = float(np.median(sum(times[name], [])))
+                res[f"{key}_{lay}_cs_spread_ms"] = max(med) - min(med)
+            ev = [_lib.TrackerEvent.from_buffer_copy(bytes(row)) for row in arms["fmt"][2].cpu().numpy().reshape(N, rec_bytes)]
+            res[f"{fmt}_{lay}_cs_streams"] = sum(e.detection == 2 for e in ev)
+
+            from torch.profiler import ProfilerActivity, profile
+            with profile(activities=[ProfilerActivity.CUDA]) as prof:
+                for _ in range(steps):
+                    now[0] += 20.0
+                    arms["fmt"][1]()
+                torch.cuda.synchronize()
+            us = 0.0
+            for e in prof.key_averages():
+                if e.key.split("(")[0].split("<")[0].endswith("k_feed_draw_yuv"):
+                    t = getattr(e, "device_time_total", None)
+                    us += t if t is not None else e.cuda_time_total
+            ms = us / 1000.0 / steps
+            video_bytes = N * sum(t.numel() * t.element_size() for t in (vid[0] if isinstance(vid[0], tuple) else (vid[0],)))
+            res[f"k_feed_draw_yuv_{fmt}_{lay}_ms"] = ms
+            res[f"k_feed_draw_yuv_{fmt}_{lay}_tb_per_s"] = (video_bytes + N * CW * CH * 4) / (ms * 1e-3) / 1e12 if ms > 0 else None
+            for c, _, _ in arms.values():
+                c.close()
+            del vid, keep, imgs
+            torch.cuda.empty_cache()
+        del rgba, conv, staged
+        torch.cuda.empty_cache()
+    res["formats_records_agree"] = True
+    return res
+
+
 def migrate_arms(torch, frames, stream, N, W, H, steps, rounds):
     """Tracker records (ht_tracker_export / ht_tracker_import) of N streams in steady tracking, W x H video on W/2 x H/2
     canvases, CUDA events on the library's stream around each call, repeated `rounds` x `steps` times:
@@ -775,6 +946,7 @@ def main():
     ap.add_argument("--migrate", action="store_true", help="only the tracker-record arms (migrate_arms)")
     ap.add_argument("--camera-streams", action="store_true", help="only the camera-controller arms (camera_arms)")
     ap.add_argument("--yuv", action="store_true", help="only the YUV video arms (yuv_arms)")
+    ap.add_argument("--formats", action="store_true", help="only the video-format arms (formats_arms)")
     ap.add_argument("--out")
     a = ap.parse_args()
     import torch
@@ -790,6 +962,9 @@ def main():
     stream = ts.cuda_stream
     if a.yuv:
         res.update(yuv_arms(torch, stream, N, a.steps, a.rounds, a.before_lib))
+        return report(res, a.out)
+    if a.formats:
+        res.update(formats_arms(torch, stream, N, a.steps, a.rounds, a.before_lib))
         return report(res, a.out)
     if a.migrate:
         res.update(migrate_arms(torch, frames, stream, N, W, H, a.steps, a.rounds))
