@@ -96,6 +96,15 @@ class YuvFrame(C.Structure):
 
 assert C.sizeof(YuvImage) == 56 and C.sizeof(YuvFrame) == 80 and YuvFrame.now_ms.offset == 72
 
+# ht_video_view.orientation: orientation & 3 = clockwise quarter turns, then HT_VIEW_MIRROR mirrors horizontally
+HT_VIEW_ROTATE_90, HT_VIEW_ROTATE_180, HT_VIEW_ROTATE_270, HT_VIEW_MIRROR = 1, 2, 3, 4
+
+
+class VideoView(C.Structure):
+    """ht_video_view: an orientation (0..7) and a source rectangle of the oriented frame (all 0 = the whole frame)"""
+    _fields_ = [("orientation", C.c_int32), ("sx", C.c_int32), ("sy", C.c_int32), ("sw", C.c_int32), ("sh", C.c_int32),
+                ("reserved", C.c_int32 * 3)]
+
 
 class DebugCanvas(C.Structure):
     """ht_debug_canvas: a stream's debug canvas for ht_tracker_set_debug (device memory; rgba NULL = none; pitch 0 =
@@ -164,7 +173,8 @@ _lib = None
 
 EXPORTS = ["ht_version", "ht_create", "ht_destroy", "ht_last_error", "ht_sync", "ht_max_rects", "ht_detect",
            "ht_track_init", "ht_track_init_from_detect", "ht_track", "ht_detect_track", "ht_stream_reset", "ht_stream_step", "ht_stream_head_config", "ht_stream_step_head",
-           "ht_tracker_config", "ht_tracker_reset", "ht_tracker_start", "ht_tracker_stop", "ht_tracker_step", "ht_tracker_feed", "ht_tracker_set_params", "ht_tracker_feed_canvases", "ht_tracker_set_debug", "ht_tracker_set_camera", "ht_tracker_export", "ht_tracker_import", "ht_tracker_feed_yuv", "ht_ingest", "ht_ingest_yuv", "ht_backprojection", "ht_whitebalance",
+           "ht_tracker_config", "ht_tracker_reset", "ht_tracker_start", "ht_tracker_stop", "ht_tracker_step", "ht_tracker_feed", "ht_tracker_set_params", "ht_tracker_feed_canvases", "ht_tracker_set_debug", "ht_tracker_set_camera", "ht_tracker_export", "ht_tracker_import", "ht_tracker_feed_yuv", "ht_ingest", "ht_ingest_yuv",
+           "ht_tracker_feed_views", "ht_tracker_feed_yuv_views", "ht_ingest_views", "ht_ingest_yuv_views", "ht_backprojection", "ht_whitebalance",
            "ht_plan_info", "ht_debug_plane", "ht_debug_raw", "ht_debug_model_hist", "ht_debug_track_stats", "ht_set_track_memo", "ht_set_pipeline", "ht_join", "ht_debug_set_exactness", "ht_debug_track_trace", "ht_debug_track_phases", "ht_launch_count",
            "ht_profile", "ht_profile_read"]
 
@@ -214,6 +224,10 @@ def lib():
     L.ht_ingest.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, vp, C.c_int, C.c_int]
     L.ht_tracker_feed_yuv.argtypes = [vp, vp, C.c_int, C.c_int, vp]
     L.ht_ingest_yuv.argtypes = [vp, vp, C.c_int, C.c_int, vp, C.c_int, C.c_int]
+    L.ht_tracker_feed_views.argtypes = [vp, vp, vp, C.c_int, C.c_int, vp]
+    L.ht_tracker_feed_yuv_views.argtypes = [vp, vp, vp, C.c_int, C.c_int, vp]
+    L.ht_ingest_views.argtypes = [vp, vp, vp, C.c_int, C.c_int, vp, C.c_int, C.c_int]
+    L.ht_ingest_yuv_views.argtypes = [vp, vp, vp, C.c_int, C.c_int, vp, C.c_int, C.c_int]
     L.ht_backprojection.argtypes = [vp, C.c_int, vp, C.c_int, C.c_int, vp]
     L.ht_whitebalance.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, vp]
     L.ht_plan_info.argtypes = [vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, C.c_int]

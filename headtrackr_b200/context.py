@@ -9,7 +9,8 @@ import numpy as np
 
 from . import _lib
 from ._lib import (Camera, CameraControl, CanvasFrame, DebugCanvas, HeadEvent, HeadParams, HtError, Rect, StreamEvent, TrackerEvent, TrackerParams, TrackObj, VideoFrame,
-                   Window, YuvFrame, YuvImage)
+                   VideoView, Window, YuvFrame, YuvImage)
+from .views import video_view
 from .synth import load_cascade_blob
 
 
@@ -111,6 +112,27 @@ def _per_record(v, n, what):
     if len(vs) != n:
         raise ValueError(f"one {what} per frame")
     return vs
+
+
+def _rgba_frame(f, on_device):
+    """one (h, w, 4) uint8 video frame, a numpy array or (on_device) a torch CUDA tensor, rows of any stride ->
+    (address, pitch in bytes, the array to keep alive)"""
+    if on_device:
+        if f.dim() != 3 or f.element_size() != 1 or f.shape[2] != 4 or f.stride(2) != 1 or f.stride(1) != 4:
+            raise ValueError("frame tensors must be uint8 (h, w, 4) with strides (pitch, 4, 1)")
+        return f.data_ptr(), f.stride(0), f
+    a = np.asarray(f)
+    if a.dtype != np.uint8 or a.ndim != 3 or a.shape[2] != 4:
+        raise ValueError("frames must be (h, w, 4) uint8")
+    if a.strides[2] != 1 or a.strides[1] != 4 or a.strides[0] < 4 * a.shape[1]:
+        a = np.ascontiguousarray(a)
+    return a.ctypes.data, a.strides[0], a
+
+
+def _views(view, n):
+    """view= of the feed and ingest methods (one view dict for all records, or a list of one per record) -> an
+    ht_video_view array"""
+    return (VideoView * n)(*[video_view(v) for v in _per_record(view, n, "view")])
 
 
 def camera_from_bytes(b):
@@ -449,14 +471,16 @@ class Context:
         self._check(self._L.ht_tracker_step(self._h, ptr, n, W, H, float(now_ms), C.addressof(ev)))
         return [tracker_event_dict(e) for e in ev]
 
-    def tracker_feed(self, streams, frames, now_ms, width, height, out=None):
+    def tracker_feed(self, streams, frames, now_ms, width, height, out=None, view=None):
         """One timer tick of each listed stream on its own video frame and clock (ht_tracker_feed): drawImage(video, 0,
         0, width, height) onto the working canvas, then what tracker_step does for that stream.  Unlisted streams do
         not tick.  streams: distinct stream ids; frames: one (h, w, 4) u8 video frame per stream, all numpy arrays or
         all torch CUDA tensors (any size; a row-padded view - last two strides (4, 1) - passes its row stride as the
         pitch); now_ms: one clock for all or one per record; width, height: one canvas for all (ht_tracker_feed) or one
-        size per record (ht_tracker_feed_canvases: each stream on its own canvas).  -> event dicts in record order;
-        with a torch CUDA `out` tensor of len(streams)*144 bytes: asynchronous, nothing returned."""
+        size per record (ht_tracker_feed_canvases: each stream on its own canvas).  view: None, or a view
+        (headtrackr_b200.views: {"rotate", "mirror", "crop"}) for all records or a list of one per record, drawn
+        through ht_tracker_feed_views.  -> event dicts in record order; with a torch CUDA `out` tensor of
+        len(streams)*144 bytes: asynchronous, nothing returned."""
         streams = list(streams)
         n = len(frames)
         if len(streams) != n or n == 0:
@@ -476,23 +500,18 @@ class Context:
         for b, (k, f) in enumerate(zip(streams, frames)):
             if _is_torch(f) != on_device:
                 raise ValueError("frames must be all numpy arrays or all torch CUDA tensors")
-            if on_device:
-                if f.dim() != 3 or f.element_size() != 1 or f.shape[2] != 4 or f.stride(2) != 1 or f.stride(1) != 4:
-                    raise ValueError("frame tensors must be uint8 (h, w, 4) with strides (pitch, 4, 1)")
-                ptr, pitch = f.data_ptr(), f.stride(0)
-            else:
-                a = np.asarray(f)
-                if a.dtype != np.uint8 or a.ndim != 3 or a.shape[2] != 4:
-                    raise ValueError("frames must be (h, w, 4) uint8")
-                if a.strides[2] != 1 or a.strides[1] != 4 or a.strides[0] < 4 * a.shape[1]:
-                    a = np.ascontiguousarray(a)
-                ptr, pitch = a.ctypes.data, a.strides[0]
-                f = a
+            ptr, pitch, f = _rgba_frame(f, on_device)
             keep.append(f)
             recs[b] = VideoFrame(ptr, int(k), f.shape[1], f.shape[0], pitch, clocks[b])
         ev = None if out is not None else (TrackerEvent * n)()
         dst = out.data_ptr() if out is not None else C.addressof(ev)
-        if per_record:
+        if view is not None:
+            widths = widths if per_record else [int(width)] * n
+            heights = heights if per_record else [int(height)] * n
+            crecs = (CanvasFrame * n)(*[CanvasFrame(recs[b], widths[b], heights[b]) for b in range(n)])
+            views = _views(view, n)
+            self._check(self._L.ht_tracker_feed_views(self._h, C.addressof(crecs), C.addressof(views), n, int(on_device), dst))
+        elif per_record:
             crecs = (CanvasFrame * n)(*[CanvasFrame(recs[b], widths[b], heights[b]) for b in range(n)])
             self._check(self._L.ht_tracker_feed_canvases(self._h, C.addressof(crecs), n, int(on_device), dst))
         else:
@@ -501,7 +520,7 @@ class Context:
             return None
         return [tracker_event_dict(e) for e in ev]
 
-    def tracker_feed_yuv(self, streams, frames, now_ms, width, height, format="nv12", color="bt601", out=None):
+    def tracker_feed_yuv(self, streams, frames, now_ms, width, height, format="nv12", color="bt601", out=None, view=None):
         """tracker_feed on video in any of _lib.YUV_FORMATS (ht_tracker_feed_yuv): each frame is a tuple of 2-D planes
         for a planar format ((Y, UV) for NV12, (Y, U, V) for I420, uint16 planes for P010) or one (h, w, channels)
         array for a packed one (YUYV, UYVY, BGRA, BGR24, RGB24; _yuv_image), numpy arrays or torch tensors (CPU, or
@@ -510,8 +529,8 @@ class Context:
             frame = (buf[:h, :w], buf[h:, :2 * ((w + 1) // 2)])
         The conversion is the library's (DESIGN.md 2): format (a key of _lib.YUV_FORMATS) and color ("bt601",
         "bt709", "bt2020", each optionally "-full"; "bt601" for the packed RGB formats), one for all or one per
-        record.  now_ms, width and height as for tracker_feed
-        (every record has its own canvas here).  -> event dicts in record order; with a torch CUDA `out` tensor of
+        record.  now_ms, width, height and view as for tracker_feed
+        (every record has its own canvas here; with a view, ht_tracker_feed_yuv_views).  -> event dicts in record order; with a torch CUDA `out` tensor of
         len(streams)*144 bytes: asynchronous, nothing returned."""
         streams = list(streams)
         n = len(frames)
@@ -533,14 +552,19 @@ class Context:
             raise ValueError("frames must be all host or all device memory")
         ev = None if out is not None else (TrackerEvent * n)()
         dst = out.data_ptr() if out is not None else C.addressof(ev)
-        self._check(self._L.ht_tracker_feed_yuv(self._h, C.addressof(recs), n, int(where.pop()), dst))
+        if view is not None:
+            views = _views(view, n)
+            self._check(self._L.ht_tracker_feed_yuv_views(self._h, C.addressof(recs), C.addressof(views), n, int(where.pop()),
+                                                          dst))
+        else:
+            self._check(self._L.ht_tracker_feed_yuv(self._h, C.addressof(recs), n, int(where.pop()), dst))
         if out is not None:
             return None
         return [tracker_event_dict(e) for e in ev]
 
-    def ingest_yuv(self, frames, width, height, format="nv12", color="bt601", out=None):
+    def ingest_yuv(self, frames, width, height, format="nv12", color="bt601", out=None, view=None):
         """drawImage(video, 0, 0, width, height) of video frames (ht_ingest_yuv): frames, format and color as for
-        tracker_feed_yuv (the frames may differ in size and format).  -> numpy (n, height, width, 4); with a torch `out` tensor
+        tracker_feed_yuv (the frames may differ in size and format); view as for tracker_feed (ht_ingest_yuv_views).  -> numpy (n, height, width, 4); with a torch `out` tensor
         of that shape (CUDA or CPU) the result is written there."""
         n = len(frames)
         if n == 0:
@@ -554,6 +578,10 @@ class Context:
         if len(where) != 1:
             raise ValueError("frames must be all host or all device memory")
         on_device = where.pop()
+        if view is not None:
+            views = _views(view, n)
+            return self._ingest_into(out, n, width, height, lambda dst: self._L.ht_ingest_yuv_views(
+                self._h, C.addressof(imgs), C.addressof(views), n, int(on_device), dst, width, height))
         if out is not None:
             if not out.is_contiguous() or tuple(out.shape) != (n, height, width, 4) or out.element_size() != 1:
                 raise ValueError(f"out must be a contiguous uint8 tensor of shape {(n, height, width, 4)}")
@@ -563,9 +591,39 @@ class Context:
         self._check(self._L.ht_ingest_yuv(self._h, C.addressof(imgs), n, int(on_device), dst.ctypes.data, width, height))
         return dst
 
-    def ingest(self, frames, width, height, out=None):
+    def _ingest_into(self, out, n, width, height, call):
+        """call(destination address) writes n width x height canvases: into `out` (a contiguous torch uint8 tensor,
+        CUDA or CPU), or into a new numpy array"""
+        if out is not None:
+            if not out.is_contiguous() or tuple(out.shape) != (n, height, width, 4) or out.element_size() != 1:
+                raise ValueError(f"out must be a contiguous uint8 tensor of shape {(n, height, width, 4)}")
+            self._check(call(out.data_ptr()))
+            return out
+        dst = np.zeros((n, height, width, 4), np.uint8)
+        self._check(call(dst.ctypes.data))
+        return dst
+
+    def ingest(self, frames, width, height, out=None, view=None):
         """drawImage(video, 0, 0, width, height) for a batch (src/main.js:170).  numpy in -> numpy (n, height, width, 4)
-        out; with a torch CUDA `out` tensor the result stays on the device."""
+        out; with a torch CUDA `out` tensor the result stays on the device.  With a view (as for tracker_feed;
+        ht_ingest_views), frames is a list of (h, w, 4) frames of any sizes, all numpy arrays or all torch CUDA
+        tensors, and `out` may also be a CPU tensor."""
+        if view is not None:
+            n = len(frames)
+            if n == 0:
+                raise ValueError("no frames")
+            on_device = _is_torch(frames[0]) and frames[0].is_cuda
+            recs = (VideoFrame * n)()
+            keep = []
+            for b, f in enumerate(frames):
+                if (_is_torch(f) and f.is_cuda) != on_device:
+                    raise ValueError("frames must be all numpy arrays or all torch CUDA tensors")
+                ptr, pitch, a = _rgba_frame(f, on_device)
+                keep.append(a)
+                recs[b] = VideoFrame(ptr, 0, a.shape[1], a.shape[0], pitch, 0.0)
+            views = _views(view, n)
+            return self._ingest_into(out, n, width, height, lambda dst: self._L.ht_ingest_views(
+                self._h, C.addressof(recs), C.addressof(views), n, int(on_device), dst, width, height))
         ptr, n, H, W, keep = _frames_ptr(frames)
         if out is not None:
             self._check(self._L.ht_ingest(self._h, ptr, n, W, H, out.data_ptr(), width, height))

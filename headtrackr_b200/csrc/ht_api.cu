@@ -2056,6 +2056,7 @@ struct FeedDraw {
   const int32_t *tile_start;
   int tiles;
   const YuvFeedRec *yuv;   // ht_tracker_feed_yuv: the records are these (recs unused), drawn by k_feed_draw_yuv
+  const ViewFeedRec *view; // ht_tracker_feed(_yuv)_views: the records are these (recs, yuv unused), k_feed_draw_view
 };
 
 // One canvas size of a tracker tick: batch entries [k0, k0 + n) on canvases of w x h (plan P) at frames (n consecutive
@@ -2074,7 +2075,7 @@ struct TickGroup {
 // per-stream kernels once per call.
 //   k_tracker_plan   modes -> VJ frame-quad mask, CS enable, whitebalance enable (feed: draw flags)
 //   k_feed_draw      (feed) drawImage(video, 0, 0, w, h) of every stream that is not IDLE   src/main.js:170,312
-//                    (k_feed_draw_yuv for the YUV records of ht_tracker_feed_yuv)
+//                    (k_feed_draw_yuv for the YUV records of ht_tracker_feed_yuv, k_feed_draw_view for views)
 //   k_wb_sums        whitebalance sums of the STARTING and WB streams only       src/whitebalance.js, src/main.js:316
 //   run_detect       per group: the VJ streams (interval 5, min_neighbors 1)     src/facetrackr.js:147-149
 //   k_hist, k_track  per group: one track() of the CS streams                    src/camshift.js:213-312
@@ -2097,7 +2098,13 @@ static int tracker_tick(ht_ctx *ctx, const TickGroup *grp, int n_groups, const u
   k_tracker_plan<<<(n + 127) / 128, 128, 0, st>>>(ts, d_ids, n, vj_mask, cs_en, init_en, wb_en, feed ? feed->draw : nullptr, geo);
   if (feed) {
     uint8_t *canvas = const_cast<uint8_t *>(d_rgba);
-    if (feed->yuv && !feed->tile_start) {
+    if (feed->view && !feed->tile_start) {
+      const int tiles_x = (g0.w + 63) / 64, tiles = tiles_x * ((g0.h + 15) / 16);
+      k_feed_draw_view<<<dim3((unsigned)tiles, (unsigned)n), 256, 0, st>>>(feed->view, feed->draw, canvas, feed->g, tiles_x,
+                                                                           nullptr, nullptr, n);
+    } else if (feed->view) {
+      k_feed_draw_view<<<(unsigned)feed->tiles, 256, 0, st>>>(feed->view, feed->draw, canvas, feed->g, 0, geo, feed->tile_start, n);
+    } else if (feed->yuv && !feed->tile_start) {
       const int tiles_x = (g0.w + 63) / 64, tiles = tiles_x * ((g0.h + 15) / 16);
       k_feed_draw_yuv<<<dim3((unsigned)tiles, (unsigned)n), 256, 0, st>>>(feed->yuv, feed->draw, canvas, feed->g, tiles_x,
                                                                           nullptr, nullptr, n);
@@ -2304,6 +2311,70 @@ static int stage_yuv(ht_ctx *ctx, const ht_yuv_image &v, YuvFeedRec &r, uint8_t 
   return yuv_record(staged, r, why);
 }
 
+static_assert(sizeof(ht_video_view) == 32 && offsetof(ht_video_view, reserved) == 20, "ht_video_view layout");
+static_assert(sizeof(ViewFeedRec) % 8 == 0, "ViewFeedRec layout");
+
+// An ht_video_view of a w x h video checked and resolved into v's map (DESIGN.md 2, "Views"; v.src and v.kind are
+// left as they are) -> HT_OK, or HT_ERR_ARG with the reason in why[256]
+static int view_record(const ht_video_view &view, int w, int h, ViewFeedRec &v, char *why) {
+  const int o = view.orientation;
+  if (o < 0 || o > 7) return snprintf(why, 256, "orientation %d outside 0..7", o), HT_ERR_ARG;
+  for (int i = 0; i < 3; ++i)
+    if (view.reserved[i]) return snprintf(why, 256, "reserved[%d] = %d must be 0", i, view.reserved[i]), HT_ERR_ARG;
+  const int W = (o & 1) ? h : w, H = (o & 1) ? w : h;   // the oriented frame
+  int sx = view.sx, sy = view.sy, sw = view.sw, sh = view.sh;
+  if ((sx | sy | sw | sh) == 0) {
+    sw = W, sh = H;
+  } else if (sw < 1 || sh < 1 || sx < 0 || sy < 0 || sx > W - sw || sy > H - sh) {
+    return snprintf(why, 256, "source rectangle (%d, %d, %d, %d) is empty or not inside the %dx%d oriented frame", sx, sy,
+                    sw, sh, W, H),
+           HT_ERR_ARG;
+  }
+  // the video pixel of oriented pixel (x, y): affine in (x, y), so three points give the map
+  auto video_of = [&](int x, int y, int &vx, int &vy) {
+    if (o & HT_VIEW_MIRROR) x = W - 1 - x;
+    switch (o & 3) {
+      case 0: vx = x, vy = y; break;
+      case 1: vx = y, vy = h - 1 - x; break;
+      case 2: vx = w - 1 - x, vy = h - 1 - y; break;
+      default: vx = w - 1 - y, vy = x; break;
+    }
+  };
+  int x0, y0, x1, y1, x2, y2;
+  video_of(sx, sy, x0, y0);
+  video_of(sx + 1, sy, x1, y1);
+  video_of(sx, sy + 1, x2, y2);
+  v.bx = x0, v.by = y0, v.mxx = x1 - x0, v.myx = y1 - y0, v.mxy = x2 - x0, v.myy = y2 - y0;
+  v.sw = sw, v.sh = sh, v.pad_ = 0;
+  return HT_OK;
+}
+static int check_view(ht_ctx *ctx, const ht_video_view &view, int w, int h, int b, ViewFeedRec &v) {
+  char why[256];
+  const int rc = view_record(view, w, h, v, why);
+  return rc == HT_OK ? HT_OK : ctx->fail(rc, "record %d: %s", b, why);
+}
+// the texel source of view record v: an RGBA8 frame (pitch in bytes), or a resolved YUV record
+static void view_source_rgba(ViewFeedRec &v, const uint8_t *rgba, int pitch, int w, int h) {
+  v.src = YuvFeedRec{};
+  v.src.y = rgba, v.src.ypitch = pitch, v.src.width = w, v.src.height = h;
+  v.kind = VIEW_RGBA;
+}
+static void view_source_yuv(ViewFeedRec &v, const YuvFeedRec &r) {
+  v.src = r;
+  v.kind = nv12_i420_path(r) ? VIEW_NV12_I420 : VIEW_FMT;
+}
+
+// an RGBA8 video frame of record b
+static int check_rgba_record(ht_ctx *ctx, const ht_video_frame &f, int b) {
+  if (!f.rgba) return ctx->fail(HT_ERR_ARG, "record %d: rgba is NULL", b);
+  if (reinterpret_cast<uintptr_t>(f.rgba) & 3u) return ctx->fail(HT_ERR_ARG, "record %d: rgba must be 4-byte aligned", b);
+  if (f.width <= 0 || f.height <= 0 || f.width > 16384 || f.height > 16384)
+    return ctx->fail(HT_ERR_SIZE, "record %d: video %dx%d outside 1..16384", b, f.width, f.height);
+  if ((f.pitch & 3) || (f.pitch != 0 && f.pitch < 4 * f.width))
+    return ctx->fail(HT_ERR_ARG, "record %d: pitch %d is not a multiple of 4 >= 4*width", b, f.pitch);
+  return HT_OK;
+}
+
 // ht_tracker_feed(_canvases).  Everything is checked before anything is enqueued (one_canvas: every record is on the
 // same canvas and the canvas errors are ht_tracker_feed's, without a record index).  The records are grouped by canvas
 // size - groups in order of first appearance, records in order within a group - and batch entry k is the k-th record
@@ -2315,9 +2386,10 @@ static int stage_yuv(ht_ctx *ctx, const ht_yuv_image &v, YuvFeedRec &r, uint8_t 
 // uniform batch.
 //
 // YUV records (ht_tracker_feed_yuv: frames NULL, yuv the records) take the same path; each is resolved into a
-// YuvFeedRec, host planes are packed plane by plane, and tracker_tick draws them with k_feed_draw_yuv.
-static int tracker_feed(ht_ctx *ctx, const ht_canvas_frame *frames, const ht_yuv_frame *yuv, int n, int frames_on_device,
-                        bool one_canvas, ht_tracker_event *out) {
+// YuvFeedRec, host planes are packed plane by plane, and tracker_tick draws them with k_feed_draw_yuv.  With views
+// (ht_tracker_feed(_yuv)_views) every record, RGBA8 or YUV, becomes a ViewFeedRec drawn by k_feed_draw_view.
+static int tracker_feed(ht_ctx *ctx, const ht_canvas_frame *frames, const ht_yuv_frame *yuv, const ht_video_view *views,
+                        int n, int frames_on_device, bool one_canvas, ht_tracker_event *out) {
   if (!ctx) return HT_ERR_ARG;
   if (!ctx->tracker_on) return ctx->fail(HT_ERR_STATE, "ht_tracker_config has not been called");
   if ((!frames && !yuv) || !out) return ctx->fail(HT_ERR_ARG, "frames or out is NULL");
@@ -2329,6 +2401,7 @@ static int tracker_feed(ht_ctx *ctx, const ht_canvas_frame *frames, const ht_yuv
   };
   std::vector<uint8_t> seen((size_t)mf, 0);
   std::vector<YuvFeedRec> yrec(yuv ? (size_t)n : 0);
+  std::vector<ViewFeedRec> vrec(views ? (size_t)n : 0);
   for (int b = 0; b < n; ++b) {
     const int s = stream_of(b);
     if (s < 0 || s >= mf) return ctx->fail(HT_ERR_ARG, "record %d: stream %d outside [0,%d)", b, s, mf);
@@ -2336,15 +2409,15 @@ static int tracker_feed(ht_ctx *ctx, const ht_canvas_frame *frames, const ht_yuv
     if (yuv) {
       const int rc = check_yuv_record(ctx, yuv[b].video, b, yrec[(size_t)b]);
       if (rc != HT_OK) return rc;
-      continue;
+    } else {
+      const int rc = check_rgba_record(ctx, frames[b].video, b);
+      if (rc != HT_OK) return rc;
     }
-    const ht_video_frame &f = frames[b].video;
-    if (!f.rgba) return ctx->fail(HT_ERR_ARG, "record %d: rgba is NULL", b);
-    if (reinterpret_cast<uintptr_t>(f.rgba) & 3u) return ctx->fail(HT_ERR_ARG, "record %d: rgba must be 4-byte aligned", b);
-    if (f.width <= 0 || f.height <= 0 || f.width > 16384 || f.height > 16384)
-      return ctx->fail(HT_ERR_SIZE, "record %d: video %dx%d outside 1..16384", b, f.width, f.height);
-    if ((f.pitch & 3) || (f.pitch != 0 && f.pitch < 4 * f.width))
-      return ctx->fail(HT_ERR_ARG, "record %d: pitch %d is not a multiple of 4 >= 4*width", b, f.pitch);
+    if (views) {
+      const int vw = yuv ? yuv[b].video.width : frames[b].video.width, vh = yuv ? yuv[b].video.height : frames[b].video.height;
+      const int rc = check_view(ctx, views[b], vw, vh, b, vrec[(size_t)b]);
+      if (rc != HT_OK) return rc;
+    }
   }
   struct Group { int w, h, first, n; IngestGeom g; Plan *P; TickGroup tick; size_t base; };
   std::vector<Group> groups;
@@ -2417,8 +2490,9 @@ static int tracker_feed(ht_ctx *ctx, const ht_canvas_frame *frames, const ht_yuv
     return off[3] + 4 * (m + 1);
   };
   static_assert(sizeof(YuvFeedRec) % 8 == 0 && sizeof(YuvFeedRec) >= sizeof(FeedRec), "YuvFeedRec layout");
+  static_assert(sizeof(ViewFeedRec) >= sizeof(YuvFeedRec), "ViewFeedRec layout");
   size_t off[4];
-  const size_t table_cap = table_offsets((size_t)mf, sizeof(YuvFeedRec), off);
+  const size_t table_cap = table_offsets((size_t)mf, sizeof(ViewFeedRec), off);
   if (!ctx->h_feed_table) {
     CK(cudaMallocHost(&ctx->h_feed_table.h, table_cap));
     CK(cudaEventCreateWithFlags(&ctx->feed_copied.h, cudaEventDisableTiming));
@@ -2428,13 +2502,15 @@ static int tracker_feed(ht_ctx *ctx, const ht_canvas_frame *frames, const ht_yuv
     CK(cudaEventSynchronize(ctx->feed_copied));           // the previous call's upload may still read the table
   }
   const bool mixed = n_groups > 1;
-  const size_t table_full = table_offsets((size_t)n, yuv ? sizeof(YuvFeedRec) : sizeof(FeedRec), off);
+  const size_t rec_bytes = views ? sizeof(ViewFeedRec) : yuv ? sizeof(YuvFeedRec) : sizeof(FeedRec);
+  const size_t table_full = table_offsets((size_t)n, rec_bytes, off);
   const size_t table_bytes = mixed ? table_full : off[2];
   uint8_t *tab = static_cast<uint8_t *>(ctx->h_feed_table.h);
   int32_t *ids = reinterpret_cast<int32_t *>(tab);
   double *now = reinterpret_cast<double *>(tab + off[0]);
   FeedRec *recs = reinterpret_cast<FeedRec *>(tab + off[1]);
   YuvFeedRec *yrecs = reinterpret_cast<YuvFeedRec *>(tab + off[1]);
+  ViewFeedRec *vrecs = reinterpret_cast<ViewFeedRec *>(tab + off[1]);
   EntryCanvas *geo = reinterpret_cast<EntryCanvas *>(tab + off[2]);
   int32_t *tile_start = reinterpret_cast<int32_t *>(tab + off[3]);
   size_t video_bytes = 0;
@@ -2464,7 +2540,12 @@ static int tracker_feed(ht_ctx *ctx, const ht_canvas_frame *frames, const ht_yuv
         if (rc != HT_OK) return rc;
         voff += yuv_staged_bytes(r);
       }
-      yrecs[e] = r;
+      if (views) {
+        vrecs[e] = vrec[(size_t)b];
+        view_source_yuv(vrecs[e], r);
+      } else {
+        yrecs[e] = r;
+      }
     } else {
       const ht_video_frame &f = frames[b].video;
       ids[e] = f.stream;
@@ -2478,7 +2559,12 @@ static int tracker_feed(ht_ctx *ctx, const ht_canvas_frame *frames, const ht_yuv
         r.pitch = 4 * f.width;
         voff += align_up<size_t>((size_t)f.width * f.height * 4, 256);
       }
-      recs[e] = r;
+      if (views) {
+        vrecs[e] = vrec[(size_t)b];
+        view_source_rgba(vrecs[e], r.src, r.pitch, r.width, r.height);
+      } else {
+        recs[e] = r;
+      }
     }
     if (mixed) {
       const int j = e - G.tick.k0;
@@ -2497,9 +2583,10 @@ static int tracker_feed(ht_ctx *ctx, const ht_canvas_frame *frames, const ht_yuv
     ticks[(size_t)i] = groups[(size_t)i].tick;
     ticks[(size_t)i].frames = arena + groups[(size_t)i].base;
   }
-  const FeedDraw feed{yuv ? nullptr : reinterpret_cast<const FeedRec *>(dtab + off[1]), ctx->d_feed_draw.as<uint8_t>(),
+  const FeedDraw feed{yuv || views ? nullptr : reinterpret_cast<const FeedRec *>(dtab + off[1]), ctx->d_feed_draw.as<uint8_t>(),
                       groups[0].g, mixed ? reinterpret_cast<const int32_t *>(dtab + off[3]) : nullptr, t0,
-                      yuv ? reinterpret_cast<const YuvFeedRec *>(dtab + off[1]) : nullptr};
+                      yuv && !views ? reinterpret_cast<const YuvFeedRec *>(dtab + off[1]) : nullptr,
+                      views ? reinterpret_cast<const ViewFeedRec *>(dtab + off[1]) : nullptr};
   return tracker_tick(ctx, ticks.data(), n_groups, arena, n, reinterpret_cast<const int32_t *>(dtab), 0.0,
                       reinterpret_cast<const double *>(dtab + off[0]), &feed,
                       mixed ? reinterpret_cast<const EntryCanvas *>(dtab + off[2]) : nullptr, out);
@@ -2513,15 +2600,29 @@ int ht_tracker_feed(ht_ctx *ctx, const ht_video_frame *frames, int n, int frames
   if (n <= 0 || n > ctx->cfg.max_frames) return ctx->fail(HT_ERR_ARG, "n=%d outside [1,%d]", n, ctx->cfg.max_frames);
   std::vector<ht_canvas_frame> recs((size_t)n);
   for (int b = 0; b < n; ++b) recs[(size_t)b] = ht_canvas_frame{frames[b], canvas_w, canvas_h, {0, 0}};
-  return tracker_feed(ctx, recs.data(), nullptr, n, frames_on_device, true, out);
+  return tracker_feed(ctx, recs.data(), nullptr, nullptr, n, frames_on_device, true, out);
 }
 
 int ht_tracker_feed_canvases(ht_ctx *ctx, const ht_canvas_frame *frames, int n, int frames_on_device, ht_tracker_event *out) {
-  return tracker_feed(ctx, frames, nullptr, n, frames_on_device, false, out);
+  return tracker_feed(ctx, frames, nullptr, nullptr, n, frames_on_device, false, out);
 }
 
 int ht_tracker_feed_yuv(ht_ctx *ctx, const ht_yuv_frame *frames, int n, int frames_on_device, ht_tracker_event *out) {
-  return tracker_feed(ctx, nullptr, frames, n, frames_on_device, false, out);
+  return tracker_feed(ctx, nullptr, frames, nullptr, n, frames_on_device, false, out);
+}
+
+int ht_tracker_feed_views(ht_ctx *ctx, const ht_canvas_frame *frames, const ht_video_view *views, int n,
+                          int frames_on_device, ht_tracker_event *out) {
+  if (!ctx) return HT_ERR_ARG;
+  if (!views) return ctx->fail(HT_ERR_ARG, "views is NULL");
+  return tracker_feed(ctx, frames, nullptr, views, n, frames_on_device, false, out);
+}
+
+int ht_tracker_feed_yuv_views(ht_ctx *ctx, const ht_yuv_frame *frames, const ht_video_view *views, int n,
+                              int frames_on_device, ht_tracker_event *out) {
+  if (!ctx) return HT_ERR_ARG;
+  if (!views) return ctx->fail(HT_ERR_ARG, "views is NULL");
+  return tracker_feed(ctx, nullptr, frames, views, n, frames_on_device, false, out);
 }
 
 // canvasContext.drawImage(video, 0, 0, canvas.width, canvas.height) for n frames (src/main.js:170)
@@ -2598,6 +2699,92 @@ int ht_ingest_yuv(ht_ctx *ctx, const ht_yuv_image *src, int n, int frames_on_dev
   ++ctx->launches;
   CK(cudaGetLastError());
   return io.finish(Outputs::SYNC_STREAM);
+}
+
+// ht_ingest(_yuv)_views: k_feed_draw_view over n records (RGBA8 frames, or YUV images), every one drawn, canvas i at
+// dst + i * dw * dh * 4
+static int ingest_views(ht_ctx *ctx, const ht_video_frame *rgba, const ht_yuv_image *yuv, const ht_video_view *views,
+                        int n, int frames_on_device, uint8_t *dst_rgba, int dw, int dh) {
+  if (!ctx) return HT_ERR_ARG;
+  if ((!rgba && !yuv) || !views || !dst_rgba) return ctx->fail(HT_ERR_ARG, "src, views or dst_rgba is NULL");
+  if (n <= 0 || n > 65535) return ctx->fail(HT_ERR_ARG, "n=%d outside [1,65535]", n);   // (grid y)
+  if (reinterpret_cast<uintptr_t>(dst_rgba) & 3u) return ctx->fail(HT_ERR_ARG, "dst_rgba must be 4-byte aligned");
+  if (dw <= 0 || dh <= 0 || dw > 16384 || dh > 16384) return ctx->fail(HT_ERR_SIZE, "canvas %dx%d outside 1..16384", dw, dh);
+  IngestGeom g;
+  if (!canvas_geom(dw, dh, g)) return ctx->fail(HT_ERR_SIZE, "canvas too large for 32-bit bilinear numerators");
+  std::vector<ViewFeedRec> recs((size_t)n);
+  std::vector<YuvFeedRec> yrec(yuv ? (size_t)n : 0);
+  size_t video_bytes = 0;
+  for (int b = 0; b < n; ++b) {
+    int rc, w, h;
+    if (yuv) {
+      rc = check_yuv_record(ctx, yuv[b], b, yrec[(size_t)b]);
+      w = yuv[b].width, h = yuv[b].height;
+      if (rc == HT_OK) video_bytes += yuv_staged_bytes(yrec[(size_t)b]);
+    } else {
+      rc = check_rgba_record(ctx, rgba[b], b);
+      w = rgba[b].width, h = rgba[b].height;
+      video_bytes += align_up<size_t>((size_t)w * h * 4, 256);
+    }
+    if (rc != HT_OK) return rc;
+    rc = check_view(ctx, views[b], w, h, b, recs[(size_t)b]);
+    if (rc != HT_OK) return rc;
+  }
+  if (is_device_ptr(yuv ? yuv[0].planes[0] : rgba[0].rgba) != (frames_on_device != 0))
+    return ctx->fail(HT_ERR_ARG, "the frames are %s memory, frames_on_device says otherwise", frames_on_device ? "host" : "device");
+  { const int jr = join_aux(ctx); if (jr != HT_OK) return jr; }
+  CK(cudaSetDevice(ctx->cfg.device));
+  cudaStream_t st = ctx->stream;
+  if (!frames_on_device) CK(ctx->d_frames.reserve(video_bytes));
+  size_t voff = 0;
+  for (int b = 0; b < n; ++b) {
+    if (yuv) {
+      YuvFeedRec r = yrec[(size_t)b];
+      if (!frames_on_device) {
+        const int rc = stage_yuv(ctx, yuv[b], r, ctx->d_frames.as<uint8_t>() + voff);
+        if (rc != HT_OK) return rc;
+        voff += yuv_staged_bytes(r);
+      }
+      view_source_yuv(recs[(size_t)b], r);
+      continue;
+    }
+    const ht_video_frame &f = rgba[b];
+    const uint8_t *src = f.rgba;
+    int pitch = f.pitch ? f.pitch : 4 * f.width;
+    if (!frames_on_device) {
+      uint8_t *dst = ctx->d_frames.as<uint8_t>() + voff;
+      CK(cudaMemcpy2DAsync(dst, 4 * (size_t)f.width, f.rgba, (size_t)pitch, 4 * (size_t)f.width, (size_t)f.height,
+                           cudaMemcpyHostToDevice, st));
+      src = dst, pitch = 4 * f.width;
+      voff += align_up<size_t>((size_t)f.width * f.height * 4, 256);
+    }
+    view_source_rgba(recs[(size_t)b], src, pitch, f.width, f.height);
+  }
+  CK(ctx->d_ingest_recs.reserve(sizeof(ViewFeedRec) * (size_t)n));
+  // pageable source: the copy is staged before it returns, so `recs` may go out of scope
+  CK(cudaMemcpyAsync(ctx->d_ingest_recs.p, recs.data(), sizeof(ViewFeedRec) * (size_t)n, cudaMemcpyHostToDevice, st));
+  const size_t dbytes = (size_t)n * dw * dh * 4;
+  Outputs io(ctx);
+  const int o_dst = io.add(dst_rgba, ctx->d_scratch, dbytes);
+  if (!io.on_device()) CK(ctx->d_scratch.reserve(dbytes));
+  const int tiles_x = (dw + 63) / 64, tiles = tiles_x * ((dh + 15) / 16);
+  k_feed_draw_view<<<dim3((unsigned)tiles, (unsigned)n), 256, 0, st>>>(ctx->d_ingest_recs.as<ViewFeedRec>(), nullptr,
+                                                                       io.dst<uint8_t>(o_dst), g, tiles_x, nullptr, nullptr, n);
+  ++ctx->launches;
+  CK(cudaGetLastError());
+  return io.finish(Outputs::SYNC_STREAM);
+}
+
+int ht_ingest_views(ht_ctx *ctx, const ht_video_frame *src, const ht_video_view *views, int n, int frames_on_device,
+                    uint8_t *dst_rgba, int dw, int dh) {
+  if (!src && ctx) return ctx->fail(HT_ERR_ARG, "src is NULL");
+  return ingest_views(ctx, src, nullptr, views, n, frames_on_device, dst_rgba, dw, dh);
+}
+
+int ht_ingest_yuv_views(ht_ctx *ctx, const ht_yuv_image *src, const ht_video_view *views, int n, int frames_on_device,
+                        uint8_t *dst_rgba, int dw, int dh) {
+  if (!src && ctx) return ctx->fail(HT_ERR_ARG, "src is NULL");
+  return ingest_views(ctx, nullptr, src, views, n, frames_on_device, dst_rgba, dw, dh);
 }
 
 int ht_backprojection(ht_ctx *ctx, int slot, const uint8_t *rgba, int w, int h, uint8_t *out_rgba) {
@@ -2989,6 +3176,40 @@ extern "C" int ht_selftest_feed_yuv(const ht_yuv_image *img, uint8_t *canvas, in
     }
   }
   return 0;
+}
+
+// k_feed_draw_view's per-record code: view record v (map and texel source resolved) onto a dw x dh canvas
+static int selftest_view_draw(const ViewFeedRec &v, uint8_t *canvas, int dw, int dh) {
+  IngestGeom g;
+  if (dw <= 0 || dh <= 0 || !canvas_geom(dw, dh, g)) return HT_ERR_SIZE;
+  uint32_t *out = reinterpret_cast<uint32_t *>(canvas);
+  for (int Y = 0; Y < dh; ++Y)
+    for (int X = 0; X < dw; ++X)
+      out[(size_t)Y * dw + X] = v.kind == VIEW_RGBA        ? view_pixel<VIEW_RGBA>(v, g, X, Y)
+                                : v.kind == VIEW_NV12_I420 ? view_pixel<VIEW_NV12_I420>(v, g, X, Y)
+                                                           : view_pixel<VIEW_FMT>(v, g, X, Y);
+  return 0;
+}
+// one image of any format (host planes) drawn through a view onto a dw x dh canvas -> 0, or the rejection's code
+extern "C" int ht_selftest_feed_view(const ht_yuv_image *img, const ht_video_view *view, uint8_t *canvas, int dw, int dh) {
+  YuvFeedRec r;
+  ViewFeedRec v;
+  char why[256];
+  int rc = yuv_record(*img, r, why);
+  if (rc == HT_OK) rc = view_record(*view, img->width, img->height, v, why);
+  if (rc != HT_OK) return rc;
+  view_source_yuv(v, r);
+  return selftest_view_draw(v, canvas, dw, dh);
+}
+// the RGBA8 twin: a frame of rows of `pitch` bytes (0: 4 * width)
+extern "C" int ht_selftest_feed_view_rgba(const ht_video_frame *f, const ht_video_view *view, uint8_t *canvas, int dw, int dh) {
+  ViewFeedRec v;
+  char why[256];
+  if (!f->rgba || f->width <= 0 || f->height <= 0 || (f->pitch & 3) || (f->pitch && f->pitch < 4 * f->width)) return HT_ERR_ARG;
+  const int rc = view_record(*view, f->width, f->height, v, why);
+  if (rc != HT_OK) return rc;
+  view_source_rgba(v, f->rgba, f->pitch ? f->pitch : 4 * f->width, f->width, f->height);
+  return selftest_view_draw(v, canvas, dw, dh);
 }
 
 // k_ingest's per-pixel code over a whole frame batch

@@ -599,6 +599,83 @@ __global__ void __launch_bounds__(256) k_feed_draw_yuv(const YuvFeedRec *__restr
   }
 }
 
+// ht_tracker_feed_views / ht_tracker_feed_yuv_views / ht_ingest_views / ht_ingest_yuv_views: a video drawn through a
+// view (DESIGN.md 2, "Views"), drawImage(O, sx, sy, sw, sh, 0, 0, dw, dh) of the oriented frame O.  The host resolves
+// the view into an integer map: tap (x, y) of the source rectangle (0 <= x < sw, 0 <= y < sh; bilinear_pixel clamps
+// the taps to it) is video pixel (bx + mxx x + mxy y, by + myx x + myy y), a 2x2 signed permutation plus an offset, so
+// no tap branches on the orientation.  src is the video as k_feed_draw_yuv takes it; a VIEW_RGBA record has its RGBA8
+// pixels at src.y, rows of src.ypitch bytes (the other fields unused).
+enum : int32_t { VIEW_RGBA = 0, VIEW_NV12_I420 = 1, VIEW_FMT = 2 };
+struct ViewFeedRec {
+  YuvFeedRec src;
+  int32_t bx, by, mxx, mxy, myx, myy;
+  int32_t sw, sh;                   // the source rectangle's size
+  int32_t kind;                     // VIEW_RGBA, VIEW_NV12_I420 (nv12_i420_path) or VIEW_FMT (every other format)
+  int32_t pad_;
+};
+// RGBA8 pixel (x, y) of the video of a record of kind KIND
+template <int KIND>
+__host__ __device__ __forceinline__ uint32_t view_texel(const YuvFeedRec &r, int x, int y) {
+  if (KIND == VIEW_RGBA) return ld_ro(reinterpret_cast<const uint32_t *>(r.y + (size_t)y * r.ypitch) + x);
+  if (KIND == VIEW_NV12_I420) return yuv_texel(r, x, y);
+  return fmt_texel(r, x, y);
+}
+// canvas pixel (X, Y) of view record v on the canvas of g: the resampler over the source rectangle through the map (a
+// 1:1 draw is a copy of the rectangle); also run on the host by ht_selftest_feed_view(_rgba)
+template <int KIND>
+__host__ __device__ __forceinline__ uint32_t view_pixel(const ViewFeedRec &v, const IngestGeom &g, int X, int Y) {
+  auto tap = [&](int x, int y) {
+    return view_texel<KIND>(v.src, v.bx + v.mxx * x + v.mxy * y, v.by + v.myx * x + v.myy * y);
+  };
+  return (v.sw == g.dw && v.sh == g.dh) ? tap(X, Y) : bilinear_pixel(tap, v.sw, v.sh, g, X, Y);
+}
+// k_feed_draw_view's CTA: the 64 x 16 tile from (X0, Y0) of canvas cv (g), 4 pixels per thread stored in 16 bytes.
+// Upright views (mxx != 0) give a warp 2 rows of 64 pixels.  Transposed views (90 / 270: canvas rows run down video
+// columns, canvas columns along video rows) give a warp 16 rows of 8 pixels instead: its 16 threads of one column
+// read 16 adjacent pixels of one video row per tap, and its stores still fill whole 32-byte sectors of 16 canvas rows.
+template <int KIND>
+__device__ __forceinline__ void view_cta(const ViewFeedRec &v, uint8_t *__restrict__ cv, const IngestGeom &g, int X0, int Y0) {
+  const int t = threadIdx.x;
+  const bool transposed = v.mxx == 0;
+  const int X = X0 + 4 * (transposed ? t >> 4 : t & 15), Y = Y0 + (transposed ? t & 15 : t >> 4);
+  if (X >= g.dw || Y >= g.dh) return;
+  uint32_t px[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) px[i] = X + i < g.dw ? view_pixel<KIND>(v, g, X + i, Y) : 0u;
+  uint32_t *row = reinterpret_cast<uint32_t *>(cv + (size_t)Y * g.dw * 4) + X;
+  if ((g.dw & 3) == 0 && aligned_to(cv, 16)) {
+    *reinterpret_cast<uint4 *>(row) = make_uint4(px[0], px[1], px[2], px[3]);
+  } else {
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+      if (X + i < g.dw) row[i] = px[i];
+  }
+}
+// the CTA of a record of kind KIND, out of line: each texel source keeps its own registers (as feed_draw_fmt does for
+// k_feed_draw_yuv), and the kernel itself holds nothing across the call
+template <int KIND>
+__device__ __noinline__ void feed_draw_view(const ViewFeedRec *__restrict__ rp, uint8_t *__restrict__ cv, const IngestGeom g,
+                                            int X0, int Y0) {
+  const ViewFeedRec v = *rp;
+  view_cta<KIND>(v, cv, g, X0, Y0);
+}
+// k_feed_draw / k_feed_draw_yuv through views: the same tiles, grid and draw flags (draw == NULL: every record, for
+// ht_ingest(_yuv)_views).  A CTA draws one record, so the texel source is uniform across it.
+__global__ void __launch_bounds__(256) k_feed_draw_view(const ViewFeedRec *__restrict__ recs, const uint8_t *__restrict__ draw,
+                                                        uint8_t *__restrict__ canvas, IngestGeom g, int tiles_x,
+                                                        const EntryCanvas *__restrict__ geo,
+                                                        const int32_t *__restrict__ tile_start, int n) {
+  int b, tile;
+  uint8_t *cv;
+  feed_cta(canvas, g, tiles_x, geo, tile_start, n, b, tile, cv);
+  const int kind = recs[b].kind;
+  if (draw && !draw[b]) return;
+  const int X0 = (tile % tiles_x) * 64, Y0 = (tile / tiles_x) * 16;
+  if (kind == VIEW_RGBA) feed_draw_view<VIEW_RGBA>(recs + b, cv, g, X0, Y0);
+  else if (kind == VIEW_NV12_I420) feed_draw_view<VIEW_NV12_I420>(recs + b, cv, g, X0, Y0);
+  else feed_draw_view<VIEW_FMT>(recs + b, cv, g, X0, Y0);
+}
+
 // ------------------------------------------------------------------------------------------------
 // K2  pyramid level = canvas-shim drawImage (exact integer bilinear, see oracle/ht_oracle.h and
 // src/ccv.js:121,128,135,140,145).  One launch per pyramid "generation" (levels whose sources are

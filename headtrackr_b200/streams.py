@@ -218,23 +218,36 @@ class TrackerSet:
         self._dispatch(range(len(recs)), recs, int((time.time() - t0) * 1000))
         return recs
 
-    def feed(self, frames, now_ms=None, width=None, height=None):
+    def feed(self, frames, now_ms=None, width=None, height=None, view=None):
         """One timer tick of the listed streams only (ht_tracker_feed): frames = {stream: (h, w, 4) u8 video frame}
         (numpy or torch CUDA, any video size), drawn onto a width x height canvas; now_ms = None (the wall clock), one
         clock, or {stream: ms}; width and height: one canvas size for all, or {stream: pixels} (each stream on its own
-        canvas, ht_tracker_feed_canvases).  Streams not listed do not tick.  -> {stream: record}."""
-        return self._feed(frames, now_ms, width, height, self.ctx.tracker_feed)
+        canvas, ht_tracker_feed_canvases).  view: None, one view for all (headtrackr_b200.views), or {stream: view}
+        (ht_tracker_feed_views).  Streams not listed do not tick.  -> {stream: record}."""
+        views = self._views(frames, view)
 
-    def feed_yuv(self, frames, now_ms=None, width=None, height=None, format="nv12", color="bt601"):
+        def call(ks, vids, now, width, height, out=None):
+            return self.ctx.tracker_feed(ks, vids, now, width, height, out=out, view=views)
+        return self._feed(frames, now_ms, width, height, call)
+
+    @staticmethod
+    def _views(frames, view):
+        """view= of feed / feed_yuv -> Context's (None, one view, or a list in the order of frames)"""
+        if isinstance(view, dict) and view and all(isinstance(k, int) for k in view):
+            return [view[k] for k in frames]
+        return view
+
+    def feed_yuv(self, frames, now_ms=None, width=None, height=None, format="nv12", color="bt601", view=None):
         """feed on video in any of _lib.YUV_FORMATS (ht_tracker_feed_yuv): frames = {stream: planes or packed array}
-        (Context.tracker_feed_yuv), format and color one for all or {stream: value}; the rest as for feed, and events
-        are dispatched as feed dispatches them."""
+        (Context.tracker_feed_yuv), format and color one for all or {stream: value}; the rest (view included) as for
+        feed, and events are dispatched as feed dispatches them."""
         ks = list(frames)
+        views = self._views(frames, view)
         fmts = [format[k] for k in ks] if isinstance(format, dict) else format
         colors = [color[k] for k in ks] if isinstance(color, dict) else color
 
         def call(ks, vids, now, width, height, out=None):
-            return self.ctx.tracker_feed_yuv(ks, vids, now, width, height, format=fmts, color=colors, out=out)
+            return self.ctx.tracker_feed_yuv(ks, vids, now, width, height, format=fmts, color=colors, out=out, view=views)
         return self._feed(frames, now_ms, width, height, call)
 
     def _feed(self, frames, now_ms, width, height, tick):

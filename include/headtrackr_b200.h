@@ -394,6 +394,46 @@ int ht_tracker_feed_yuv(ht_ctx *ctx, const ht_yuv_frame *frames, int n, int fram
  * resampler. */
 int ht_ingest_yuv(ht_ctx *ctx, const ht_yuv_image *src, int n, int frames_on_device, uint8_t *dst_rgba, int dw, int dh);
 
+/* A view of a video frame (DESIGN.md 2, "Views"): an orientation, then a source rectangle of the oriented frame.
+ * orientation & 3 rotates the w x h video V clockwise by 0, 90, 180 or 270 degrees, and HT_VIEW_MIRROR then mirrors
+ * the rotated frame horizontally.  The oriented frame O is w x h (0, 180) or h x w (90, 270), and its pixel (x, y) is
+ * V(x, y), V(y, h-1-x), V(w-1-x, h-1-y) or V(w-1-y, x) for 0, 90, 180, 270; with the mirror bit, O(W'-1-x, y) of that.
+ * For YUV formats the orientation maps luma coordinates and chroma is looked up as the format says, so a rotated
+ * frame is the rotation of its converted RGBA8 frame.  (sx, sy, sw, sh) is a rectangle of O, all 0 for the whole of
+ * it, otherwise sw, sh >= 1, sx, sy >= 0, sx + sw <= W' and sy + sh <= H'.  The canvas is then drawImage(O, sx, sy, sw,
+ * sh, 0, 0, canvas_w, canvas_h): taps are clamped to the rectangle, and an sw x sh rectangle on an sw x sh canvas is
+ * copied.  EXIF orientations 1..8 are views 0, 4, 2, 6, 5, 1, 7, 3; a rotation r (clockwise, applied first) with a
+ * horizontal flip is r / 90 | HT_VIEW_MIRROR.  Events, debug canvases and cameras stay in canvas coordinates. */
+#define HT_VIEW_ROTATE_90 1
+#define HT_VIEW_ROTATE_180 2
+#define HT_VIEW_ROTATE_270 3
+#define HT_VIEW_MIRROR 4
+typedef struct {
+  int32_t orientation;          /* 0..7 */
+  int32_t sx, sy, sw, sh;       /* in the oriented frame; all 0 = the whole frame */
+  int32_t reserved[3];          /* must be 0 */
+} ht_video_view;                /* 32 bytes */
+/* ht_tracker_feed_canvases with a view per record: record i's video is drawn through views[i].  The contract is
+ * ht_tracker_feed_canvases's (any subset of streams, canvases of any size, host or device video, out[n] in record
+ * order, the same launches); several records may point into the same device frame.  A record with the identity view
+ * (orientation 0, whole frame) gives exactly the canvas and event of ht_tracker_feed_canvases.
+ * Errors (nothing is enqueued): those of ht_tracker_feed_canvases, and HT_ERR_ARG for views == NULL and, with the
+ * record's index in ht_last_error, for an orientation outside 0..7, a non-zero reserved field, or a rectangle that is
+ * not (0, 0, 0, 0) and is empty or not inside the oriented frame. */
+int ht_tracker_feed_views(ht_ctx *ctx, const ht_canvas_frame *frames, const ht_video_view *views, int n,
+                          int frames_on_device, ht_tracker_event *out);
+/* ht_tracker_feed_yuv with a view per record, as ht_tracker_feed_views is to ht_tracker_feed_canvases. */
+int ht_tracker_feed_yuv_views(ht_ctx *ctx, const ht_yuv_frame *frames, const ht_video_view *views, int n,
+                              int frames_on_device, ht_tracker_event *out);
+/* ht_ingest through views: src[i] (an RGBA8 frame; its stream and now_ms are ignored) drawn through views[i] onto the
+ * i-th tightly packed dw x dh canvas of dst_rgba.  The frames may differ in size.  One launch.  Errors: those of
+ * ht_ingest_yuv, for RGBA8 records those of ht_tracker_feed's, and the view errors of ht_tracker_feed_views. */
+int ht_ingest_views(ht_ctx *ctx, const ht_video_frame *src, const ht_video_view *views, int n, int frames_on_device,
+                    uint8_t *dst_rgba, int dw, int dh);
+/* ht_ingest_yuv through views, as ht_ingest_views. */
+int ht_ingest_yuv_views(ht_ctx *ctx, const ht_yuv_image *src, const ht_video_view *views, int n, int frames_on_device,
+                        uint8_t *dst_rgba, int dw, int dh);
+
 /* A stream's debug canvas: `params.debug` of its headtrackr.Tracker (src/main.js:42-50). */
 typedef struct {
   uint8_t *rgba;          /* DEVICE memory, `height` rows of `pitch` bytes; NULL: the stream has no debug canvas */

@@ -34,6 +34,8 @@
 //   trackerFeedYuv(handle, [{stream, nowMs, canvasWidth, canvasHeight, format, color, width, height, y, uv | u, v}])
 //        -> Array<record> (ht_tracker_feed_yuv: NV12 / I420 host planes, tight pitches)
 //   ingestYuv(handle, [{format, color, width, height, y, uv | u, v}], dw, dh) -> Uint8ClampedArray   (ht_ingest_yuv)
+//   trackerFeedViews / trackerFeedYuvViews / ingestYuvViews: the same records with a "view" each, {rotate, mirror,
+//     crop: [x, y, w, h]}; ingestViews(handle, [{width, height, rgba, view}], dw, dh)   (ht_*_views)
 //   destroy(handle)
 #include <node_api.h>
 
@@ -622,7 +624,39 @@ static napi_value TrackerStep(napi_env env, napi_callback_info info) {
 // trackerFeed(handle, [{stream, rgba, width, height, nowMs, canvasWidth?, canvasHeight?}], canvasWidth, canvasHeight)
 // -> Array<record>, in record order (ht_tracker_feed_canvases with host frames: one tick of each listed stream on its
 // own video, clock and canvas; a record without its own canvas size uses the call's)
-static napi_value TrackerFeed(napi_env env, napi_callback_info info) {
+// a record's optional "view": {rotate: 0 | 90 | 180 | 270, mirror: bool, crop: [x, y, w, h] of the oriented frame}
+// -> an ht_video_view (absent: the identity view); false for a bad object
+static bool ViewOf(napi_env env, napi_value r, ht_video_view *view) {
+  std::memset(view, 0, sizeof(*view));
+  bool has = false;
+  napi_value v, c;
+  if (napi_has_named_property(env, r, "view", &has) != napi_ok || !has) return true;
+  if (napi_get_named_property(env, r, "view", &v) != napi_ok) return false;
+  const int rotate = (int)GetNumProp(env, v, "rotate", 0);
+  if (rotate != 0 && rotate != 90 && rotate != 180 && rotate != 270) return false;
+  bool mirror = false;
+  napi_value m;
+  if (napi_has_named_property(env, v, "mirror", &has) == napi_ok && has && napi_get_named_property(env, v, "mirror", &m) == napi_ok)
+    napi_get_value_bool(env, m, &mirror);
+  view->orientation = rotate / 90 | (mirror ? HT_VIEW_MIRROR : 0);
+  if (napi_has_named_property(env, v, "crop", &has) == napi_ok && has && napi_get_named_property(env, v, "crop", &c) == napi_ok) {
+    napi_valuetype t;
+    napi_typeof(env, c, &t);
+    if (t != napi_null && t != napi_undefined) {
+      uint32_t len = 0;
+      if (napi_get_array_length(env, c, &len) != napi_ok || len != 4) return false;
+      int32_t *dst[4] = {&view->sx, &view->sy, &view->sw, &view->sh};
+      for (uint32_t i = 0; i < 4; ++i) {
+        napi_value e;
+        if (napi_get_element(env, c, i, &e) != napi_ok || napi_get_value_int32(env, e, dst[i]) != napi_ok) return false;
+      }
+    }
+  }
+  return true;
+}
+
+// trackerFeed(handle, records, cw, ch), and with views (each record's "view", ViewOf) ht_tracker_feed_views
+static napi_value TrackerFeedAny(napi_env env, napi_callback_info info, bool with_views) {
   size_t argc = 4;
   napi_value argv[4];
   NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
@@ -633,10 +667,12 @@ static napi_value TrackerFeed(napi_env env, napi_callback_info info) {
   napi_get_value_int32(env, argv[2], &cw); napi_get_value_int32(env, argv[3], &ch);
   if (n == 0) return Throw(env, ctx, HT_ERR_ARG);
   std::vector<ht_canvas_frame> frames(n);
+  std::vector<ht_video_view> views(n);
   for (uint32_t b = 0; b < n; ++b) {
     napi_value r, v;
     NAPI_OK(napi_get_element(env, argv[1], b, &r));
     std::memset(&frames[b], 0, sizeof(frames[b]));
+    if (!ViewOf(env, r, &views[b])) return Throw(env, ctx, HT_ERR_ARG);
     frames[b].canvas_w = (int32_t)GetNumProp(env, r, "canvasWidth", cw);
     frames[b].canvas_h = (int32_t)GetNumProp(env, r, "canvasHeight", ch);
     ht_video_frame &f = frames[b].video;
@@ -650,13 +686,17 @@ static napi_value TrackerFeed(napi_env env, napi_callback_info info) {
     f.rgba = rgba;
   }
   std::vector<ht_tracker_event> ev(n);
-  int rc = ht_tracker_feed_canvases(ctx, frames.data(), (int)n, 0, ev.data());
+  int rc = with_views ? ht_tracker_feed_views(ctx, frames.data(), views.data(), (int)n, 0, ev.data())
+                      : ht_tracker_feed_canvases(ctx, frames.data(), (int)n, 0, ev.data());
   if (rc < 0) return Throw(env, ctx, rc);
   napi_value out;
   napi_create_array_with_length(env, (size_t)n, &out);
   for (uint32_t b = 0; b < n; ++b) napi_set_element(env, out, b, TrackerEventObject(env, ev[b]));
   return out;
 }
+
+static napi_value TrackerFeed(napi_env env, napi_callback_info info) { return TrackerFeedAny(env, info, false); }
+static napi_value TrackerFeedViews(napi_env env, napi_callback_info info) { return TrackerFeedAny(env, info, true); }
 
 // a video frame object {format, color, width, height, planes}: format "nv12" (the default), "i420", "nv21", "i422",
 // "i444", "yuyv", "uyvy", "p010", "bgra", "bgr24" or "rgb24"; color "bt601" (the default), "bt709", "bt2020", each
@@ -715,7 +755,7 @@ static bool YuvImageOf(napi_env env, napi_value r, ht_yuv_image *img) {
 
 // trackerFeedYuv(handle, [{stream, nowMs, canvasWidth, canvasHeight, ...a YUV frame object}]) -> Array<record>
 // (ht_tracker_feed_yuv with host planes)
-static napi_value TrackerFeedYuv(napi_env env, napi_callback_info info) {
+static napi_value TrackerFeedYuvAny(napi_env env, napi_callback_info info, bool with_views) {
   size_t argc = 2;
   napi_value argv[2];
   NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
@@ -724,18 +764,20 @@ static napi_value TrackerFeedYuv(napi_env env, napi_callback_info info) {
   NAPI_OK(napi_get_array_length(env, argv[1], &n));
   if (n == 0) return Throw(env, ctx, HT_ERR_ARG);
   std::vector<ht_yuv_frame> frames(n);
+  std::vector<ht_video_view> views(n);
   for (uint32_t b = 0; b < n; ++b) {
     napi_value r;
     NAPI_OK(napi_get_element(env, argv[1], b, &r));
     std::memset(&frames[b], 0, sizeof(frames[b]));
-    if (!YuvImageOf(env, r, &frames[b].video)) return Throw(env, ctx, HT_ERR_ARG);
+    if (!YuvImageOf(env, r, &frames[b].video) || !ViewOf(env, r, &views[b])) return Throw(env, ctx, HT_ERR_ARG);
     frames[b].stream = (int32_t)GetNumProp(env, r, "stream", -1);
     frames[b].canvas_w = (int32_t)GetNumProp(env, r, "canvasWidth", 0);
     frames[b].canvas_h = (int32_t)GetNumProp(env, r, "canvasHeight", 0);
     frames[b].now_ms = GetNumProp(env, r, "nowMs", 0.0);
   }
   std::vector<ht_tracker_event> ev(n);
-  int rc = ht_tracker_feed_yuv(ctx, frames.data(), (int)n, 0, ev.data());
+  int rc = with_views ? ht_tracker_feed_yuv_views(ctx, frames.data(), views.data(), (int)n, 0, ev.data())
+                      : ht_tracker_feed_yuv(ctx, frames.data(), (int)n, 0, ev.data());
   if (rc < 0) return Throw(env, ctx, rc);
   napi_value out;
   napi_create_array_with_length(env, (size_t)n, &out);
@@ -743,8 +785,12 @@ static napi_value TrackerFeedYuv(napi_env env, napi_callback_info info) {
   return out;
 }
 
-// ingestYuv(handle, [YUV frame object, ...], dw, dh) -> Uint8ClampedArray (n canvases)   (ht_ingest_yuv)
-static napi_value IngestYuv(napi_env env, napi_callback_info info) {
+static napi_value TrackerFeedYuv(napi_env env, napi_callback_info info) { return TrackerFeedYuvAny(env, info, false); }
+static napi_value TrackerFeedYuvViews(napi_env env, napi_callback_info info) { return TrackerFeedYuvAny(env, info, true); }
+
+// ingestYuv(handle, [YUV frame object, ...], dw, dh) -> Uint8ClampedArray (n canvases)   (ht_ingest_yuv); with views
+// (each object's "view", ViewOf) ht_ingest_yuv_views
+static napi_value IngestYuvAny(napi_env env, napi_callback_info info, bool with_views) {
   size_t argc = 4;
   napi_value argv[4];
   NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
@@ -755,14 +801,53 @@ static napi_value IngestYuv(napi_env env, napi_callback_info info) {
   napi_get_value_int32(env, argv[2], &dw); napi_get_value_int32(env, argv[3], &dh);
   if (n == 0 || dw <= 0 || dh <= 0) return Throw(env, ctx, HT_ERR_ARG);
   std::vector<ht_yuv_image> imgs(n);
+  std::vector<ht_video_view> views(n);
   for (uint32_t b = 0; b < n; ++b) {
     napi_value r;
     NAPI_OK(napi_get_element(env, argv[1], b, &r));
-    if (!YuvImageOf(env, r, &imgs[b])) return Throw(env, ctx, HT_ERR_ARG);
+    if (!YuvImageOf(env, r, &imgs[b]) || !ViewOf(env, r, &views[b])) return Throw(env, ctx, HT_ERR_ARG);
   }
   void *data; napi_value ab, ta;
   NAPI_OK(napi_create_arraybuffer(env, (size_t)n * dw * dh * 4, &data, &ab));
-  int rc = ht_ingest_yuv(ctx, imgs.data(), (int)n, 0, static_cast<uint8_t *>(data), dw, dh);
+  int rc = with_views ? ht_ingest_yuv_views(ctx, imgs.data(), views.data(), (int)n, 0, static_cast<uint8_t *>(data), dw, dh)
+                      : ht_ingest_yuv(ctx, imgs.data(), (int)n, 0, static_cast<uint8_t *>(data), dw, dh);
+  if (rc < 0) return Throw(env, ctx, rc);
+  NAPI_OK(napi_create_typedarray(env, napi_uint8_clamped_array, (size_t)n * dw * dh * 4, ab, 0, &ta));
+  return ta;
+}
+
+static napi_value IngestYuv(napi_env env, napi_callback_info info) { return IngestYuvAny(env, info, false); }
+static napi_value IngestYuvViews(napi_env env, napi_callback_info info) { return IngestYuvAny(env, info, true); }
+
+// ingestViews(handle, [{width, height, rgba, view}], dw, dh) -> Uint8ClampedArray (n canvases)   (ht_ingest_views)
+static napi_value IngestViews(napi_env env, napi_callback_info info) {
+  size_t argc = 4;
+  napi_value argv[4];
+  NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+  ht_ctx *ctx = Ctx(env, argv[0]);
+  uint32_t n = 0;
+  int32_t dw, dh;
+  NAPI_OK(napi_get_array_length(env, argv[1], &n));
+  napi_get_value_int32(env, argv[2], &dw); napi_get_value_int32(env, argv[3], &dh);
+  if (n == 0 || dw <= 0 || dh <= 0) return Throw(env, ctx, HT_ERR_ARG);
+  std::vector<ht_video_frame> frames(n);
+  std::vector<ht_video_view> views(n);
+  for (uint32_t b = 0; b < n; ++b) {
+    napi_value r, v;
+    NAPI_OK(napi_get_element(env, argv[1], b, &r));
+    std::memset(&frames[b], 0, sizeof(frames[b]));
+    ht_video_frame &f = frames[b];
+    f.width = (int32_t)GetNumProp(env, r, "width", 0);
+    f.height = (int32_t)GetNumProp(env, r, "height", 0);
+    uint8_t *rgba; size_t len;
+    NAPI_OK(napi_get_named_property(env, r, "rgba", &v));
+    if (!GetBytes(env, v, &rgba, &len) || len < (size_t)f.width * f.height * 4 || !ViewOf(env, r, &views[b]))
+      return Throw(env, ctx, HT_ERR_ARG);
+    f.rgba = rgba;
+  }
+  void *data; napi_value ab, ta;
+  NAPI_OK(napi_create_arraybuffer(env, (size_t)n * dw * dh * 4, &data, &ab));
+  int rc = ht_ingest_views(ctx, frames.data(), views.data(), (int)n, 0, static_cast<uint8_t *>(data), dw, dh);
   if (rc < 0) return Throw(env, ctx, rc);
   NAPI_OK(napi_create_typedarray(env, napi_uint8_clamped_array, (size_t)n * dw * dh * 4, ab, 0, &ta));
   return ta;
@@ -783,6 +868,10 @@ static napi_value Init(napi_env env, napi_value exports) {
       {"trackerFeed", nullptr, TrackerFeed, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerFeedYuv", nullptr, TrackerFeedYuv, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"ingestYuv", nullptr, IngestYuv, nullptr, nullptr, nullptr, napi_default, nullptr},
+      {"trackerFeedViews", nullptr, TrackerFeedViews, nullptr, nullptr, nullptr, napi_default, nullptr},
+      {"trackerFeedYuvViews", nullptr, TrackerFeedYuvViews, nullptr, nullptr, nullptr, napi_default, nullptr},
+      {"ingestViews", nullptr, IngestViews, nullptr, nullptr, nullptr, napi_default, nullptr},
+      {"ingestYuvViews", nullptr, IngestYuvViews, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"create", nullptr, Create, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"detect", nullptr, Detect, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackInit", nullptr, TrackInit, nullptr, nullptr, nullptr, napi_default, nullptr},

@@ -22,6 +22,10 @@ streams: N 640x480 streams, device-resident frames and outputs, CUDA events arou
   <fmt>_*         (--formats) ht_tracker_feed_yuv from every video format against ht_ingest_yuv + ht_tracker_feed and
                   ht_tracker_feed from the converted RGBA video, NV12 / I420 / RGBA also against --before-lib, and
                   k_feed_draw_yuv's time per format (formats_arms)
+  <fmt>_<config>_*
+                  (--views) ht_tracker_feed(_yuv)_views from RGBA and NV12 video through rotations, mirrors and crops
+                  against the plain feed of the upright video and against a separate rotate / crop pass + plain feed
+                  (also --before-lib), and k_feed_draw_view's time (views_arms)
 
 Prints one JSON line with the card's name and power limit read in the same run; --out also writes it to a file."""
 import argparse
@@ -844,6 +848,164 @@ def formats_arms(torch, stream, N, steps, rounds, before_lib=None):
     return res
 
 
+# (name, video W x H, canvas, orientation, crop of the oriented frame or None)
+VIEW_CONFIGS = [("identity", (1280, 720), (320, 240), 0, None), ("rot180", (1280, 720), (320, 240), 2, None),
+                ("mirror", (1280, 720), (320, 240), 4, None), ("crop960", (1280, 720), (320, 240), 0, (160, 0, 960, 720)),
+                ("rot90", (1280, 720), (240, 320), 1, None), ("rot270", (1280, 720), (240, 320), 3, None),
+                ("1to1", (640, 480), (640, 480), 0, None), ("1to1_rot90", (640, 480), (480, 640), 1, None)]
+
+
+def views_arms(torch, stream, N, steps, rounds, before_lib=None):
+    """Video drawn through views (ht_tracker_feed_views / ht_tracker_feed_yuv_views) in steady tracking, RGBA and NV12,
+    for each of VIEW_CONFIGS: N streams, each with its own device video V in memory orientation, every arm on its own
+    context, the arms alternating tick by tick (the order rotates), CUDA events around each tick:
+
+      <fmt>_<config>_view_cs     the feed of V through the view
+      <fmt>_<config>_plain_cs    the plain feed (ht_tracker_feed / ht_tracker_feed_yuv) of the upright crop of V,
+                                 prepared beforehand, on the same canvas
+      <fmt>_<config>_twopass_cs  ht_ingest(_yuv)_views of V into an RGBA buffer of the crop's size, then ht_tracker_feed
+      <fmt>_<config>_before_cs   the plain arm with the library at `before_lib` (e.g. the parent commit's build)
+
+    Then, in a run of its own under torch.profiler, k_feed_draw_view's time per tick and its achieved bytes/s (video
+    bytes read once + canvas written), and the plain arm's draw kernel.  The records of every arm must agree on every
+    timed tick (even-sized 4:2:0 orientations and crops keep chroma blocks whole, so the upright NV12 twin is exact)."""
+    import ctypes as C
+    from headtrackr_b200 import Context, _lib, synth, views
+    from headtrackr_b200.context import _views, _yuv_image
+    rec_bytes = C.sizeof(_lib.TrackerEvent)
+    res = {}
+
+    def unorient(a, o):          # V with orient(V, o) == a, on the first two dimensions
+        return torch.rot90(torch.flip(a, dims=(1,)) if o & 4 else a, o & 3, dims=(0, 1)).contiguous()
+
+    for name, (W, H), (CW, CH), o, crop in VIEW_CONFIGS:
+        OW, OH = (H, W) if o & 1 else (W, H)
+        sx, sy, sw, sh = crop or (0, 0, OW, OH)
+        v = {"rotate": 90 * (o & 3), "mirror": bool(o & 4), "crop": crop}
+        assert views.oriented_size(v, W, H) == (OW, OH)
+        base = torch.stack([torch.from_numpy(synth.frame(i, OW, OH, n_faces=1)) for i in range(8)]).cuda()
+        up = torch.empty((N, OH, OW, 4), dtype=torch.uint8, device="cuda")     # the oriented frames O
+        for k in range(N):
+            up[k] = torch.roll(base[k % 8], shifts=2 * (k // 8) % 64, dims=1)
+        del base
+        for fmt in ("rgba", "nv12"):
+            kw = dict(max_width=max(CW, 640), max_height=max(CH, 640), max_frames=N, stream=stream)
+            keep = []
+            if fmt == "rgba":
+                vid = [unorient(up[k], o) for k in range(N)]
+                plain = [up[k, sy:sy + sh, sx:sx + sw].contiguous() for k in range(N)]
+                vrecs = [_lib.VideoFrame(x.data_ptr(), k, W, H, 0, 0.0) for k, x in enumerate(vid)]
+                precs = (_lib.VideoFrame * N)(*[_lib.VideoFrame(x.data_ptr(), k, sw, sh, 0, 0.0) for k, x in enumerate(plain)])
+                vcanv = (_lib.CanvasFrame * N)(*[_lib.CanvasFrame(r, CW, CH) for r in vrecs])
+                ingest_src = (_lib.VideoFrame * N)(*vrecs)
+            else:
+                yu = format_video(torch, up, "nv12")                           # the oriented frames in NV12
+                pair = lambda p: p.reshape(p.shape[0], p.shape[1] // 2, 2)      # noqa: E731
+                vid = [(unorient(y, o), unorient(pair(uv), o).reshape(H // 2, W)) for y, uv in yu]
+                plain = [(y[sy:sy + sh, sx:sx + sw].contiguous(), uv[sy // 2:(sy + sh) // 2, sx:sx + sw].contiguous())
+                         for y, uv in yu]
+                del yu
+                imgs = [_yuv_image(x, "nv12", "bt601", keep)[0] for x in vid]
+                pimgs = [_yuv_image(x, "nv12", "bt601", keep)[0] for x in plain]
+                vcanv = (_lib.YuvFrame * N)(*[_lib.YuvFrame(imgs[k], k, CW, CH, 0, 0.0) for k in range(N)])
+                precs = (_lib.YuvFrame * N)(*[_lib.YuvFrame(pimgs[k], k, CW, CH, 0, 0.0) for k in range(N)])
+                ingest_src = (_lib.YuvImage * N)(*imgs)
+            staged = torch.empty((N, sh, sw, 4), dtype=torch.uint8, device="cuda")
+            srecs = (_lib.VideoFrame * N)(*[_lib.VideoFrame(staged[k].data_ptr(), k, sw, sh, 0, 0.0) for k in range(N)])
+            vviews = _views(v, N)
+            now = [1.0e12]
+
+            def arm(kind):
+                c = other_build_context(before_lib, **kw) if kind == "before" else Context(**kw)
+                c.tracker_config()
+                c.tracker_reset(0, N)
+                c.tracker_start(0, N)
+                out = torch.empty(N * rec_bytes, dtype=torch.uint8, device="cuda")
+
+                def run():
+                    t = now[0]
+                    if kind == "view":
+                        for k in range(N):
+                            if fmt == "rgba":
+                                vcanv[k].video.now_ms = t
+                            else:
+                                vcanv[k].now_ms = t
+                        f = c._L.ht_tracker_feed_views if fmt == "rgba" else c._L.ht_tracker_feed_yuv_views
+                        c._check(f(c._h, C.addressof(vcanv), C.addressof(vviews), N, 1, out.data_ptr()))
+                        return
+                    recs = precs
+                    if kind == "twopass":
+                        f = c._L.ht_ingest_views if fmt == "rgba" else c._L.ht_ingest_yuv_views
+                        c._check(f(c._h, C.addressof(ingest_src), C.addressof(vviews), N, 1, staged.data_ptr(), sw, sh))
+                        recs = srecs
+                    for k in range(N):
+                        recs[k].now_ms = t
+                    if fmt == "nv12" and kind != "twopass":
+                        c._check(c._L.ht_tracker_feed_yuv(c._h, C.addressof(recs), N, 1, out.data_ptr()))
+                    else:
+                        c._check(c._L.ht_tracker_feed(c._h, C.addressof(recs), N, 1, CW, CH, out.data_ptr()))
+                return c, run, out
+
+            kinds = ["view", "plain", "twopass"] + (["before"] if before_lib else [])
+            arms = {k: arm(k) for k in kinds}
+
+            def tick(arm_name):
+                a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                a.record()
+                arms[arm_name][1]()
+                b.record()
+                b.synchronize()
+                return a.elapsed_time(b)
+
+            for _ in range(17):
+                now[0] += 20.0
+                for k in kinds:
+                    tick(k)
+            times = {k: [[] for _ in range(rounds)] for k in kinds}
+            for r in range(rounds):
+                for s in range(steps):
+                    now[0] += 20.0
+                    rot = (r * steps + s) % len(kinds)
+                    for k in kinds[rot:] + kinds[:rot]:
+                        times[k][r].append(tick(k))
+                    if any(not torch.equal(arms["view"][2], arms[k][2]) for k in kinds[1:]):
+                        raise SystemExit(f"view arms disagree on the records of a timed tick ({fmt}, {name})")
+            key = f"{fmt}_{name}"
+            for k in kinds:
+                med = [float(np.median(t)) for t in times[k]]
+                res[f"{key}_{k}_cs_ms"] = float(np.median(sum(times[k], [])))
+                res[f"{key}_{k}_cs_spread_ms"] = max(med) - min(med)
+            ev = [_lib.TrackerEvent.from_buffer_copy(bytes(row)) for row in arms["view"][2].cpu().numpy().reshape(N, rec_bytes)]
+            res[f"{key}_cs_streams"] = sum(e.detection == 2 for e in ev)
+
+            from torch.profiler import ProfilerActivity, profile
+            for k, kernel in (("view", "k_feed_draw_view"), ("plain", "k_feed_draw_yuv" if fmt == "nv12" else "k_feed_draw")):
+                with profile(activities=[ProfilerActivity.CUDA]) as prof:
+                    for _ in range(steps):
+                        now[0] += 20.0
+                        arms[k][1]()
+                    torch.cuda.synchronize()
+                us = 0.0
+                for e in prof.key_averages():
+                    if e.key.split("(")[0].split("<")[0].endswith(kernel):
+                        t = getattr(e, "device_time_total", None)
+                        us += t if t is not None else e.cuda_time_total
+                ms = us / 1000.0 / steps
+                res[f"{kernel}_{key}_ms"] = ms
+            # bytes a view draw needs at least: the video it samples read once (the crop of each plane) + the canvas
+            ms = res[f"k_feed_draw_view_{key}_ms"]
+            video_bytes = N * sw * sh * (4 if fmt == "rgba" else 1.5)
+            res[f"k_feed_draw_view_{key}_tb_per_s"] = (video_bytes + N * CW * CH * 4) / (ms * 1e-3) / 1e12 if ms > 0 else None
+            for c, _, _ in arms.values():
+                c.close()
+            del vid, plain, keep, staged
+            torch.cuda.empty_cache()
+        del up
+        torch.cuda.empty_cache()
+    res["views_records_agree"] = True
+    return res
+
+
 def migrate_arms(torch, frames, stream, N, W, H, steps, rounds):
     """Tracker records (ht_tracker_export / ht_tracker_import) of N streams in steady tracking, W x H video on W/2 x H/2
     canvases, CUDA events on the library's stream around each call, repeated `rounds` x `steps` times:
@@ -947,6 +1109,7 @@ def main():
     ap.add_argument("--camera-streams", action="store_true", help="only the camera-controller arms (camera_arms)")
     ap.add_argument("--yuv", action="store_true", help="only the YUV video arms (yuv_arms)")
     ap.add_argument("--formats", action="store_true", help="only the video-format arms (formats_arms)")
+    ap.add_argument("--views", action="store_true", help="only the video-view arms (views_arms)")
     ap.add_argument("--out")
     a = ap.parse_args()
     import torch
@@ -962,6 +1125,9 @@ def main():
     stream = ts.cuda_stream
     if a.yuv:
         res.update(yuv_arms(torch, stream, N, a.steps, a.rounds, a.before_lib))
+        return report(res, a.out)
+    if a.views:
+        res.update(views_arms(torch, stream, N, a.steps, a.rounds, a.before_lib))
         return report(res, a.out)
     if a.formats:
         res.update(formats_arms(torch, stream, N, a.steps, a.rounds, a.before_lib))
