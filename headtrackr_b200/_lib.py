@@ -173,7 +173,7 @@ _lib = None
 
 EXPORTS = ["ht_version", "ht_create", "ht_destroy", "ht_last_error", "ht_sync", "ht_max_rects", "ht_detect",
            "ht_track_init", "ht_track_init_from_detect", "ht_track", "ht_detect_track", "ht_stream_reset", "ht_stream_step", "ht_stream_head_config", "ht_stream_step_head",
-           "ht_tracker_config", "ht_tracker_reset", "ht_tracker_start", "ht_tracker_stop", "ht_tracker_step", "ht_tracker_feed", "ht_tracker_set_params", "ht_tracker_feed_canvases", "ht_tracker_set_debug", "ht_tracker_set_camera", "ht_tracker_export", "ht_tracker_import", "ht_tracker_feed_yuv", "ht_ingest", "ht_ingest_yuv",
+           "ht_tracker_config", "ht_tracker_reset", "ht_tracker_start", "ht_tracker_stop", "ht_tracker_step", "ht_tracker_feed", "ht_tracker_set_params", "ht_tracker_feed_canvases", "ht_tracker_set_debug", "ht_tracker_set_debug_strokes", "ht_tracker_set_camera", "ht_tracker_export", "ht_tracker_import", "ht_tracker_feed_yuv", "ht_ingest", "ht_ingest_yuv",
            "ht_tracker_feed_views", "ht_tracker_feed_yuv_views", "ht_ingest_views", "ht_ingest_yuv_views", "ht_backprojection", "ht_whitebalance",
            "ht_plan_info", "ht_debug_plane", "ht_debug_raw", "ht_debug_model_hist", "ht_debug_track_stats", "ht_set_track_memo", "ht_set_pipeline", "ht_join", "ht_debug_set_exactness", "ht_debug_track_trace", "ht_debug_track_phases", "ht_launch_count",
            "ht_profile", "ht_profile_read"]
@@ -218,6 +218,7 @@ def lib():
     L.ht_tracker_set_params.argtypes = [vp, C.c_int, C.c_int, vp]
     L.ht_tracker_feed_canvases.argtypes = [vp, vp, C.c_int, C.c_int, vp]
     L.ht_tracker_set_debug.argtypes = [vp, C.c_int, C.c_int, vp]
+    L.ht_tracker_set_debug_strokes.argtypes = [vp, C.c_int, C.c_int, vp]
     L.ht_tracker_set_camera.argtypes = [vp, C.c_int, C.c_int, vp]
     L.ht_tracker_export.argtypes = [vp, vp, C.c_int, vp]
     L.ht_tracker_import.argtypes = [vp, vp, C.c_int, vp]

@@ -386,6 +386,16 @@ class Context:
             else:
                 self._debug[int(first) + i] = t
 
+    def tracker_set_debug_strokes(self, first, flags):
+        """Whether streams first, first+1, ... stroke main.js's face rectangles onto their debug canvases
+        (ht_tracker_set_debug_strokes): after every tick, on top of its back-projection, the "VJ" box in #0000CC or the
+        "CS" box rotated about its centre in #00CC00 (src/main.js:199-219), rasterized as DESIGN.md 2 defines.  The
+        flag is the stream's: it outlives set_debug, set_params, stop, start, reset and import; tracker_config clears
+        it."""
+        flags = [bool(f) for f in flags]
+        arr = (C.c_int32 * max(1, len(flags)))(*[int(f) for f in flags])
+        self._check(self._L.ht_tracker_set_debug_strokes(self._h, int(first), len(flags), arr))
+
     def tracker_set_camera(self, first, controls):
         """Head-coupled camera controllers of streams first, first+1, ...: per stream None (none) or a dict of
         realisticAbsoluteCameraControl's arguments (src/controllers.js:28-38) - scaling, fixedPosition, lookAt (three

@@ -574,6 +574,9 @@ struct ht_ctx {
   DevBuf d_debug, d_debug_tab;
   std::vector<DebugCanvas> h_debug;
   int debug_count = 0;
+  // ht_tracker_set_debug_strokes: the streams whose flag is on, and those of them that have a canvas (0: a tick
+  // launches no k_debug_strokes)
+  int stroke_flags = 0, stroke_count = 0;
   // ht_tracker_set_camera: per stream its CameraCtl (device array and host copy) and the number of streams that have
   // one (0: a tick launches nothing for cameras)
   DevBuf d_camera;
@@ -1745,10 +1748,10 @@ int ht_tracker_config(ht_ctx *ctx, const ht_tracker_params *params) {
   CK(cudaSetDevice(ctx->cfg.device));
   const size_t mf = (size_t)ctx->cfg.max_frames;
   if (params && !tracker_params_ok(*params)) return ctx->fail(HT_ERR_ARG, "bad head parameters");
-  if (ctx->debug_count > 0) {    // either form discards the debug canvases (the device array is all NULL otherwise)
-    CK(cudaMemsetAsync(ctx->d_debug.p, 0, mf * sizeof(DebugCanvas), ctx->stream));
+  if (ctx->debug_count > 0 || ctx->stroke_flags > 0) {   // either form discards the debug canvases and stroke flags
+    CK(cudaMemsetAsync(ctx->d_debug.p, 0, mf * sizeof(DebugCanvas), ctx->stream));   // (the array is all 0 otherwise)
     ctx->h_debug.assign(mf, DebugCanvas{});
-    ctx->debug_count = 0;
+    ctx->debug_count = ctx->stroke_flags = ctx->stroke_count = 0;
   }
   if (ctx->camera_count > 0) {   // and every camera controller
     CK(cudaMemsetAsync(ctx->d_camera.p, 0, mf * sizeof(CameraCtl), ctx->stream));
@@ -1809,6 +1812,30 @@ static_assert(sizeof(ht_debug_canvas) == 24 && sizeof(DebugCanvas) == sizeof(ht_
                   offsetof(ht_debug_canvas, pitch) == offsetof(DebugCanvas, pitch),
               "ht_debug_canvas layout");
 
+// Streams [first, first + n) of `next` (every stream's DebugCanvas after a checked call) go to the device, and the
+// counts that decide a tick's debug launches follow them.
+static int debug_commit(ht_ctx *ctx, int first, int n, std::vector<DebugCanvas> &next) {
+  const size_t mf = (size_t)ctx->cfg.max_frames;
+  { const int jr = join_aux(ctx); if (jr != HT_OK) return jr; }
+  CK(cudaSetDevice(ctx->cfg.device));
+  if (!ctx->d_debug.p) {
+    CK(ctx->d_debug.reserve(mf * sizeof(DebugCanvas)));
+    CK(ctx->d_debug_tab.reserve(mf * DBG_TAB));
+    CK(cudaMemsetAsync(ctx->d_debug.p, 0, mf * sizeof(DebugCanvas), ctx->stream));
+  }
+  CK(cudaMemcpyAsync(ctx->d_debug.as<DebugCanvas>() + first, next.data() + first, (size_t)n * sizeof(DebugCanvas),
+                     cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));    // `next` is the caller's local
+  ctx->debug_count = ctx->stroke_flags = ctx->stroke_count = 0;
+  for (const DebugCanvas &d : next) {
+    ctx->debug_count += d.rgba != nullptr;
+    ctx->stroke_flags += d.strokes;
+    ctx->stroke_count += d.rgba != nullptr && d.strokes;
+  }
+  ctx->h_debug.swap(next);
+  return HT_OK;
+}
+
 // The debug canvases of streams [first, first + n).  Everything is checked on the host before anything changes,
 // overlap over every stream that has a canvas after the call.
 int ht_tracker_set_debug(ht_ctx *ctx, int first, int n, const ht_debug_canvas *canvases) {
@@ -1831,6 +1858,7 @@ int ht_tracker_set_debug(ht_ctx *ctx, int first, int n, const ht_debug_canvas *c
         return ctx->fail(HT_ERR_ARG, "record %d: pitch %d is not a multiple of 4 >= 4*width", i, c.pitch);
       d = DebugCanvas{c.rgba, c.width, c.height, c.pitch ? c.pitch : 4 * c.width, 0};
     }
+    d.strokes = next[(size_t)(first + i)].strokes;     // the stream's stroke flag stays
     next[(size_t)(first + i)] = d;
   }
   // two canvases of one tick's streams must not share a byte: [start, end) of every canvas, sorted by start
@@ -1844,19 +1872,23 @@ int ht_tracker_set_debug(ht_ctx *ctx, int first, int n, const ht_debug_canvas *c
   for (size_t i = 1; i < spans.size(); ++i)
     if (spans[i].first < spans[i - 1].second)
       return ctx->fail(HT_ERR_ARG, "a debug canvas overlaps another stream's debug canvas");
-  { const int jr = join_aux(ctx); if (jr != HT_OK) return jr; }
-  CK(cudaSetDevice(ctx->cfg.device));
-  if (!ctx->d_debug.p) {
-    CK(ctx->d_debug.reserve((size_t)mf * sizeof(DebugCanvas)));
-    CK(ctx->d_debug_tab.reserve((size_t)mf * DBG_TAB));
-    CK(cudaMemsetAsync(ctx->d_debug.p, 0, (size_t)mf * sizeof(DebugCanvas), ctx->stream));
-  }
-  CK(cudaMemcpyAsync(ctx->d_debug.as<DebugCanvas>() + first, next.data() + first, (size_t)n * sizeof(DebugCanvas),
-                     cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));    // `next` is a local
-  ctx->debug_count = (int)spans.size();
-  ctx->h_debug.swap(next);
-  return HT_OK;
+  return debug_commit(ctx, first, n, next);
+}
+
+// Streams first+i stroke main.js's rectangles on their debug canvases (enable[i] 1) or not (0).  The flag is the
+// stream's, kept in the pad word of its DebugCanvas.
+int ht_tracker_set_debug_strokes(ht_ctx *ctx, int first, int n, const int32_t *enable) {
+  if (!ctx) return HT_ERR_ARG;
+  if (!ctx->tracker_on) return ctx->fail(HT_ERR_STATE, "ht_tracker_config has not been called");
+  const int mf = ctx->cfg.max_frames;
+  if (first < 0 || n <= 0 || first > mf - n) return ctx->fail(HT_ERR_ARG, "stream range outside [0,%d)", mf);
+  if (!enable) return ctx->fail(HT_ERR_ARG, "enable is NULL");
+  for (int i = 0; i < n; ++i)
+    if (enable[i] != 0 && enable[i] != 1) return ctx->fail(HT_ERR_ARG, "record %d: enable %d is not 0 or 1", i, enable[i]);
+  std::vector<DebugCanvas> next = ctx->h_debug;
+  next.resize((size_t)mf, DebugCanvas{});
+  for (int i = 0; i < n; ++i) next[(size_t)(first + i)].strokes = enable[i];
+  return debug_commit(ctx, first, n, next);
 }
 
 static_assert(sizeof(ht_camera) == HT_CAMERA_BYTES && HT_CAMERA_BYTES == 224 && offsetof(ht_camera, fov) == 24 &&
@@ -2163,6 +2195,10 @@ static int tracker_tick(ht_ctx *ctx, const TickGroup *grp, int n_groups, const u
                                                     ctx->d_rects.as<int32_t>(), init_en, now_ms, d_now, g0.w, g0.h, geo, d_ev);
   if (ctx->camera_count > 0) {  // the cameras of the entries whose record has a headtrackingEvent
     k_camera_update<<<(n + 127) / 128, 128, 0, st>>>(d_ids, geo, n, d_ev, ctx->d_camera.as<CameraCtl>());
+    ++ctx->launches;
+  }
+  if (ctx->stroke_count > 0) {   // main.js's strokes, after this tick's back-projections (src/main.js:199-219)
+    k_debug_strokes<<<(unsigned)n, 256, 0, st>>>(d_ids, geo, d_ev, ctx->d_debug.as<DebugCanvas>());
     ++ctx->launches;
   }
   ctx->prof_begin(HT_PROF_TRACK_INIT, st);
@@ -3134,6 +3170,29 @@ extern "C" int ht_selftest_debug_table(const uint32_t *mh, const uint32_t *ch, u
 // k_debug_backproj's tile walk and per-thread writer on the host: the bin plane (w x h, 8 * bin or BIN_ZERO per pixel)
 // through `table` onto a debug canvas (dw x dh, pitch bytes per row), clipped as the kernel clips it.  -> the number of
 // 16-byte stores (vec paths taken).
+// stroke_sincos -> sc[2] = {sin, cos}
+extern "C" void ht_selftest_stroke_sincos(double t, double *sc) { stroke_sincos(t, sc[0], sc[1]); }
+
+// k_debug_strokes's per-stream code on the host, span walk included: the stroke of `ev` (an ht_tracker_event) onto a
+// dw x dh debug canvas of `pitch` bytes per row.  -> the number of pixels visited.
+extern "C" int ht_selftest_debug_strokes(const ht_tracker_event *ev, uint8_t *rgba, int dw, int dh, int pitch) {
+  const TrackerEvent &e = *reinterpret_cast<const TrackerEvent *>(ev);
+  Stroke S;
+  if (!stroke_make(e.detection, e.confidence, e.x, e.y, e.width, e.height, e.angle, dw, dh, S)) return 0;
+  int visited = 0;
+  for (int Y = S.y0; Y < S.y1; ++Y) {
+    int seg[4];
+    stroke_row_spans(S, Y, dw, seg);
+    for (int s = 0; s < 4; s += 2)
+      for (int X = seg[s]; X <= seg[s + 1]; ++X, ++visited) {
+        int c = 0;
+        for (int j = 0; j < 16; ++j) c += stroke_row_count(S, X, Y, j);
+        if (c > 0) stroke_blend(rgba + (size_t)Y * pitch + 4 * (size_t)X, c, S.rgb);
+      }
+  }
+  return visited;
+}
+
 extern "C" int ht_selftest_debug_write(const uint16_t *bins, int w, int h, const uint8_t *table, uint8_t *rgba, int dw,
                                        int dh, int pitch) {
   const int cw = std::min(w, dw), chh = std::min(h, dh);

@@ -1078,10 +1078,11 @@ __global__ void k_backproj(const uint8_t *__restrict__ rgba, int n_px, const uin
 // ------------------------------------------------------------------------------------------------
 // The debug canvas of a headtrackr.Tracker stream (ht_tracker_set_debug): on every CS pass facetrackr puts
 // getBackProjectionImg() at (0, 0) of params.debug (src/facetrackr.js:193-196), clipped to that canvas.
-// Layout of ht_debug_canvas, with the pitch resolved; rgba NULL: the stream has none.
+// Layout of ht_debug_canvas, with the pitch resolved; rgba NULL: the stream has none.  strokes (the header's pad word):
+// ht_tracker_set_debug_strokes's flag, which belongs to the stream whether or not it has a canvas.
 struct DebugCanvas {
   uint8_t *rgba;
-  int32_t w, h, pitch, pad_;
+  int32_t w, h, pitch, strokes;
 };
 constexpr int DBG_TAB = 4112;                     // bytes per value table: 4096 bins + BIN_ZERO's 0, padded to 16 B
 constexpr int DBG_TX = 128, DBG_TY = 32;          // pixels per tile of k_debug_backproj
@@ -1104,6 +1105,234 @@ __host__ __device__ __forceinline__ void debug_px4(const uint16_t *src, const ui
   } else {
     for (int i = 0; i < m; ++i) reinterpret_cast<uint32_t *>(dst)[x + i] = o[i];
   }
+}
+
+// ------------------------------------------------------------------------------------------------
+// The strokes main.js draws on the debug canvas after a tick (src/main.js:199-219), rasterized by one definition
+// (DESIGN.md 2, "Strokes"): lineWidth 1, miter joins, butt caps; corners through translate . rotate in fp64, quantised
+// to 1/256 px; 16 x 16 samples per pixel tested with integer edge functions and the top-left rule; alpha
+// (255 c + 128) >> 8 of the c covered samples; non-premultiplied source-over.  Host and device round alike: products
+// are rounded before they are added (no contraction), so both give the same corners.
+__host__ __device__ __forceinline__ double sk_mul(double a, double b) {
+#ifdef __CUDA_ARCH__
+  return __dmul_rn(a, b);
+#else
+  volatile double p = a * b;   // a host compiler with FMA could otherwise fuse it into the next add
+  return p;
+#endif
+}
+__host__ __device__ __forceinline__ double sk_add(double a, double b) {
+#ifdef __CUDA_ARCH__
+  return __dadd_rn(a, b);
+#else
+  return a + b;
+#endif
+}
+
+// sin and cos of theta: fdlibm's kernels (k_sin.c, k_cos.c) after a three-part Cody-Waite reduction by pi/2, every
+// operation rounded as written.  (0, 1) exactly at 0; within 2 ulp of sin / cos on [-pi/2, pi/2]; a non-finite theta
+// is no rotation, as the 2D context ignores rotate(NaN).
+__host__ __device__ inline void stroke_sincos(double t, double &s, double &c) {
+  if (!isfinite(t)) { s = 0.0; c = 1.0; return; }
+  const double k = rint(sk_mul(t, 6.36619772367581382433e-01));
+  double r = sk_add(t, -sk_mul(k, 1.57079632673412561417e+00));
+  r = sk_add(r, -sk_mul(k, 6.07710050630396597660e-11));
+  r = sk_add(r, -sk_mul(k, 2.02226624879595063154e-21));
+  const double z = sk_mul(r, r), w = sk_mul(z, z);
+  const double S1 = -1.66666666666666324348e-01, S2 = 8.33333333332248946124e-03, S3 = -1.98412698298579493134e-04,
+               S4 = 2.75573137070700676789e-06, S5 = -2.50507602534068634195e-08, S6 = 1.58969099521155010221e-10;
+  const double C1 = 4.16666666666666019037e-02, C2 = -1.38888888888741095749e-03, C3 = 2.48015872894767294178e-05,
+               C4 = -2.75573143513906633035e-07, C5 = 2.08757232129817482790e-09, C6 = -1.13596475577881948265e-11;
+  // sin r = r + r^3 (S1 + z (S2 + z (S3 + z S4) + z w (S5 + z S6)))
+  const double sr = sk_add(sk_add(S2, sk_mul(z, sk_add(S3, sk_mul(z, S4)))), sk_mul(sk_mul(z, w), sk_add(S5, sk_mul(z, S6))));
+  const double sn = sk_add(r, sk_mul(sk_mul(z, r), sk_add(S1, sk_mul(z, sr))));
+  // cos r = (1 - z/2) + (((1 - (1 - z/2)) - z/2) + z cr)
+  const double cr = sk_add(sk_mul(z, sk_add(C1, sk_mul(z, sk_add(C2, sk_mul(z, C3))))),
+                           sk_mul(sk_mul(w, w), sk_add(C4, sk_mul(z, sk_add(C5, sk_mul(z, C6))))));
+  const double hz = sk_mul(0.5, z), one_hz = sk_add(1.0, -hz);
+  const double cs = sk_add(one_hz, sk_add(sk_add(sk_add(1.0, -one_hz), -hz), sk_mul(z, cr)));
+  switch ((int)(k - 4.0 * floor(k * 0.25))) {   // the quadrant, k mod 4
+    case 0: s = sn; c = cs; break;
+    case 1: s = cs; c = -sn; break;
+    case 2: s = -sn; c = -cs; break;
+    default: s = -cs; c = sn; break;
+  }
+}
+
+// One quad of a stroke: corners in 1/256 px, in the order (x0, y0), (x1, y0), (x1, y1), (x0, y1) of the rectangle's
+// local coordinates, so its inside is E > 0 for every edge function E(p) = d x (p - a) of edge a -> a + d.  bias: 0
+// for a top or left edge (a sample on it is inside), 1 otherwise.
+struct StrokeQuad {
+  long long ax[4], ay[4], dx[4], dy[4];
+  int32_t bias[4];
+};
+// One tick's stroke on one debug canvas: the outer quad and the inner one (n_q == 2), the colour, and the canvas rows
+// [y0, y1) that the outer quad's bounding box meets.
+struct Stroke {
+  StrokeQuad q[2];
+  int32_t n_q, y0, y1;
+  uint32_t rgb;   // 0x00BBGGRR
+};
+
+__host__ __device__ inline void stroke_quad(StrokeQuad &q, double tx, double ty, double s, double c, double x0, double y0,
+                                            double x1, double y1) {
+  const double lx[4] = {x0, x1, x1, x0}, ly[4] = {y0, y0, y1, y1};
+  long long px[4], py[4];
+  for (int i = 0; i < 4; ++i) {
+    const double X = sk_add(tx, sk_add(sk_mul(c, lx[i]), -sk_mul(s, ly[i])));
+    const double Y = sk_add(ty, sk_add(sk_mul(s, lx[i]), sk_mul(c, ly[i])));
+    px[i] = (long long)floor(sk_add(sk_mul(X, 256.0), 0.5));
+    py[i] = (long long)floor(sk_add(sk_mul(Y, 256.0), 0.5));
+  }
+  for (int i = 0; i < 4; ++i) {
+    const int e = (i + 1) & 3;
+    q.ax[i] = px[i]; q.ay[i] = py[i];
+    q.dx[i] = px[e] - px[i]; q.dy[i] = py[e] - py[i];
+    q.bias[i] = (q.dy[i] < 0 || (q.dy[i] == 0 && q.dx[i] > 0)) ? 0 : 1;
+  }
+}
+
+// The stroke of one ht_tracker_event on a dw x dh debug canvas: the rule of streams.debug_calls (nothing when
+// confidence is 0 or the pass is not "VJ" / "CS"; a VJ box as it is; a CS box rotated by angle - pi/2 about (x, y)
+// at ToInt32(-w/2), ToInt32(-h/2)).  Boxes with a field that is not finite or beyond 65536 px draw nothing, as the
+// 2D context ignores non-finite arguments; the tracker produces neither.  -> whether anything may be drawn.
+__host__ __device__ inline bool stroke_make(int detection, double confidence, double x, double y, double w, double h,
+                                            double angle, int dw, int dh, Stroke &S) {
+  S.n_q = 0; S.y0 = S.y1 = 0; S.rgb = 0;
+  if (confidence == 0.0 || (detection != 1 && detection != 2)) return false;
+  const double v[4] = {x, y, w, h};
+  for (int i = 0; i < 4; ++i)
+    if (!(fabs(v[i]) <= 65536.0)) return false;
+  double tx = 0.0, ty = 0.0, s = 0.0, c = 1.0, rx = x, ry = y;
+  S.rgb = 0xCC0000u;                                 // "#0000CC"
+  if (detection == 2) {
+    tx = x; ty = y;
+    stroke_sincos(sk_add(angle, -1.5707963267948966), s, c);
+    rx = trunc(-(w / 2)); ry = trunc(-(h / 2));      // ToInt32 of values within +-32768
+    S.rgb = 0x00CC00u;                               // "#00CC00"
+  }
+  if (w < 0) { rx = sk_add(rx, w); w = -w; }
+  if (h < 0) { ry = sk_add(ry, h); h = -h; }
+  if (w == 0 && h == 0) return false;
+  const double xe = sk_add(rx, w), ye = sk_add(ry, h);
+  if (h == 0) {                                      // a butt-capped line
+    stroke_quad(S.q[0], tx, ty, s, c, rx, sk_add(ry, -0.5), xe, sk_add(ry, 0.5));
+    S.n_q = 1;
+  } else if (w == 0) {
+    stroke_quad(S.q[0], tx, ty, s, c, sk_add(rx, -0.5), ry, sk_add(rx, 0.5), ye);
+    S.n_q = 1;
+  } else {
+    stroke_quad(S.q[0], tx, ty, s, c, sk_add(rx, -0.5), sk_add(ry, -0.5), sk_add(xe, 0.5), sk_add(ye, 0.5));
+    S.n_q = 1;
+    if (w > 1 && h > 1) {
+      stroke_quad(S.q[1], tx, ty, s, c, sk_add(rx, 0.5), sk_add(ry, 0.5), sk_add(xe, -0.5), sk_add(ye, -0.5));
+      S.n_q = 2;
+    }
+  }
+  long long lo = S.q[0].ay[0], hi = lo;
+  for (int i = 1; i < 4; ++i) { lo = S.q[0].ay[i] < lo ? S.q[0].ay[i] : lo; hi = S.q[0].ay[i] > hi ? S.q[0].ay[i] : hi; }
+  const long long r0 = lo >= 0 ? lo / 256 : -((255 - lo) / 256), r1 = (hi >= 0 ? hi / 256 : -((255 - hi) / 256)) + 1;
+  S.y0 = (int)(r0 < 0 ? 0 : r0);
+  S.y1 = (int)(r1 > dh ? dh : r1);
+  return S.y0 < S.y1 && dw > 0;
+}
+
+// x-range of quad q at height y (1/256 px units), over its edges that reach y.  -> false if no edge does.
+__host__ __device__ inline bool stroke_cross(const StrokeQuad &q, double y, double &l, double &r) {
+  l = 1e300; r = -1e300;
+  for (int i = 0; i < 4; ++i) {
+    const double ay = (double)q.ay[i], by = (double)(q.ay[i] + q.dy[i]), ax = (double)q.ax[i], bx = (double)(q.ax[i] + q.dx[i]);
+    if (y < fmin(ay, by) || y > fmax(ay, by)) continue;
+    if (ay == by) {
+      l = fmin(l, fmin(ax, bx)); r = fmax(r, fmax(ax, bx));
+    } else {
+      const double xc = ax + (y - ay) * (bx - ax) / (by - ay);
+      l = fmin(l, xc); r = fmax(r, xc);
+    }
+  }
+  return l <= r;
+}
+
+// The pixels of row Y that the kernel visits: [seg[0], seg[1]] and [seg[2], seg[3]] (empty when first > last).  They
+// cover every pixel whose square meets the outer quad in this row, less those whose square lies inside the inner quad
+// by 1/16 px or more (all their samples are inside it: c = 0).  Floating point only decides which pixels are visited,
+// with a 1/16 px margin against its rounding; coverage itself is stroke_row_count's exact integer count.
+__host__ __device__ inline void stroke_row_spans(const Stroke &S, int Y, int dw, int seg[4]) {
+  const double y0 = 256.0 * Y, y1 = y0 + 256.0;
+  double lo = 1e300, hi = -1e300;
+  const StrokeQuad &o = S.q[0];
+  for (int i = 0; i < 4; ++i) {                       // each edge clipped to the band [y0, y1]
+    const double ay = (double)o.ay[i], by = (double)(o.ay[i] + o.dy[i]), ax = (double)o.ax[i], bx = (double)(o.ax[i] + o.dx[i]);
+    const double ylo = fmax(fmin(ay, by), y0), yhi = fmin(fmax(ay, by), y1);
+    if (ylo > yhi) continue;
+    if (ay == by) {
+      lo = fmin(lo, fmin(ax, bx)); hi = fmax(hi, fmax(ax, bx));
+    } else {
+      const double xa = ax + (ylo - ay) * (bx - ax) / (by - ay), xb = ax + (yhi - ay) * (bx - ax) / (by - ay);
+      lo = fmin(lo, fmin(xa, xb)); hi = fmax(hi, fmax(xa, xb));
+    }
+  }
+  seg[0] = 0; seg[1] = -1; seg[2] = 0; seg[3] = -1;
+  if (lo > hi) return;
+  const double a = floor((lo - 16.0) / 256.0), b = floor((hi + 16.0) / 256.0);
+  if (b < 0.0 || a > dw - 1.0) return;
+  seg[0] = a < 0.0 ? 0 : (int)a;
+  seg[1] = b > dw - 1.0 ? dw - 1 : (int)b;
+  double l0, r0, l1, r1;
+  if (S.n_q == 2 && stroke_cross(S.q[1], y0, l0, r0) && stroke_cross(S.q[1], y1, l1, r1)) {
+    const double sa = ceil((fmax(l0, l1) + 16.0) / 256.0), sb = floor((fmin(r0, r1) - 16.0) / 256.0) - 1.0;
+    if (sa <= sb && sb >= seg[0] && sa <= seg[1]) {
+      seg[2] = sb + 1.0 > seg[0] ? (int)sb + 1 : seg[0];
+      seg[3] = seg[1];
+      seg[1] = sa - 1.0 < seg[1] ? (int)sa - 1 : seg[1];
+    }
+  }
+}
+
+// Samples of sample row j of pixel (X, Y) inside quad q: edges that every sample of the row passes are skipped, the
+// others stepped sample by sample with adds.
+__host__ __device__ __forceinline__ int stroke_quad_row(const StrokeQuad &q, long long px, long long py) {
+  uint32_t m = 0xffffu;
+  for (int i = 0; i < 4; ++i) {
+    const long long b = q.bias[i], step = -16 * q.dy[i];
+    long long e = q.dx[i] * (py - q.ay[i]) - q.dy[i] * (px - q.ax[i]);
+    const long long e15 = e + 15 * step;
+    if (e >= b && e15 >= b) continue;
+    if (e < b && e15 < b) return 0;
+    uint32_t mk = 0;
+    for (int s = 0; s < 16; ++s) {
+      mk |= (uint32_t)(e >= b) << s;
+      e += step;
+    }
+    m &= mk;
+  }
+#ifdef __CUDA_ARCH__
+  return __popc(m);
+#else
+  return __builtin_popcount(m);
+#endif
+}
+
+// c of sample row j (0..15) of pixel (X, Y): samples at (X + (2i+1)/32, Y + (2j+1)/32) in the outer quad and not in the
+// inner one (which lies inside the outer).
+__host__ __device__ __forceinline__ int stroke_row_count(const Stroke &S, int X, int Y, int j) {
+  const long long px = 256LL * X + 8, py = 256LL * Y + 16 * j + 8;
+  int c = stroke_quad_row(S.q[0], px, py);
+  if (c && S.n_q == 2) c -= stroke_quad_row(S.q[1], px, py);
+  return c;
+}
+
+// Source-over of colour rgb at coverage c (1..256) onto one non-premultiplied RGBA pixel, rounding half up.
+__host__ __device__ __forceinline__ void stroke_blend(uint8_t *p, int c, uint32_t rgb) {
+  const uint32_t a = (255u * (uint32_t)c + 128u) >> 8;
+  const uint32_t d = *reinterpret_cast<const uint32_t *>(p), da = d >> 24;
+  const uint32_t A = a * 255u + da * (255u - a);
+  uint32_t o = ((A + 127u) / 255u) << 24;
+  for (int ch = 0; ch < 3; ++ch) {
+    const uint32_t s = (rgb >> (8 * ch)) & 0xffu, v = (d >> (8 * ch)) & 0xffu;
+    o |= ((s * a * 255u + v * da * (255u - a) + A / 2u) / A) << (8 * ch);
+  }
+  *reinterpret_cast<uint32_t *>(p) = o;
 }
 
 // One CTA per batch entry: the value table of each entry that ran track() (cs_en) on a stream with a debug canvas.
@@ -1487,6 +1716,42 @@ __global__ void k_camera_update(const int32_t *__restrict__ ids, const EntryCanv
   ht_camera cam = *c.camera;
   camera_step(cam, c, h.x, h.y, h.z);
   *c.camera = cam;
+}
+
+// After k_tracker_update (and k_debug_backproj, so CS strokes land on the back-projection): one CTA per batch entry
+// strokes its record (events[geo[k].record], geo NULL: k) onto its stream's debug canvas, if the stream has one and
+// strokes on (DebugCanvas::strokes).  Warp w walks rows y0 + w, y0 + w + 8, ... of the stroke; each half-warp takes one
+// visited pixel at a time, lane j its sample row j, and lane 0 of the half writes the pixel.
+__global__ void __launch_bounds__(256, 1) k_debug_strokes(const int32_t *__restrict__ ids, const EntryCanvas *__restrict__ geo,
+                                                       const TrackerEvent *__restrict__ events,
+                                                       const DebugCanvas *__restrict__ dbg) {
+  const int k = blockIdx.x;
+  const DebugCanvas d = dbg[ids ? ids[k] : k];
+  if (!d.rgba || !d.strokes) return;
+  __shared__ Stroke S;
+  __shared__ int draw;
+  if (threadIdx.x == 0) {
+    const TrackerEvent &e = events[geo ? geo[k].record : k];
+    draw = stroke_make(e.detection, e.confidence, e.x, e.y, e.width, e.height, e.angle, d.w, d.h, S);
+  }
+  __syncthreads();
+  if (!draw) return;
+  const int half = (threadIdx.x >> 4) & 1, j = threadIdx.x & 15;
+  for (int Y = S.y0 + (int)(threadIdx.x >> 5); Y < S.y1; Y += 8) {
+    int seg[4];
+    stroke_row_spans(S, Y, d.w, seg);
+    const int na = seg[1] - seg[0] + 1 > 0 ? seg[1] - seg[0] + 1 : 0, nb = seg[3] - seg[2] + 1 > 0 ? seg[3] - seg[2] + 1 : 0;
+    for (int p0 = 0; p0 < na + nb; p0 += 2) {
+      const int p = p0 + half;
+      const int X = p < na ? seg[0] + p : seg[2] + (p - na);
+      int c = p < na + nb ? stroke_row_count(S, X, Y, j) : 0;
+      c += __shfl_xor_sync(0xffffffffu, c, 8);
+      c += __shfl_xor_sync(0xffffffffu, c, 4);
+      c += __shfl_xor_sync(0xffffffffu, c, 2);
+      c += __shfl_xor_sync(0xffffffffu, c, 1);
+      if (j == 0 && c > 0) stroke_blend(d.rgba + (size_t)Y * d.pitch + 4 * (size_t)X, c, S.rgb);
+    }
+  }
 }
 
 // ht_tracker_set_camera: one CTA constructs the cameras of streams [first, first + n) that have a controller

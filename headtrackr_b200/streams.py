@@ -133,7 +133,8 @@ class TrackerSet:
     a list of n dicts, one per stream (each stream its own `new headtrackr.Tracker(params)`); set_params(k, params)
     changes one stream's.  A stream's "debug" key is its debug canvas, a torch CUDA uint8 (Dh, Dw, 4) tensor: the
     library puts the back-projection image of every "CS" tick on it, and debug_calls(k) gives the strokes main.js
-    draws on top.  No two streams may share a debug canvas.  A stream's "camera" key is its head-coupled camera
+    draws on top; with "debugStrokes": True the library also draws those strokes on the device (DESIGN.md 2,
+    "Strokes").  No two streams may share a debug canvas.  A stream's "camera" key is its head-coupled camera
     controller, a dict as Context.tracker_set_camera takes (realisticAbsoluteCameraControl on the device, written to
     its `out` tensor on every tick with a headtrackingEvent).
     Differs from the reference in one place: start() on a running stream does nothing (the reference runs an extra,
@@ -158,6 +159,9 @@ class TrackerSet:
         debug = [(p or {}).get("debug") for p in (params if per_stream else [params] * n_streams)]
         if any(d is not None for d in debug):      # after tracker_config, which clears every debug canvas
             context.tracker_set_debug(0, debug)
+        strokes = [bool((p or {}).get("debugStrokes")) for p in (params if per_stream else [params] * n_streams)]
+        if any(strokes):                           # and every stroke flag
+            context.tracker_set_debug_strokes(0, strokes)
         camera = [(p or {}).get("camera") for p in (params if per_stream else [params] * n_streams)]
         if any(c is not None for c in camera):     # likewise for camera controllers
             context.tracker_set_camera(0, camera)
@@ -169,6 +173,7 @@ class TrackerSet:
             raise ValueError(f"stream {k} outside [0, {self.n})")
         self.ctx.tracker_set_params(k, [_tracker_kwargs(params)])
         self.ctx.tracker_set_debug(k, [(params or {}).get("debug")])   # no "debug" key: none, as in the reference
+        self.ctx.tracker_set_debug_strokes(k, [bool((params or {}).get("debugStrokes"))])   # no key: off
         self.ctx.tracker_set_camera(k, [(params or {}).get("camera")])  # no "camera" key: none
 
     def addEventListener(self, fn):

@@ -448,9 +448,9 @@ typedef struct {
  * where current[bin] is 0), with this frame's histogram; the image is clipped to the debug canvas, and pixels outside
  * min(w, width) x min(h, height) keep what they held.  IDLE, STARTING, WB and VJ ticks (also the VJ tick that finds a
  * face) write nothing.  The canvas is never cleared, and survives stop, start, reset and a lost face, as main.js hands
- * one params.debug to every facetrackr it creates.  The strokes main.js draws on top (src/main.js:199-219) are not
- * rasterized: they are pure functions of the tick's ht_tracker_event (streams.debug_calls in the Python package).
- * The writes are enqueued on the context's stream before a tick's outputs: with host `out` they have landed when the
+ * one params.debug to every facetrackr it creates.  The strokes main.js draws on top (src/main.js:199-219) are drawn
+ * only for streams that turn them on (ht_tracker_set_debug_strokes); otherwise they are left to the caller, as pure
+ * functions of the tick's ht_tracker_event (streams.debug_calls in the Python package).  The writes are enqueued on the context's stream before a tick's outputs: with host `out` they have landed when the
  * tick returns, with device `out` after ht_sync or in stream order.  ht_tracker_config clears every stream's debug
  * canvas; ht_tracker_set_params does not.
  * Two streams may not share bytes of their debug canvases: the streams of one tick run concurrently and would race,
@@ -460,6 +460,19 @@ typedef struct {
  * canvas whose byte range overlaps another stream's (over all streams that have a canvas after the call);
  * HT_ERR_SIZE for a size outside 1..16384. */
 int ht_tracker_set_debug(ht_ctx *ctx, int first, int n, const ht_debug_canvas *canvases);
+
+/* Stream first+i strokes main.js's face rectangles onto its debug canvas (enable[i] == 1) or not (0), for i in
+ * [0, n).  After each tick, on top of that tick's back-projection, the library draws what src/main.js:199-219 strokes
+ * for the tick's ht_tracker_event: a "VJ" record with confidence != 0 strokes its box in #0000CC, a "CS" record with
+ * confidence != 0 its box rotated by angle - pi/2 about (x, y) in #00CC00 (a NaN angle: unrotated); other ticks draw
+ * nothing.  The raster is the one of DESIGN.md 2, "Strokes": lineWidth 1, miter joins, butt caps, 16 x 16 samples
+ * per pixel, non-premultiplied source-over, clipped to the canvas.  A stroke is a function of the record alone.
+ * The flag belongs to the stream: ht_tracker_set_debug keeps it (a stream without a canvas draws nothing),
+ * ht_tracker_config clears every stream's, ht_tracker_set_params, stop, start, reset and ht_tracker_import keep it.
+ * While no stream has both the flag and a canvas, a tick launches nothing for strokes.
+ * Errors (nothing changes): HT_ERR_STATE before ht_tracker_config; HT_ERR_ARG for a range outside [0, max_frames),
+ * n <= 0, enable NULL, or a value other than 0 and 1. */
+int ht_tracker_set_debug_strokes(ht_ctx *ctx, int first, int n, const int32_t *enable);
 
 /* A stream's head-coupled camera: the three.js r48 PerspectiveCamera that realisticAbsoluteCameraControl moves
  * (src/controllers.js:28-68), in caller-owned DEVICE memory that a renderer can bind directly.  Byte offsets:

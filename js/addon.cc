@@ -24,6 +24,7 @@
 //   trackerStep(handle, rgba /* n canvases */, n, w, h, nowMs) -> Array<{detection, status: [...], running, fov, ...}>
 //   trackerSetParams(handle, first, [params, ...])   (ht_tracker_set_params: each stream its own Tracker parameters)
 //   trackerSetDebug(handle, first, [canvas|null, ...])  (ht_tracker_set_debug: each stream's debug canvas, device memory)
+//   trackerSetDebugStrokes(handle, first, [bool, ...])  (ht_tracker_set_debug_strokes: main.js's strokes on the device)
 //   trackerSetCamera(handle, first, [control|null, ...])  (ht_tracker_set_camera: each stream's head-coupled camera,
 //        realisticAbsoluteCameraControl on an ht_camera in device memory)
 //   trackerExport(handle, [stream, ...]) -> Buffer of records; trackerImport(handle, [stream, ...], records)
@@ -451,6 +452,30 @@ static napi_value TrackerSetDebug(napi_env env, napi_callback_info info) {
   return nullptr;
 }
 
+// trackerSetDebugStrokes(handle, first, [bool, ...]): stream first+i strokes main.js's face rectangles onto its debug
+// canvas when flags[i] is truthy
+static napi_value TrackerSetDebugStrokes(napi_env env, napi_callback_info info) {
+  size_t argc = 3;
+  napi_value argv[3];
+  NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+  ht_ctx *ctx = Ctx(env, argv[0]);
+  int32_t first = 0;
+  uint32_t n = 0;
+  napi_get_value_int32(env, argv[1], &first);
+  NAPI_OK(napi_get_array_length(env, argv[2], &n));
+  std::vector<int32_t> flags(n, 0);
+  for (uint32_t i = 0; i < n; ++i) {
+    napi_value r, b;
+    bool on = false;
+    NAPI_OK(napi_get_element(env, argv[2], i, &r));
+    if (napi_coerce_to_bool(env, r, &b) == napi_ok) napi_get_value_bool(env, b, &on);
+    flags[i] = on ? 1 : 0;
+  }
+  int rc = ht_tracker_set_debug_strokes(ctx, first, (int)n, flags.data());
+  if (rc < 0) return Throw(env, ctx, rc);
+  return nullptr;
+}
+
 static double GetNumber(napi_env env, napi_value obj, const char *name, double dflt) {
   napi_value v;
   napi_valuetype t = napi_undefined;
@@ -862,6 +887,7 @@ static napi_value Init(napi_env env, napi_value exports) {
       {"trackerStep", nullptr, TrackerStep, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerSetParams", nullptr, TrackerSetParams, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerSetDebug", nullptr, TrackerSetDebug, nullptr, nullptr, nullptr, napi_default, nullptr},
+      {"trackerSetDebugStrokes", nullptr, TrackerSetDebugStrokes, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerSetCamera", nullptr, TrackerSetCamera, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerExport", nullptr, TrackerExport, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerImport", nullptr, TrackerImport, nullptr, nullptr, nullptr, napi_default, nullptr},

@@ -10,6 +10,9 @@ streams: N 640x480 streams, device-resident frames and outputs, CUDA events arou
                   one-size ht_tracker_feed against another build of the library (--before-lib) (canvas_arms)
   migrate_*       (--migrate) ht_tracker_export + ht_tracker_import of every stream, device to device and through
                   pinned host memory, and a steady tick before and after an import (migrate_arms)
+  strokes_*       (--strokes) ht_tracker_feed with a debug canvas on every stream and main.js's strokes on none,
+                  1/64 and all of them, k_debug_strokes's kernel time, and the strokes-off arm against --before-lib
+                  (strokes_arms)
   debug_*         (--debug-streams) ht_tracker_feed with debug canvases on none, 1/64 and all of the streams, the
                   achieved bandwidth of k_debug_backproj, and the no-debug arm against --before-lib (debug_arms)
   camera_*        (--camera-streams) ht_tracker_feed with head-coupled camera controllers on none, 1/64 and all of
@@ -198,6 +201,8 @@ def other_build_context(before_lib, **kw):
     L.ht_tracker_feed.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp]
     if hasattr(L, "ht_tracker_feed_yuv"):
         L.ht_tracker_feed_yuv.argtypes = [vp, vp, C.c_int, C.c_int, vp]
+    if hasattr(L, "ht_tracker_set_debug"):
+        L.ht_tracker_set_debug.argtypes = [vp, C.c_int, C.c_int, vp]
     saved = _lib.lib
     _lib.lib = lambda: L
     try:
@@ -438,6 +443,94 @@ def debug_arms(torch, frames, stream, N, W, H, steps, rounds, before_lib=None):
         res["k_debug_backproj_of_3.35TBps"] = rate / HBM_BYTES_PER_S
     if "k_debug_table" in kernel_us:
         res["k_debug_table_GBps"] = tab_bytes / (kernel_us["k_debug_table"] / steps * 1e-6) / 1e9
+    for c, _ in arms.values():
+        c.close()
+    return res
+
+
+def strokes_arms(torch, frames, stream, N, W, H, steps, rounds, before_lib=None):
+    """Strokes (ht_tracker_set_debug_strokes) in steady tracking: N streams of W x H device video fed onto W x H canvases
+    by ht_tracker_feed, every stream with a W x H debug canvas, every arm on its own context, all arms alternating
+    tick by tick (the arm order rotates), CUDA events around each tick:
+
+      strokes0_cs         no stream strokes (the tick launches what it launched before strokes)
+      strokes64_cs        every 64th stream strokes
+      strokesall_cs       every stream strokes
+      strokes0_before_cs  strokes0_cs with the library at `before_lib` (e.g. the parent commit's build)
+
+    Then, in a run of its own under torch.profiler, the kernel time of k_debug_strokes over `steps` ticks of
+    strokesall_cs.  The records of every arm must agree."""
+    import ctypes as C
+    from headtrackr_b200 import Context, _lib
+    rec_bytes = C.sizeof(_lib.TrackerEvent)
+    now = [1.0e12]
+    recs_arr = (_lib.VideoFrame * N)()
+    for k in range(N):
+        recs_arr[k] = _lib.VideoFrame(frames[k].data_ptr(), k, W, H, 0, 0.0)
+    kw = dict(max_width=W, max_height=H, max_frames=N, stream=stream)
+
+    def arm(every, before=False):
+        c = other_build_context(before_lib, **kw) if before else Context(**kw)
+        c.tracker_config()
+        c.tracker_reset(0, N)
+        c.tracker_start(0, N)
+        c.tracker_set_debug(0, [torch.zeros((H, W, 4), dtype=torch.uint8, device="cuda") for _ in range(N)])
+        if every:
+            c.tracker_set_debug_strokes(0, [k % every == 0 for k in range(N)])
+        return c, torch.empty(N * rec_bytes, dtype=torch.uint8, device="cuda")
+
+    arms = {"strokes0_cs": arm(0), "strokes64_cs": arm(64), "strokesall_cs": arm(1)}
+    if before_lib:
+        arms["strokes0_before_cs"] = arm(0, before=True)
+    names = list(arms)
+
+    def tick(name):
+        c, out = arms[name]
+        for k in range(N):
+            recs_arr[k].now_ms = now[0]
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        a.record()
+        c._check(c._L.ht_tracker_feed(c._h, C.addressof(recs_arr), N, 1, W, H, out.data_ptr()))
+        b.record()
+        b.synchronize()
+        return a.elapsed_time(b)
+
+    for _ in range(17):                          # the whitebalance gate, detection, the first CS frames
+        now[0] += 20.0
+        for name in names:
+            tick(name)
+    times = {name: [[] for _ in range(rounds)] for name in names}
+    for r in range(rounds):
+        for s in range(steps):
+            now[0] += 20.0
+            rot = (r * steps + s) % len(names)
+            for name in names[rot:] + names[:rot]:
+                times[name][r].append(tick(name))
+            first = arms[names[0]][1].cpu()
+            if any(not torch.equal(first, arms[name][1].cpu()) for name in names[1:]):
+                raise SystemExit("stroke arms disagree on the records of a timed tick")
+    res = {}
+    for name in names:
+        med = [float(np.median(t)) for t in times[name]]
+        res[f"{name}_ms"] = float(np.median(sum(times[name], [])))
+        res[f"{name}_spread_ms"] = max(med) - min(med)
+    ev = [_lib.TrackerEvent.from_buffer_copy(bytes(row))
+          for row in arms["strokesall_cs"][1].cpu().numpy().reshape(N, rec_bytes)]
+    res["strokes_cs_streams"] = sum(e.detection == 2 for e in ev)
+    res["strokes_records_agree"] = True
+
+    from torch.profiler import ProfilerActivity, profile
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(steps):
+            now[0] += 20.0
+            tick("strokesall_cs")
+        torch.cuda.synchronize()
+    us = 0.0
+    for e in prof.key_averages():
+        if "k_debug_strokes" in e.key:
+            t = getattr(e, "device_time_total", None)
+            us += t if t is not None else e.cuda_time_total
+    res["k_debug_strokes_ms"] = us / 1000.0 / steps
     for c, _ in arms.values():
         c.close()
     return res
@@ -1105,6 +1198,7 @@ def main():
     ap.add_argument("--before-lib", help="another build of libheadtrackr_b200.so for the one-size feed arm")
     ap.add_argument("--only-canvases", action="store_true", help="only the canvas arms (canvas_arms)")
     ap.add_argument("--debug-streams", action="store_true", help="only the debug-canvas arms (debug_arms)")
+    ap.add_argument("--strokes", action="store_true", help="only the debug-stroke arms (strokes_arms)")
     ap.add_argument("--migrate", action="store_true", help="only the tracker-record arms (migrate_arms)")
     ap.add_argument("--camera-streams", action="store_true", help="only the camera-controller arms (camera_arms)")
     ap.add_argument("--yuv", action="store_true", help="only the YUV video arms (yuv_arms)")
@@ -1137,6 +1231,9 @@ def main():
         return report(res, a.out)
     if a.camera_streams:
         res.update(camera_arms(torch, frames, stream, N, W, H, a.steps, a.rounds, a.before_lib))
+        return report(res, a.out)
+    if a.strokes:
+        res.update(strokes_arms(torch, frames, stream, N, W, H, a.steps, a.rounds, a.before_lib))
         return report(res, a.out)
     if a.debug_streams:
         res.update(debug_arms(torch, frames, stream, N, W, H, a.steps, a.rounds, a.before_lib))
