@@ -8,7 +8,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from ._lib import (Camera, CameraControl, CanvasFrame, DebugCanvas, HeadEvent, HeadParams, HtError, Rect, StreamEvent, TrackerEvent, TrackerParams, TrackObj, VideoFrame,
+from ._lib import (Camera, CameraControl, CanvasFrame, DebugCanvas, FaceCrop, HeadEvent, HeadParams, HtError, Rect, StreamEvent, TrackerEvent, TrackerParams, TrackObj, VideoFrame,
                    VideoView, Window, YuvFrame, YuvImage)
 from .views import video_view
 from .synth import load_cascade_blob
@@ -176,6 +176,7 @@ class Context:
         self.last_warning = None
         self._debug = {}                  # stream -> its debug canvas tensor, kept alive while the library writes it
         self._camera = {}                 # stream -> its camera tensor, likewise
+        self._crops = {}                  # stream -> its face crop tensor, likewise
 
     def close(self):
         if getattr(self, "_h", None) and self._h.value:
@@ -349,12 +350,14 @@ class Context:
             self._check(self._L.ht_tracker_config(self._h, None))
             self._debug = {}
             self._camera = {}
+            self._crops = {}
             return
         p = tracker_params(retryDetection, calcAngles, smoothing, fov, cameraOffset, headPosition, edgecorrection, alpha,
                            distance_to_screen)
         self._check(self._L.ht_tracker_config(self._h, C.addressof(p)))
         self._debug = {}                  # ht_tracker_config discards every debug canvas
         self._camera = {}                 # and every camera controller
+        self._crops = {}                  # and every face crop
 
     def tracker_set_params(self, first, params):
         """Parameters of streams first, first+1, ...: one dict of tracker_config's keywords (enable excluded) per stream,
@@ -395,6 +398,32 @@ class Context:
         flags = [bool(f) for f in flags]
         arr = (C.c_int32 * max(1, len(flags)))(*[int(f) for f in flags])
         self._check(self._L.ht_tracker_set_debug_strokes(self._h, int(first), len(flags), arr))
+
+    def tracker_set_face_crop(self, first, crops):
+        """Face crops of streams first, first+1, ... (ht_tracker_set_face_crop): per stream None (none) or a dict
+        {"out": torch CUDA uint8 (S_h, S_w, 4) tensor, "scale": 1.0}; a row-padded view - last two strides (4, 1) -
+        passes its row stride as the pitch.  After every tick on which track() kept the face ("CS", width and height
+        > 0), `out` holds the green rectangle main.js strokes, scaled by `scale` about its centre and grown to the
+        crop's aspect ratio, cut upright out of the tick's video at video resolution (DESIGN.md 2, "Face crops").  The
+        crop is the stream's: it outlives set_params, stop, start, reset and import; tracker_config removes it.  The
+        context keeps the tensors alive while they are set."""
+        crops = list(crops)
+        arr = (FaceCrop * max(1, len(crops)))()
+        for i, c in enumerate(crops):
+            if c is None:
+                continue
+            t = c["out"]
+            if not _is_torch(t) or not t.is_cuda:
+                raise ValueError("a face crop is a torch CUDA tensor")
+            if t.dim() != 3 or t.element_size() != 1 or t.shape[2] != 4 or t.stride(2) != 1 or t.stride(1) != 4:
+                raise ValueError("face crops must be uint8 (S_h, S_w, 4) with strides (pitch, 4, 1)")
+            arr[i] = FaceCrop(t.data_ptr(), t.shape[1], t.shape[0], t.stride(0), 0, float(c.get("scale", 1.0)))
+        self._check(self._L.ht_tracker_set_face_crop(self._h, int(first), len(crops), C.addressof(arr)))
+        for i, c in enumerate(crops):
+            if c is None:
+                self._crops.pop(int(first) + i, None)
+            else:
+                self._crops[int(first) + i] = c["out"]
 
     def tracker_set_camera(self, first, controls):
         """Head-coupled camera controllers of streams first, first+1, ...: per stream None (none) or a dict of

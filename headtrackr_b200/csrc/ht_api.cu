@@ -582,6 +582,11 @@ struct ht_ctx {
   DevBuf d_camera;
   std::vector<CameraCtl> h_camera;
   int camera_count = 0;
+  // ht_tracker_set_face_crop: per stream its FaceCrop (device array and host copy), the number of streams that have
+  // one (0: a tick launches no k_face_crop) and the tiles of the largest (k_face_crop's grid.x)
+  DevBuf d_crop;
+  std::vector<FaceCrop> h_crop;
+  int crop_count = 0, crop_tiles = 0;
   // ht_tracker_feed(_canvases): the record table {ids[n], clocks[n], FeedRec[n], EntryCanvas[n], tile starts[n+1]}
   // goes up in one copy from pinned memory; the videos are drawn into the canvas arena (batch entry k's canvas at
   // EntryCanvas::base), zeroed when it grows
@@ -1758,6 +1763,11 @@ int ht_tracker_config(ht_ctx *ctx, const ht_tracker_params *params) {
     ctx->h_camera.assign(mf, CameraCtl{});
     ctx->camera_count = 0;
   }
+  if (ctx->crop_count > 0) {     // and every face crop
+    CK(cudaMemsetAsync(ctx->d_crop.p, 0, mf * sizeof(FaceCrop), ctx->stream));
+    ctx->h_crop.assign(mf, FaceCrop{});
+    ctx->crop_count = ctx->crop_tiles = 0;
+  }
   if (!params) {                 // off: every stream as after ht_stream_reset (the lifecycle has used the tracker slots)
     if (ctx->tracker_on) {
       ctx->tracker_on = false;
@@ -1836,6 +1846,24 @@ static int debug_commit(ht_ctx *ctx, int first, int n, std::vector<DebugCanvas> 
   return HT_OK;
 }
 
+// Whether two of the images written during a tick - every debug canvas and every face crop - share a byte: the streams
+// of a tick run concurrently.
+static bool images_overlap(const std::vector<DebugCanvas> &dbg, const std::vector<FaceCrop> &crops) {
+  std::vector<std::pair<uintptr_t, uintptr_t>> spans;
+  auto add = [&](const uint8_t *p, int w, int h, int pitch) {
+    const uintptr_t s = reinterpret_cast<uintptr_t>(p);
+    spans.emplace_back(s, s + (size_t)(h - 1) * pitch + 4 * (size_t)w);
+  };
+  for (const DebugCanvas &d : dbg)
+    if (d.rgba) add(d.rgba, d.w, d.h, d.pitch);
+  for (const FaceCrop &f : crops)
+    if (f.rgba) add(f.rgba, f.w, f.h, f.pitch);
+  std::sort(spans.begin(), spans.end());
+  for (size_t i = 1; i < spans.size(); ++i)
+    if (spans[i].first < spans[i - 1].second) return true;
+  return false;
+}
+
 // The debug canvases of streams [first, first + n).  Everything is checked on the host before anything changes,
 // overlap over every stream that has a canvas after the call.
 int ht_tracker_set_debug(ht_ctx *ctx, int first, int n, const ht_debug_canvas *canvases) {
@@ -1872,6 +1900,8 @@ int ht_tracker_set_debug(ht_ctx *ctx, int first, int n, const ht_debug_canvas *c
   for (size_t i = 1; i < spans.size(); ++i)
     if (spans[i].first < spans[i - 1].second)
       return ctx->fail(HT_ERR_ARG, "a debug canvas overlaps another stream's debug canvas");
+  if (ctx->crop_count > 0 && images_overlap(next, ctx->h_crop))
+    return ctx->fail(HT_ERR_ARG, "a debug canvas overlaps a face crop");
   return debug_commit(ctx, first, n, next);
 }
 
@@ -1889,6 +1919,87 @@ int ht_tracker_set_debug_strokes(ht_ctx *ctx, int first, int n, const int32_t *e
   next.resize((size_t)mf, DebugCanvas{});
   for (int i = 0; i < n; ++i) next[(size_t)(first + i)].strokes = enable[i];
   return debug_commit(ctx, first, n, next);
+}
+
+static_assert(sizeof(ht_face_crop) == 32 && sizeof(FaceCrop) == sizeof(ht_face_crop) &&
+                  offsetof(ht_face_crop, pitch) == offsetof(FaceCrop, pitch) &&
+                  offsetof(ht_face_crop, scale) == offsetof(FaceCrop, scale),
+              "ht_face_crop layout");
+
+// The face crops of streams [first, first + n).  Everything is checked on the host before anything changes, overlap
+// over every crop and debug canvas after the call.
+int ht_tracker_set_face_crop(ht_ctx *ctx, int first, int n, const ht_face_crop *crops) {
+  if (!ctx) return HT_ERR_ARG;
+  if (!ctx->tracker_on) return ctx->fail(HT_ERR_STATE, "ht_tracker_config has not been called");
+  const int mf = ctx->cfg.max_frames;
+  if (first < 0 || n <= 0 || first > mf - n) return ctx->fail(HT_ERR_ARG, "stream range outside [0,%d)", mf);
+  if (!crops) return ctx->fail(HT_ERR_ARG, "crops is NULL");
+  std::vector<FaceCrop> next = ctx->h_crop;
+  next.resize((size_t)mf, FaceCrop{});
+  for (int i = 0; i < n; ++i) {
+    const ht_face_crop &c = crops[i];
+    FaceCrop f{};
+    if (c.rgba) {
+      if (reinterpret_cast<uintptr_t>(c.rgba) & 3u) return ctx->fail(HT_ERR_ARG, "record %d: rgba must be 4-byte aligned", i);
+      if (!is_device_ptr(c.rgba)) return ctx->fail(HT_ERR_ARG, "record %d: rgba is not device memory", i);
+      if (c.width < 1 || c.height < 1 || c.width > 2048 || c.height > 2048)
+        return ctx->fail(HT_ERR_SIZE, "record %d: face crop %dx%d outside 1..2048", i, c.width, c.height);
+      if ((c.pitch & 3) || (c.pitch != 0 && c.pitch < 4 * c.width))
+        return ctx->fail(HT_ERR_ARG, "record %d: pitch %d is not a multiple of 4 >= 4*width", i, c.pitch);
+      if (!(c.scale > 0.0 && c.scale <= 16.0)) return ctx->fail(HT_ERR_ARG, "record %d: scale %g outside (0, 16]", i, c.scale);
+      f = FaceCrop{c.rgba, c.width, c.height, c.pitch ? c.pitch : 4 * c.width, 0, c.scale};
+    }
+    next[(size_t)(first + i)] = f;
+  }
+  if (images_overlap(ctx->h_debug, next))
+    return ctx->fail(HT_ERR_ARG, "a face crop overlaps another stream's face crop or a debug canvas");
+  { const int jr = join_aux(ctx); if (jr != HT_OK) return jr; }
+  CK(cudaSetDevice(ctx->cfg.device));
+  if (!ctx->d_crop.p) {
+    CK(ctx->d_crop.reserve((size_t)mf * sizeof(FaceCrop)));
+    CK(cudaMemsetAsync(ctx->d_crop.p, 0, (size_t)mf * sizeof(FaceCrop), ctx->stream));
+  }
+  CK(cudaMemcpyAsync(ctx->d_crop.as<FaceCrop>() + first, next.data() + first, (size_t)n * sizeof(FaceCrop),
+                     cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));    // `next` is a local
+  ctx->crop_count = ctx->crop_tiles = 0;
+  for (const FaceCrop &f : next)
+    if (f.rgba) {
+      ++ctx->crop_count;
+      ctx->crop_tiles = std::max(ctx->crop_tiles, ((f.w + CROP_TX - 1) / CROP_TX) * ((f.h + CROP_TY - 1) / CROP_TY));
+    }
+  ctx->h_crop.swap(next);
+  return HT_OK;
+}
+
+static int view_record(const ht_video_view &view, int w, int h, ViewFeedRec &v, char *why);
+
+// The map k_face_crop uses for `ev`, in the video's tap coordinates: crop_map's values in the source rectangle, taken
+// through the view's signed permutation exactly.
+int ht_face_crop_map(const ht_tracker_event *ev, int canvas_w, int canvas_h, int video_w, int video_h,
+                     const ht_video_view *view, const ht_face_crop *crop, int64_t out[6]) {
+  if (!ev || !crop || !out) return HT_ERR_ARG;
+  if (canvas_w < 1 || canvas_h < 1 || canvas_w > 16384 || canvas_h > 16384 || video_w < 1 || video_h < 1 ||
+      video_w > 16384 || video_h > 16384 || crop->width < 1 || crop->height < 1 || crop->width > 2048 || crop->height > 2048)
+    return HT_ERR_SIZE;
+  if (!(crop->scale > 0.0 && crop->scale <= 16.0)) return HT_ERR_ARG;
+  const ht_video_view whole{};
+  ViewFeedRec v{};
+  char why[256];
+  if (view_record(view ? *view : whole, video_w, video_h, v, why) != HT_OK) return HT_ERR_ARG;
+  const TrackerEvent &e = *reinterpret_cast<const TrackerEvent *>(ev);
+  long long M[6];
+  for (int i = 0; i < 6; ++i) out[i] = 0;
+  if (!crop_map(e.detection, e.x, e.y, e.width, e.height, e.angle, canvas_w, canvas_h, v.sw, v.sh, crop->width, crop->height,
+                crop->scale, M))
+    return 0;
+  out[0] = 65536LL * v.bx + v.mxx * M[0] + v.mxy * M[1];
+  out[1] = 65536LL * v.by + v.myx * M[0] + v.myy * M[1];
+  for (int s = 2; s < 6; s += 2) {
+    out[s] = v.mxx * M[s] + v.mxy * M[s + 1];
+    out[s + 1] = v.myx * M[s] + v.myy * M[s + 1];
+  }
+  return 1;
 }
 
 static_assert(sizeof(ht_camera) == HT_CAMERA_BYTES && HT_CAMERA_BYTES == 224 && offsetof(ht_camera, fov) == 24 &&
@@ -2199,6 +2310,15 @@ static int tracker_tick(ht_ctx *ctx, const TickGroup *grp, int n_groups, const u
   }
   if (ctx->stroke_count > 0) {   // main.js's strokes, after this tick's back-projections (src/main.js:199-219)
     k_debug_strokes<<<(unsigned)n, 256, 0, st>>>(d_ids, geo, d_ev, ctx->d_debug.as<DebugCanvas>());
+    ++ctx->launches;
+  }
+  if (ctx->crop_count > 0) {     // the face crops of the entries whose record is a kept "CS" face, from this tick's video
+    CropSource src{CROP_FRAMES, g0.w, g0.h, 0, d_rgba};     // ht_tracker_step: the frames are the canvases
+    if (feed && feed->view) src = CropSource{CROP_VIEW, 0, 0, 0, feed->view};
+    else if (feed && feed->yuv) src = CropSource{CROP_YUV, 0, 0, 0, feed->yuv};
+    else if (feed) src = CropSource{CROP_FEED, 0, 0, 0, feed->recs};
+    k_face_crop<<<dim3((unsigned)ctx->crop_tiles, (unsigned)n), 256, 0, st>>>(d_ids, geo, g0.w, g0.h, d_ev,
+                                                                              ctx->d_crop.as<FaceCrop>(), src);
     ++ctx->launches;
   }
   ctx->prof_begin(HT_PROF_TRACK_INIT, st);
@@ -3269,6 +3389,45 @@ extern "C" int ht_selftest_feed_view_rgba(const ht_video_frame *f, const ht_vide
   if (rc != HT_OK) return rc;
   view_source_rgba(v, f->rgba, f->pitch ? f->pitch : 4 * f->width, f->width, f->height);
   return selftest_view_draw(v, canvas, dw, dh);
+}
+
+// k_face_crop's per-crop code: the crop of record `ev` on a cw x ch canvas drawn from view record v (map and texel
+// source resolved) -> 1 if the record wrote the crop, 0 if not
+static int selftest_face_crop(const ht_tracker_event *ev, int cw, int ch, const ViewFeedRec &v, const ht_face_crop *crop) {
+  const TrackerEvent &e = *reinterpret_cast<const TrackerEvent *>(ev);
+  const FaceCrop f{crop->rgba, crop->width, crop->height, crop->pitch ? crop->pitch : 4 * crop->width, 0, crop->scale};
+  long long M[6];
+  if (!crop_map(e.detection, e.x, e.y, e.width, e.height, e.angle, cw, ch, v.sw, v.sh, f.w, f.h, f.scale, M)) return 0;
+  for (int j = 0; j < f.h; ++j)
+    for (int i = 0; i < f.w; ++i)
+      reinterpret_cast<uint32_t *>(f.rgba + (size_t)j * f.pitch)[i] =
+          v.kind == VIEW_RGBA ? crop_pixel<VIEW_RGBA>(v, M, i, j)
+          : v.kind == VIEW_NV12_I420 ? crop_pixel<VIEW_NV12_I420>(v, M, i, j) : crop_pixel<VIEW_FMT>(v, M, i, j);
+  return 1;
+}
+// ... of an image of any format (host planes) through a view (NULL: the whole frame upright)
+extern "C" int ht_selftest_face_crop(const ht_tracker_event *ev, int cw, int ch, const ht_yuv_image *img,
+                                     const ht_video_view *view, const ht_face_crop *crop) {
+  YuvFeedRec r;
+  ViewFeedRec v;
+  char why[256];
+  const ht_video_view whole{};
+  int rc = yuv_record(*img, r, why);
+  if (rc == HT_OK) rc = view_record(view ? *view : whole, img->width, img->height, v, why);
+  if (rc != HT_OK) return rc;
+  view_source_yuv(v, r);
+  return selftest_face_crop(ev, cw, ch, v, crop);
+}
+// ... of an RGBA8 frame of rows of `pitch` bytes (0: 4 * width)
+extern "C" int ht_selftest_face_crop_rgba(const ht_tracker_event *ev, int cw, int ch, const ht_video_frame *f,
+                                          const ht_video_view *view, const ht_face_crop *crop) {
+  ViewFeedRec v;
+  char why[256];
+  const ht_video_view whole{};
+  const int rc = view_record(view ? *view : whole, f->width, f->height, v, why);
+  if (rc != HT_OK) return rc;
+  view_source_rgba(v, f->rgba, f->pitch ? f->pitch : 4 * f->width, f->width, f->height);
+  return selftest_face_crop(ev, cw, ch, v, crop);
 }
 
 // k_ingest's per-pixel code over a whole frame batch

@@ -1754,6 +1754,156 @@ __global__ void __launch_bounds__(256, 1) k_debug_strokes(const int32_t *__restr
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// Face crops (ht_tracker_set_face_crop; DESIGN.md 2, "Face crops"): after a tick whose record is "CS" with width > 0
+// and height > 0, the rectangle main.js strokes in green, scaled about its centre, grown to the crop's aspect ratio and
+// resampled upright from the tick's video at video resolution.
+// Layout of ht_face_crop, with the pitch resolved; rgba NULL: the stream has none.
+struct FaceCrop {
+  uint8_t *rgba;
+  int32_t w, h, pitch, pad_;
+  double scale;
+};
+constexpr int CROP_TX = 64, CROP_TY = 16;        // crop pixels per tile of k_face_crop
+
+__host__ __device__ __forceinline__ double sk_div(double a, double b) {
+#ifdef __CUDA_ARCH__
+  return __ddiv_rn(a, b);
+#else
+  return a / b;
+#endif
+}
+
+// The crop map of one record: M = {U0, V0, Ui, Vi, Uj, Vj}, so that crop pixel (i, j) samples tap coordinates
+// (U0 + i Ui + j Uj, V0 + i Vi + j Vj) / 65536 of the sw x sh source rectangle (the whole video without a view) that a
+// cw x ch canvas is drawn from.  fp64 in this order, every operation rounded as written, then each value quantised
+// with floor(v 65536 + 1/2).  Records that are not "CS" with width > 0 and height > 0 make no crop; neither do boxes
+// with a field that is not finite or beyond 65536 px (the tracker produces none), which also keeps every tap
+// coordinate of a 2048 x 2048 crop within int64.  -> whether the record makes a crop.
+__host__ __device__ inline bool crop_map(int detection, double x, double y, double w, double h, double angle, int cw, int ch,
+                                         int sw, int sh, int Sw, int Sh, double scale, long long M[6]) {
+  if (detection != 2 || !(w > 0.0) || !(h > 0.0)) return false;
+  const double f[4] = {x, y, w, h};
+  for (int i = 0; i < 4; ++i)
+    if (!(fabs(f[i]) <= 65536.0)) return false;
+  double s, c;
+  stroke_sincos(sk_add(angle, -1.5707963267948966), s, c);
+  const double rx = trunc(-(w / 2)), ry = trunc(-(h / 2));           // as main.js strokes it (DESIGN.md 2, "Strokes")
+  const double cx = sk_add(rx, sk_mul(w, 0.5)), cy = sk_add(ry, sk_mul(h, 0.5));
+  double hw = sk_mul(sk_mul(w, scale), 0.5), hh = sk_mul(sk_mul(h, scale), 0.5);
+  const double aw = sk_mul(hw, (double)Sh), ah = sk_mul(hh, (double)Sw);
+  if (aw < ah) hw = sk_div(ah, (double)Sh);                            // the shorter side grows to S_w : S_h
+  else if (ah < aw) hh = sk_div(aw, (double)Sw);
+  const double px = sk_div(sk_mul(hw, 2.0), (double)Sw), py = sk_div(sk_mul(hh, 2.0), (double)Sh);
+  const double lx = sk_add(sk_add(cx, -hw), sk_mul(px, 0.5)), ly = sk_add(sk_add(cy, -hh), sk_mul(py, 0.5));
+  const double X = sk_add(x, sk_add(sk_mul(c, lx), -sk_mul(s, ly)));
+  const double Y = sk_add(y, sk_add(sk_mul(s, lx), sk_mul(c, ly)));
+  const double kx = sk_div((double)sw, (double)cw), ky = sk_div((double)sh, (double)ch);
+  const double v[6] = {sk_add(sk_mul(X, kx), -0.5), sk_add(sk_mul(Y, ky), -0.5), sk_mul(sk_mul(c, px), kx),
+                       sk_mul(sk_mul(s, px), ky),   sk_mul(-sk_mul(s, py), kx),  sk_mul(sk_mul(c, py), ky)};
+  for (int i = 0; i < 6; ++i) M[i] = (long long)floor(sk_add(sk_mul(v[i], 65536.0), 0.5));
+  return true;
+}
+
+// Crop pixel (i, j) of the map M over view record v (map, source rectangle and texel source resolved): bilinear with
+// 8-bit weights between the taps (U >> 16, V >> 16) and their right and lower neighbours, taken in the rectangle and
+// mapped to the video through the view, so a turned or mirrored video samples the same taps with the same weights as
+// its upright twin.  A tap outside the rectangle reads (0, 0, 0, 0).
+template <int KIND>
+__host__ __device__ __forceinline__ uint32_t crop_pixel(const ViewFeedRec &v, const long long M[6], int i, int j) {
+  const long long U = M[0] + (long long)i * M[2] + (long long)j * M[4], V = M[1] + (long long)i * M[3] + (long long)j * M[5];
+  const long long x0 = U >> 16, y0 = V >> 16;
+  const uint32_t fx = (uint32_t)(U >> 8) & 255u, fy = (uint32_t)(V >> 8) & 255u;
+  auto tap = [&](long long x, long long y) -> uint32_t {
+    if (x < 0 || y < 0 || x >= v.sw || y >= v.sh) return 0u;
+    const int xi = (int)x, yi = (int)y;
+    return view_texel<KIND>(v.src, v.bx + v.mxx * xi + v.mxy * yi, v.by + v.myx * xi + v.myy * yi);
+  };
+  const uint32_t p00 = tap(x0, y0), p01 = tap(x0 + 1, y0), p10 = tap(x0, y0 + 1), p11 = tap(x0 + 1, y0 + 1);
+  const uint32_t w00 = (256u - fx) * (256u - fy), w01 = fx * (256u - fy), w10 = (256u - fx) * fy, w11 = fx * fy;
+  uint32_t out = 0;
+#pragma unroll
+  for (int ch = 0; ch < 4; ++ch) {
+    const uint32_t num = w00 * byte_of(p00, ch) + w01 * byte_of(p01, ch) + w10 * byte_of(p10, ch) + w11 * byte_of(p11, ch);
+    out |= ((num + 32768u) >> 16) << (8 * ch);
+  }
+  return out;
+}
+
+// The video of batch entry k as a view record: the tick's frames (ht_tracker_step: frame k, one canvas size, 1:1),
+// or the feed table's record k as k_feed_draw / k_feed_draw_yuv / k_feed_draw_view drew it.
+enum : int32_t { CROP_FRAMES = 0, CROP_FEED = 1, CROP_YUV = 2, CROP_VIEW = 3 };
+struct CropSource {
+  int32_t mode, fw, fh, pad_;          // CROP_*; the frames' size
+  const void *recs;                    // FeedRec / YuvFeedRec / ViewFeedRec table, or the frames
+};
+__device__ __forceinline__ void crop_source(const CropSource &s, int k, ViewFeedRec &v) {
+  if (s.mode == CROP_VIEW) { v = reinterpret_cast<const ViewFeedRec *>(s.recs)[k]; return; }
+  v.src = YuvFeedRec{};
+  v.bx = v.by = v.mxy = v.myx = 0;
+  v.mxx = v.myy = 1;
+  v.pad_ = 0;
+  if (s.mode == CROP_YUV) {
+    v.src = reinterpret_cast<const YuvFeedRec *>(s.recs)[k];
+    v.kind = nv12_i420_path(v.src) ? VIEW_NV12_I420 : VIEW_FMT;
+  } else if (s.mode == CROP_FEED) {
+    const FeedRec r = reinterpret_cast<const FeedRec *>(s.recs)[k];
+    v.src.y = r.src, v.src.ypitch = r.pitch, v.src.width = r.width, v.src.height = r.height;
+    v.kind = VIEW_RGBA;
+  } else {
+    v.src.y = reinterpret_cast<const uint8_t *>(s.recs) + (size_t)k * s.fw * s.fh * 4;
+    v.src.ypitch = 4 * s.fw, v.src.width = s.fw, v.src.height = s.fh;
+    v.kind = VIEW_RGBA;
+  }
+  v.sw = v.src.width, v.sh = v.src.height;
+}
+
+// One 64 x 16 tile from (X0, Y0) of crop f: a warp writes 128 consecutive bytes of a crop row.  Out of line per texel
+// source, as feed_draw_view, so that each keeps its own registers.
+template <int KIND>
+__device__ __noinline__ void face_crop_tile(const ViewFeedRec *__restrict__ vp, const long long *__restrict__ Mp,
+                                            const FaceCrop f, int X0, int Y0) {
+  const ViewFeedRec v = *vp;
+  long long M[6];
+#pragma unroll
+  for (int i = 0; i < 6; ++i) M[i] = Mp[i];
+  const int X = X0 + (threadIdx.x & 63);
+  if (X >= f.w) return;
+#pragma unroll
+  for (int r = 0; r < 4; ++r) {
+    const int Y = Y0 + 4 * r + (threadIdx.x >> 6);
+    if (Y < f.h) reinterpret_cast<uint32_t *>(f.rgba + (size_t)Y * f.pitch)[X] = crop_pixel<KIND>(v, M, X, Y);
+  }
+}
+
+// After k_tracker_update: grid (tiles of the largest crop, batch entries).  Entry k's CTAs read its record
+// (events[geo[k].record], geo NULL: k) and canvas size (geo[k], geo NULL: cw x ch), and write the tiles of its stream's
+// crop on a crop tick; entries without a crop, without a crop tick, or past their own crop's tiles exit at once.
+__global__ void __launch_bounds__(256) k_face_crop(const int32_t *__restrict__ ids, const EntryCanvas *__restrict__ geo,
+                                                   int cw, int ch, const TrackerEvent *__restrict__ events,
+                                                   const FaceCrop *__restrict__ crops, CropSource src) {
+  const int k = blockIdx.y;
+  const FaceCrop f = crops[ids ? ids[k] : k];
+  if (!f.rgba) return;
+  const int tiles_x = (f.w + CROP_TX - 1) / CROP_TX;
+  if ((int)blockIdx.x >= tiles_x * ((f.h + CROP_TY - 1) / CROP_TY)) return;
+  __shared__ ViewFeedRec v;
+  __shared__ long long M[6];
+  __shared__ int on;
+  if (threadIdx.x == 0) {
+    crop_source(src, k, v);
+    const TrackerEvent &e = events[geo ? geo[k].record : k];
+    on = crop_map(e.detection, e.x, e.y, e.width, e.height, e.angle, geo ? geo[k].w : cw, geo ? geo[k].h : ch, v.sw, v.sh,
+                  f.w, f.h, f.scale, M);
+  }
+  __syncthreads();
+  if (!on) return;
+  const int X0 = ((int)blockIdx.x % tiles_x) * CROP_TX, Y0 = ((int)blockIdx.x / tiles_x) * CROP_TY;
+  if (v.kind == VIEW_RGBA) face_crop_tile<VIEW_RGBA>(&v, M, f, X0, Y0);
+  else if (v.kind == VIEW_NV12_I420) face_crop_tile<VIEW_NV12_I420>(&v, M, f, X0, Y0);
+  else face_crop_tile<VIEW_FMT>(&v, M, f, X0, Y0);
+}
+
 // ht_tracker_set_camera: one CTA constructs the cameras of streams [first, first + n) that have a controller
 __global__ void k_camera_construct(const CameraCtl *__restrict__ ctl, int first, int n) {
   for (int i = threadIdx.x; i < n; i += blockDim.x) {

@@ -136,7 +136,9 @@ class TrackerSet:
     draws on top; with "debugStrokes": True the library also draws those strokes on the device (DESIGN.md 2,
     "Strokes").  No two streams may share a debug canvas.  A stream's "camera" key is its head-coupled camera
     controller, a dict as Context.tracker_set_camera takes (realisticAbsoluteCameraControl on the device, written to
-    its `out` tensor on every tick with a headtrackingEvent).
+    its `out` tensor on every tick with a headtrackingEvent).  A stream's "faceCrop" key is its face crop, a dict as
+    Context.tracker_set_face_crop takes: the tracked face cut upright out of the video into its `out` tensor on every
+    tick that keeps the face.
     Differs from the reference in one place: start() on a running stream does nothing (the reference runs an extra,
     unscheduled pass)."""
 
@@ -165,6 +167,9 @@ class TrackerSet:
         camera = [(p or {}).get("camera") for p in (params if per_stream else [params] * n_streams)]
         if any(c is not None for c in camera):     # likewise for camera controllers
             context.tracker_set_camera(0, camera)
+        crops = [(p or {}).get("faceCrop") for p in (params if per_stream else [params] * n_streams)]
+        if any(c is not None for c in crops):      # and face crops
+            context.tracker_set_face_crop(0, crops)
 
     def set_params(self, k, params):
         """The parameters of stream k (a dict as for the constructor).  Its state is kept: calcAngles takes effect at
@@ -175,6 +180,7 @@ class TrackerSet:
         self.ctx.tracker_set_debug(k, [(params or {}).get("debug")])   # no "debug" key: none, as in the reference
         self.ctx.tracker_set_debug_strokes(k, [bool((params or {}).get("debugStrokes"))])   # no key: off
         self.ctx.tracker_set_camera(k, [(params or {}).get("camera")])  # no "camera" key: none
+        self.ctx.tracker_set_face_crop(k, [(params or {}).get("faceCrop")])   # no "faceCrop" key: none
 
     def addEventListener(self, fn):
         """fn(stream_index, evt): evt is a headtrackrStatus / facetrackingEvent / headtrackingEvent payload dict."""

@@ -8,9 +8,10 @@ coordinates of the video as it sits in memory, e.g. to draw an overlay on the de
 
 Coordinates here are continuous: pixel (x, y) covers [x, x + 1) x [y, y + 1), so its centre is (x + 0.5, y + 0.5).
 """
+import ctypes as C
 import math
 
-from ._lib import HT_VIEW_MIRROR, VideoView
+from ._lib import HT_VIEW_MIRROR, FaceCrop, TrackerEvent, VideoView, lib
 
 # EXIF orientation tag (1..8) -> view orientation; a tag says how to turn the stored image to show it upright
 EXIF_ORIENTATION = {1: 0, 2: 4, 3: 2, 4: 6, 5: 5, 6: 1, 7: 7, 8: 3}
@@ -115,3 +116,41 @@ def cs_to_video(view, width, height, canvas_w, canvas_h, x, y, w, h, angle):
     if a >= math.pi:
         a -= math.pi
     return cx, cy, w * lw, h * lh, a
+
+
+def crop_map(view, width, height, canvas_w, canvas_h, record, crop_w, crop_h, scale=1.0):
+    """ht_face_crop_map: the exact fixed-point map (U0, V0, Ui, Vi, Uj, Vj) of a crop_w x crop_h face crop for a
+    tracker record (a dict with detection "CS" / 2, x, y, width, height, angle, or an ht_tracker_event), on a
+    canvas_w x canvas_h canvas drawn from a width x height video through `view`; crop pixel (i, j) samples video tap
+    coordinates (U0 + i Ui + j Uj, V0 + i Vi + j Vj) / 65536 (tap u is pixel centre u + 0.5).  -> None when the
+    record makes no crop."""
+    if isinstance(record, TrackerEvent):
+        ev = record
+    else:
+        ev = TrackerEvent()
+        det = record.get("detection", 0)
+        ev.detection = {"VJ": 1, "CS": 2}.get(det, 0) if isinstance(det, str) else int(det)
+        for k in ("x", "y", "width", "height", "angle"):
+            setattr(ev, k, float(record[k]))
+        ev.confidence = float(record.get("confidence", 1.0))
+    vv = video_view(view)
+    crop = FaceCrop(None, int(crop_w), int(crop_h), 0, 0, float(scale))
+    out = (C.c_int64 * 6)()
+    rc = lib().ht_face_crop_map(C.addressof(ev), int(canvas_w), int(canvas_h), int(width), int(height), C.addressof(vv),
+                                C.addressof(crop), out)
+    if rc < 0:
+        raise ValueError(f"ht_face_crop_map rejected its arguments ({rc})")
+    return tuple(out) if rc == 1 else None
+
+
+def crop_to_video(view, width, height, canvas_w, canvas_h, record, crop_w, crop_h, scale=1.0):
+    """the 2x3 affine ((a, b, c), (d, e, f)) from continuous crop pixel coordinates (p, q) to the video's:
+    x = a p + b q + c, y = d p + e q + f, exactly the map the device samples with (crop_map); e.g. to put landmarks
+    found in the crop back onto the video.  -> None when the record makes no crop."""
+    m = crop_map(view, width, height, canvas_w, canvas_h, record, crop_w, crop_h, scale)
+    if m is None:
+        return None
+    U0, V0, Ui, Vi, Uj, Vj = m
+    # crop pixel centre p = i + 1/2 samples tap u = (U0 + i Ui + j Uj) / 65536, the video coordinate u + 1/2
+    return ((Ui / 65536, Uj / 65536, (U0 - (Ui + Uj) / 2) / 65536 + 0.5),
+            (Vi / 65536, Vj / 65536, (V0 - (Vi + Vj) / 2) / 65536 + 0.5))

@@ -474,6 +474,43 @@ int ht_tracker_set_debug(ht_ctx *ctx, int first, int n, const ht_debug_canvas *c
  * n <= 0, enable NULL, or a value other than 0 and 1. */
 int ht_tracker_set_debug_strokes(ht_ctx *ctx, int first, int n, const int32_t *enable);
 
+/* A stream's face crop: the tracked face cut out of its video, upright and at video resolution (DESIGN.md 2, "Face
+ * crops").  Byte offsets: 0 rgba, 8 width, 12 height, 16 pitch, 20 pad_, 24 scale. */
+typedef struct {
+  uint8_t *rgba;          /* DEVICE memory, `height` rows of `pitch` bytes of RGBA8; NULL: the stream has no crop */
+  int32_t width, height;  /* S_w x S_h, 1..2048 */
+  int32_t pitch;          /* 0 -> 4*width; a multiple of 4, >= 4*width */
+  int32_t pad_;
+  double scale;           /* the face box is scaled by this about its centre; finite, in (0, 16] */
+} ht_face_crop;           /* 32 bytes */
+/* Stream first+i gets crops[i] (host array), for i in [0, n); stream states are kept.  After every tick whose record
+ * is "CS" with width > 0 and height > 0 - track() kept the face - every pixel of the crop is written: the rectangle
+ * main.js strokes in green (translate(x, y) . rotate(angle - pi/2), local box [ToInt32(-w/2), +w] x [ToInt32(-h/2),
+ * +h]), scaled about its centre by `scale`, its shorter side grown until the aspect ratio is width : height, sampled
+ * bilinearly from the tick's video (the frame ht_tracker_step was given, or the video of the feed record, through its
+ * view) with 8-bit weights.  Taps outside the video or the view's source rectangle read (0, 0, 0, 0), so alpha shows
+ * where the crop leaves the video.  Every other tick (IDLE, STARTING, WB, VJ - also the VJ tick that finds the face -
+ * and the CS tick that loses it) leaves the crop as it was.  ht_face_crop_map gives the exact map.  The writes are
+ * enqueued on the context's stream after the tick's records are computed: with host `out` they have landed when the
+ * tick returns, with device `out` after ht_sync or in stream order.  The crop belongs to the stream id: stop, start,
+ * reset, a lost face, ht_tracker_set_params and ht_tracker_import keep it; ht_tracker_config removes every stream's.
+ * A tick launches one more kernel while some stream has a crop, and nothing more otherwise.
+ * Errors (nothing changes): HT_ERR_STATE before ht_tracker_config; HT_ERR_ARG for a range outside [0, max_frames),
+ * n <= 0, crops NULL, a host pointer, a pointer or pitch that is not a multiple of 4, a pitch below 4*width, a scale
+ * that is not finite or outside (0, 16], or a crop whose bytes overlap another stream's crop or any debug canvas (over
+ * all streams after the call: the streams of a tick run concurrently); HT_ERR_SIZE for a size outside 1..2048. */
+int ht_tracker_set_face_crop(ht_ctx *ctx, int first, int n, const ht_face_crop *crops);
+
+/* The map of the crop `crop` (its size and scale; rgba and pitch are ignored) for tracker record `ev`, on a canvas of
+ * canvas_w x canvas_h drawn from a video_w x video_h video through `view` (NULL: the whole frame upright; for
+ * ht_tracker_step the video is the canvas): crop pixel (i, j) samples video tap coordinates (U0 + i Ui + j Uj,
+ * V0 + i Vi + j Vj) / 65536, with out = {U0, V0, Ui, Vi, Uj, Vj} exactly as the device computes them.  A tap coordinate
+ * u is video pixel centre u + 1/2.  Host only; needs no context.  -> 1 if the record makes a crop, 0 if not (out all
+ * 0), HT_ERR_ARG for NULL pointers, a scale outside (0, 16] or a bad view, HT_ERR_SIZE for a canvas or video outside
+ * 1..16384 or a crop outside 1..2048. */
+int ht_face_crop_map(const ht_tracker_event *ev, int canvas_w, int canvas_h, int video_w, int video_h,
+                     const ht_video_view *view, const ht_face_crop *crop, int64_t out[6]);
+
 /* A stream's head-coupled camera: the three.js r48 PerspectiveCamera that realisticAbsoluteCameraControl moves
  * (src/controllers.js:28-68), in caller-owned DEVICE memory that a renderer can bind directly.  Byte offsets:
  *     0  double position[3]      camera.position

@@ -25,6 +25,8 @@
 //   trackerSetParams(handle, first, [params, ...])   (ht_tracker_set_params: each stream its own Tracker parameters)
 //   trackerSetDebug(handle, first, [canvas|null, ...])  (ht_tracker_set_debug: each stream's debug canvas, device memory)
 //   trackerSetDebugStrokes(handle, first, [bool, ...])  (ht_tracker_set_debug_strokes: main.js's strokes on the device)
+//   trackerSetFaceCrop(handle, first, [crop|null, ...])  (ht_tracker_set_face_crop: each stream's face crop, device
+//        memory)
 //   trackerSetCamera(handle, first, [control|null, ...])  (ht_tracker_set_camera: each stream's head-coupled camera,
 //        realisticAbsoluteCameraControl on an ht_camera in device memory)
 //   trackerExport(handle, [stream, ...]) -> Buffer of records; trackerImport(handle, [stream, ...], records)
@@ -476,6 +478,40 @@ static napi_value TrackerSetDebugStrokes(napi_env env, napi_callback_info info) 
   return nullptr;
 }
 
+// trackerSetFaceCrop(handle, first, [{rgba: BigInt device address, width, height, pitch, scale}, null, ...]): stream
+// first+i gets crops[i] (scale defaults to 1); null or undefined: none
+static napi_value TrackerSetFaceCrop(napi_env env, napi_callback_info info) {
+  size_t argc = 3;
+  napi_value argv[3];
+  NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+  ht_ctx *ctx = Ctx(env, argv[0]);
+  int32_t first = 0;
+  uint32_t n = 0;
+  napi_get_value_int32(env, argv[1], &first);
+  NAPI_OK(napi_get_array_length(env, argv[2], &n));
+  std::vector<ht_face_crop> cs(n, ht_face_crop{nullptr, 0, 0, 0, 0, 1.0});
+  for (uint32_t i = 0; i < n; ++i) {
+    napi_value r, v;
+    napi_valuetype t = napi_undefined;
+    NAPI_OK(napi_get_element(env, argv[2], i, &r));
+    napi_typeof(env, r, &t);
+    if (t != napi_object) continue;
+    uint64_t addr = 0;
+    bool lossless = false;
+    if (napi_get_named_property(env, r, "rgba", &v) == napi_ok) napi_get_value_bigint_uint64(env, v, &addr, &lossless);
+    cs[i].rgba = reinterpret_cast<uint8_t *>(static_cast<uintptr_t>(addr));
+    if (napi_get_named_property(env, r, "width", &v) == napi_ok) napi_get_value_int32(env, v, &cs[i].width);
+    if (napi_get_named_property(env, r, "height", &v) == napi_ok) napi_get_value_int32(env, v, &cs[i].height);
+    if (napi_get_named_property(env, r, "pitch", &v) == napi_ok) napi_get_value_int32(env, v, &cs[i].pitch);
+    napi_valuetype st = napi_undefined;
+    if (napi_get_named_property(env, r, "scale", &v) == napi_ok && napi_typeof(env, v, &st) == napi_ok && st == napi_number)
+      napi_get_value_double(env, v, &cs[i].scale);
+  }
+  int rc = ht_tracker_set_face_crop(ctx, first, (int)n, cs.data());
+  if (rc < 0) return Throw(env, ctx, rc);
+  return nullptr;
+}
+
 static double GetNumber(napi_env env, napi_value obj, const char *name, double dflt) {
   napi_value v;
   napi_valuetype t = napi_undefined;
@@ -888,6 +924,7 @@ static napi_value Init(napi_env env, napi_value exports) {
       {"trackerSetParams", nullptr, TrackerSetParams, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerSetDebug", nullptr, TrackerSetDebug, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerSetDebugStrokes", nullptr, TrackerSetDebugStrokes, nullptr, nullptr, nullptr, napi_default, nullptr},
+      {"trackerSetFaceCrop", nullptr, TrackerSetFaceCrop, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerSetCamera", nullptr, TrackerSetCamera, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerExport", nullptr, TrackerExport, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerImport", nullptr, TrackerImport, nullptr, nullptr, nullptr, napi_default, nullptr},

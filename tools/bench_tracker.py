@@ -29,6 +29,10 @@ streams: N 640x480 streams, device-resident frames and outputs, CUDA events arou
                   (--views) ht_tracker_feed(_yuv)_views from RGBA and NV12 video through rotations, mirrors and crops
                   against the plain feed of the upright video and against a separate rotate / crop pass + plain feed
                   (also --before-lib), and k_feed_draw_view's time (views_arms)
+  crop*_* twopass*_*
+                  (--crops) ht_tracker_feed_yuv from 1280x720 NV12 onto 320x240 canvases with 112x112 and 224x224 face
+                  crops on none, 1/64 and all of the streams, against ht_ingest_yuv + grid_sample of the boxes (also
+                  --before-lib), and k_face_crop's time (crops_arms)
 
 Prints one JSON line with the card's name and power limit read in the same run; --out also writes it to a file."""
 import argparse
@@ -636,6 +640,166 @@ def camera_arms(torch, frames, stream, N, W, H, steps, rounds, before_lib=None):
 YUV_LAYOUTS = [((1280, 720), (320, 240)), ((1280, 720), (640, 480)), ((640, 480), (640, 480))]
 
 
+def nv12_streams(torch, N, W, H):
+    """N NV12 device videos of W x H (BT.601 limited range) -> (Y planes (N, H, W), UV planes (N, H/2, W)).  Each
+    stream its own video: one of 8 synth frames, shifted right by its own offset, so that every tick reads N distinct
+    frames from HBM as N cameras would."""
+    from headtrackr_b200 import synth
+    base = torch.stack([torch.from_numpy(synth.frame(i, W, H, n_faces=1)) for i in range(8)]).cuda()
+    ys = torch.empty((N, H, W), dtype=torch.uint8, device="cuda")
+    uvs = torch.empty((N, H // 2, W), dtype=torch.uint8, device="cuda")
+    for k0 in range(0, N, 64):
+        k1 = min(N, k0 + 64)
+        f = torch.stack([torch.roll(base[k % 8], shifts=2 * (k // 8) % 64, dims=1) for k in range(k0, k1)]).float()
+        r, g, b = f[..., 0], f[..., 1], f[..., 2]
+        y = 16 + (65.481 * r + 128.553 * g + 24.966 * b) / 255
+        u = 128 + (-37.797 * r - 74.203 * g + 112.0 * b) / 255
+        v = 128 + (112.0 * r - 93.786 * g - 18.214 * b) / 255
+        uv = torch.stack([u[:, 0::2, 0::2], v[:, 0::2, 0::2]], dim=-1).reshape(k1 - k0, H // 2, W)
+        ys[k0:k1] = torch.floor(y + 0.5).clamp(0, 255).to(torch.uint8)
+        uvs[k0:k1] = torch.floor(uv + 0.5).clamp(0, 255).to(torch.uint8)
+    return ys, uvs
+
+
+def crop_theta(torch, ev, W, H, CW, CH, Sw, Sh, scale):
+    """affine_grid thetas (N, 2, 3) of the face crops of device records `ev` (N x 144 bytes) in fp32: the geometry of
+    DESIGN.md 2, "Face crops" as a caller writes it with torch (records without a crop give some finite theta)"""
+    import math
+    f = ev.view(torch.float64).reshape(ev.numel() // 144, 18)
+    x, y, w, h, angle = (f[:, i].float() for i in (1, 2, 3, 4, 5))
+    t = torch.nan_to_num(angle - math.pi / 2, nan=0.0)
+    s, c = torch.sin(t), torch.cos(t)
+    cx, cy = torch.trunc(-w / 2) + w / 2, torch.trunc(-h / 2) + h / 2
+    hw, hh = w * scale / 2, h * scale / 2
+    hw, hh = torch.maximum(hw, hh * Sw / Sh), torch.maximum(hh, hw * Sh / Sw)
+    kx, ky = W / CW, H / CH
+    # video coordinates of crop point (p, q): x = a p + b q + e, y = d p + g q + k (pixel centres at +0.5)
+    a, b, d, g = c * 2 * hw / Sw * kx, -s * 2 * hh / Sh * kx, s * 2 * hw / Sw * ky, c * 2 * hh / Sh * ky
+    lx, ly = cx - hw, cy - hh
+    e, k = (x + c * lx - s * ly) * kx, (y + s * lx + c * ly) * ky
+    # normalised output (u, v) in [-1, 1] is crop point ((u + 1) Sw / 2, (v + 1) Sh / 2); input x -> 2 x / W - 1
+    row0 = torch.stack([a * Sw / W, b * Sh / W, (a * Sw / 2 + b * Sh / 2 + e) * 2 / W - 1], 1)
+    row1 = torch.stack([d * Sw / H, g * Sh / H, (d * Sw / 2 + g * Sh / 2 + k) * 2 / H - 1], 1)
+    return torch.stack([row0, row1], 1)
+
+
+def crops_arms(torch, stream, N, steps, rounds, before_lib=None):
+    """Face crops (ht_tracker_set_face_crop) in steady tracking: N streams of 1280x720 NV12 device video fed onto
+    320x240 canvases by ht_tracker_feed_yuv, every arm on its own context, all arms alternating tick by tick (the arm
+    order rotates), CUDA events around each tick:
+
+      crop0_cs              no crops (the tick launches what it launched before crops)
+      crop0_before_cs       crop0_cs with the library at `before_lib` (e.g. the parent commit's build)
+      crop<S>all_cs         an S x S crop (S = 112, 224) on every stream, scale 1
+      crop<S>64_cs          an S x S crop on every 64th stream
+      twopass<S>_cs         what a caller does without crops: the crops-off tick, ht_ingest_yuv of every video to
+                            RGBA8 at video size, then torch's grid_sample (fp16, bilinear) of every stream's box
+
+    Then, in runs of their own under torch.profiler, k_face_crop's kernel time per tick in the crop<S>all arms.  The
+    records of every arm must agree on every timed tick."""
+    import ctypes as C
+    import torch.nn.functional as F
+    from headtrackr_b200 import Context, _lib
+    from headtrackr_b200.context import _yuv_image
+    W, H, CW, CH = 1280, 720, 320, 240
+    rec_bytes = C.sizeof(_lib.TrackerEvent)
+    now = [1.0e12]
+    kw = dict(max_width=CW, max_height=CH, max_frames=N, stream=stream)
+    ys, uvs = nv12_streams(torch, N, W, H)
+    keep = []
+    imgs = [_yuv_image((ys[k], uvs[k]), "nv12", "bt601", keep)[0] for k in range(N)]
+    yrecs = (_lib.YuvFrame * N)()
+    for k in range(N):
+        yrecs[k] = _lib.YuvFrame(imgs[k], k, CW, CH, 0, 0.0)
+    ingest_src = (_lib.YuvImage * N)(*imgs)
+    rgba = torch.empty((N, H, W, 4), dtype=torch.uint8, device="cuda")
+    crops = {S: torch.zeros((N, S, S, 4), dtype=torch.uint8, device="cuda") for S in (112, 224)}
+    twopass_out = {}
+
+    def arm(kind, S=0, every=0):
+        c = other_build_context(before_lib, **kw) if kind == "before" else Context(**kw)
+        c.tracker_config()
+        c.tracker_reset(0, N)
+        c.tracker_start(0, N)
+        if every:
+            c.tracker_set_face_crop(0, [{"out": crops[S][k]} if k % every == 0 else None for k in range(N)])
+        out = torch.empty(N * rec_bytes, dtype=torch.uint8, device="cuda")
+
+        def run():
+            for k in range(N):
+                yrecs[k].now_ms = now[0]
+            c._check(c._L.ht_tracker_feed_yuv(c._h, C.addressof(yrecs), N, 1, out.data_ptr()))
+            if kind == "twopass":
+                c._check(c._L.ht_ingest_yuv(c._h, C.addressof(ingest_src), N, 1, rgba.data_ptr(), W, H))
+                theta = crop_theta(torch, out, W, H, CW, CH, S, S, 1.0)
+                src = rgba.permute(0, 3, 1, 2).half()
+                grid = F.affine_grid(theta.half(), (N, 4, S, S), align_corners=False)
+                twopass_out[S] = F.grid_sample(src, grid, mode="bilinear", padding_mode="zeros", align_corners=False)
+        return c, run, out
+
+    arms = {"crop0_cs": arm("plain"), "crop112all_cs": arm("crop", 112, 1), "crop11264_cs": arm("crop", 112, 64),
+            "crop224all_cs": arm("crop", 224, 1), "crop22464_cs": arm("crop", 224, 64),
+            "twopass112_cs": arm("twopass", 112), "twopass224_cs": arm("twopass", 224)}
+    if before_lib:
+        arms["crop0_before_cs"] = arm("before")
+    names = list(arms)
+
+    def tick(name):
+        _, run, _ = arms[name]
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        a.record()
+        run()
+        b.record()
+        b.synchronize()
+        return a.elapsed_time(b)
+
+    for _ in range(17):                          # the whitebalance gate, detection, the first CS frames
+        now[0] += 20.0
+        for name in names:
+            tick(name)
+    times = {name: [[] for _ in range(rounds)] for name in names}
+    for r in range(rounds):
+        for s in range(steps):
+            now[0] += 20.0
+            rot = (r * steps + s) % len(names)
+            for name in names[rot:] + names[:rot]:
+                times[name][r].append(tick(name))
+            first = arms[names[0]][2]
+            if any(not torch.equal(first, arms[name][2]) for name in names[1:]):
+                raise SystemExit("crop arms disagree on the records of a timed tick")
+    res = {}
+    for name in names:
+        med = [float(np.median(t)) for t in times[name]]
+        res[f"{name}_ms"] = float(np.median(sum(times[name], [])))
+        res[f"{name}_spread_ms"] = max(med) - min(med)
+    ev = [_lib.TrackerEvent.from_buffer_copy(bytes(row)) for row in arms["crop0_cs"][2].cpu().numpy().reshape(N, rec_bytes)]
+    cs = [e.detection == 2 and e.width > 0 and e.height > 0 for e in ev]
+    res["crops_cs_streams"] = sum(cs)
+    res["crops_records_agree"] = True
+    for S in (112, 224):                         # the two paths cut the same faces (different resamplers)
+        fused = crops[S].permute(0, 3, 1, 2).float()[torch.tensor(cs, device="cuda")]
+        two = twopass_out[S].float()[torch.tensor(cs, device="cuda")]
+        res[f"twopass{S}_vs_fused_mean_abs_diff"] = float((fused - two).abs().mean())
+
+    from torch.profiler import ProfilerActivity, profile
+    for S in (112, 224):
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(steps):
+                now[0] += 20.0
+                arms[f"crop{S}all_cs"][1]()
+            torch.cuda.synchronize()
+        us = 0.0
+        for e in prof.key_averages():
+            if "k_face_crop" in e.key:
+                t = getattr(e, "device_time_total", None)
+                us += t if t is not None else e.cuda_time_total
+        res[f"k_face_crop_{S}_ms"] = us / 1000.0 / steps
+        res[f"k_face_crop_{S}_write_GBps"] = N * S * S * 4 / (us * 1e-6 / steps) / 1e9 if us > 0 else None
+    for c, _, _ in arms.values():
+        c.close()
+    return res
+
+
 def yuv_arms(torch, stream, N, steps, rounds, before_lib=None):
     """YUV video (ht_tracker_feed_yuv) in steady tracking, for each (video, canvas) of YUV_LAYOUTS: N streams, each
     with its own NV12 device video (BT.601 limited range), every arm on its own context, all arms of a layout
@@ -659,22 +823,7 @@ def yuv_arms(torch, stream, N, steps, rounds, before_lib=None):
         lay = f"{W}x{H}_{CW}x{CH}"
         now = [1.0e12]
         kw = dict(max_width=CW, max_height=CH, max_frames=N, stream=stream)
-        # each stream its own video: one of 8 synth frames, shifted right by its own offset, so that every tick reads
-        # N distinct frames from HBM as N cameras would
-        base = torch.stack([torch.from_numpy(synth.frame(i, W, H, n_faces=1)) for i in range(8)]).cuda()
-        ys = torch.empty((N, H, W), dtype=torch.uint8, device="cuda")
-        uvs = torch.empty((N, H // 2, W), dtype=torch.uint8, device="cuda")
-        for k0 in range(0, N, 64):
-            k1 = min(N, k0 + 64)
-            f = torch.stack([torch.roll(base[k % 8], shifts=2 * (k // 8) % 64, dims=1) for k in range(k0, k1)]).float()
-            r, g, b = f[..., 0], f[..., 1], f[..., 2]
-            y = 16 + (65.481 * r + 128.553 * g + 24.966 * b) / 255
-            u = 128 + (-37.797 * r - 74.203 * g + 112.0 * b) / 255
-            v = 128 + (112.0 * r - 93.786 * g - 18.214 * b) / 255
-            uv = torch.stack([u[:, 0::2, 0::2], v[:, 0::2, 0::2]], dim=-1).reshape(k1 - k0, H // 2, W)
-            ys[k0:k1] = torch.floor(y + 0.5).clamp(0, 255).to(torch.uint8)
-            uvs[k0:k1] = torch.floor(uv + 0.5).clamp(0, 255).to(torch.uint8)
-        del base, f, r, g, b, y, u, v, uv
+        ys, uvs = nv12_streams(torch, N, W, H)
         planes = [(ys[k], uvs[k]) for k in range(N)]
         keep = []
         imgs = [_yuv_image(p, "nv12", "bt601", keep)[0] for p in planes]
@@ -1204,6 +1353,7 @@ def main():
     ap.add_argument("--yuv", action="store_true", help="only the YUV video arms (yuv_arms)")
     ap.add_argument("--formats", action="store_true", help="only the video-format arms (formats_arms)")
     ap.add_argument("--views", action="store_true", help="only the video-view arms (views_arms)")
+    ap.add_argument("--crops", action="store_true", help="only the face-crop arms (crops_arms)")
     ap.add_argument("--out")
     a = ap.parse_args()
     import torch
@@ -1222,6 +1372,9 @@ def main():
         return report(res, a.out)
     if a.views:
         res.update(views_arms(torch, stream, N, a.steps, a.rounds, a.before_lib))
+        return report(res, a.out)
+    if a.crops:
+        res.update(crops_arms(torch, stream, N, a.steps, a.rounds, a.before_lib))
         return report(res, a.out)
     if a.formats:
         res.update(formats_arms(torch, stream, N, a.steps, a.rounds, a.before_lib))
