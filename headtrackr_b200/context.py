@@ -8,7 +8,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from ._lib import (Camera, CameraControl, CanvasFrame, DebugCanvas, FaceCrop, HeadEvent, HeadParams, HtError, Rect, StreamEvent, TrackerEvent, TrackerParams, TrackObj, VideoFrame,
+from ._lib import (Camera, CameraControl, CanvasFrame, DebugCanvas, FaceCrop, FaceCropYuv, HeadEvent, HeadParams, HtError, Rect, StreamEvent, TrackerEvent, TrackerParams, TrackObj, VideoFrame,
                    VideoView, Window, YuvFrame, YuvImage)
 from .views import video_view
 from .synth import load_cascade_blob
@@ -107,6 +107,54 @@ def _yuv_image(planes, fmt, color, keep):
     return img, where.pop()
 
 
+def _face_crop_record(c):
+    """a face crop dict of Context.tracker_set_face_crop -> its FaceCrop or FaceCropYuv (None: no crop)"""
+    if c is None:
+        return None
+    fmt, out = c.get("format", "rgba"), c["out"]
+    if fmt == "rgba":
+        if not _is_torch(out) or not out.is_cuda:
+            raise ValueError("a face crop is a torch CUDA tensor")
+        if out.dim() != 3 or out.element_size() != 1 or out.shape[2] != 4 or out.stride(2) != 1 or out.stride(1) != 4:
+            raise ValueError("face crops must be uint8 (S_h, S_w, 4) with strides (pitch, 4, 1)")
+        return FaceCrop(out.data_ptr(), out.shape[1], out.shape[0], out.stride(0), 0, float(c.get("scale", 1.0)))
+    if fmt not in ("nv12", "i420"):
+        raise ValueError("a face crop's format is 'rgba', 'nv12' or 'i420'")
+    color = c.get("color", "bt601")
+    if color not in _lib.YUV_COLORS:
+        raise ValueError(f"color must be one of {sorted(_lib.YUV_COLORS)}")
+    planes = tuple(out) if isinstance(out, (tuple, list)) else (out,)
+    if len(planes) != (2 if fmt == "nv12" else 3):
+        raise ValueError("an NV12 face crop is (Y, UV), an I420 face crop (Y, U, V)")
+    for p in planes:
+        if not _is_torch(p) or not p.is_cuda or p.dim() != 2 or p.element_size() != 1 or p.is_floating_point() \
+                or p.stride(1) != 1:
+            raise ValueError("YUV face crop planes are 2-D uint8 torch CUDA tensors with unit column stride")
+    h, w = planes[0].shape
+    need = (h // 2, w if fmt == "nv12" else w // 2)
+    for i, p in enumerate(planes[1:], 1):
+        if p.shape[0] < need[0] or p.shape[1] < need[1]:
+            raise ValueError(f"plane {i} is {tuple(p.shape)}, a {w}x{h} {fmt} face crop needs {need}")
+    ptrs = [p.data_ptr() for p in planes] + [None] * (3 - len(planes))
+    pitches = [p.stride(0) for p in planes] + [0] * (3 - len(planes))
+    return FaceCropYuv((C.c_void_p * 3)(*ptrs), (C.c_int32 * 3)(*pitches), w, h, _lib.YUV_FORMATS[fmt],
+                       _lib.YUV_COLORS[color], 0, float(c.get("scale", 1.0)))
+
+
+def _crop_runs(recs):
+    """[a, b) ranges of records of one layout, each as long as possible (None joins any run)"""
+    runs, kind = [], None
+    for i, r in enumerate(recs):
+        k = None if r is None else isinstance(r, FaceCropYuv)
+        if runs and (k is None or kind is None or k == kind):
+            runs[-1][1] = i + 1
+            kind = k if kind is None else kind
+        else:
+            runs.append([i, i + 1])
+            kind = k
+    return [tuple(r) for r in runs]
+
+
 def _per_record(v, n, what):
     vs = list(v) if isinstance(v, (list, tuple)) else [v] * n
     if len(vs) != n:
@@ -176,7 +224,7 @@ class Context:
         self.last_warning = None
         self._debug = {}                  # stream -> its debug canvas tensor, kept alive while the library writes it
         self._camera = {}                 # stream -> its camera tensor, likewise
-        self._crops = {}                  # stream -> its face crop tensor, likewise
+        self._crops = {}                  # stream -> its face crop dict (and so its tensors), likewise
 
     def close(self):
         if getattr(self, "_h", None) and self._h.value:
@@ -400,30 +448,46 @@ class Context:
         self._check(self._L.ht_tracker_set_debug_strokes(self._h, int(first), len(flags), arr))
 
     def tracker_set_face_crop(self, first, crops):
-        """Face crops of streams first, first+1, ... (ht_tracker_set_face_crop): per stream None (none) or a dict
-        {"out": torch CUDA uint8 (S_h, S_w, 4) tensor, "scale": 1.0}; a row-padded view - last two strides (4, 1) -
-        passes its row stride as the pitch.  After every tick on which track() kept the face ("CS", width and height
-        > 0), `out` holds the green rectangle main.js strokes, scaled by `scale` about its centre and grown to the
-        crop's aspect ratio, cut upright out of the tick's video at video resolution (DESIGN.md 2, "Face crops").  The
-        crop is the stream's: it outlives set_params, stop, start, reset and import; tracker_config removes it.  The
-        context keeps the tensors alive while they are set."""
-        crops = list(crops)
-        arr = (FaceCrop * max(1, len(crops)))()
+        """Face crops of streams first, first+1, ... (ht_tracker_set_face_crop / ht_tracker_set_face_crop_yuv): per
+        stream None (none) or a dict {"out": ..., "scale": 1.0, "format": "rgba", "color": "bt601"}.  With format
+        "rgba" (the default) `out` is a torch CUDA uint8 (S_h, S_w, 4) tensor; a row-padded view - last two strides
+        (4, 1) - passes its row stride as the pitch.  With "nv12" or "i420" - what video encoders take - `out` is a
+        tuple of 2-D uint8 CUDA planes as tracker_feed_yuv takes them, (Y, UV) or (Y, U, V), with unit column stride
+        (row strides become pitches); the Y plane is S_h x S_w, both even, and `color` is one of _lib.YUV_COLORS
+        (BT.2020 is rejected).  After every tick on which track() kept the face ("CS", width and height > 0), `out`
+        holds the green rectangle main.js strokes, scaled by `scale` about its centre and grown to the crop's aspect
+        ratio, cut upright out of the tick's video at video resolution; a YUV crop is the RGBA crop of its size and
+        scale converted, alpha ignored (DESIGN.md 2, "Face crops").  A stream has one crop, in one layout: setting
+        either replaces it.  The crop is the stream's: it outlives set_params, stop, start, reset and import;
+        tracker_config removes it.  The context keeps the tensors alive while they are set.  A list mixing RGBA and
+        YUV crops is set one run of equal layout at a time; if the library rejects a run, the runs before it are set
+        back, so a rejected call changes nothing."""
+        first, crops = int(first), list(crops)
+        recs = [_face_crop_record(c) for c in crops]
+        prev = [self._crops.get(first + i) for i in range(len(crops))]
+        done = 0
+        try:
+            for a, b in _crop_runs(recs) or [(0, 0)]:   # no crops at all: the library's rejection of n = 0
+                self._set_crop_run(first + a, recs[a:b])
+                done = b
+        except HtError:
+            back = [_face_crop_record(c) for c in prev[:done]]
+            for a, b in _crop_runs(back):             # the state before the call, which the library accepted
+                self._set_crop_run(first + a, back[a:b])
+            raise
         for i, c in enumerate(crops):
             if c is None:
-                continue
-            t = c["out"]
-            if not _is_torch(t) or not t.is_cuda:
-                raise ValueError("a face crop is a torch CUDA tensor")
-            if t.dim() != 3 or t.element_size() != 1 or t.shape[2] != 4 or t.stride(2) != 1 or t.stride(1) != 4:
-                raise ValueError("face crops must be uint8 (S_h, S_w, 4) with strides (pitch, 4, 1)")
-            arr[i] = FaceCrop(t.data_ptr(), t.shape[1], t.shape[0], t.stride(0), 0, float(c.get("scale", 1.0)))
-        self._check(self._L.ht_tracker_set_face_crop(self._h, int(first), len(crops), C.addressof(arr)))
-        for i, c in enumerate(crops):
-            if c is None:
-                self._crops.pop(int(first) + i, None)
+                self._crops.pop(first + i, None)
             else:
-                self._crops[int(first) + i] = c["out"]
+                self._crops[first + i] = c
+
+    def _set_crop_run(self, first, recs):
+        """one setter call over records of one layout (None: no crop) from _face_crop_record"""
+        yuv = any(isinstance(r, FaceCropYuv) for r in recs)
+        T = FaceCropYuv if yuv else FaceCrop
+        arr = (T * len(recs))(*[r if r is not None else T() for r in recs])
+        setter = self._L.ht_tracker_set_face_crop_yuv if yuv else self._L.ht_tracker_set_face_crop
+        self._check(setter(self._h, first, len(recs), C.addressof(arr)))
 
     def tracker_set_camera(self, first, controls):
         """Head-coupled camera controllers of streams first, first+1, ...: per stream None (none) or a dict of

@@ -582,10 +582,11 @@ struct ht_ctx {
   DevBuf d_camera;
   std::vector<CameraCtl> h_camera;
   int camera_count = 0;
-  // ht_tracker_set_face_crop: per stream its FaceCrop (device array and host copy), the number of streams that have
-  // one (0: a tick launches no k_face_crop) and the tiles of the largest (k_face_crop's grid.x)
-  DevBuf d_crop;
+  // ht_tracker_set_face_crop(_yuv): per stream its FaceCrop and CropPlanes (device arrays and host copies), the number
+  // of streams that have one (0: a tick launches no k_face_crop) and the tiles of the largest (k_face_crop's grid.x)
+  DevBuf d_crop, d_crop_planes;
   std::vector<FaceCrop> h_crop;
+  std::vector<CropPlanes> h_crop_planes;
   int crop_count = 0, crop_tiles = 0;
   // ht_tracker_feed(_canvases): the record table {ids[n], clocks[n], FeedRec[n], EntryCanvas[n], tile starts[n+1]}
   // goes up in one copy from pinned memory; the videos are drawn into the canvas arena (batch entry k's canvas at
@@ -1766,6 +1767,7 @@ int ht_tracker_config(ht_ctx *ctx, const ht_tracker_params *params) {
   if (ctx->crop_count > 0) {     // and every face crop
     CK(cudaMemsetAsync(ctx->d_crop.p, 0, mf * sizeof(FaceCrop), ctx->stream));
     ctx->h_crop.assign(mf, FaceCrop{});
+    ctx->h_crop_planes.assign(mf, CropPlanes{});
     ctx->crop_count = ctx->crop_tiles = 0;
   }
   if (!params) {                 // off: every stream as after ht_stream_reset (the lifecycle has used the tracker slots)
@@ -1846,22 +1848,41 @@ static int debug_commit(ht_ctx *ctx, int first, int n, std::vector<DebugCanvas> 
   return HT_OK;
 }
 
-// Whether two of the images written during a tick - every debug canvas and every face crop - share a byte: the streams
-// of a tick run concurrently.
-static bool images_overlap(const std::vector<DebugCanvas> &dbg, const std::vector<FaceCrop> &crops) {
-  std::vector<std::pair<uintptr_t, uintptr_t>> spans;
-  auto add = [&](const uint8_t *p, int w, int h, int pitch) {
+// Whether two of the images written during a tick - every debug canvas and every plane of every face crop - share a
+// byte: the streams of a tick run concurrently.  -> -1 if none do; otherwise a stream whose crop takes part, one in
+// [first, first + n) if there is one (so that a setter can name the record), or -2 if only debug canvases do.
+static int images_overlap(const std::vector<DebugCanvas> &dbg, const std::vector<FaceCrop> &crops,
+                          const std::vector<CropPlanes> &planes, int first = 0, int n = 0) {
+  struct Span { uintptr_t start, end; int crop; };        // crop: its stream, -2 for a debug canvas
+  std::vector<Span> spans;
+  auto add = [&](const uint8_t *p, int bytes, int rows, int pitch, int crop) {
     const uintptr_t s = reinterpret_cast<uintptr_t>(p);
-    spans.emplace_back(s, s + (size_t)(h - 1) * pitch + 4 * (size_t)w);
+    spans.push_back(Span{s, s + (size_t)(rows - 1) * pitch + (size_t)bytes, crop});
   };
   for (const DebugCanvas &d : dbg)
-    if (d.rgba) add(d.rgba, d.w, d.h, d.pitch);
-  for (const FaceCrop &f : crops)
-    if (f.rgba) add(f.rgba, f.w, f.h, f.pitch);
-  std::sort(spans.begin(), spans.end());
+    if (d.rgba) add(d.rgba, 4 * d.w, d.h, d.pitch, -2);
+  for (size_t k = 0; k < crops.size(); ++k) {
+    const FaceCrop &f = crops[k];
+    if (!f.rgba) continue;
+    if (f.layout == CROP_RGBA) { add(f.rgba, 4 * f.w, f.h, f.pitch, (int)k); continue; }
+    const CropPlanes &c = planes[k];
+    add(f.rgba, f.w, f.h, f.pitch, (int)k);
+    if (f.layout == CROP_NV12) {
+      add(c.u, f.w, f.h / 2, c.upitch, (int)k);
+    } else {
+      add(c.u, f.w / 2, f.h / 2, c.upitch, (int)k);
+      add(c.v, f.w / 2, f.h / 2, c.vpitch, (int)k);
+    }
+  }
+  std::sort(spans.begin(), spans.end(), [](const Span &a, const Span &b) { return a.start < b.start; });
+  int found = -1;
   for (size_t i = 1; i < spans.size(); ++i)
-    if (spans[i].first < spans[i - 1].second) return true;
-  return false;
+    if (spans[i].start < spans[i - 1].end)
+      for (const Span *s : {&spans[i - 1], &spans[i]}) {
+        if (s->crop >= first && s->crop < first + n) return s->crop;
+        if (found < 0 || s->crop >= 0) found = std::max(found, s->crop);
+      }
+  return found;
 }
 
 // The debug canvases of streams [first, first + n).  Everything is checked on the host before anything changes,
@@ -1900,7 +1921,7 @@ int ht_tracker_set_debug(ht_ctx *ctx, int first, int n, const ht_debug_canvas *c
   for (size_t i = 1; i < spans.size(); ++i)
     if (spans[i].first < spans[i - 1].second)
       return ctx->fail(HT_ERR_ARG, "a debug canvas overlaps another stream's debug canvas");
-  if (ctx->crop_count > 0 && images_overlap(next, ctx->h_crop))
+  if (ctx->crop_count > 0 && images_overlap(next, ctx->h_crop, ctx->h_crop_planes) != -1)
     return ctx->fail(HT_ERR_ARG, "a debug canvas overlaps a face crop");
   return debug_commit(ctx, first, n, next);
 }
@@ -1926,6 +1947,8 @@ static_assert(sizeof(ht_face_crop) == 32 && sizeof(FaceCrop) == sizeof(ht_face_c
                   offsetof(ht_face_crop, scale) == offsetof(FaceCrop, scale),
               "ht_face_crop layout");
 
+static int crop_commit(ht_ctx *ctx, int first, int n, std::vector<FaceCrop> &next, std::vector<CropPlanes> &planes);
+
 // The face crops of streams [first, first + n).  Everything is checked on the host before anything changes, overlap
 // over every crop and debug canvas after the call.
 int ht_tracker_set_face_crop(ht_ctx *ctx, int first, int n, const ht_face_crop *crops) {
@@ -1935,7 +1958,9 @@ int ht_tracker_set_face_crop(ht_ctx *ctx, int first, int n, const ht_face_crop *
   if (first < 0 || n <= 0 || first > mf - n) return ctx->fail(HT_ERR_ARG, "stream range outside [0,%d)", mf);
   if (!crops) return ctx->fail(HT_ERR_ARG, "crops is NULL");
   std::vector<FaceCrop> next = ctx->h_crop;
+  std::vector<CropPlanes> planes = ctx->h_crop_planes;
   next.resize((size_t)mf, FaceCrop{});
+  planes.resize((size_t)mf, CropPlanes{});
   for (int i = 0; i < n; ++i) {
     const ht_face_crop &c = crops[i];
     FaceCrop f{};
@@ -1947,21 +1972,32 @@ int ht_tracker_set_face_crop(ht_ctx *ctx, int first, int n, const ht_face_crop *
       if ((c.pitch & 3) || (c.pitch != 0 && c.pitch < 4 * c.width))
         return ctx->fail(HT_ERR_ARG, "record %d: pitch %d is not a multiple of 4 >= 4*width", i, c.pitch);
       if (!(c.scale > 0.0 && c.scale <= 16.0)) return ctx->fail(HT_ERR_ARG, "record %d: scale %g outside (0, 16]", i, c.scale);
-      f = FaceCrop{c.rgba, c.width, c.height, c.pitch ? c.pitch : 4 * c.width, 0, c.scale};
+      f = FaceCrop{c.rgba, c.width, c.height, c.pitch ? c.pitch : 4 * c.width, CROP_RGBA, c.scale};
     }
     next[(size_t)(first + i)] = f;
+    planes[(size_t)(first + i)] = CropPlanes{};
   }
-  if (images_overlap(ctx->h_debug, next))
+  if (images_overlap(ctx->h_debug, next, planes) != -1)
     return ctx->fail(HT_ERR_ARG, "a face crop overlaps another stream's face crop or a debug canvas");
+  return crop_commit(ctx, first, n, next, planes);
+}
+
+// The checked crops of streams [first, first + n), of either layout, into the device tables and the context.
+static int crop_commit(ht_ctx *ctx, int first, int n, std::vector<FaceCrop> &next, std::vector<CropPlanes> &planes) {
+  const int mf = ctx->cfg.max_frames;
   { const int jr = join_aux(ctx); if (jr != HT_OK) return jr; }
   CK(cudaSetDevice(ctx->cfg.device));
   if (!ctx->d_crop.p) {
     CK(ctx->d_crop.reserve((size_t)mf * sizeof(FaceCrop)));
     CK(cudaMemsetAsync(ctx->d_crop.p, 0, (size_t)mf * sizeof(FaceCrop), ctx->stream));
+    CK(ctx->d_crop_planes.reserve((size_t)mf * sizeof(CropPlanes)));
+    CK(cudaMemsetAsync(ctx->d_crop_planes.p, 0, (size_t)mf * sizeof(CropPlanes), ctx->stream));
   }
   CK(cudaMemcpyAsync(ctx->d_crop.as<FaceCrop>() + first, next.data() + first, (size_t)n * sizeof(FaceCrop),
                      cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));    // `next` is a local
+  CK(cudaMemcpyAsync(ctx->d_crop_planes.as<CropPlanes>() + first, planes.data() + first, (size_t)n * sizeof(CropPlanes),
+                     cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));    // `next` and `planes` are the caller's locals
   ctx->crop_count = ctx->crop_tiles = 0;
   for (const FaceCrop &f : next)
     if (f.rgba) {
@@ -1969,7 +2005,73 @@ int ht_tracker_set_face_crop(ht_ctx *ctx, int first, int n, const ht_face_crop *
       ctx->crop_tiles = std::max(ctx->crop_tiles, ((f.w + CROP_TX - 1) / CROP_TX) * ((f.h + CROP_TY - 1) / CROP_TY));
     }
   ctx->h_crop.swap(next);
+  ctx->h_crop_planes.swap(planes);
   return HT_OK;
+}
+
+static_assert(sizeof(ht_face_crop_yuv) == 64 && offsetof(ht_face_crop_yuv, pitch) == 24 &&
+                  offsetof(ht_face_crop_yuv, width) == 36 && offsetof(ht_face_crop_yuv, height) == 40 &&
+                  offsetof(ht_face_crop_yuv, format) == 44 && offsetof(ht_face_crop_yuv, color) == 48 &&
+                  offsetof(ht_face_crop_yuv, pad_) == 52 && offsetof(ht_face_crop_yuv, scale) == 56,
+              "ht_face_crop_yuv layout");
+
+// A YUV crop as k_face_crop takes it, pitches resolved (the record is not checked)
+static void crop_yuv_record(const ht_face_crop_yuv &c, FaceCrop &f, CropPlanes &q) {
+  const bool nv12 = c.format == HT_YUV_NV12;
+  const int row[3] = {c.width, nv12 ? c.width : c.width / 2, c.width / 2};
+  int pitch[3];
+  for (int p = 0; p < 3; ++p) pitch[p] = c.pitch[p] ? c.pitch[p] : row[p];
+  f = FaceCrop{c.planes[0], c.width, c.height, pitch[0], nv12 ? CROP_NV12 : CROP_I420, c.scale};
+  q = CropPlanes{c.planes[1], nv12 ? c.planes[1] + 1 : c.planes[2], pitch[1], nv12 ? pitch[1] : pitch[2], c.color, 0};
+}
+
+// The YUV face crops of streams [first, first + n).  Everything is checked on the host before anything changes,
+// overlap over every plane of every crop and every debug canvas after the call.
+int ht_tracker_set_face_crop_yuv(ht_ctx *ctx, int first, int n, const ht_face_crop_yuv *crops) {
+  if (!ctx) return HT_ERR_ARG;
+  if (!ctx->tracker_on) return ctx->fail(HT_ERR_STATE, "ht_tracker_config has not been called");
+  const int mf = ctx->cfg.max_frames;
+  if (first < 0 || n <= 0 || first > mf - n) return ctx->fail(HT_ERR_ARG, "stream range outside [0,%d)", mf);
+  if (!crops) return ctx->fail(HT_ERR_ARG, "crops is NULL");
+  std::vector<FaceCrop> next = ctx->h_crop;
+  std::vector<CropPlanes> planes = ctx->h_crop_planes;
+  next.resize((size_t)mf, FaceCrop{});
+  planes.resize((size_t)mf, CropPlanes{});
+  for (int i = 0; i < n; ++i) {
+    const ht_face_crop_yuv &c = crops[i];
+    FaceCrop f{};
+    CropPlanes q{};
+    if (c.planes[0]) {
+      const bool nv12 = c.format == HT_YUV_NV12;
+      if (!nv12 && c.format != HT_YUV_I420)
+        return ctx->fail(HT_ERR_ARG, "record %d: format %d is not HT_YUV_NV12 or HT_YUV_I420", i, c.format);
+      if (c.color < 0 || c.color > (HT_YUV_BT709 | HT_YUV_FULL_RANGE))
+        return ctx->fail(HT_ERR_ARG, "record %d: color %d is not HT_YUV_BT601 or HT_YUV_BT709 [| HT_YUV_FULL_RANGE]", i, c.color);
+      if (c.width < 2 || c.height < 2 || c.width > 2048 || c.height > 2048 || (c.width & 1) || (c.height & 1))
+        return ctx->fail(HT_ERR_SIZE, "record %d: YUV face crop %dx%d is not even sizes in 2..2048", i, c.width, c.height);
+      const int used = nv12 ? 2 : 3;
+      for (int p = 0; p < 3; ++p) {
+        if ((p < used) != (c.planes[p] != nullptr))
+          return ctx->fail(HT_ERR_ARG, p < used ? "record %d: plane %d is missing" : "record %d: plane %d must be NULL", i, p);
+        if (c.planes[p] && !is_device_ptr(c.planes[p]))
+          return ctx->fail(HT_ERR_ARG, "record %d: plane %d is not device memory", i, p);
+      }
+      const int row[3] = {c.width, nv12 ? c.width : c.width / 2, c.width / 2};
+      for (int p = 0; p < used; ++p)
+        if (c.pitch[p] != 0 && c.pitch[p] < row[p])
+          return ctx->fail(HT_ERR_ARG, "record %d: pitch[%d] %d is below the row's %d bytes", i, p, c.pitch[p], row[p]);
+      if (c.pad_ != 0) return ctx->fail(HT_ERR_ARG, "record %d: pad_ is %d, not 0", i, c.pad_);
+      if (!(c.scale > 0.0 && c.scale <= 16.0)) return ctx->fail(HT_ERR_ARG, "record %d: scale %g outside (0, 16]", i, c.scale);
+      crop_yuv_record(c, f, q);
+    }
+    next[(size_t)(first + i)] = f;
+    planes[(size_t)(first + i)] = q;
+  }
+  const int clash = images_overlap(ctx->h_debug, next, planes, first, n);
+  if (clash != -1)
+    return ctx->fail(HT_ERR_ARG, "record %d: a plane overlaps another plane of the crop, another stream's face crop or a debug canvas",
+                     clash - first);
+  return crop_commit(ctx, first, n, next, planes);
 }
 
 static int view_record(const ht_video_view &view, int w, int h, ViewFeedRec &v, char *why);
@@ -2317,8 +2419,8 @@ static int tracker_tick(ht_ctx *ctx, const TickGroup *grp, int n_groups, const u
     if (feed && feed->view) src = CropSource{CROP_VIEW, 0, 0, 0, feed->view};
     else if (feed && feed->yuv) src = CropSource{CROP_YUV, 0, 0, 0, feed->yuv};
     else if (feed) src = CropSource{CROP_FEED, 0, 0, 0, feed->recs};
-    k_face_crop<<<dim3((unsigned)ctx->crop_tiles, (unsigned)n), 256, 0, st>>>(d_ids, geo, g0.w, g0.h, d_ev,
-                                                                              ctx->d_crop.as<FaceCrop>(), src);
+    k_face_crop<<<dim3((unsigned)ctx->crop_tiles, (unsigned)n), 256, 0, st>>>(
+        d_ids, geo, g0.w, g0.h, d_ev, ctx->d_crop.as<FaceCrop>(), ctx->d_crop_planes.as<CropPlanes>(), src);
     ++ctx->launches;
   }
   ctx->prof_begin(HT_PROF_TRACK_INIT, st);
@@ -3428,6 +3530,46 @@ extern "C" int ht_selftest_face_crop_rgba(const ht_tracker_event *ev, int cw, in
   if (rc != HT_OK) return rc;
   view_source_rgba(v, f->rgba, f->pitch ? f->pitch : 4 * f->width, f->width, f->height);
   return selftest_face_crop(ev, cw, ch, v, crop);
+}
+// k_face_crop's per-crop code for a YUV crop (the record is not checked): the crop of record `ev` on a cw x ch canvas
+// drawn from an image of any format (img, host planes) or an RGBA8 frame (rgba; exactly one of the two) through a view
+// (NULL: the whole frame upright) -> 1 if the record wrote the crop, 0 if not
+extern "C" int ht_selftest_face_crop_yuv(const ht_tracker_event *ev, int cw, int ch, const ht_yuv_image *img,
+                                         const ht_video_frame *rgba, const ht_video_view *view, const ht_face_crop_yuv *crop) {
+  YuvFeedRec r;
+  ViewFeedRec v;
+  char why[256];
+  const ht_video_view whole{};
+  const int w = img ? img->width : rgba->width, h = img ? img->height : rgba->height;
+  int rc = img ? yuv_record(*img, r, why) : HT_OK;
+  if (rc == HT_OK) rc = view_record(view ? *view : whole, w, h, v, why);
+  if (rc != HT_OK) return rc;
+  if (img) view_source_yuv(v, r);
+  else view_source_rgba(v, rgba->rgba, rgba->pitch ? rgba->pitch : 4 * w, w, h);
+  FaceCrop f;
+  CropPlanes c;
+  crop_yuv_record(*crop, f, c);
+  const TrackerEvent &e = *reinterpret_cast<const TrackerEvent *>(ev);
+  long long M[6];
+  if (!crop_map(e.detection, e.x, e.y, e.width, e.height, e.angle, cw, ch, v.sw, v.sh, f.w, f.h, f.scale, M)) return 0;
+  const bool nv12 = f.layout == CROP_NV12;
+  for (int j = 0; j < f.h; j += 2)
+    for (int i = 0; i < f.w; i += 2) {
+      if (v.kind == VIEW_RGBA) nv12 ? crop_yuv_block<VIEW_RGBA, true>(v, M, f, c, i, j) : crop_yuv_block<VIEW_RGBA, false>(v, M, f, c, i, j);
+      else if (v.kind == VIEW_NV12_I420)
+        nv12 ? crop_yuv_block<VIEW_NV12_I420, true>(v, M, f, c, i, j) : crop_yuv_block<VIEW_NV12_I420, false>(v, M, f, c, i, j);
+      else nv12 ? crop_yuv_block<VIEW_FMT, true>(v, M, f, c, i, j) : crop_yuv_block<VIEW_FMT, false>(v, M, f, c, i, j);
+    }
+  return 1;
+}
+// rgba_to_yuv420 over n 2 x 2 blocks: blocks[4k..4k+3] = p00, p01, p10, p11 -> out[6k..6k+5] = their Y, U, V
+extern "C" void ht_selftest_rgba_to_yuv420(int color, const uint32_t *blocks, long long n, uint8_t *out) {
+  for (long long k = 0; k < n; ++k) {
+    uint32_t uv;
+    const uint32_t y4 = rgba_to_yuv420(color, blocks[4 * k], blocks[4 * k + 1], blocks[4 * k + 2], blocks[4 * k + 3], uv);
+    for (int b = 0; b < 4; ++b) out[6 * k + b] = (uint8_t)(y4 >> (8 * b));
+    out[6 * k + 4] = (uint8_t)uv, out[6 * k + 5] = (uint8_t)(uv >> 8);
+  }
 }
 
 // k_ingest's per-pixel code over a whole frame batch

@@ -245,6 +245,43 @@ __host__ __device__ __forceinline__ uint32_t yuv_to_rgba(int color, uint32_t Y, 
   auto clamp255 = [](int v) { return (uint32_t)(v < 0 ? 0 : (v > 255 ? 255 : v)); };
   return clamp255(r) | clamp255(gr) << 8 | clamp255(b) << 16 | 0xff000000u;
 }
+// The way back, for YUV face crops (DESIGN.md 2, "Face crops", item 5): one 2 x 2 block of RGBA8 pixels becomes 4:2:0
+// in integers only, alpha ignored.  Y = y0 + ((yr R + yg G + yb B + 128) >> 8) per pixel; one chroma sample per block
+// from the block's sums, U = clamp255(128 + ((ur SR + ug SG + ub SB + 512) >> 10)) and V likewise: the centre-sited
+// box mean.  Each coefficient is round(256 x the real one), then each row is made to hit its exact sum (220 limited /
+// 256 full for Y, 0 for U and V) by moving the coefficient with the largest rounding error one step toward its real
+// value, the chroma rows keeping their primary 112 / 128: greys give U = V = 128 exactly and limited range stays in
+// Y 16..235, U / V 16..240.  Every row is within 1 level of the real-valued conversion rounded half up, over all 2^24
+// triples (tests/test_face_crop_yuv_host.py).  color: HT_YUV_BT601 / HT_YUV_BT709, optionally | HT_YUV_FULL_RANGE.
+//                          y0   yr   yg   yb    ur   ug   ub    vr   vg   vb
+//   BT.601 limited range   16   66  129   25   -38  -74  112   112  -94  -18
+//   BT.709 limited range   16   47  157   16   -26  -86  112   112 -102  -10
+//   BT.601 full range       0   77  150   29   -43  -85  128   128 -107  -21
+//   BT.709 full range       0   54  183   19   -29  -99  128   128 -116  -12
+// Every intermediate is below 2^18 in magnitude: int32 throughout, >> arithmetic.  p00 p01 / p10 p11 are the block's
+// rows -> their Y in bytes 0..3 in that order, and uv = U | V << 8.
+__host__ __device__ __forceinline__ uint32_t rgba_to_yuv420(int color, uint32_t p00, uint32_t p01, uint32_t p10,
+                                                            uint32_t p11, uint32_t &uv) {
+  const bool bt709 = (color & HT_YUV_BT709) != 0, full = (color & HT_YUV_FULL_RANGE) != 0;
+  const int y0 = full ? 0 : 16;
+  const int yr = full ? (bt709 ? 54 : 77) : (bt709 ? 47 : 66), yg = full ? (bt709 ? 183 : 150) : (bt709 ? 157 : 129);
+  const int yb = full ? (bt709 ? 19 : 29) : (bt709 ? 16 : 25), cp = full ? 128 : 112;
+  const int ur = full ? (bt709 ? -29 : -43) : (bt709 ? -26 : -38), ug = full ? (bt709 ? -99 : -85) : (bt709 ? -86 : -74);
+  const int vg = full ? (bt709 ? -116 : -107) : (bt709 ? -102 : -94), vb = full ? (bt709 ? -12 : -21) : (bt709 ? -10 : -18);
+  const uint32_t p[4] = {p00, p01, p10, p11};
+  uint32_t y4 = 0;
+  int sr = 0, sg = 0, sb = 0;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const int r = (int)(p[k] & 0xffu), g = (int)((p[k] >> 8) & 0xffu), b = (int)((p[k] >> 16) & 0xffu);
+    y4 |= (uint32_t)(y0 + ((yr * r + yg * g + yb * b + 128) >> 8)) << (8 * k);
+    sr += r, sg += g, sb += b;
+  }
+  auto clamp255 = [](int v) { return (uint32_t)(v < 0 ? 0 : (v > 255 ? 255 : v)); };
+  uv = clamp255(128 + ((ur * sr + ug * sg + cp * sb + 512) >> 10)) |
+       clamp255(128 + ((cp * sr + vg * sg + vb * sb + 512) >> 10)) << 8;
+  return y4;
+}
 // ht_tracker_feed_yuv / ht_ingest_yuv: one video frame of any ht_yuv_image format, pitches resolved.  Channel 0 (Y, or
 // R of a packed RGB format) of pixel (x, y) is the sample at y[y * ypitch + x * ystep]; channels 1 and 2 (U and V, or
 // G and B) are at u[(y >> sy) * upitch + (x >> sx) * cstep] and v[(y >> sy) * vpitch + (x >> sx) * cstep].  NV12 is

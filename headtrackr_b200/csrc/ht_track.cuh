@@ -1758,11 +1758,19 @@ __global__ void __launch_bounds__(256, 1) k_debug_strokes(const int32_t *__restr
 // Face crops (ht_tracker_set_face_crop; DESIGN.md 2, "Face crops"): after a tick whose record is "CS" with width > 0
 // and height > 0, the rectangle main.js strokes in green, scaled about its centre, grown to the crop's aspect ratio and
 // resampled upright from the tick's video at video resolution.
-// Layout of ht_face_crop, with the pitch resolved; rgba NULL: the stream has none.
+// Layout of ht_face_crop, with the pitch resolved; rgba NULL: the stream has none.  A YUV crop
+// (ht_tracker_set_face_crop_yuv) keeps its Y plane in rgba / pitch, its layout in `layout` and the rest in the stream's
+// CropPlanes.
+enum : int32_t { CROP_RGBA = 0, CROP_NV12 = 1, CROP_I420 = 2 };
 struct FaceCrop {
   uint8_t *rgba;
-  int32_t w, h, pitch, pad_;
+  int32_t w, h, pitch, layout;          // CROP_*
   double scale;
+};
+// The chroma planes and colour of a YUV crop, pitches resolved.  NV12 is v = u + 1 in one interleaved plane.
+struct CropPlanes {
+  uint8_t *u, *v;
+  int32_t upitch, vpitch, color, pad_;
 };
 constexpr int CROP_TX = 64, CROP_TY = 16;        // crop pixels per tile of k_face_crop
 
@@ -1876,14 +1884,54 @@ __device__ __noinline__ void face_crop_tile(const ViewFeedRec *__restrict__ vp, 
   }
 }
 
+// Two bytes at p (an even address: one 16-bit store)
+__host__ __device__ __forceinline__ void crop_put2(uint8_t *p, uint32_t lo, uint32_t hi) {
+  if ((reinterpret_cast<uintptr_t>(p) & 1u) == 0) *reinterpret_cast<uint16_t *>(p) = (uint16_t)(lo | hi << 8);
+  else p[0] = (uint8_t)lo, p[1] = (uint8_t)hi;
+}
+// The 2 x 2 block from even (X, Y) of YUV crop f / c: the four RGBA8 pixels of the crop of the same size and scale
+// (crop_pixel), converted by rgba_to_yuv420 into their four Y samples and one U and one V sample.
+template <int KIND, bool NV12>
+__host__ __device__ __forceinline__ void crop_yuv_block(const ViewFeedRec &v, const long long M[6], const FaceCrop &f,
+                                                        const CropPlanes &c, int X, int Y) {
+  uint32_t uv;
+  const uint32_t y4 = rgba_to_yuv420(c.color, crop_pixel<KIND>(v, M, X, Y), crop_pixel<KIND>(v, M, X + 1, Y),
+                                     crop_pixel<KIND>(v, M, X, Y + 1), crop_pixel<KIND>(v, M, X + 1, Y + 1), uv);
+  uint8_t *y = f.rgba + (size_t)Y * f.pitch + X;
+  crop_put2(y, y4 & 0xffu, (y4 >> 8) & 0xffu);
+  crop_put2(y + f.pitch, (y4 >> 16) & 0xffu, y4 >> 24);
+  const size_t row = (size_t)(Y >> 1);
+  if (NV12) {
+    crop_put2(c.u + row * c.upitch + X, uv & 0xffu, uv >> 8);
+  } else {
+    c.u[row * c.upitch + (X >> 1)] = (uint8_t)uv;
+    c.v[row * c.vpitch + (X >> 1)] = (uint8_t)(uv >> 8);
+  }
+}
+
+// One 64 x 16 tile from (X0, Y0) of YUV crop f / c: each thread one 2 x 2 block, a warp 64 consecutive Y bytes of two
+// rows.  Out of line per texel source and output layout, as face_crop_tile.  The view record and the map stay in
+// k_face_crop's shared memory (vp, Mp): copied into registers, as face_crop_tile does, they would lift k_face_crop from
+// 64 to 80 registers and cost every crop, RGBA included, a quarter of its resident CTAs.
+template <int KIND, bool NV12>
+__device__ __noinline__ void face_crop_yuv_tile(const ViewFeedRec *__restrict__ vp, const long long *__restrict__ Mp,
+                                                const FaceCrop f, const CropPlanes c, int X0, int Y0) {
+  const ViewFeedRec &v = *vp;
+  const long long *M = Mp;
+  const int X = X0 + 2 * (int)(threadIdx.x & 31), Y = Y0 + 2 * (int)(threadIdx.x >> 5);
+  if (X < f.w && Y < f.h) crop_yuv_block<KIND, NV12>(v, M, f, c, X, Y);
+}
+
 // After k_tracker_update: grid (tiles of the largest crop, batch entries).  Entry k's CTAs read its record
 // (events[geo[k].record], geo NULL: k) and canvas size (geo[k], geo NULL: cw x ch), and write the tiles of its stream's
-// crop on a crop tick; entries without a crop, without a crop tick, or past their own crop's tiles exit at once.
+// crop on a crop tick; entries without a crop, without a crop tick, or past their own crop's tiles exit at once.  An
+// RGBA crop's tiles go to face_crop_tile, a YUV crop's (layout, then planes[id]) to face_crop_yuv_tile.
 __global__ void __launch_bounds__(256) k_face_crop(const int32_t *__restrict__ ids, const EntryCanvas *__restrict__ geo,
                                                    int cw, int ch, const TrackerEvent *__restrict__ events,
-                                                   const FaceCrop *__restrict__ crops, CropSource src) {
-  const int k = blockIdx.y;
-  const FaceCrop f = crops[ids ? ids[k] : k];
+                                                   const FaceCrop *__restrict__ crops,
+                                                   const CropPlanes *__restrict__ planes, CropSource src) {
+  const int k = blockIdx.y, id = ids ? ids[k] : k;
+  const FaceCrop f = crops[id];
   if (!f.rgba) return;
   const int tiles_x = (f.w + CROP_TX - 1) / CROP_TX;
   if ((int)blockIdx.x >= tiles_x * ((f.h + CROP_TY - 1) / CROP_TY)) return;
@@ -1899,9 +1947,22 @@ __global__ void __launch_bounds__(256) k_face_crop(const int32_t *__restrict__ i
   __syncthreads();
   if (!on) return;
   const int X0 = ((int)blockIdx.x % tiles_x) * CROP_TX, Y0 = ((int)blockIdx.x / tiles_x) * CROP_TY;
-  if (v.kind == VIEW_RGBA) face_crop_tile<VIEW_RGBA>(&v, M, f, X0, Y0);
-  else if (v.kind == VIEW_NV12_I420) face_crop_tile<VIEW_NV12_I420>(&v, M, f, X0, Y0);
-  else face_crop_tile<VIEW_FMT>(&v, M, f, X0, Y0);
+  if (f.layout == CROP_RGBA) {
+    if (v.kind == VIEW_RGBA) face_crop_tile<VIEW_RGBA>(&v, M, f, X0, Y0);
+    else if (v.kind == VIEW_NV12_I420) face_crop_tile<VIEW_NV12_I420>(&v, M, f, X0, Y0);
+    else face_crop_tile<VIEW_FMT>(&v, M, f, X0, Y0);
+    return;
+  }
+  const CropPlanes c = planes[id];
+  if (f.layout == CROP_NV12) {
+    if (v.kind == VIEW_RGBA) face_crop_yuv_tile<VIEW_RGBA, true>(&v, M, f, c, X0, Y0);
+    else if (v.kind == VIEW_NV12_I420) face_crop_yuv_tile<VIEW_NV12_I420, true>(&v, M, f, c, X0, Y0);
+    else face_crop_yuv_tile<VIEW_FMT, true>(&v, M, f, c, X0, Y0);
+  } else {
+    if (v.kind == VIEW_RGBA) face_crop_yuv_tile<VIEW_RGBA, false>(&v, M, f, c, X0, Y0);
+    else if (v.kind == VIEW_NV12_I420) face_crop_yuv_tile<VIEW_NV12_I420, false>(&v, M, f, c, X0, Y0);
+    else face_crop_yuv_tile<VIEW_FMT, false>(&v, M, f, c, X0, Y0);
+  }
 }
 
 // ht_tracker_set_camera: one CTA constructs the cameras of streams [first, first + n) that have a controller

@@ -137,8 +137,9 @@ class TrackerSet:
     "Strokes").  No two streams may share a debug canvas.  A stream's "camera" key is its head-coupled camera
     controller, a dict as Context.tracker_set_camera takes (realisticAbsoluteCameraControl on the device, written to
     its `out` tensor on every tick with a headtrackingEvent).  A stream's "faceCrop" key is its face crop, a dict as
-    Context.tracker_set_face_crop takes: the tracked face cut upright out of the video into its `out` tensor on every
-    tick that keeps the face.
+    Context.tracker_set_face_crop takes: the tracked face cut upright out of the video into its `out` tensor (or, with
+    "format": "nv12" / "i420" and a "color", its NV12 / I420 planes for a video encoder) on every tick that keeps the
+    face.
     Differs from the reference in one place: start() on a running stream does nothing (the reference runs an extra,
     unscheduled pass)."""
 

@@ -457,7 +457,8 @@ typedef struct {
  * where the reference's timers write one after another.
  * Errors (nothing changes): HT_ERR_STATE before ht_tracker_config; HT_ERR_ARG for a range outside [0, max_frames),
  * n <= 0, canvases NULL, a host pointer, a pointer or pitch that is not a multiple of 4, a pitch below 4*width, or a
- * canvas whose byte range overlaps another stream's (over all streams that have a canvas after the call);
+ * canvas whose byte range overlaps another stream's (over all streams that have a canvas after the call) or any plane
+ * of any face crop, RGBA or YUV;
  * HT_ERR_SIZE for a size outside 1..16384. */
 int ht_tracker_set_debug(ht_ctx *ctx, int first, int n, const ht_debug_canvas *canvases);
 
@@ -501,7 +502,48 @@ typedef struct {
  * all streams after the call: the streams of a tick run concurrently); HT_ERR_SIZE for a size outside 1..2048. */
 int ht_tracker_set_face_crop(ht_ctx *ctx, int first, int n, const ht_face_crop *crops);
 
-/* The map of the crop `crop` (its size and scale; rgba and pitch are ignored) for tracker record `ev`, on a canvas of
+/* A stream's face crop as 4:2:0 video for an encoder: NVENC takes NV12; openh264, libx264, libvpx and WebRTC frame
+ * buffers take I420 (DESIGN.md 2, "Face crops", item 5).  It is, bit for bit, the RGBA8 crop of the same size and
+ * scale (ht_face_crop) converted with alpha ignored - so the part that leaves the video is black - by the library's one
+ * RGB-to-YUV conversion: Y = y0 + ((yr R + yg G + yb B + 128) >> 8) per pixel, and per 2 x 2 block
+ * U = clamp255(128 + ((ur SR + ug SG + ub SB + 512) >> 10)) of the block's sums (V likewise):
+ *     color          y0   yr  yg  yb    ur   ug   ub    vr   vg   vb
+ *     BT601          16   66 129  25   -38  -74  112   112  -94  -18
+ *     BT709          16   47 157  16   -26  -86  112   112 -102  -10
+ *     BT601 | FULL    0   77 150  29   -43  -85  128   128 -107  -21
+ *     BT709 | FULL    0   54 183  19   -29  -99  128   128 -116  -12
+ * Byte offsets, mirroring ht_yuv_image:
+ *     0  uint8_t *planes[3]   DEVICE memory: NV12 Y, UV (U first), NULL; I420 Y, U, V; planes[0] NULL: no crop
+ *    24  int32 pitch[3]       bytes per row; 0 -> tight (w, then w for NV12's UV or w/2 for I420's U and V); otherwise
+ *                             >= that; any pointer or pitch alignment
+ *    36  int32 width, height  S_w x S_h, both even, 2..2048
+ *    44  int32 format         HT_YUV_NV12 or HT_YUV_I420
+ *    48  int32 color          HT_YUV_BT601 or HT_YUV_BT709, optionally | HT_YUV_FULL_RANGE
+ *    52  int32 pad_           0
+ *    56  double scale         as ht_face_crop's */
+typedef struct {
+  uint8_t *planes[3];
+  int32_t pitch[3];
+  int32_t width, height;
+  int32_t format;
+  int32_t color;
+  int32_t pad_;
+  double scale;
+} ht_face_crop_yuv;       /* 64 bytes */
+/* Stream first+i gets the YUV crop crops[i] (host array), for i in [0, n).  A stream has at most one face crop in one
+ * layout: this call and ht_tracker_set_face_crop each replace it, whatever its layout, and a NULL crop removes it.  It
+ * is written on exactly the ticks, and lives exactly as long, as an RGBA crop (ht_tracker_set_face_crop); a tick with
+ * crops of either layout launches one kernel more, and ht_face_crop_map gives its map (that of the RGBA crop of its
+ * size and scale).
+ * Errors (nothing changes; the message names the record): HT_ERR_STATE before ht_tracker_config; HT_ERR_SIZE for a size
+ * that is odd or outside 2..2048; HT_ERR_ARG for a range outside [0, max_frames), n <= 0, crops NULL, a format other
+ * than NV12 / I420, a colour other than the four above, a missing or extra plane, a host pointer, a pitch below its
+ * row's bytes, a non-zero pad_, a scale that is not finite or outside (0, 16], or a plane whose bytes overlap another
+ * plane of the crop, another stream's crop of either layout or any debug canvas (over all streams after the call). */
+int ht_tracker_set_face_crop_yuv(ht_ctx *ctx, int first, int n, const ht_face_crop_yuv *crops);
+
+/* The map of the crop `crop` (its size and scale; rgba and pitch are ignored; a YUV crop has the map of the RGBA crop of
+ * its size and scale) for tracker record `ev`, on a canvas of
  * canvas_w x canvas_h drawn from a video_w x video_h video through `view` (NULL: the whole frame upright; for
  * ht_tracker_step the video is the canvas): crop pixel (i, j) samples video tap coordinates (U0 + i Ui + j Uj,
  * V0 + i Vi + j Vj) / 65536, with out = {U0, V0, Ui, Vi, Uj, Vj} exactly as the device computes them.  A tap coordinate

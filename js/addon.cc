@@ -27,6 +27,8 @@
 //   trackerSetDebugStrokes(handle, first, [bool, ...])  (ht_tracker_set_debug_strokes: main.js's strokes on the device)
 //   trackerSetFaceCrop(handle, first, [crop|null, ...])  (ht_tracker_set_face_crop: each stream's face crop, device
 //        memory)
+//   trackerSetFaceCropYuv(handle, first, [crop|null, ...])  (ht_tracker_set_face_crop_yuv: each stream's NV12 / I420
+//        face crop, device planes)
 //   trackerSetCamera(handle, first, [control|null, ...])  (ht_tracker_set_camera: each stream's head-coupled camera,
 //        realisticAbsoluteCameraControl on an ht_camera in device memory)
 //   trackerExport(handle, [stream, ...]) -> Buffer of records; trackerImport(handle, [stream, ...], records)
@@ -512,6 +514,58 @@ static napi_value TrackerSetFaceCrop(napi_env env, napi_callback_info info) {
   return nullptr;
 }
 
+static double GetNumber(napi_env env, napi_value obj, const char *name, double dflt);
+
+// trackerSetFaceCropYuv(handle, first, [{y, uv | u, v: BigInt device addresses, yPitch?, uvPitch? | uPitch?, vPitch?,
+// width, height, format: "nv12" | "i420", color: "bt601" | "bt709" | "bt601-full" | "bt709-full", scale?}, null, ...]):
+// stream first+i gets crops[i] (pitches default to tight, scale to 1); null or undefined: none
+static napi_value TrackerSetFaceCropYuv(napi_env env, napi_callback_info info) {
+  size_t argc = 3;
+  napi_value argv[3];
+  NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+  ht_ctx *ctx = Ctx(env, argv[0]);
+  int32_t first = 0;
+  uint32_t n = 0;
+  napi_get_value_int32(env, argv[1], &first);
+  NAPI_OK(napi_get_array_length(env, argv[2], &n));
+  std::vector<ht_face_crop_yuv> cs(n, ht_face_crop_yuv{{nullptr, nullptr, nullptr}, {0, 0, 0}, 0, 0, HT_YUV_NV12, HT_YUV_BT601, 0, 1.0});
+  for (uint32_t i = 0; i < n; ++i) {
+    napi_value r, v;
+    napi_valuetype t = napi_undefined;
+    NAPI_OK(napi_get_element(env, argv[2], i, &r));
+    napi_typeof(env, r, &t);
+    if (t != napi_object) continue;
+    char s[16] = {0};
+    size_t sl = 0;
+    if (napi_get_named_property(env, r, "format", &v) == napi_ok) napi_get_value_string_utf8(env, v, s, sizeof s, &sl);
+    const bool nv12 = strcmp(s, "i420") != 0;
+    cs[i].format = strcmp(s, "nv12") == 0 ? HT_YUV_NV12 : nv12 ? -1 : HT_YUV_I420;
+    static const struct { const char *name; int32_t code; } colors[] = {
+        {"bt601", HT_YUV_BT601}, {"bt709", HT_YUV_BT709}, {"bt601-full", HT_YUV_FULL_RANGE},
+        {"bt709-full", HT_YUV_BT709 | HT_YUV_FULL_RANGE}};
+    sl = 0;
+    s[0] = 0;
+    if (napi_get_named_property(env, r, "color", &v) == napi_ok) napi_get_value_string_utf8(env, v, s, sizeof s, &sl);
+    cs[i].color = sl == 0 ? HT_YUV_BT601 : -1;
+    for (const auto &c : colors)
+      if (strcmp(s, c.name) == 0) cs[i].color = c.code;
+    const char *planes[3] = {"y", nv12 ? "uv" : "u", "v"}, *pitches[3] = {"yPitch", nv12 ? "uvPitch" : "uPitch", "vPitch"};
+    for (int p = 0; p < (nv12 ? 2 : 3); ++p) {
+      uint64_t addr = 0;
+      bool lossless = false;
+      if (napi_get_named_property(env, r, planes[p], &v) == napi_ok) napi_get_value_bigint_uint64(env, v, &addr, &lossless);
+      cs[i].planes[p] = reinterpret_cast<uint8_t *>(static_cast<uintptr_t>(addr));
+      cs[i].pitch[p] = (int32_t)GetNumber(env, r, pitches[p], 0.0);
+    }
+    if (napi_get_named_property(env, r, "width", &v) == napi_ok) napi_get_value_int32(env, v, &cs[i].width);
+    if (napi_get_named_property(env, r, "height", &v) == napi_ok) napi_get_value_int32(env, v, &cs[i].height);
+    cs[i].scale = GetNumber(env, r, "scale", 1.0);
+  }
+  int rc = ht_tracker_set_face_crop_yuv(ctx, first, (int)n, cs.data());
+  if (rc < 0) return Throw(env, ctx, rc);
+  return nullptr;
+}
+
 static double GetNumber(napi_env env, napi_value obj, const char *name, double dflt) {
   napi_value v;
   napi_valuetype t = napi_undefined;
@@ -925,6 +979,7 @@ static napi_value Init(napi_env env, napi_value exports) {
       {"trackerSetDebug", nullptr, TrackerSetDebug, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerSetDebugStrokes", nullptr, TrackerSetDebugStrokes, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerSetFaceCrop", nullptr, TrackerSetFaceCrop, nullptr, nullptr, nullptr, napi_default, nullptr},
+      {"trackerSetFaceCropYuv", nullptr, TrackerSetFaceCropYuv, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerSetCamera", nullptr, TrackerSetCamera, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerExport", nullptr, TrackerExport, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerImport", nullptr, TrackerImport, nullptr, nullptr, nullptr, napi_default, nullptr},

@@ -32,7 +32,8 @@ streams: N 640x480 streams, device-resident frames and outputs, CUDA events arou
   crop*_* twopass*_*
                   (--crops) ht_tracker_feed_yuv from 1280x720 NV12 onto 320x240 canvases with 112x112 and 224x224 face
                   crops on none, 1/64 and all of the streams, against ht_ingest_yuv + grid_sample of the boxes (also
-                  --before-lib), and k_face_crop's time (crops_arms)
+                  --before-lib), NV12 and I420 crops against RGBA crops + a torch conversion, and k_face_crop's time
+                  (crops_arms)
 
 Prints one JSON line with the card's name and power limit read in the same run; --out also writes it to a file."""
 import argparse
@@ -683,6 +684,19 @@ def crop_theta(torch, ev, W, H, CW, CH, Sw, Sh, scale):
     return torch.stack([row0, row1], 1)
 
 
+def torch_nv12(torch, rgba):
+    """(N, S, S, 4) uint8 RGBA crops -> (Y (N, S, S), UV (N, S/2, S)) uint8: the library's BT.601 limited-range
+    conversion (DESIGN.md 2, "Face crops", item 5) as a caller writes it in torch"""
+    c = rgba[..., :3].to(torch.int32)
+    r, g, b = c[..., 0], c[..., 1], c[..., 2]
+    y = 16 + ((66 * r + 129 * g + 25 * b + 128) >> 8)
+    s = c.reshape(c.shape[0], c.shape[1] // 2, 2, c.shape[2] // 2, 2, 3).sum(dim=(2, 4))
+    sr, sg, sb = s[..., 0], s[..., 1], s[..., 2]
+    u = (128 + ((-38 * sr - 74 * sg + 112 * sb + 512) >> 10)).clamp(0, 255)
+    v = (128 + ((112 * sr - 94 * sg - 18 * sb + 512) >> 10)).clamp(0, 255)
+    return y.to(torch.uint8), torch.stack([u, v], -1).reshape(c.shape[0], c.shape[1] // 2, c.shape[2]).to(torch.uint8)
+
+
 def crops_arms(torch, stream, N, steps, rounds, before_lib=None):
     """Face crops (ht_tracker_set_face_crop) in steady tracking: N streams of 1280x720 NV12 device video fed onto
     320x240 canvases by ht_tracker_feed_yuv, every arm on its own context, all arms alternating tick by tick (the arm
@@ -694,9 +708,15 @@ def crops_arms(torch, stream, N, steps, rounds, before_lib=None):
       crop<S>64_cs          an S x S crop on every 64th stream
       twopass<S>_cs         what a caller does without crops: the crops-off tick, ht_ingest_yuv of every video to
                             RGBA8 at video size, then torch's grid_sample (fp16, bilinear) of every stream's box
+      crop<S>nv12_cs        an S x S NV12 crop on every stream (ht_tracker_set_face_crop_yuv, BT.601)
+      crop<S>i420_cs        an S x S I420 crop on every stream
+      rgbaconv<S>_cs        what a caller who encodes crops does without YUV crops: the crop<S>all tick, then the
+                            same BT.601 conversion to NV12 written in torch (integer ops on the device)
+      crop<S>all_before_cs  crop<S>all_cs with the library at `before_lib`
 
-    Then, in runs of their own under torch.profiler, k_face_crop's kernel time per tick in the crop<S>all arms.  The
-    records of every arm must agree on every timed tick."""
+    Then, in runs of their own under torch.profiler, k_face_crop's kernel time per tick in the crop<S>all,
+    crop<S>nv12 / crop<S>i420 and crop<S>all_before arms.  The records of every arm must agree on every timed tick, and every YUV crop must
+    equal the torch conversion of the RGBA crop of its stream."""
     import ctypes as C
     import torch.nn.functional as F
     from headtrackr_b200 import Context, _lib
@@ -714,14 +734,23 @@ def crops_arms(torch, stream, N, steps, rounds, before_lib=None):
     ingest_src = (_lib.YuvImage * N)(*imgs)
     rgba = torch.empty((N, H, W, 4), dtype=torch.uint8, device="cuda")
     crops = {S: torch.zeros((N, S, S, 4), dtype=torch.uint8, device="cuda") for S in (112, 224)}
-    twopass_out = {}
+
+    def planes(S, fmt):
+        def z(h, w):
+            return torch.zeros((N, h, w), dtype=torch.uint8, device="cuda")
+        return (z(S, S), z(S // 2, S)) if fmt == "nv12" else (z(S, S), z(S // 2, S // 2), z(S // 2, S // 2))
+    yuv = {(S, fmt): planes(S, fmt) for S in (112, 224) for fmt in ("nv12", "i420")}
+    twopass_out, conv_out = {}, {}
 
     def arm(kind, S=0, every=0):
         c = other_build_context(before_lib, **kw) if kind == "before" else Context(**kw)
         c.tracker_config()
         c.tracker_reset(0, N)
         c.tracker_start(0, N)
-        if every:
+        if kind in ("nv12", "i420"):
+            c.tracker_set_face_crop(0, [{"out": tuple(p[k] for p in yuv[(S, kind)]), "format": kind, "color": "bt601"}
+                                        for k in range(N)])
+        elif every:
             c.tracker_set_face_crop(0, [{"out": crops[S][k]} if k % every == 0 else None for k in range(N)])
         out = torch.empty(N * rec_bytes, dtype=torch.uint8, device="cuda")
 
@@ -735,13 +764,20 @@ def crops_arms(torch, stream, N, steps, rounds, before_lib=None):
                 src = rgba.permute(0, 3, 1, 2).half()
                 grid = F.affine_grid(theta.half(), (N, 4, S, S), align_corners=False)
                 twopass_out[S] = F.grid_sample(src, grid, mode="bilinear", padding_mode="zeros", align_corners=False)
+            if kind == "rgbaconv":
+                conv_out[S] = torch_nv12(torch, crops[S])
         return c, run, out
 
     arms = {"crop0_cs": arm("plain"), "crop112all_cs": arm("crop", 112, 1), "crop11264_cs": arm("crop", 112, 64),
             "crop224all_cs": arm("crop", 224, 1), "crop22464_cs": arm("crop", 224, 64),
             "twopass112_cs": arm("twopass", 112), "twopass224_cs": arm("twopass", 224)}
+    for S in (112, 224):
+        arms[f"crop{S}nv12_cs"], arms[f"crop{S}i420_cs"] = arm("nv12", S), arm("i420", S)
+        arms[f"rgbaconv{S}_cs"] = arm("rgbaconv", S, 1)
     if before_lib:
         arms["crop0_before_cs"] = arm("before")
+        for S in (112, 224):
+            arms[f"crop{S}all_before_cs"] = arm("before", S, 1)
     names = list(arms)
 
     def tick(name):
@@ -780,21 +816,32 @@ def crops_arms(torch, stream, N, steps, rounds, before_lib=None):
         fused = crops[S].permute(0, 3, 1, 2).float()[torch.tensor(cs, device="cuda")]
         two = twopass_out[S].float()[torch.tensor(cs, device="cuda")]
         res[f"twopass{S}_vs_fused_mean_abs_diff"] = float((fused - two).abs().mean())
+        # every YUV crop is the conversion of its RGBA crop (streams that never kept a face have no crop yet)
+        m = torch.tensor(cs, device="cuda")
+        want = torch_nv12(torch, crops[S])
+        y, uv = yuv[(S, "nv12")]
+        y4, u4, v4 = yuv[(S, "i420")]
+        res[f"crop{S}_yuv_equals_converted_rgba"] = bool(
+            torch.equal(y[m], want[0][m]) and torch.equal(uv[m], want[1][m]) and torch.equal(y4[m], want[0][m]) and
+            torch.equal(u4[m], want[1][..., 0::2][m]) and torch.equal(v4[m], want[1][..., 1::2][m]) and
+            torch.equal(conv_out[S][0], want[0]) and torch.equal(conv_out[S][1], want[1]))
 
     from torch.profiler import ProfilerActivity, profile
     for S in (112, 224):
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            for _ in range(steps):
-                now[0] += 20.0
-                arms[f"crop{S}all_cs"][1]()
-            torch.cuda.synchronize()
-        us = 0.0
-        for e in prof.key_averages():
-            if "k_face_crop" in e.key:
-                t = getattr(e, "device_time_total", None)
-                us += t if t is not None else e.cuda_time_total
-        res[f"k_face_crop_{S}_ms"] = us / 1000.0 / steps
-        res[f"k_face_crop_{S}_write_GBps"] = N * S * S * 4 / (us * 1e-6 / steps) / 1e9 if us > 0 else None
+        for layout, bpp in (("all", 4), ("nv12", 1.5), ("i420", 1.5)) + ((("all_before", 4),) if before_lib else ()):
+            with profile(activities=[ProfilerActivity.CUDA]) as prof:
+                for _ in range(steps):
+                    now[0] += 20.0
+                    arms[f"crop{S}{layout}_cs"][1]()
+                torch.cuda.synchronize()
+            us = 0.0
+            for e in prof.key_averages():
+                if "k_face_crop" in e.key:
+                    t = getattr(e, "device_time_total", None)
+                    us += t if t is not None else e.cuda_time_total
+            name = f"k_face_crop_{S}" + ("" if layout == "all" else f"_{layout}")
+            res[f"{name}_ms"] = us / 1000.0 / steps
+            res[f"{name}_write_GBps"] = N * S * S * bpp / (us * 1e-6 / steps) / 1e9 if us > 0 else None
     for c, _, _ in arms.values():
         c.close()
     return res
