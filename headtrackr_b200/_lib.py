@@ -133,6 +133,25 @@ class FaceCropYuv(C.Structure):
 assert C.sizeof(FaceCropYuv) == 64 and FaceCropYuv.scale.offset == 56
 
 
+# ht_face_tensor.dtype / .layout / .channels
+HT_TENSOR_U8, HT_TENSOR_F16, HT_TENSOR_BF16, HT_TENSOR_F32 = 0, 1, 2, 3
+HT_TENSOR_CHW, HT_TENSOR_HWC = 0, 1
+HT_TENSOR_RGB, HT_TENSOR_BGR, HT_TENSOR_GRAY = 0, 1, 2
+
+
+class FaceTensor(C.Structure):
+    """ht_face_tensor: a stream's face as a model's input for ht_tracker_set_face_tensor (device memory; data NULL =
+    none; strides in elements; the element (k, j, i) at k plane_stride + j row_stride + i (CHW) or j row_stride + i C + k
+    (HWC); value fmaf(c, mul[k], add[k]) rounded to the dtype; scale in (0, 16])"""
+    _fields_ = [("data", C.c_void_p), ("row_stride", C.c_int64), ("plane_stride", C.c_int64), ("width", C.c_int32),
+                ("height", C.c_int32), ("dtype", C.c_int32), ("layout", C.c_int32), ("channels", C.c_int32),
+                ("pad_", C.c_int32), ("mul", C.c_float * 3), ("add", C.c_float * 3), ("scale", C.c_double)]
+
+
+assert C.sizeof(FaceTensor) == 80 and FaceTensor.width.offset == 24 and FaceTensor.mul.offset == 48 and \
+    FaceTensor.add.offset == 60 and FaceTensor.scale.offset == 72
+
+
 class Camera(C.Structure):
     """ht_camera: a stream's head-coupled camera (HT_CAMERA_BYTES, in device memory; camera_from_bytes decodes it)"""
     _fields_ = [("position", C.c_double * 3), ("fov", C.c_double), ("view", C.c_double * 6), ("events", C.c_uint32),
@@ -193,7 +212,7 @@ _lib = None
 
 EXPORTS = ["ht_version", "ht_create", "ht_destroy", "ht_last_error", "ht_sync", "ht_max_rects", "ht_detect",
            "ht_track_init", "ht_track_init_from_detect", "ht_track", "ht_detect_track", "ht_stream_reset", "ht_stream_step", "ht_stream_head_config", "ht_stream_step_head",
-           "ht_tracker_config", "ht_tracker_reset", "ht_tracker_start", "ht_tracker_stop", "ht_tracker_step", "ht_tracker_feed", "ht_tracker_set_params", "ht_tracker_feed_canvases", "ht_tracker_set_debug", "ht_tracker_set_debug_strokes", "ht_tracker_set_face_crop", "ht_tracker_set_face_crop_yuv", "ht_face_crop_map", "ht_tracker_set_camera", "ht_tracker_export", "ht_tracker_import", "ht_tracker_feed_yuv", "ht_ingest", "ht_ingest_yuv",
+           "ht_tracker_config", "ht_tracker_reset", "ht_tracker_start", "ht_tracker_stop", "ht_tracker_step", "ht_tracker_feed", "ht_tracker_set_params", "ht_tracker_feed_canvases", "ht_tracker_set_debug", "ht_tracker_set_debug_strokes", "ht_tracker_set_face_crop", "ht_tracker_set_face_crop_yuv", "ht_tracker_set_face_tensor", "ht_face_crop_map", "ht_tracker_set_camera", "ht_tracker_export", "ht_tracker_import", "ht_tracker_feed_yuv", "ht_ingest", "ht_ingest_yuv",
            "ht_tracker_feed_views", "ht_tracker_feed_yuv_views", "ht_ingest_views", "ht_ingest_yuv_views", "ht_backprojection", "ht_whitebalance",
            "ht_plan_info", "ht_debug_plane", "ht_debug_raw", "ht_debug_model_hist", "ht_debug_track_stats", "ht_set_track_memo", "ht_set_pipeline", "ht_join", "ht_debug_set_exactness", "ht_debug_track_trace", "ht_debug_track_phases", "ht_launch_count",
            "ht_profile", "ht_profile_read"]
@@ -241,6 +260,7 @@ def lib():
     L.ht_tracker_set_debug_strokes.argtypes = [vp, C.c_int, C.c_int, vp]
     L.ht_tracker_set_face_crop.argtypes = [vp, C.c_int, C.c_int, vp]
     L.ht_tracker_set_face_crop_yuv.argtypes = [vp, C.c_int, C.c_int, vp]
+    L.ht_tracker_set_face_tensor.argtypes = [vp, C.c_int, C.c_int, vp]
     L.ht_face_crop_map.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp]
     L.ht_tracker_set_camera.argtypes = [vp, C.c_int, C.c_int, vp]
     L.ht_tracker_export.argtypes = [vp, vp, C.c_int, vp]

@@ -4,11 +4,12 @@ Accepts numpy uint8 arrays (host memory) or torch CUDA uint8 tensors (device mem
 shape (n, H, W, 4) or (H, W, 4).  torch is optional and only used for device-resident batches.
 """
 import ctypes as C
+import math
 
 import numpy as np
 
 from . import _lib
-from ._lib import (Camera, CameraControl, CanvasFrame, DebugCanvas, FaceCrop, FaceCropYuv, HeadEvent, HeadParams, HtError, Rect, StreamEvent, TrackerEvent, TrackerParams, TrackObj, VideoFrame,
+from ._lib import (Camera, CameraControl, CanvasFrame, DebugCanvas, FaceCrop, FaceCropYuv, FaceTensor, HeadEvent, HeadParams, HtError, Rect, StreamEvent, TrackerEvent, TrackerParams, TrackObj, VideoFrame,
                    VideoView, Window, YuvFrame, YuvImage)
 from .views import video_view
 from .synth import load_cascade_blob
@@ -155,6 +156,78 @@ def _crop_runs(recs):
     return [tuple(r) for r in runs]
 
 
+_TENSOR_LAYOUTS = {"chw": _lib.HT_TENSOR_CHW, "hwc": _lib.HT_TENSOR_HWC}
+_TENSOR_CHANNELS = {"rgb": _lib.HT_TENSOR_RGB, "bgr": _lib.HT_TENSOR_BGR, "gray": _lib.HT_TENSOR_GRAY}
+
+
+def _tensor_dtype(dtype):
+    import torch
+    codes = {torch.uint8: _lib.HT_TENSOR_U8, torch.float16: _lib.HT_TENSOR_F16, torch.bfloat16: _lib.HT_TENSOR_BF16,
+             torch.float32: _lib.HT_TENSOR_F32}
+    if dtype not in codes:
+        raise ValueError("a face tensor is uint8, float16, bfloat16 or float32")
+    return codes[dtype]
+
+
+def _channel_values(v, n, fill, what):
+    """a scalar, n per-channel values or all 3 of the record -> 3 floats, the unused ones `fill`"""
+    vs = [float(x) for x in v] if isinstance(v, (list, tuple)) or hasattr(v, "__len__") else [float(v)] * n
+    if len(vs) == 3:
+        return vs
+    if len(vs) != n:
+        raise ValueError(f"{what} needs {n} value(s), one per channel")
+    return vs + [fill] * (3 - n)
+
+
+def tensor_affine(dtype, channels="rgb", mean=None, std=None):
+    """(mul, add) of a face tensor, 3 floats each, from a torchvision-style mean / std (in the tensor's channel order,
+    on the 0..1 scale): mul = float32(1 / (255 std)) and add = float32(-mean / std), each computed in float64 and
+    rounded once.  A uint8 tensor takes no mean / std: (1, 0).  Floats without mean / std: mean 0, std 1 (x / 255)."""
+    n = 1 if channels == "gray" else 3
+    if _tensor_dtype(dtype) == _lib.HT_TENSOR_U8:
+        if mean is not None or std is not None:
+            raise ValueError("a uint8 face tensor takes no mean / std")
+        return [1.0] * 3, [0.0] * 3
+    m = _channel_values(0.0 if mean is None else mean, n, 0.0, "mean")
+    sd = _channel_values(1.0 if std is None else std, n, 1.0, "std")
+    if not all(math.isfinite(x) and x != 0 for x in sd):
+        raise ValueError("std must be finite and non-zero")
+    f32 = lambda x: float(np.float32(x))  # noqa: E731
+    return [f32(1.0 / (255.0 * x)) for x in sd], [f32(-a / b) for a, b in zip(m, sd)]
+
+
+def _face_tensor_record(c):
+    """a face tensor dict of Context.tracker_set_face_tensor -> its FaceTensor (None: no tensor)"""
+    if c is None:
+        return None
+    out = c["out"]
+    if not _is_torch(out) or not out.is_cuda:
+        raise ValueError("a face tensor is a torch CUDA tensor")
+    layout, channels = c.get("layout", "chw"), c.get("channels", "rgb")
+    if layout not in _TENSOR_LAYOUTS or channels not in _TENSOR_CHANNELS:
+        raise ValueError("a face tensor's layout is 'chw' or 'hwc', its channels 'rgb', 'bgr' or 'gray'")
+    dtype, n = _tensor_dtype(out.dtype), 1 if channels == "gray" else 3
+    if out.dim() != 3:
+        raise ValueError("a face tensor is 3-D: (C, S_h, S_w) or (S_h, S_w, C)")
+    if layout == "chw":
+        if out.shape[0] != n or out.stride(2) != 1:
+            raise ValueError(f"a CHW {channels} face tensor is ({n}, S_h, S_w) with unit x stride")
+        h, w, row, plane = out.shape[1], out.shape[2], out.stride(1), out.stride(0) if n == 3 else 0
+    else:
+        if out.shape[2] != n or out.stride(2) != 1 or out.stride(1) != n:
+            raise ValueError(f"an HWC {channels} face tensor is (S_h, S_w, {n}) with strides (row, {n}, 1)")
+        h, w, row, plane = out.shape[0], out.shape[1], out.stride(0), 0
+    if "mul" in c or "add" in c:
+        if "mean" in c or "std" in c:
+            raise ValueError("a face tensor takes mean / std or mul / add, not both")
+        mul = _channel_values(c.get("mul", 1.0), n, 1.0, "mul")
+        add = _channel_values(c.get("add", 0.0), n, 0.0, "add")
+    else:
+        mul, add = tensor_affine(out.dtype, channels, c.get("mean"), c.get("std"))
+    return FaceTensor(out.data_ptr(), row, plane, w, h, dtype, _TENSOR_LAYOUTS[layout], _TENSOR_CHANNELS[channels], 0,
+                      (C.c_float * 3)(*mul), (C.c_float * 3)(*add), float(c.get("scale", 1.0)))
+
+
 def _per_record(v, n, what):
     vs = list(v) if isinstance(v, (list, tuple)) else [v] * n
     if len(vs) != n:
@@ -225,6 +298,7 @@ class Context:
         self._debug = {}                  # stream -> its debug canvas tensor, kept alive while the library writes it
         self._camera = {}                 # stream -> its camera tensor, likewise
         self._crops = {}                  # stream -> its face crop dict (and so its tensors), likewise
+        self._tensors = {}                # stream -> its face tensor dict, likewise
 
     def close(self):
         if getattr(self, "_h", None) and self._h.value:
@@ -399,6 +473,7 @@ class Context:
             self._debug = {}
             self._camera = {}
             self._crops = {}
+            self._tensors = {}
             return
         p = tracker_params(retryDetection, calcAngles, smoothing, fov, cameraOffset, headPosition, edgecorrection, alpha,
                            distance_to_screen)
@@ -406,6 +481,7 @@ class Context:
         self._debug = {}                  # ht_tracker_config discards every debug canvas
         self._camera = {}                 # and every camera controller
         self._crops = {}                  # and every face crop
+        self._tensors = {}                # and every face tensor
 
     def tracker_set_params(self, first, params):
         """Parameters of streams first, first+1, ...: one dict of tracker_config's keywords (enable excluded) per stream,
@@ -488,6 +564,55 @@ class Context:
         arr = (T * len(recs))(*[r if r is not None else T() for r in recs])
         setter = self._L.ht_tracker_set_face_crop_yuv if yuv else self._L.ht_tracker_set_face_crop
         self._check(setter(self._h, first, len(recs), C.addressof(arr)))
+
+    def tracker_set_face_tensor(self, first, tensors):
+        """Face tensors of streams first, first+1, ... (ht_tracker_set_face_tensor): per stream None (none) or a dict
+        {"out": torch CUDA tensor, "layout": "chw", "channels": "rgb", "mean": ..., "std": ... | "mul": ..., "add": ...,
+        "scale": 1.0}.  `out` is uint8, float16, bfloat16 or float32 - its dtype is the tensor's - shaped (C, S_h, S_w)
+        with unit x stride ("chw") or (S_h, S_w, C) with strides (row, C, 1) ("hwc"), C = 3 ("rgb", "bgr") or 1
+        ("gray", the detector's gray); other strides pass through, so a slice of a batch tensor works.  Each element is
+        fmaf(c, mul[k], add[k]) rounded to the dtype, c the channel byte of the RGBA crop of the same size and scale
+        (uint8: c itself).  mean / std (scalars or one per channel, in the tensor's channel order, on the 0..1 scale
+        as torchvision's Normalize takes them) give mul = float32(1 / (255 std)), add = float32(-mean / std), computed
+        in float64 and rounded once (tensor_affine); without either, a float tensor holds c / 255.  After every tick
+        on which track() kept the face, `out` holds that tick's face (DESIGN.md 2, "Face crops", item 6).  The tensor
+        is independent of the stream's face crop - tracker_set_face_crop never touches it - and outlives set_params,
+        stop, start, reset and import; tracker_config removes it.  The context keeps the tensors alive while set."""
+        first, tensors = int(first), list(tensors)
+        recs = [_face_tensor_record(t) for t in tensors]
+        arr = (FaceTensor * max(1, len(recs)))(*[r if r is not None else FaceTensor() for r in recs])
+        self._check(self._L.ht_tracker_set_face_tensor(self._h, first, len(recs), C.addressof(arr)))
+        for i, t in enumerate(tensors):
+            if t is None:
+                self._tensors.pop(first + i, None)
+            else:
+                self._tensors[first + i] = t
+
+    def face_tensor_batch(self, first, n, height, width, dtype=None, layout="chw", channels="rgb", mean=None, std=None,
+                          scale=1.0):
+        """A batch of face tensors for streams first .. first+n-1: allocates (n, C, height, width) ("chw") or
+        (n, height, width, C) ("hwc") of `dtype` (default torch.float16) on the context's device, sets stream first+i
+        to slice i (tracker_set_face_tensor, mean / std as there) and returns it.  It starts as what a black crop
+        converts to (add[k] per channel), so a slot without a face yet reads as black; streams.face_written(records)
+        says which slots a tick refreshed.  The fill has completed when this returns, whatever stream the library and
+        torch run on."""
+        import torch
+        dtype = torch.float16 if dtype is None else dtype
+        c = 1 if channels == "gray" else 3
+        shape = (n, c, height, width) if layout == "chw" else (n, height, width, c)
+        out = torch.empty(shape, dtype=dtype, device=f"cuda:{self.device}")
+        _, add = tensor_affine(dtype, channels, mean, std)
+        for k in range(c):
+            (out[:, k] if layout == "chw" else out[..., k]).fill_(add[k] + 0.0)   # fmaf(0, mul, -0.0) is +0.0
+        # the fill runs on torch's stream, the ticks that write faces on the library's: the fill must have landed
+        # before a tick can write, or it would blacken faces that face_written reports as fresh
+        torch.cuda.current_stream(out.device).synchronize()
+        keys = {} if mean is None else {"mean": mean}
+        if std is not None:
+            keys["std"] = std
+        self.tracker_set_face_tensor(first, [dict(out=out[i], layout=layout, channels=channels, scale=scale, **keys)
+                                             for i in range(n)])
+        return out
 
     def tracker_set_camera(self, first, controls):
         """Head-coupled camera controllers of streams first, first+1, ...: per stream None (none) or a dict of

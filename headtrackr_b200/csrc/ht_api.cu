@@ -588,6 +588,11 @@ struct ht_ctx {
   std::vector<FaceCrop> h_crop;
   std::vector<CropPlanes> h_crop_planes;
   int crop_count = 0, crop_tiles = 0;
+  // ht_tracker_set_face_tensor: per stream its FaceTensor (device array and host copy), the number of streams that have
+  // one (0: k_face_crop has no tensor slice) and the tiles of the largest
+  DevBuf d_tensor;
+  std::vector<FaceTensor> h_tensor;
+  int tensor_count = 0, tensor_tiles = 0;
   // ht_tracker_feed(_canvases): the record table {ids[n], clocks[n], FeedRec[n], EntryCanvas[n], tile starts[n+1]}
   // goes up in one copy from pinned memory; the videos are drawn into the canvas arena (batch entry k's canvas at
   // EntryCanvas::base), zeroed when it grows
@@ -1770,6 +1775,11 @@ int ht_tracker_config(ht_ctx *ctx, const ht_tracker_params *params) {
     ctx->h_crop_planes.assign(mf, CropPlanes{});
     ctx->crop_count = ctx->crop_tiles = 0;
   }
+  if (ctx->tensor_count > 0) {   // and every face tensor
+    CK(cudaMemsetAsync(ctx->d_tensor.p, 0, mf * sizeof(FaceTensor), ctx->stream));
+    ctx->h_tensor.assign(mf, FaceTensor{});
+    ctx->tensor_count = ctx->tensor_tiles = 0;
+  }
   if (!params) {                 // off: every stream as after ht_stream_reset (the lifecycle has used the tracker slots)
     if (ctx->tracker_on) {
       ctx->tracker_on = false;
@@ -1848,17 +1858,39 @@ static int debug_commit(ht_ctx *ctx, int first, int n, std::vector<DebugCanvas> 
   return HT_OK;
 }
 
-// Whether two of the images written during a tick - every debug canvas and every plane of every face crop - share a
-// byte: the streams of a tick run concurrently.  -> -1 if none do; otherwise a stream whose crop takes part, one in
-// [first, first + n) if there is one (so that a setter can name the record), or -2 if only debug canvases do.
+// Bytes a face tensor's span covers: `rows` rows of `row` elements of `es` bytes each, the last one `last` elements
+static size_t tensor_span(const FaceTensor &t, long long last) {
+  const size_t es = t.dtype == HT_TENSOR_U8 ? 1 : t.dtype == HT_TENSOR_F32 ? 4 : 2;
+  return ((size_t)(t.h - 1) * (size_t)t.row + (size_t)last) * es;
+}
+
+// Whether two of the images written during a tick - every debug canvas, every plane of every face crop and every
+// channel plane (CHW) or whole tensor (HWC) of every face tensor - share a byte: the streams of a tick run
+// concurrently.  -> -1 if none do; otherwise a stream whose crop (tensor_side false) or tensor (true) takes part, one
+// in [first, first + n) if there is one (so that a setter can name the record), or -2 if only debug canvases do.
 static int images_overlap(const std::vector<DebugCanvas> &dbg, const std::vector<FaceCrop> &crops,
-                          const std::vector<CropPlanes> &planes, int first = 0, int n = 0) {
-  struct Span { uintptr_t start, end; int crop; };        // crop: its stream, -2 for a debug canvas
+                          const std::vector<CropPlanes> &planes, const std::vector<FaceTensor> &tensors, int first = 0,
+                          int n = 0, bool tensor_side = false) {
+  struct Span { uintptr_t start, end; int crop; bool tensor; };   // crop: its stream, -2 for a debug canvas
   std::vector<Span> spans;
   auto add = [&](const uint8_t *p, int bytes, int rows, int pitch, int crop) {
     const uintptr_t s = reinterpret_cast<uintptr_t>(p);
-    spans.push_back(Span{s, s + (size_t)(rows - 1) * pitch + (size_t)bytes, crop});
+    spans.push_back(Span{s, s + (size_t)(rows - 1) * pitch + (size_t)bytes, crop, false});
   };
+  for (size_t k = 0; k < tensors.size(); ++k) {
+    const FaceTensor &t = tensors[k];
+    if (!t.data) continue;
+    const uintptr_t s = reinterpret_cast<uintptr_t>(t.data);
+    const size_t es = t.dtype == HT_TENSOR_U8 ? 1 : t.dtype == HT_TENSOR_F32 ? 4 : 2;
+    const int C = t.channels == HT_TENSOR_GRAY ? 1 : 3;
+    if (t.layout == HT_TENSOR_HWC) {
+      spans.push_back(Span{s, s + tensor_span(t, (long long)C * t.w), (int)k, true});
+    } else {
+      for (int c = 0; c < C; ++c)
+        spans.push_back(Span{s + (size_t)c * (size_t)t.plane * es, s + (size_t)c * (size_t)t.plane * es + tensor_span(t, t.w),
+                             (int)k, true});
+    }
+  }
   for (const DebugCanvas &d : dbg)
     if (d.rgba) add(d.rgba, 4 * d.w, d.h, d.pitch, -2);
   for (size_t k = 0; k < crops.size(); ++k) {
@@ -1879,7 +1911,7 @@ static int images_overlap(const std::vector<DebugCanvas> &dbg, const std::vector
   for (size_t i = 1; i < spans.size(); ++i)
     if (spans[i].start < spans[i - 1].end)
       for (const Span *s : {&spans[i - 1], &spans[i]}) {
-        if (s->crop >= first && s->crop < first + n) return s->crop;
+        if (s->tensor == tensor_side && s->crop >= first && s->crop < first + n) return s->crop;
         if (found < 0 || s->crop >= 0) found = std::max(found, s->crop);
       }
   return found;
@@ -1921,8 +1953,10 @@ int ht_tracker_set_debug(ht_ctx *ctx, int first, int n, const ht_debug_canvas *c
   for (size_t i = 1; i < spans.size(); ++i)
     if (spans[i].first < spans[i - 1].second)
       return ctx->fail(HT_ERR_ARG, "a debug canvas overlaps another stream's debug canvas");
-  if (ctx->crop_count > 0 && images_overlap(next, ctx->h_crop, ctx->h_crop_planes) != -1)
+  if (ctx->crop_count > 0 && images_overlap(next, ctx->h_crop, ctx->h_crop_planes, {}) != -1)
     return ctx->fail(HT_ERR_ARG, "a debug canvas overlaps a face crop");
+  if (ctx->tensor_count > 0 && images_overlap(next, {}, {}, ctx->h_tensor) != -1)
+    return ctx->fail(HT_ERR_ARG, "a debug canvas overlaps a face tensor");
   return debug_commit(ctx, first, n, next);
 }
 
@@ -1977,22 +2011,32 @@ int ht_tracker_set_face_crop(ht_ctx *ctx, int first, int n, const ht_face_crop *
     next[(size_t)(first + i)] = f;
     planes[(size_t)(first + i)] = CropPlanes{};
   }
-  if (images_overlap(ctx->h_debug, next, planes) != -1)
+  if (images_overlap(ctx->h_debug, next, planes, {}) != -1)
     return ctx->fail(HT_ERR_ARG, "a face crop overlaps another stream's face crop or a debug canvas");
+  if (ctx->tensor_count > 0 && images_overlap({}, next, planes, ctx->h_tensor) != -1)
+    return ctx->fail(HT_ERR_ARG, "a face crop overlaps a face tensor");
   return crop_commit(ctx, first, n, next, planes);
+}
+
+// k_face_crop's tables - every stream's FaceCrop, CropPlanes and FaceTensor, all 0 at first - on first use of either
+// setter: a grid with a tensor slice also has the crop slice, which reads the crop table.
+static int crop_tables(ht_ctx *ctx) {
+  const size_t mf = (size_t)ctx->cfg.max_frames;
+  if (ctx->d_crop.p) return HT_OK;
+  CK(ctx->d_crop.reserve(mf * sizeof(FaceCrop)));
+  CK(cudaMemsetAsync(ctx->d_crop.p, 0, mf * sizeof(FaceCrop), ctx->stream));
+  CK(ctx->d_crop_planes.reserve(mf * sizeof(CropPlanes)));
+  CK(cudaMemsetAsync(ctx->d_crop_planes.p, 0, mf * sizeof(CropPlanes), ctx->stream));
+  CK(ctx->d_tensor.reserve(mf * sizeof(FaceTensor)));
+  CK(cudaMemsetAsync(ctx->d_tensor.p, 0, mf * sizeof(FaceTensor), ctx->stream));
+  return HT_OK;
 }
 
 // The checked crops of streams [first, first + n), of either layout, into the device tables and the context.
 static int crop_commit(ht_ctx *ctx, int first, int n, std::vector<FaceCrop> &next, std::vector<CropPlanes> &planes) {
-  const int mf = ctx->cfg.max_frames;
   { const int jr = join_aux(ctx); if (jr != HT_OK) return jr; }
   CK(cudaSetDevice(ctx->cfg.device));
-  if (!ctx->d_crop.p) {
-    CK(ctx->d_crop.reserve((size_t)mf * sizeof(FaceCrop)));
-    CK(cudaMemsetAsync(ctx->d_crop.p, 0, (size_t)mf * sizeof(FaceCrop), ctx->stream));
-    CK(ctx->d_crop_planes.reserve((size_t)mf * sizeof(CropPlanes)));
-    CK(cudaMemsetAsync(ctx->d_crop_planes.p, 0, (size_t)mf * sizeof(CropPlanes), ctx->stream));
-  }
+  { const int tr = crop_tables(ctx); if (tr != HT_OK) return tr; }
   CK(cudaMemcpyAsync(ctx->d_crop.as<FaceCrop>() + first, next.data() + first, (size_t)n * sizeof(FaceCrop),
                      cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaMemcpyAsync(ctx->d_crop_planes.as<CropPlanes>() + first, planes.data() + first, (size_t)n * sizeof(CropPlanes),
@@ -2067,11 +2111,102 @@ int ht_tracker_set_face_crop_yuv(ht_ctx *ctx, int first, int n, const ht_face_cr
     next[(size_t)(first + i)] = f;
     planes[(size_t)(first + i)] = q;
   }
-  const int clash = images_overlap(ctx->h_debug, next, planes, first, n);
+  const int clash = images_overlap(ctx->h_debug, next, planes, {}, first, n);
   if (clash != -1)
     return ctx->fail(HT_ERR_ARG, "record %d: a plane overlaps another plane of the crop, another stream's face crop or a debug canvas",
                      clash - first);
+  const int tclash = ctx->tensor_count > 0 ? images_overlap({}, next, planes, ctx->h_tensor, first, n) : -1;
+  if (tclash != -1) return ctx->fail(HT_ERR_ARG, "record %d: a plane overlaps a face tensor", tclash - first);
   return crop_commit(ctx, first, n, next, planes);
+}
+
+static_assert(sizeof(ht_face_tensor) == 80 && sizeof(FaceTensor) == sizeof(ht_face_tensor) &&
+                  offsetof(ht_face_tensor, row_stride) == 8 && offsetof(FaceTensor, row) == 8 &&
+                  offsetof(ht_face_tensor, plane_stride) == 16 && offsetof(FaceTensor, plane) == 16 &&
+                  offsetof(ht_face_tensor, width) == 24 && offsetof(FaceTensor, w) == 24 &&
+                  offsetof(ht_face_tensor, dtype) == 32 && offsetof(FaceTensor, dtype) == 32 &&
+                  offsetof(ht_face_tensor, layout) == 36 && offsetof(FaceTensor, layout) == 36 &&
+                  offsetof(ht_face_tensor, channels) == 40 && offsetof(FaceTensor, channels) == 40 &&
+                  offsetof(ht_face_tensor, mul) == 48 && offsetof(FaceTensor, mul) == 48 &&
+                  offsetof(ht_face_tensor, add) == 60 && offsetof(FaceTensor, add) == 60 &&
+                  offsetof(ht_face_tensor, scale) == 72 && offsetof(FaceTensor, scale) == 72,
+              "ht_face_tensor layout");
+
+// A face tensor record as k_face_crop takes it: the same bytes
+static FaceTensor tensor_record(const ht_face_tensor &t) {
+  FaceTensor f;
+  memcpy(&f, &t, sizeof f);
+  return f;
+}
+
+// The face tensors of streams [first, first + n).  Everything is checked on the host before anything changes, overlap
+// over every tensor plane, crop plane and debug canvas after the call.  Crops are untouched.
+int ht_tracker_set_face_tensor(ht_ctx *ctx, int first, int n, const ht_face_tensor *tensors) {
+  if (!ctx) return HT_ERR_ARG;
+  if (!ctx->tracker_on) return ctx->fail(HT_ERR_STATE, "ht_tracker_config has not been called");
+  const int mf = ctx->cfg.max_frames;
+  if (first < 0 || n <= 0 || first > mf - n) return ctx->fail(HT_ERR_ARG, "stream range outside [0,%d)", mf);
+  if (!tensors) return ctx->fail(HT_ERR_ARG, "tensors is NULL");
+  std::vector<FaceTensor> next = ctx->h_tensor;
+  next.resize((size_t)mf, FaceTensor{});
+  const long long cap = 1ll << 40;
+  for (int i = 0; i < n; ++i) {
+    const ht_face_tensor &t = tensors[i];
+    FaceTensor f{};
+    if (t.data) {
+      if (t.dtype < HT_TENSOR_U8 || t.dtype > HT_TENSOR_F32)
+        return ctx->fail(HT_ERR_ARG, "record %d: dtype %d is not HT_TENSOR_U8 / F16 / BF16 / F32", i, t.dtype);
+      if (t.layout != HT_TENSOR_CHW && t.layout != HT_TENSOR_HWC)
+        return ctx->fail(HT_ERR_ARG, "record %d: layout %d is not HT_TENSOR_CHW / HWC", i, t.layout);
+      if (t.channels < HT_TENSOR_RGB || t.channels > HT_TENSOR_GRAY)
+        return ctx->fail(HT_ERR_ARG, "record %d: channels %d is not HT_TENSOR_RGB / BGR / GRAY", i, t.channels);
+      if (t.width < 1 || t.height < 1 || t.width > 2048 || t.height > 2048)
+        return ctx->fail(HT_ERR_SIZE, "record %d: face tensor %dx%d outside 1..2048", i, t.width, t.height);
+      const int es = t.dtype == HT_TENSOR_U8 ? 1 : t.dtype == HT_TENSOR_F32 ? 4 : 2;
+      if (reinterpret_cast<uintptr_t>(t.data) % (uintptr_t)es)
+        return ctx->fail(HT_ERR_ARG, "record %d: data is not aligned to its %d-byte elements", i, es);
+      if (!is_device_ptr(t.data)) return ctx->fail(HT_ERR_ARG, "record %d: data is not device memory", i);
+      const int C = t.channels == HT_TENSOR_GRAY ? 1 : 3;
+      const long long row = t.layout == HT_TENSOR_HWC ? (long long)C * t.width : t.width;
+      if (t.row_stride < row || t.row_stride > cap)
+        return ctx->fail(HT_ERR_ARG, "record %d: row_stride %lld outside [%lld, 2^40]", i, (long long)t.row_stride, row);
+      if (t.layout == HT_TENSOR_CHW && C == 3) {
+        const long long plane = (long long)(t.height - 1) * t.row_stride + t.width;
+        if (t.plane_stride < plane || t.plane_stride > cap)
+          return ctx->fail(HT_ERR_ARG, "record %d: plane_stride %lld outside [%lld, 2^40]", i, (long long)t.plane_stride, plane);
+      } else if (t.plane_stride != 0) {
+        return ctx->fail(HT_ERR_ARG, "record %d: plane_stride %lld must be 0 without three CHW planes", i, (long long)t.plane_stride);
+      }
+      if (t.pad_ != 0) return ctx->fail(HT_ERR_ARG, "record %d: pad_ is %d, not 0", i, t.pad_);
+      for (int k = 0; k < 3; ++k) {
+        if (!std::isfinite(t.mul[k]) || !std::isfinite(t.add[k]))
+          return ctx->fail(HT_ERR_ARG, "record %d: mul[%d] or add[%d] is not finite", i, k, k);
+        if (t.dtype == HT_TENSOR_U8 && k < C && (t.mul[k] != 1.0f || t.add[k] != 0.0f))
+          return ctx->fail(HT_ERR_ARG, "record %d: a U8 tensor takes mul 1 and add 0 (channel %d)", i, k);
+      }
+      if (!(t.scale > 0.0 && t.scale <= 16.0)) return ctx->fail(HT_ERR_ARG, "record %d: scale %g outside (0, 16]", i, t.scale);
+      f = tensor_record(t);
+    }
+    next[(size_t)(first + i)] = f;
+  }
+  const int clash = images_overlap(ctx->h_debug, ctx->h_crop, ctx->h_crop_planes, next, first, n, true);
+  if (clash != -1)
+    return ctx->fail(HT_ERR_ARG, "record %d: a face tensor overlaps itself, another stream's face tensor, a face crop or a debug canvas",
+                     clash - first);
+  { const int jr = join_aux(ctx); if (jr != HT_OK) return jr; }
+  CK(cudaSetDevice(ctx->cfg.device));
+  { const int tr = crop_tables(ctx); if (tr != HT_OK) return tr; }
+  CK(cudaMemcpyAsync(ctx->d_tensor.as<FaceTensor>() + first, next.data() + first, (size_t)n * sizeof(FaceTensor),
+                     cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));    // `next` is a local
+  ctx->tensor_count = ctx->tensor_tiles = 0;
+  for (const FaceTensor &f : next)
+    if (f.data) {
+      ++ctx->tensor_count;
+      ctx->tensor_tiles = std::max(ctx->tensor_tiles, ((f.w + CROP_TX - 1) / CROP_TX) * ((f.h + CROP_TY - 1) / CROP_TY));
+    }
+  ctx->h_tensor.swap(next);
+  return HT_OK;
 }
 
 static int view_record(const ht_video_view &view, int w, int h, ViewFeedRec &v, char *why);
@@ -2414,13 +2549,17 @@ static int tracker_tick(ht_ctx *ctx, const TickGroup *grp, int n_groups, const u
     k_debug_strokes<<<(unsigned)n, 256, 0, st>>>(d_ids, geo, d_ev, ctx->d_debug.as<DebugCanvas>());
     ++ctx->launches;
   }
-  if (ctx->crop_count > 0) {     // the face crops of the entries whose record is a kept "CS" face, from this tick's video
+  if (ctx->crop_count > 0 || ctx->tensor_count > 0) {   // the face crops and tensors of the entries whose record is a
+                                                         // kept "CS" face, from this tick's video
     CropSource src{CROP_FRAMES, g0.w, g0.h, 0, d_rgba};     // ht_tracker_step: the frames are the canvases
     if (feed && feed->view) src = CropSource{CROP_VIEW, 0, 0, 0, feed->view};
     else if (feed && feed->yuv) src = CropSource{CROP_YUV, 0, 0, 0, feed->yuv};
     else if (feed) src = CropSource{CROP_FEED, 0, 0, 0, feed->recs};
-    k_face_crop<<<dim3((unsigned)ctx->crop_tiles, (unsigned)n), 256, 0, st>>>(
-        d_ids, geo, g0.w, g0.h, d_ev, ctx->d_crop.as<FaceCrop>(), ctx->d_crop_planes.as<CropPlanes>(), src);
+    const int tz = ctx->crop_count > 0 ? 1 : 0;           // the tensor slice (unreached without tensors)
+    const unsigned slices = (unsigned)(tz + (ctx->tensor_count > 0 ? 1 : 0));
+    k_face_crop<<<dim3((unsigned)std::max(ctx->crop_tiles, ctx->tensor_tiles), (unsigned)n, slices), 256, 0, st>>>(
+        d_ids, geo, g0.w, g0.h, d_ev, ctx->d_crop.as<FaceCrop>(), ctx->d_crop_planes.as<CropPlanes>(),
+        ctx->d_tensor.as<FaceTensor>(), tz, src);
     ++ctx->launches;
   }
   ctx->prof_begin(HT_PROF_TRACK_INIT, st);
@@ -3561,6 +3700,37 @@ extern "C" int ht_selftest_face_crop_yuv(const ht_tracker_event *ev, int cw, int
       else nv12 ? crop_yuv_block<VIEW_FMT, true>(v, M, f, c, i, j) : crop_yuv_block<VIEW_FMT, false>(v, M, f, c, i, j);
     }
   return 1;
+}
+// k_face_crop's per-tensor code (the record is not checked): the face tensor of record `ev` on a cw x ch canvas drawn
+// from an image of any format (img, host planes) or an RGBA8 frame (rgba; exactly one of the two) through a view (NULL:
+// the whole frame upright), written into t->data (host memory) -> 1 if the record wrote the tensor, 0 if not
+extern "C" int ht_selftest_face_tensor(const ht_tracker_event *ev, int cw, int ch, const ht_yuv_image *img,
+                                       const ht_video_frame *rgba, const ht_video_view *view, const ht_face_tensor *tensor) {
+  YuvFeedRec r;
+  ViewFeedRec v;
+  char why[256];
+  const ht_video_view whole{};
+  const int w = img ? img->width : rgba->width, h = img ? img->height : rgba->height;
+  int rc = img ? yuv_record(*img, r, why) : HT_OK;
+  if (rc == HT_OK) rc = view_record(view ? *view : whole, w, h, v, why);
+  if (rc != HT_OK) return rc;
+  if (img) view_source_yuv(v, r);
+  else view_source_rgba(v, rgba->rgba, rgba->pitch ? rgba->pitch : 4 * w, w, h);
+  const FaceTensor t = tensor_record(*tensor);
+  const TrackerEvent &e = *reinterpret_cast<const TrackerEvent *>(ev);
+  long long M[6];
+  if (!crop_map(e.detection, e.x, e.y, e.width, e.height, e.angle, cw, ch, v.sw, v.sh, t.w, t.h, t.scale, M)) return 0;
+  for (int j = 0; j < t.h; ++j)
+    for (int i = 0; i < t.w; ++i)
+      tensor_put(t, v.kind == VIEW_RGBA ? crop_pixel<VIEW_RGBA>(v, M, i, j)
+                    : v.kind == VIEW_NV12_I420 ? crop_pixel<VIEW_NV12_I420>(v, M, i, j) : crop_pixel<VIEW_FMT>(v, M, i, j),
+                 i, j);
+  return 1;
+}
+// tensor_put over n RGBA8 pixels taken as row 0 of a tensor n pixels wide (the record's width is ignored)
+extern "C" void ht_selftest_tensor_pixels(const ht_face_tensor *tensor, const uint32_t *px, int n) {
+  const FaceTensor t = tensor_record(*tensor);
+  for (int i = 0; i < n; ++i) tensor_put(t, px[i], i, 0);
 }
 // rgba_to_yuv420 over n 2 x 2 blocks: blocks[4k..4k+3] = p00, p01, p10, p11 -> out[6k..6k+5] = their Y, U, V
 extern "C" void ht_selftest_rgba_to_yuv420(int color, const uint32_t *blocks, long long n, uint8_t *out) {

@@ -7,6 +7,8 @@
 // few window passes that stay in L2.
 #pragma once
 #include <cooperative_groups.h>
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
 
 #include <cstring>
 #include <limits>
@@ -1922,16 +1924,95 @@ __device__ __noinline__ void face_crop_yuv_tile(const ViewFeedRec *__restrict__ 
   if (X < f.w && Y < f.h) crop_yuv_block<KIND, NV12>(v, M, f, c, X, Y);
 }
 
-// After k_tracker_update: grid (tiles of the largest crop, batch entries).  Entry k's CTAs read its record
-// (events[geo[k].record], geo NULL: k) and canvas size (geo[k], geo NULL: cw x ch), and write the tiles of its stream's
-// crop on a crop tick; entries without a crop, without a crop tick, or past their own crop's tiles exit at once.  An
-// RGBA crop's tiles go to face_crop_tile, a YUV crop's (layout, then planes[id]) to face_crop_yuv_tile.
+// Face tensors (ht_tracker_set_face_tensor; DESIGN.md 2, "Face crops", item 6): a stream's face as a model's input, the
+// RGBA8 crop of the same size and scale converted per pixel, alpha ignored.  Layout of ht_face_tensor (strides in
+// elements); data NULL: the stream has none.
+struct FaceTensor {
+  void *data;
+  long long row, plane;
+  int32_t w, h, dtype, layout, channels, pad_;   // HT_TENSOR_*
+  float mul[3], add[3];
+  double scale;
+};
+
+// One channel value c of a face tensor as its element's bits: U8 c; F32 fmaf(c, mul, add), one rounding; F16 / BF16
+// that float rounded to nearest even (overflow: +-inf).
+__host__ __device__ __forceinline__ uint32_t tensor_value(int dtype, uint32_t c, float mul, float add) {
+  if (dtype == HT_TENSOR_U8) return c;
+#ifdef __CUDA_ARCH__
+  const float v = __fmaf_rn((float)c, mul, add);     // explicit: the build contracts nothing (-fmad=false)
+#else
+  const float v = fmaf((float)c, mul, add);
+#endif
+  if (dtype == HT_TENSOR_F16) return __half_raw(__float2half_rn(v)).x;
+  if (dtype == HT_TENSOR_BF16) return __nv_bfloat16_raw(__float2bfloat16_rn(v)).x;
+#ifdef __CUDA_ARCH__
+  return __float_as_uint(v);
+#else
+  uint32_t u;
+  memcpy(&u, &v, 4);
+  return u;
+#endif
+}
+
+// Pixel (i, j) of face tensor t from px, the pixel (i, j) of the RGBA8 crop of its size and scale: channel k of
+// HT_TENSOR_RGB is byte k of px, of HT_TENSOR_BGR byte 2 - k, and HT_TENSOR_GRAY's one channel is gray_of(px); each is
+// converted by tensor_value and stored at k plane + j row + i (CHW) or j row + i C + k (HWC).
+__host__ __device__ __forceinline__ void tensor_put(const FaceTensor &t, uint32_t px, int i, int j) {
+  const bool gray = t.channels == HT_TENSOR_GRAY, bgr = t.channels == HT_TENSOR_BGR, hwc = t.layout == HT_TENSOR_HWC;
+  const int C = gray ? 1 : 3;
+  const long long at = (long long)j * t.row + (hwc ? (long long)i * C : (long long)i), step = hwc ? 1 : t.plane;
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    if (k >= C) break;
+    const uint32_t c = gray ? gray_of(px) : byte_of(px, bgr ? 2 - k : k);
+    const uint32_t bits = tensor_value(t.dtype, c, t.mul[k], t.add[k]);
+    const long long e = at + k * step;
+    if (t.dtype == HT_TENSOR_U8) static_cast<uint8_t *>(t.data)[e] = (uint8_t)bits;
+    else if (t.dtype == HT_TENSOR_F32) static_cast<uint32_t *>(t.data)[e] = bits;
+    else static_cast<uint16_t *>(t.data)[e] = (uint16_t)bits;
+  }
+}
+
+// One 64 x 16 tile from (X0, Y0) of face tensor *tp: a warp converts 32 consecutive pixels of one row, so each plane's
+// stores (CHW) or the row's interleaved ones (HWC) are consecutive elements.  Out of line per texel source; dtype,
+// layout and channel order are warp-uniform runtime branches.  The view record and the map stay in k_face_crop's shared
+// memory and the tensor record in global memory, as face_crop_yuv_tile keeps them, so k_face_crop stays at 64
+// registers.
+template <int KIND>
+__device__ __noinline__ void face_tensor_tile(const ViewFeedRec *__restrict__ vp, const long long *__restrict__ Mp,
+                                              const FaceTensor *__restrict__ tp, int X0, int Y0) {
+  const ViewFeedRec &v = *vp;
+  const FaceTensor &t = *tp;
+  const int X = X0 + (threadIdx.x & 63);
+  if (X >= t.w) return;
+#pragma unroll 1
+  for (int r = 0; r < 4; ++r) {
+    const int Y = Y0 + 4 * r + (threadIdx.x >> 6);
+    if (Y < t.h) tensor_put(t, crop_pixel<KIND>(v, Mp, X, Y), X, Y);
+  }
+}
+
+// After k_tracker_update: grid (tiles of the largest crop or tensor, batch entries, slices).  Slice tz is the face
+// tensors' (tz = 1 while some stream has a crop, else 0; a grid without a tensor slice never reaches it), the other one
+// the crops'.  Entry k's CTAs read its record (events[geo[k].record], geo NULL: k) and canvas size (geo[k], geo NULL:
+// cw x ch), and write the tiles of its stream's crop or tensor on a crop tick; entries without one, without a crop tick,
+// or past their own tiles exit at once.  An RGBA crop's tiles go to face_crop_tile, a YUV crop's (layout, then
+// planes[id]) to face_crop_yuv_tile, a tensor's to face_tensor_tile.
 __global__ void __launch_bounds__(256) k_face_crop(const int32_t *__restrict__ ids, const EntryCanvas *__restrict__ geo,
                                                    int cw, int ch, const TrackerEvent *__restrict__ events,
                                                    const FaceCrop *__restrict__ crops,
-                                                   const CropPlanes *__restrict__ planes, CropSource src) {
+                                                   const CropPlanes *__restrict__ planes,
+                                                   const FaceTensor *__restrict__ tensors, int tz, CropSource src) {
   const int k = blockIdx.y, id = ids ? ids[k] : k;
-  const FaceCrop f = crops[id];
+  const bool tensor = (int)blockIdx.z == tz;
+  FaceCrop f;
+  if (tensor) {                        // only the geometry: the body reads the rest of the record
+    const FaceTensor &t = tensors[id];
+    f = FaceCrop{static_cast<uint8_t *>(t.data), t.w, t.h, 0, 0, t.scale};
+  } else {
+    f = crops[id];
+  }
   if (!f.rgba) return;
   const int tiles_x = (f.w + CROP_TX - 1) / CROP_TX;
   if ((int)blockIdx.x >= tiles_x * ((f.h + CROP_TY - 1) / CROP_TY)) return;
@@ -1947,6 +2028,12 @@ __global__ void __launch_bounds__(256) k_face_crop(const int32_t *__restrict__ i
   __syncthreads();
   if (!on) return;
   const int X0 = ((int)blockIdx.x % tiles_x) * CROP_TX, Y0 = ((int)blockIdx.x / tiles_x) * CROP_TY;
+  if (tensor) {
+    if (v.kind == VIEW_RGBA) face_tensor_tile<VIEW_RGBA>(&v, M, tensors + id, X0, Y0);
+    else if (v.kind == VIEW_NV12_I420) face_tensor_tile<VIEW_NV12_I420>(&v, M, tensors + id, X0, Y0);
+    else face_tensor_tile<VIEW_FMT>(&v, M, tensors + id, X0, Y0);
+    return;
+  }
   if (f.layout == CROP_RGBA) {
     if (v.kind == VIEW_RGBA) face_crop_tile<VIEW_RGBA>(&v, M, f, X0, Y0);
     else if (v.kind == VIEW_NV12_I420) face_crop_tile<VIEW_NV12_I420>(&v, M, f, X0, Y0);

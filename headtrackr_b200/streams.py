@@ -10,6 +10,8 @@ for records with detection == "CS" (src/facetrackr.js:112-125).
 import math
 import time
 
+import numpy as np
+
 from . import _lib
 from .context import tracker_events_from_bytes
 
@@ -87,6 +89,30 @@ def lifecycle_events(rec, status):
     return out, status
 
 
+def face_written(records):
+    """Which slots a tick refreshed in its face crops and tensors: the bool mask detection == "CS" (2) and width > 0 and
+    height > 0, per record.  records: the tick's record dicts (Context.tracker_step / tracker_feed; None: not ticked),
+    raw ht_tracker_event bytes (host), or a torch CUDA uint8 buffer of device records (the `out` of a tick) - then the
+    mask is a torch CUDA bool tensor, computed by torch ops on torch's current stream without a host sync.  The library
+    writes `out` on the context's stream, so those ops read the tick's records only if they are ordered after it: create
+    the Context with stream= torch's current stream (then the tick, this mask and a model reading the face tensors run
+    in order on one stream), or call Context.sync() (or wait on an event recorded on the context's stream) first."""
+    if hasattr(records, "is_cuda"):
+        import torch
+        b = records.reshape(-1)
+        det = b.view(torch.int32).reshape(-1, 36)[:, 0]          # detection at byte 0
+        wh = b.view(torch.float64).reshape(-1, 18)                 # width at byte 24, height at 32
+        return (det == 2) & (wh[:, 3] > 0) & (wh[:, 4] > 0)
+    if isinstance(records, (bytes, bytearray, memoryview)) or hasattr(records, "dtype"):
+        raw = np.frombuffer(bytes(records) if not hasattr(records, "dtype") else np.ascontiguousarray(records).tobytes(),
+                            np.uint8).reshape(-1, 144)
+        det = raw[:, 0:4].copy().view(np.int32)[:, 0]
+        wh = raw[:, 24:40].copy().view(np.float64)
+        return (det == 2) & (wh[:, 0] > 0) & (wh[:, 1] > 0)
+    return np.array([r is not None and r["detection"] == "CS" and r["width"] > 0 and r["height"] > 0 for r in records],
+                    dtype=bool)
+
+
 def _to_int32(v):
     """JavaScript's `v >> 0` (ToInt32)"""
     if not math.isfinite(v):
@@ -139,7 +165,8 @@ class TrackerSet:
     its `out` tensor on every tick with a headtrackingEvent).  A stream's "faceCrop" key is its face crop, a dict as
     Context.tracker_set_face_crop takes: the tracked face cut upright out of the video into its `out` tensor (or, with
     "format": "nv12" / "i420" and a "color", its NV12 / I420 planes for a video encoder) on every tick that keeps the
-    face.
+    face.  A stream's "faceTensor" key is its face tensor, a dict as Context.tracker_set_face_tensor takes: the same
+    face as a model's normalised input, independent of "faceCrop".
     Differs from the reference in one place: start() on a running stream does nothing (the reference runs an extra,
     unscheduled pass)."""
 
@@ -171,6 +198,9 @@ class TrackerSet:
         crops = [(p or {}).get("faceCrop") for p in (params if per_stream else [params] * n_streams)]
         if any(c is not None for c in crops):      # and face crops
             context.tracker_set_face_crop(0, crops)
+        tensors = [(p or {}).get("faceTensor") for p in (params if per_stream else [params] * n_streams)]
+        if any(t is not None for t in tensors):    # and face tensors
+            context.tracker_set_face_tensor(0, tensors)
 
     def set_params(self, k, params):
         """The parameters of stream k (a dict as for the constructor).  Its state is kept: calcAngles takes effect at
@@ -182,6 +212,7 @@ class TrackerSet:
         self.ctx.tracker_set_debug_strokes(k, [bool((params or {}).get("debugStrokes"))])   # no key: off
         self.ctx.tracker_set_camera(k, [(params or {}).get("camera")])  # no "camera" key: none
         self.ctx.tracker_set_face_crop(k, [(params or {}).get("faceCrop")])   # no "faceCrop" key: none
+        self.ctx.tracker_set_face_tensor(k, [(params or {}).get("faceTensor")])   # no "faceTensor" key: none
 
     def addEventListener(self, fn):
         """fn(stream_index, evt): evt is a headtrackrStatus / facetrackingEvent / headtrackingEvent payload dict."""

@@ -542,6 +542,56 @@ typedef struct {
  * plane of the crop, another stream's crop of either layout or any debug canvas (over all streams after the call). */
 int ht_tracker_set_face_crop_yuv(ht_ctx *ctx, int first, int n, const ht_face_crop_yuv *crops);
 
+/* A stream's face tensor: its face as a model's input, a normalised CHW or HWC tensor (DESIGN.md 2, "Face crops", item
+ * 6).  It is a second output of the stream, next to and independent of its face crop.  It is, bit for bit, the RGBA8
+ * crop of the same size and scale (ht_face_crop) with alpha ignored, converted per pixel P(i, j) = (R, G, B):
+ *   channels  HT_TENSOR_RGB: c = R, G, B; HT_TENSOR_BGR: c = B, G, R; HT_TENSOR_GRAY: one channel,
+ *             c = the detector's gray, ccv.grayscale: R 0.3 + G 0.59 + B 0.11 in fp64, left to right, stored
+ *             round-half-even as a Uint8ClampedArray stores it
+ *   value     HT_TENSOR_F32: v = fmaf((float)c, mul[k], add[k]), one rounding; HT_TENSOR_F16 / HT_TENSOR_BF16: that v
+ *             rounded to nearest even (overflow gives +-inf); HT_TENSOR_U8: c itself (mul 1, add 0)
+ *   layout    element (k, j, i) at data + k plane_stride + j row_stride + i (HT_TENSOR_CHW) or
+ *             data + j row_stride + i C + k (HT_TENSOR_HWC), strides in elements; no other element is written
+ * A pixel outside the video converts from (0, 0, 0): value add[k].  For a torchvision-style (x / 255 - mean) / std,
+ * mul = 1 / (255 std) and add = -mean / std, each rounded once to float. */
+#define HT_TENSOR_U8 0
+#define HT_TENSOR_F16 1
+#define HT_TENSOR_BF16 2
+#define HT_TENSOR_F32 3
+#define HT_TENSOR_CHW 0
+#define HT_TENSOR_HWC 1
+#define HT_TENSOR_RGB 0
+#define HT_TENSOR_BGR 1
+#define HT_TENSOR_GRAY 2
+typedef struct {
+  void *data;             /*  0 DEVICE memory of the context's device, aligned to the element size; NULL: none */
+  int64_t row_stride;     /*  8 elements; CHW >= S_w, HWC >= C*S_w; at most 2^40 */
+  int64_t plane_stride;   /* 16 elements; CHW with 3 channels: >= (S_h-1)*row_stride + S_w, at most 2^40; otherwise 0 */
+  int32_t width, height;  /* 24 S_w x S_h, 1..2048 */
+  int32_t dtype;          /* 32 HT_TENSOR_U8 / F16 / BF16 / F32 */
+  int32_t layout;         /* 36 HT_TENSOR_CHW / HWC */
+  int32_t channels;       /* 40 HT_TENSOR_RGB / BGR / GRAY */
+  int32_t pad_;           /* 44 0 */
+  float mul[3], add[3];   /* 48, 60 finite; GRAY uses [0]; U8: 1 and 0 */
+  double scale;           /* 72 as ht_face_crop's, (0, 16] */
+} ht_face_tensor;         /* 80 bytes */
+/* Stream first+i gets the face tensor tensors[i] (host array), for i in [0, n); a NULL data removes the stream's.  A
+ * stream has at most one tensor, and it is independent of the stream's face crop: ht_tracker_set_face_crop(_yuv) never
+ * touch it, and this call never touches the crop.  It is written on exactly the ticks, and lives exactly as long, as a
+ * crop: after every "CS" tick with width > 0 and height > 0, every element above is written; every other tick leaves
+ * it as it was.  ht_face_crop_map gives its map (that of the RGBA crop of its size and scale).  The tensor belongs to
+ * the stream id: stop, start, reset, a lost face, ht_tracker_set_params and ht_tracker_import keep it;
+ * ht_tracker_config removes every stream's.  A tick with crops, tensors or both launches one kernel more, and nothing
+ * more otherwise.  The tracker record format is unchanged.
+ * Errors (nothing changes; the message names the record): HT_ERR_STATE before ht_tracker_config; HT_ERR_SIZE for a size
+ * outside 1..2048; HT_ERR_ARG for a range outside [0, max_frames), n <= 0, tensors NULL, a dtype, layout or channels
+ * value other than the above, a host pointer, a pointer not aligned to the element size, a stride outside its range
+ * above, a non-zero pad_, a mul or add that is not finite, a U8 tensor whose used mul is not 1 or add not 0, a scale
+ * that is not finite or outside (0, 16], or a tensor whose bytes - one span per channel plane for CHW, one span for HWC
+ * - overlap one another, another stream's tensor, any plane of any face crop or any debug canvas (over all streams
+ * after the call).  ht_tracker_set_debug and both crop setters likewise refuse overlap with a tensor. */
+int ht_tracker_set_face_tensor(ht_ctx *ctx, int first, int n, const ht_face_tensor *tensors);
+
 /* The map of the crop `crop` (its size and scale; rgba and pitch are ignored; a YUV crop has the map of the RGBA crop of
  * its size and scale) for tracker record `ev`, on a canvas of
  * canvas_w x canvas_h drawn from a video_w x video_h video through `view` (NULL: the whole frame upright; for

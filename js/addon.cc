@@ -29,6 +29,8 @@
 //        memory)
 //   trackerSetFaceCropYuv(handle, first, [crop|null, ...])  (ht_tracker_set_face_crop_yuv: each stream's NV12 / I420
 //        face crop, device planes)
+//   trackerSetFaceTensor(handle, first, [tensor|null, ...])  (ht_tracker_set_face_tensor: each stream's normalised
+//        face tensor for a model, device memory)
 //   trackerSetCamera(handle, first, [control|null, ...])  (ht_tracker_set_camera: each stream's head-coupled camera,
 //        realisticAbsoluteCameraControl on an ht_camera in device memory)
 //   trackerExport(handle, [stream, ...]) -> Buffer of records; trackerImport(handle, [stream, ...], records)
@@ -46,6 +48,7 @@
 
 #include <cstdint>
 #include <cstring>
+#include <initializer_list>
 #include <vector>
 
 #include "../include/headtrackr_b200.h"
@@ -583,6 +586,65 @@ static void GetVec3(napi_env env, napi_value obj, const char *name, double out[3
     if (napi_get_element(env, v, i, &e) == napi_ok) napi_get_value_double(env, e, &out[i]);
 }
 
+// trackerSetFaceTensor(handle, first, [{data: BigInt device address, rowStride, planeStride?, width, height,
+// dtype: "u8" | "f16" | "bf16" | "f32", layout: "chw" | "hwc", channels: "rgb" | "bgr" | "gray", mul: [3], add: [3],
+// scale?}, null, ...]): stream first+i gets tensors[i] (strides in elements; mul defaults to 1, add to 0, scale to 1);
+// null or undefined: none
+static napi_value TrackerSetFaceTensor(napi_env env, napi_callback_info info) {
+  size_t argc = 3;
+  napi_value argv[3];
+  NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+  ht_ctx *ctx = Ctx(env, argv[0]);
+  int32_t first = 0;
+  uint32_t n = 0;
+  napi_get_value_int32(env, argv[1], &first);
+  NAPI_OK(napi_get_array_length(env, argv[2], &n));
+  std::vector<ht_face_tensor> ts(n, ht_face_tensor{});
+  auto pick = [&](napi_value r, const char *name, std::initializer_list<const char *> names, int32_t dflt) {
+    napi_value v;
+    char s[16] = {0};
+    size_t sl = 0;
+    if (napi_get_named_property(env, r, name, &v) == napi_ok) napi_get_value_string_utf8(env, v, s, sizeof s, &sl);
+    if (sl == 0) return dflt;
+    int32_t code = 0;
+    for (const char *nm : names) {
+      if (strcmp(s, nm) == 0) return code;
+      ++code;
+    }
+    return (int32_t)-1;                     // the library rejects it
+  };
+  for (uint32_t i = 0; i < n; ++i) {
+    napi_value r, v;
+    napi_valuetype t = napi_undefined;
+    NAPI_OK(napi_get_element(env, argv[2], i, &r));
+    napi_typeof(env, r, &t);
+    if (t != napi_object) continue;
+    ht_face_tensor &f = ts[i];
+    uint64_t addr = 0;
+    bool lossless = false;
+    if (napi_get_named_property(env, r, "data", &v) == napi_ok) napi_get_value_bigint_uint64(env, v, &addr, &lossless);
+    f.data = reinterpret_cast<void *>(static_cast<uintptr_t>(addr));
+    f.row_stride = (int64_t)GetNumber(env, r, "rowStride", 0.0);
+    f.plane_stride = (int64_t)GetNumber(env, r, "planeStride", 0.0);
+    if (napi_get_named_property(env, r, "width", &v) == napi_ok) napi_get_value_int32(env, v, &f.width);
+    if (napi_get_named_property(env, r, "height", &v) == napi_ok) napi_get_value_int32(env, v, &f.height);
+    f.dtype = pick(r, "dtype", {"u8", "f16", "bf16", "f32"}, HT_TENSOR_F16);
+    f.layout = pick(r, "layout", {"chw", "hwc"}, HT_TENSOR_CHW);
+    f.channels = pick(r, "channels", {"rgb", "bgr", "gray"}, HT_TENSOR_RGB);
+    double mul[3], add[3];
+    GetVec3(env, r, "mul", mul);
+    GetVec3(env, r, "add", add);
+    napi_value mv;
+    const bool has_mul = napi_get_named_property(env, r, "mul", &mv) == napi_ok && napi_typeof(env, mv, &t) == napi_ok &&
+                         t == napi_object;
+    for (int k = 0; k < 3; ++k) f.mul[k] = has_mul ? (float)mul[k] : 1.0f, f.add[k] = (float)add[k];
+    f.scale = GetNumber(env, r, "scale", 1.0);
+  }
+  int rc = ht_tracker_set_face_tensor(ctx, first, (int)n, ts.data());
+  if (rc < 0) return Throw(env, ctx, rc);
+  return nullptr;
+}
+
 // trackerSetCamera(handle, first, [{camera: BigInt device address, scaling, fixedPosition: [x, y, z], lookAt: [x, y, z],
 // screenHeight?, damping?, fov, aspect, near, far}, null, ...]): stream first+i gets controls[i]; null or undefined:
 // none.  screenHeight and damping default to the reference's 20 and 1 (src/controllers.js:31-38).
@@ -980,6 +1042,7 @@ static napi_value Init(napi_env env, napi_value exports) {
       {"trackerSetDebugStrokes", nullptr, TrackerSetDebugStrokes, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerSetFaceCrop", nullptr, TrackerSetFaceCrop, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerSetFaceCropYuv", nullptr, TrackerSetFaceCropYuv, nullptr, nullptr, nullptr, napi_default, nullptr},
+      {"trackerSetFaceTensor", nullptr, TrackerSetFaceTensor, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerSetCamera", nullptr, TrackerSetCamera, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerExport", nullptr, TrackerExport, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerImport", nullptr, TrackerImport, nullptr, nullptr, nullptr, napi_default, nullptr},

@@ -713,10 +713,16 @@ def crops_arms(torch, stream, N, steps, rounds, before_lib=None):
       rgbaconv<S>_cs        what a caller who encodes crops does without YUV crops: the crop<S>all tick, then the
                             same BT.601 conversion to NV12 written in torch (integer ops on the device)
       crop<S>all_before_cs  crop<S>all_cs with the library at `before_lib`
+      tensor<S>_cs          an S x S fp16 CHW RGB face tensor on every stream, normalised with ImageNet's mean / std
+                            (ht_tracker_set_face_tensor through Context.face_tensor_batch), no crop
+      tensornv12<S>_cs      that tensor and an S x S NV12 crop on every stream (one k_face_crop, two grid slices)
+      rgbanorm<S>_cs        what a caller who feeds a model does without tensors: the crop<S>all tick, then
+                            crop[..., :3].permute(0, 3, 1, 2).float().div(255).sub(mean).div(std).half() into a batch
 
     Then, in runs of their own under torch.profiler, k_face_crop's kernel time per tick in the crop<S>all,
-    crop<S>nv12 / crop<S>i420 and crop<S>all_before arms.  The records of every arm must agree on every timed tick, and every YUV crop must
-    equal the torch conversion of the RGBA crop of its stream."""
+    crop<S>nv12 / crop<S>i420, tensor<S>, tensornv12<S> and crop<S>all_before arms.  The records of every arm must
+    agree on every timed tick, every YUV crop must equal the torch conversion of the RGBA crop of its stream, and the
+    largest difference between the tensors and the torch normalise pass is reported."""
     import ctypes as C
     import torch.nn.functional as F
     from headtrackr_b200 import Context, _lib
@@ -740,18 +746,24 @@ def crops_arms(torch, stream, N, steps, rounds, before_lib=None):
             return torch.zeros((N, h, w), dtype=torch.uint8, device="cuda")
         return (z(S, S), z(S // 2, S)) if fmt == "nv12" else (z(S, S), z(S // 2, S // 2), z(S // 2, S // 2))
     yuv = {(S, fmt): planes(S, fmt) for S in (112, 224) for fmt in ("nv12", "i420")}
-    twopass_out, conv_out = {}, {}
+    twopass_out, conv_out, norm_out, tens = {}, {}, {}, {}
+    mean, std = (0.485, 0.456, 0.406), (0.229, 0.224, 0.225)
+    mean_t = torch.tensor(mean, device="cuda").view(1, 3, 1, 1)
+    std_t = torch.tensor(std, device="cuda").view(1, 3, 1, 1)
 
     def arm(kind, S=0, every=0):
         c = other_build_context(before_lib, **kw) if kind == "before" else Context(**kw)
         c.tracker_config()
         c.tracker_reset(0, N)
         c.tracker_start(0, N)
-        if kind in ("nv12", "i420"):
-            c.tracker_set_face_crop(0, [{"out": tuple(p[k] for p in yuv[(S, kind)]), "format": kind, "color": "bt601"}
+        if kind in ("nv12", "i420", "tensornv12"):
+            fmt = "nv12" if kind == "tensornv12" else kind
+            c.tracker_set_face_crop(0, [{"out": tuple(p[k] for p in yuv[(S, fmt)]), "format": fmt, "color": "bt601"}
                                         for k in range(N)])
         elif every:
             c.tracker_set_face_crop(0, [{"out": crops[S][k]} if k % every == 0 else None for k in range(N)])
+        if kind in ("tensor", "tensornv12"):
+            tens[(S, kind)] = c.face_tensor_batch(0, N, S, S, torch.float16, "chw", "rgb", mean, std)
         out = torch.empty(N * rec_bytes, dtype=torch.uint8, device="cuda")
 
         def run():
@@ -766,6 +778,8 @@ def crops_arms(torch, stream, N, steps, rounds, before_lib=None):
                 twopass_out[S] = F.grid_sample(src, grid, mode="bilinear", padding_mode="zeros", align_corners=False)
             if kind == "rgbaconv":
                 conv_out[S] = torch_nv12(torch, crops[S])
+            if kind == "rgbanorm":
+                norm_out[S] = crops[S][..., :3].permute(0, 3, 1, 2).float().div(255).sub(mean_t).div(std_t).half()
         return c, run, out
 
     arms = {"crop0_cs": arm("plain"), "crop112all_cs": arm("crop", 112, 1), "crop11264_cs": arm("crop", 112, 64),
@@ -774,6 +788,8 @@ def crops_arms(torch, stream, N, steps, rounds, before_lib=None):
     for S in (112, 224):
         arms[f"crop{S}nv12_cs"], arms[f"crop{S}i420_cs"] = arm("nv12", S), arm("i420", S)
         arms[f"rgbaconv{S}_cs"] = arm("rgbaconv", S, 1)
+        arms[f"tensor{S}_cs"], arms[f"tensornv12{S}_cs"] = arm("tensor", S), arm("tensornv12", S)
+        arms[f"rgbanorm{S}_cs"] = arm("rgbanorm", S, 1)
     if before_lib:
         arms["crop0_before_cs"] = arm("before")
         for S in (112, 224):
@@ -825,14 +841,20 @@ def crops_arms(torch, stream, N, steps, rounds, before_lib=None):
             torch.equal(y[m], want[0][m]) and torch.equal(uv[m], want[1][m]) and torch.equal(y4[m], want[0][m]) and
             torch.equal(u4[m], want[1][..., 0::2][m]) and torch.equal(v4[m], want[1][..., 1::2][m]) and
             torch.equal(conv_out[S][0], want[0]) and torch.equal(conv_out[S][1], want[1]))
+        # the tensors against the torch normalise pass of the RGBA crops (one fmaf against two-step fp32, then fp16)
+        res[f"tensor{S}_vs_torch_norm_max_abs_diff"] = max(
+            float((tens[(S, kind)][m].float() - norm_out[S][m].float()).abs().max()) for kind in ("tensor", "tensornv12"))
+        res[f"tensor{S}_equals_tensornv12"] = bool(torch.equal(tens[(S, "tensor")][m], tens[(S, "tensornv12")][m]))
 
     from torch.profiler import ProfilerActivity, profile
     for S in (112, 224):
-        for layout, bpp in (("all", 4), ("nv12", 1.5), ("i420", 1.5)) + ((("all_before", 4),) if before_lib else ()):
+        for layout, bpp in (("all", 4), ("nv12", 1.5), ("i420", 1.5), ("tensor", 6), ("tensornv12", 7.5)) + \
+                ((("all_before", 4),) if before_lib else ()):
+            arm_name = f"{layout}{S}_cs" if layout.startswith("tensor") else f"crop{S}{layout}_cs"
             with profile(activities=[ProfilerActivity.CUDA]) as prof:
                 for _ in range(steps):
                     now[0] += 20.0
-                    arms[f"crop{S}{layout}_cs"][1]()
+                    arms[arm_name][1]()
                 torch.cuda.synchronize()
             us = 0.0
             for e in prof.key_averages():
