@@ -295,10 +295,7 @@ class Context:
         self.max_frames = max_frames
         self.max_width, self.max_height, self.device = max_width, max_height, device
         self.last_warning = None
-        self._debug = {}                  # stream -> its debug canvas tensor, kept alive while the library writes it
-        self._camera = {}                 # stream -> its camera tensor, likewise
-        self._crops = {}                  # stream -> its face crop dict (and so its tensors), likewise
-        self._tensors = {}                # stream -> its face tensor dict, likewise
+        self._outputs = {}                # (kind, stream) -> what the library writes for that output, kept alive while set
 
     def close(self):
         if getattr(self, "_h", None) and self._h.value:
@@ -468,20 +465,18 @@ class Context:
                        headPosition=True, edgecorrection=True, alpha=0.35, distance_to_screen=60.0, enable=True):
         """Switch the per-stream headtrackr.Tracker lifecycle on with the reference's parameters (src/main.js:39-55),
         or off (enable=False: every stream goes back to stream_reset's state)."""
-        if not enable:
-            self._check(self._L.ht_tracker_config(self._h, None))
-            self._debug = {}
-            self._camera = {}
-            self._crops = {}
-            self._tensors = {}
-            return
         p = tracker_params(retryDetection, calcAngles, smoothing, fov, cameraOffset, headPosition, edgecorrection, alpha,
-                           distance_to_screen)
-        self._check(self._L.ht_tracker_config(self._h, C.addressof(p)))
-        self._debug = {}                  # ht_tracker_config discards every debug canvas
-        self._camera = {}                 # and every camera controller
-        self._crops = {}                  # and every face crop
-        self._tensors = {}                # and every face tensor
+                           distance_to_screen) if enable else None
+        self._check(self._L.ht_tracker_config(self._h, None if p is None else C.addressof(p)))
+        self._outputs = {}                # ht_tracker_config discards every stream's outputs
+
+    def _keep(self, kind, first, items):
+        """keeps items[i] (None: nothing) alive as stream first+i's `kind` output, after the library accepted them"""
+        for i, v in enumerate(items):
+            if v is None:
+                self._outputs.pop((kind, first + i), None)
+            else:
+                self._outputs[(kind, first + i)] = v
 
     def tracker_set_params(self, first, params):
         """Parameters of streams first, first+1, ...: one dict of tracker_config's keywords (enable excluded) per stream,
@@ -507,11 +502,7 @@ class Context:
                 raise ValueError("debug canvases must be uint8 (Dh, Dw, 4) with strides (pitch, 4, 1)")
             arr[i] = DebugCanvas(t.data_ptr(), t.shape[1], t.shape[0], t.stride(0), 0)
         self._check(self._L.ht_tracker_set_debug(self._h, int(first), len(canvases), C.addressof(arr)))
-        for i, t in enumerate(canvases):
-            if t is None:
-                self._debug.pop(int(first) + i, None)
-            else:
-                self._debug[int(first) + i] = t
+        self._keep("debug", int(first), canvases)
 
     def tracker_set_debug_strokes(self, first, flags):
         """Whether streams first, first+1, ... stroke main.js's face rectangles onto their debug canvases
@@ -540,7 +531,7 @@ class Context:
         back, so a rejected call changes nothing."""
         first, crops = int(first), list(crops)
         recs = [_face_crop_record(c) for c in crops]
-        prev = [self._crops.get(first + i) for i in range(len(crops))]
+        prev = [self._outputs.get(("crop", first + i)) for i in range(len(crops))]
         done = 0
         try:
             for a, b in _crop_runs(recs) or [(0, 0)]:   # no crops at all: the library's rejection of n = 0
@@ -551,11 +542,7 @@ class Context:
             for a, b in _crop_runs(back):             # the state before the call, which the library accepted
                 self._set_crop_run(first + a, back[a:b])
             raise
-        for i, c in enumerate(crops):
-            if c is None:
-                self._crops.pop(first + i, None)
-            else:
-                self._crops[first + i] = c
+        self._keep("crop", first, crops)
 
     def _set_crop_run(self, first, recs):
         """one setter call over records of one layout (None: no crop) from _face_crop_record"""
@@ -582,11 +569,7 @@ class Context:
         recs = [_face_tensor_record(t) for t in tensors]
         arr = (FaceTensor * max(1, len(recs)))(*[r if r is not None else FaceTensor() for r in recs])
         self._check(self._L.ht_tracker_set_face_tensor(self._h, first, len(recs), C.addressof(arr)))
-        for i, t in enumerate(tensors):
-            if t is None:
-                self._tensors.pop(first + i, None)
-            else:
-                self._tensors[first + i] = t
+        self._keep("tensor", first, tensors)
 
     def face_tensor_batch(self, first, n, height, width, dtype=None, layout="chw", channels="rgb", mean=None, std=None,
                           scale=1.0):
@@ -637,11 +620,7 @@ class Context:
                                    float(d.get("damping", 1.0)), float(d["fov"]), float(d["aspect"]),
                                    float(d["near"]), float(d["far"]))
         self._check(self._L.ht_tracker_set_camera(self._h, int(first), len(controls), C.addressof(arr)))
-        for i, d in enumerate(controls):
-            if d is None:
-                self._camera.pop(int(first) + i, None)
-            else:
-                self._camera[int(first) + i] = d["out"]
+        self._keep("camera", int(first), [None if d is None else d["out"] for d in controls])
 
     def tracker_export(self, streams, out=None):
         """The tracker records of the listed streams (ht_tracker_export): a (len(streams), TRACKER_RECORD_BYTES) uint8

@@ -75,6 +75,39 @@ struct DevBuf {
   template <class T> T *as() const { return reinterpret_cast<T *>(p); }
 };
 
+// One record per stream that a tick reads (a debug canvas, a camera, a face crop, ...): the device table and its host
+// mirror.  Every record is 0 (none) until a setter puts one; an empty mirror is all 0.
+template <class T>
+struct StreamTable {
+  DevBuf d;
+  std::vector<T> h;
+  T *dev() const { return d.as<T>(); }
+  // every stream's current record, for a setter to edit
+  std::vector<T> edit(int max_frames) const {
+    std::vector<T> next = h;
+    next.resize((size_t)max_frames, T{});
+    return next;
+  }
+  // the device table, all 0, on first use
+  cudaError_t reserve(size_t max_frames, cudaStream_t st) {
+    if (d.p) return cudaSuccess;
+    const cudaError_t e = d.reserve(max_frames * sizeof(T));
+    return e != cudaSuccess ? e : cudaMemsetAsync(d.p, 0, max_frames * sizeof(T), st);
+  }
+  // records [first, first + n) of `next` (edit's table, checked) to the device on `st`; the caller synchronises `st`
+  // before `next` goes and then makes it the mirror
+  cudaError_t commit(const std::vector<T> &next, int first, int n, cudaStream_t st) {
+    const cudaError_t e = reserve(next.size(), st);
+    return e != cudaSuccess ? e : cudaMemcpyAsync(dev() + first, next.data() + first, (size_t)n * sizeof(T),
+                                                  cudaMemcpyHostToDevice, st);
+  }
+  // every record 0
+  cudaError_t clear(cudaStream_t st) {
+    h.clear();
+    return d.p ? cudaMemsetAsync(d.p, 0, d.cap, st) : cudaSuccess;
+  }
+};
+
 // ------------------------------------------------------------------------------------------------
 // Plan: everything that depends only on (w, h, interval) — src/ccv.js:110-160
 struct Plan {
@@ -569,30 +602,20 @@ struct ht_ctx {
   // ht_tracker_config: per stream its state, its TrackerParams (ht_tracker_set_params), its event, its whitebalance flag
   DevBuf d_tracker_state, d_tracker_params, d_tracker_events, d_tracker_wb;
   bool tracker_on = false;
-  // ht_tracker_set_debug: per stream its DebugCanvas (device array and host copy), the number of streams that have
-  // one (0: a tick launches nothing for debug), and the value tables of a tick's entries [max_frames][DBG_TAB]
-  DevBuf d_debug, d_debug_tab;
-  std::vector<DebugCanvas> h_debug;
-  int debug_count = 0;
-  // ht_tracker_set_debug_strokes: the streams whose flag is on, and those of them that have a canvas (0: a tick
-  // launches no k_debug_strokes)
-  int stroke_flags = 0, stroke_count = 0;
-  // ht_tracker_set_camera: per stream its CameraCtl (device array and host copy) and the number of streams that have
-  // one (0: a tick launches nothing for cameras)
-  DevBuf d_camera;
-  std::vector<CameraCtl> h_camera;
-  int camera_count = 0;
-  // ht_tracker_set_face_crop(_yuv): per stream its FaceCrop and CropPlanes (device arrays and host copies), the number
-  // of streams that have one (0: a tick launches no k_face_crop) and the tiles of the largest (k_face_crop's grid.x)
-  DevBuf d_crop, d_crop_planes;
-  std::vector<FaceCrop> h_crop;
-  std::vector<CropPlanes> h_crop_planes;
-  int crop_count = 0, crop_tiles = 0;
-  // ht_tracker_set_face_tensor: per stream its FaceTensor (device array and host copy), the number of streams that have
-  // one (0: k_face_crop has no tensor slice) and the tiles of the largest
-  DevBuf d_tensor;
-  std::vector<FaceTensor> h_tensor;
-  int tensor_count = 0, tensor_tiles = 0;
+  // The per-stream outputs of a tick: ht_tracker_set_debug(_strokes), _set_camera, _set_face_crop(_yuv) (a FaceCrop
+  // and its CropPlanes) and _set_face_tensor.  The crop, plane and tensor tables are allocated together: k_face_crop's
+  // tensor slice reads the crop table.  d_debug_tab holds the value tables of a tick's entries [max_frames][DBG_TAB].
+  StreamTable<DebugCanvas> debug;
+  StreamTable<CameraCtl> camera;
+  StreamTable<FaceCrop> crop;
+  StreamTable<CropPlanes> crop_planes;
+  StreamTable<FaceTensor> tensor;
+  DevBuf d_debug_tab;
+  // what a tick launches for them, from the tables (count_outputs): the streams with a debug canvas, with a canvas and
+  // strokes on, with a camera, with a crop and with a tensor (0: no launch for them), and the tiles of the largest
+  // crop and tensor (k_face_crop's grid.x)
+  int debug_count = 0, stroke_count = 0, camera_count = 0;
+  int crop_count = 0, crop_tiles = 0, tensor_count = 0, tensor_tiles = 0;
   // ht_tracker_feed(_canvases): the record table {ids[n], clocks[n], FeedRec[n], EntryCanvas[n], tile starts[n+1]}
   // goes up in one copy from pinned memory; the videos are drawn into the canvas arena (batch entry k's canvas at
   // EntryCanvas::base), zeroed when it grows
@@ -1643,10 +1666,17 @@ static int ensure_stream_buffers(ht_ctx *ctx, cudaStream_t st) {
   return HT_OK;
 }
 
+// Streams [first, first + n) inside [0, max_frames), checked in a form that cannot overflow
+static int check_streams(ht_ctx *ctx, int first, int n) {
+  const int mf = ctx->cfg.max_frames;
+  if (first < 0 || n <= 0 || first > mf - n) return ctx->fail(HT_ERR_ARG, "stream range outside [0,%d)", mf);
+  return HT_OK;
+}
+
 int ht_stream_reset(ht_ctx *ctx, int first, int n) {
   if (!ctx) return HT_ERR_ARG;
   { const int jr = join_aux(ctx); if (jr != HT_OK) return jr; }
-  if (first < 0 || n <= 0 || first + n > ctx->cfg.max_frames) return ctx->fail(HT_ERR_ARG, "stream range outside [0,%d)", ctx->cfg.max_frames);
+  { const int sr = check_streams(ctx, first, n); if (sr != HT_OK) return sr; }
   CK(cudaSetDevice(ctx->cfg.device));
   int rc = ensure_stream_buffers(ctx, ctx->stream);
   if (rc != HT_OK) return rc;
@@ -1737,10 +1767,15 @@ static TrackerParams make_tracker_params(const ht_tracker_params *p) {
   return tp;
 }
 
-static int tracker_control(ht_ctx *ctx, int first, int n, int op) {
+// What every call on tracker streams [first, first + n) checks first
+static int tracker_streams(ht_ctx *ctx, int first, int n) {
   if (!ctx) return HT_ERR_ARG;
   if (!ctx->tracker_on) return ctx->fail(HT_ERR_STATE, "ht_tracker_config has not been called");
-  if (first < 0 || n <= 0 || first + n > ctx->cfg.max_frames) return ctx->fail(HT_ERR_ARG, "stream range outside [0,%d)", ctx->cfg.max_frames);
+  return check_streams(ctx, first, n);
+}
+
+static int tracker_control(ht_ctx *ctx, int first, int n, int op) {
+  { const int ar = tracker_streams(ctx, first, n); if (ar != HT_OK) return ar; }
   { const int jr = join_aux(ctx); if (jr != HT_OK) return jr; }
   CK(cudaSetDevice(ctx->cfg.device));
   k_tracker_control<<<(unsigned)((n + 127) / 128), 128, 0, ctx->stream>>>(ctx->d_tracker_state.as<TrackerState>(), first, n, op);
@@ -1753,33 +1788,41 @@ static bool tracker_params_ok(const ht_tracker_params &p) {
   return tracker_head_ok(p.head.alpha, p.head.distance_to_screen);
 }
 
+// What a tick launches for the per-stream outputs, from their tables: after every change to a table
+static void count_outputs(ht_ctx *ctx) {
+  const auto tiles = [](int w, int h) { return ((w + CROP_TX - 1) / CROP_TX) * ((h + CROP_TY - 1) / CROP_TY); };
+  ctx->debug_count = ctx->stroke_count = ctx->camera_count = 0;
+  ctx->crop_count = ctx->crop_tiles = ctx->tensor_count = ctx->tensor_tiles = 0;
+  for (const DebugCanvas &d : ctx->debug.h) {
+    ctx->debug_count += d.rgba != nullptr;
+    ctx->stroke_count += d.rgba != nullptr && d.strokes;
+  }
+  for (const CameraCtl &k : ctx->camera.h) ctx->camera_count += k.camera != nullptr;
+  for (const FaceCrop &f : ctx->crop.h)
+    if (f.rgba) {
+      ++ctx->crop_count;
+      ctx->crop_tiles = std::max(ctx->crop_tiles, tiles(f.w, f.h));
+    }
+  for (const FaceTensor &t : ctx->tensor.h)
+    if (t.data) {
+      ++ctx->tensor_count;
+      ctx->tensor_tiles = std::max(ctx->tensor_tiles, tiles(t.w, t.h));
+    }
+}
+
 int ht_tracker_config(ht_ctx *ctx, const ht_tracker_params *params) {
   if (!ctx) return HT_ERR_ARG;
   { const int jr = join_aux(ctx); if (jr != HT_OK) return jr; }
   CK(cudaSetDevice(ctx->cfg.device));
   const size_t mf = (size_t)ctx->cfg.max_frames;
   if (params && !tracker_params_ok(*params)) return ctx->fail(HT_ERR_ARG, "bad head parameters");
-  if (ctx->debug_count > 0 || ctx->stroke_flags > 0) {   // either form discards the debug canvases and stroke flags
-    CK(cudaMemsetAsync(ctx->d_debug.p, 0, mf * sizeof(DebugCanvas), ctx->stream));   // (the array is all 0 otherwise)
-    ctx->h_debug.assign(mf, DebugCanvas{});
-    ctx->debug_count = ctx->stroke_flags = ctx->stroke_count = 0;
-  }
-  if (ctx->camera_count > 0) {   // and every camera controller
-    CK(cudaMemsetAsync(ctx->d_camera.p, 0, mf * sizeof(CameraCtl), ctx->stream));
-    ctx->h_camera.assign(mf, CameraCtl{});
-    ctx->camera_count = 0;
-  }
-  if (ctx->crop_count > 0) {     // and every face crop
-    CK(cudaMemsetAsync(ctx->d_crop.p, 0, mf * sizeof(FaceCrop), ctx->stream));
-    ctx->h_crop.assign(mf, FaceCrop{});
-    ctx->h_crop_planes.assign(mf, CropPlanes{});
-    ctx->crop_count = ctx->crop_tiles = 0;
-  }
-  if (ctx->tensor_count > 0) {   // and every face tensor
-    CK(cudaMemsetAsync(ctx->d_tensor.p, 0, mf * sizeof(FaceTensor), ctx->stream));
-    ctx->h_tensor.assign(mf, FaceTensor{});
-    ctx->tensor_count = ctx->tensor_tiles = 0;
-  }
+  // either form discards every stream's debug canvas and stroke flag, camera, face crop and face tensor
+  CK(ctx->debug.clear(ctx->stream));
+  CK(ctx->camera.clear(ctx->stream));
+  CK(ctx->crop.clear(ctx->stream));
+  CK(ctx->crop_planes.clear(ctx->stream));
+  CK(ctx->tensor.clear(ctx->stream));
+  count_outputs(ctx);
   if (!params) {                 // off: every stream as after ht_stream_reset (the lifecycle has used the tracker slots)
     if (ctx->tracker_on) {
       ctx->tracker_on = false;
@@ -1813,10 +1856,7 @@ int ht_tracker_config(ht_ctx *ctx, const ht_tracker_params *params) {
 // The parameters of streams [first, first + n), each its own headtrackr.Tracker's.  Stream states are kept; calcAngles
 // reaches a stream at its next initTracker (k_track_init reads it per entry), the rest at its next tick.
 int ht_tracker_set_params(ht_ctx *ctx, int first, int n, const ht_tracker_params *params) {
-  if (!ctx) return HT_ERR_ARG;
-  if (!ctx->tracker_on) return ctx->fail(HT_ERR_STATE, "ht_tracker_config has not been called");
-  const int mf = ctx->cfg.max_frames;
-  if (first < 0 || n <= 0 || first > mf - n) return ctx->fail(HT_ERR_ARG, "stream range outside [0,%d)", mf);
+  { const int ar = tracker_streams(ctx, first, n); if (ar != HT_OK) return ar; }
   if (!params) return ctx->fail(HT_ERR_ARG, "params is NULL");
   for (int i = 0; i < n; ++i)
     if (!tracker_params_ok(params[i])) return ctx->fail(HT_ERR_ARG, "record %d: bad head parameters", i);
@@ -1834,99 +1874,139 @@ static_assert(sizeof(ht_debug_canvas) == 24 && sizeof(DebugCanvas) == sizeof(ht_
                   offsetof(ht_debug_canvas, pitch) == offsetof(DebugCanvas, pitch),
               "ht_debug_canvas layout");
 
-// Streams [first, first + n) of `next` (every stream's DebugCanvas after a checked call) go to the device, and the
-// counts that decide a tick's debug launches follow them.
-static int debug_commit(ht_ctx *ctx, int first, int n, std::vector<DebugCanvas> &next) {
-  const size_t mf = (size_t)ctx->cfg.max_frames;
-  { const int jr = join_aux(ctx); if (jr != HT_OK) return jr; }
-  CK(cudaSetDevice(ctx->cfg.device));
-  if (!ctx->d_debug.p) {
-    CK(ctx->d_debug.reserve(mf * sizeof(DebugCanvas)));
-    CK(ctx->d_debug_tab.reserve(mf * DBG_TAB));
-    CK(cudaMemsetAsync(ctx->d_debug.p, 0, mf * sizeof(DebugCanvas), ctx->stream));
-  }
-  CK(cudaMemcpyAsync(ctx->d_debug.as<DebugCanvas>() + first, next.data() + first, (size_t)n * sizeof(DebugCanvas),
-                     cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));    // `next` is the caller's local
-  ctx->debug_count = ctx->stroke_flags = ctx->stroke_count = 0;
-  for (const DebugCanvas &d : next) {
-    ctx->debug_count += d.rgba != nullptr;
-    ctx->stroke_flags += d.strokes;
-    ctx->stroke_count += d.rgba != nullptr && d.strokes;
-  }
-  ctx->h_debug.swap(next);
-  return HT_OK;
-}
+// The kinds of byte range a tick writes for a stream, as the overlap messages name them
+enum { OUT_DEBUG, OUT_CROP, OUT_TENSOR, OUT_CAMERA };
+static const char *const OUT_NAME[] ={"debug canvas", "face crop plane", "face tensor plane", "camera"};
 
-// Bytes a face tensor's span covers: `rows` rows of `row` elements of `es` bytes each, the last one `last` elements
-static size_t tensor_span(const FaceTensor &t, long long last) {
-  const size_t es = t.dtype == HT_TENSOR_U8 ? 1 : t.dtype == HT_TENSOR_F32 ? 4 : 2;
-  return ((size_t)(t.h - 1) * (size_t)t.row + (size_t)last) * es;
-}
+// One byte range [start, end) that a tick writes: part of the `kind` output of stream `stream`
+struct TickWrite { uintptr_t start, end; int kind, stream; };
 
-// Whether two of the images written during a tick - every debug canvas, every plane of every face crop and every
-// channel plane (CHW) or whole tensor (HWC) of every face tensor - share a byte: the streams of a tick run
-// concurrently.  -> -1 if none do; otherwise a stream whose crop (tensor_side false) or tensor (true) takes part, one
-// in [first, first + n) if there is one (so that a setter can name the record), or -2 if only debug canvases do.
-static int images_overlap(const std::vector<DebugCanvas> &dbg, const std::vector<FaceCrop> &crops,
-                          const std::vector<CropPlanes> &planes, const std::vector<FaceTensor> &tensors, int first = 0,
-                          int n = 0, bool tensor_side = false) {
-  struct Span { uintptr_t start, end; int crop; bool tensor; };   // crop: its stream, -2 for a debug canvas
-  std::vector<Span> spans;
-  auto add = [&](const uint8_t *p, int bytes, int rows, int pitch, int crop) {
-    const uintptr_t s = reinterpret_cast<uintptr_t>(p);
-    spans.push_back(Span{s, s + (size_t)(rows - 1) * pitch + (size_t)bytes, crop, false});
+// Whether two of the byte ranges a tick writes share a byte (the streams of a tick run concurrently): each debug
+// canvas (one span over its rows), each plane of each face crop, each channel plane (CHW) or whole tensor (HWC) of
+// each face tensor, and each camera.  The first clashing pair in order of start goes to clash[0..1].
+static bool tick_writes_overlap(const std::vector<DebugCanvas> &debug, const std::vector<FaceCrop> &crop,
+                                const std::vector<CropPlanes> &crop_planes, const std::vector<FaceTensor> &tensor,
+                                const std::vector<CameraCtl> &camera, TickWrite clash[2]) {
+  std::vector<TickWrite> w;
+  const auto add = [&](const void *p, size_t rows, size_t pitch, size_t row_bytes, int kind, size_t s) {
+    const uintptr_t a = reinterpret_cast<uintptr_t>(p);
+    w.push_back(TickWrite{a, a + (rows - 1) * pitch + row_bytes, kind, (int)s});
   };
-  for (size_t k = 0; k < tensors.size(); ++k) {
-    const FaceTensor &t = tensors[k];
+  for (size_t s = 0; s < debug.size(); ++s) {
+    const DebugCanvas &d = debug[s];
+    if (d.rgba) add(d.rgba, d.h, d.pitch, 4 * (size_t)d.w, OUT_DEBUG, s);
+  }
+  for (size_t s = 0; s < crop.size(); ++s) {
+    const FaceCrop &f = crop[s];
+    if (!f.rgba) continue;
+    if (f.layout == CROP_RGBA) {
+      add(f.rgba, f.h, f.pitch, 4 * (size_t)f.w, OUT_CROP, s);
+      continue;
+    }
+    const CropPlanes &q = crop_planes[s];
+    add(f.rgba, f.h, f.pitch, f.w, OUT_CROP, s);
+    if (f.layout == CROP_NV12) {
+      add(q.u, f.h / 2, q.upitch, f.w, OUT_CROP, s);
+    } else {
+      add(q.u, f.h / 2, q.upitch, f.w / 2, OUT_CROP, s);
+      add(q.v, f.h / 2, q.vpitch, f.w / 2, OUT_CROP, s);
+    }
+  }
+  for (size_t s = 0; s < tensor.size(); ++s) {
+    const FaceTensor &t = tensor[s];
     if (!t.data) continue;
-    const uintptr_t s = reinterpret_cast<uintptr_t>(t.data);
     const size_t es = t.dtype == HT_TENSOR_U8 ? 1 : t.dtype == HT_TENSOR_F32 ? 4 : 2;
     const int C = t.channels == HT_TENSOR_GRAY ? 1 : 3;
     if (t.layout == HT_TENSOR_HWC) {
-      spans.push_back(Span{s, s + tensor_span(t, (long long)C * t.w), (int)k, true});
+      add(t.data, t.h, (size_t)t.row * es, (size_t)C * t.w * es, OUT_TENSOR, s);
     } else {
       for (int c = 0; c < C; ++c)
-        spans.push_back(Span{s + (size_t)c * (size_t)t.plane * es, s + (size_t)c * (size_t)t.plane * es + tensor_span(t, t.w),
-                             (int)k, true});
+        add(static_cast<const uint8_t *>(t.data) + (size_t)c * (size_t)t.plane * es, t.h, (size_t)t.row * es,
+            (size_t)t.w * es, OUT_TENSOR, s);
     }
   }
-  for (const DebugCanvas &d : dbg)
-    if (d.rgba) add(d.rgba, 4 * d.w, d.h, d.pitch, -2);
-  for (size_t k = 0; k < crops.size(); ++k) {
-    const FaceCrop &f = crops[k];
-    if (!f.rgba) continue;
-    if (f.layout == CROP_RGBA) { add(f.rgba, 4 * f.w, f.h, f.pitch, (int)k); continue; }
-    const CropPlanes &c = planes[k];
-    add(f.rgba, f.w, f.h, f.pitch, (int)k);
-    if (f.layout == CROP_NV12) {
-      add(c.u, f.w, f.h / 2, c.upitch, (int)k);
-    } else {
-      add(c.u, f.w / 2, f.h / 2, c.upitch, (int)k);
-      add(c.v, f.w / 2, f.h / 2, c.vpitch, (int)k);
+  for (size_t s = 0; s < camera.size(); ++s)
+    if (camera[s].camera) add(camera[s].camera, 1, 0, sizeof(ht_camera), OUT_CAMERA, s);
+  std::sort(w.begin(), w.end(), [](const TickWrite &a, const TickWrite &b) { return a.start < b.start; });
+  for (size_t i = 1; i < w.size(); ++i)
+    if (w[i].start < w[i - 1].end) {
+      clash[0] = w[i - 1];
+      clash[1] = w[i];
+      return true;
     }
-  }
-  std::sort(spans.begin(), spans.end(), [](const Span &a, const Span &b) { return a.start < b.start; });
-  int found = -1;
-  for (size_t i = 1; i < spans.size(); ++i)
-    if (spans[i].start < spans[i - 1].end)
-      for (const Span *s : {&spans[i - 1], &spans[i]}) {
-        if (s->tensor == tensor_side && s->crop >= first && s->crop < first + n) return s->crop;
-        if (found < 0 || s->crop >= 0) found = std::max(found, s->crop);
-      }
-  return found;
+  return false;
 }
 
-// The debug canvases of streams [first, first + n).  Everything is checked on the host before anything changes,
-// overlap over every stream that has a canvas after the call.
+// A setter's checked tables: every stream's records of the output it sets, as they are to be after the call.  NULL:
+// the context's table stands.
+struct OutputEdit {
+  std::vector<DebugCanvas> *debug = nullptr;
+  std::vector<CameraCtl> *camera = nullptr;
+  std::vector<FaceCrop> *crop = nullptr;
+  std::vector<CropPlanes> *crop_planes = nullptr;
+  std::vector<FaceTensor> *tensor = nullptr;
+};
+
+// How every setter's records reach the tick.  The call is refused if two byte ranges a tick would write share a byte
+// (the tables before it share none, so a clash takes in one of its records, which the message names).  Otherwise
+// streams [first, first + n) of the edited tables go to the device, a new camera is constructed there, and the tables
+// and the tick's counts follow.
+static int commit_outputs(ht_ctx *ctx, int first, int n, const OutputEdit &e) {
+  const int kind = e.debug ? OUT_DEBUG : e.crop ? OUT_CROP : e.tensor ? OUT_TENSOR : OUT_CAMERA;
+  TickWrite c[2];
+  if (tick_writes_overlap(e.debug ? *e.debug : ctx->debug.h, e.crop ? *e.crop : ctx->crop.h,
+                          e.crop_planes ? *e.crop_planes : ctx->crop_planes.h, e.tensor ? *e.tensor : ctx->tensor.h,
+                          e.camera ? *e.camera : ctx->camera.h, c)) {
+    const int own = c[0].kind == kind && c[0].stream >= first && c[0].stream - first < n ? 0 : 1;
+    return ctx->fail(HT_ERR_ARG, "record %d: its %s overlaps the %s of stream %d", c[own].stream - first,
+                     OUT_NAME[c[own].kind], OUT_NAME[c[1 - own].kind], c[1 - own].stream);
+  }
+  { const int jr = join_aux(ctx); if (jr != HT_OK) return jr; }
+  CK(cudaSetDevice(ctx->cfg.device));
+  const size_t mf = (size_t)ctx->cfg.max_frames;
+  cudaStream_t st = ctx->stream;
+  if (e.debug) {
+    CK(ctx->d_debug_tab.reserve(mf * DBG_TAB));
+    CK(ctx->debug.commit(*e.debug, first, n, st));
+  }
+  if (e.crop || e.tensor) {   // k_face_crop's tables, allocated together
+    CK(ctx->crop.reserve(mf, st));
+    CK(ctx->crop_planes.reserve(mf, st));
+    CK(ctx->tensor.reserve(mf, st));
+  }
+  if (e.crop) {
+    CK(ctx->crop.commit(*e.crop, first, n, st));
+    CK(ctx->crop_planes.commit(*e.crop_planes, first, n, st));
+  }
+  if (e.tensor) CK(ctx->tensor.commit(*e.tensor, first, n, st));
+  if (e.camera) {
+    CK(ctx->camera.commit(*e.camera, first, n, st));
+    k_camera_construct<<<1, 256, 0, st>>>(ctx->camera.dev(), first, n);
+    ++ctx->launches;
+    CK(cudaGetLastError());
+  }
+  CK(cudaStreamSynchronize(st));    // the edited tables are the setter's locals
+  if (e.debug) ctx->debug.h.swap(*e.debug);
+  if (e.camera) ctx->camera.h.swap(*e.camera);
+  if (e.crop) {
+    ctx->crop.h.swap(*e.crop);
+    ctx->crop_planes.h.swap(*e.crop_planes);
+  }
+  if (e.tensor) ctx->tensor.h.swap(*e.tensor);
+  count_outputs(ctx);
+  return HT_OK;
+}
+
+// A debug canvas as the tick takes it, pitch resolved (the record is not checked)
+static DebugCanvas debug_record(const ht_debug_canvas &c) {
+  return DebugCanvas{c.rgba, c.width, c.height, c.pitch ? c.pitch : 4 * c.width, 0};
+}
+
+// The debug canvases of streams [first, first + n).  Everything is checked on the host before anything changes.
 int ht_tracker_set_debug(ht_ctx *ctx, int first, int n, const ht_debug_canvas *canvases) {
-  if (!ctx) return HT_ERR_ARG;
-  if (!ctx->tracker_on) return ctx->fail(HT_ERR_STATE, "ht_tracker_config has not been called");
-  const int mf = ctx->cfg.max_frames;
-  if (first < 0 || n <= 0 || first > mf - n) return ctx->fail(HT_ERR_ARG, "stream range outside [0,%d)", mf);
+  { const int ar = tracker_streams(ctx, first, n); if (ar != HT_OK) return ar; }
   if (!canvases) return ctx->fail(HT_ERR_ARG, "canvases is NULL");
-  std::vector<DebugCanvas> next = ctx->h_debug;
-  next.resize((size_t)mf, DebugCanvas{});
+  std::vector<DebugCanvas> next = ctx->debug.edit(ctx->cfg.max_frames);
   for (int i = 0; i < n; ++i) {
     const ht_debug_canvas &c = canvases[i];
     DebugCanvas d{};
@@ -1937,43 +2017,28 @@ int ht_tracker_set_debug(ht_ctx *ctx, int first, int n, const ht_debug_canvas *c
         return ctx->fail(HT_ERR_SIZE, "record %d: debug canvas %dx%d outside 1..16384", i, c.width, c.height);
       if ((c.pitch & 3) || (c.pitch != 0 && c.pitch < 4 * c.width))
         return ctx->fail(HT_ERR_ARG, "record %d: pitch %d is not a multiple of 4 >= 4*width", i, c.pitch);
-      d = DebugCanvas{c.rgba, c.width, c.height, c.pitch ? c.pitch : 4 * c.width, 0};
+      d = debug_record(c);
     }
     d.strokes = next[(size_t)(first + i)].strokes;     // the stream's stroke flag stays
     next[(size_t)(first + i)] = d;
   }
-  // two canvases of one tick's streams must not share a byte: [start, end) of every canvas, sorted by start
-  std::vector<std::pair<uintptr_t, uintptr_t>> spans;
-  for (const DebugCanvas &d : next)
-    if (d.rgba) {
-      const uintptr_t s = reinterpret_cast<uintptr_t>(d.rgba);
-      spans.emplace_back(s, s + (size_t)(d.h - 1) * d.pitch + 4 * (size_t)d.w);
-    }
-  std::sort(spans.begin(), spans.end());
-  for (size_t i = 1; i < spans.size(); ++i)
-    if (spans[i].first < spans[i - 1].second)
-      return ctx->fail(HT_ERR_ARG, "a debug canvas overlaps another stream's debug canvas");
-  if (ctx->crop_count > 0 && images_overlap(next, ctx->h_crop, ctx->h_crop_planes, {}) != -1)
-    return ctx->fail(HT_ERR_ARG, "a debug canvas overlaps a face crop");
-  if (ctx->tensor_count > 0 && images_overlap(next, {}, {}, ctx->h_tensor) != -1)
-    return ctx->fail(HT_ERR_ARG, "a debug canvas overlaps a face tensor");
-  return debug_commit(ctx, first, n, next);
+  OutputEdit e;
+  e.debug = &next;
+  return commit_outputs(ctx, first, n, e);
 }
 
 // Streams first+i stroke main.js's rectangles on their debug canvases (enable[i] 1) or not (0).  The flag is the
 // stream's, kept in the pad word of its DebugCanvas.
 int ht_tracker_set_debug_strokes(ht_ctx *ctx, int first, int n, const int32_t *enable) {
-  if (!ctx) return HT_ERR_ARG;
-  if (!ctx->tracker_on) return ctx->fail(HT_ERR_STATE, "ht_tracker_config has not been called");
-  const int mf = ctx->cfg.max_frames;
-  if (first < 0 || n <= 0 || first > mf - n) return ctx->fail(HT_ERR_ARG, "stream range outside [0,%d)", mf);
+  { const int ar = tracker_streams(ctx, first, n); if (ar != HT_OK) return ar; }
   if (!enable) return ctx->fail(HT_ERR_ARG, "enable is NULL");
   for (int i = 0; i < n; ++i)
     if (enable[i] != 0 && enable[i] != 1) return ctx->fail(HT_ERR_ARG, "record %d: enable %d is not 0 or 1", i, enable[i]);
-  std::vector<DebugCanvas> next = ctx->h_debug;
-  next.resize((size_t)mf, DebugCanvas{});
+  std::vector<DebugCanvas> next = ctx->debug.edit(ctx->cfg.max_frames);
   for (int i = 0; i < n; ++i) next[(size_t)(first + i)].strokes = enable[i];
-  return debug_commit(ctx, first, n, next);
+  OutputEdit e;
+  e.debug = &next;
+  return commit_outputs(ctx, first, n, e);
 }
 
 static_assert(sizeof(ht_face_crop) == 32 && sizeof(FaceCrop) == sizeof(ht_face_crop) &&
@@ -1981,20 +2046,17 @@ static_assert(sizeof(ht_face_crop) == 32 && sizeof(FaceCrop) == sizeof(ht_face_c
                   offsetof(ht_face_crop, scale) == offsetof(FaceCrop, scale),
               "ht_face_crop layout");
 
-static int crop_commit(ht_ctx *ctx, int first, int n, std::vector<FaceCrop> &next, std::vector<CropPlanes> &planes);
+// An RGBA crop as k_face_crop takes it, pitch resolved (the record is not checked)
+static FaceCrop crop_record(const ht_face_crop &c) {
+  return FaceCrop{c.rgba, c.width, c.height, c.pitch ? c.pitch : 4 * c.width, CROP_RGBA, c.scale};
+}
 
-// The face crops of streams [first, first + n).  Everything is checked on the host before anything changes, overlap
-// over every crop and debug canvas after the call.
+// The face crops of streams [first, first + n).  Everything is checked on the host before anything changes.
 int ht_tracker_set_face_crop(ht_ctx *ctx, int first, int n, const ht_face_crop *crops) {
-  if (!ctx) return HT_ERR_ARG;
-  if (!ctx->tracker_on) return ctx->fail(HT_ERR_STATE, "ht_tracker_config has not been called");
-  const int mf = ctx->cfg.max_frames;
-  if (first < 0 || n <= 0 || first > mf - n) return ctx->fail(HT_ERR_ARG, "stream range outside [0,%d)", mf);
+  { const int ar = tracker_streams(ctx, first, n); if (ar != HT_OK) return ar; }
   if (!crops) return ctx->fail(HT_ERR_ARG, "crops is NULL");
-  std::vector<FaceCrop> next = ctx->h_crop;
-  std::vector<CropPlanes> planes = ctx->h_crop_planes;
-  next.resize((size_t)mf, FaceCrop{});
-  planes.resize((size_t)mf, CropPlanes{});
+  std::vector<FaceCrop> next = ctx->crop.edit(ctx->cfg.max_frames);
+  std::vector<CropPlanes> planes = ctx->crop_planes.edit(ctx->cfg.max_frames);
   for (int i = 0; i < n; ++i) {
     const ht_face_crop &c = crops[i];
     FaceCrop f{};
@@ -2006,51 +2068,15 @@ int ht_tracker_set_face_crop(ht_ctx *ctx, int first, int n, const ht_face_crop *
       if ((c.pitch & 3) || (c.pitch != 0 && c.pitch < 4 * c.width))
         return ctx->fail(HT_ERR_ARG, "record %d: pitch %d is not a multiple of 4 >= 4*width", i, c.pitch);
       if (!(c.scale > 0.0 && c.scale <= 16.0)) return ctx->fail(HT_ERR_ARG, "record %d: scale %g outside (0, 16]", i, c.scale);
-      f = FaceCrop{c.rgba, c.width, c.height, c.pitch ? c.pitch : 4 * c.width, CROP_RGBA, c.scale};
+      f = crop_record(c);
     }
     next[(size_t)(first + i)] = f;
     planes[(size_t)(first + i)] = CropPlanes{};
   }
-  if (images_overlap(ctx->h_debug, next, planes, {}) != -1)
-    return ctx->fail(HT_ERR_ARG, "a face crop overlaps another stream's face crop or a debug canvas");
-  if (ctx->tensor_count > 0 && images_overlap({}, next, planes, ctx->h_tensor) != -1)
-    return ctx->fail(HT_ERR_ARG, "a face crop overlaps a face tensor");
-  return crop_commit(ctx, first, n, next, planes);
-}
-
-// k_face_crop's tables - every stream's FaceCrop, CropPlanes and FaceTensor, all 0 at first - on first use of either
-// setter: a grid with a tensor slice also has the crop slice, which reads the crop table.
-static int crop_tables(ht_ctx *ctx) {
-  const size_t mf = (size_t)ctx->cfg.max_frames;
-  if (ctx->d_crop.p) return HT_OK;
-  CK(ctx->d_crop.reserve(mf * sizeof(FaceCrop)));
-  CK(cudaMemsetAsync(ctx->d_crop.p, 0, mf * sizeof(FaceCrop), ctx->stream));
-  CK(ctx->d_crop_planes.reserve(mf * sizeof(CropPlanes)));
-  CK(cudaMemsetAsync(ctx->d_crop_planes.p, 0, mf * sizeof(CropPlanes), ctx->stream));
-  CK(ctx->d_tensor.reserve(mf * sizeof(FaceTensor)));
-  CK(cudaMemsetAsync(ctx->d_tensor.p, 0, mf * sizeof(FaceTensor), ctx->stream));
-  return HT_OK;
-}
-
-// The checked crops of streams [first, first + n), of either layout, into the device tables and the context.
-static int crop_commit(ht_ctx *ctx, int first, int n, std::vector<FaceCrop> &next, std::vector<CropPlanes> &planes) {
-  { const int jr = join_aux(ctx); if (jr != HT_OK) return jr; }
-  CK(cudaSetDevice(ctx->cfg.device));
-  { const int tr = crop_tables(ctx); if (tr != HT_OK) return tr; }
-  CK(cudaMemcpyAsync(ctx->d_crop.as<FaceCrop>() + first, next.data() + first, (size_t)n * sizeof(FaceCrop),
-                     cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemcpyAsync(ctx->d_crop_planes.as<CropPlanes>() + first, planes.data() + first, (size_t)n * sizeof(CropPlanes),
-                     cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));    // `next` and `planes` are the caller's locals
-  ctx->crop_count = ctx->crop_tiles = 0;
-  for (const FaceCrop &f : next)
-    if (f.rgba) {
-      ++ctx->crop_count;
-      ctx->crop_tiles = std::max(ctx->crop_tiles, ((f.w + CROP_TX - 1) / CROP_TX) * ((f.h + CROP_TY - 1) / CROP_TY));
-    }
-  ctx->h_crop.swap(next);
-  ctx->h_crop_planes.swap(planes);
-  return HT_OK;
+  OutputEdit e;
+  e.crop = &next;
+  e.crop_planes = &planes;
+  return commit_outputs(ctx, first, n, e);
 }
 
 static_assert(sizeof(ht_face_crop_yuv) == 64 && offsetof(ht_face_crop_yuv, pitch) == 24 &&
@@ -2069,18 +2095,12 @@ static void crop_yuv_record(const ht_face_crop_yuv &c, FaceCrop &f, CropPlanes &
   q = CropPlanes{c.planes[1], nv12 ? c.planes[1] + 1 : c.planes[2], pitch[1], nv12 ? pitch[1] : pitch[2], c.color, 0};
 }
 
-// The YUV face crops of streams [first, first + n).  Everything is checked on the host before anything changes,
-// overlap over every plane of every crop and every debug canvas after the call.
+// The YUV face crops of streams [first, first + n).  Everything is checked on the host before anything changes.
 int ht_tracker_set_face_crop_yuv(ht_ctx *ctx, int first, int n, const ht_face_crop_yuv *crops) {
-  if (!ctx) return HT_ERR_ARG;
-  if (!ctx->tracker_on) return ctx->fail(HT_ERR_STATE, "ht_tracker_config has not been called");
-  const int mf = ctx->cfg.max_frames;
-  if (first < 0 || n <= 0 || first > mf - n) return ctx->fail(HT_ERR_ARG, "stream range outside [0,%d)", mf);
+  { const int ar = tracker_streams(ctx, first, n); if (ar != HT_OK) return ar; }
   if (!crops) return ctx->fail(HT_ERR_ARG, "crops is NULL");
-  std::vector<FaceCrop> next = ctx->h_crop;
-  std::vector<CropPlanes> planes = ctx->h_crop_planes;
-  next.resize((size_t)mf, FaceCrop{});
-  planes.resize((size_t)mf, CropPlanes{});
+  std::vector<FaceCrop> next = ctx->crop.edit(ctx->cfg.max_frames);
+  std::vector<CropPlanes> planes = ctx->crop_planes.edit(ctx->cfg.max_frames);
   for (int i = 0; i < n; ++i) {
     const ht_face_crop_yuv &c = crops[i];
     FaceCrop f{};
@@ -2111,13 +2131,10 @@ int ht_tracker_set_face_crop_yuv(ht_ctx *ctx, int first, int n, const ht_face_cr
     next[(size_t)(first + i)] = f;
     planes[(size_t)(first + i)] = q;
   }
-  const int clash = images_overlap(ctx->h_debug, next, planes, {}, first, n);
-  if (clash != -1)
-    return ctx->fail(HT_ERR_ARG, "record %d: a plane overlaps another plane of the crop, another stream's face crop or a debug canvas",
-                     clash - first);
-  const int tclash = ctx->tensor_count > 0 ? images_overlap({}, next, planes, ctx->h_tensor, first, n) : -1;
-  if (tclash != -1) return ctx->fail(HT_ERR_ARG, "record %d: a plane overlaps a face tensor", tclash - first);
-  return crop_commit(ctx, first, n, next, planes);
+  OutputEdit e;
+  e.crop = &next;
+  e.crop_planes = &planes;
+  return commit_outputs(ctx, first, n, e);
 }
 
 static_assert(sizeof(ht_face_tensor) == 80 && sizeof(FaceTensor) == sizeof(ht_face_tensor) &&
@@ -2139,16 +2156,12 @@ static FaceTensor tensor_record(const ht_face_tensor &t) {
   return f;
 }
 
-// The face tensors of streams [first, first + n).  Everything is checked on the host before anything changes, overlap
-// over every tensor plane, crop plane and debug canvas after the call.  Crops are untouched.
+// The face tensors of streams [first, first + n).  Everything is checked on the host before anything changes.  Crops
+// are untouched.
 int ht_tracker_set_face_tensor(ht_ctx *ctx, int first, int n, const ht_face_tensor *tensors) {
-  if (!ctx) return HT_ERR_ARG;
-  if (!ctx->tracker_on) return ctx->fail(HT_ERR_STATE, "ht_tracker_config has not been called");
-  const int mf = ctx->cfg.max_frames;
-  if (first < 0 || n <= 0 || first > mf - n) return ctx->fail(HT_ERR_ARG, "stream range outside [0,%d)", mf);
+  { const int ar = tracker_streams(ctx, first, n); if (ar != HT_OK) return ar; }
   if (!tensors) return ctx->fail(HT_ERR_ARG, "tensors is NULL");
-  std::vector<FaceTensor> next = ctx->h_tensor;
-  next.resize((size_t)mf, FaceTensor{});
+  std::vector<FaceTensor> next = ctx->tensor.edit(ctx->cfg.max_frames);
   const long long cap = 1ll << 40;
   for (int i = 0; i < n; ++i) {
     const ht_face_tensor &t = tensors[i];
@@ -2189,24 +2202,9 @@ int ht_tracker_set_face_tensor(ht_ctx *ctx, int first, int n, const ht_face_tens
     }
     next[(size_t)(first + i)] = f;
   }
-  const int clash = images_overlap(ctx->h_debug, ctx->h_crop, ctx->h_crop_planes, next, first, n, true);
-  if (clash != -1)
-    return ctx->fail(HT_ERR_ARG, "record %d: a face tensor overlaps itself, another stream's face tensor, a face crop or a debug canvas",
-                     clash - first);
-  { const int jr = join_aux(ctx); if (jr != HT_OK) return jr; }
-  CK(cudaSetDevice(ctx->cfg.device));
-  { const int tr = crop_tables(ctx); if (tr != HT_OK) return tr; }
-  CK(cudaMemcpyAsync(ctx->d_tensor.as<FaceTensor>() + first, next.data() + first, (size_t)n * sizeof(FaceTensor),
-                     cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));    // `next` is a local
-  ctx->tensor_count = ctx->tensor_tiles = 0;
-  for (const FaceTensor &f : next)
-    if (f.data) {
-      ++ctx->tensor_count;
-      ctx->tensor_tiles = std::max(ctx->tensor_tiles, ((f.w + CROP_TX - 1) / CROP_TX) * ((f.h + CROP_TY - 1) / CROP_TY));
-    }
-  ctx->h_tensor.swap(next);
-  return HT_OK;
+  OutputEdit e;
+  e.tensor = &next;
+  return commit_outputs(ctx, first, n, e);
 }
 
 static int view_record(const ht_video_view &view, int w, int h, ViewFeedRec &v, char *why);
@@ -2269,16 +2267,12 @@ static const char *camera_ctl_make(const ht_camera_control &c, CameraCtl *out) {
   return nullptr;
 }
 
-// The camera controllers of streams [first, first + n).  Everything is checked on the host before anything changes,
-// overlap over every stream that has a controller after the call; then one launch constructs the new cameras.
+// The camera controllers of streams [first, first + n).  Everything is checked on the host before anything changes;
+// then one launch constructs the new cameras.
 int ht_tracker_set_camera(ht_ctx *ctx, int first, int n, const ht_camera_control *controls) {
-  if (!ctx) return HT_ERR_ARG;
-  if (!ctx->tracker_on) return ctx->fail(HT_ERR_STATE, "ht_tracker_config has not been called");
-  const int mf = ctx->cfg.max_frames;
-  if (first < 0 || n <= 0 || first > mf - n) return ctx->fail(HT_ERR_ARG, "stream range outside [0,%d)", mf);
+  { const int ar = tracker_streams(ctx, first, n); if (ar != HT_OK) return ar; }
   if (!controls) return ctx->fail(HT_ERR_ARG, "controls is NULL");
-  std::vector<CameraCtl> next = ctx->h_camera;
-  next.resize((size_t)mf, CameraCtl{});
+  std::vector<CameraCtl> next = ctx->camera.edit(ctx->cfg.max_frames);
   for (int i = 0; i < n; ++i) {
     const ht_camera_control &c = controls[i];
     CameraCtl k{};
@@ -2296,29 +2290,9 @@ int ht_tracker_set_camera(ht_ctx *ctx, int first, int n, const ht_camera_control
     }
     next[(size_t)(first + i)] = k;
   }
-  // two cameras of one tick's streams must not share a byte
-  std::vector<uintptr_t> starts;
-  for (const CameraCtl &k : next)
-    if (k.camera) starts.push_back(reinterpret_cast<uintptr_t>(k.camera));
-  std::sort(starts.begin(), starts.end());
-  for (size_t i = 1; i < starts.size(); ++i)
-    if (starts[i] < starts[i - 1] + sizeof(ht_camera))
-      return ctx->fail(HT_ERR_ARG, "a camera overlaps another stream's camera");
-  { const int jr = join_aux(ctx); if (jr != HT_OK) return jr; }
-  CK(cudaSetDevice(ctx->cfg.device));
-  if (!ctx->d_camera.p) {
-    CK(ctx->d_camera.reserve((size_t)mf * sizeof(CameraCtl)));
-    CK(cudaMemsetAsync(ctx->d_camera.p, 0, (size_t)mf * sizeof(CameraCtl), ctx->stream));
-  }
-  CK(cudaMemcpyAsync(ctx->d_camera.as<CameraCtl>() + first, next.data() + first, (size_t)n * sizeof(CameraCtl),
-                     cudaMemcpyHostToDevice, ctx->stream));
-  k_camera_construct<<<1, 256, 0, ctx->stream>>>(ctx->d_camera.as<CameraCtl>(), first, n);
-  ++ctx->launches;
-  CK(cudaGetLastError());
-  CK(cudaStreamSynchronize(ctx->stream));    // `next` is a local
-  ctx->camera_count = (int)starts.size();
-  ctx->h_camera.swap(next);
-  return HT_OK;
+  OutputEdit e;
+  e.camera = &next;
+  return commit_outputs(ctx, first, n, e);
 }
 
 static_assert(REC_BYTES == HT_TRACKER_RECORD_BYTES && REC_MAGIC == HT_TRACKER_RECORD_MAGIC &&
@@ -2519,7 +2493,7 @@ static int tracker_tick(ht_ctx *ctx, const TickGroup *grp, int n_groups, const u
     if (rc != HT_OK) return rc;
     if (ctx->debug_count > 0) {   // the debug canvases of this group's CS entries, from this frame's histogram
       const int32_t *ids = d_ids ? d_ids + G.k0 : nullptr;
-      const DebugCanvas *dbg = ctx->d_debug.as<DebugCanvas>();
+      const DebugCanvas *dbg = ctx->debug.dev();
       uint8_t *tab = ctx->d_debug_tab.as<uint8_t>() + (size_t)G.k0 * DBG_TAB;
       k_debug_table<<<(unsigned)G.n, 256, 0, st>>>(ids, cs_en + G.k0, dbg, ctx->model_hist.as<uint32_t>(), ch, tab);
       const int tiles_x = (G.w + DBG_TX - 1) / DBG_TX, tiles = tiles_x * ((G.h + DBG_TY - 1) / DBG_TY);
@@ -2542,11 +2516,11 @@ static int tracker_tick(ht_ctx *ctx, const TickGroup *grp, int n_groups, const u
                                                     ctx->d_out_counts.as<int32_t>(), ctx->d_objs.as<int32_t>(),
                                                     ctx->d_rects.as<int32_t>(), init_en, now_ms, d_now, g0.w, g0.h, geo, d_ev);
   if (ctx->camera_count > 0) {  // the cameras of the entries whose record has a headtrackingEvent
-    k_camera_update<<<(n + 127) / 128, 128, 0, st>>>(d_ids, geo, n, d_ev, ctx->d_camera.as<CameraCtl>());
+    k_camera_update<<<(n + 127) / 128, 128, 0, st>>>(d_ids, geo, n, d_ev, ctx->camera.dev());
     ++ctx->launches;
   }
   if (ctx->stroke_count > 0) {   // main.js's strokes, after this tick's back-projections (src/main.js:199-219)
-    k_debug_strokes<<<(unsigned)n, 256, 0, st>>>(d_ids, geo, d_ev, ctx->d_debug.as<DebugCanvas>());
+    k_debug_strokes<<<(unsigned)n, 256, 0, st>>>(d_ids, geo, d_ev, ctx->debug.dev());
     ++ctx->launches;
   }
   if (ctx->crop_count > 0 || ctx->tensor_count > 0) {   // the face crops and tensors of the entries whose record is a
@@ -2558,8 +2532,7 @@ static int tracker_tick(ht_ctx *ctx, const TickGroup *grp, int n_groups, const u
     const int tz = ctx->crop_count > 0 ? 1 : 0;           // the tensor slice (unreached without tensors)
     const unsigned slices = (unsigned)(tz + (ctx->tensor_count > 0 ? 1 : 0));
     k_face_crop<<<dim3((unsigned)std::max(ctx->crop_tiles, ctx->tensor_tiles), (unsigned)n, slices), 256, 0, st>>>(
-        d_ids, geo, g0.w, g0.h, d_ev, ctx->d_crop.as<FaceCrop>(), ctx->d_crop_planes.as<CropPlanes>(),
-        ctx->d_tensor.as<FaceTensor>(), tz, src);
+        d_ids, geo, g0.w, g0.h, d_ev, ctx->crop.dev(), ctx->crop_planes.dev(), ctx->tensor.dev(), tz, src);
     ++ctx->launches;
   }
   ctx->prof_begin(HT_PROF_TRACK_INIT, st);
@@ -3731,6 +3704,29 @@ extern "C" int ht_selftest_face_tensor(const ht_tracker_event *ev, int cw, int c
 extern "C" void ht_selftest_tensor_pixels(const ht_face_tensor *tensor, const uint32_t *px, int n) {
   const FaceTensor t = tensor_record(*tensor);
   for (int i = 0; i < n; ++i) tensor_put(t, px[i], i, 0);
+}
+// The setters' overlap verdict on n streams' records, addresses as integers: stream s has debug canvas debug[s], face
+// crop crops[s] (RGBA) or yuv[s] (YUV, if crops[s].rgba is NULL), face tensor tensors[s] and camera cameras[s]; a NULL
+// address is none.  -> 1 with the clashing pair's kinds and streams in clash[4] {kind, stream, kind, stream}, or 0.
+extern "C" int ht_selftest_tick_writes(int n, const ht_debug_canvas *debug, const ht_face_crop *crops,
+                                       const ht_face_crop_yuv *yuv, const ht_face_tensor *tensors, void *const *cameras,
+                                       int32_t *clash) {
+  std::vector<DebugCanvas> d((size_t)n);
+  std::vector<FaceCrop> f((size_t)n);
+  std::vector<CropPlanes> q((size_t)n);
+  std::vector<FaceTensor> t((size_t)n);
+  std::vector<CameraCtl> k((size_t)n);
+  for (int s = 0; s < n; ++s) {
+    if (debug[s].rgba) d[s] = debug_record(debug[s]);
+    if (crops[s].rgba) f[s] = crop_record(crops[s]);
+    else if (yuv[s].planes[0]) crop_yuv_record(yuv[s], f[s], q[s]);
+    if (tensors[s].data) t[s] = tensor_record(tensors[s]);
+    k[s].camera = static_cast<ht_camera *>(cameras[s]);
+  }
+  TickWrite c[2];
+  if (!tick_writes_overlap(d, f, q, t, k, c)) return 0;
+  for (int i = 0; i < 2; ++i) clash[2 * i] = c[i].kind, clash[2 * i + 1] = c[i].stream;
+  return 1;
 }
 // rgba_to_yuv420 over n 2 x 2 blocks: blocks[4k..4k+3] = p00, p01, p10, p11 -> out[6k..6k+5] = their Y, U, V
 extern "C" void ht_selftest_rgba_to_yuv420(int color, const uint32_t *blocks, long long n, uint8_t *out) {

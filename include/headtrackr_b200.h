@@ -453,13 +453,12 @@ typedef struct {
  * functions of the tick's ht_tracker_event (streams.debug_calls in the Python package).  The writes are enqueued on the context's stream before a tick's outputs: with host `out` they have landed when the
  * tick returns, with device `out` after ht_sync or in stream order.  ht_tracker_config clears every stream's debug
  * canvas; ht_tracker_set_params does not.
- * Two streams may not share bytes of their debug canvases: the streams of one tick run concurrently and would race,
- * where the reference's timers write one after another.
+ * No two streams' outputs may share bytes: the streams of one tick run concurrently and would race, where the
+ * reference's timers write one after another.
  * Errors (nothing changes): HT_ERR_STATE before ht_tracker_config; HT_ERR_ARG for a range outside [0, max_frames),
  * n <= 0, canvases NULL, a host pointer, a pointer or pitch that is not a multiple of 4, a pitch below 4*width, or a
- * canvas whose byte range overlaps another stream's (over all streams that have a canvas after the call) or any plane
- * of any face crop, RGBA or YUV;
- * HT_ERR_SIZE for a size outside 1..16384. */
+ * canvas that overlaps any debug canvas, crop plane, tensor plane or camera of any stream after the call (the one
+ * rule of ht_tracker_set_face_tensor); HT_ERR_SIZE for a size outside 1..16384. */
 int ht_tracker_set_debug(ht_ctx *ctx, int first, int n, const ht_debug_canvas *canvases);
 
 /* Stream first+i strokes main.js's face rectangles onto its debug canvas (enable[i] == 1) or not (0), for i in
@@ -498,8 +497,8 @@ typedef struct {
  * A tick launches one more kernel while some stream has a crop, and nothing more otherwise.
  * Errors (nothing changes): HT_ERR_STATE before ht_tracker_config; HT_ERR_ARG for a range outside [0, max_frames),
  * n <= 0, crops NULL, a host pointer, a pointer or pitch that is not a multiple of 4, a pitch below 4*width, a scale
- * that is not finite or outside (0, 16], or a crop whose bytes overlap another stream's crop or any debug canvas (over
- * all streams after the call: the streams of a tick run concurrently); HT_ERR_SIZE for a size outside 1..2048. */
+ * that is not finite or outside (0, 16], or a crop that overlaps any debug canvas, crop plane, tensor plane or camera
+ * of any stream after the call (the one rule of ht_tracker_set_face_tensor); HT_ERR_SIZE for a size outside 1..2048. */
 int ht_tracker_set_face_crop(ht_ctx *ctx, int first, int n, const ht_face_crop *crops);
 
 /* A stream's face crop as 4:2:0 video for an encoder: NVENC takes NV12; openh264, libx264, libvpx and WebRTC frame
@@ -538,8 +537,9 @@ typedef struct {
  * Errors (nothing changes; the message names the record): HT_ERR_STATE before ht_tracker_config; HT_ERR_SIZE for a size
  * that is odd or outside 2..2048; HT_ERR_ARG for a range outside [0, max_frames), n <= 0, crops NULL, a format other
  * than NV12 / I420, a colour other than the four above, a missing or extra plane, a host pointer, a pitch below its
- * row's bytes, a non-zero pad_, a scale that is not finite or outside (0, 16], or a plane whose bytes overlap another
- * plane of the crop, another stream's crop of either layout or any debug canvas (over all streams after the call). */
+ * row's bytes, a non-zero pad_, a scale that is not finite or outside (0, 16], or a plane that overlaps any debug
+ * canvas, crop plane (its own crop's other planes included), tensor plane or camera of any stream after the call (the
+ * one rule of ht_tracker_set_face_tensor). */
 int ht_tracker_set_face_crop_yuv(ht_ctx *ctx, int first, int n, const ht_face_crop_yuv *crops);
 
 /* A stream's face tensor: its face as a model's input, a normalised CHW or HWC tensor (DESIGN.md 2, "Face crops", item
@@ -587,9 +587,12 @@ typedef struct {
  * outside 1..2048; HT_ERR_ARG for a range outside [0, max_frames), n <= 0, tensors NULL, a dtype, layout or channels
  * value other than the above, a host pointer, a pointer not aligned to the element size, a stride outside its range
  * above, a non-zero pad_, a mul or add that is not finite, a U8 tensor whose used mul is not 1 or add not 0, a scale
- * that is not finite or outside (0, 16], or a tensor whose bytes - one span per channel plane for CHW, one span for HWC
- * - overlap one another, another stream's tensor, any plane of any face crop or any debug canvas (over all streams
- * after the call).  ht_tracker_set_debug and both crop setters likewise refuse overlap with a tensor. */
+ * that is not finite or outside (0, 16], or a tensor plane that overlaps any debug canvas, crop plane, tensor plane
+ * (its own tensor's others included) or camera of any stream after the call.
+ * That is the one overlap rule of the per-stream outputs, which ht_tracker_set_debug, both crop setters and
+ * ht_tracker_set_camera apply too: the streams of a tick run concurrently, so no two of the byte spans a tick writes
+ * may share a byte.  The spans: each debug canvas, (height-1)*pitch + 4*width bytes; each plane of each face crop,
+ * RGBA or YUV; each channel plane of a CHW tensor, or the whole of an HWC tensor; each camera, HT_CAMERA_BYTES. */
 int ht_tracker_set_face_tensor(ht_ctx *ctx, int first, int n, const ht_face_tensor *tensors);
 
 /* The map of the crop `crop` (its size and scale; rgba and pitch are ignored; a YUV crop has the map of the RGBA crop of
@@ -648,10 +651,10 @@ typedef struct {
  * ht_tracker_config removes every controller; ht_tracker_set_params does not.  A tick launches one more kernel while
  * some stream has a controller, and nothing more otherwise.
  * Errors (nothing changes): HT_ERR_STATE before ht_tracker_config; HT_ERR_ARG for a range outside [0, max_frames),
- * n <= 0, controls NULL, a camera that is host memory, memory of another device or not 16-byte aligned, two streams
- * whose cameras share bytes (over all streams that have one after the call: the streams of a tick run concurrently),
- * a non-finite field, aspect <= 0, near <= 0, far <= near, fov outside (0, 180), or a degenerate lookAt (fixed_position
- * == look_at, or a view direction parallel to +y). */
+ * n <= 0, controls NULL, a camera that is host memory, memory of another device or not 16-byte aligned, a camera that
+ * overlaps any debug canvas, crop plane, tensor plane or camera of any stream after the call (the one rule of
+ * ht_tracker_set_face_tensor), a non-finite field, aspect <= 0, near <= 0, far <= near, fov outside (0, 180), or a
+ * degenerate lookAt (fixed_position == look_at, or a view direction parallel to +y). */
 int ht_tracker_set_camera(ht_ctx *ctx, int first, int n, const ht_camera_control *controls);
 
 /* Tracker records: a stream's whole headtrackr.Tracker as one fixed-size, position-independent, little-endian byte

@@ -490,3 +490,60 @@ def test_rejections_change_nothing():
         assert raw(ctx, 0, [cc(base)]) == 0
     finally:
         ctx.close()
+
+
+def test_cameras_and_images_share_no_byte():
+    """A camera is bytes the tick writes, like a debug canvas, a face crop or a face tensor: a camera on any of them,
+    and any of them on a camera, is refused, and the outputs in force stay as they were."""
+    T = torch()
+    mf = 4
+    ctx = Context(max_width=160, max_height=120, max_frames=mf)
+    buf = T.zeros(64 * NB, dtype=T.uint8, device="cuda")
+    base = buf.data_ptr()
+    regions = [(0, 1024), (2048, 3072), (4096, 5120), (8192, 8192 + NB)]     # canvas, crop, tensor, camera
+    try:
+        ctx.tracker_config()
+        ctx.tracker_reset(0, mf)
+        ctx.tracker_start(0, mf)
+        ctx.tracker_set_debug(0, [buf[0:1024].view(16, 16, 4)])
+        ctx.tracker_set_face_crop(1, [dict(out=buf[2048:3072].view(16, 16, 4))])
+        ctx.tracker_set_face_tensor(2, [dict(out=buf[4096:5120].view(T.float32).view(1, 16, 16), channels="gray")])
+        ctx.tracker_set_camera(3, [dict(CONTROL, out=buf[8192:8192 + NB])])
+        for t in range(30):
+            ctx.tracker_feed(range(mf), [face(t)] * mf, 1.0e12 + 35.0 * t, 160, 120)
+        L, h = ctx._L, ctx._h
+        canvas = (_lib.DebugCanvas * 1)(_lib.DebugCanvas(base + 8192 - 64, 8, 4, 0, 0))
+        crop = (_lib.FaceCrop * 1)(_lib.FaceCrop(base + 8192 + NB - 32, 4, 4, 0, 0, 1.0))
+        tensor = (_lib.FaceTensor * 1)(_lib.FaceTensor(base + 8192 - 32, 4, 0, 4, 4, _lib.HT_TENSOR_F32, _lib.HT_TENSOR_CHW,
+                                                       _lib.HT_TENSOR_GRAY, 0, (1.0,) * 3, (0.0,) * 3, 1.0))
+        cases = [
+            ("camera on the canvas", lambda: raw(ctx, 0, [cc(base + 512)])),
+            ("camera on the crop", lambda: raw(ctx, 0, [cc(base + 2048 + 512)])),
+            ("camera on the tensor", lambda: raw(ctx, 0, [cc(base + 4096 + 1024 - 16)])),
+            ("canvas on the camera", lambda: L.ht_tracker_set_debug(h, 3, 1, C.addressof(canvas))),
+            ("crop on the camera", lambda: L.ht_tracker_set_face_crop(h, 1, 1, C.addressof(crop))),
+            ("tensor on the camera", lambda: L.ht_tracker_set_face_tensor(h, 2, 1, C.addressof(tensor))),
+        ]
+        for name, call in cases:
+            T.cuda.synchronize()
+            before = buf.clone()
+            assert call() == HT_ERR_ARG, (name, L.ht_last_error(h))
+            assert "overlaps" in L.ht_last_error(h).decode(), name
+            T.cuda.synchronize()
+            assert T.equal(buf, before), name
+        # every output still in force, and nothing written outside them
+        events = camera_from_bytes(buf[8192:8192 + NB])["events"]
+        buf[:8192].zero_()                                # the camera keeps its state
+        buf[8192 + NB:].zero_()
+        T.cuda.synchronize()
+        for t in range(30, 36):
+            ctx.tracker_feed(range(mf), [face(t)] * mf, 1.0e12 + 35.0 * t, 160, 120)
+        T.cuda.synchronize()
+        assert all(buf[a:b].any() for a, b in regions[:3])
+        assert camera_from_bytes(buf[8192:8192 + NB])["events"] > events > 0
+        outside = T.ones_like(buf, dtype=T.bool)
+        for a, b in regions:
+            outside[a:b] = False
+        assert not buf[outside].any()
+    finally:
+        ctx.close()

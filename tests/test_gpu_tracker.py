@@ -6,7 +6,7 @@ import numpy as np
 import pytest
 
 from headtrackr_b200 import Context
-from headtrackr_b200._lib import HT_ERR_STATE, HtError
+from headtrackr_b200._lib import HT_ERR_ARG, HT_ERR_STATE, HtError
 from headtrackr_b200.streams import TrackerSet
 from test_host_lifecycle import GOLD_L, case_spec, make_frame, strip_time
 from test_host_main import GOLD_M, check_events, same
@@ -111,3 +111,21 @@ def replay(batch, io):
 @pytest.mark.parametrize("batch", list(BATCHES))
 def test_tracker_step_replays_main_js_from_frame_0(batch, io):
     replay(batch, io)
+
+
+def test_stream_ranges_past_int_max_are_refused():
+    """A stream range whose end overflows int is outside [0, max_frames) like any other: ht_stream_reset and
+    ht_tracker_reset / start / stop refuse it, and the tracker states stay as they were."""
+    c = Context(max_width=W, max_height=H, max_frames=4)
+    try:
+        c.tracker_config()
+        c.tracker_reset(0, 4)
+        c.tracker_start(0, 2)
+        states = c.tracker_export(list(range(4)))
+        for fn in ("ht_stream_reset", "ht_tracker_reset", "ht_tracker_start", "ht_tracker_stop"):
+            for first, n in ((2**31 - 1, 1), (1, 2**31 - 1), (3, 2), (-1, 1), (0, 0)):
+                assert getattr(c._L, fn)(c._h, first, n) == HT_ERR_ARG, (fn, first, n)
+                assert c._L.ht_last_error(c._h).decode() == "stream range outside [0,4)", (fn, first, n)
+        assert np.array_equal(c.tracker_export(list(range(4))), states)
+    finally:
+        c.close()
