@@ -169,6 +169,28 @@ class CameraControl(C.Structure):
 CAMERA_BYTES = 224
 assert C.sizeof(Camera) == CAMERA_BYTES and C.sizeof(CameraControl) == 112
 
+# ht_framing.outputs
+HT_FRAMING_CROP, HT_FRAMING_TENSOR = 1, 2
+
+
+class FramedBox(C.Structure):
+    """ht_framed_box: a stream's framed box, the state of its framing (FRAMED_BOX_BYTES, in device memory;
+    framing.box_from_bytes decodes it)"""
+    _fields_ = [("cx", C.c_double), ("cy", C.c_double), ("width", C.c_double), ("height", C.c_double),
+                ("canvas_w", C.c_int32), ("canvas_h", C.c_int32), ("updates", C.c_uint32), ("valid", C.c_int32)]
+
+
+class Framing(C.Structure):
+    """ht_framing: one stream's framing for ht_tracker_set_framing (box NULL = none; alpha in (0, 1]; dead_zone in
+    [0, 0.5]; outputs a nonzero mask of HT_FRAMING_CROP | HT_FRAMING_TENSOR)"""
+    _fields_ = [("box", C.c_void_p), ("alpha", C.c_double), ("dead_zone", C.c_double), ("outputs", C.c_int32),
+                ("pad_", C.c_int32)]
+
+
+FRAMED_BOX_BYTES = 48
+assert C.sizeof(FramedBox) == FRAMED_BOX_BYTES and FramedBox.canvas_w.offset == 32 and FramedBox.valid.offset == 44 \
+    and C.sizeof(Framing) == 32 and Framing.outputs.offset == 24
+
 # ht_tracker_export / ht_tracker_import: bytes of one tracker record (HT_TRACKER_RECORD_BYTES)
 TRACKER_RECORD_BYTES = 16864
 
@@ -212,7 +234,7 @@ _lib = None
 
 EXPORTS = ["ht_version", "ht_create", "ht_destroy", "ht_last_error", "ht_sync", "ht_max_rects", "ht_detect",
            "ht_track_init", "ht_track_init_from_detect", "ht_track", "ht_detect_track", "ht_stream_reset", "ht_stream_step", "ht_stream_head_config", "ht_stream_step_head",
-           "ht_tracker_config", "ht_tracker_reset", "ht_tracker_start", "ht_tracker_stop", "ht_tracker_step", "ht_tracker_feed", "ht_tracker_set_params", "ht_tracker_feed_canvases", "ht_tracker_set_debug", "ht_tracker_set_debug_strokes", "ht_tracker_set_face_crop", "ht_tracker_set_face_crop_yuv", "ht_tracker_set_face_tensor", "ht_face_crop_map", "ht_tracker_set_camera", "ht_tracker_export", "ht_tracker_import", "ht_tracker_feed_yuv", "ht_ingest", "ht_ingest_yuv",
+           "ht_tracker_config", "ht_tracker_reset", "ht_tracker_start", "ht_tracker_stop", "ht_tracker_step", "ht_tracker_feed", "ht_tracker_set_params", "ht_tracker_feed_canvases", "ht_tracker_set_debug", "ht_tracker_set_debug_strokes", "ht_tracker_set_face_crop", "ht_tracker_set_face_crop_yuv", "ht_tracker_set_face_tensor", "ht_face_crop_map", "ht_tracker_set_framing", "ht_face_crop_map_framed", "ht_tracker_set_camera", "ht_tracker_export", "ht_tracker_import", "ht_tracker_feed_yuv", "ht_ingest", "ht_ingest_yuv",
            "ht_tracker_feed_views", "ht_tracker_feed_yuv_views", "ht_ingest_views", "ht_ingest_yuv_views", "ht_backprojection", "ht_whitebalance",
            "ht_plan_info", "ht_debug_plane", "ht_debug_raw", "ht_debug_model_hist", "ht_debug_track_stats", "ht_set_track_memo", "ht_set_pipeline", "ht_join", "ht_debug_set_exactness", "ht_debug_track_trace", "ht_debug_track_phases", "ht_launch_count",
            "ht_profile", "ht_profile_read"]
@@ -262,6 +284,8 @@ def lib():
     L.ht_tracker_set_face_crop_yuv.argtypes = [vp, C.c_int, C.c_int, vp]
     L.ht_tracker_set_face_tensor.argtypes = [vp, C.c_int, C.c_int, vp]
     L.ht_face_crop_map.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp]
+    L.ht_tracker_set_framing.argtypes = [vp, C.c_int, C.c_int, vp]
+    L.ht_face_crop_map_framed.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp]
     L.ht_tracker_set_camera.argtypes = [vp, C.c_int, C.c_int, vp]
     L.ht_tracker_export.argtypes = [vp, vp, C.c_int, vp]
     L.ht_tracker_import.argtypes = [vp, vp, C.c_int, vp]

@@ -8,7 +8,7 @@ import math
 
 import numpy as np
 
-from . import _lib
+from . import _lib, framing
 from ._lib import (Camera, CameraControl, CanvasFrame, DebugCanvas, FaceCrop, FaceCropYuv, FaceTensor, HeadEvent, HeadParams, HtError, Rect, StreamEvent, TrackerEvent, TrackerParams, TrackObj, VideoFrame,
                    VideoView, Window, YuvFrame, YuvImage)
 from .views import video_view
@@ -621,6 +621,34 @@ class Context:
                                    float(d["near"]), float(d["far"]))
         self._check(self._L.ht_tracker_set_camera(self._h, int(first), len(controls), C.addressof(arr)))
         self._keep("camera", int(first), [None if d is None else d["out"] for d in controls])
+
+    def tracker_set_framing(self, first, framings):
+        """Framings of streams first, first+1, ... (ht_tracker_set_framing): per stream None (none) or a dict {"out":
+        torch CUDA uint8 tensor of FRAMED_BOX_BYTES bytes, 8-byte aligned, on this context's device; "alpha": 0.25;
+        "dead_zone": 0.1; "crop": True; "tensor": False}.  `out` holds the framed box, a steady face-cam box: on every
+        tick that writes crops it snaps to the tracked face when the face has left it (or on the first such tick, or
+        a canvas-size change) and otherwise glides towards it by `alpha` of the error outside a dead zone of
+        `dead_zone` times its size (DESIGN.md 2, "Face crops", item 7; framing.py replays it on the host and
+        box_from_bytes decodes it).  The face crop ("crop") and / or the face tensor ("tensor") are then cut upright
+        from the framed box, the others from the tracked one.  Setting a framing starts its box anew.  The framing is
+        the stream's: it outlives set_params, stop, start, reset and import; tracker_config removes it.  The context
+        keeps the tensors alive while they are set."""
+        framings = list(framings)
+        arr = (_lib.Framing * max(1, len(framings)))()
+        for i, d in enumerate(framings):
+            if d is None:
+                continue
+            t = d["out"]
+            if not _is_torch(t) or not t.is_cuda:
+                raise ValueError("a framed box is a torch CUDA tensor")
+            if t.element_size() != 1 or t.numel() != _lib.FRAMED_BOX_BYTES or not t.is_contiguous():
+                raise ValueError(f"a framed box is a contiguous uint8 tensor of {_lib.FRAMED_BOX_BYTES} bytes")
+            outputs = (_lib.HT_FRAMING_CROP if d.get("crop", True) else 0) | \
+                (_lib.HT_FRAMING_TENSOR if d.get("tensor", False) else 0)
+            arr[i] = _lib.Framing(t.data_ptr(), float(d.get("alpha", framing.ALPHA)),
+                                  float(d.get("dead_zone", framing.DEAD_ZONE)), outputs, 0)
+        self._check(self._L.ht_tracker_set_framing(self._h, int(first), len(framings), C.addressof(arr)))
+        self._keep("framing", int(first), [None if d is None else d["out"] for d in framings])
 
     def tracker_export(self, streams, out=None):
         """The tracker records of the listed streams (ht_tracker_export): a (len(streams), TRACKER_RECORD_BYTES) uint8

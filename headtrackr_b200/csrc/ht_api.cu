@@ -610,11 +610,12 @@ struct ht_ctx {
   StreamTable<FaceCrop> crop;
   StreamTable<CropPlanes> crop_planes;
   StreamTable<FaceTensor> tensor;
+  StreamTable<ht_framing> framing;          // ht_tracker_set_framing
   DevBuf d_debug_tab;
   // what a tick launches for them, from the tables (count_outputs): the streams with a debug canvas, with a canvas and
-  // strokes on, with a camera, with a crop and with a tensor (0: no launch for them), and the tiles of the largest
-  // crop and tensor (k_face_crop's grid.x)
-  int debug_count = 0, stroke_count = 0, camera_count = 0;
+  // strokes on, with a camera, with a crop, with a tensor and with a framing (0: no launch for them), and the tiles
+  // of the largest crop and tensor (k_face_crop's grid.x)
+  int debug_count = 0, stroke_count = 0, camera_count = 0, framing_count = 0;
   int crop_count = 0, crop_tiles = 0, tensor_count = 0, tensor_tiles = 0;
   // ht_tracker_feed(_canvases): the record table {ids[n], clocks[n], FeedRec[n], EntryCanvas[n], tile starts[n+1]}
   // goes up in one copy from pinned memory; the videos are drawn into the canvas arena (batch entry k's canvas at
@@ -1791,13 +1792,14 @@ static bool tracker_params_ok(const ht_tracker_params &p) {
 // What a tick launches for the per-stream outputs, from their tables: after every change to a table
 static void count_outputs(ht_ctx *ctx) {
   const auto tiles = [](int w, int h) { return ((w + CROP_TX - 1) / CROP_TX) * ((h + CROP_TY - 1) / CROP_TY); };
-  ctx->debug_count = ctx->stroke_count = ctx->camera_count = 0;
+  ctx->debug_count = ctx->stroke_count = ctx->camera_count = ctx->framing_count = 0;
   ctx->crop_count = ctx->crop_tiles = ctx->tensor_count = ctx->tensor_tiles = 0;
   for (const DebugCanvas &d : ctx->debug.h) {
     ctx->debug_count += d.rgba != nullptr;
     ctx->stroke_count += d.rgba != nullptr && d.strokes;
   }
   for (const CameraCtl &k : ctx->camera.h) ctx->camera_count += k.camera != nullptr;
+  for (const ht_framing &g : ctx->framing.h) ctx->framing_count += g.box != nullptr;
   for (const FaceCrop &f : ctx->crop.h)
     if (f.rgba) {
       ++ctx->crop_count;
@@ -1816,9 +1818,10 @@ int ht_tracker_config(ht_ctx *ctx, const ht_tracker_params *params) {
   CK(cudaSetDevice(ctx->cfg.device));
   const size_t mf = (size_t)ctx->cfg.max_frames;
   if (params && !tracker_params_ok(*params)) return ctx->fail(HT_ERR_ARG, "bad head parameters");
-  // either form discards every stream's debug canvas and stroke flag, camera, face crop and face tensor
+  // either form discards every stream's debug canvas and stroke flag, camera, face crop, face tensor and framing
   CK(ctx->debug.clear(ctx->stream));
   CK(ctx->camera.clear(ctx->stream));
+  CK(ctx->framing.clear(ctx->stream));
   CK(ctx->crop.clear(ctx->stream));
   CK(ctx->crop_planes.clear(ctx->stream));
   CK(ctx->tensor.clear(ctx->stream));
@@ -1875,18 +1878,19 @@ static_assert(sizeof(ht_debug_canvas) == 24 && sizeof(DebugCanvas) == sizeof(ht_
               "ht_debug_canvas layout");
 
 // The kinds of byte range a tick writes for a stream, as the overlap messages name them
-enum { OUT_DEBUG, OUT_CROP, OUT_TENSOR, OUT_CAMERA };
-static const char *const OUT_NAME[] ={"debug canvas", "face crop plane", "face tensor plane", "camera"};
+enum { OUT_DEBUG, OUT_CROP, OUT_TENSOR, OUT_CAMERA, OUT_FRAMING };
+static const char *const OUT_NAME[] ={"debug canvas", "face crop plane", "face tensor plane", "camera", "framed box"};
 
 // One byte range [start, end) that a tick writes: part of the `kind` output of stream `stream`
 struct TickWrite { uintptr_t start, end; int kind, stream; };
 
 // Whether two of the byte ranges a tick writes share a byte (the streams of a tick run concurrently): each debug
 // canvas (one span over its rows), each plane of each face crop, each channel plane (CHW) or whole tensor (HWC) of
-// each face tensor, and each camera.  The first clashing pair in order of start goes to clash[0..1].
+// each face tensor, each camera, and each framed box.  The first clashing pair in order of start goes to clash[0..1].
 static bool tick_writes_overlap(const std::vector<DebugCanvas> &debug, const std::vector<FaceCrop> &crop,
                                 const std::vector<CropPlanes> &crop_planes, const std::vector<FaceTensor> &tensor,
-                                const std::vector<CameraCtl> &camera, TickWrite clash[2]) {
+                                const std::vector<CameraCtl> &camera, const std::vector<ht_framing> &framing,
+                                TickWrite clash[2]) {
   std::vector<TickWrite> w;
   const auto add = [&](const void *p, size_t rows, size_t pitch, size_t row_bytes, int kind, size_t s) {
     const uintptr_t a = reinterpret_cast<uintptr_t>(p);
@@ -1927,6 +1931,8 @@ static bool tick_writes_overlap(const std::vector<DebugCanvas> &debug, const std
   }
   for (size_t s = 0; s < camera.size(); ++s)
     if (camera[s].camera) add(camera[s].camera, 1, 0, sizeof(ht_camera), OUT_CAMERA, s);
+  for (size_t s = 0; s < framing.size(); ++s)
+    if (framing[s].box) add(framing[s].box, 1, 0, sizeof(ht_framed_box), OUT_FRAMING, s);
   std::sort(w.begin(), w.end(), [](const TickWrite &a, const TickWrite &b) { return a.start < b.start; });
   for (size_t i = 1; i < w.size(); ++i)
     if (w[i].start < w[i - 1].end) {
@@ -1945,18 +1951,19 @@ struct OutputEdit {
   std::vector<FaceCrop> *crop = nullptr;
   std::vector<CropPlanes> *crop_planes = nullptr;
   std::vector<FaceTensor> *tensor = nullptr;
+  std::vector<ht_framing> *framing = nullptr;
 };
 
 // How every setter's records reach the tick.  The call is refused if two byte ranges a tick would write share a byte
 // (the tables before it share none, so a clash takes in one of its records, which the message names).  Otherwise
-// streams [first, first + n) of the edited tables go to the device, a new camera is constructed there, and the tables
-// and the tick's counts follow.
+// streams [first, first + n) of the edited tables go to the device, a new camera is constructed there, a new framed
+// box is made invalid there, and the tables and the tick's counts follow.
 static int commit_outputs(ht_ctx *ctx, int first, int n, const OutputEdit &e) {
-  const int kind = e.debug ? OUT_DEBUG : e.crop ? OUT_CROP : e.tensor ? OUT_TENSOR : OUT_CAMERA;
+  const int kind = e.debug ? OUT_DEBUG : e.crop ? OUT_CROP : e.tensor ? OUT_TENSOR : e.framing ? OUT_FRAMING : OUT_CAMERA;
   TickWrite c[2];
   if (tick_writes_overlap(e.debug ? *e.debug : ctx->debug.h, e.crop ? *e.crop : ctx->crop.h,
                           e.crop_planes ? *e.crop_planes : ctx->crop_planes.h, e.tensor ? *e.tensor : ctx->tensor.h,
-                          e.camera ? *e.camera : ctx->camera.h, c)) {
+                          e.camera ? *e.camera : ctx->camera.h, e.framing ? *e.framing : ctx->framing.h, c)) {
     const int own = c[0].kind == kind && c[0].stream >= first && c[0].stream - first < n ? 0 : 1;
     return ctx->fail(HT_ERR_ARG, "record %d: its %s overlaps the %s of stream %d", c[own].stream - first,
                      OUT_NAME[c[own].kind], OUT_NAME[c[1 - own].kind], c[1 - own].stream);
@@ -1985,9 +1992,16 @@ static int commit_outputs(ht_ctx *ctx, int first, int n, const OutputEdit &e) {
     ++ctx->launches;
     CK(cudaGetLastError());
   }
+  if (e.framing) {
+    CK(ctx->framing.commit(*e.framing, first, n, st));
+    k_framing_reset<<<1, 256, 0, st>>>(ctx->framing.dev(), first, n);
+    ++ctx->launches;
+    CK(cudaGetLastError());
+  }
   CK(cudaStreamSynchronize(st));    // the edited tables are the setter's locals
   if (e.debug) ctx->debug.h.swap(*e.debug);
   if (e.camera) ctx->camera.h.swap(*e.camera);
+  if (e.framing) ctx->framing.h.swap(*e.framing);
   if (e.crop) {
     ctx->crop.h.swap(*e.crop);
     ctx->crop_planes.h.swap(*e.crop_planes);
@@ -2211,30 +2225,60 @@ static int view_record(const ht_video_view &view, int w, int h, ViewFeedRec &v, 
 
 // The map k_face_crop uses for `ev`, in the video's tap coordinates: crop_map's values in the source rectangle, taken
 // through the view's signed permutation exactly.
-int ht_face_crop_map(const ht_tracker_event *ev, int canvas_w, int canvas_h, int video_w, int video_h,
-                     const ht_video_view *view, const ht_face_crop *crop, int64_t out[6]) {
-  if (!ev || !crop || !out) return HT_ERR_ARG;
+static void map_to_video(const ViewFeedRec &v, const long long M[6], int64_t out[6]);
+
+// The checks of ht_face_crop_map(_framed) past the record, and the view record v -> HT_OK or the error code
+static int crop_map_args(const ht_face_crop *crop, const int64_t *out, int canvas_w, int canvas_h, int video_w,
+                         int video_h, const ht_video_view *view, ViewFeedRec &v) {
+  if (!crop || !out) return HT_ERR_ARG;
   if (canvas_w < 1 || canvas_h < 1 || canvas_w > 16384 || canvas_h > 16384 || video_w < 1 || video_h < 1 ||
       video_w > 16384 || video_h > 16384 || crop->width < 1 || crop->height < 1 || crop->width > 2048 || crop->height > 2048)
     return HT_ERR_SIZE;
   if (!(crop->scale > 0.0 && crop->scale <= 16.0)) return HT_ERR_ARG;
   const ht_video_view whole{};
-  ViewFeedRec v{};
   char why[256];
-  if (view_record(view ? *view : whole, video_w, video_h, v, why) != HT_OK) return HT_ERR_ARG;
+  return view_record(view ? *view : whole, video_w, video_h, v, why) != HT_OK ? HT_ERR_ARG : HT_OK;
+}
+
+int ht_face_crop_map(const ht_tracker_event *ev, int canvas_w, int canvas_h, int video_w, int video_h,
+                     const ht_video_view *view, const ht_face_crop *crop, int64_t out[6]) {
+  if (!ev) return HT_ERR_ARG;
+  ViewFeedRec v{};
+  const int rc = crop_map_args(crop, out, canvas_w, canvas_h, video_w, video_h, view, v);
+  if (rc != HT_OK) return rc;
   const TrackerEvent &e = *reinterpret_cast<const TrackerEvent *>(ev);
   long long M[6];
   for (int i = 0; i < 6; ++i) out[i] = 0;
   if (!crop_map(e.detection, e.x, e.y, e.width, e.height, e.angle, canvas_w, canvas_h, v.sw, v.sh, crop->width, crop->height,
                 crop->scale, M))
     return 0;
+  map_to_video(v, M, out);
+  return 1;
+}
+
+// The map k_face_crop uses for a framed crop cut from `box`, as ht_face_crop_map's
+int ht_face_crop_map_framed(const ht_framed_box *box, int canvas_w, int canvas_h, int video_w, int video_h,
+                            const ht_video_view *view, const ht_face_crop *crop, int64_t out[6]) {
+  if (!box) return HT_ERR_ARG;
+  ViewFeedRec v{};
+  const int rc = crop_map_args(crop, out, canvas_w, canvas_h, video_w, video_h, view, v);
+  if (rc != HT_OK) return rc;
+  long long M[6];
+  for (int i = 0; i < 6; ++i) out[i] = 0;
+  if (!crop_map_framed(*box, canvas_w, canvas_h, v.sw, v.sh, crop->width, crop->height, crop->scale, M)) return 0;
+  map_to_video(v, M, out);
+  return 1;
+}
+
+// crop_map's values M, in the source rectangle of view record v, in the video's tap coordinates: taken through the
+// view's signed permutation exactly
+static void map_to_video(const ViewFeedRec &v, const long long M[6], int64_t out[6]) {
   out[0] = 65536LL * v.bx + v.mxx * M[0] + v.mxy * M[1];
   out[1] = 65536LL * v.by + v.myx * M[0] + v.myy * M[1];
   for (int s = 2; s < 6; s += 2) {
     out[s] = v.mxx * M[s] + v.mxy * M[s + 1];
     out[s + 1] = v.myx * M[s] + v.myy * M[s + 1];
   }
-  return 1;
 }
 
 static_assert(sizeof(ht_camera) == HT_CAMERA_BYTES && HT_CAMERA_BYTES == 224 && offsetof(ht_camera, fov) == 24 &&
@@ -2292,6 +2336,52 @@ int ht_tracker_set_camera(ht_ctx *ctx, int first, int n, const ht_camera_control
   }
   OutputEdit e;
   e.camera = &next;
+  return commit_outputs(ctx, first, n, e);
+}
+
+static_assert(sizeof(ht_framed_box) == HT_FRAMED_BOX_BYTES && HT_FRAMED_BOX_BYTES == 48 &&
+                  offsetof(ht_framed_box, width) == 16 && offsetof(ht_framed_box, canvas_w) == 32 &&
+                  offsetof(ht_framed_box, updates) == 40 && offsetof(ht_framed_box, valid) == 44 &&
+                  sizeof(ht_framing) == 32 && offsetof(ht_framing, alpha) == 8 && offsetof(ht_framing, dead_zone) == 16 &&
+                  offsetof(ht_framing, outputs) == 24 && offsetof(ht_framing, pad_) == 28,
+              "ht_framed_box / ht_framing layout (include/headtrackr_b200.h)");
+
+// One framing's fields past its box -> NULL, or what is wrong with them
+static const char *framing_check(const ht_framing &g) {
+  if (!(g.alpha > 0.0 && g.alpha <= 1.0)) return "alpha outside (0, 1]";
+  if (!(g.dead_zone >= 0.0 && g.dead_zone <= 0.5)) return "dead_zone outside [0, 0.5]";
+  if (g.outputs == 0 || (g.outputs & ~(HT_FRAMING_CROP | HT_FRAMING_TENSOR)))
+    return "outputs is not a nonzero mask of HT_FRAMING_CROP and HT_FRAMING_TENSOR";
+  if (g.pad_ != 0) return "pad_ is not 0";
+  return nullptr;
+}
+
+// The framings of streams [first, first + n).  Everything is checked on the host before anything changes; then one
+// launch makes the new boxes invalid.
+int ht_tracker_set_framing(ht_ctx *ctx, int first, int n, const ht_framing *framings) {
+  { const int ar = tracker_streams(ctx, first, n); if (ar != HT_OK) return ar; }
+  if (!framings) return ctx->fail(HT_ERR_ARG, "framings is NULL");
+  std::vector<ht_framing> next = ctx->framing.edit(ctx->cfg.max_frames);
+  for (int i = 0; i < n; ++i) {
+    const ht_framing &g = framings[i];
+    ht_framing k{};
+    if (g.box) {
+      if (reinterpret_cast<uintptr_t>(g.box) & 7u) return ctx->fail(HT_ERR_ARG, "record %d: box must be 8-byte aligned", i);
+      cudaPointerAttributes a{};
+      if (cudaPointerGetAttributes(&a, g.box) != cudaSuccess) { cudaGetLastError(); a.type = cudaMemoryTypeUnregistered; }
+      if (a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged)
+        return ctx->fail(HT_ERR_ARG, "record %d: box is not device memory", i);
+      if (a.device != ctx->cfg.device)
+        return ctx->fail(HT_ERR_ARG, "record %d: box is memory of device %d, the context is on device %d", i, a.device,
+                         ctx->cfg.device);
+      const char *why = framing_check(g);
+      if (why) return ctx->fail(HT_ERR_ARG, "record %d: %s", i, why);
+      k = g;
+    }
+    next[(size_t)(first + i)] = k;
+  }
+  OutputEdit e;
+  e.framing = &next;
   return commit_outputs(ctx, first, n, e);
 }
 
@@ -2519,6 +2609,10 @@ static int tracker_tick(ht_ctx *ctx, const TickGroup *grp, int n_groups, const u
     k_camera_update<<<(n + 127) / 128, 128, 0, st>>>(d_ids, geo, n, d_ev, ctx->camera.dev());
     ++ctx->launches;
   }
+  if (ctx->framing_count > 0) {   // the framed boxes of the entries whose record is a crop tick, before their crops
+    k_framing_update<<<(n + 127) / 128, 128, 0, st>>>(d_ids, geo, n, g0.w, g0.h, d_ev, ctx->framing.dev());
+    ++ctx->launches;
+  }
   if (ctx->stroke_count > 0) {   // main.js's strokes, after this tick's back-projections (src/main.js:199-219)
     k_debug_strokes<<<(unsigned)n, 256, 0, st>>>(d_ids, geo, d_ev, ctx->debug.dev());
     ++ctx->launches;
@@ -2532,7 +2626,8 @@ static int tracker_tick(ht_ctx *ctx, const TickGroup *grp, int n_groups, const u
     const int tz = ctx->crop_count > 0 ? 1 : 0;           // the tensor slice (unreached without tensors)
     const unsigned slices = (unsigned)(tz + (ctx->tensor_count > 0 ? 1 : 0));
     k_face_crop<<<dim3((unsigned)std::max(ctx->crop_tiles, ctx->tensor_tiles), (unsigned)n, slices), 256, 0, st>>>(
-        d_ids, geo, g0.w, g0.h, d_ev, ctx->crop.dev(), ctx->crop_planes.dev(), ctx->tensor.dev(), tz, src);
+        d_ids, geo, g0.w, g0.h, d_ev, ctx->crop.dev(), ctx->crop_planes.dev(), ctx->tensor.dev(), tz, src,
+        ctx->framing_count > 0 ? ctx->framing.dev() : nullptr);
     ++ctx->launches;
   }
   ctx->prof_begin(HT_PROF_TRACK_INIT, st);
@@ -3706,11 +3801,12 @@ extern "C" void ht_selftest_tensor_pixels(const ht_face_tensor *tensor, const ui
   for (int i = 0; i < n; ++i) tensor_put(t, px[i], i, 0);
 }
 // The setters' overlap verdict on n streams' records, addresses as integers: stream s has debug canvas debug[s], face
-// crop crops[s] (RGBA) or yuv[s] (YUV, if crops[s].rgba is NULL), face tensor tensors[s] and camera cameras[s]; a NULL
-// address is none.  -> 1 with the clashing pair's kinds and streams in clash[4] {kind, stream, kind, stream}, or 0.
-extern "C" int ht_selftest_tick_writes(int n, const ht_debug_canvas *debug, const ht_face_crop *crops,
-                                       const ht_face_crop_yuv *yuv, const ht_face_tensor *tensors, void *const *cameras,
-                                       int32_t *clash) {
+// crop crops[s] (RGBA) or yuv[s] (YUV, if crops[s].rgba is NULL), face tensor tensors[s], camera cameras[s] and framed
+// box boxes[s] (boxes NULL: none); a NULL address is none.  -> 1 with the clashing pair's kinds and streams in
+// clash[4] {kind, stream, kind, stream}, or 0.
+extern "C" int ht_selftest_tick_writes_framed(int n, const ht_debug_canvas *debug, const ht_face_crop *crops,
+                                              const ht_face_crop_yuv *yuv, const ht_face_tensor *tensors,
+                                              void *const *cameras, void *const *boxes, int32_t *clash) {
   std::vector<DebugCanvas> d((size_t)n);
   std::vector<FaceCrop> f((size_t)n);
   std::vector<CropPlanes> q((size_t)n);
@@ -3723,9 +3819,43 @@ extern "C" int ht_selftest_tick_writes(int n, const ht_debug_canvas *debug, cons
     if (tensors[s].data) t[s] = tensor_record(tensors[s]);
     k[s].camera = static_cast<ht_camera *>(cameras[s]);
   }
+  std::vector<ht_framing> g((size_t)n);
+  for (int s = 0; s < n && boxes; ++s) g[s].box = static_cast<ht_framed_box *>(boxes[s]);
   TickWrite c[2];
-  if (!tick_writes_overlap(d, f, q, t, k, c)) return 0;
+  if (!tick_writes_overlap(d, f, q, t, k, g, c)) return 0;
   for (int i = 0; i < 2; ++i) clash[2 * i] = c[i].kind, clash[2 * i + 1] = c[i].stream;
+  return 1;
+}
+// ... without framed boxes
+extern "C" int ht_selftest_tick_writes(int n, const ht_debug_canvas *debug, const ht_face_crop *crops,
+                                       const ht_face_crop_yuv *yuv, const ht_face_tensor *tensors, void *const *cameras,
+                                       int32_t *clash) {
+  return ht_selftest_tick_writes_framed(n, debug, crops, yuv, tensors, cameras, nullptr, clash);
+}
+// framing_step on the host, as k_framing_update runs it: record `ev` on a cw x ch canvas moves *box.  -> 1 on a crop
+// tick, 0 otherwise (the box unchanged); -1 for a framing ht_tracker_set_framing rejects
+extern "C" int ht_selftest_framing_step(ht_framed_box *box, double alpha, double dead_zone, const ht_tracker_event *ev,
+                                        int cw, int ch) {
+  ht_framing g{box, alpha, dead_zone, HT_FRAMING_CROP, 0};
+  if (framing_check(g)) return -1;
+  const TrackerEvent &e = *reinterpret_cast<const TrackerEvent *>(ev);
+  return framing_step(*box, alpha, dead_zone, e.detection, e.x, e.y, e.width, e.height, e.angle, cw, ch) ? 1 : 0;
+}
+// k_face_crop's per-crop code for a crop cut from framed box `box`: an RGBA8 frame of rows of `pitch` bytes (0:
+// 4 * width) through a view (NULL: the whole frame upright) on a cw x ch canvas -> 1 if the box made the crop, 0 if not
+extern "C" int ht_selftest_face_crop_framed_rgba(const ht_framed_box *box, int cw, int ch, const ht_video_frame *fr,
+                                                 const ht_video_view *view, const ht_face_crop *crop) {
+  ViewFeedRec v;
+  char why[256];
+  const ht_video_view whole{};
+  const int rc = view_record(view ? *view : whole, fr->width, fr->height, v, why);
+  if (rc != HT_OK) return rc;
+  view_source_rgba(v, fr->rgba, fr->pitch ? fr->pitch : 4 * fr->width, fr->width, fr->height);
+  const FaceCrop f{crop->rgba, crop->width, crop->height, crop->pitch ? crop->pitch : 4 * crop->width, 0, crop->scale};
+  long long M[6];
+  if (!crop_map_framed(*box, cw, ch, v.sw, v.sh, f.w, f.h, f.scale, M)) return 0;
+  for (int j = 0; j < f.h; ++j)
+    for (int i = 0; i < f.w; ++i) reinterpret_cast<uint32_t *>(f.rgba + (size_t)j * f.pitch)[i] = crop_pixel<VIEW_RGBA>(v, M, i, j);
   return 1;
 }
 // rgba_to_yuv420 over n 2 x 2 blocks: blocks[4k..4k+3] = p00, p01, p10, p11 -> out[6k..6k+5] = their Y, U, V

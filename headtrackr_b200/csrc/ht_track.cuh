@@ -1790,16 +1790,28 @@ __host__ __device__ __forceinline__ double sk_div(double a, double b) {
 // with floor(v 65536 + 1/2).  Records that are not "CS" with width > 0 and height > 0 make no crop; neither do boxes
 // with a field that is not finite or beyond 65536 px (the tracker produces none), which also keeps every tap
 // coordinate of a 2048 x 2048 crop within int64.  -> whether the record makes a crop.
-__host__ __device__ inline bool crop_map(int detection, double x, double y, double w, double h, double angle, int cw, int ch,
-                                         int sw, int sh, int Sw, int Sh, double scale, long long M[6]) {
+// crop_tick: whether a record makes a crop, a crop tick
+__host__ __device__ __forceinline__ bool crop_tick(int detection, double x, double y, double w, double h) {
   if (detection != 2 || !(w > 0.0) || !(h > 0.0)) return false;
   const double f[4] = {x, y, w, h};
   for (int i = 0; i < 4; ++i)
     if (!(fabs(f[i]) <= 65536.0)) return false;
-  double s, c;
+  return true;
+}
+// The rotation (s, c) of a record's green rectangle and its local centre (cx, cy), as main.js strokes it (DESIGN.md 2,
+// "Strokes")
+__host__ __device__ __forceinline__ void crop_frame(double w, double h, double angle, double &s, double &c, double &cx,
+                                                    double &cy) {
   stroke_sincos(sk_add(angle, -1.5707963267948966), s, c);
-  const double rx = trunc(-(w / 2)), ry = trunc(-(h / 2));           // as main.js strokes it (DESIGN.md 2, "Strokes")
-  const double cx = sk_add(rx, sk_mul(w, 0.5)), cy = sk_add(ry, sk_mul(h, 0.5));
+  const double rx = trunc(-(w / 2)), ry = trunc(-(h / 2));
+  cx = sk_add(rx, sk_mul(w, 0.5));
+  cy = sk_add(ry, sk_mul(h, 0.5));
+}
+// crop_map's steps from the rotation on: a w x h box about local centre (cx, cy), rotated by (s, c) and translated to
+// (x, y)
+__host__ __device__ __forceinline__ void crop_map_box(double x, double y, double cx, double cy, double s, double c, double w,
+                                                      double h, int cw, int ch, int sw, int sh, int Sw, int Sh,
+                                                      double scale, long long M[6]) {
   double hw = sk_mul(sk_mul(w, scale), 0.5), hh = sk_mul(sk_mul(h, scale), 0.5);
   const double aw = sk_mul(hw, (double)Sh), ah = sk_mul(hh, (double)Sw);
   if (aw < ah) hw = sk_div(ah, (double)Sh);                            // the shorter side grows to S_w : S_h
@@ -1812,6 +1824,54 @@ __host__ __device__ inline bool crop_map(int detection, double x, double y, doub
   const double v[6] = {sk_add(sk_mul(X, kx), -0.5), sk_add(sk_mul(Y, ky), -0.5), sk_mul(sk_mul(c, px), kx),
                        sk_mul(sk_mul(s, px), ky),   sk_mul(-sk_mul(s, py), kx),  sk_mul(sk_mul(c, py), ky)};
   for (int i = 0; i < 6; ++i) M[i] = (long long)floor(sk_add(sk_mul(v[i], 65536.0), 0.5));
+}
+__host__ __device__ inline bool crop_map(int detection, double x, double y, double w, double h, double angle, int cw, int ch,
+                                         int sw, int sh, int Sw, int Sh, double scale, long long M[6]) {
+  if (!crop_tick(detection, x, y, w, h)) return false;
+  double s, c, cx, cy;
+  crop_frame(w, h, angle, s, c, cx, cy);
+  crop_map_box(x, y, cx, cy, s, c, w, h, cw, ch, sw, sh, Sw, Sh, scale, M);
+  return true;
+}
+
+// Framing (ht_tracker_set_framing; DESIGN.md 2, "Face crops", item 7): a per-stream filter whose state, the framed box
+// (ht_framed_box, in caller-owned device memory), moves only on crop ticks (crop_tick: the ticks that write crops).
+// The target is the green rectangle's centre, as crop_map places it, and the record's size.  The box snaps to the
+// target when it is not valid yet, lies on another canvas size, or no longer holds the target's centre; otherwise
+// each of cx, cy, width, height glides by alpha times the part of its error outside the dead zone, dead_zone times
+// the old width (cx, width) or height (cy, height).  fp64 from the old state, every operation rounded as written.
+__host__ __device__ __forceinline__ double framing_glide(double v, double t, double size, double alpha, double dead_zone) {
+  const double band = sk_mul(dead_zone, size), e = sk_add(t, -v);
+  return fabs(e) > band ? sk_add(v, sk_mul(alpha, sk_add(e, -copysign(band, e)))) : v;
+}
+// -> whether the record is a crop tick (and the box moved)
+__host__ __device__ inline bool framing_step(ht_framed_box &b, double alpha, double dead_zone, int detection, double x,
+                                             double y, double w, double h, double angle, int cw, int ch) {
+  if (!crop_tick(detection, x, y, w, h)) return false;
+  double s, c, cx, cy;
+  crop_frame(w, h, angle, s, c, cx, cy);
+  const double tx = sk_add(x, sk_add(sk_mul(c, cx), -sk_mul(s, cy)));
+  const double ty = sk_add(y, sk_add(sk_mul(s, cx), sk_mul(c, cy)));
+  if (!b.valid || b.canvas_w != cw || b.canvas_h != ch || fabs(sk_add(tx, -b.cx)) > sk_mul(b.width, 0.5) ||
+      fabs(sk_add(ty, -b.cy)) > sk_mul(b.height, 0.5)) {
+    b.cx = tx; b.cy = ty; b.width = w; b.height = h;
+    b.canvas_w = cw; b.canvas_h = ch; b.valid = 1;
+  } else {
+    const double ow = b.width, oh = b.height;
+    b.cx = framing_glide(b.cx, tx, ow, alpha, dead_zone);
+    b.cy = framing_glide(b.cy, ty, oh, alpha, dead_zone);
+    b.width = framing_glide(ow, w, ow, alpha, dead_zone);
+    b.height = framing_glide(oh, h, oh, alpha, dead_zone);
+  }
+  ++b.updates;
+  return true;
+}
+// The crop map of a framed box: crop_map's with local centre (0, 0), no rotation, and the box's centre and size.
+// -> false for a box that is not valid (or, as crop_map, has a field that is not finite or beyond 65536 px).
+__host__ __device__ inline bool crop_map_framed(const ht_framed_box &b, int cw, int ch, int sw, int sh, int Sw, int Sh,
+                                                double scale, long long M[6]) {
+  if (!b.valid || !crop_tick(2, b.cx, b.cy, b.width, b.height)) return false;
+  crop_map_box(b.cx, b.cy, 0.0, 0.0, 0.0, 1.0, b.width, b.height, cw, ch, sw, sh, Sw, Sh, scale, M);
   return true;
 }
 
@@ -1999,11 +2059,14 @@ __device__ __noinline__ void face_tensor_tile(const ViewFeedRec *__restrict__ vp
 // cw x ch), and write the tiles of its stream's crop or tensor on a crop tick; entries without one, without a crop tick,
 // or past their own tiles exit at once.  An RGBA crop's tiles go to face_crop_tile, a YUV crop's (layout, then
 // planes[id]) to face_crop_yuv_tile, a tensor's to face_tensor_tile.
+// framing (NULL while no stream has one): a stream whose framing's `outputs` has the output's bit takes the map of
+// its framed box (k_framing_update has moved it for this tick) in place of the record's.
 __global__ void __launch_bounds__(256) k_face_crop(const int32_t *__restrict__ ids, const EntryCanvas *__restrict__ geo,
                                                    int cw, int ch, const TrackerEvent *__restrict__ events,
                                                    const FaceCrop *__restrict__ crops,
                                                    const CropPlanes *__restrict__ planes,
-                                                   const FaceTensor *__restrict__ tensors, int tz, CropSource src) {
+                                                   const FaceTensor *__restrict__ tensors, int tz, CropSource src,
+                                                   const ht_framing *__restrict__ framing) {
   const int k = blockIdx.y, id = ids ? ids[k] : k;
   const bool tensor = (int)blockIdx.z == tz;
   FaceCrop f;
@@ -2022,8 +2085,13 @@ __global__ void __launch_bounds__(256) k_face_crop(const int32_t *__restrict__ i
   if (threadIdx.x == 0) {
     crop_source(src, k, v);
     const TrackerEvent &e = events[geo ? geo[k].record : k];
-    on = crop_map(e.detection, e.x, e.y, e.width, e.height, e.angle, geo ? geo[k].w : cw, geo ? geo[k].h : ch, v.sw, v.sh,
-                  f.w, f.h, f.scale, M);
+    const int ew = geo ? geo[k].w : cw, eh = geo ? geo[k].h : ch;
+    on = crop_map(e.detection, e.x, e.y, e.width, e.height, e.angle, ew, eh, v.sw, v.sh, f.w, f.h, f.scale, M);
+    if (on && framing) {
+      const ht_framing &g = framing[id];
+      if (g.box && (g.outputs & (tensor ? HT_FRAMING_TENSOR : HT_FRAMING_CROP)))
+        on = crop_map_framed(*g.box, ew, eh, v.sw, v.sh, f.w, f.h, f.scale, M);
+    }
   }
   __syncthreads();
   if (!on) return;
@@ -2050,6 +2118,28 @@ __global__ void __launch_bounds__(256) k_face_crop(const int32_t *__restrict__ i
     else if (v.kind == VIEW_NV12_I420) face_crop_yuv_tile<VIEW_NV12_I420, false>(&v, M, f, c, X0, Y0);
     else face_crop_yuv_tile<VIEW_FMT, false>(&v, M, f, c, X0, Y0);
   }
+}
+
+// After k_tracker_update, before k_face_crop: batch entry k (stream ids[k], NULL: k; its record events[geo[k].record]
+// and canvas geo[k], geo NULL: k and cw x ch) moves its stream's framed box, if the stream has a framing.
+__global__ void k_framing_update(const int32_t *__restrict__ ids, const EntryCanvas *__restrict__ geo, int n, int cw, int ch,
+                                 const TrackerEvent *__restrict__ events, const ht_framing *__restrict__ framing) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  const ht_framing &g = framing[ids ? ids[k] : k];
+  if (!g.box) return;
+  const TrackerEvent &e = events[geo ? geo[k].record : k];
+  ht_framed_box b = *g.box;
+  if (framing_step(b, g.alpha, g.dead_zone, e.detection, e.x, e.y, e.width, e.height, e.angle, geo ? geo[k].w : cw,
+                   geo ? geo[k].h : ch))
+    *g.box = b;
+}
+
+// ht_tracker_set_framing: one CTA makes the framed boxes of streams [first, first + n) that have a framing invalid,
+// with no updates
+__global__ void k_framing_reset(const ht_framing *__restrict__ framing, int first, int n) {
+  for (int i = threadIdx.x; i < n; i += blockDim.x)
+    if (framing[first + i].box) *framing[first + i].box = ht_framed_box{};
 }
 
 // ht_tracker_set_camera: one CTA constructs the cameras of streams [first, first + n) that have a controller

@@ -166,7 +166,9 @@ class TrackerSet:
     Context.tracker_set_face_crop takes: the tracked face cut upright out of the video into its `out` tensor (or, with
     "format": "nv12" / "i420" and a "color", its NV12 / I420 planes for a video encoder) on every tick that keeps the
     face.  A stream's "faceTensor" key is its face tensor, a dict as Context.tracker_set_face_tensor takes: the same
-    face as a model's normalised input, independent of "faceCrop".
+    face as a model's normalised input, independent of "faceCrop".  A stream's "framing" key is its framing, a dict as
+    Context.tracker_set_framing takes: a steady face-cam box in its `out` tensor that the crop (and, with "tensor":
+    True, the tensor) is cut from instead of the tracked box.
     Differs from the reference in one place: start() on a running stream does nothing (the reference runs an extra,
     unscheduled pass)."""
 
@@ -201,6 +203,9 @@ class TrackerSet:
         tensors = [(p or {}).get("faceTensor") for p in (params if per_stream else [params] * n_streams)]
         if any(t is not None for t in tensors):    # and face tensors
             context.tracker_set_face_tensor(0, tensors)
+        framings = [(p or {}).get("framing") for p in (params if per_stream else [params] * n_streams)]
+        if any(f is not None for f in framings):   # and framings
+            context.tracker_set_framing(0, framings)
 
     def set_params(self, k, params):
         """The parameters of stream k (a dict as for the constructor).  Its state is kept: calcAngles takes effect at
@@ -213,6 +218,7 @@ class TrackerSet:
         self.ctx.tracker_set_camera(k, [(params or {}).get("camera")])  # no "camera" key: none
         self.ctx.tracker_set_face_crop(k, [(params or {}).get("faceCrop")])   # no "faceCrop" key: none
         self.ctx.tracker_set_face_tensor(k, [(params or {}).get("faceTensor")])   # no "faceTensor" key: none
+        self.ctx.tracker_set_framing(k, [(params or {}).get("framing")])   # no "framing" key: none
 
     def addEventListener(self, fn):
         """fn(stream_index, evt): evt is a headtrackrStatus / facetrackingEvent / headtrackingEvent payload dict."""

@@ -11,6 +11,7 @@ Coordinates here are continuous: pixel (x, y) covers [x, x + 1) x [y, y + 1), so
 import ctypes as C
 import math
 
+from . import framing
 from ._lib import HT_VIEW_MIRROR, FaceCrop, TrackerEvent, VideoView, lib
 
 # EXIF orientation tag (1..8) -> view orientation; a tag says how to turn the stored image to show it upright
@@ -122,8 +123,19 @@ def crop_map(view, width, height, canvas_w, canvas_h, record, crop_w, crop_h, sc
     """ht_face_crop_map: the exact fixed-point map (U0, V0, Ui, Vi, Uj, Vj) of a crop_w x crop_h face crop for a
     tracker record (a dict with detection "CS" / 2, x, y, width, height, angle, or an ht_tracker_event), on a
     canvas_w x canvas_h canvas drawn from a width x height video through `view`; crop pixel (i, j) samples video tap
-    coordinates (U0 + i Ui + j Uj, V0 + i Vi + j Vj) / 65536 (tap u is pixel centre u + 0.5).  -> None when the
-    record makes no crop."""
+    coordinates (U0 + i Ui + j Uj, V0 + i Vi + j Vj) / 65536 (tap u is pixel centre u + 0.5).  `record` may also be
+    a framed box (a framing.py box dict or an ht_framed_box; ht_face_crop_map_framed): the map of a crop cut from it.
+    -> None when the record makes no crop (or the box is not valid)."""
+    vv = video_view(view)
+    crop = FaceCrop(None, int(crop_w), int(crop_h), 0, 0, float(scale))
+    out = (C.c_int64 * 6)()
+    if framing.is_box(record):
+        box = framing.as_struct(record)
+        rc = lib().ht_face_crop_map_framed(C.addressof(box), int(canvas_w), int(canvas_h), int(width), int(height),
+                                           C.addressof(vv), C.addressof(crop), out)
+        if rc < 0:
+            raise ValueError(f"ht_face_crop_map_framed rejected its arguments ({rc})")
+        return tuple(out) if rc == 1 else None
     if isinstance(record, TrackerEvent):
         ev = record
     else:
@@ -133,9 +145,6 @@ def crop_map(view, width, height, canvas_w, canvas_h, record, crop_w, crop_h, sc
         for k in ("x", "y", "width", "height", "angle"):
             setattr(ev, k, float(record[k]))
         ev.confidence = float(record.get("confidence", 1.0))
-    vv = video_view(view)
-    crop = FaceCrop(None, int(crop_w), int(crop_h), 0, 0, float(scale))
-    out = (C.c_int64 * 6)()
     rc = lib().ht_face_crop_map(C.addressof(ev), int(canvas_w), int(canvas_h), int(width), int(height), C.addressof(vv),
                                 C.addressof(crop), out)
     if rc < 0:
@@ -146,7 +155,8 @@ def crop_map(view, width, height, canvas_w, canvas_h, record, crop_w, crop_h, sc
 def crop_to_video(view, width, height, canvas_w, canvas_h, record, crop_w, crop_h, scale=1.0):
     """the 2x3 affine ((a, b, c), (d, e, f)) from continuous crop pixel coordinates (p, q) to the video's:
     x = a p + b q + c, y = d p + e q + f, exactly the map the device samples with (crop_map); e.g. to put landmarks
-    found in the crop back onto the video.  -> None when the record makes no crop."""
+    found in the crop back onto the video; `record` may be a framed box, as for crop_map.  -> None when the record
+    makes no crop."""
     m = crop_map(view, width, height, canvas_w, canvas_h, record, crop_w, crop_h, scale)
     if m is None:
         return None

@@ -457,7 +457,7 @@ typedef struct {
  * reference's timers write one after another.
  * Errors (nothing changes): HT_ERR_STATE before ht_tracker_config; HT_ERR_ARG for a range outside [0, max_frames),
  * n <= 0, canvases NULL, a host pointer, a pointer or pitch that is not a multiple of 4, a pitch below 4*width, or a
- * canvas that overlaps any debug canvas, crop plane, tensor plane or camera of any stream after the call (the one
+ * canvas that overlaps any debug canvas, crop plane, tensor plane, camera or framed box of any stream after the call (the one
  * rule of ht_tracker_set_face_tensor); HT_ERR_SIZE for a size outside 1..16384. */
 int ht_tracker_set_debug(ht_ctx *ctx, int first, int n, const ht_debug_canvas *canvases);
 
@@ -497,8 +497,8 @@ typedef struct {
  * A tick launches one more kernel while some stream has a crop, and nothing more otherwise.
  * Errors (nothing changes): HT_ERR_STATE before ht_tracker_config; HT_ERR_ARG for a range outside [0, max_frames),
  * n <= 0, crops NULL, a host pointer, a pointer or pitch that is not a multiple of 4, a pitch below 4*width, a scale
- * that is not finite or outside (0, 16], or a crop that overlaps any debug canvas, crop plane, tensor plane or camera
- * of any stream after the call (the one rule of ht_tracker_set_face_tensor); HT_ERR_SIZE for a size outside 1..2048. */
+ * that is not finite or outside (0, 16], or a crop that overlaps any debug canvas, crop plane, tensor plane, camera
+ * or framed box of any stream after the call (the one rule of ht_tracker_set_face_tensor); HT_ERR_SIZE for a size outside 1..2048. */
 int ht_tracker_set_face_crop(ht_ctx *ctx, int first, int n, const ht_face_crop *crops);
 
 /* A stream's face crop as 4:2:0 video for an encoder: NVENC takes NV12; openh264, libx264, libvpx and WebRTC frame
@@ -538,7 +538,7 @@ typedef struct {
  * that is odd or outside 2..2048; HT_ERR_ARG for a range outside [0, max_frames), n <= 0, crops NULL, a format other
  * than NV12 / I420, a colour other than the four above, a missing or extra plane, a host pointer, a pitch below its
  * row's bytes, a non-zero pad_, a scale that is not finite or outside (0, 16], or a plane that overlaps any debug
- * canvas, crop plane (its own crop's other planes included), tensor plane or camera of any stream after the call (the
+ * canvas, crop plane (its own crop's other planes included), tensor plane, camera or framed box of any stream after the call (the
  * one rule of ht_tracker_set_face_tensor). */
 int ht_tracker_set_face_crop_yuv(ht_ctx *ctx, int first, int n, const ht_face_crop_yuv *crops);
 
@@ -588,11 +588,12 @@ typedef struct {
  * value other than the above, a host pointer, a pointer not aligned to the element size, a stride outside its range
  * above, a non-zero pad_, a mul or add that is not finite, a U8 tensor whose used mul is not 1 or add not 0, a scale
  * that is not finite or outside (0, 16], or a tensor plane that overlaps any debug canvas, crop plane, tensor plane
- * (its own tensor's others included) or camera of any stream after the call.
+ * (its own tensor's others included), camera or framed box of any stream after the call.
  * That is the one overlap rule of the per-stream outputs, which ht_tracker_set_debug, both crop setters and
  * ht_tracker_set_camera apply too: the streams of a tick run concurrently, so no two of the byte spans a tick writes
  * may share a byte.  The spans: each debug canvas, (height-1)*pitch + 4*width bytes; each plane of each face crop,
- * RGBA or YUV; each channel plane of a CHW tensor, or the whole of an HWC tensor; each camera, HT_CAMERA_BYTES. */
+ * RGBA or YUV; each channel plane of a CHW tensor, or the whole of an HWC tensor; each camera, HT_CAMERA_BYTES; each
+ * framed box (ht_tracker_set_framing), HT_FRAMED_BOX_BYTES. */
 int ht_tracker_set_face_tensor(ht_ctx *ctx, int first, int n, const ht_face_tensor *tensors);
 
 /* The map of the crop `crop` (its size and scale; rgba and pitch are ignored; a YUV crop has the map of the RGBA crop of
@@ -605,6 +606,59 @@ int ht_tracker_set_face_tensor(ht_ctx *ctx, int first, int n, const ht_face_tens
  * 1..16384 or a crop outside 1..2048. */
 int ht_face_crop_map(const ht_tracker_event *ev, int canvas_w, int canvas_h, int video_w, int video_h,
                      const ht_video_view *view, const ht_face_crop *crop, int64_t out[6]);
+
+/* A stream's framed box: the state of its framing (DESIGN.md 2, "Face crops", item 7), in caller-owned DEVICE memory,
+ * an upright box in canvas pixels.  Byte offsets:
+ *     0  double cx, cy            its centre
+ *    16  double width, height     its size
+ *    32  int32  canvas_w, canvas_h  the canvas it lies on
+ *    40  uint32 updates           crop ticks applied since the framing was set
+ *    44  int32  valid             0 until the first crop tick, then 1 */
+typedef struct {
+  double cx, cy;
+  double width, height;
+  int32_t canvas_w, canvas_h;
+  uint32_t updates;
+  int32_t valid;
+} ht_framed_box;          /* 48 bytes */
+#define HT_FRAMING_CROP 1     /* the face crop (RGBA or YUV) takes the framed box */
+#define HT_FRAMING_TENSOR 2   /* the face tensor takes the framed box */
+/* A stream's framing: a steady face-cam box that glides instead of jumping with every camshift box.  Explicit values:
+ * the wrappers' defaults (alpha 0.25, dead zone 0.1) belong to the wrappers.  Byte offsets: 0 box, 8 alpha,
+ * 16 dead_zone, 24 outputs, 28 pad_. */
+typedef struct {
+  ht_framed_box *box;     /* 8-byte aligned DEVICE memory of the context's device; NULL removes the framing */
+  double alpha;           /* the share of the error outside the dead zone that a crop tick takes: (0, 1] */
+  double dead_zone;       /* half-width of the dead zone, a fraction of the box's width (x) or height (y): [0, 0.5] */
+  int32_t outputs;        /* HT_FRAMING_CROP | HT_FRAMING_TENSOR, nonzero: the outputs that take the framed box */
+  int32_t pad_;           /* 0 */
+} ht_framing;             /* 32 bytes */
+/* Stream first+i gets framings[i] (host array), for i in [0, n); stream states are kept.  Setting a framing enqueues
+ * its box to become invalid with updates = 0.  Then on every crop tick of the stream - a "CS" record with width > 0
+ * and height > 0, the ticks that write face crops - the box moves, in fp64 with every operation rounded as written,
+ * from its old state, towards the target: the centre (t_x, t_y) of the green rectangle as the crop places it, and the
+ * record's width and height.  It snaps to the target when it is not valid, lies on another canvas size, or
+ * |t_x - cx| > width / 2 or |t_y - cy| > height / 2 (the face has left the box); otherwise each of cx, cy, width,
+ * height with target t moves by v += alpha (e - copysign(band, e)) where e = t - v exceeds band = dead_zone * the old
+ * width (cx, width) or height (cy, height), and stays otherwise.  Every crop tick adds 1 to updates; other ticks leave
+ * the box as it is.  The outputs named in `outputs` are then cut from the framed box instead of the record's: crop_map's
+ * geometry with local centre (0, 0), no rotation and the box's centre and size, so they are always upright (with
+ * alpha 1 and dead zone 0 an unrotated record gives exactly the tracked crop); the others keep the record's box.  Which
+ * ticks write an output is unchanged.  The framing belongs to the stream id: stop, start, reset, a lost face,
+ * ht_tracker_set_params and ht_tracker_import keep it; ht_tracker_config removes every stream's.  A tick launches one
+ * more kernel while some stream has a framing, and nothing more otherwise.  ht_face_crop_map_framed gives the map.
+ * Errors (nothing changes; the message names the record): HT_ERR_STATE before ht_tracker_config; HT_ERR_ARG for a
+ * range outside [0, max_frames), n <= 0, framings NULL, a box that is host memory, memory of another device or not
+ * 8-byte aligned, an alpha outside (0, 1] or a dead_zone outside [0, 0.5] (NaN included), an outputs mask that is 0
+ * or has other bits, a non-zero pad_, or a box that overlaps any debug canvas, crop plane, tensor plane, camera or
+ * framed box of any stream after the call (the one rule of ht_tracker_set_face_tensor; a box is HT_FRAMED_BOX_BYTES). */
+#define HT_FRAMED_BOX_BYTES 48
+int ht_tracker_set_framing(ht_ctx *ctx, int first, int n, const ht_framing *framings);
+/* The map of the crop `crop` (as for ht_face_crop_map) cut from framed box `box` (host memory) on a canvas_w x canvas_h
+ * canvas drawn from a video_w x video_h video through `view`, exactly as the device computes it.  Host only.  -> 1, 0
+ * for a box that is not valid (out all 0), or the errors of ht_face_crop_map. */
+int ht_face_crop_map_framed(const ht_framed_box *box, int canvas_w, int canvas_h, int video_w, int video_h,
+                            const ht_video_view *view, const ht_face_crop *crop, int64_t out[6]);
 
 /* A stream's head-coupled camera: the three.js r48 PerspectiveCamera that realisticAbsoluteCameraControl moves
  * (src/controllers.js:28-68), in caller-owned DEVICE memory that a renderer can bind directly.  Byte offsets:
@@ -652,7 +706,7 @@ typedef struct {
  * some stream has a controller, and nothing more otherwise.
  * Errors (nothing changes): HT_ERR_STATE before ht_tracker_config; HT_ERR_ARG for a range outside [0, max_frames),
  * n <= 0, controls NULL, a camera that is host memory, memory of another device or not 16-byte aligned, a camera that
- * overlaps any debug canvas, crop plane, tensor plane or camera of any stream after the call (the one rule of
+ * overlaps any debug canvas, crop plane, tensor plane, camera or framed box of any stream after the call (the one rule of
  * ht_tracker_set_face_tensor), a non-finite field, aspect <= 0, near <= 0, far <= near, fov outside (0, 180), or a
  * degenerate lookAt (fixed_position == look_at, or a view direction parallel to +y). */
 int ht_tracker_set_camera(ht_ctx *ctx, int first, int n, const ht_camera_control *controls);
@@ -683,8 +737,9 @@ int ht_tracker_set_camera(ht_ctx *ctx, int first, int n, const ht_camera_control
  * a device `streams`, an id out of range or listed twice, or device records of another device or misaligned. */
 int ht_tracker_export(ht_ctx *ctx, const int32_t *streams, int n, void *records);
 /* Stream streams[i] := records[i], for i in [0, n): its lifecycle state, parameters and camshift tracker become exactly
- * the exported stream's, and what it held before is discarded.  Its debug canvas (ht_tracker_set_debug) and camera
- * controller (ht_tracker_set_camera) stay as they were: those are device resources of this stream id, not part of the
+ * the exported stream's, and what it held before is discarded.  Its debug canvas (ht_tracker_set_debug), camera
+ * controller (ht_tracker_set_camera) and framing with its box (ht_tracker_set_framing) stay as they were: those are
+ * device resources of this stream id, not part of the
  * Tracker's state.  streams and records as for
  * ht_tracker_export; the source and the destination may be one context (clone: import into an idle id; swap: export
  * [a, b], import [b, a]).  Every record is checked on the device first - magic, format version (records of another

@@ -33,6 +33,8 @@
 //        face tensor for a model, device memory)
 //   trackerSetCamera(handle, first, [control|null, ...])  (ht_tracker_set_camera: each stream's head-coupled camera,
 //        realisticAbsoluteCameraControl on an ht_camera in device memory)
+//   trackerSetFraming(handle, first, [framing|null, ...])  (ht_tracker_set_framing: each stream's steady face-cam box,
+//        an ht_framed_box in device memory, that its crop and / or tensor is cut from)
 //   trackerExport(handle, [stream, ...]) -> Buffer of records; trackerImport(handle, [stream, ...], records)
 //        (ht_tracker_export / ht_tracker_import: a stream's whole Tracker as HT_TRACKER_RECORD_BYTES per stream)
 //   trackerFeed(handle, [{stream, rgba, width, height, nowMs, canvasWidth?, canvasHeight?}], canvasWidth, canvasHeight)
@@ -685,6 +687,43 @@ static napi_value TrackerSetCamera(napi_env env, napi_callback_info info) {
   return nullptr;
 }
 
+// trackerSetFraming(handle, first, [{box: BigInt device address, alpha?, deadZone?, crop?, tensor?}, null, ...]): stream
+// first+i gets framings[i]; null or undefined: none.  alpha and deadZone default to 0.25 and 0.1, crop to true and
+// tensor to false, as in the Python wrapper.
+static napi_value TrackerSetFraming(napi_env env, napi_callback_info info) {
+  size_t argc = 3;
+  napi_value argv[3];
+  NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+  ht_ctx *ctx = Ctx(env, argv[0]);
+  int32_t first = 0;
+  uint32_t n = 0;
+  napi_get_value_int32(env, argv[1], &first);
+  NAPI_OK(napi_get_array_length(env, argv[2], &n));
+  std::vector<ht_framing> fs(n);
+  memset(fs.data(), 0, n * sizeof(ht_framing));
+  for (uint32_t i = 0; i < n; ++i) {
+    napi_value r, v;
+    napi_valuetype t = napi_undefined;
+    NAPI_OK(napi_get_element(env, argv[2], i, &r));
+    napi_typeof(env, r, &t);
+    if (t != napi_object) continue;
+    uint64_t addr = 0;
+    bool lossless = false;
+    if (napi_get_named_property(env, r, "box", &v) == napi_ok) napi_get_value_bigint_uint64(env, v, &addr, &lossless);
+    ht_framing &f = fs[i];
+    f.box = reinterpret_cast<ht_framed_box *>(static_cast<uintptr_t>(addr));
+    f.alpha = GetNumber(env, r, "alpha", 0.25);
+    f.dead_zone = GetNumber(env, r, "deadZone", 0.1);
+    bool crop = true, tensor = false;
+    if (napi_get_named_property(env, r, "crop", &v) == napi_ok) napi_get_value_bool(env, v, &crop);
+    if (napi_get_named_property(env, r, "tensor", &v) == napi_ok) napi_get_value_bool(env, v, &tensor);
+    f.outputs = (crop ? HT_FRAMING_CROP : 0) | (tensor ? HT_FRAMING_TENSOR : 0);
+  }
+  int rc = ht_tracker_set_framing(ctx, first, (int)n, fs.data());
+  if (rc < 0) return Throw(env, ctx, rc);
+  return nullptr;
+}
+
 // stream ids of an Array of numbers
 static bool GetStreams(napi_env env, napi_value arr, std::vector<int32_t> *ids) {
   uint32_t n = 0;
@@ -1044,6 +1083,7 @@ static napi_value Init(napi_env env, napi_value exports) {
       {"trackerSetFaceCropYuv", nullptr, TrackerSetFaceCropYuv, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerSetFaceTensor", nullptr, TrackerSetFaceTensor, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerSetCamera", nullptr, TrackerSetCamera, nullptr, nullptr, nullptr, napi_default, nullptr},
+      {"trackerSetFraming", nullptr, TrackerSetFraming, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerExport", nullptr, TrackerExport, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerImport", nullptr, TrackerImport, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerFeed", nullptr, TrackerFeed, nullptr, nullptr, nullptr, napi_default, nullptr},

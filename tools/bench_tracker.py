@@ -34,6 +34,9 @@ streams: N 640x480 streams, device-resident frames and outputs, CUDA events arou
                   crops on none, 1/64 and all of the streams, against ht_ingest_yuv + grid_sample of the boxes (also
                   --before-lib), NV12 and I420 crops against RGBA crops + a torch conversion, and k_face_crop's time
                   (crops_arms)
+  framing*_*      (--framing) the --crops workload with 224x224 NV12 crops on every stream, with a framing on no, every
+                  and every 64th stream (no framing also against --before-lib), arms alternating tick by tick
+                  (framing_arms)
 
 Prints one JSON line with the card's name and power limit read in the same run; --out also writes it to a file."""
 import argparse
@@ -1408,6 +1411,101 @@ def migrate_arms(torch, frames, stream, N, W, H, steps, rounds):
     return res
 
 
+def framing_arms(torch, stream, N, steps, rounds, before_lib=None):
+    """f15's workload (N streams of 1280x720 NV12 through ht_tracker_feed_yuv onto 320x240 canvases, 224x224 NV12 face
+    crops on every stream), with arms alternating tick by tick: framing off (framingoff_cs), framing off on another
+    build (framingoff_before_cs, --before-lib), a framing on every stream (framingall_cs) and on every 64th stream
+    (framing64_cs), alpha 0.25 and dead zone 0.1.  The records of every arm must agree on every timed tick, and the
+    framed arms' boxes must equal headtrackr_b200.framing's replay of the records on a sample of streams."""
+    import ctypes as C
+    from headtrackr_b200 import Context, _lib, framing
+    from headtrackr_b200.context import _yuv_image
+    W, H, CW, CH, S = 1280, 720, 320, 240, 224
+    rec_bytes = C.sizeof(_lib.TrackerEvent)
+    now = [1.0e12]
+    kw = dict(max_width=CW, max_height=CH, max_frames=N, stream=stream)
+    ys, uvs = nv12_streams(torch, N, W, H)
+    keep = []
+    imgs = [_yuv_image((ys[k], uvs[k]), "nv12", "bt601", keep)[0] for k in range(N)]
+    yrecs = (_lib.YuvFrame * N)()
+    for k in range(N):
+        yrecs[k] = _lib.YuvFrame(imgs[k], k, CW, CH, 0, 0.0)
+    boxes = {}
+
+    def arm(every, before=False):
+        c = other_build_context(before_lib, **kw) if before else Context(**kw)
+        c._L.ht_tracker_set_face_crop_yuv.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p]
+        c.tracker_config()
+        c.tracker_reset(0, N)
+        c.tracker_start(0, N)
+        y = torch.zeros((N, S, S), dtype=torch.uint8, device="cuda")
+        uv = torch.zeros((N, S // 2, S), dtype=torch.uint8, device="cuda")
+        c.tracker_set_face_crop(0, [{"out": (y[k], uv[k]), "format": "nv12", "color": "bt601"} for k in range(N)])
+        if every:
+            b = torch.zeros((N, 64), dtype=torch.uint8, device="cuda")
+            c.tracker_set_framing(0, [{"out": b[k, :48]} if k % every == 0 else None for k in range(N)])
+            boxes[every] = b
+        out = torch.empty(N * rec_bytes, dtype=torch.uint8, device="cuda")
+
+        def run():
+            for k in range(N):
+                yrecs[k].now_ms = now[0]
+            c._check(c._L.ht_tracker_feed_yuv(c._h, C.addressof(yrecs), N, 1, out.data_ptr()))
+        return c, run, out
+
+    arms = {"framingoff_cs": arm(0), "framingall_cs": arm(1), "framing64_cs": arm(64)}
+    if before_lib:
+        arms["framingoff_before_cs"] = arm(0, before=True)
+    names = list(arms)
+    sample = list(range(0, N, max(1, N // 32)))
+    replay = {k: framing.new_box() for k in sample}
+
+    def tick(name):
+        _, run, _ = arms[name]
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        a.record()
+        run()
+        b.record()
+        b.synchronize()
+        return a.elapsed_time(b)
+
+    def follow():
+        recs = arms["framingoff_cs"][2].cpu().numpy().reshape(N, rec_bytes)
+        for k in sample:
+            e = _lib.TrackerEvent.from_buffer_copy(bytes(recs[k]))
+            framing.framing_step(replay[k], dict(detection=e.detection, x=e.x, y=e.y, width=e.width, height=e.height,
+                                                 angle=e.angle), CW, CH)
+
+    for _ in range(17):                          # the whitebalance gate, detection, the first CS frames
+        now[0] += 20.0
+        for name in names:
+            tick(name)
+        follow()
+    times = {name: [[] for _ in range(rounds)] for name in names}
+    for r in range(rounds):
+        for s in range(steps):
+            now[0] += 20.0
+            rot = (r * steps + s) % len(names)
+            for name in names[rot:] + names[:rot]:
+                times[name][r].append(tick(name))
+            first = arms[names[0]][2]
+            if any(not torch.equal(first, arms[name][2]) for name in names[1:]):
+                raise SystemExit("framing arms disagree on the records of a timed tick")
+            follow()
+    res = {}
+    for name in names:
+        med = [float(np.median(t)) for t in times[name]]
+        res[f"{name}_ms"] = float(np.median(sum(times[name], [])))
+        res[f"{name}_spread_ms"] = max(med) - min(med)
+    res["framing_records_agree"] = True
+    got = boxes[1].cpu().numpy()
+    res["framing_boxes_equal_replay"] = all(bytes(got[k, :48]) == framing.box_to_bytes(replay[k]) for k in sample)
+    res["framing_updates_max"] = max(replay[k]["updates"] for k in sample)
+    for c, _, _ in arms.values():
+        c.close()
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--streams", type=int, default=1024)
@@ -1423,6 +1521,7 @@ def main():
     ap.add_argument("--formats", action="store_true", help="only the video-format arms (formats_arms)")
     ap.add_argument("--views", action="store_true", help="only the video-view arms (views_arms)")
     ap.add_argument("--crops", action="store_true", help="only the face-crop arms (crops_arms)")
+    ap.add_argument("--framing", action="store_true", help="only the framing arms (framing_arms)")
     ap.add_argument("--out")
     a = ap.parse_args()
     import torch
@@ -1444,6 +1543,9 @@ def main():
         return report(res, a.out)
     if a.crops:
         res.update(crops_arms(torch, stream, N, a.steps, a.rounds, a.before_lib))
+        return report(res, a.out)
+    if a.framing:
+        res.update(framing_arms(torch, stream, N, a.steps, a.rounds, a.before_lib))
         return report(res, a.out)
     if a.formats:
         res.update(formats_arms(torch, stream, N, a.steps, a.rounds, a.before_lib))
