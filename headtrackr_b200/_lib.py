@@ -191,6 +191,21 @@ FRAMED_BOX_BYTES = 48
 assert C.sizeof(FramedBox) == FRAMED_BOX_BYTES and FramedBox.canvas_w.offset == 32 and FramedBox.valid.offset == 44 \
     and C.sizeof(Framing) == 32 and Framing.outputs.offset == 24
 
+# ht_face_redact.mode
+HT_REDACT_OFF, HT_REDACT_MOSAIC, HT_REDACT_FILL = 0, 1, 2
+
+
+class FaceRedact(C.Structure):
+    """ht_face_redact: one stream's face redaction for ht_tracker_set_redact (mode HT_REDACT_OFF = none; block even in
+    2..128; hold 0..65535 ticks; fill_rgb for RGBA8 and packed RGB video, fill_yuv for YUV video; scale in (0, 16])"""
+    _fields_ = [("mode", C.c_int32), ("block", C.c_int32), ("hold", C.c_int32), ("fill_rgb", C.c_uint8 * 3),
+                ("pad0", C.c_uint8), ("fill_yuv", C.c_uint8 * 3), ("pad1", C.c_uint8), ("pad_", C.c_int32),
+                ("scale", C.c_double)]
+
+
+assert C.sizeof(FaceRedact) == 32 and FaceRedact.fill_rgb.offset == 12 and FaceRedact.fill_yuv.offset == 16 \
+    and FaceRedact.pad_.offset == 20 and FaceRedact.scale.offset == 24
+
 # ht_tracker_export / ht_tracker_import: bytes of one tracker record (HT_TRACKER_RECORD_BYTES)
 TRACKER_RECORD_BYTES = 16864
 
@@ -234,7 +249,7 @@ _lib = None
 
 EXPORTS = ["ht_version", "ht_create", "ht_destroy", "ht_last_error", "ht_sync", "ht_max_rects", "ht_detect",
            "ht_track_init", "ht_track_init_from_detect", "ht_track", "ht_detect_track", "ht_stream_reset", "ht_stream_step", "ht_stream_head_config", "ht_stream_step_head",
-           "ht_tracker_config", "ht_tracker_reset", "ht_tracker_start", "ht_tracker_stop", "ht_tracker_step", "ht_tracker_feed", "ht_tracker_set_params", "ht_tracker_feed_canvases", "ht_tracker_set_debug", "ht_tracker_set_debug_strokes", "ht_tracker_set_face_crop", "ht_tracker_set_face_crop_yuv", "ht_tracker_set_face_tensor", "ht_face_crop_map", "ht_tracker_set_framing", "ht_face_crop_map_framed", "ht_tracker_set_camera", "ht_tracker_export", "ht_tracker_import", "ht_tracker_feed_yuv", "ht_ingest", "ht_ingest_yuv",
+           "ht_tracker_config", "ht_tracker_reset", "ht_tracker_start", "ht_tracker_stop", "ht_tracker_step", "ht_tracker_feed", "ht_tracker_set_params", "ht_tracker_feed_canvases", "ht_tracker_set_debug", "ht_tracker_set_debug_strokes", "ht_tracker_set_face_crop", "ht_tracker_set_face_crop_yuv", "ht_tracker_set_face_tensor", "ht_face_crop_map", "ht_tracker_set_framing", "ht_face_crop_map_framed", "ht_tracker_set_redact", "ht_face_redact_rect", "ht_tracker_set_camera", "ht_tracker_export", "ht_tracker_import", "ht_tracker_feed_yuv", "ht_ingest", "ht_ingest_yuv",
            "ht_tracker_feed_views", "ht_tracker_feed_yuv_views", "ht_ingest_views", "ht_ingest_yuv_views", "ht_backprojection", "ht_whitebalance",
            "ht_plan_info", "ht_debug_plane", "ht_debug_raw", "ht_debug_model_hist", "ht_debug_track_stats", "ht_set_track_memo", "ht_set_pipeline", "ht_join", "ht_debug_set_exactness", "ht_debug_track_trace", "ht_debug_track_phases", "ht_launch_count",
            "ht_profile", "ht_profile_read"]
@@ -286,6 +301,8 @@ def lib():
     L.ht_face_crop_map.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp]
     L.ht_tracker_set_framing.argtypes = [vp, C.c_int, C.c_int, vp]
     L.ht_face_crop_map_framed.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp]
+    L.ht_tracker_set_redact.argtypes = [vp, C.c_int, C.c_int, vp]
+    L.ht_face_redact_rect.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp]
     L.ht_tracker_set_camera.argtypes = [vp, C.c_int, C.c_int, vp]
     L.ht_tracker_export.argtypes = [vp, vp, C.c_int, vp]
     L.ht_tracker_import.argtypes = [vp, vp, C.c_int, vp]

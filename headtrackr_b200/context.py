@@ -650,6 +650,31 @@ class Context:
         self._check(self._L.ht_tracker_set_framing(self._h, int(first), len(framings), C.addressof(arr)))
         self._keep("framing", int(first), [None if d is None else d["out"] for d in framings])
 
+    def tracker_set_redact(self, first, redactions):
+        """Face redactions of streams first, first+1, ... (ht_tracker_set_redact): per stream None (none) or a dict
+        {"mode": "mosaic" | "fill"; "block": 16; "scale": 1.25; "hold": 10; "fill_rgb": (0, 0, 0); "fill_yuv": (16, 128,
+        128)}.  After each tick the stream's tracked face is hidden in its own video, in place: every cell of a block x
+        block grid anchored at video pixel (0, 0) that meets the face box scaled by `scale` becomes its mean (mosaic)
+        or the fill colour (fill_rgb on RGBA8 and packed RGB video, fill_yuv on YUV video), and the last face box
+        stays hidden for `hold` ticks after the face is lost (DESIGN.md 2, "Face redaction"; views.redact_rect gives
+        the rectangle).  headtrackr tracks one face per stream: this hides that face, not every face in the frame.
+        The library writes the stream's video, which must then be device memory and shared with no other redacting
+        stream of the tick.  The crops and tensors of the tick see the unredacted face.  The redaction is the
+        stream's: it outlives set_params, stop, start, reset and import; tracker_config removes it."""
+        redactions = list(redactions)
+        arr = (_lib.FaceRedact * max(1, len(redactions)))()
+        modes = {"mosaic": _lib.HT_REDACT_MOSAIC, "fill": _lib.HT_REDACT_FILL}
+        for i, d in enumerate(redactions):
+            if d is None:
+                continue
+            mode = d.get("mode", "mosaic")
+            r = arr[i]
+            r.mode = modes[mode] if isinstance(mode, str) else int(mode)
+            r.block, r.hold, r.scale = int(d.get("block", 16)), int(d.get("hold", 10)), float(d.get("scale", 1.25))
+            r.fill_rgb[:] = [int(v) for v in d.get("fill_rgb", (0, 0, 0))]
+            r.fill_yuv[:] = [int(v) for v in d.get("fill_yuv", (16, 128, 128))]
+        self._check(self._L.ht_tracker_set_redact(self._h, int(first), len(redactions), C.addressof(arr)))
+
     def tracker_export(self, streams, out=None):
         """The tracker records of the listed streams (ht_tracker_export): a (len(streams), TRACKER_RECORD_BYTES) uint8
         numpy array, or with a contiguous torch CUDA uint8 `out` of that many bytes on this context's device the

@@ -611,11 +611,12 @@ struct ht_ctx {
   StreamTable<CropPlanes> crop_planes;
   StreamTable<FaceTensor> tensor;
   StreamTable<ht_framing> framing;          // ht_tracker_set_framing
+  StreamTable<Redact> redact;               // ht_tracker_set_redact: the records and their holds
   DevBuf d_debug_tab;
   // what a tick launches for them, from the tables (count_outputs): the streams with a debug canvas, with a canvas and
-  // strokes on, with a camera, with a crop, with a tensor and with a framing (0: no launch for them), and the tiles
-  // of the largest crop and tensor (k_face_crop's grid.x)
-  int debug_count = 0, stroke_count = 0, camera_count = 0, framing_count = 0;
+  // strokes on, with a camera, with a crop, with a tensor, with a framing and with a redaction (0: no launch for
+  // them), and the tiles of the largest crop and tensor (k_face_crop's grid.x)
+  int debug_count = 0, stroke_count = 0, camera_count = 0, framing_count = 0, redact_count = 0;
   int crop_count = 0, crop_tiles = 0, tensor_count = 0, tensor_tiles = 0;
   // ht_tracker_feed(_canvases): the record table {ids[n], clocks[n], FeedRec[n], EntryCanvas[n], tile starts[n+1]}
   // goes up in one copy from pinned memory; the videos are drawn into the canvas arena (batch entry k's canvas at
@@ -1792,7 +1793,7 @@ static bool tracker_params_ok(const ht_tracker_params &p) {
 // What a tick launches for the per-stream outputs, from their tables: after every change to a table
 static void count_outputs(ht_ctx *ctx) {
   const auto tiles = [](int w, int h) { return ((w + CROP_TX - 1) / CROP_TX) * ((h + CROP_TY - 1) / CROP_TY); };
-  ctx->debug_count = ctx->stroke_count = ctx->camera_count = ctx->framing_count = 0;
+  ctx->debug_count = ctx->stroke_count = ctx->camera_count = ctx->framing_count = ctx->redact_count = 0;
   ctx->crop_count = ctx->crop_tiles = ctx->tensor_count = ctx->tensor_tiles = 0;
   for (const DebugCanvas &d : ctx->debug.h) {
     ctx->debug_count += d.rgba != nullptr;
@@ -1800,6 +1801,7 @@ static void count_outputs(ht_ctx *ctx) {
   }
   for (const CameraCtl &k : ctx->camera.h) ctx->camera_count += k.camera != nullptr;
   for (const ht_framing &g : ctx->framing.h) ctx->framing_count += g.box != nullptr;
+  for (const Redact &r : ctx->redact.h) ctx->redact_count += r.d.mode != HT_REDACT_OFF;
   for (const FaceCrop &f : ctx->crop.h)
     if (f.rgba) {
       ++ctx->crop_count;
@@ -1818,10 +1820,12 @@ int ht_tracker_config(ht_ctx *ctx, const ht_tracker_params *params) {
   CK(cudaSetDevice(ctx->cfg.device));
   const size_t mf = (size_t)ctx->cfg.max_frames;
   if (params && !tracker_params_ok(*params)) return ctx->fail(HT_ERR_ARG, "bad head parameters");
-  // either form discards every stream's debug canvas and stroke flag, camera, face crop, face tensor and framing
+  // either form discards every stream's debug canvas and stroke flag, camera, face crop, face tensor, framing and
+  // redaction
   CK(ctx->debug.clear(ctx->stream));
   CK(ctx->camera.clear(ctx->stream));
   CK(ctx->framing.clear(ctx->stream));
+  CK(ctx->redact.clear(ctx->stream));
   CK(ctx->crop.clear(ctx->stream));
   CK(ctx->crop_planes.clear(ctx->stream));
   CK(ctx->tensor.clear(ctx->stream));
@@ -1952,12 +1956,14 @@ struct OutputEdit {
   std::vector<CropPlanes> *crop_planes = nullptr;
   std::vector<FaceTensor> *tensor = nullptr;
   std::vector<ht_framing> *framing = nullptr;
+  std::vector<Redact> *redact = nullptr;    // writes no byte range of its own: only the video, checked per tick
 };
 
 // How every setter's records reach the tick.  The call is refused if two byte ranges a tick would write share a byte
 // (the tables before it share none, so a clash takes in one of its records, which the message names).  Otherwise
 // streams [first, first + n) of the edited tables go to the device, a new camera is constructed there, a new framed
-// box is made invalid there, and the tables and the tick's counts follow.
+// box is made invalid there (a redaction's hold goes up empty with its record), and the tables and the tick's counts
+// follow.
 static int commit_outputs(ht_ctx *ctx, int first, int n, const OutputEdit &e) {
   const int kind = e.debug ? OUT_DEBUG : e.crop ? OUT_CROP : e.tensor ? OUT_TENSOR : e.framing ? OUT_FRAMING : OUT_CAMERA;
   TickWrite c[2];
@@ -1998,10 +2004,12 @@ static int commit_outputs(ht_ctx *ctx, int first, int n, const OutputEdit &e) {
     ++ctx->launches;
     CK(cudaGetLastError());
   }
+  if (e.redact) CK(ctx->redact.commit(*e.redact, first, n, st));
   CK(cudaStreamSynchronize(st));    // the edited tables are the setter's locals
   if (e.debug) ctx->debug.h.swap(*e.debug);
   if (e.camera) ctx->camera.h.swap(*e.camera);
   if (e.framing) ctx->framing.h.swap(*e.framing);
+  if (e.redact) ctx->redact.h.swap(*e.redact);
   if (e.crop) {
     ctx->crop.h.swap(*e.crop);
     ctx->crop_planes.h.swap(*e.crop_planes);
@@ -2385,6 +2393,133 @@ int ht_tracker_set_framing(ht_ctx *ctx, int first, int n, const ht_framing *fram
   return commit_outputs(ctx, first, n, e);
 }
 
+static_assert(sizeof(ht_face_redact) == 32 && offsetof(ht_face_redact, block) == 4 && offsetof(ht_face_redact, hold) == 8 &&
+                  offsetof(ht_face_redact, fill_rgb) == 12 && offsetof(ht_face_redact, pad0) == 15 &&
+                  offsetof(ht_face_redact, fill_yuv) == 16 && offsetof(ht_face_redact, pad1) == 19 &&
+                  offsetof(ht_face_redact, pad_) == 20 && offsetof(ht_face_redact, scale) == 24,
+              "ht_face_redact layout (include/headtrackr_b200.h)");
+
+// One redaction whose mode is not HT_REDACT_OFF -> NULL, or what is wrong with it
+static const char *redact_check(const ht_face_redact &d) {
+  if (d.mode != HT_REDACT_MOSAIC && d.mode != HT_REDACT_FILL)
+    return "mode is not HT_REDACT_OFF, HT_REDACT_MOSAIC or HT_REDACT_FILL";
+  if (d.block < 2 || d.block > 128 || (d.block & 1)) return "block is odd or outside 2..128";
+  if (d.hold < 0 || d.hold > 65535) return "hold outside 0..65535";
+  if (d.pad0 || d.pad1 || d.pad_) return "a pad field is not 0";
+  if (!(d.scale > 0.0 && d.scale <= 16.0)) return "scale is not finite or outside (0, 16]";
+  return nullptr;
+}
+
+// The redactions of streams [first, first + n).  Everything is checked on the host before anything changes; the
+// records go up with empty holds.
+int ht_tracker_set_redact(ht_ctx *ctx, int first, int n, const ht_face_redact *redactions) {
+  { const int ar = tracker_streams(ctx, first, n); if (ar != HT_OK) return ar; }
+  if (!redactions) return ctx->fail(HT_ERR_ARG, "redactions is NULL");
+  std::vector<Redact> next = ctx->redact.edit(ctx->cfg.max_frames);
+  for (int i = 0; i < n; ++i) {
+    const ht_face_redact &d = redactions[i];
+    Redact k{};
+    if (d.mode != HT_REDACT_OFF) {
+      const char *why = redact_check(d);
+      if (why) return ctx->fail(HT_ERR_ARG, "record %d: %s", i, why);
+      k.d = d;
+    }
+    next[(size_t)(first + i)] = k;
+  }
+  OutputEdit e;
+  e.redact = &next;
+  return commit_outputs(ctx, first, n, e);
+}
+
+// Whether stream s has a face redaction
+static bool redacting(const ht_ctx *ctx, int s) {
+  return ctx->redact_count > 0 && ctx->redact.h[(size_t)s].d.mode != HT_REDACT_OFF;
+}
+
+static int yuv_planes(int format, int w, int h, int tight[3], int rows[3]);
+
+// The rules of face redaction for a tick's records (ht_tracker_set_redact): the video of every record whose stream
+// redacts is device memory, and no two such records have video planes that share a byte (each plane a span of
+// (rows - 1) * pitch + its row's bytes).  Records checked (ht_tracker_feed's and ht_tracker_feed_yuv's checks).
+static int check_redact_videos(ht_ctx *ctx, const ht_canvas_frame *frames, const ht_yuv_frame *yuv, int n) {
+  struct Span { uintptr_t start, end; int record; };
+  std::vector<Span> w;
+  for (int b = 0; b < n; ++b) {
+    const int s = yuv ? yuv[b].stream : frames[b].video.stream;
+    if (!redacting(ctx, s)) continue;
+    const uint8_t *plane[3] = {nullptr, nullptr, nullptr};
+    size_t pitch[3], rows[3], bytes[3];
+    int planes = 1;
+    if (yuv) {
+      const ht_yuv_image &v = yuv[b].video;
+      int tight[3], r[3];
+      planes = yuv_planes(v.format, v.width, v.height, tight, r);
+      for (int p = 0; p < planes; ++p) {
+        plane[p] = v.planes[p];
+        pitch[p] = v.pitch[p] ? (size_t)v.pitch[p] : (size_t)tight[p];
+        rows[p] = (size_t)r[p];
+        bytes[p] = (size_t)tight[p];
+      }
+    } else {
+      const ht_video_frame &f = frames[b].video;
+      plane[0] = f.rgba;
+      pitch[0] = f.pitch ? (size_t)f.pitch : 4 * (size_t)f.width;
+      rows[0] = (size_t)f.height;
+      bytes[0] = 4 * (size_t)f.width;
+    }
+    for (int p = 0; p < planes; ++p) {
+      if (!is_device_ptr(plane[p]))
+        return ctx->fail(HT_ERR_ARG, "record %d: stream %d redacts its face, so its video must be device memory", b, s);
+      const uintptr_t a = reinterpret_cast<uintptr_t>(plane[p]);
+      w.push_back(Span{a, a + (rows[p] - 1) * pitch[p] + bytes[p], b});
+    }
+  }
+  std::sort(w.begin(), w.end(), [](const Span &a, const Span &b) { return a.start < b.start; });
+  // the largest end so far (e1, of record r1) and the largest end of any other record (e2, of r2)
+  uintptr_t e1 = 0, e2 = 0;
+  int r1 = -1, r2 = -1;
+  for (const Span &x : w) {
+    const int other = x.record != r1 ? r1 : r2;
+    const uintptr_t end = x.record != r1 ? e1 : e2;
+    if (other >= 0 && x.start < end)
+      return ctx->fail(HT_ERR_ARG, "record %d: its video shares bytes with record %d's, and both streams redact their "
+                       "faces", std::max(x.record, other), std::min(x.record, other));
+    if (x.record == r1) {
+      e1 = std::max(e1, x.end);
+    } else if (x.end > e1) {
+      e2 = e1, r2 = r1;
+      e1 = x.end, r1 = x.record;
+    } else if (x.end > e2 || r2 < 0) {
+      e2 = x.end, r2 = x.record;
+    }
+  }
+  return HT_OK;
+}
+
+// The redacted rectangle of k_face_redact for a face record, on the host
+int ht_face_redact_rect(const ht_tracker_event *ev, int canvas_w, int canvas_h, int video_w, int video_h,
+                        const ht_video_view *view, const ht_face_redact *redact, int32_t out[4]) {
+  if (!ev || !redact || !out) return HT_ERR_ARG;
+  if (canvas_w < 1 || canvas_h < 1 || canvas_w > 16384 || canvas_h > 16384 || video_w < 1 || video_h < 1 ||
+      video_w > 16384 || video_h > 16384)
+    return HT_ERR_SIZE;
+  ht_face_redact d = *redact;
+  d.mode = HT_REDACT_MOSAIC;
+  if (redact_check(d)) return HT_ERR_ARG;
+  const ht_video_view whole{};
+  ViewFeedRec v{};
+  char why[256];
+  if (view_record(view ? *view : whole, video_w, video_h, v, why) != HT_OK) return HT_ERR_ARG;
+  for (int i = 0; i < 4; ++i) out[i] = 0;
+  const TrackerEvent &e = *reinterpret_cast<const TrackerEvent *>(ev);
+  int r[4];
+  if (!redact_tick(e.detection, e.confidence, e.x, e.y, e.width, e.height) ||
+      !redact_rect(e.detection, e.x, e.y, e.width, e.height, e.angle, canvas_w, canvas_h, v, d.block, d.scale, r))
+    return 0;
+  for (int i = 0; i < 4; ++i) out[i] = r[i];
+  return 1;
+}
+
 static_assert(REC_BYTES == HT_TRACKER_RECORD_BYTES && REC_MAGIC == HT_TRACKER_RECORD_MAGIC &&
                   REC_VERSION == HT_TRACKER_RECORD_VERSION,
               "tracker record (include/headtrackr_b200.h)");
@@ -2525,6 +2660,8 @@ struct TickGroup {
 //   k_hist, k_track  per group: one track() of the CS streams                    src/camshift.js:213-312
 //   k_tracker_update starter, whitebalance gate, facetrackr and main.js transitions, status bits, head epilogue
 //   k_track_init     initTracker for the streams that found their face           src/facetrackr.js:97-108
+// and after them, each only while some stream has one: k_camera_update, k_framing_update, k_debug_strokes, k_face_crop
+// (after k_tracker_update) and, last, k_face_redact, which writes the videos the others read.
 static int tracker_tick(ht_ctx *ctx, const TickGroup *grp, int n_groups, const uint8_t *d_rgba, int n, const int32_t *d_ids,
                         double now_ms, const double *d_now, const FeedDraw *feed, const EntryCanvas *geo,
                         ht_tracker_event *out) {
@@ -2617,12 +2754,12 @@ static int tracker_tick(ht_ctx *ctx, const TickGroup *grp, int n_groups, const u
     k_debug_strokes<<<(unsigned)n, 256, 0, st>>>(d_ids, geo, d_ev, ctx->debug.dev());
     ++ctx->launches;
   }
+  CropSource src{CROP_FRAMES, g0.w, g0.h, 0, d_rgba};     // ht_tracker_step: the frames are the canvases
+  if (feed && feed->view) src = CropSource{CROP_VIEW, 0, 0, 0, feed->view};
+  else if (feed && feed->yuv) src = CropSource{CROP_YUV, 0, 0, 0, feed->yuv};
+  else if (feed) src = CropSource{CROP_FEED, 0, 0, 0, feed->recs};
   if (ctx->crop_count > 0 || ctx->tensor_count > 0) {   // the face crops and tensors of the entries whose record is a
                                                          // kept "CS" face, from this tick's video
-    CropSource src{CROP_FRAMES, g0.w, g0.h, 0, d_rgba};     // ht_tracker_step: the frames are the canvases
-    if (feed && feed->view) src = CropSource{CROP_VIEW, 0, 0, 0, feed->view};
-    else if (feed && feed->yuv) src = CropSource{CROP_YUV, 0, 0, 0, feed->yuv};
-    else if (feed) src = CropSource{CROP_FEED, 0, 0, 0, feed->recs};
     const int tz = ctx->crop_count > 0 ? 1 : 0;           // the tensor slice (unreached without tensors)
     const unsigned slices = (unsigned)(tz + (ctx->tensor_count > 0 ? 1 : 0));
     k_face_crop<<<dim3((unsigned)std::max(ctx->crop_tiles, ctx->tensor_tiles), (unsigned)n, slices), 256, 0, st>>>(
@@ -2637,6 +2774,11 @@ static int tracker_tick(ht_ctx *ctx, const TickGroup *grp, int n_groups, const u
                                   ctx->d_track_cost.as<int32_t>());
   ctx->prof_end(st);
   ctx->launches += 2;
+  if (ctx->redact_count > 0) {   // last: the crops, the tensors and k_track_init have read the unredacted video
+    const int R = std::min(64, std::max(1, 8 * ctx->sms / n));
+    k_face_redact<<<dim3((unsigned)R, (unsigned)n), 256, 0, st>>>(d_ids, geo, g0.w, g0.h, d_ev, ctx->redact.dev(), src);
+    ++ctx->launches;
+  }
   CK(cudaGetLastError());
   ctx->last_plan = gl.P;
   ctx->last_n = gl.n;
@@ -2649,6 +2791,12 @@ int ht_tracker_step(ht_ctx *ctx, const uint8_t *rgba, int n, int w, int h, doubl
   if (!out) return ctx->fail(HT_ERR_ARG, "out is NULL");
   int rc = check_batch(ctx, n);
   if (rc != HT_OK) return rc;
+  for (int k = 0; rgba && k < n && ctx->redact_count > 0; ++k)   // the library writes the frames of redacting streams
+    if (redacting(ctx, k)) {
+      if (!is_device_ptr(rgba))
+        return ctx->fail(HT_ERR_ARG, "stream %d redacts its face, so the frames must be device memory", k);
+      break;
+    }
   CK(cudaSetDevice(ctx->cfg.device));
   Plan *P = nullptr;
   rc = get_plan(ctx, w, h, 5, &P);
@@ -2883,6 +3031,10 @@ static int tracker_feed(ht_ctx *ctx, const ht_canvas_frame *frames, const ht_yuv
       const int rc = check_view(ctx, views[b], vw, vh, b, vrec[(size_t)b]);
       if (rc != HT_OK) return rc;
     }
+  }
+  if (ctx->redact_count > 0) {
+    const int rc = check_redact_videos(ctx, frames, yuv, n);
+    if (rc != HT_OK) return rc;
   }
   struct Group { int w, h, first, n; IngestGeom g; Plan *P; TickGroup tick; size_t base; };
   std::vector<Group> groups;
@@ -3856,6 +4008,45 @@ extern "C" int ht_selftest_face_crop_framed_rgba(const ht_framed_box *box, int c
   if (!crop_map_framed(*box, cw, ch, v.sw, v.sh, f.w, f.h, f.scale, M)) return 0;
   for (int j = 0; j < f.h; ++j)
     for (int i = 0; i < f.w; ++i) reinterpret_cast<uint32_t *>(f.rgba + (size_t)j * f.pitch)[i] = crop_pixel<VIEW_RGBA>(v, M, i, j);
+  return 1;
+}
+// redact_hold_step on the host, as k_face_redact runs it: record `ev` on a cw x ch canvas moves *s (a RedactHold,
+// REDACT_HOLD_BYTES) under a redaction of `hold` ticks -> 1 if the tick redacts (s then holds its box), 0 if not
+extern "C" int ht_selftest_redact_hold(void *s, int hold, const ht_tracker_event *ev, int cw, int ch) {
+  const TrackerEvent &e = *reinterpret_cast<const TrackerEvent *>(ev);
+  return redact_hold_step(*static_cast<RedactHold *>(s), hold, e.detection, e.confidence, e.x, e.y, e.width, e.height,
+                          e.angle, cw, ch) ? 1 : 0;
+}
+extern "C" int ht_selftest_redact_hold_bytes() { return (int)sizeof(RedactHold); }
+// k_face_redact's per-entry code on the host, one lane: the redaction `redact` of an image of any format (img, host
+// planes) or an RGBA8 frame (rgba, rows of `pitch` bytes, 0: 4 * width; exactly one of the two) through a view (NULL:
+// the whole frame upright), for record `ev` on a cw x ch canvas and the hold *s (NULL: none) -> 1 if it redacted, 0
+// if not, or the rejection's code
+extern "C" int ht_selftest_face_redact(const ht_tracker_event *ev, int cw, int ch, const ht_yuv_image *img,
+                                       const ht_video_frame *rgba, const ht_video_view *view, const ht_face_redact *redact,
+                                       void *s) {
+  if (!redact || redact->mode == HT_REDACT_OFF || redact_check(*redact)) return HT_ERR_ARG;
+  ViewFeedRec v{};
+  char why[256];
+  const ht_video_view whole{};
+  const int w = img ? img->width : rgba->width, h = img ? img->height : rgba->height;
+  int rc = view_record(view ? *view : whole, w, h, v, why);
+  if (rc != HT_OK) return rc;
+  if (img) {
+    YuvFeedRec r;
+    rc = yuv_record(*img, r, why);
+    if (rc != HT_OK) return rc;
+    view_source_yuv(v, r);
+  } else {
+    view_source_rgba(v, rgba->rgba, rgba->pitch ? rgba->pitch : 4 * w, w, h);
+  }
+  const TrackerEvent &e = *reinterpret_cast<const TrackerEvent *>(ev);
+  RedactHold none{}, &hs = s ? *static_cast<RedactHold *>(s) : none;
+  int r[4];
+  if (!redact_hold_step(hs, redact->hold, e.detection, e.confidence, e.x, e.y, e.width, e.height, e.angle, cw, ch) ||
+      !redact_rect(hs.detection, hs.x, hs.y, hs.w, hs.h, hs.angle, cw, ch, v, redact->block, redact->scale, r))
+    return 0;
+  redact_cells(v, *redact, r, 0, 1, 0, 1, [](uint32_t x) { return x; });
   return 1;
 }
 // rgba_to_yuv420 over n 2 x 2 blocks: blocks[4k..4k+3] = p00, p01, p10, p11 -> out[6k..6k+5] = their Y, U, V

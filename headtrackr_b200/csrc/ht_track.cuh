@@ -1875,6 +1875,148 @@ __host__ __device__ inline bool crop_map_framed(const ht_framed_box &b, int cw, 
   return true;
 }
 
+// Face redaction (ht_tracker_set_redact; DESIGN.md 2, "Face redaction"): after the tick's crops, the cells of a
+// B x B grid anchored at video pixel (0, 0) that meet the tracked face are overwritten in the video itself, with their
+// mean (mosaic) or a colour (fill).
+// A face tick: a record main.js strokes ("VJ" or "CS" with confidence != 0) with width > 0 and height > 0, its box
+// finite and within 65536 px as crop_tick bounds it.
+__host__ __device__ __forceinline__ bool redact_tick(int detection, double confidence, double x, double y, double w, double h) {
+  if ((detection != 1 && detection != 2) || confidence == 0.0) return false;
+  return crop_tick(2, x, y, w, h);
+}
+// A stream's hold: the box of its last face tick (record fields and canvas size) and the ticks it may still redact
+// without one.  All 0 when the redaction is set.
+struct RedactHold {
+  double x, y, w, h, angle;
+  int32_t detection, cw, ch, remaining;
+};
+// One tick of the hold for a record on a cw x ch canvas.  A face tick stores its box and remaining = hold; any other
+// tick redacts the stored box while remaining > 0, if it ran a pass (detection != 0) on the stored canvas size, and
+// takes one from remaining; an IDLE tick or a canvas-size change ends the hold.  -> whether the tick redacts, s then
+// holding the box it redacts.
+__host__ __device__ inline bool redact_hold_step(RedactHold &s, int hold, int detection, double confidence, double x,
+                                                 double y, double w, double h, double angle, int cw, int ch) {
+  if (redact_tick(detection, confidence, x, y, w, h)) {
+    s.x = x; s.y = y; s.w = w; s.h = h; s.angle = angle;
+    s.detection = detection; s.cw = cw; s.ch = ch; s.remaining = hold;
+    return true;
+  }
+  if (detection == 0 || s.cw != cw || s.ch != ch) {
+    s.remaining = 0;
+    return false;
+  }
+  if (s.remaining <= 0) return false;
+  --s.remaining;
+  return true;
+}
+// The video pixels [r0, r2) x [r1, r3) of source-rectangle pixels [s0, s2) x [s1, s3) through view record v: its map
+// is a signed permutation, so the two opposite corner pixels give the rectangle
+__host__ __device__ __forceinline__ void redact_to_video(const ViewFeedRec &v, int s0, int s1, int s2, int s3, int r[4]) {
+  const int ax = v.bx + v.mxx * s0 + v.mxy * s1, ay = v.by + v.myx * s0 + v.myy * s1;
+  const int bx = v.bx + v.mxx * (s2 - 1) + v.mxy * (s3 - 1), by = v.by + v.myx * (s2 - 1) + v.myy * (s3 - 1);
+  r[0] = ax < bx ? ax : bx; r[1] = ay < by ? ay : by;
+  r[2] = (ax > bx ? ax : bx) + 1; r[3] = (ay > by ? ay : by) + 1;
+}
+// The redacted video rectangle r = [r0, r2) x [r1, r3) of a face box (a face tick's record fields) on a cw x ch canvas
+// drawn from view record v's sw x sh source rectangle.  The region's four corners in canvas pixels - a VJ box upright,
+// a CS box as crop_frame places the green rectangle, each scaled by `scale` about its centre - are computed in fp64,
+// every operation rounded as written, and scaled by sw / cw and sh / ch; pixels floor(min) .. ceil(max) - 1, clipped to
+// the rectangle, go through the view, every B x B cell (grid at video pixel 0) they meet is taken, and that is
+// clipped to the rectangle in video pixels.  -> false for an empty region.
+__host__ __device__ inline bool redact_rect(int detection, double x, double y, double w, double h, double angle, int cw,
+                                            int ch, const ViewFeedRec &v, int block, double scale, int r[4]) {
+  double s = 0.0, c = 1.0, lx = sk_mul(w, 0.5), ly = sk_mul(h, 0.5);     // VJ: the upright box's centre
+  if (detection == 2) crop_frame(w, h, angle, s, c, lx, ly);
+  const double hw = sk_mul(sk_mul(w, scale), 0.5), hh = sk_mul(sk_mul(h, scale), 0.5);
+  const double kx = sk_div((double)v.sw, (double)cw), ky = sk_div((double)v.sh, (double)ch);
+  double x0 = 0.0, x1 = 0.0, y0 = 0.0, y1 = 0.0;
+  for (int i = 0; i < 4; ++i) {
+    const double ax = sk_add(lx, (i & 1) ? hw : -hw), ay = sk_add(ly, (i & 2) ? hh : -hh);
+    const double X = sk_mul(sk_add(x, sk_add(sk_mul(c, ax), -sk_mul(s, ay))), kx);
+    const double Y = sk_mul(sk_add(y, sk_add(sk_mul(s, ax), sk_mul(c, ay))), ky);
+    x0 = i == 0 || X < x0 ? X : x0; x1 = i == 0 || X > x1 ? X : x1;
+    y0 = i == 0 || Y < y0 ? Y : y0; y1 = i == 0 || Y > y1 ? Y : y1;
+  }
+  x0 = fmax(floor(x0), 0.0); y0 = fmax(floor(y0), 0.0);
+  x1 = fmin(ceil(x1), (double)v.sw); y1 = fmin(ceil(y1), (double)v.sh);
+  if (!(x0 < x1) || !(y0 < y1)) return false;
+  int f[4], a[4];
+  redact_to_video(v, (int)x0, (int)y0, (int)x1, (int)y1, f);
+  redact_to_video(v, 0, 0, v.sw, v.sh, a);                          // the source rectangle in video pixels
+  const int B = block;
+  r[0] = f[0] / B * B; r[1] = f[1] / B * B;
+  r[2] = (f[2] + B - 1) / B * B; r[3] = (f[3] + B - 1) / B * B;
+  r[0] = r[0] > a[0] ? r[0] : a[0]; r[1] = r[1] > a[1] ? r[1] : a[1];
+  r[2] = r[2] < a[2] ? r[2] : a[2]; r[3] = r[3] < a[3] ? r[3] : a[3];
+  return true;
+}
+// Sample channel k (0..2) of a view record's video: sample (i, j) at p + j pitch + i step, one byte or (wide) one
+// 16-bit word, covering luma pixels with x >> sx == i and y >> sy == j.  RGBA8 video: R, G, B at step 4.  rgb: the
+// channels are R, G, B (fill_rgb), otherwise Y, U, V (fill_yuv).
+struct RedactChan {
+  uint8_t *p;
+  int32_t pitch, step, sx, sy, wide, rgb;
+};
+__host__ __device__ __forceinline__ RedactChan redact_chan(const ViewFeedRec &v, int k) {
+  const YuvFeedRec &r = v.src;
+  if (v.kind == VIEW_RGBA) return RedactChan{const_cast<uint8_t *>(r.y) + k, r.ypitch, 4, 0, 0, 0, 1};
+  const int wide = r.sample_bytes == 2, rgb = r.rgb;
+  if (k == 0) return RedactChan{const_cast<uint8_t *>(r.y), r.ypitch, r.ystep, 0, 0, wide, rgb};
+  return RedactChan{const_cast<uint8_t *>(k == 1 ? r.u : r.v), k == 1 ? r.upitch : r.vpitch, r.cstep, r.sx, r.sy, wide, rgb};
+}
+// Cell [X0, X1) x [Y0, Y1) (luma pixels) of channel c: its samples [X0 >> sx, ((X1 - 1) >> sx) + 1) x (likewise in y)
+// become (sum + cnt / 2) / cnt of them (mosaic) or `fill` (P010: fill << 8).  Lane `lane` of `lanes` visits samples
+// lane, lane + lanes, ... in row order; sum(v) is the lanes' total, given to every lane (on the host, one lane: v).
+template <class Sum>
+__host__ __device__ __forceinline__ void redact_cell(const RedactChan &c, int X0, int Y0, int X1, int Y1, bool mosaic,
+                                                     uint32_t fill, int lane, int lanes, Sum sum) {
+  const int x0 = X0 >> c.sx, y0 = Y0 >> c.sy, w = ((X1 - 1) >> c.sx) + 1 - x0, y1 = ((Y1 - 1) >> c.sy) + 1;
+  auto walk = [&](auto visit) {
+    int i = lane, j = y0;
+    while (i >= w) i -= w, ++j;
+    while (j < y1) {
+      visit(c.p + (size_t)j * c.pitch + (size_t)(x0 + i) * c.step);
+      i += lanes;
+      while (i >= w) i -= w, ++j;
+    }
+  };
+  uint32_t value = c.wide ? fill << 8 : fill;
+  if (mosaic) {
+    uint32_t part = 0;
+    walk([&](const uint8_t *p) { part += c.wide ? *reinterpret_cast<const uint16_t *>(p) : *p; });
+    const uint32_t cnt = (uint32_t)w * (uint32_t)(y1 - y0);
+    value = (sum(part) + cnt / 2) / cnt;
+  }
+  walk([&](uint8_t *p) {
+    if (c.wide) *reinterpret_cast<uint16_t *>(p) = (uint16_t)value;
+    else *p = (uint8_t)value;
+  });
+}
+// Every cell of redacted rectangle r for channels 0..2 of view record v, cell `first`, first + stride, ... of the row-
+// major cell grid (also run on the host by ht_selftest_face_redact)
+template <class Sum>
+__host__ __device__ __forceinline__ void redact_cells(const ViewFeedRec &v, const ht_face_redact &d, const int r[4], int first,
+                                                      int stride, int lane, int lanes, Sum sum) {
+  const int B = d.block, gx = r[0] / B, gy = r[1] / B;
+  const int nx = (r[2] - 1) / B - gx + 1, ny = (r[3] - 1) / B - gy + 1;
+  for (int cell = first; cell < nx * ny; cell += stride) {
+    const int cx = gx + cell % nx, cy = gy + cell / nx;
+    const int X0 = cx * B > r[0] ? cx * B : r[0], Y0 = cy * B > r[1] ? cy * B : r[1];
+    const int X1 = (cx + 1) * B < r[2] ? (cx + 1) * B : r[2], Y1 = (cy + 1) * B < r[3] ? (cy + 1) * B : r[3];
+    for (int k = 0; k < 3; ++k) {
+      const RedactChan c = redact_chan(v, k);
+      redact_cell(c, X0, Y0, X1, Y1, d.mode == HT_REDACT_MOSAIC, c.rgb ? d.fill_rgb[k] : d.fill_yuv[k], lane, lanes, sum);
+    }
+  }
+}
+// A stream's redaction in the device table: the caller's record (mode HT_REDACT_OFF: none) and its hold, which only
+// k_face_redact and the setter write.  ticket counts the CTAs of a tick's entry that have read the hold.
+struct Redact {
+  ht_face_redact d;
+  RedactHold s;
+  uint32_t ticket, pad_;
+};
+
 // Crop pixel (i, j) of the map M over view record v (map, source rectangle and texel source resolved): bilinear with
 // 8-bit weights between the taps (U >> 16, V >> 16) and their right and lower neighbours, taken in the rectangle and
 // mapped to the video through the view, so a turned or mirrored video samples the same taps with the same weights as
@@ -2140,6 +2282,41 @@ __global__ void k_framing_update(const int32_t *__restrict__ ids, const EntryCan
 __global__ void k_framing_reset(const ht_framing *__restrict__ framing, int first, int n) {
   for (int i = threadIdx.x; i < n; i += blockDim.x)
     if (framing[first + i].box) *framing[first + i].box = ht_framed_box{};
+}
+
+// The tick's last launch, after k_face_crop and k_track_init have read the video: grid (R, batch entries).  Thread 0
+// of each of entry k's R CTAs resolves its video (src), its record (events[geo[k].record], geo NULL: k; canvas geo[k],
+// geo NULL: cw x ch), the hold of its stream's redaction and the redacted rectangle; the CTAs then share out the cells,
+// one warp per cell.  Each CTA reads the hold before it takes a ticket, and the entry's last ticket writes the hold
+// back, so every CTA sees the hold as the tick found it.  Entries whose stream has no redaction exit at once.
+__global__ void __launch_bounds__(256) k_face_redact(const int32_t *__restrict__ ids, const EntryCanvas *__restrict__ geo,
+                                                     int cw, int ch, const TrackerEvent *__restrict__ events,
+                                                     Redact *redact, CropSource src) {
+  const int k = blockIdx.y, id = ids ? ids[k] : k;
+  Redact &t = redact[id];
+  if (t.d.mode == HT_REDACT_OFF) return;
+  __shared__ ViewFeedRec v;
+  __shared__ int r[4], on;
+  if (threadIdx.x == 0) {
+    crop_source(src, k, v);
+    const TrackerEvent &e = events[geo ? geo[k].record : k];
+    const int ew = geo ? geo[k].w : cw, eh = geo ? geo[k].h : ch;
+    RedactHold s = t.s;
+    on = redact_hold_step(s, t.d.hold, e.detection, e.confidence, e.x, e.y, e.width, e.height, e.angle, ew, eh) &&
+         redact_rect(s.detection, s.x, s.y, s.w, s.h, s.angle, ew, eh, v, t.d.block, t.d.scale, r);
+    __threadfence();
+    if (atomicAdd(&t.ticket, 1u) == gridDim.x - 1) {
+      t.s = s;
+      t.ticket = 0;
+    }
+  }
+  __syncthreads();
+  if (!on) return;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  redact_cells(v, t.d, r, (int)blockIdx.x * 8 + warp, (int)gridDim.x * 8, lane, 32, [](uint32_t x) {
+    for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
+    return x;
+  });
 }
 
 // ht_tracker_set_camera: one CTA constructs the cameras of streams [first, first + n) that have a controller

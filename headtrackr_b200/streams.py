@@ -168,7 +168,8 @@ class TrackerSet:
     face.  A stream's "faceTensor" key is its face tensor, a dict as Context.tracker_set_face_tensor takes: the same
     face as a model's normalised input, independent of "faceCrop".  A stream's "framing" key is its framing, a dict as
     Context.tracker_set_framing takes: a steady face-cam box in its `out` tensor that the crop (and, with "tensor":
-    True, the tensor) is cut from instead of the tracked box.
+    True, the tensor) is cut from instead of the tracked box.  A stream's "redact" key is its face redaction, a dict
+    as Context.tracker_set_redact takes: its tracked face hidden in its own (device) video after each tick.
     Differs from the reference in one place: start() on a running stream does nothing (the reference runs an extra,
     unscheduled pass)."""
 
@@ -206,6 +207,9 @@ class TrackerSet:
         framings = [(p or {}).get("framing") for p in (params if per_stream else [params] * n_streams)]
         if any(f is not None for f in framings):   # and framings
             context.tracker_set_framing(0, framings)
+        redactions = [(p or {}).get("redact") for p in (params if per_stream else [params] * n_streams)]
+        if any(r is not None for r in redactions):   # and face redactions
+            context.tracker_set_redact(0, redactions)
 
     def set_params(self, k, params):
         """The parameters of stream k (a dict as for the constructor).  Its state is kept: calcAngles takes effect at
@@ -219,6 +223,7 @@ class TrackerSet:
         self.ctx.tracker_set_face_crop(k, [(params or {}).get("faceCrop")])   # no "faceCrop" key: none
         self.ctx.tracker_set_face_tensor(k, [(params or {}).get("faceTensor")])   # no "faceTensor" key: none
         self.ctx.tracker_set_framing(k, [(params or {}).get("framing")])   # no "framing" key: none
+        self.ctx.tracker_set_redact(k, [(params or {}).get("redact")])   # no "redact" key: none
 
     def addEventListener(self, fn):
         """fn(stream_index, evt): evt is a headtrackrStatus / facetrackingEvent / headtrackingEvent payload dict."""

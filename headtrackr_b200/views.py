@@ -12,7 +12,7 @@ import ctypes as C
 import math
 
 from . import framing
-from ._lib import HT_VIEW_MIRROR, FaceCrop, TrackerEvent, VideoView, lib
+from ._lib import HT_REDACT_MOSAIC, HT_VIEW_MIRROR, FaceCrop, FaceRedact, TrackerEvent, VideoView, lib
 
 # EXIF orientation tag (1..8) -> view orientation; a tag says how to turn the stored image to show it upright
 EXIF_ORIENTATION = {1: 0, 2: 4, 3: 2, 4: 6, 5: 5, 6: 1, 7: 7, 8: 3}
@@ -149,6 +149,35 @@ def crop_map(view, width, height, canvas_w, canvas_h, record, crop_w, crop_h, sc
                                 C.addressof(crop), out)
     if rc < 0:
         raise ValueError(f"ht_face_crop_map rejected its arguments ({rc})")
+    return tuple(out) if rc == 1 else None
+
+
+def _event(record):
+    """an ht_tracker_event of a record dict (detection "VJ" / "CS" / 1 / 2, x, y, width, height, angle, confidence)"""
+    if isinstance(record, TrackerEvent):
+        return record
+    ev = TrackerEvent()
+    det = record.get("detection", 0)
+    ev.detection = {"VJ": 1, "CS": 2}.get(det, 0) if isinstance(det, str) else int(det)
+    for k in ("x", "y", "width", "height", "angle"):
+        setattr(ev, k, float(record.get(k, 0.0)))
+    ev.confidence = float(record.get("confidence", 1.0))
+    return ev
+
+
+def redact_rect(view, width, height, canvas_w, canvas_h, record, block=16, scale=1.25):
+    """ht_face_redact_rect: the video pixels (x0, y0, x1, y1), half-open, that a face redaction with cells of `block`
+    px and `scale` hides for a tracker record (a dict or an ht_tracker_event) on a canvas_w x canvas_h canvas drawn
+    from a width x height video through `view`, exactly as the device computes them (DESIGN.md 2, "Face
+    redaction").  -> None when the record is not a face tick or the region is empty."""
+    vv = video_view(view)
+    d = FaceRedact(HT_REDACT_MOSAIC, int(block), 0)
+    d.scale = float(scale)
+    out, ev = (C.c_int32 * 4)(), _event(record)
+    rc = lib().ht_face_redact_rect(C.addressof(ev), int(canvas_w), int(canvas_h), int(width), int(height),
+                                   C.addressof(vv), C.addressof(d), out)
+    if rc < 0:
+        raise ValueError(f"ht_face_redact_rect rejected its arguments ({rc})")
     return tuple(out) if rc == 1 else None
 
 

@@ -265,7 +265,9 @@ int ht_tracker_reset(ht_ctx *ctx, int first, int n);   /* new headtrackr.Tracker
 int ht_tracker_start(ht_ctx *ctx, int first, int n);   /* start(): the next frame of the stream goes through starter() */
 int ht_tracker_stop(ht_ctx *ctx, int first, int n);    /* stop() (src/main.js:347-355); the caller emits "stopped" */
 /* one frame per stream for streams [0, n): rgba = n frames, stream-major; now_ms = (new Date).getTime() of this tick
- * (the "hints" timer, src/main.js:187-194); out[n] host or device (device: enqueue only) */
+ * (the "hints" timer, src/main.js:187-194); out[n] host or device (device: enqueue only).  While one of the streams
+ * has a face redaction (ht_tracker_set_redact) the library writes the frames in place, and they must be device
+ * memory (HT_ERR_ARG otherwise, nothing enqueued). */
 int ht_tracker_step(ht_ctx *ctx, const uint8_t *rgba, int n, int w, int h, double now_ms, ht_tracker_event *out);
 
 /* One stream's video frame for ht_tracker_feed (ABI 1.2). */
@@ -292,6 +294,8 @@ typedef struct {
  * stream id out of range or listed twice, a NULL pixel pointer, a pointer or pitch that is not a multiple of 4, a
  * pitch below 4*width, or a first pointer whose memory space contradicts frames_on_device; HT_ERR_SIZE for a video
  * size outside 1..16384 or a canvas that is 0-sized, larger than max_width x max_height or too small for the pyramid.
+ * A record whose stream has a face redaction (ht_tracker_set_redact) must have device video that shares no byte with
+ * another redacting record's; the library writes it in place (HT_ERR_ARG otherwise, nothing enqueued).
  * ht_tracker_step and ht_tracker_feed may be mixed on one context: both tick the same per-stream state.  In both, the
  * "VJ" pick is over the whole grouped list (as for ht_stream_step), unless the raw list overflowed (HT_WARN_OVERFLOW). */
 int ht_tracker_feed(ht_ctx *ctx, const ht_video_frame *frames, int n, int frames_on_device, int canvas_w, int canvas_h,
@@ -659,6 +663,70 @@ int ht_tracker_set_framing(ht_ctx *ctx, int first, int n, const ht_framing *fram
  * for a box that is not valid (out all 0), or the errors of ht_face_crop_map. */
 int ht_face_crop_map_framed(const ht_framed_box *box, int canvas_w, int canvas_h, int video_w, int video_h,
                             const ht_video_view *view, const ht_face_crop *crop, int64_t out[6]);
+
+/* A stream's face redaction: its tracked face hidden in its own video, in place, after the tick's crops (DESIGN.md 2,
+ * "Face redaction").  headtrackr tracks ONE face per stream: this hides the stream's tracked face, it is not a
+ * detector of every face in the frame.  Explicit values: the wrappers' defaults (mosaic, block 16, scale 1.25, hold
+ * 10, black) belong to the wrappers.  Byte offsets:
+ *     0  int32  mode          HT_REDACT_OFF (removes the redaction), HT_REDACT_MOSAIC or HT_REDACT_FILL
+ *     4  int32  block         B, the cell size in video pixels: even, 2..128
+ *     8  int32  hold          0..65535 ticks the last face box stays redacted after the face is lost
+ *    12  uint8  fill_rgb[3]   HT_REDACT_FILL on RGBA8 video and the packed RGB formats: R, G, B
+ *    15  uint8  pad0          0
+ *    16  uint8  fill_yuv[3]   HT_REDACT_FILL on the YUV formats: Y, U, V (8-bit; P010 writes v << 8)
+ *    19  uint8  pad1          0
+ *    20  int32  pad_          0
+ *    24  double scale         the face box is scaled by this about its centre; finite, in (0, 16] */
+#define HT_REDACT_OFF 0
+#define HT_REDACT_MOSAIC 1
+#define HT_REDACT_FILL 2
+typedef struct {
+  int32_t mode;
+  int32_t block;
+  int32_t hold;
+  uint8_t fill_rgb[3];
+  uint8_t pad0;
+  uint8_t fill_yuv[3];
+  uint8_t pad1;
+  int32_t pad_;
+  double scale;
+} ht_face_redact;         /* 32 bytes */
+/* Stream first+i gets redactions[i] (host array), for i in [0, n); stream states are kept, and the stream's hold
+ * starts empty.  The library then WRITES the stream's video - the frames given to ht_tracker_step, the feed record's
+ * planes - in place, although those pointers are const:
+ *   face ticks   a record main.js strokes ("VJ" or "CS" with confidence != 0, the VJ tick that finds the face included,
+ *                the CS tick that loses it not) with width, height > 0 and x, y, width, height finite and within 65536
+ *   region       the VJ box upright, or the CS green rectangle as the face crop places it (angle - pi/2 about (x, y),
+ *                a NaN angle unrotated), scaled by `scale` about its centre, its corners in fp64 scaled by sw / cw and
+ *                sh / ch into the view's sw x sh source rectangle (the video without a view, the canvas for
+ *                ht_tracker_step); pixels floor(min) .. ceil(max) - 1, clipped to the rectangle, through the view
+ *   cells        every cell of a B x B grid anchored at video pixel (0, 0) that meets that, clipped to the rectangle
+ *   values       in each channel a cell covers samples [x0 >> sx, ((x1 - 1) >> sx) + 1) (likewise in y), which become
+ *                their integer mean (sum + cnt / 2) / cnt (mosaic; P010 on whole 16-bit words) or the fill; nothing
+ *                else is written: no alpha, no pitch padding, no other pixel
+ *   hold         a face tick stores its box and canvas size and sets remaining = hold; a later tick that ran a pass
+ *                (detection != 0) on the same canvas size redacts that box through its own view and video while
+ *                remaining > 0, taking one from it.  An IDLE tick, a canvas-size change or setting the redaction
+ *                again ends the hold.
+ * It runs last in the tick, after the face crops, tensors and the camshift model have read the unredacted video.  The
+ * redaction belongs to the stream id: stop, start, reset, a lost face, ht_tracker_set_params and ht_tracker_import keep
+ * it; ht_tracker_config removes every stream's.  A tick launches one more kernel while some stream has a redaction,
+ * and nothing more otherwise.  It writes no caller buffer of its own, so the overlap rule of the outputs is unchanged.
+ * Two rules then hold for every tick (ht_tracker_step and every feed), checked before anything is enqueued, with the
+ * record named: a redacting stream's video must be device memory (a staged copy would hide the result), and no two
+ * redacting records of one tick may have video planes that share a byte (their cells would race): one camera frame
+ * shared through views may be redacted by one stream only.  Streams without a redaction are not affected.
+ * Errors (nothing changes; the message names the record): HT_ERR_STATE before ht_tracker_config; HT_ERR_ARG for a
+ * range outside [0, max_frames), n <= 0, redactions NULL, a mode other than the three, a block that is odd or outside
+ * 2..128, a hold outside 0..65535, a non-zero pad, or a scale that is not finite or outside (0, 16]. */
+int ht_tracker_set_redact(ht_ctx *ctx, int first, int n, const ht_face_redact *redactions);
+/* The video rectangle a redaction `redact` (mode ignored) hides for face record `ev` on a canvas_w x canvas_h canvas
+ * drawn from a video_w x video_h video through `view` (NULL: the whole frame upright), exactly as the device computes
+ * it: video pixels [out[0], out[2]) x [out[1], out[3]), aligned to the B grid and clipped to the source rectangle.
+ * Host only; needs no context.  -> 1, 0 for a record that is not a face tick or an empty region (out all 0),
+ * HT_ERR_ARG for NULL pointers or a bad redaction or view, HT_ERR_SIZE for a canvas or video outside 1..16384. */
+int ht_face_redact_rect(const ht_tracker_event *ev, int canvas_w, int canvas_h, int video_w, int video_h,
+                        const ht_video_view *view, const ht_face_redact *redact, int32_t out[4]);
 
 /* A stream's head-coupled camera: the three.js r48 PerspectiveCamera that realisticAbsoluteCameraControl moves
  * (src/controllers.js:28-68), in caller-owned DEVICE memory that a renderer can bind directly.  Byte offsets:

@@ -35,6 +35,8 @@
 //        realisticAbsoluteCameraControl on an ht_camera in device memory)
 //   trackerSetFraming(handle, first, [framing|null, ...])  (ht_tracker_set_framing: each stream's steady face-cam box,
 //        an ht_framed_box in device memory, that its crop and / or tensor is cut from)
+//   trackerSetRedact(handle, first, [redaction|null, ...])  (ht_tracker_set_redact: each stream's tracked face hidden
+//        in its own device video after each tick, a mosaic or a fill)
 //   trackerExport(handle, [stream, ...]) -> Buffer of records; trackerImport(handle, [stream, ...], records)
 //        (ht_tracker_export / ht_tracker_import: a stream's whole Tracker as HT_TRACKER_RECORD_BYTES per stream)
 //   trackerFeed(handle, [{stream, rgba, width, height, nowMs, canvasWidth?, canvasHeight?}], canvasWidth, canvasHeight)
@@ -724,6 +726,57 @@ static napi_value TrackerSetFraming(napi_env env, napi_callback_info info) {
   return nullptr;
 }
 
+// trackerSetRedact(handle, first, [{mode?: "mosaic" | "fill", block?, scale?, hold?, fillRgb?: [r, g, b],
+// fillYuv?: [y, u, v]}, null, ...]): stream first+i gets redactions[i]; null or undefined: none.  The defaults are the
+// Python wrapper's: mosaic, block 16, scale 1.25, hold 10, black.
+static napi_value TrackerSetRedact(napi_env env, napi_callback_info info) {
+  size_t argc = 3;
+  napi_value argv[3];
+  NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+  ht_ctx *ctx = Ctx(env, argv[0]);
+  int32_t first = 0;
+  uint32_t n = 0;
+  napi_get_value_int32(env, argv[1], &first);
+  NAPI_OK(napi_get_array_length(env, argv[2], &n));
+  std::vector<ht_face_redact> rs(n);
+  memset(rs.data(), 0, n * sizeof(ht_face_redact));
+  for (uint32_t i = 0; i < n; ++i) {
+    napi_value r, v;
+    napi_valuetype t = napi_undefined;
+    NAPI_OK(napi_get_element(env, argv[2], i, &r));
+    napi_typeof(env, r, &t);
+    if (t != napi_object) continue;
+    ht_face_redact &d = rs[i];
+    d.mode = HT_REDACT_MOSAIC;
+    char mode[16] = "";
+    size_t len = 0;
+    if (napi_get_named_property(env, r, "mode", &v) == napi_ok &&
+        napi_get_value_string_utf8(env, v, mode, sizeof(mode), &len) == napi_ok && strcmp(mode, "fill") == 0)
+      d.mode = HT_REDACT_FILL;
+    else if (len > 0 && strcmp(mode, "mosaic") != 0)
+      d.mode = -1;                                   // refused by the library, naming the record
+    d.block = (int32_t)GetNumber(env, r, "block", 16);
+    d.hold = (int32_t)GetNumber(env, r, "hold", 10);
+    d.scale = GetNumber(env, r, "scale", 1.25);
+    const uint8_t yuv_black[3] = {16, 128, 128};
+    for (int k = 0; k < 3; ++k) d.fill_yuv[k] = yuv_black[k];
+    for (int c = 0; c < 2; ++c) {
+      napi_value arr, e;
+      bool is_array = false;
+      if (napi_get_named_property(env, r, c ? "fillYuv" : "fillRgb", &arr) != napi_ok) continue;
+      napi_is_array(env, arr, &is_array);
+      for (uint32_t k = 0; is_array && k < 3; ++k) {
+        int32_t x = 0;
+        if (napi_get_element(env, arr, k, &e) == napi_ok && napi_get_value_int32(env, e, &x) == napi_ok)
+          (c ? d.fill_yuv : d.fill_rgb)[k] = (uint8_t)x;
+      }
+    }
+  }
+  int rc = ht_tracker_set_redact(ctx, first, (int)n, rs.data());
+  if (rc < 0) return Throw(env, ctx, rc);
+  return nullptr;
+}
+
 // stream ids of an Array of numbers
 static bool GetStreams(napi_env env, napi_value arr, std::vector<int32_t> *ids) {
   uint32_t n = 0;
@@ -1084,6 +1137,7 @@ static napi_value Init(napi_env env, napi_value exports) {
       {"trackerSetFaceTensor", nullptr, TrackerSetFaceTensor, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerSetCamera", nullptr, TrackerSetCamera, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerSetFraming", nullptr, TrackerSetFraming, nullptr, nullptr, nullptr, napi_default, nullptr},
+      {"trackerSetRedact", nullptr, TrackerSetRedact, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerExport", nullptr, TrackerExport, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerImport", nullptr, TrackerImport, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerFeed", nullptr, TrackerFeed, nullptr, nullptr, nullptr, napi_default, nullptr},

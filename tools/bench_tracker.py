@@ -37,6 +37,9 @@ streams: N 640x480 streams, device-resident frames and outputs, CUDA events arou
   framing*_*      (--framing) the --crops workload with 224x224 NV12 crops on every stream, with a framing on no, every
                   and every 64th stream (no framing also against --before-lib), arms alternating tick by tick
                   (framing_arms)
+  redact*_*       (--redact) 1024 streams of 1280x720 NV12 onto 320x240 canvases with a mosaic (B = 16, scale 1.5) on
+                  no, every and every 64th stream (no redaction also against --before-lib), arms alternating tick by
+                  tick, each arm on its own copy of the video (redact_arms)
 
 Prints one JSON line with the card's name and power limit read in the same run; --out also writes it to a file."""
 import argparse
@@ -1506,6 +1509,90 @@ def framing_arms(torch, stream, N, steps, rounds, before_lib=None):
     return res
 
 
+def redact_arms(torch, stream, N, steps, rounds, before_lib=None):
+    """N streams of 1280x720 NV12 through ht_tracker_feed_yuv onto 320x240 canvases, with arms alternating tick by
+    tick: redaction off (redactoff_cs), off on another build (redactoff_before_cs, --before-lib), a mosaic (B = 16,
+    scale 1.5) on every stream (redactall_cs) and on every 64th stream (redact64_cs).  The redaction writes the video,
+    so every arm has its own copy, restored from the pristine planes before each tick, outside the timed window.  The
+    records of every arm must agree on every timed tick."""
+    import ctypes as C
+    from headtrackr_b200 import Context, _lib
+    from headtrackr_b200.context import _yuv_image
+    W, H, CW, CH = 1280, 720, 320, 240
+    rec_bytes = C.sizeof(_lib.TrackerEvent)
+    now = [1.0e12]
+    kw = dict(max_width=CW, max_height=CH, max_frames=N, stream=stream)
+    ys, uvs = nv12_streams(torch, N, W, H)
+
+    def arm(every, before=False):
+        c = other_build_context(before_lib, **kw) if before else Context(**kw)
+        c.tracker_config()
+        c.tracker_reset(0, N)
+        c.tracker_start(0, N)
+        if every:
+            c.tracker_set_redact(0, [{"mode": "mosaic", "block": 16, "scale": 1.5} if k % every == 0 else None
+                                     for k in range(N)])
+        y, uv = [t.clone() for t in ys], [t.clone() for t in uvs]
+        keep = []
+        imgs = [_yuv_image((y[k], uv[k]), "nv12", "bt601", keep)[0] for k in range(N)]
+        recs = (_lib.YuvFrame * N)()
+        for k in range(N):
+            recs[k] = _lib.YuvFrame(imgs[k], k, CW, CH, 0, 0.0)
+        out = torch.empty(N * rec_bytes, dtype=torch.uint8, device="cuda")
+
+        def restore():
+            for k in range(N):
+                y[k].copy_(ys[k])
+                uv[k].copy_(uvs[k])
+
+        def run():
+            for k in range(N):
+                recs[k].now_ms = now[0]
+            c._check(c._L.ht_tracker_feed_yuv(c._h, C.addressof(recs), N, 1, out.data_ptr()))
+        return c, run, out, restore, (y, uv, keep)
+
+    arms = {"redactoff_cs": arm(0), "redactall_cs": arm(1), "redact64_cs": arm(64)}
+    if before_lib:
+        arms["redactoff_before_cs"] = arm(0, before=True)
+    names = list(arms)
+
+    def tick(name):
+        _, run, _, restore, _ = arms[name]
+        restore()
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        a.record()
+        run()
+        b.record()
+        b.synchronize()
+        return a.elapsed_time(b)
+
+    for _ in range(17):                          # the whitebalance gate, detection, the first CS frames
+        now[0] += 20.0
+        for name in names:
+            tick(name)
+    times = {name: [[] for _ in range(rounds)] for name in names}
+    for r in range(rounds):
+        for s in range(steps):
+            now[0] += 20.0
+            rot = (r * steps + s) % len(names)
+            for name in names[rot:] + names[:rot]:
+                times[name][r].append(tick(name))
+            first = arms[names[0]][2]
+            if any(not torch.equal(first, arms[name][2]) for name in names[1:]):
+                raise SystemExit("redaction arms disagree on the records of a timed tick")
+    res = {}
+    for name in names:
+        med = [float(np.median(t)) for t in times[name]]
+        res[f"{name}_ms"] = float(np.median(sum(times[name], [])))
+        res[f"{name}_spread_ms"] = max(med) - min(med)
+    res["redact_records_agree"] = True
+    y = arms["redactall_cs"][4][0]
+    res["redact_streams_changed"] = sum(int(not torch.equal(y[k], ys[k])) for k in range(N))
+    for c, _, _, _, _ in arms.values():
+        c.close()
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--streams", type=int, default=1024)
@@ -1522,6 +1609,7 @@ def main():
     ap.add_argument("--views", action="store_true", help="only the video-view arms (views_arms)")
     ap.add_argument("--crops", action="store_true", help="only the face-crop arms (crops_arms)")
     ap.add_argument("--framing", action="store_true", help="only the framing arms (framing_arms)")
+    ap.add_argument("--redact", action="store_true", help="only the face-redaction arms (redact_arms)")
     ap.add_argument("--out")
     a = ap.parse_args()
     import torch
@@ -1546,6 +1634,9 @@ def main():
         return report(res, a.out)
     if a.framing:
         res.update(framing_arms(torch, stream, N, a.steps, a.rounds, a.before_lib))
+        return report(res, a.out)
+    if a.redact:
+        res.update(redact_arms(torch, stream, N, a.steps, a.rounds, a.before_lib))
         return report(res, a.out)
     if a.formats:
         res.update(formats_arms(torch, stream, N, a.steps, a.rounds, a.before_lib))
