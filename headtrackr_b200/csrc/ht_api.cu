@@ -671,6 +671,23 @@ int join_aux(ht_ctx *ctx) {
   return HT_OK;
 }
 
+// (ht_set_pipeline) where the pipelined call of parity `parity` puts its bin planes and current-frame histograms, for
+// a bin-plane buffer of cap_bytes (element offsets into ctx->bins / ctx->cur_hist).  grow_bytes > 0: the buffer must
+// first grow to that size, behind a synchronisation of both streams.
+// The parities are the two halves of the buffer, whatever the frame size of the call: the tracking of call s reads its
+// half while the gray pass of call s+1 writes the other one, unordered, also when the two calls differ in frame or
+// batch size (a half cut from this call's w * h would overlap the previous call's planes).  The buffer only changes
+// behind the synchronisation, so consecutive calls always cut the same halves.  Halves are whole multiples of 8
+// entries: every slice is 16-byte aligned.  (At one frame size with max_frames * w * h a multiple of 8 the halves are
+// exactly max_frames * w * h entries.)
+struct PipeSlices { size_t grow_bytes, bins_off, hist_off; };
+__host__ inline PipeSlices pipe_plane_offsets(int parity, size_t cap_bytes, int max_frames, int w, int h) {
+  const size_t plane_elems = ((size_t)max_frames * w * h + 7) & ~(size_t)7;   // one parity's bin planes
+  const size_t need = 2 * plane_elems * sizeof(uint16_t);
+  const size_t half = (std::max(cap_bytes, need) / sizeof(uint16_t) / 2) & ~(size_t)7;
+  return PipeSlices{cap_bytes < need ? need : 0, (size_t)parity * half, (size_t)parity * max_frames * 4096};
+}
+
 int get_plan(ht_ctx *ctx, int w, int h, int interval, Plan **out) {
   if (w <= 0 || h <= 0 || interval < 0 || interval > 15) return ctx->fail(HT_ERR_ARG, "bad w/h/interval");
   if (w > ctx->cfg.max_width || h > ctx->cfg.max_height)
@@ -1516,18 +1533,18 @@ int ht_detect_track(ht_ctx *ctx, const uint8_t *rgba, int n, int w, int h, int i
   int32_t *d_counts = io.dst<int32_t>(o_counts), *d_found = io.dst<int32_t>(o_found);
   int32_t *d_objs = io.dst<int32_t>(o_objs), *d_win = io.dst<int32_t>(o_win);
   if (deferred) {
-    const size_t plane_elems = (size_t)ctx->cfg.max_frames * w * h;     // one parity's bin planes
-    if (ctx->bins.cap < 2 * plane_elems * sizeof(uint16_t)) {
+    const PipeSlices ps = pipe_plane_offsets(ctx->pipe_parity ^ 1, ctx->bins.cap, ctx->cfg.max_frames, w, h);
+    if (ps.grow_bytes) {
       if (ctx->aux_stream) CK(cudaStreamSynchronize(ctx->aux_stream));   // the buffer about to be replaced may still be read
       CK(cudaStreamSynchronize(st));
-      CK(ctx->bins.reserve(2 * plane_elems * sizeof(uint16_t)));
+      CK(ctx->bins.reserve(ps.grow_bytes));
     }
     rc = ensure_aux_stream(ctx, true);
     if (rc != HT_OK) return rc;
     if (!ctx->pipe_detect_done) CK(cudaEventCreateWithFlags(&ctx->pipe_detect_done.h, cudaEventDisableTiming));
     ctx->pipe_parity ^= 1;
-    ctx->bins_off = (size_t)ctx->pipe_parity * plane_elems;
-    ctx->hist_off = (size_t)ctx->pipe_parity * (size_t)ctx->cfg.max_frames * 4096;
+    ctx->bins_off = ps.bins_off;
+    ctx->hist_off = ps.hist_off;
     rc = run_detect(ctx, st, P, rgba, 0, n, min_neighbors, d_rects, d_counts,
                     HistOut{ctx->cur_hist.as<uint32_t>() + ctx->hist_off, ctx->bins.as<uint16_t>() + ctx->bins_off}, nullptr,
                     ctx->aux_pending ? ctx->aux_done.h : nullptr);
@@ -3631,6 +3648,13 @@ extern "C" int ht_selftest_planes(int w, int h, int interval, int32_t *out, int 
     o[0] = (int32_t)P.planes[i].off; o[1] = P.planes[i].pitch; o[2] = P.planes[i].w; o[3] = P.planes[i].h; o[4] = slot; o[5] = q;
   }
   return 0;
+}
+
+// the bin-plane / histogram slices of a pipelined ht_detect_track call (pipe_plane_offsets) -> out[3] = {grow_bytes,
+// bins_off, hist_off}
+extern "C" void ht_selftest_pipe_offsets(int parity, size_t cap_bytes, int max_frames, int w, int h, uint64_t *out) {
+  const PipeSlices ps = pipe_plane_offsets(parity, cap_bytes, max_frames, w, h);
+  out[0] = ps.grow_bytes; out[1] = ps.bins_off; out[2] = ps.hist_off;
 }
 
 // the head-position epilogue of k_stream_update (head_step) over a sequence of CS results of one stream

@@ -869,7 +869,9 @@ int ht_set_track_memo(ht_ctx *ctx, int enable);
  * unpipelined call.  The caller's side of the contract: out_found / out_objs / out_windows of call s are complete
  * after ht_sync or ht_join (or any other entry point of the context, which all join first) - NOT merely after the
  * next ht_detect_track; out_rects / out_counts may be reused by the next call (the library orders the accesses);
- * the frames of call s must stay unchanged until then as well. */
+ * the frames of call s must stay unchanged until then as well.  Consecutive pipelined calls may differ in frame size,
+ * batch size and interval: the bin planes of the two calls in flight are the two fixed halves of one buffer, sized
+ * for the largest max_frames x w x h pipelined so far (it grows only behind a synchronisation). */
 int ht_set_pipeline(ht_ctx *ctx, int enable);
 /* Stream-level join: later work on the context's stream waits for a pipelined call's tracking.  No host wait. */
 int ht_join(ht_ctx *ctx);
