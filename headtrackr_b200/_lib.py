@@ -206,6 +206,31 @@ class FaceRedact(C.Structure):
 assert C.sizeof(FaceRedact) == 32 and FaceRedact.fill_rgb.offset == 12 and FaceRedact.fill_yuv.offset == 16 \
     and FaceRedact.pad_.offset == 20 and FaceRedact.scale.offset == 24
 
+# ht_best_shot_state.flags
+HT_BEST_BEGAN, HT_BEST_IMPROVED, HT_BEST_ENDED = 1, 2, 4
+
+
+class BestShotState(C.Structure):
+    """ht_best_shot_state: a stream's best-shot state (BEST_SHOT_STATE_BYTES, in device memory; bestshot.state_from_bytes
+    decodes it)"""
+    _fields_ = [("best_score", C.c_uint64), ("score", C.c_uint64), ("x", C.c_double), ("y", C.c_double),
+                ("width", C.c_double), ("height", C.c_double), ("angle", C.c_double), ("now_ms", C.c_double),
+                ("canvas_w", C.c_int32), ("canvas_h", C.c_int32), ("track", C.c_uint32), ("ended", C.c_uint32),
+                ("ticks", C.c_uint32), ("best_tick", C.c_uint32), ("buffer", C.c_int32), ("flags", C.c_uint32)]
+
+
+class BestShot(C.Structure):
+    """ht_best_shot: one stream's best shot for ht_tracker_set_best_shot (device memory; rgba[0] NULL = none, rgba[1]
+    NULL = one image; 3..2048 pixels a side; pitch 0 = 4 * width; scale in (0, 16])"""
+    _fields_ = [("rgba", C.c_void_p * 2), ("state", C.c_void_p), ("width", C.c_int32), ("height", C.c_int32),
+                ("pitch", C.c_int32), ("pad_", C.c_int32), ("scale", C.c_double)]
+
+
+BEST_SHOT_STATE_BYTES = 96
+assert C.sizeof(BestShotState) == BEST_SHOT_STATE_BYTES and BestShotState.now_ms.offset == 56 \
+    and BestShotState.track.offset == 72 and BestShotState.flags.offset == 92 and C.sizeof(BestShot) == 48 \
+    and BestShot.state.offset == 16 and BestShot.scale.offset == 40
+
 # ht_tracker_export / ht_tracker_import: bytes of one tracker record (HT_TRACKER_RECORD_BYTES)
 TRACKER_RECORD_BYTES = 16864
 
@@ -249,7 +274,7 @@ _lib = None
 
 EXPORTS = ["ht_version", "ht_create", "ht_destroy", "ht_last_error", "ht_sync", "ht_max_rects", "ht_detect",
            "ht_track_init", "ht_track_init_from_detect", "ht_track", "ht_detect_track", "ht_stream_reset", "ht_stream_step", "ht_stream_head_config", "ht_stream_step_head",
-           "ht_tracker_config", "ht_tracker_reset", "ht_tracker_start", "ht_tracker_stop", "ht_tracker_step", "ht_tracker_feed", "ht_tracker_set_params", "ht_tracker_feed_canvases", "ht_tracker_set_debug", "ht_tracker_set_debug_strokes", "ht_tracker_set_face_crop", "ht_tracker_set_face_crop_yuv", "ht_tracker_set_face_tensor", "ht_face_crop_map", "ht_tracker_set_framing", "ht_face_crop_map_framed", "ht_tracker_set_redact", "ht_face_redact_rect", "ht_tracker_set_camera", "ht_tracker_export", "ht_tracker_import", "ht_tracker_feed_yuv", "ht_ingest", "ht_ingest_yuv",
+           "ht_tracker_config", "ht_tracker_reset", "ht_tracker_start", "ht_tracker_stop", "ht_tracker_step", "ht_tracker_feed", "ht_tracker_set_params", "ht_tracker_feed_canvases", "ht_tracker_set_debug", "ht_tracker_set_debug_strokes", "ht_tracker_set_face_crop", "ht_tracker_set_face_crop_yuv", "ht_tracker_set_face_tensor", "ht_face_crop_map", "ht_tracker_set_framing", "ht_face_crop_map_framed", "ht_tracker_set_redact", "ht_face_redact_rect", "ht_tracker_set_best_shot", "ht_best_shot_score", "ht_tracker_set_camera", "ht_tracker_export", "ht_tracker_import", "ht_tracker_feed_yuv", "ht_ingest", "ht_ingest_yuv",
            "ht_tracker_feed_views", "ht_tracker_feed_yuv_views", "ht_ingest_views", "ht_ingest_yuv_views", "ht_backprojection", "ht_whitebalance",
            "ht_plan_info", "ht_debug_plane", "ht_debug_raw", "ht_debug_model_hist", "ht_debug_track_stats", "ht_set_track_memo", "ht_set_pipeline", "ht_join", "ht_debug_set_exactness", "ht_debug_track_trace", "ht_debug_track_phases", "ht_launch_count",
            "ht_profile", "ht_profile_read"]
@@ -303,6 +328,8 @@ def lib():
     L.ht_face_crop_map_framed.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp]
     L.ht_tracker_set_redact.argtypes = [vp, C.c_int, C.c_int, vp]
     L.ht_face_redact_rect.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp]
+    L.ht_tracker_set_best_shot.argtypes = [vp, C.c_int, C.c_int, vp]
+    L.ht_best_shot_score.argtypes = [vp, C.c_int, C.c_int, C.c_int, vp]
     L.ht_tracker_set_camera.argtypes = [vp, C.c_int, C.c_int, vp]
     L.ht_tracker_export.argtypes = [vp, vp, C.c_int, vp]
     L.ht_tracker_import.argtypes = [vp, vp, C.c_int, vp]

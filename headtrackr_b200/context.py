@@ -650,6 +650,44 @@ class Context:
         self._check(self._L.ht_tracker_set_framing(self._h, int(first), len(framings), C.addressof(arr)))
         self._keep("framing", int(first), [None if d is None else d["out"] for d in framings])
 
+    def tracker_set_best_shot(self, first, shots):
+        """Best shots of streams first, first+1, ... (ht_tracker_set_best_shot): per stream None (none) or a dict
+        {"out": torch CUDA uint8 (S_h, S_w, 4) tensor, or a pair of two such of one shape and row stride; "state":
+        torch CUDA uint8 tensor of BEST_SHOT_STATE_BYTES bytes, 8-byte aligned, on this context's device; "scale":
+        1.0}.  A row-padded view - last two strides (4, 1) - passes its row stride as the pitch.  On every tick that
+        writes crops the candidate - the RGBA crop of the shot's size and scale, before any redaction, never framed -
+        is scored by its Laplacian energy (bestshot.score); the first tick of a track and every later one that scores
+        strictly higher write it into `out` (with a pair: track t's into out[(t - 1) % 2], so the last track's best
+        stays intact during the next one) and into the state (bestshot.state_from_bytes decodes it; a track ends on
+        the stream's first tick that is not a crop tick).  Setting a best shot zeroes its state; the images are not
+        touched.  The best shot is the stream's: it outlives set_params, stop, start and reset; import ends its open
+        track; tracker_config removes it.  The context keeps the tensors alive while they are set."""
+        shots = list(shots)
+        arr = (_lib.BestShot * max(1, len(shots)))()
+        for i, d in enumerate(shots):
+            if d is None:
+                continue
+            outs = tuple(d["out"]) if isinstance(d["out"], (tuple, list)) else (d["out"],)
+            if len(outs) not in (1, 2):
+                raise ValueError("a best shot's out is one image or a pair")
+            for t in outs:
+                if not _is_torch(t) or not t.is_cuda:
+                    raise ValueError("a best-shot image is a torch CUDA tensor")
+                if t.dim() != 3 or t.element_size() != 1 or t.shape[2] != 4 or t.stride(2) != 1 or t.stride(1) != 4:
+                    raise ValueError("best-shot images must be uint8 (S_h, S_w, 4) with strides (pitch, 4, 1)")
+            if len(outs) == 2 and (outs[0].shape != outs[1].shape or outs[0].stride(0) != outs[1].stride(0)):
+                raise ValueError("the two images of a best shot have one shape and one row stride")
+            st = d["state"]
+            if not _is_torch(st) or not st.is_cuda:
+                raise ValueError("a best-shot state is a torch CUDA tensor")
+            if st.element_size() != 1 or st.numel() != _lib.BEST_SHOT_STATE_BYTES or not st.is_contiguous():
+                raise ValueError(f"a best-shot state is a contiguous uint8 tensor of {_lib.BEST_SHOT_STATE_BYTES} bytes")
+            o = outs[0]
+            arr[i] = _lib.BestShot((C.c_void_p * 2)(o.data_ptr(), outs[1].data_ptr() if len(outs) == 2 else None),
+                                   st.data_ptr(), o.shape[1], o.shape[0], o.stride(0), 0, float(d.get("scale", 1.0)))
+        self._check(self._L.ht_tracker_set_best_shot(self._h, int(first), len(shots), C.addressof(arr)))
+        self._keep("best_shot", int(first), [None if d is None else (d["out"], d["state"]) for d in shots])
+
     def tracker_set_redact(self, first, redactions):
         """Face redactions of streams first, first+1, ... (ht_tracker_set_redact): per stream None (none) or a dict
         {"mode": "mosaic" | "fill"; "block": 16; "scale": 1.25; "hold": 10; "fill_rgb": (0, 0, 0); "fill_yuv": (16, 128,

@@ -612,12 +612,13 @@ struct ht_ctx {
   StreamTable<FaceTensor> tensor;
   StreamTable<ht_framing> framing;          // ht_tracker_set_framing
   StreamTable<Redact> redact;               // ht_tracker_set_redact: the records and their holds
+  StreamTable<BestShot> best;               // ht_tracker_set_best_shot: the records and their tick sums
   DevBuf d_debug_tab;
   // what a tick launches for them, from the tables (count_outputs): the streams with a debug canvas, with a canvas and
-  // strokes on, with a camera, with a crop, with a tensor, with a framing and with a redaction (0: no launch for
-  // them), and the tiles of the largest crop and tensor (k_face_crop's grid.x)
+  // strokes on, with a camera, with a crop, with a tensor, with a framing, with a redaction and with a best shot (0: no
+  // launch for them), and the tiles of the largest crop, tensor and best shot (k_face_crop's and k_best_score's grid.x)
   int debug_count = 0, stroke_count = 0, camera_count = 0, framing_count = 0, redact_count = 0;
-  int crop_count = 0, crop_tiles = 0, tensor_count = 0, tensor_tiles = 0;
+  int crop_count = 0, crop_tiles = 0, tensor_count = 0, tensor_tiles = 0, best_count = 0, best_tiles = 0;
   // ht_tracker_feed(_canvases): the record table {ids[n], clocks[n], FeedRec[n], EntryCanvas[n], tile starts[n+1]}
   // goes up in one copy from pinned memory; the videos are drawn into the canvas arena (batch entry k's canvas at
   // EntryCanvas::base), zeroed when it grows
@@ -1811,7 +1812,7 @@ static bool tracker_params_ok(const ht_tracker_params &p) {
 static void count_outputs(ht_ctx *ctx) {
   const auto tiles = [](int w, int h) { return ((w + CROP_TX - 1) / CROP_TX) * ((h + CROP_TY - 1) / CROP_TY); };
   ctx->debug_count = ctx->stroke_count = ctx->camera_count = ctx->framing_count = ctx->redact_count = 0;
-  ctx->crop_count = ctx->crop_tiles = ctx->tensor_count = ctx->tensor_tiles = 0;
+  ctx->crop_count = ctx->crop_tiles = ctx->tensor_count = ctx->tensor_tiles = ctx->best_count = ctx->best_tiles = 0;
   for (const DebugCanvas &d : ctx->debug.h) {
     ctx->debug_count += d.rgba != nullptr;
     ctx->stroke_count += d.rgba != nullptr && d.strokes;
@@ -1829,6 +1830,11 @@ static void count_outputs(ht_ctx *ctx) {
       ++ctx->tensor_count;
       ctx->tensor_tiles = std::max(ctx->tensor_tiles, tiles(t.w, t.h));
     }
+  for (const BestShot &b : ctx->best.h)
+    if (b.d.rgba[0]) {
+      ++ctx->best_count;
+      ctx->best_tiles = std::max(ctx->best_tiles, tiles(b.d.width, b.d.height));
+    }
 }
 
 int ht_tracker_config(ht_ctx *ctx, const ht_tracker_params *params) {
@@ -1837,12 +1843,13 @@ int ht_tracker_config(ht_ctx *ctx, const ht_tracker_params *params) {
   CK(cudaSetDevice(ctx->cfg.device));
   const size_t mf = (size_t)ctx->cfg.max_frames;
   if (params && !tracker_params_ok(*params)) return ctx->fail(HT_ERR_ARG, "bad head parameters");
-  // either form discards every stream's debug canvas and stroke flag, camera, face crop, face tensor, framing and
-  // redaction
+  // either form discards every stream's debug canvas and stroke flag, camera, face crop, face tensor, framing,
+  // redaction and best shot
   CK(ctx->debug.clear(ctx->stream));
   CK(ctx->camera.clear(ctx->stream));
   CK(ctx->framing.clear(ctx->stream));
   CK(ctx->redact.clear(ctx->stream));
+  CK(ctx->best.clear(ctx->stream));
   CK(ctx->crop.clear(ctx->stream));
   CK(ctx->crop_planes.clear(ctx->stream));
   CK(ctx->tensor.clear(ctx->stream));
@@ -1899,19 +1906,21 @@ static_assert(sizeof(ht_debug_canvas) == 24 && sizeof(DebugCanvas) == sizeof(ht_
               "ht_debug_canvas layout");
 
 // The kinds of byte range a tick writes for a stream, as the overlap messages name them
-enum { OUT_DEBUG, OUT_CROP, OUT_TENSOR, OUT_CAMERA, OUT_FRAMING };
-static const char *const OUT_NAME[] ={"debug canvas", "face crop plane", "face tensor plane", "camera", "framed box"};
+enum { OUT_DEBUG, OUT_CROP, OUT_TENSOR, OUT_CAMERA, OUT_FRAMING, OUT_BEST_IMAGE, OUT_BEST_STATE };
+static const char *const OUT_NAME[] ={"debug canvas", "face crop plane", "face tensor plane", "camera", "framed box",
+                                      "best-shot image", "best-shot state"};
 
 // One byte range [start, end) that a tick writes: part of the `kind` output of stream `stream`
 struct TickWrite { uintptr_t start, end; int kind, stream; };
 
 // Whether two of the byte ranges a tick writes share a byte (the streams of a tick run concurrently): each debug
 // canvas (one span over its rows), each plane of each face crop, each channel plane (CHW) or whole tensor (HWC) of
-// each face tensor, each camera, and each framed box.  The first clashing pair in order of start goes to clash[0..1].
+// each face tensor, each camera, each framed box, and each image and state of each best shot.  The first clashing
+// pair in order of start goes to clash[0..1].
 static bool tick_writes_overlap(const std::vector<DebugCanvas> &debug, const std::vector<FaceCrop> &crop,
                                 const std::vector<CropPlanes> &crop_planes, const std::vector<FaceTensor> &tensor,
                                 const std::vector<CameraCtl> &camera, const std::vector<ht_framing> &framing,
-                                TickWrite clash[2]) {
+                                const std::vector<BestShot> &best, TickWrite clash[2]) {
   std::vector<TickWrite> w;
   const auto add = [&](const void *p, size_t rows, size_t pitch, size_t row_bytes, int kind, size_t s) {
     const uintptr_t a = reinterpret_cast<uintptr_t>(p);
@@ -1954,6 +1963,13 @@ static bool tick_writes_overlap(const std::vector<DebugCanvas> &debug, const std
     if (camera[s].camera) add(camera[s].camera, 1, 0, sizeof(ht_camera), OUT_CAMERA, s);
   for (size_t s = 0; s < framing.size(); ++s)
     if (framing[s].box) add(framing[s].box, 1, 0, sizeof(ht_framed_box), OUT_FRAMING, s);
+  for (size_t s = 0; s < best.size(); ++s) {
+    const ht_best_shot &b = best[s].d;
+    if (!b.rgba[0]) continue;
+    for (int i = 0; i < 2; ++i)
+      if (b.rgba[i]) add(b.rgba[i], b.height, b.pitch, 4 * (size_t)b.width, OUT_BEST_IMAGE, s);
+    add(b.state, 1, 0, sizeof(ht_best_shot_state), OUT_BEST_STATE, s);
+  }
   std::sort(w.begin(), w.end(), [](const TickWrite &a, const TickWrite &b) { return a.start < b.start; });
   for (size_t i = 1; i < w.size(); ++i)
     if (w[i].start < w[i - 1].end) {
@@ -1974,20 +1990,27 @@ struct OutputEdit {
   std::vector<FaceTensor> *tensor = nullptr;
   std::vector<ht_framing> *framing = nullptr;
   std::vector<Redact> *redact = nullptr;    // writes no byte range of its own: only the video, checked per tick
+  std::vector<BestShot> *best = nullptr;
 };
 
 // How every setter's records reach the tick.  The call is refused if two byte ranges a tick would write share a byte
 // (the tables before it share none, so a clash takes in one of its records, which the message names).  Otherwise
 // streams [first, first + n) of the edited tables go to the device, a new camera is constructed there, a new framed
-// box is made invalid there (a redaction's hold goes up empty with its record), and the tables and the tick's counts
-// follow.
+// box is made invalid there, a new best shot's state is zeroed there (a redaction's hold goes up empty with its
+// record), and the tables and the tick's counts follow.
 static int commit_outputs(ht_ctx *ctx, int first, int n, const OutputEdit &e) {
-  const int kind = e.debug ? OUT_DEBUG : e.crop ? OUT_CROP : e.tensor ? OUT_TENSOR : e.framing ? OUT_FRAMING : OUT_CAMERA;
+  const int kind = e.debug ? OUT_DEBUG : e.crop ? OUT_CROP : e.tensor ? OUT_TENSOR : e.framing ? OUT_FRAMING
+                   : e.best ? OUT_BEST_IMAGE : OUT_CAMERA;
   TickWrite c[2];
   if (tick_writes_overlap(e.debug ? *e.debug : ctx->debug.h, e.crop ? *e.crop : ctx->crop.h,
                           e.crop_planes ? *e.crop_planes : ctx->crop_planes.h, e.tensor ? *e.tensor : ctx->tensor.h,
-                          e.camera ? *e.camera : ctx->camera.h, e.framing ? *e.framing : ctx->framing.h, c)) {
-    const int own = c[0].kind == kind && c[0].stream >= first && c[0].stream - first < n ? 0 : 1;
+                          e.camera ? *e.camera : ctx->camera.h, e.framing ? *e.framing : ctx->framing.h,
+                          e.best ? *e.best : ctx->best.h, c)) {
+    const auto mine = [&](const TickWrite &w) {
+      return (w.kind == kind || (kind == OUT_BEST_IMAGE && w.kind == OUT_BEST_STATE)) && w.stream >= first &&
+             w.stream - first < n;
+    };
+    const int own = mine(c[0]) ? 0 : 1;
     return ctx->fail(HT_ERR_ARG, "record %d: its %s overlaps the %s of stream %d", c[own].stream - first,
                      OUT_NAME[c[own].kind], OUT_NAME[c[1 - own].kind], c[1 - own].stream);
   }
@@ -2022,11 +2045,18 @@ static int commit_outputs(ht_ctx *ctx, int first, int n, const OutputEdit &e) {
     CK(cudaGetLastError());
   }
   if (e.redact) CK(ctx->redact.commit(*e.redact, first, n, st));
+  if (e.best) {
+    CK(ctx->best.commit(*e.best, first, n, st));
+    k_best_reset<<<1, 256, 0, st>>>(ctx->best.dev(), first, n);
+    ++ctx->launches;
+    CK(cudaGetLastError());
+  }
   CK(cudaStreamSynchronize(st));    // the edited tables are the setter's locals
   if (e.debug) ctx->debug.h.swap(*e.debug);
   if (e.camera) ctx->camera.h.swap(*e.camera);
   if (e.framing) ctx->framing.h.swap(*e.framing);
   if (e.redact) ctx->redact.h.swap(*e.redact);
+  if (e.best) ctx->best.h.swap(*e.best);
   if (e.crop) {
     ctx->crop.h.swap(*e.crop);
     ctx->crop_planes.h.swap(*e.crop_planes);
@@ -2537,6 +2567,82 @@ int ht_face_redact_rect(const ht_tracker_event *ev, int canvas_w, int canvas_h, 
   return 1;
 }
 
+static_assert(sizeof(ht_best_shot_state) == HT_BEST_SHOT_STATE_BYTES && HT_BEST_SHOT_STATE_BYTES == 96 &&
+                  offsetof(ht_best_shot_state, score) == 8 && offsetof(ht_best_shot_state, x) == 16 &&
+                  offsetof(ht_best_shot_state, angle) == 48 && offsetof(ht_best_shot_state, now_ms) == 56 &&
+                  offsetof(ht_best_shot_state, canvas_w) == 64 && offsetof(ht_best_shot_state, track) == 72 &&
+                  offsetof(ht_best_shot_state, ended) == 76 && offsetof(ht_best_shot_state, ticks) == 80 &&
+                  offsetof(ht_best_shot_state, best_tick) == 84 && offsetof(ht_best_shot_state, buffer) == 88 &&
+                  offsetof(ht_best_shot_state, flags) == 92 && sizeof(ht_best_shot) == 48 &&
+                  offsetof(ht_best_shot, state) == 16 && offsetof(ht_best_shot, width) == 24 &&
+                  offsetof(ht_best_shot, pitch) == 32 && offsetof(ht_best_shot, pad_) == 36 &&
+                  offsetof(ht_best_shot, scale) == 40,
+              "ht_best_shot_state / ht_best_shot layout (include/headtrackr_b200.h)");
+
+// The best shots of streams [first, first + n).  Everything is checked on the host before anything changes; then one
+// launch zeroes the new states.
+int ht_tracker_set_best_shot(ht_ctx *ctx, int first, int n, const ht_best_shot *shots) {
+  { const int ar = tracker_streams(ctx, first, n); if (ar != HT_OK) return ar; }
+  if (!shots) return ctx->fail(HT_ERR_ARG, "shots is NULL");
+  std::vector<BestShot> next = ctx->best.edit(ctx->cfg.max_frames);
+  for (int i = 0; i < n; ++i) {
+    const ht_best_shot &b = shots[i];
+    BestShot k{};
+    if (b.rgba[0]) {
+      for (int p = 0; p < 2; ++p) {
+        if (!b.rgba[p]) continue;
+        if (reinterpret_cast<uintptr_t>(b.rgba[p]) & 3u)
+          return ctx->fail(HT_ERR_ARG, "record %d: rgba[%d] must be 4-byte aligned", i, p);
+        if (!is_device_ptr(b.rgba[p])) return ctx->fail(HT_ERR_ARG, "record %d: rgba[%d] is not device memory", i, p);
+      }
+      if (!b.state) return ctx->fail(HT_ERR_ARG, "record %d: state is NULL", i);
+      if (reinterpret_cast<uintptr_t>(b.state) & 7u) return ctx->fail(HT_ERR_ARG, "record %d: state must be 8-byte aligned", i);
+      cudaPointerAttributes a{};
+      if (cudaPointerGetAttributes(&a, b.state) != cudaSuccess) { cudaGetLastError(); a.type = cudaMemoryTypeUnregistered; }
+      if (a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged)
+        return ctx->fail(HT_ERR_ARG, "record %d: state is not device memory", i);
+      if (a.device != ctx->cfg.device)
+        return ctx->fail(HT_ERR_ARG, "record %d: state is memory of device %d, the context is on device %d", i, a.device,
+                         ctx->cfg.device);
+      if (b.width < 3 || b.height < 3 || b.width > 2048 || b.height > 2048)
+        return ctx->fail(HT_ERR_SIZE, "record %d: best shot %dx%d outside 3..2048", i, b.width, b.height);
+      if ((b.pitch & 3) || (b.pitch != 0 && b.pitch < 4 * b.width))
+        return ctx->fail(HT_ERR_ARG, "record %d: pitch %d is not a multiple of 4 >= 4*width", i, b.pitch);
+      if (b.pad_ != 0) return ctx->fail(HT_ERR_ARG, "record %d: pad_ is %d, not 0", i, b.pad_);
+      if (!(b.scale > 0.0 && b.scale <= 16.0)) return ctx->fail(HT_ERR_ARG, "record %d: scale %g outside (0, 16]", i, b.scale);
+      k.d = b;
+      if (!k.d.pitch) k.d.pitch = 4 * b.width;
+    }
+    next[(size_t)(first + i)] = k;
+  }
+  OutputEdit e;
+  e.best = &next;
+  return commit_outputs(ctx, first, n, e);
+}
+
+// The best-shot score of an RGBA8 image on the host, with k_best_score's best_gray and best_term
+int ht_best_shot_score(const uint8_t *rgba, int w, int h, int pitch, uint64_t *out) {
+  if (!rgba || !out) return HT_ERR_ARG;
+  if (w < 3 || h < 3 || w > 2048 || h > 2048) return HT_ERR_SIZE;
+  if (!pitch) pitch = 4 * w;
+  if (pitch < 4 * w) return HT_ERR_ARG;
+  std::vector<int> g((size_t)w * h);
+  for (int j = 0; j < h; ++j)
+    for (int i = 0; i < w; ++i) {
+      uint32_t px;
+      memcpy(&px, rgba + (size_t)j * pitch + 4 * (size_t)i, 4);
+      g[(size_t)j * w + i] = best_gray(px);
+    }
+  unsigned long long sum = 0;
+  for (int j = 1; j < h - 1; ++j)
+    for (int i = 1; i < w - 1; ++i) {
+      const size_t c = (size_t)j * w + i;
+      sum += best_term(g[c], g[c - 1], g[c + 1], g[c - w], g[c + w]);
+    }
+  *out = sum;
+  return HT_OK;
+}
+
 static_assert(REC_BYTES == HT_TRACKER_RECORD_BYTES && REC_MAGIC == HT_TRACKER_RECORD_MAGIC &&
                   REC_VERSION == HT_TRACKER_RECORD_VERSION,
               "tracker record (include/headtrackr_b200.h)");
@@ -2634,6 +2740,10 @@ int ht_tracker_import(ht_ctx *ctx, const int32_t *streams, int n, const void *re
                                                 ctx->d_tracker_params.as<TrackerParams>(), ctx->track_state.as<TrackState>(),
                                                 ctx->model_hist.as<uint32_t>(), ctx->d_track_cost.as<int32_t>());
   ++ctx->launches;
+  if (ctx->best_count > 0) {   // an imported stream is another tracker: its best shot's open track ends
+    k_best_end<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(ctx->d_slots.as<int32_t>(), n, ctx->best.dev());
+    ++ctx->launches;
+  }
   CK(cudaGetLastError());
   CK(cudaStreamSynchronize(st));
   return HT_OK;
@@ -2677,8 +2787,9 @@ struct TickGroup {
 //   k_hist, k_track  per group: one track() of the CS streams                    src/camshift.js:213-312
 //   k_tracker_update starter, whitebalance gate, facetrackr and main.js transitions, status bits, head epilogue
 //   k_track_init     initTracker for the streams that found their face           src/facetrackr.js:97-108
-// and after them, each only while some stream has one: k_camera_update, k_framing_update, k_debug_strokes, k_face_crop
-// (after k_tracker_update) and, last, k_face_redact, which writes the videos the others read.
+// and after them, each only while some stream has one: k_camera_update, k_framing_update, k_debug_strokes, k_face_crop,
+// k_best_score and k_best_write (after k_tracker_update) and, last, k_face_redact, which writes the videos the others
+// read.
 static int tracker_tick(ht_ctx *ctx, const TickGroup *grp, int n_groups, const uint8_t *d_rgba, int n, const int32_t *d_ids,
                         double now_ms, const double *d_now, const FeedDraw *feed, const EntryCanvas *geo,
                         ht_tracker_event *out) {
@@ -2783,6 +2894,12 @@ static int tracker_tick(ht_ctx *ctx, const TickGroup *grp, int n_groups, const u
         d_ids, geo, g0.w, g0.h, d_ev, ctx->crop.dev(), ctx->crop_planes.dev(), ctx->tensor.dev(), tz, src,
         ctx->framing_count > 0 ? ctx->framing.dev() : nullptr);
     ++ctx->launches;
+  }
+  if (ctx->best_count > 0) {   // score every crop tick's candidate and step the state, then write the new bests
+    const dim3 grid((unsigned)ctx->best_tiles, (unsigned)n);
+    k_best_score<<<grid, 256, 0, st>>>(d_ids, geo, g0.w, g0.h, d_ev, now_ms, d_now, ctx->best.dev(), src);
+    k_best_write<<<grid, 256, 0, st>>>(d_ids, geo, g0.w, g0.h, d_ev, ctx->best.dev(), src);
+    ctx->launches += 2;
   }
   ctx->prof_begin(HT_PROF_TRACK_INIT, st);
   // calc_angles -1: each entry's own, from its stream's parameters (k_tracker_update)
@@ -3978,11 +4095,12 @@ extern "C" void ht_selftest_tensor_pixels(const ht_face_tensor *tensor, const ui
 }
 // The setters' overlap verdict on n streams' records, addresses as integers: stream s has debug canvas debug[s], face
 // crop crops[s] (RGBA) or yuv[s] (YUV, if crops[s].rgba is NULL), face tensor tensors[s], camera cameras[s] and framed
-// box boxes[s] (boxes NULL: none); a NULL address is none.  -> 1 with the clashing pair's kinds and streams in
-// clash[4] {kind, stream, kind, stream}, or 0.
-extern "C" int ht_selftest_tick_writes_framed(int n, const ht_debug_canvas *debug, const ht_face_crop *crops,
-                                              const ht_face_crop_yuv *yuv, const ht_face_tensor *tensors,
-                                              void *const *cameras, void *const *boxes, int32_t *clash) {
+// box boxes[s] (boxes NULL: none) and best shot shots[s] (shots NULL: none; pitch 0 resolved); a NULL address is none.
+// -> 1 with the clashing pair's kinds and streams in clash[4] {kind, stream, kind, stream}, or 0.
+extern "C" int ht_selftest_tick_writes_best(int n, const ht_debug_canvas *debug, const ht_face_crop *crops,
+                                            const ht_face_crop_yuv *yuv, const ht_face_tensor *tensors,
+                                            void *const *cameras, void *const *boxes, const ht_best_shot *shots,
+                                            int32_t *clash) {
   std::vector<DebugCanvas> d((size_t)n);
   std::vector<FaceCrop> f((size_t)n);
   std::vector<CropPlanes> q((size_t)n);
@@ -3997,10 +4115,22 @@ extern "C" int ht_selftest_tick_writes_framed(int n, const ht_debug_canvas *debu
   }
   std::vector<ht_framing> g((size_t)n);
   for (int s = 0; s < n && boxes; ++s) g[s].box = static_cast<ht_framed_box *>(boxes[s]);
+  std::vector<BestShot> b((size_t)n);
+  for (int s = 0; s < n && shots; ++s)
+    if (shots[s].rgba[0]) {
+      b[s].d = shots[s];
+      if (!b[s].d.pitch) b[s].d.pitch = 4 * shots[s].width;
+    }
   TickWrite c[2];
-  if (!tick_writes_overlap(d, f, q, t, k, g, c)) return 0;
+  if (!tick_writes_overlap(d, f, q, t, k, g, b, c)) return 0;
   for (int i = 0; i < 2; ++i) clash[2 * i] = c[i].kind, clash[2 * i + 1] = c[i].stream;
   return 1;
+}
+// ... without best shots
+extern "C" int ht_selftest_tick_writes_framed(int n, const ht_debug_canvas *debug, const ht_face_crop *crops,
+                                              const ht_face_crop_yuv *yuv, const ht_face_tensor *tensors,
+                                              void *const *cameras, void *const *boxes, int32_t *clash) {
+  return ht_selftest_tick_writes_best(n, debug, crops, yuv, tensors, cameras, boxes, nullptr, clash);
 }
 // ... without framed boxes
 extern "C" int ht_selftest_tick_writes(int n, const ht_debug_canvas *debug, const ht_face_crop *crops,
@@ -4042,6 +4172,15 @@ extern "C" int ht_selftest_redact_hold(void *s, int hold, const ht_tracker_event
                           e.angle, cw, ch) ? 1 : 0;
 }
 extern "C" int ht_selftest_redact_hold_bytes() { return (int)sizeof(RedactHold); }
+// best_shot_step on the host, as k_best_score runs it: record `ev` on a cw x ch canvas at clock now_ms, whose candidate
+// scored `score`, moves *s of a best shot with two images (two 1) or one (two 0) -> 1 if the tick set a new best
+extern "C" int ht_selftest_best_shot_step(ht_best_shot_state *s, int two, unsigned long long score,
+                                          const ht_tracker_event *ev, double now_ms, int cw, int ch) {
+  const TrackerEvent &e = *reinterpret_cast<const TrackerEvent *>(ev);
+  return best_shot_step(*s, two != 0, score, e.detection, e.x, e.y, e.width, e.height, e.angle, now_ms, cw, ch) ? 1 : 0;
+}
+// best_shot_end on the host, as ht_tracker_import runs it
+extern "C" void ht_selftest_best_shot_end(ht_best_shot_state *s) { best_shot_end(*s); }
 // k_face_redact's per-entry code on the host, one lane: the redaction `redact` of an image of any format (img, host
 // planes) or an RGBA8 frame (rgba, rows of `pitch` bytes, 0: 4 * width; exactly one of the two) through a view (NULL:
 // the whole frame upright), for record `ev` on a cw x ch canvas and the hold *s (NULL: none) -> 1 if it redacted, 0

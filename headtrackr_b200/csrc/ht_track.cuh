@@ -2042,6 +2042,56 @@ __host__ __device__ __forceinline__ uint32_t crop_pixel(const ViewFeedRec &v, co
   return out;
 }
 
+// Best shots (ht_tracker_set_best_shot; DESIGN.md 2, "Best shots"): per track, the crop tick whose candidate - the
+// RGBA8 crop of the best shot's size and scale - has the highest Laplacian energy.
+// A candidate pixel as the score reads it: its gray (gray_of), or -1 where its alpha is below 255
+__host__ __device__ __forceinline__ int best_gray(uint32_t px) { return (px >> 24) == 255u ? (int)gray_of(px) : -1; }
+// The score's term of one pixel from the best_gray of it and of its left, right, upper and lower neighbours: L^2 with
+// L = 4 c - l - r - u - d, or 0 if one of the five is -1.  At most 1020^2.
+__host__ __device__ __forceinline__ uint32_t best_term(int c, int l, int r, int u, int d) {
+  if ((c | l | r | u | d) < 0) return 0u;
+  const int L = 4 * c - l - r - u - d;
+  return (uint32_t)(L * L);
+}
+// Ends the stream's open track, if one is open (flags HT_BEST_ENDED); otherwise changes nothing
+__host__ __device__ __forceinline__ void best_shot_end(ht_best_shot_state &s) {
+  if (s.ended != s.track) {
+    s.ended = s.track;
+    s.flags = HT_BEST_ENDED;
+  }
+}
+// One tick of a stream's best shot (two: it has two images): a record on a cw x ch canvas at clock now_ms whose
+// candidate scored `score` (read only on a crop tick).  A crop tick begins a track if none is open, and sets the
+// track's best on its first tick or with a score strictly above best_score; any other tick ends an open track.
+// flags become the tick's.  -> whether the tick set a new best (the candidate is then to be written to rgba[buffer]).
+__host__ __device__ inline bool best_shot_step(ht_best_shot_state &s, bool two, unsigned long long score, int detection,
+                                               double x, double y, double w, double h, double angle, double now_ms, int cw,
+                                               int ch) {
+  s.flags = 0;
+  if (!crop_tick(detection, x, y, w, h)) {
+    best_shot_end(s);
+    return false;
+  }
+  if (s.ended == s.track) {
+    ++s.track;
+    s.ticks = 0;
+    s.buffer = two ? (int32_t)((s.track - 1u) & 1u) : 0;
+    s.flags = HT_BEST_BEGAN;
+  }
+  s.score = score;
+  const bool best = s.ticks == 0 || score > s.best_score;
+  if (best) {
+    s.best_score = score;
+    s.x = x; s.y = y; s.width = w; s.height = h; s.angle = angle;
+    s.now_ms = now_ms;
+    s.canvas_w = cw; s.canvas_h = ch;
+    s.best_tick = s.ticks;
+    s.flags |= HT_BEST_IMPROVED;
+  }
+  ++s.ticks;
+  return best;
+}
+
 // The video of batch entry k as a view record: the tick's frames (ht_tracker_step: frame k, one canvas size, 1:1),
 // or the feed table's record k as k_feed_draw / k_feed_draw_yuv / k_feed_draw_view drew it.
 enum : int32_t { CROP_FRAMES = 0, CROP_FEED = 1, CROP_YUV = 2, CROP_VIEW = 3 };
@@ -2071,8 +2121,9 @@ __device__ __forceinline__ void crop_source(const CropSource &s, int k, ViewFeed
 }
 
 // One 64 x 16 tile from (X0, Y0) of crop f: a warp writes 128 consecutive bytes of a crop row.  Out of line per texel
-// source, as feed_draw_view, so that each keeps its own registers.
-template <int KIND>
+// source, as feed_draw_view, so that each keeps its own registers.  COPY: one instantiation per calling kernel
+// (k_face_crop 0, k_best_write 1), since ptxas allocates an out-of-line function's registers across all its callers.
+template <int KIND, int COPY = 0>
 __device__ __noinline__ void face_crop_tile(const ViewFeedRec *__restrict__ vp, const long long *__restrict__ Mp,
                                             const FaceCrop f, int X0, int Y0) {
   const ViewFeedRec v = *vp;
@@ -2317,6 +2368,146 @@ __global__ void __launch_bounds__(256) k_face_redact(const int32_t *__restrict__
     for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
     return x;
   });
+}
+
+// A stream's best shot in the device table: the caller's record with the pitch resolved (rgba[0] NULL: none), and the
+// running sum and ticket of its tick, which only k_best_score writes (0 between ticks).
+struct BestShot {
+  ht_best_shot d;
+  unsigned long long acc;
+  uint32_t ticket, pad_;
+};
+constexpr int BEST_HX = CROP_TX + 2, BEST_HY = CROP_TY + 2;   // a score tile with its one-pixel halo
+
+// The best_gray of the candidate pixels [X0 - 1, X0 + CROP_TX] x [Y0 - 1, Y0 + CROP_TY] inside the W x H candidate
+// into g (k_best_score's shared memory; the others are never read).  Out of line per texel source, as face_crop_tile;
+// the view record and the map stay in shared memory (vp, Mp), as face_tensor_tile keeps them, which holds the kernel
+// to 64 registers.
+template <int KIND>
+__device__ __noinline__ void best_tile_gray(const ViewFeedRec *__restrict__ vp, const long long *__restrict__ Mp,
+                                            int16_t (*g)[BEST_HX], int X0, int Y0, int W, int H) {
+  const ViewFeedRec &v = *vp;
+  const long long *M = Mp;
+  for (int t = threadIdx.x; t < BEST_HX * BEST_HY; t += blockDim.x) {
+    const int x = t % BEST_HX, y = t / BEST_HX, i = X0 - 1 + x, j = Y0 - 1 + y;
+    if (i >= 0 && j >= 0 && i < W && j < H) g[y][x] = (int16_t)best_gray(crop_pixel<KIND>(v, M, i, j));
+  }
+}
+
+// After k_face_crop, before k_face_redact: grid (tiles of the largest best shot, batch entries).  Entry k (stream
+// ids[k], NULL: k; record events[geo[k].record] and canvas geo[k], geo NULL: k and cw x ch; clock now[k], NULL:
+// now_ms) scores the candidate of its stream's best shot on a crop tick: each of its CTAs samples one 64 x 16 tile and
+// its halo with crop_pixel, sums best_term over the tile's scored pixels and adds that to the stream's acc; the last
+// ticket takes the total, steps the state and resets acc and ticket.  On any other tick CTA 0 alone steps the state.
+// Streams without a best shot and CTAs past their own tiles exit at once.
+__global__ void __launch_bounds__(256) k_best_score(const int32_t *__restrict__ ids, const EntryCanvas *__restrict__ geo,
+                                                    int cw, int ch, const TrackerEvent *__restrict__ events, double now_ms,
+                                                    const double *__restrict__ now, BestShot *best, CropSource src) {
+  const int k = blockIdx.y, id = ids ? ids[k] : k;
+  BestShot &b = best[id];
+  if (!b.d.rgba[0]) return;
+  const int W = b.d.width, H = b.d.height, tiles_x = (W + CROP_TX - 1) / CROP_TX;
+  const unsigned tiles = (unsigned)(tiles_x * ((H + CROP_TY - 1) / CROP_TY));
+  if (blockIdx.x >= tiles) return;
+  const TrackerEvent &e = events[geo ? geo[k].record : k];
+  const int ew = geo ? geo[k].w : cw, eh = geo ? geo[k].h : ch;
+  const double t = now ? now[k] : now_ms;
+  const bool two = b.d.rgba[1] != nullptr;
+  if (!crop_tick(e.detection, e.x, e.y, e.width, e.height)) {
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+      ht_best_shot_state s = *b.d.state;
+      best_shot_step(s, two, 0, e.detection, e.x, e.y, e.width, e.height, e.angle, t, ew, eh);
+      *b.d.state = s;
+    }
+    return;
+  }
+  __shared__ ViewFeedRec v;
+  __shared__ long long M[6];
+  __shared__ int16_t g[BEST_HY][BEST_HX];
+  __shared__ uint32_t part[8];
+  if (threadIdx.x == 0) {
+    crop_source(src, k, v);
+    crop_map(e.detection, e.x, e.y, e.width, e.height, e.angle, ew, eh, v.sw, v.sh, W, H, b.d.scale, M);
+  }
+  __syncthreads();
+  const int X0 = ((int)blockIdx.x % tiles_x) * CROP_TX, Y0 = ((int)blockIdx.x / tiles_x) * CROP_TY;
+  if (v.kind == VIEW_RGBA) best_tile_gray<VIEW_RGBA>(&v, M, g, X0, Y0, W, H);
+  else if (v.kind == VIEW_NV12_I420) best_tile_gray<VIEW_NV12_I420>(&v, M, g, X0, Y0, W, H);
+  else best_tile_gray<VIEW_FMT>(&v, M, g, X0, Y0, W, H);
+  __syncthreads();
+  // a CTA's sum stays below 2^32: 1024 pixels of at most 1020^2
+  uint32_t sum = 0;
+  const int x = threadIdx.x & 63, i = X0 + x;
+#pragma unroll
+  for (int r = 0; r < 4; ++r) {
+    const int y = 4 * r + (threadIdx.x >> 6), j = Y0 + y;
+    if (i >= 1 && i <= W - 2 && j >= 1 && j <= H - 2)
+      sum += best_term(g[y + 1][x + 1], g[y + 1][x], g[y + 1][x + 2], g[y][x + 1], g[y + 2][x + 1]);
+  }
+  for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+  if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = sum;
+  __syncthreads();
+  if (threadIdx.x != 0) return;
+  for (int w = 1; w < 8; ++w) sum += part[w];
+  atomicAdd(&b.acc, (unsigned long long)sum);
+  __threadfence();
+  if (atomicAdd(&b.ticket, 1u) != tiles - 1) return;
+  __threadfence();
+  const unsigned long long score = atomicExch(&b.acc, 0ull);
+  b.ticket = 0;
+  ht_best_shot_state s = *b.d.state;
+  best_shot_step(s, two, score, e.detection, e.x, e.y, e.width, e.height, e.angle, t, ew, eh);
+  *b.d.state = s;
+}
+
+// After k_best_score: grid (tiles of the largest best shot, batch entries).  Entry k's CTAs write the candidate (the
+// crop of its best shot's size and scale, by face_crop_tile) into rgba[buffer] if its tick set a new best
+// (HT_BEST_IMPROVED in the state k_best_score has just stepped).
+__global__ void __launch_bounds__(256) k_best_write(const int32_t *__restrict__ ids, const EntryCanvas *__restrict__ geo,
+                                                    int cw, int ch, const TrackerEvent *__restrict__ events,
+                                                    const BestShot *__restrict__ best, CropSource src) {
+  const int k = blockIdx.y, id = ids ? ids[k] : k;
+  const BestShot &b = best[id];
+  if (!b.d.rgba[0]) return;
+  const int W = b.d.width, H = b.d.height, tiles_x = (W + CROP_TX - 1) / CROP_TX;
+  if ((int)blockIdx.x >= tiles_x * ((H + CROP_TY - 1) / CROP_TY)) return;
+  __shared__ ViewFeedRec v;
+  __shared__ long long M[6];
+  __shared__ int buffer;
+  if (threadIdx.x == 0) {
+    const ht_best_shot_state &s = *b.d.state;
+    buffer = (s.flags & HT_BEST_IMPROVED) ? s.buffer : -1;
+    if (buffer >= 0) {
+      crop_source(src, k, v);
+      const TrackerEvent &e = events[geo ? geo[k].record : k];
+      crop_map(e.detection, e.x, e.y, e.width, e.height, e.angle, geo ? geo[k].w : cw, geo ? geo[k].h : ch, v.sw, v.sh, W,
+               H, b.d.scale, M);
+    }
+  }
+  __syncthreads();
+  if (buffer < 0) return;
+  const FaceCrop f{b.d.rgba[buffer], W, H, b.d.pitch, CROP_RGBA, b.d.scale};
+  const int X0 = ((int)blockIdx.x % tiles_x) * CROP_TX, Y0 = ((int)blockIdx.x / tiles_x) * CROP_TY;
+  if (v.kind == VIEW_RGBA) face_crop_tile<VIEW_RGBA, 1>(&v, M, f, X0, Y0);
+  else if (v.kind == VIEW_NV12_I420) face_crop_tile<VIEW_NV12_I420, 1>(&v, M, f, X0, Y0);
+  else face_crop_tile<VIEW_FMT, 1>(&v, M, f, X0, Y0);
+}
+
+// ht_tracker_set_best_shot: one CTA zeroes the states of streams [first, first + n) that have a best shot
+__global__ void k_best_reset(const BestShot *__restrict__ best, int first, int n) {
+  for (int i = threadIdx.x; i < n; i += blockDim.x)
+    if (best[first + i].d.rgba[0]) *best[first + i].d.state = ht_best_shot_state{};
+}
+
+// ht_tracker_import: the n streams ids[0..n) that have a best shot end their open tracks
+__global__ void k_best_end(const int32_t *__restrict__ ids, int n, const BestShot *__restrict__ best) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  const BestShot &b = best[ids[k]];
+  if (!b.d.rgba[0]) return;
+  ht_best_shot_state s = *b.d.state;
+  best_shot_end(s);
+  *b.d.state = s;
 }
 
 // ht_tracker_set_camera: one CTA constructs the cameras of streams [first, first + n) that have a controller

@@ -169,7 +169,9 @@ class TrackerSet:
     face as a model's normalised input, independent of "faceCrop".  A stream's "framing" key is its framing, a dict as
     Context.tracker_set_framing takes: a steady face-cam box in its `out` tensor that the crop (and, with "tensor":
     True, the tensor) is cut from instead of the tracked box.  A stream's "redact" key is its face redaction, a dict
-    as Context.tracker_set_redact takes: its tracked face hidden in its own (device) video after each tick.
+    as Context.tracker_set_redact takes: its tracked face hidden in its own (device) video after each tick.  A
+    stream's "bestShot" key is its best shot, a dict as Context.tracker_set_best_shot takes: the sharpest face of its
+    current or last track in its `out` image(s), with its state.
     Differs from the reference in one place: start() on a running stream does nothing (the reference runs an extra,
     unscheduled pass)."""
 
@@ -210,6 +212,9 @@ class TrackerSet:
         redactions = [(p or {}).get("redact") for p in (params if per_stream else [params] * n_streams)]
         if any(r is not None for r in redactions):   # and face redactions
             context.tracker_set_redact(0, redactions)
+        shots = [(p or {}).get("bestShot") for p in (params if per_stream else [params] * n_streams)]
+        if any(b is not None for b in shots):     # and best shots
+            context.tracker_set_best_shot(0, shots)
 
     def set_params(self, k, params):
         """The parameters of stream k (a dict as for the constructor).  Its state is kept: calcAngles takes effect at
@@ -224,6 +229,7 @@ class TrackerSet:
         self.ctx.tracker_set_face_tensor(k, [(params or {}).get("faceTensor")])   # no "faceTensor" key: none
         self.ctx.tracker_set_framing(k, [(params or {}).get("framing")])   # no "framing" key: none
         self.ctx.tracker_set_redact(k, [(params or {}).get("redact")])   # no "redact" key: none
+        self.ctx.tracker_set_best_shot(k, [(params or {}).get("bestShot")])   # no "bestShot" key: none
 
     def addEventListener(self, fn):
         """fn(stream_index, evt): evt is a headtrackrStatus / facetrackingEvent / headtrackingEvent payload dict."""

@@ -461,7 +461,7 @@ typedef struct {
  * reference's timers write one after another.
  * Errors (nothing changes): HT_ERR_STATE before ht_tracker_config; HT_ERR_ARG for a range outside [0, max_frames),
  * n <= 0, canvases NULL, a host pointer, a pointer or pitch that is not a multiple of 4, a pitch below 4*width, or a
- * canvas that overlaps any debug canvas, crop plane, tensor plane, camera or framed box of any stream after the call (the one
+ * canvas that overlaps any debug canvas, crop plane, tensor plane, camera, framed box or best-shot image or state of any stream after the call (the one
  * rule of ht_tracker_set_face_tensor); HT_ERR_SIZE for a size outside 1..16384. */
 int ht_tracker_set_debug(ht_ctx *ctx, int first, int n, const ht_debug_canvas *canvases);
 
@@ -501,8 +501,8 @@ typedef struct {
  * A tick launches one more kernel while some stream has a crop, and nothing more otherwise.
  * Errors (nothing changes): HT_ERR_STATE before ht_tracker_config; HT_ERR_ARG for a range outside [0, max_frames),
  * n <= 0, crops NULL, a host pointer, a pointer or pitch that is not a multiple of 4, a pitch below 4*width, a scale
- * that is not finite or outside (0, 16], or a crop that overlaps any debug canvas, crop plane, tensor plane, camera
- * or framed box of any stream after the call (the one rule of ht_tracker_set_face_tensor); HT_ERR_SIZE for a size outside 1..2048. */
+ * that is not finite or outside (0, 16], or a crop that overlaps any debug canvas, crop plane, tensor plane, camera,
+ * framed box or best-shot image or state of any stream after the call (the one rule of ht_tracker_set_face_tensor); HT_ERR_SIZE for a size outside 1..2048. */
 int ht_tracker_set_face_crop(ht_ctx *ctx, int first, int n, const ht_face_crop *crops);
 
 /* A stream's face crop as 4:2:0 video for an encoder: NVENC takes NV12; openh264, libx264, libvpx and WebRTC frame
@@ -542,7 +542,7 @@ typedef struct {
  * that is odd or outside 2..2048; HT_ERR_ARG for a range outside [0, max_frames), n <= 0, crops NULL, a format other
  * than NV12 / I420, a colour other than the four above, a missing or extra plane, a host pointer, a pitch below its
  * row's bytes, a non-zero pad_, a scale that is not finite or outside (0, 16], or a plane that overlaps any debug
- * canvas, crop plane (its own crop's other planes included), tensor plane, camera or framed box of any stream after the call (the
+ * canvas, crop plane (its own crop's other planes included), tensor plane, camera, framed box or best-shot image or state of any stream after the call (the
  * one rule of ht_tracker_set_face_tensor). */
 int ht_tracker_set_face_crop_yuv(ht_ctx *ctx, int first, int n, const ht_face_crop_yuv *crops);
 
@@ -592,12 +592,13 @@ typedef struct {
  * value other than the above, a host pointer, a pointer not aligned to the element size, a stride outside its range
  * above, a non-zero pad_, a mul or add that is not finite, a U8 tensor whose used mul is not 1 or add not 0, a scale
  * that is not finite or outside (0, 16], or a tensor plane that overlaps any debug canvas, crop plane, tensor plane
- * (its own tensor's others included), camera or framed box of any stream after the call.
+ * (its own tensor's others included), camera, framed box or best-shot image or state of any stream after the call.
  * That is the one overlap rule of the per-stream outputs, which ht_tracker_set_debug, both crop setters and
  * ht_tracker_set_camera apply too: the streams of a tick run concurrently, so no two of the byte spans a tick writes
  * may share a byte.  The spans: each debug canvas, (height-1)*pitch + 4*width bytes; each plane of each face crop,
  * RGBA or YUV; each channel plane of a CHW tensor, or the whole of an HWC tensor; each camera, HT_CAMERA_BYTES; each
- * framed box (ht_tracker_set_framing), HT_FRAMED_BOX_BYTES. */
+ * framed box (ht_tracker_set_framing), HT_FRAMED_BOX_BYTES; each best-shot image (ht_tracker_set_best_shot),
+ * (height-1)*pitch + 4*width bytes, and each best-shot state, HT_BEST_SHOT_STATE_BYTES. */
 int ht_tracker_set_face_tensor(ht_ctx *ctx, int first, int n, const ht_face_tensor *tensors);
 
 /* The map of the crop `crop` (its size and scale; rgba and pitch are ignored; a YUV crop has the map of the RGBA crop of
@@ -655,7 +656,8 @@ typedef struct {
  * range outside [0, max_frames), n <= 0, framings NULL, a box that is host memory, memory of another device or not
  * 8-byte aligned, an alpha outside (0, 1] or a dead_zone outside [0, 0.5] (NaN included), an outputs mask that is 0
  * or has other bits, a non-zero pad_, or a box that overlaps any debug canvas, crop plane, tensor plane, camera or
- * framed box of any stream after the call (the one rule of ht_tracker_set_face_tensor; a box is HT_FRAMED_BOX_BYTES). */
+ * framed box or best-shot image or state of any stream after the call (the one rule of ht_tracker_set_face_tensor; a box
+ * is HT_FRAMED_BOX_BYTES). */
 #define HT_FRAMED_BOX_BYTES 48
 int ht_tracker_set_framing(ht_ctx *ctx, int first, int n, const ht_framing *framings);
 /* The map of the crop `crop` (as for ht_face_crop_map) cut from framed box `box` (host memory) on a canvas_w x canvas_h
@@ -728,6 +730,76 @@ int ht_tracker_set_redact(ht_ctx *ctx, int first, int n, const ht_face_redact *r
 int ht_face_redact_rect(const ht_tracker_event *ev, int canvas_w, int canvas_h, int video_w, int video_h,
                         const ht_video_view *view, const ht_face_redact *redact, int32_t out[4]);
 
+/* A stream's best shot: the sharpest face of its current or last track, one RGBA8 image per track (DESIGN.md 2, "Best
+ * shots").  The state lives in caller-owned DEVICE memory.  Byte offsets:
+ *     0  uint64 best_score     the score of the track's best tick
+ *     8  uint64 score          the score of the stream's latest crop tick
+ *    16  double x, y, width, height, angle   the best tick's record fields
+ *    56  double now_ms         the best tick's clock
+ *    64  int32  canvas_w, canvas_h   the best tick's canvas size (with x .. angle: ht_face_crop_map's input)
+ *    72  uint32 track          tracks begun since the best shot was set; the current or last one is track
+ *    76  uint32 ended          tracks ended; track t is final once ended >= t, a track is open while ended != track
+ *    80  uint32 ticks          crop ticks in the current or last track
+ *    84  uint32 best_tick      the best tick's index in that track, 0 for its first tick
+ *    88  int32  buffer         the image the current or last track writes: rgba[buffer]
+ *    92  uint32 flags          HT_BEST_* of the stream's latest tick (0: none of them) */
+typedef struct {
+  uint64_t best_score;
+  uint64_t score;
+  double x, y, width, height, angle;
+  double now_ms;
+  int32_t canvas_w, canvas_h;
+  uint32_t track, ended;
+  uint32_t ticks, best_tick;
+  int32_t buffer;
+  uint32_t flags;
+} ht_best_shot_state;     /* 96 bytes */
+#define HT_BEST_SHOT_STATE_BYTES 96
+#define HT_BEST_BEGAN 1       /* the tick began a track */
+#define HT_BEST_IMPROVED 2    /* the tick set the track's best (its first tick always does): rgba[buffer] was written */
+#define HT_BEST_ENDED 4       /* the tick ended the open track (its best is final) */
+/* A stream's best shot record.  Explicit values: the wrappers' default (scale 1) belongs to the wrappers.  Byte offsets:
+ * 0 rgba[2], 16 state, 24 width, 28 height, 32 pitch, 36 pad_, 40 scale. */
+typedef struct {
+  uint8_t *rgba[2];       /* 4-byte aligned DEVICE images of S_h rows; rgba[0] NULL removes the best shot, rgba[1] NULL:
+                             one image */
+  ht_best_shot_state *state;  /* 8-byte aligned DEVICE memory of the context's device */
+  int32_t width, height;  /* S_w x S_h, 3..2048 */
+  int32_t pitch;          /* bytes per image row (both images); 0 = 4*width; a multiple of 4, >= 4*width */
+  int32_t pad_;           /* 0 */
+  double scale;           /* as ht_face_crop's, (0, 16] */
+} ht_best_shot;           /* 48 bytes */
+/* Stream first+i gets shots[i] (host array), for i in [0, n); stream states are kept.  Setting a best shot enqueues
+ * its state to be zeroed (no track open); the images are not touched.  Then on every tick of the stream:
+ *   crop tick   a "CS" record with width > 0 and height > 0 (the ticks that write face crops).  The candidate is, bit
+ *               for bit, the RGBA8 face crop of the best shot's width, height and scale (ht_face_crop) from the tick's
+ *               video, before any redaction; a framing never applies to it.  Its score is sum L^2 (uint64) over the
+ *               pixels 1 <= i <= S_w-2, 1 <= j <= S_h-2 whose alpha and whose four neighbours' alphas are all 255, with
+ *               L = 4 g(i,j) - g(i-1,j) - g(i+1,j) - g(i,j-1) - g(i,j+1) and g the detector's gray (HT_TENSOR_GRAY's).
+ *               With no track open the tick begins track t = track + 1 (HT_BEST_BEGAN), whose image is rgba[(t-1) & 1]
+ *               with two images and rgba[0] with one.  The track's first tick, and a later one whose score is strictly
+ *               greater than best_score, set the best (HT_BEST_IMPROVED): the candidate is written to the image, every
+ *               pixel, and the state takes its score and record.  The earliest tick wins a tie.
+ *   other tick  (the CS tick that loses the face, any tick after stop or reset, ...) ends an open track (HT_BEST_ENDED).
+ * ht_tracker_import ends the open tracks of the streams it writes (flags HT_BEST_ENDED): an imported stream is another
+ * tracker.  A stream that a feed does not list does not tick: its track neither advances nor ends.  With two images
+ * the previous track's final best stays intact for the whole next track.  The best shot belongs to the stream id:
+ * stop, start, reset, ht_tracker_set_params and ht_tracker_import keep it; ht_tracker_config removes every stream's.  A
+ * tick launches two more kernels while some stream has a best shot, and nothing more otherwise.  The tracker record
+ * format is unchanged.
+ * Errors (nothing changes; the message names the record): HT_ERR_STATE before ht_tracker_config; HT_ERR_SIZE for a size
+ * outside 3..2048; HT_ERR_ARG for a range outside [0, max_frames), n <= 0, shots NULL, an image that is host memory or
+ * not 4-byte aligned, a state that is host memory, memory of another device or not 8-byte aligned, a pitch that is not
+ * a multiple of 4 >= 4*width, a non-zero pad_, a scale that is not finite or outside (0, 16], or an image or state that
+ * overlaps any debug canvas, crop plane, tensor plane, camera, framed box, best-shot image (the shot's other image
+ * included) or best-shot state of any stream after the call (the one rule of ht_tracker_set_face_tensor; an image is
+ * (height-1)*pitch + 4*width bytes, a state HT_BEST_SHOT_STATE_BYTES). */
+int ht_tracker_set_best_shot(ht_ctx *ctx, int first, int n, const ht_best_shot *shots);
+/* The best-shot score of a w x h RGBA8 image (host memory, rows of `pitch` bytes, 0: 4*w), exactly as the device
+ * computes it for a candidate.  Host only; needs no context.  -> HT_OK, HT_ERR_ARG for NULL pointers or a pitch below
+ * 4*w, HT_ERR_SIZE for a size outside 3..2048. */
+int ht_best_shot_score(const uint8_t *rgba, int w, int h, int pitch, uint64_t *out);
+
 /* A stream's head-coupled camera: the three.js r48 PerspectiveCamera that realisticAbsoluteCameraControl moves
  * (src/controllers.js:28-68), in caller-owned DEVICE memory that a renderer can bind directly.  Byte offsets:
  *     0  double position[3]      camera.position
@@ -774,7 +846,7 @@ typedef struct {
  * some stream has a controller, and nothing more otherwise.
  * Errors (nothing changes): HT_ERR_STATE before ht_tracker_config; HT_ERR_ARG for a range outside [0, max_frames),
  * n <= 0, controls NULL, a camera that is host memory, memory of another device or not 16-byte aligned, a camera that
- * overlaps any debug canvas, crop plane, tensor plane, camera or framed box of any stream after the call (the one rule of
+ * overlaps any debug canvas, crop plane, tensor plane, camera, framed box or best-shot image or state of any stream after the call (the one rule of
  * ht_tracker_set_face_tensor), a non-finite field, aspect <= 0, near <= 0, far <= near, fov outside (0, 180), or a
  * degenerate lookAt (fixed_position == look_at, or a view direction parallel to +y). */
 int ht_tracker_set_camera(ht_ctx *ctx, int first, int n, const ht_camera_control *controls);

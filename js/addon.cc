@@ -37,6 +37,8 @@
 //        an ht_framed_box in device memory, that its crop and / or tensor is cut from)
 //   trackerSetRedact(handle, first, [redaction|null, ...])  (ht_tracker_set_redact: each stream's tracked face hidden
 //        in its own device video after each tick, a mosaic or a fill)
+//   trackerSetBestShot(handle, first, [shot|null, ...])  (ht_tracker_set_best_shot: each stream's sharpest face of its
+//        current or last track, in one or two device RGBA8 images, with its state in device memory)
 //   trackerExport(handle, [stream, ...]) -> Buffer of records; trackerImport(handle, [stream, ...], records)
 //        (ht_tracker_export / ht_tracker_import: a stream's whole Tracker as HT_TRACKER_RECORD_BYTES per stream)
 //   trackerFeed(handle, [{stream, rgba, width, height, nowMs, canvasWidth?, canvasHeight?}], canvasWidth, canvasHeight)
@@ -726,6 +728,53 @@ static napi_value TrackerSetFraming(napi_env env, napi_callback_info info) {
   return nullptr;
 }
 
+// trackerSetBestShot(handle, first, [{rgba: BigInt device address | [BigInt, BigInt], state: BigInt device address,
+// width, height, pitch?, scale?}, null, ...]): stream first+i gets shots[i]; null or undefined: none.  pitch defaults
+// to 4 * width and scale to 1, as in the Python wrapper.
+static napi_value TrackerSetBestShot(napi_env env, napi_callback_info info) {
+  size_t argc = 3;
+  napi_value argv[3];
+  NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+  ht_ctx *ctx = Ctx(env, argv[0]);
+  int32_t first = 0;
+  uint32_t n = 0;
+  napi_get_value_int32(env, argv[1], &first);
+  NAPI_OK(napi_get_array_length(env, argv[2], &n));
+  std::vector<ht_best_shot> bs(n);
+  memset(bs.data(), 0, n * sizeof(ht_best_shot));
+  for (uint32_t i = 0; i < n; ++i) {
+    napi_value r, v;
+    napi_valuetype t = napi_undefined;
+    NAPI_OK(napi_get_element(env, argv[2], i, &r));
+    napi_typeof(env, r, &t);
+    if (t != napi_object) continue;
+    ht_best_shot &b = bs[i];
+    bool lossless = false, pair = false;
+    uint64_t addr[2] = {0, 0}, state = 0;
+    if (napi_get_named_property(env, r, "rgba", &v) == napi_ok) {
+      napi_is_array(env, v, &pair);
+      if (pair) {
+        for (uint32_t k = 0; k < 2; ++k) {
+          napi_value e;
+          if (napi_get_element(env, v, k, &e) == napi_ok) napi_get_value_bigint_uint64(env, e, &addr[k], &lossless);
+        }
+      } else {
+        napi_get_value_bigint_uint64(env, v, &addr[0], &lossless);
+      }
+    }
+    if (napi_get_named_property(env, r, "state", &v) == napi_ok) napi_get_value_bigint_uint64(env, v, &state, &lossless);
+    for (int k = 0; k < 2; ++k) b.rgba[k] = reinterpret_cast<uint8_t *>(static_cast<uintptr_t>(addr[k]));
+    b.state = reinterpret_cast<ht_best_shot_state *>(static_cast<uintptr_t>(state));
+    b.width = (int32_t)GetNumber(env, r, "width", 0);
+    b.height = (int32_t)GetNumber(env, r, "height", 0);
+    b.pitch = (int32_t)GetNumber(env, r, "pitch", 0);
+    b.scale = GetNumber(env, r, "scale", 1.0);
+  }
+  int rc = ht_tracker_set_best_shot(ctx, first, (int)n, bs.data());
+  if (rc < 0) return Throw(env, ctx, rc);
+  return nullptr;
+}
+
 // trackerSetRedact(handle, first, [{mode?: "mosaic" | "fill", block?, scale?, hold?, fillRgb?: [r, g, b],
 // fillYuv?: [y, u, v]}, null, ...]): stream first+i gets redactions[i]; null or undefined: none.  The defaults are the
 // Python wrapper's: mosaic, block 16, scale 1.25, hold 10, black.
@@ -1138,6 +1187,7 @@ static napi_value Init(napi_env env, napi_value exports) {
       {"trackerSetCamera", nullptr, TrackerSetCamera, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerSetFraming", nullptr, TrackerSetFraming, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerSetRedact", nullptr, TrackerSetRedact, nullptr, nullptr, nullptr, napi_default, nullptr},
+      {"trackerSetBestShot", nullptr, TrackerSetBestShot, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerExport", nullptr, TrackerExport, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerImport", nullptr, TrackerImport, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"trackerFeed", nullptr, TrackerFeed, nullptr, nullptr, nullptr, napi_default, nullptr},

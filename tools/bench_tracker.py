@@ -40,6 +40,9 @@ streams: N 640x480 streams, device-resident frames and outputs, CUDA events arou
   redact*_*       (--redact) 1024 streams of 1280x720 NV12 onto 320x240 canvases with a mosaic (B = 16, scale 1.5) on
                   no, every and every 64th stream (no redaction also against --before-lib), arms alternating tick by
                   tick, each arm on its own copy of the video (redact_arms)
+  best*_*         (--best-shot) the --crops workload with 224x224 NV12 crops on every stream, with a 224x224 best
+                  shot (two images) on no, every and every 64th stream (none also against --before-lib), arms
+                  alternating tick by tick, and the kernel times of k_best_score and k_best_write (best_shot_arms)
 
 Prints one JSON line with the card's name and power limit read in the same run; --out also writes it to a file."""
 import argparse
@@ -1593,6 +1596,129 @@ def redact_arms(torch, stream, N, steps, rounds, before_lib=None):
     return res
 
 
+def best_shot_arms(torch, stream, N, steps, rounds, before_lib=None):
+    """f15's workload (N streams of 1280x720 NV12 through ht_tracker_feed_yuv onto 320x240 canvases, 224x224 NV12 face
+    crops on every stream), with arms alternating tick by tick: no best shot (bestoff_cs), none on another build
+    (bestoff_before_cs, --before-lib), a 224x224 best shot with two images on every stream (bestall_cs) and on every
+    64th stream (best64_cs).  The records of every arm must agree on every timed tick, and the states of a sample of
+    streams must equal headtrackr_b200.bestshot's replay of the records and the host score of the images' candidates.
+    Then, in runs of their own under torch.profiler, the kernel times of k_best_score and k_best_write per tick."""
+    import ctypes as C
+    from headtrackr_b200 import Context, _lib, bestshot
+    from headtrackr_b200.context import _yuv_image
+    W, H, CW, CH, S = 1280, 720, 320, 240, 224
+    rec_bytes = C.sizeof(_lib.TrackerEvent)
+    now = [1.0e12]
+    kw = dict(max_width=CW, max_height=CH, max_frames=N, stream=stream)
+    ys, uvs = nv12_streams(torch, N, W, H)
+    keep = []
+    imgs = [_yuv_image((ys[k], uvs[k]), "nv12", "bt601", keep)[0] for k in range(N)]
+    yrecs = (_lib.YuvFrame * N)()
+    for k in range(N):
+        yrecs[k] = _lib.YuvFrame(imgs[k], k, CW, CH, 0, 0.0)
+    shots = {}
+
+    def arm(every, before=False):
+        c = other_build_context(before_lib, **kw) if before else Context(**kw)
+        c._L.ht_tracker_set_face_crop_yuv.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p]
+        c.tracker_config()
+        c.tracker_reset(0, N)
+        c.tracker_start(0, N)
+        y = torch.zeros((N, S, S), dtype=torch.uint8, device="cuda")
+        uv = torch.zeros((N, S // 2, S), dtype=torch.uint8, device="cuda")
+        c.tracker_set_face_crop(0, [{"out": (y[k], uv[k]), "format": "nv12", "color": "bt601"} for k in range(N)])
+        if every:
+            img = torch.zeros((N, 2, S, S, 4), dtype=torch.uint8, device="cuda")
+            st = torch.zeros((N, 128), dtype=torch.uint8, device="cuda")
+            c.tracker_set_best_shot(0, [{"out": (img[k, 0], img[k, 1]), "state": st[k, :96]} if k % every == 0 else None
+                                        for k in range(N)])
+            shots[every] = (img, st)
+        out = torch.empty(N * rec_bytes, dtype=torch.uint8, device="cuda")
+
+        def run():
+            for k in range(N):
+                yrecs[k].now_ms = now[0]
+            c._check(c._L.ht_tracker_feed_yuv(c._h, C.addressof(yrecs), N, 1, out.data_ptr()))
+        return c, run, out
+
+    arms = {"bestoff_cs": arm(0), "bestall_cs": arm(1), "best64_cs": arm(64)}
+    if before_lib:
+        arms["bestoff_before_cs"] = arm(0, before=True)
+    names = list(arms)
+    sample = list(range(0, N, max(1, N // 32)))
+    replay = {k: bestshot.new_state() for k in sample}
+    candidate = {}
+
+    def tick(name):
+        _, run, _ = arms[name]
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        a.record()
+        run()
+        b.record()
+        b.synchronize()
+        return a.elapsed_time(b)
+
+    def follow():
+        # a written image is the candidate of a best tick: its score is the state's best_score when it was written
+        recs = arms["bestoff_cs"][2].cpu().numpy().reshape(N, rec_bytes)
+        img, st = shots[1]
+        states = st.cpu().numpy()
+        for k in sample:
+            e = _lib.TrackerEvent.from_buffer_copy(bytes(recs[k]))
+            r = dict(detection=e.detection, x=e.x, y=e.y, width=e.width, height=e.height, angle=e.angle)
+            got = bestshot.state_from_bytes(states[k, :96])
+            score = got["score"] if bestshot.crop_tick(r) else 0
+            if bestshot.step(replay[k], r, score, now[0], CW, CH):
+                candidate[k] = bestshot.score(img[k, replay[k]["buffer"]].cpu().numpy())
+            if bestshot.state_to_bytes(replay[k]) != bytes(states[k, :96]) or \
+                    (k in candidate and candidate[k] != replay[k]["best_score"]):
+                raise SystemExit(f"best-shot state or image of stream {k} disagrees with the replay")
+
+    for _ in range(17):                          # the whitebalance gate, detection, the first CS frames
+        now[0] += 20.0
+        for name in names:
+            tick(name)
+        follow()
+    times = {name: [[] for _ in range(rounds)] for name in names}
+    for r in range(rounds):
+        for s in range(steps):
+            now[0] += 20.0
+            rot = (r * steps + s) % len(names)
+            for name in names[rot:] + names[:rot]:
+                times[name][r].append(tick(name))
+            first = arms[names[0]][2]
+            if any(not torch.equal(first, arms[name][2]) for name in names[1:]):
+                raise SystemExit("best-shot arms disagree on the records of a timed tick")
+            follow()
+    res = {}
+    for name in names:
+        med = [float(np.median(t)) for t in times[name]]
+        res[f"{name}_ms"] = float(np.median(sum(times[name], [])))
+        res[f"{name}_spread_ms"] = max(med) - min(med)
+    res["best_records_agree"] = True
+    res["best_states_equal_replay"] = True
+    res["best_tracks_max"] = max(replay[k]["track"] for k in sample)
+    res["best_improved_ticks_sampled"] = sum(replay[k]["best_tick"] for k in sample)
+
+    from torch.profiler import ProfilerActivity, profile
+    for name in ("bestall_cs", "best64_cs"):
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(steps):
+                now[0] += 20.0
+                arms[name][1]()
+            torch.cuda.synchronize()
+        for kern in ("k_best_score", "k_best_write", "k_face_crop"):
+            us = 0.0
+            for e in prof.key_averages():
+                if kern in e.key:
+                    t = getattr(e, "device_time_total", None)
+                    us += t if t is not None else e.cuda_time_total
+            res[f"{kern}_{name[:-3]}_ms"] = us / 1000.0 / steps
+    for c, _, _ in arms.values():
+        c.close()
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--streams", type=int, default=1024)
@@ -1610,6 +1736,7 @@ def main():
     ap.add_argument("--crops", action="store_true", help="only the face-crop arms (crops_arms)")
     ap.add_argument("--framing", action="store_true", help="only the framing arms (framing_arms)")
     ap.add_argument("--redact", action="store_true", help="only the face-redaction arms (redact_arms)")
+    ap.add_argument("--best-shot", action="store_true", help="only the best-shot arms (best_shot_arms)")
     ap.add_argument("--out")
     a = ap.parse_args()
     import torch
@@ -1637,6 +1764,9 @@ def main():
         return report(res, a.out)
     if a.redact:
         res.update(redact_arms(torch, stream, N, a.steps, a.rounds, a.before_lib))
+        return report(res, a.out)
+    if a.best_shot:
+        res.update(best_shot_arms(torch, stream, N, a.steps, a.rounds, a.before_lib))
         return report(res, a.out)
     if a.formats:
         res.update(formats_arms(torch, stream, N, a.steps, a.rounds, a.before_lib))
